@@ -1,4 +1,4 @@
-"""bench.py -- ZMW windows/sec of the DeepConsensus model path on B200 (BASELINE.json metric).
+"""bench.py -- ZMW windows/sec of the DeepConsensus model path on H100 (BASELINE.json metric).
 
   python bench.py --gpus 1 --steps K --warmup W            # the dcb200 engine
   python bench.py --impl reference --gpus 1 --steps K ...   # reference algorithm on host cores
@@ -14,18 +14,22 @@ e2e    : the same metric through the reference-facing call with HOST buffers -- 
          and the base / quality characters copied D2H inside the timed region, every step.  `value` uses the
          pipelined C-ABI pair dcb_submit / dcb_wait exactly as inference.run_model_on_examples does (the copy of
          batch i+1 overlaps the kernels of batch i); `blocking_value` is dcb_forward one batch at a time.
-roofline: tensor-core roofline of the dominant kernel (stack_pair_kernel: the whole encoder stack), timed with CUDA
-         events on the engine's stream over K steps of the same workload (a separate pass: the `value` trials run
-         with the per-kernel events off).  `frac` is against the BURST cuBLAS bf16 figure of MEASURED_PEAKS.json (the
-         K-step region is tens of milliseconds); `roofline.sustained` repeats the measurement over >= 2 s of
-         back-to-back steps against the sustained figure, with the clocks seen during it.
+roofline: tensor-core roofline of the dominant stage (the FFN GEMMs of every layer), timed with CUDA events on the
+         engine's stream over K steps of the same workload (a separate pass: the `value` trials run with the per-kernel
+         events off).  `frac` is against the H100 SXM data-sheet dense bf16 rate (989 TFLOP/s at 700 W), a bound that
+         is not reached; the card's power limit and clocks are reported under `clocks`.
 trials  : the K-step region is timed TRIALS (5) times, each bracketed by barrier + synchronize and reduced with MAX over
          ranks; `value` / `e2e` are the MEDIAN trial (all trials are listed).
 parity  : the default (bf16 tensor-core) path against the engine's strict-fp32 path on the whole batch, on the
-         device -- bases identical %, QV exact %, max |dQ|, max logit error (BASELINE.md section 3.4).
+         device -- bases identical %, QV exact %, max |dQ|, max logit error.
 cpu_baseline / --impl reference: the oracle (torch-CPU fp32 restatement of the reference
          model, oracle/model.py) on the box's host cores.  This is the only place bench.py
          executes oracle/ -- as the baseline being reported, never as the product.
+--dump-outputs DIR: after the timed trials, the base and quality characters (ASCII codes, float32 [windows, L]) of the
+         last timed step of the resident path are written as DIR/bases.npy and DIR/quals.npy, with the batch index of
+         each window in DIR/window_index.npy.  Above 64 MB in all a fixed seeded sample of windows is written; with
+         several GPUs every rank writes its shard as DIR/<name>_rank<r>.npy.  Inputs and weights are seeded, so two
+         builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -53,29 +57,20 @@ WORKLOAD = dict(workload="synthetic pileup windows (BASELINE configs[1])", max_p
                 window=120, d_model=280, layers=6, heads=2, filter_size=2048, attn_win_size=12,
                 batch_per_gpu=1024)
 CALIBRATION = "0,1.197654,-0.99781"   # the fixture params.json's dc_calibration
+DUMP_BYTES = 64 << 20                  # --dump-outputs: at most this many bytes over all files and ranks
 
 
 def config_dict(world: int, batch: int):
   """The `config` of the JSON line -- identical for the engine arm and the --impl reference arm."""
   return dict(WORKLOAD, batch_per_gpu=batch, global_batch=batch * world,
               parallelism="dp%d (independent shards)" % world,
-              l2="inputs larger than L2: the timed steps rotate over resident packed batches spanning > 126 MB of addresses, and "
-                 "every step streams the 151 MB fp32 residual image through L2 (details under `timing`)")
+              l2="inputs larger than L2: the timed steps rotate over resident packed batches spanning > 50 MB of addresses, and "
+                 "every step streams the fp32 residual image through L2 (details under `timing`)")
 
 
 def cpu_threads() -> int:
-  """Threads of the CPU arm: the best count of a committed sweep on this pool's host (profiles/r02_cpu_sweep.json,
-  scripts/cpu_sweep.py) when present, else every core the process may use."""
-  avail = len(os.sched_getaffinity(0))
-  path = os.path.join(ROOT, "profiles", "r02_cpu_sweep.json")
-  if os.path.exists(path):
-    try:
-      with open(path) as f:
-        best = int(json.load(f)["best_threads"])
-      return max(1, min(best, avail))
-    except Exception:
-      pass
-  return avail
+  """Threads of the CPU arm: every core the process may use."""
+  return len(os.sched_getaffinity(0))
 
 
 def model_params():
@@ -84,22 +79,16 @@ def model_params():
 
 
 def flops_per_window(p) -> float:
-  """Algorithmic (un-padded, banded) FLOPs per window -- SURVEY.md section 8(d)."""
+  """Algorithmic (un-padded, banded) FLOPs per window."""
   L, d, ff, w = p.max_length, p.hidden_size, p.filter_size, p.attn_win_size
   E = params_lib.embedded_width(p)
   pairs = L * (2 * w + 1) - w * (w + 1)
   return 2 * L * E * d + p.num_hidden_layers * (8 * L * d * d + 4 * pairs * d + 4 * L * d * ff) + 2 * L * d * 5
 
 
-def measured_peaks():
-  path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-  if os.path.exists(path):
-    with open(path) as f:
-      pk = json.load(f)
-    return dict(bf16_tflops=pk["bf16_tflops"], bf16_tflops_sustained=pk.get("bf16_tflops_sustained"),
-                hbm_gbs=pk["hbm_gbs"], source="MEASURED_PEAKS.json")
-  return dict(bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, hbm_gbs=6650.0,
-              source="fallback (B200_PROFILING.md)")
+def datasheet_peaks():
+  """NVIDIA H100 SXM data sheet (700 W): dense bf16 tensor rate and HBM3 bandwidth.  Upper bounds, not measurements."""
+  return dict(bf16_tflops=989.0, hbm_gbs=3350.0, source="H100 SXM data sheet, dense bf16, 700 W")
 
 
 class ClockSampler(threading.Thread):
@@ -109,18 +98,20 @@ class ClockSampler(threading.Thread):
     super().__init__(daemon=True)
     self.index, self.samples, self.stop_flag = index, [], threading.Event()
     self.max_mhz = None
+    self.power_limit_w = None
 
   def run(self):
     q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit")
     while not self.stop_flag.is_set():
       try:
         out = subprocess.run(["nvidia-smi", "-i", str(self.index), "--query-gpu=" + q,
                               "--format=csv,noheader,nounits"], capture_output=True, text=True,
                              timeout=5).stdout.strip().split(",")
-        self.samples.append((float(out[0]), [o.strip() for o in out[2:]]))
+        self.samples.append((float(out[0]), [o.strip() for o in out[2:6]]))
         self.max_mhz = float(out[1])
+        self.power_limit_w = float(out[6])
       except Exception:
         pass
       self.stop_flag.wait(0.05)
@@ -128,9 +119,10 @@ class ClockSampler(threading.Thread):
   def summary(self):
     names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
     if not self.samples:
-      return dict(sm_mhz=None, sm_max_mhz=self.max_mhz, reasons=[], samples=0)
+      return dict(sm_mhz=None, sm_max_mhz=self.max_mhz, power_limit_w=self.power_limit_w, reasons=[], samples=0)
     reasons = sorted({names[i] for _, fl in self.samples for i, v in enumerate(fl) if v.lower().startswith("active")})
     return dict(sm_mhz=float(np.median([s[0] for s in self.samples])), sm_max_mhz=self.max_mhz,
+                power_limit_w=self.power_limit_w,
                 reasons=reasons, samples=len(self.samples))
 
 
@@ -220,8 +212,11 @@ def main():
   ap.add_argument("--batch", type=int, default=WORKLOAD["batch_per_gpu"])
   ap.add_argument("--no-cpu-baseline", action="store_true")
   ap.add_argument("--nccl-scatter", action="store_true",
-                  help="N > 1: also time the step fed by ONE reader rank over NCCL (BASELINE configs[3]; secondary record, "
-                       "profiles/r02_bench_{2,4,8}gpu.json were produced with it)")
+                  help="N > 1: also time the step fed by ONE reader rank over NCCL (BASELINE configs[3]; secondary record)")
+  ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                  help="write the bases / quals (float32 [windows, L]) of the last timed step and the batch indices of "
+                       "those windows as DIR/<name>.npy; more than 64 MB in all keeps a fixed seeded sample of windows; "
+                       "with --gpus > 1 every rank writes its own shard as DIR/<name>_rank<r>.npy")
   args = ap.parse_args()
   args.warmup = max(args.warmup, 3)
 
@@ -273,7 +268,7 @@ def main():
     model.pack_rows(h, out=arr.reshape(B, stride))
     ppin_addr.append(a)
     ppin.append(arr)
-  NPK = max(NBUF, int(140e6 // packed_bytes) + 1)     # resident packed batches rotate over > 126 MB (L2) of addresses
+  NPK = max(NBUF, int(60e6 // packed_bytes) + 1)      # resident packed batches rotate over > 50 MB (L2) of addresses
   for i in range(NPK):
     d = model.alloc_device(packed_bytes)
     model.memcpy_h2d(d, ppin[i % NBUF][:packed_bytes])
@@ -370,8 +365,8 @@ def main():
     step_resident(i)
   sampler = ClockSampler(local)
   sampler.start()
-  # per-kernel device times right after warm-up, before the timed trials heat the GPU into its power cap: the state the
-  # burst cuBLAS peak was measured in (reported next to the post-trial measurement, which is the `roofline` proper)
+  # per-kernel device times right after warm-up, before the timed trials heat the GPU into its power cap (reported next
+  # to the post-trial measurement, which is the `roofline` proper)
   model.set_profile(True)
   barrier()
   run_resident_pipelined(args.steps)
@@ -383,6 +378,18 @@ def main():
   for _ in range(TRIALS):       # resident and host-buffer trials alternate, so both see the same thermal / power state
     res_trials.append(trial(run_resident_pipelined))                             # per-kernel events OFF
     e2e_trials.append(trial(run_e2e_pipelined))
+  if args.dump_outputs:
+    # dev_bases / dev_quals still hold the last step of the last resident trial (the e2e trials write host buffers).
+    # Every rank writes its own shard; past DUMP_BYTES in all, a fixed seeded sample of windows is kept.
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    keep = min(B, DUMP_BYTES // (world * 2 * L * 4))
+    idx = np.arange(B) if keep == B else np.sort(np.random.default_rng(12345).choice(B, keep, replace=False))
+    suffix = "" if world == 1 else "_rank%d" % rank
+    for name, ptr in (("bases", dev_bases), ("quals", dev_quals)):
+      host = np.empty((B, L), dtype=np.uint8)
+      model.memcpy_d2h(host, ptr)
+      np.save(os.path.join(args.dump_outputs, name + suffix + ".npy"), host[idx].astype(np.float32))
+    np.save(os.path.join(args.dump_outputs, "window_index" + suffix + ".npy"), idx.astype(np.float64))
   res_f32 = [trial(lambda n: run_resident_pipelined(n, packed=False)) for _ in range(3)]
   run_e2e_pipelined(3, packed=False)
   f32_trials = [trial(lambda n: run_e2e_pipelined(n, packed=False)) for _ in range(3)]
@@ -441,7 +448,7 @@ def main():
   # double-buffered; results gathered back) instead of every rank holding its own shard.  Secondary record: the
   # natural split for this path is the replica form above (no data-path collective).
   # Opt-in (--nccl-scatter): of three 8-GPU runs of this record one ended in an unexplained "unspecified launch failure" on
-  # one receiving rank (not reproduced in 3000 overlapped steps on 2 GPUs, scripts/gpu_scatter_stress.py; DESIGN.md section 7),
+  # one receiving rank (not reproduced in 3000 overlapped steps on 2 GPUs, not reproduced since),
   # and a secondary record must not be able to take the primary line down with it.
   scatter_info = None
   if world > 1 and args.nccl_scatter:
@@ -496,35 +503,23 @@ def main():
   value = total_windows / dt
   e2e_value = total_windows / dt_e2e
   F = flops_per_window(p)
-  peaks = measured_peaks()
-  # dominant kernel.  fused_oproj == 2: the whole encoder stack runs in ONE kernel (stack_pair_kernel) -- algorithmic
-  # FLOPs per launch = tokens * layers * (8 d^2 + 4 d ff) + banded attention pairs; otherwise the per-layer fused
-  # out-proj + FFN kernel: tokens * (4 d ff [+ 2 d d]).
-  d, ff, wdw, Lp = p.hidden_size, p.filter_size, p.attn_win_size, p.max_length
-  if prof["fused_oproj"] == 2:
-    pairs = Lp * (2 * wdw + 1) - wdw * (wdw + 1)
-    per_token = p.num_hidden_layers * (8.0 * d * d + 4.0 * d * ff + 4.0 * pairs * d / Lp)
-    kname = ("stack_pair_kernel (all %d layers: QKV + banded attention + out-proj + FFN, residual in TMEM; final LayerNorm, fc1 "
-             "and the quality epilogue in its tail -- their flops are not counted)" % p.num_hidden_layers)
-  else:
-    per_token = 4.0 * d * ff + (2.0 * d * d if prof["fused_oproj"] else 0.0)
-    kname = "ffn_pair_kernel<fused out-proj>" if prof["fused_oproj"] else "ffn_pair_kernel"
+  peaks = datasheet_peaks()
+  # dominant stage: the two FFN GEMMs of every layer (up-projection with bias + ReLU, down-projection with the residual
+  # row epilogue) -- algorithmic FLOPs per token and layer = 4 d ff
+  d, ff = p.hidden_size, p.filter_size
+  per_token = 4.0 * d * ff
+  kname = "gemm_kernel (FFN up- and down-projection, every layer)"
 
   def kernel_tflops(pr):
     return pr["ffn_tokens"] * per_token / (pr["ffn_ms_total"] * 1e-3) / 1e12 if pr["ffn_ms_total"] > 0 else None
   ffn_tflops = kernel_tflops(prof)
-  traffic = None
-  tpath = os.path.join(ROOT, "profiles", "stack_dram_traffic.json" if prof["fused_oproj"] == 2 else "ffn_dram_traffic.json")
-  if os.path.exists(tpath):
-    with open(tpath) as f:
-      traffic = json.load(f).get("dram_bytes_per_launch")
   kshare = {k: round(v["ms"] / max(sum(x["ms"] for x in prof["kernels"].values()), 1e-9), 4) for k, v in prof["kernels"].items()}
-  peak_used, peak_src = peaks["bf16_tflops"], peaks["source"] + " (burst cuBLAS bf16; the K-step region is tens of ms)"
+  peak_used, peak_src = peaks["bf16_tflops"], peaks["source"]
   roof = dict(bound="tensor", kernel=kname,
               achieved=ffn_tflops, flops_per_token=per_token, kernel_time_share=kshare,
               kernel_ms_per_step={k: round(v["ms"] / args.steps, 4) for k, v in prof["kernels"].items()}, peak=peak_used,
               unit="TFLOP/s", frac=(ffn_tflops / peak_used) if ffn_tflops else None,
-              traffic=traffic, peak_source=peak_src,
+              peak_source=peak_src,
               launches_timed=prof["ffn_launches"],
               avg_launch_ms=prof["ffn_ms_total"] / max(prof["ffn_launches"], 1),
               model_tflops_whole_step=value / world * F / 1e12,
@@ -532,16 +527,15 @@ def main():
   cool = kernel_tflops(prof_cool)
   roof["first_pass_after_warmup"] = dict(achieved=cool, frac=(cool / peak_used) if cool else None,
                                          avg_launch_ms=prof_cool["ffn_ms_total"] / max(prof_cool["ffn_launches"], 1),
-                                         note="same K steps timed before the trials (GPU not yet at its power cap, as when the "
-                                              "burst peak was measured); `achieved` / `frac` above are from the pass after the trials")
-  if sus is not None and peaks.get("bf16_tflops_sustained"):
+                                         note="same K steps timed before the trials; `achieved` / `frac` above are from the "
+                                              "pass after the trials")
+  if sus is not None:
     st = kernel_tflops(sus["prof"])
     roof["sustained"] = dict(seconds=round(sus["seconds"], 3), steps=sus["steps"], value=sus["value"],
-                             achieved=st, peak=peaks["bf16_tflops_sustained"],
-                             frac=(st / peaks["bf16_tflops_sustained"]) if st else None,
+                             achieved=st, frac=(st / peak_used) if st else None,
                              model_tflops_whole_step=sus["value"] / world * F / 1e12,
                              clocks=sus["clocks"],
-                             note=">= 2 s of back-to-back steps (per-kernel events on); peak = sustained cuBLAS bf16")
+                             note=">= 2 s of back-to-back steps (per-kernel events on)")
   line = dict(metric=METRIC, value=value, unit=UNIT, n_gpus=world, steps=args.steps, warmup=args.warmup,
               ms_per_step=dt / args.steps * 1e3, device_ms_per_step=dev_ms / args.steps,
               higher_is_better=True, scaling="weak", vs_baseline=None, dtype="bf16",
@@ -553,8 +547,8 @@ def main():
                                                   "e2e trials alternate (same thermal / power state)" % args.steps,
                           value_trials=[round(total_windows / t[0], 1) for t in res_trials],
                           e2e_trials=[round(total_windows / t[0], 1) for t in e2e_trials],
-                          l2="inputs rotate over %d resident packed batches (%.0f MB of addresses > 126 MB L2); every step also "
-                             "streams the 151 MB fp32 residual image through L2" % (NPK, NPK * packed_bytes / 1e6),
+                          l2="inputs rotate over %d resident packed batches (%.0f MB of addresses > 50 MB L2); every step also "
+                             "streams the fp32 residual image through L2" % (NPK, NPK * packed_bytes / 1e6),
                           input="packed rows, %d B/window (include/dcb200.h), resident in HBM" % stride,
                           gflop_per_window=F / 1e9),
               e2e=dict(value=e2e_value, unit=UNIT, h2d_bytes_per_step=packed_bytes * world,
@@ -568,7 +562,7 @@ def main():
                                               % (row_bytes // B)),
                        blocking_value=total_windows / dt_e2e_blocking,
                        blocking_call="dcb_forward on float32 rows, one batch at a time"),
-              gpu_launches=launches, roofline=roof, parity=par, nccl_scatter=scatter_info, clocks=sampler.summary(), numa_node=numa, stitch=stitch_info)
+              gpu=torch.cuda.get_device_name(local), gpu_launches=launches, roofline=roof, parity=par, nccl_scatter=scatter_info, clocks=sampler.summary(), numa_node=numa, stitch=stitch_info)
   if rank == 0 and world == 1 and not args.no_cpu_baseline:
     os.sched_setaffinity(0, full_affinity)   # the CPU arm may use every host core again
     cores = cpu_threads()

@@ -1,6 +1,6 @@
-"""dcb200: B200-native (sm_100a) inference engine for the DeepConsensus hot path.
+"""dcb200: H100-native (sm_90a) inference engine for the DeepConsensus hot path.
 
-Scope (SURVEY.md section 8): `quick_inference.run_model_on_examples` ->
+Scope: `quick_inference.run_model_on_examples` ->
 `EncoderOnlyLearnedValuesTransformer` forward -> argmax/QV -> `stitch_utils`
 output surface.  The compute path is hand-written CUDA behind a C-ABI
 (`include/dcb200.h`, built into `deepconsensus_b200/csrc/libdcb200.so`); this

@@ -1,4 +1,4 @@
-// Feature construction from BAM, htslib-free (SURVEY.md section 8(f)3 + the producer half of 8(f)1): the part of
+// Feature construction from BAM, htslib-free (and the producer half of the packed rows): the part of
 // `deepconsensus run` that sits in front of the model path, as host C++ behind the C ABI (include/dcb200.h "dcb_prep_*",
 // "dcb_bamw_*").
 //

@@ -1,14 +1,14 @@
 #!/bin/bash
-# Builds the C-ABI library of include/dcb200.h for sm_100a, in-tree:
+# Builds the C-ABI library of include/dcb200.h for sm_90a (H100), in-tree:
 #   libdcb200.so      the product (ignores the environment)
-#   libdcb200_dev.so  the same sources with -DDCB_DEV_SWITCHES: environment switches select the measured alternative
-#                     kernel paths (tests/test_gpu_parity.py::test_unfused_fallback_paths_agree_with_fused, scripts/)
+#   libdcb200_dev.so  the same sources with -DDCB_DEV_SWITCHES: environment switches select the alternative
+#                     token layout and chunking (tests/test_gpu_parity.py::test_unfused_fallback_paths_agree_with_fused)
 # Experiment builds: DCB_OUT=libdcb200_exp.so DCB_EXTRA_FLAGS=-D... (loaded via DCB200_LIB); DCB_SKIP_DEV=1 skips the
 # developer library.
 set -euo pipefail
 cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-BASE="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -diag-suppress 177 -Xcompiler -fPIC -Xcompiler -fvisibility=hidden"
+BASE="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -diag-suppress 177 -Xcompiler -fPIC -Xcompiler -fvisibility=hidden"
 
 build_one() {   # $1 = output .so, $2 = extra flags
   local out=$1 flags="$BASE $2" tag=${1%.so}
@@ -19,7 +19,7 @@ build_one() {   # $1 = output .so, $2 = extra flags
   $NVCC $flags -Xcompiler -fvisibility=default -c bam_prep.cpp -o $tag.bam.o & pids+=($!)
   $NVCC $flags -Xcompiler -fvisibility=default -c engine.cu -o $tag.engine.o & pids+=($!)
   for p in "${pids[@]}"; do wait $p; done     # a failed compile fails the build (set -e)
-  $NVCC -gencode arch=compute_100a,code=sm_100a -shared -o $out $tag.kernels.o $tag.strict.o $tag.post.o $tag.bam.o $tag.engine.o -lz -Xlinker -soname=$out
+  $NVCC -gencode arch=compute_90a,code=sm_90a -shared -o $out $tag.kernels.o $tag.strict.o $tag.post.o $tag.bam.o $tag.engine.o -lz -Xlinker -soname=$out
   echo "built $(pwd)/$out"
 }
 

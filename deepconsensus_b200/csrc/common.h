@@ -11,14 +11,15 @@ namespace dcb {
 // (model_configs.py:84,139); the engine fixes these at compile time and validates
 // params.json against them in dcb_create().  Everything else (max_passes,
 // max_length, layers, filter_size, ReZero vs LayerNorm, ccs_bq, band) is runtime.
-constexpr int kTileM = 128;     // tokens per tile == UMMA M == TMEM lanes
+constexpr int kTileM = 128;     // tokens per tile (two wgmma M=64 warpgroups)
 constexpr int kD = 280;         // hidden_size
-constexpr int kDP = 288;        // hidden_size padded to a multiple of 16 (UMMA K / N granularity)
+constexpr int kDP = 288;        // hidden_size padded to a multiple of 16 (wgmma K granularity)
 constexpr int kHeads = 2;
 constexpr int kDH = 140;        // size per head
 constexpr int kDHP = 144;       // padded per-head size (multiple of 16)
 constexpr int kQKVN = 3 * kHeads * kDHP;  // 864: [q_h0|q_h1|k_h0|k_h1|v_h0|v_h1]
-constexpr int kNC = 144;        // UMMA N per instruction for the d-wide GEMMs (288 = 2 x 144)
+constexpr int kQKVGroup = 144;  // q/k/v columns per GEMM n-group (6 groups: one accumulator chunk per consumer)
+constexpr int kNC = 144;        // wgmma N per instruction for the d-wide GEMMs (288 = 2 x 144)
 constexpr int kVocab = 5;       // ' ATCG' (dc_constants.py:39-42)
 constexpr int kFFChunk = 128;   // filter_size is processed in chunks of 128 hidden units
 
@@ -113,35 +114,14 @@ struct RowEpi {
   int L;                 // tokens per window in the flattened layout (Lw): position = token % L
 };
 
-// ------------------------------------------------------------------ whole-stack kernel
-constexpr int kMaxLayers = 8;
-struct StackParams {
-  const uint8_t* wq3[kMaxLayers];    // per layer: [head][rank][q|k|v] x [36 k-chunks][72 rows][8] bf16
-  const uint8_t* wo2[kMaxLayers];    // per layer: [rank][36][144][8] (ReZero alpha folded in)
-  const uint8_t* wffn2[kMaxLayers];  // per layer: [chunk][rank]{[36][64][8], [16][144][8]}
-  const float* b2[kMaxLayers];       // [288] (alpha folded in)
-  // The eight padding rows 280..287 of the q/k/v and W1 images carry rank-1 terms as bf16 hi / lo pairs, against which the
-  // row pass writes operand columns 280..287 = (-dmean) hi, hi, lo, lo, (1 / rstd) hi, hi, lo, lo:
-  //   rows 280..283 = cs_hi, cs_lo, cs_hi, cs_lo    rows 284..287 = bw_hi, bw_lo, bw_hi, bw_lo
-  // ReZero models: dmean = 0, rstd = 1, cs = 0 and bw = b1 for W1 (0 for q/k/v) -- the GEMM adds the bias, the hidden
-  // epilogue loads nothing.  Pre-LayerNorm models (deferred_ln = 1): the normalisation is DEFERRED -- the operand tile is
-  // bf16(x - shift), gamma is folded into rows 0..279, cs = column sums of the rounded folded weights, bw = beta^T W
-  // (+ b1 for W1), dmean = mean - shift; the accumulator is (LN(x) W + bw) / rstd and its reader multiplies by rstd.
-  int deferred_ln;
-  float b2_mean[kMaxLayers];         // mean over the 280 columns of b2 (the row pass moves its centring shift by it)
-  int num_layers;
-  int ff;
-};
-
 struct HeadParams {
   const float* x;        // fp32 residual image
   const float* ln_g;     // final LayerNorm gamma/beta [288]
   const float* ln_b;
   const float* wfc;      // [280][5]
   const float* bfc;      // [5]
-  const float* gw8;      // [280][8]: gamma_c * Wfc[c][j] for j < 5, then b2_c of the last layer (fused head), zero padded
-  const float* ab;       // [32]: A_j = sum_c gamma_c Wfc[c][j] at 0..4, B_j = sum_c beta_c Wfc[c][j] at 8..12; fused head:
-                         // H_j = sum_c b2_c gamma_c Wfc[c][j] at 16..20, sum b2 at 24, sum b2^2 at 25
+  const float* gw8;      // [280][8]: gamma_c * Wfc[c][j] for j < 5, zero padded
+  const float* ab;       // [16]: A_j = sum_c gamma_c Wfc[c][j] at 0..4, B_j = sum_c beta_c Wfc[c][j] at 8..12
   uint8_t* bases;        // [M] ASCII ' ATCG'
   uint8_t* quals;        // [M] Phred+33
   float* probs;          // [M][5] or null

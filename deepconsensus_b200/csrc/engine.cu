@@ -17,10 +17,6 @@
 #include "../../include/dcb200_debug.h"
 #include "kernels.h"
 
-#ifndef DCB_FUSE_HEAD_DEFAULT
-#define DCB_FUSE_HEAD_DEFAULT 1
-#endif
-
 using namespace dcb;
 
 namespace {
@@ -28,16 +24,10 @@ namespace {
 thread_local std::string g_create_error;
 
 struct LayerDev {
-  __nv_bfloat16* wqkv = nullptr;  // 2 groups x [36][432][8]
-  uint8_t* wqkv2 = nullptr;       // 9 groups x [36][96][8] (qkv2_kernel)
-  uint8_t* wq3 = nullptr;         // stack kernel: per (head, rank, q|k|v) [36][72][8]
-  uint8_t* wqa = nullptr;         // fused QKV+attention: per (head, rank) [36][216][8], rows = q|k|v halves
-  __nv_bfloat16* wo = nullptr;    // [36][288][8]
-  uint8_t* wffn = nullptr;        // per ff chunk: [36][128][8] then [16][288][8]
-  uint8_t* wffn2 = nullptr;       // CTA-pair image: per (chunk, rank): [36][64][8] then [16][144][8]
-  float b2_mean = 0.f;            // mean of b2 over its 280 columns (stack kernel, deferred LayerNorm)
-  uint8_t* wffn2s = nullptr;      // the stack kernel's copy: b1 / deferred-LayerNorm terms in the padding rows (common.h, StackParams)
-  uint8_t* wo2 = nullptr;         // CTA-pair out-proj image: per rank [36][144][8]
+  __nv_bfloat16* wqkv = nullptr;  // 6 groups x split-bf16 [72][144][8]: q_h0, q_h1, k_h0, k_h1, v_h0, v_h1
+  __nv_bfloat16* wo = nullptr;    // split-bf16 [72][288][8]
+  __nv_bfloat16* w1 = nullptr;    // ff / kFFChunk groups x [36][kFFChunk][8]
+  __nv_bfloat16* w2 = nullptr;    // [ff/8][288][8] (ReZero alpha folded in)
   float* b1 = nullptr;            // [ff]
   float* b2 = nullptr;            // [288] (gain folded)
   float* ln_g[2] = {nullptr, nullptr};  // pre-norm gamma/beta of the attention / FFN sub-layer
@@ -52,7 +42,7 @@ struct dcb_engine {
   int R = 0, L = 0, Lw = 0, E = 0, Epad = 0, echunks = 0;   // Lw: tokens per window in the layout (>= L)
   PackedLayout pl{};
   int chunk_tiles = 0, chunk_windows = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   cudaStream_t stream = nullptr;        // compute (+ result D2H)
   cudaStream_t copy_stream = nullptr;   // H2D of the rows of the NEXT submission, overlapping the kernels of the current one
   cudaStream_t out_stream = nullptr;    // D2H of the results of the PREVIOUS submission, off the compute stream
@@ -76,19 +66,8 @@ struct dcb_engine {
   int64_t next_ticket = 0;
   bool weights_loaded = false;
   bool debug = false;
-  bool ffn_pair = true;
-  bool fuse_oproj = true;
-  bool fuse_embed = true;
-  bool fuse_qa = true;
-  bool fuse_head = DCB_FUSE_HEAD_DEFAULT != 0;   // head in the tail of the stack kernel (one pipelined pass over the row, the
-                           // gamma * Wfc table in the idle staging area): +1.7 % against the separate head_kernel, and the
-                           // residual image is never written back.  DCB_FUSE_HEAD=0 (developer build): head_kernel
-  bool stack = true;   // whole encoder stack in one launch (stack_pair_kernel) when the configuration allows it
-  bool qkv2 = false;   // measured: not faster than gemm_kernel<3,QKV> (both sit on the per-SM L2 port), kept as an option
-  bool fused_last = false;
-  bool stack_last = false;
   bool profile = false;
-  float prof_ms[6] = {0, 0, 0, 0, 0, 0};   // embed, gemm_row, qkv, attention, ffn(+out-proj), head
+  float prof_ms[6] = {0, 0, 0, 0, 0, 0};   // embed, gemm_row, qkv, attention, ffn, head
   int prof_n[6] = {0, 0, 0, 0, 0, 0};
   float prof_ffn_ms = 0.f;
   int prof_ffn_launches = 0;
@@ -101,7 +80,7 @@ struct dcb_engine {
   EmbedRow* d_rowmeta = nullptr;
   int table_elems = 0;
   __nv_bfloat16* d_tables = nullptr;
-  __nv_bfloat16* d_wc = nullptr;
+  __nv_bfloat16* d_wc = nullptr;   // split-bf16 condenser [2 Epad / 8][288][8]
   float* d_pe = nullptr;
   float* d_pe_img = nullptr;   // same table in residual-image order (window-aligned layout only)
   std::vector<LayerDev> layers;
@@ -112,6 +91,7 @@ struct dcb_engine {
   float* d_x = nullptr;
   __nv_bfloat16* d_xb = nullptr;
   __nv_bfloat16* d_att = nullptr;
+  __nv_bfloat16* d_hid = nullptr;   // FFN hidden activation, bf16 operand image [tile][ff/8][128][8]
   // stitch scratch (grown on demand)
   uint8_t *d_st_in = nullptr, *d_st_out = nullptr;   // [2][cap] each: bases|quals, seq|qual
   int32_t *d_st_start = nullptr, *d_st_len = nullptr;
@@ -185,6 +165,18 @@ std::vector<__nv_bfloat16> pack_b(int kpad, int n, const std::function<float(int
   return img;
 }
 
+// Split-bf16 B image [2 * kpad / 8][N][8]: the pack_b image of bf16(W), then that of bf16(W - bf16(W)).  The GEMM reads
+// its A k-steps twice against it, so the product carries the weight to ~16 mantissa bits.
+std::vector<__nv_bfloat16> pack_b_split(int kpad, int n, const std::function<float(int, int)>& w) {
+  std::vector<__nv_bfloat16> img = pack_b(kpad, n, w);
+  auto lo = pack_b(kpad, n, [&](int k, int nn) {
+    const float v = w(k, nn);
+    return v - __bfloat162float(__float2bfloat16(v));
+  });
+  img.insert(img.end(), lo.begin(), lo.end());
+  return img;
+}
+
 struct TensorMap {
   std::map<std::string, const dcb_tensor*> m;
   dcb_engine* e;
@@ -216,7 +208,7 @@ std::vector<float> pad288(const float* src, float scale = 1.f) {
 
 extern "C" {
 
-const char* dcb_version(void) { return "dcb200 0.1.0 (sm_100a)"; }
+const char* dcb_version(void) { return "dcb200 0.1.0 (sm_90a)"; }
 
 const char* dcb_last_error(const dcb_engine* e) { return e ? e->err.c_str() : g_create_error.c_str(); }
 
@@ -242,8 +234,8 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
     return fail(nullptr, DCB_ERR_CUDA, "no CUDA device available (the dcb200 engine has no CPU fallback)");
   if (cfg->device < 0 || cfg->device >= ndev) return fail(nullptr, DCB_ERR_INVALID, "bad device ordinal %d", cfg->device);
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 10)
-    return fail(nullptr, DCB_ERR_CUDA, "device %d is not an sm_100 GPU (compute capability %d.%d)", cfg->device,
+  if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 9)
+    return fail(nullptr, DCB_ERR_CUDA, "device %d is not an sm_90 GPU (compute capability %d.%d)", cfg->device,
                 prop.major, prop.minor);
 
   dcb_engine* e = new dcb_engine();
@@ -254,26 +246,14 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
   bool align = true;
   int ct = cfg->chunk_tiles;
 #ifdef DCB_DEV_SWITCHES
-  // Developer build only (libdcb200_dev.so, csrc/build.sh): environment switches that select the measured
-  // alternative kernel paths.  The product library ignores the environment.
+  // Developer build only (libdcb200_dev.so, csrc/build.sh): environment switches that select the alternative token
+  // layout and chunking.  The product library ignores the environment.
   if (const char* env = getenv("DCB_ALIGN")) align = atoi(env) != 0;
-  if (const char* env = getenv("DCB_FFN_PAIR")) e->ffn_pair = atoi(env) != 0;
-  if (const char* env = getenv("DCB_FUSE_OPROJ")) e->fuse_oproj = atoi(env) != 0;
-  if (const char* env = getenv("DCB_QKV2")) e->qkv2 = atoi(env) != 0;
-  if (const char* env = getenv("DCB_FUSE_EMBED")) e->fuse_embed = atoi(env) != 0;
-  if (const char* env = getenv("DCB_FUSE_QA")) e->fuse_qa = atoi(env) != 0;
-  if (const char* env = getenv("DCB_STACK")) e->stack = atoi(env) != 0;
-  if (const char* env = getenv("DCB_FUSE_HEAD")) e->fuse_head = atoi(env) != 0;
   if (const char* env = getenv("DCB_CHUNK_TILES")) ct = atoi(env);
 #endif
-  // window-aligned tiling: one window per 128-token tile when it fits (lets QKV + attention fuse);
-  // otherwise windows are packed back to back
+  // window-aligned tiling: one window per 128-token tile when it fits (the positional table is then read in residual-
+  // image order); otherwise windows are packed back to back
   if (align && e->L <= kTileM) e->Lw = kTileM;
-  // 128 < L <= 256: one window per tile PAIR, so that the one-kernel stack (a CTA pair per window, attention halo
-  // across the pair) applies -- when the rest of its conditions hold
-  else if (align && e->L <= 2 * kTileM && e->stack && cfg->attn_win_size > 0 && cfg->attn_win_size <= 16 &&
-           cfg->num_hidden_layers <= kMaxLayers)
-    e->Lw = 2 * kTileM;
   e->R = 4 * cfg->max_passes + (cfg->use_ccs_bq ? 6 : 5);  // data_providers.py:61-78
   e->pl = make_packed_layout(cfg->max_passes, cfg->max_length, cfg->use_ccs_bq ? 1 : 0);
   e->E = cfg->max_passes * (cfg->per_base_hidden_size + cfg->pw_hidden_size + cfg->ip_hidden_size +
@@ -316,6 +296,7 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
   TRY(dev_alloc(e, &e->d_x, T * x_image_elems()));
   TRY(dev_alloc(e, &e->d_xb, T * act_image_elems(kDP)));
   TRY(dev_alloc(e, &e->d_att, T * act_image_elems(kDP)));
+  TRY(dev_alloc(e, &e->d_hid, T * act_image_elems(cfg->filter_size)));
   const size_t mtok = (size_t)cfg->max_batch * e->L;
   for (auto& sl : e->slots) {
     TRY(dev_alloc(e, &sl.d_bases, mtok));
@@ -437,7 +418,7 @@ int dcb_load_weights(dcb_engine* e, const dcb_tensor* tensors, int32_t n) {
     const float* wc = tm.get("model/transformer_input_condenser/kernel", {e->E, kD}, &rc);
     if (rc) return rc;
     const int E = e->E;
-    auto img = pack_b(e->Epad, kDP, [&](int k, int nn) { return (k < E && nn < kD) ? wc[(size_t)k * kD + nn] : 0.f; });
+    auto img = pack_b_split(e->Epad, kDP, [&](int k, int nn) { return (k < E && nn < kD) ? wc[(size_t)k * kD + nn] : 0.f; });
     if ((rc = upload(e, &e->d_wc, img))) return rc;
   }
   // ---- positional encoding table [L][288] (tf-models RelativePositionEmbedding; networks.py:301-323)
@@ -467,33 +448,12 @@ int dcb_load_weights(dcb_engine* e, const dcb_tensor* tensors, int32_t n) {
   // ---- encoder layers
   const int ff = c.filter_size;
   e->layers.assign(c.num_hidden_layers, LayerDev());
-  std::vector<float> last_b2(kD, 0.f);   // output bias of the last layer's FFN (ReZero gain folded in), for the fused head
   for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
     LayerDev& ld = e->layers[n_];
     char pre[128];
     snprintf(pre, sizeof pre, "model/encoder_stack/layers/%d", n_);
     const std::string P0 = std::string(pre) + "/0", P1 = std::string(pre) + "/1";
     float alpha0 = 1.f, alpha1 = 1.f;
-    const float *gam[2] = {nullptr, nullptr}, *bet[2] = {nullptr, nullptr};   // pre-LN gamma / beta of the two sub-layers
-    // Padding rows 280..287 of a stack-kernel [kDP/8][n][8] image (common.h, StackParams).  beta != null: deferred
-    // LayerNorm, rows 0..279 hold bf16(gamma * W), wcol(k, nn) = the unfolded weight, extra(nn) = a bias that joins
-    // beta^T W.  beta == null (ReZero): only the bias rows.
-    auto deferred_rows = [&](std::vector<__nv_bfloat16>& part, int n, const float* beta,
-                             const std::function<float(int, int)>& wcol, const std::function<float(int)>& extra) {
-      for (int nn = 0; nn < n; ++nn) {
-        float cs = 0.f, bw = extra(nn);
-        for (int k = 0; beta && k < kD; ++k) {
-          cs += __bfloat162float(part[((size_t)(k / 8) * n + nn) * 8 + k % 8]);
-          bw += beta[k] * wcol(k, nn);
-        }
-        const __nv_bfloat16 ch = __float2bfloat16(cs), cl = __float2bfloat16(cs - __bfloat162float(ch));
-        const __nv_bfloat16 bh = __float2bfloat16(bw), bl = __float2bfloat16(bw - __bfloat162float(bh));
-        __nv_bfloat16* row = &part[((size_t)(kD / 8) * n + nn) * 8];
-        row[0] = ch; row[1] = cl; row[2] = ch; row[3] = cl;
-        row[4] = bh; row[5] = bl; row[6] = bh; row[7] = bl;
-      }
-    };
-    static_assert(kDP - kD == 8 && kD % 8 == 0, "deferred LayerNorm uses the eight padding rows of the operand tile");
     if (c.rezero) {
       const float* a0 = tm.get(P0 + "/alpha", std::initializer_list<int64_t>{}, &rc); if (rc) return rc;
       const float* a1 = tm.get(P1 + "/alpha", std::initializer_list<int64_t>{}, &rc); if (rc) return rc;
@@ -503,7 +463,6 @@ int dcb_load_weights(dcb_engine* e, const dcb_tensor* tensors, int32_t n) {
         const std::string P = s ? P1 : P0;
         const float* g = tm.get(P + "/layer_norm/gamma", {kD}, &rc); if (rc) return rc;
         const float* b = tm.get(P + "/layer_norm/beta", {kD}, &rc); if (rc) return rc;
-        gam[s] = g; bet[s] = b;
         if ((rc = upload(e, &ld.ln_g[s], pad288(g)))) return rc;
         if ((rc = upload(e, &ld.ln_b[s], pad288(b)))) return rc;
       }
@@ -514,11 +473,11 @@ int dcb_load_weights(dcb_engine* e, const dcb_tensor* tensors, int32_t n) {
     const float* wo = tm.get(P0 + "/layer/output_dense_layer/kernel", {kHeads, kDH, kD}, &rc); if (rc) return rc;
     const float qscale = 1.0f / sqrtf((float)kDH);  // query *= depth**-0.5 (attention_layer.py:196-197)
     {
-      // two n-groups of 432 columns: [q_h0 q_h1 k_h0 | k_h1 v_h0 v_h1], each slot 144 wide (140 + 4 zero)
+      // kQKVN / kQKVGroup n-groups of 288 columns: [q_h0 q_h1 | k_h0 k_h1 | v_h0 v_h1], each slot 144 wide (140 + 4 zero)
       std::vector<__nv_bfloat16> img;
-      for (int grp = 0; grp < 2; ++grp) {
-        auto part = pack_b(kDP, 3 * kNC, [&](int k, int nn) {
-          const int colg = grp * 3 * kNC + nn;
+      for (int grp = 0; grp < kQKVN / kQKVGroup; ++grp) {
+        auto part = pack_b_split(kDP, kQKVGroup, [&](int k, int nn) {
+          const int colg = grp * kQKVGroup + nn;
           const int slot = colg / kDHP, dd = colg % kDHP;
           if (k >= kD || dd >= kDH) return 0.f;
           const int proj = slot / kHeads, head = slot % kHeads;
@@ -529,155 +488,35 @@ int dcb_load_weights(dcb_engine* e, const dcb_tensor* tensors, int32_t n) {
         img.insert(img.end(), part.begin(), part.end());
       }
       if ((rc = upload(e, &ld.wqkv, img))) return rc;
-      // 9 column groups of 96 for qkv2_kernel
-      std::vector<__nv_bfloat16> img9;
-      for (int grp = 0; grp < kQKVN / 96; ++grp) {
-        auto part = pack_b(kDP, 96, [&](int k, int nn) {
-          const int colg = grp * 96 + nn;
-          const int slot = colg / kDHP, dd = colg % kDHP;
-          if (k >= kD || dd >= kDH) return 0.f;
-          const int proj = slot / kHeads, head = slot % kHeads;
-          const float* w = proj == 0 ? wq : (proj == 1 ? wk : wv);
-          const float v = w[((size_t)k * kHeads + head) * kDH + dd];
-          return proj == 0 ? v * qscale : v;
-        });
-        img9.insert(img9.end(), part.begin(), part.end());
-      }
-      __nv_bfloat16* dptr = nullptr;
-      if ((rc = upload(e, &dptr, img9))) return rc;
-      ld.wqkv2 = reinterpret_cast<uint8_t*>(dptr);
-      // fused QKV + attention (CTA pairs): for head h and rank rk the 216 rows of a k-step are
-      // [q_h | k_h | v_h], each the rk-th half (72 columns) of that 144-wide matrix
-      std::vector<__nv_bfloat16> imga;
-      for (int h = 0; h < kHeads; ++h)
-        for (int rk = 0; rk < 2; ++rk) {
-          auto part = pack_b(kDP, 3 * (kDHP / 2), [&](int k, int nn) {
-            const int m = nn / (kDHP / 2), dd = rk * (kDHP / 2) + nn % (kDHP / 2);
-            if (k >= kD || dd >= kDH) return 0.f;
-            const float* w = m == 0 ? wq : (m == 1 ? wk : wv);
-            const float v = w[((size_t)k * kHeads + h) * kDH + dd];
-            return m == 0 ? v * qscale : v;
-          });
-          imga.insert(imga.end(), part.begin(), part.end());
-        }
-      __nv_bfloat16* dptr2 = nullptr;
-      if ((rc = upload(e, &dptr2, imga))) return rc;
-      ld.wqa = reinterpret_cast<uint8_t*>(dptr2);
-      // stack kernel: one [36][72][8] block per (head, rank, q|k|v), consumed as three 6-k-step stages
-      std::vector<__nv_bfloat16> img3;
-      for (int h = 0; h < kHeads; ++h)
-        for (int rk = 0; rk < 2; ++rk)
-          for (int m = 0; m < 3; ++m) {
-            auto wval = [&](int k, int nn) {
-              const int dd = rk * (kDHP / 2) + nn;
-              if (k >= kD || dd >= kDH) return 0.f;
-              const float* w = m == 0 ? wq : (m == 1 ? wk : wv);
-              const float v = w[((size_t)k * kHeads + h) * kDH + dd];
-              return m == 0 ? v * qscale : v;
-            };
-            auto part = pack_b(kDP, kDHP / 2, [&](int k, int nn) {
-              return (gam[0] && k < kD) ? gam[0][k] * wval(k, nn) : wval(k, nn);     // pre-LN: gamma_0 folded into the rows
-            });
-            if (gam[0]) deferred_rows(part, kDHP / 2, bet[0], wval, [](int) { return 0.f; });
-            img3.insert(img3.end(), part.begin(), part.end());
-          }
-      __nv_bfloat16* dptr3 = nullptr;
-      if ((rc = upload(e, &dptr3, img3))) return rc;
-      ld.wq3 = reinterpret_cast<uint8_t*>(dptr3);
     }
     {
       // out-proj: K index = head*144 + dd, N = e; ReZero alpha folded in (encoder_stack.py:88-90)
-      auto img = pack_b(kDP, kDP, [&](int k, int nn) {
+      auto img = pack_b_split(kDP, kDP, [&](int k, int nn) {
         const int head = k / kDHP, dd = k % kDHP;
         if (dd >= kDH || nn >= kD) return 0.f;
         return wo[((size_t)head * kDH + dd) * kD + nn] * alpha0;
       });
       if ((rc = upload(e, &ld.wo, img))) return rc;
-      // CTA-pair halves: rank r holds, for each 144-wide N chunk j, output rows j*144 + r*72 + [0,72)
-      std::vector<__nv_bfloat16> img2;
-      for (int rk = 0; rk < 2; ++rk) {
-        auto part = pack_b(kDP, kDP / 2, [&](int k, int nn) {
-          const int col = (nn / (kNC / 2)) * kNC + rk * (kNC / 2) + nn % (kNC / 2);
-          const int head = k / kDHP, dd = k % kDHP;
-          if (dd >= kDH || col >= kD) return 0.f;
-          return wo[((size_t)head * kDH + dd) * kD + col] * alpha0;
-        });
-        img2.insert(img2.end(), part.begin(), part.end());
-      }
-      __nv_bfloat16* dptr = nullptr;
-      if ((rc = upload(e, &dptr, img2))) return rc;
-      ld.wo2 = reinterpret_cast<uint8_t*>(dptr);
     }
     const float* w1 = tm.get(P1 + "/layer/filter_dense_layer/kernel", {kD, ff}, &rc); if (rc) return rc;
     const float* b1 = tm.get(P1 + "/layer/filter_dense_layer/bias", {ff}, &rc); if (rc) return rc;
     const float* w2 = tm.get(P1 + "/layer/output_dense_layer/kernel", {ff, kD}, &rc); if (rc) return rc;
     const float* b2 = tm.get(P1 + "/layer/output_dense_layer/bias", {kD}, &rc); if (rc) return rc;
     {
+      // W1 in n-groups of kFFChunk hidden units, W2 as one [ff/8][288][8] image (ReZero alpha folded in)
+      const int gw = kFFChunk;
       std::vector<__nv_bfloat16> img;
-      img.reserve((size_t)ff * kDP * 2);
-      for (int ch = 0; ch < ff / kFFChunk; ++ch) {
-        auto p1 = pack_b(kDP, kFFChunk, [&](int k, int nn) {
-          return k < kD ? w1[(size_t)k * ff + ch * kFFChunk + nn] : 0.f;
-        });
-        auto p2 = pack_b(kFFChunk, kDP, [&](int k, int nn) {
-          return nn < kD ? w2[(size_t)(ch * kFFChunk + k) * kD + nn] * alpha1 : 0.f;
-        });
-        img.insert(img.end(), p1.begin(), p1.end());
-        img.insert(img.end(), p2.begin(), p2.end());
+      img.reserve((size_t)ff * kDP);
+      for (int grp = 0; grp < ff / gw; ++grp) {
+        auto part = pack_b(kDP, gw, [&](int k, int nn) { return k < kD ? w1[(size_t)k * ff + grp * gw + nn] : 0.f; });
+        img.insert(img.end(), part.begin(), part.end());
       }
-      __nv_bfloat16* dptr = nullptr;
-      if ((rc = upload(e, &dptr, img))) return rc;
-      ld.wffn = reinterpret_cast<uint8_t*>(dptr);
-    }
-    {
-      // CTA-pair image: rank r holds hidden units c*128 + r*64 + [0,64) of W1 and, for each 144-wide
-      // N chunk j of W2, output rows j*144 + r*72 + [0,72)
-      std::vector<__nv_bfloat16> img;
-      img.reserve((size_t)ff * kDP * 2);
-      for (int ch = 0; ch < ff / kFFChunk; ++ch)
-        for (int rk = 0; rk < 2; ++rk) {
-          auto p1 = pack_b(kDP, kFFChunk / 2, [&](int k, int nn) {
-            return k < kD ? w1[(size_t)k * ff + ch * kFFChunk + rk * (kFFChunk / 2) + nn] : 0.f;
-          });
-          auto p2 = pack_b(kFFChunk, kDP / 2, [&](int k, int nn) {
-            const int col = (nn / (kNC / 2)) * kNC + rk * (kNC / 2) + nn % (kNC / 2);
-            return col < kD ? w2[(size_t)(ch * kFFChunk + k) * kD + col] * alpha1 : 0.f;
-          });
-          img.insert(img.end(), p1.begin(), p1.end());
-          img.insert(img.end(), p2.begin(), p2.end());
-        }
-      __nv_bfloat16* dptr = nullptr;
-      if ((rc = upload(e, &dptr, img))) return rc;
-      ld.wffn2 = reinterpret_cast<uint8_t*>(dptr);
-      {
-        // the stack kernel's copy: b1 in the padding rows of W1; pre-LN models: gamma_1 folded in, deferred-LayerNorm rows
-        std::vector<__nv_bfloat16> imgs;
-        imgs.reserve(img.size());
-        for (int ch = 0; ch < ff / kFFChunk; ++ch)
-          for (int rk = 0; rk < 2; ++rk) {
-            const int c0 = ch * kFFChunk + rk * (kFFChunk / 2);
-            auto w1col = [&](int k, int nn) { return k < kD ? w1[(size_t)k * ff + c0 + nn] : 0.f; };
-            auto p1 = pack_b(kDP, kFFChunk / 2, [&](int k, int nn) { return (gam[1] && k < kD) ? gam[1][k] * w1col(k, nn) : w1col(k, nn); });
-            deferred_rows(p1, kFFChunk / 2, bet[1], w1col, [&](int nn) { return b1[c0 + nn]; });
-            auto p2 = pack_b(kFFChunk, kDP / 2, [&](int k, int nn) {
-              const int col = (nn / (kNC / 2)) * kNC + rk * (kNC / 2) + nn % (kNC / 2);
-              return col < kD ? w2[(size_t)(ch * kFFChunk + k) * kD + col] * alpha1 : 0.f;
-            });
-            imgs.insert(imgs.end(), p1.begin(), p1.end());
-            imgs.insert(imgs.end(), p2.begin(), p2.end());
-          }
-        __nv_bfloat16* dps = nullptr;
-        if ((rc = upload(e, &dps, imgs))) return rc;
-        ld.wffn2s = reinterpret_cast<uint8_t*>(dps);
-      }
+      if ((rc = upload(e, &ld.w1, img))) return rc;
+      auto img2 = pack_b(ff, kDP, [&](int k, int nn) { return nn < kD ? w2[(size_t)k * kD + nn] * alpha1 : 0.f; });
+      if ((rc = upload(e, &ld.w2, img2))) return rc;
     }
     if ((rc = upload(e, &ld.b1, std::vector<float>(b1, b1 + ff)))) return rc;
     if ((rc = upload(e, &ld.b2, pad288(b2, alpha1)))) return rc;
-    last_b2.assign(kD, 0.f);
-    for (int k = 0; k < kD; ++k) last_b2[k] = b2[k] * alpha1;      // what the stack kernel adds to Y after this layer
-    ld.b2_mean = 0.f;
-    for (int k = 0; k < kD; ++k) ld.b2_mean += last_b2[k];
-    ld.b2_mean /= (float)kD;
   }
   // ---- head
   {
@@ -690,23 +529,15 @@ int dcb_load_weights(dcb_engine* e, const dcb_tensor* tensors, int32_t n) {
     if ((rc = upload(e, &e->d_wfc, std::vector<float>(w, w + kD * kVocab)))) return rc;
     if ((rc = upload(e, &e->d_bfc, std::vector<float>(bb, bb + kVocab)))) return rc;
     // head_kernel folds the final LayerNorm into the fc1 sums (one pass over the row): logits_j = rstd * (sum_c y_c g_c W_cj
-    // - mean_y * A_j) + B_j + bfc_j.  The products are formed here once, in float32 in the same order the kernel used to.
-    // The fused tail of the stack kernel works on Y = x - b2 (b2 of the last layer joins here): column 5 of the table and
-    // H_j, sum b2, sum b2^2 carry it (stack_kernel.cuh, fused head).
-    std::vector<float> gw8((size_t)kD * 8, 0.f), ab(32, 0.f);
-    for (int cc = 0; cc < kD; ++cc) {
+    // - mean_y * A_j) + B_j + bfc_j.  The products are formed here once, in float32.
+    std::vector<float> gw8((size_t)kD * 8, 0.f), ab(16, 0.f);
+    for (int cc = 0; cc < kD; ++cc)
       for (int j = 0; j < kVocab; ++j) gw8[(size_t)cc * 8 + j] = g[cc] * w[cc * kVocab + j];
-      gw8[(size_t)cc * 8 + 5] = last_b2[cc];
-    }
     for (int j = 0; j < kVocab; ++j) {
-      float a = 0.f, bsum = 0.f, h = 0.f;
-      for (int cc = 0; cc < kD; ++cc) {
-        a += g[cc] * w[cc * kVocab + j]; bsum += b[cc] * w[cc * kVocab + j];
-        h += last_b2[cc] * (g[cc] * w[cc * kVocab + j]);
-      }
-      ab[j] = a; ab[8 + j] = bsum; ab[16 + j] = h;
+      float a = 0.f, bsum = 0.f;
+      for (int cc = 0; cc < kD; ++cc) { a += g[cc] * w[cc * kVocab + j]; bsum += b[cc] * w[cc * kVocab + j]; }
+      ab[j] = a; ab[8 + j] = bsum;
     }
-    for (int cc = 0; cc < kD; ++cc) { ab[24] += last_b2[cc]; ab[25] += last_b2[cc] * last_b2[cc]; }
     if ((rc = upload(e, &e->d_head_gw8, gw8))) return rc;
     if ((rc = upload(e, &e->d_head_ab, ab))) return rc;
   }
@@ -899,15 +730,12 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
     CU(e, cudaStreamWaitEvent(st, sl.rows_ready, 0));
   }
   const uint8_t* packed_base = packed ? (rows_dev ? packed : sl.d_packed) : nullptr;
-  // the embedding kernel reads packed rows directly on the window-aligned fast path; every other path gets the float32
-  // rows they stand for
-  const bool packed_direct = packed_base && !strict && e->fuse_embed && embed_condense_reads_packed(L, e->Lw) &&
-                             embed_condense_smem_bytes(R, e->echunks, e->table_elems, e->pl.stride) <= 225 * 1024;
-  if (packed_base && !packed_direct) launch_unpack_rows(packed_base, e->pl, batch, sl.d_rows, st);
+  // the default path's embedding kernel reads packed rows directly; the strict path gets the float32 rows they stand for
+  if (packed_base && strict) launch_unpack_rows(packed_base, e->pl, batch, sl.d_rows, st);
   const float* rows_base = packed ? sl.d_rows : (rows_dev ? rows : sl.d_rows);
   CU(e, cudaMemsetAsync(sl.d_status, 0, sizeof(int), st));
   CU(e, cudaEventRecord(sl.ev0, st));
-  int launches = (packed_base && !packed_direct) ? 1 : 0;
+  int launches = (packed_base && strict) ? 1 : 0;
   const size_t ximg = x_image_elems();
   bool prof_err = false;
   auto pbegin = [&](int kind) {
@@ -946,7 +774,6 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
       const int bw = std::min(e->strict.chunk_windows, batch - w0);
       launches += strict_forward_chunk(e, rows_base + (size_t)w0 * R * L, bw, make_head_at(w0), sl.d_status, st);
     }
-    e->stack_last = false;
   }
   for (int w0 = 0; !strict && w0 < batch; w0 += e->chunk_windows) {
     const int bw = std::min(e->chunk_windows, batch - w0);
@@ -964,116 +791,61 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
       hp.M = M; hp.L = L; hp.Lw = Lw;
       return hp;
     };
-    const bool use_stack = e->stack && e->fuse_qa && e->ffn_pair && e->fuse_oproj && e->fuse_embed && !e->debug &&
-                           (Lw == kTileM || (Lw == 2 * kTileM && L > kTileM)) &&
-                           c.attn_win_size > 0 && c.attn_win_size <= 16 && c.num_hidden_layers <= kMaxLayers;
     {
       RowEpi epi{};
-      // the one-kernel stack builds every operand tile from the residual in TMEM: no bf16 operand image needed
-      epi.x = e->d_x; epi.xb = use_stack ? nullptr : e->d_xb; epi.bias = nullptr;
+      epi.x = e->d_x; epi.xb = e->d_xb; epi.bias = nullptr;
       epi.pe = c.add_pos_encoding ? e->d_pe : nullptr;
       epi.pe_img = c.add_pos_encoding ? e->d_pe_img : nullptr;
-      epi.ln_g = (c.rezero || use_stack) ? nullptr : e->layers[0].ln_g[0];
-      epi.ln_b = (c.rezero || use_stack) ? nullptr : e->layers[0].ln_b[0];
+      epi.ln_g = c.rezero ? nullptr : e->layers[0].ln_g[0];
+      epi.ln_b = c.rezero ? nullptr : e->layers[0].ln_b[0];
       epi.has_xold = 0; epi.L = Lw;
-      bool fused_embed = false;
-      if (e->fuse_embed) {
-        pbegin(1);
-        fused_embed = launch_embed_condense(rows_chunk, packed_direct ? packed_base + (size_t)w0 * e->pl.stride : nullptr, e->pl,
-                                            R, L, Lw, M, T, e->echunks, e->d_cols, e->d_rowmeta, e->d_tables,
-                                            e->table_elems, e->d_wc, epi, sl.d_status, st);
-        if (!fused_embed && packed_direct) return fail(e, DCB_ERR_INVALID, "internal: packed rows on a path that cannot read them");
-        pend();
-        if (fused_embed) ++launches;
-      }
-      if (!fused_embed) {
-        pbegin(0);
-        launch_embed(rows_chunk, R, L, Lw, M, T, e->echunks, e->d_cols, e->d_rowmeta, e->d_tables, e->table_elems, e->d_embqkv, sl.d_status, st);
-        pend();
-        pbegin(1);
-        launch_gemm_row(e->d_embqkv, e->d_wc, e->Epad / 16, T, epi, st);
-        pend();
-        launches += 2;
-      }
+      pbegin(0);
+      launch_embed(packed_base ? nullptr : rows_chunk, packed_base ? packed_base + (size_t)w0 * e->pl.stride : nullptr, e->pl,
+                   R, L, Lw, M, T, e->echunks, e->d_cols, e->d_rowmeta, e->d_tables, e->table_elems, e->d_embqkv, sl.d_status, st);
+      pend();
+      pbegin(1);
+      launch_gemm_row(e->d_embqkv, e->d_wc, e->Epad / 16, 2 * (e->Epad / 16), T, epi, st);
+      pend();
+      launches += 2;
       snap();
     }
-    if (use_stack) {
-      StackParams sp{};
-      sp.num_layers = c.num_hidden_layers;
-      sp.ff = c.filter_size;
-      sp.deferred_ln = c.rezero ? 0 : 1;
-      for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
-        const LayerDev& ld = e->layers[n_];
-        sp.wq3[n_] = ld.wq3; sp.wo2[n_] = ld.wo2; sp.wffn2[n_] = ld.wffn2s;
-        sp.b2[n_] = ld.b2; sp.b2_mean[n_] = ld.b2_mean;
-      }
-      HeadParams hs{};
-      if (e->fuse_head) { hs = make_head(); }
-      pbegin(4);
-      launch_stack(e->d_x, T, L, c.attn_win_size, sp, hs, st);
-      pend();
-      if (e->profile) e->prof_ffn_tokens += (long long)bw * L;
-      e->fused_last = true;
-      e->stack_last = true;
-      ++launches;
-    } else e->stack_last = false;
-    for (int n_ = 0; !use_stack && n_ < c.num_hidden_layers; ++n_) {
+    for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
       const LayerDev& ld = e->layers[n_];
       const bool last = n_ + 1 == c.num_hidden_layers;
-      if (e->fuse_qa && Lw == kTileM) {
-        pbegin(2);
-        launch_qkv_attn(e->d_xb, ld.wqa, T, L, c.attn_win_size, e->d_att, st);
-        pend();
-        --launches;   // one launch instead of two (3 per layer are added below)
-      } else {
-        pbegin(2);
-        if (e->qkv2) launch_qkv2(e->d_xb, ld.wqkv2, T, e->d_embqkv, st);
-        else launch_gemm_qkv(e->d_xb, ld.wqkv, T, e->d_embqkv, st);
-        pend();
-        pbegin(3);
-        launch_attention(e->d_embqkv, e->d_att, L, Lw, c.attn_win_size, bw, st);
-        pend();
-      }
-      // attention out-proj + FFN: fused into one CTA-pair kernel unless debugging the intermediate
-      const bool fused = e->ffn_pair && e->fuse_oproj && !e->debug;
+      pbegin(2);
+      launch_gemm_qkv(e->d_xb, ld.wqkv, T, e->d_embqkv, st);
+      pend();
+      pbegin(3);
+      launch_attention(e->d_embqkv, e->d_att, L, Lw, c.attn_win_size, bw, st);
+      pend();
+      // attention out-projection + residual; xb = the FFN sub-layer's input (pre-LayerNorm or identity)
+      RowEpi ea{};
+      ea.x = e->d_x; ea.xb = e->d_xb; ea.bias = nullptr; ea.pe = nullptr;
+      ea.ln_g = c.rezero ? nullptr : ld.ln_g[1];
+      ea.ln_b = c.rezero ? nullptr : ld.ln_b[1];
+      ea.has_xold = 1; ea.L = Lw;
+      pbegin(1);
+      launch_gemm_row(e->d_att, ld.wo, kDP / 16, 2 * (kDP / 16), T, ea, st);
+      pend();
+      snap();
+      // FFN: hidden = relu(xb W1 + b1), then hidden W2 + b2 + residual; xb = the next layer's input
       RowEpi ef{};
       ef.x = e->d_x; ef.xb = last ? nullptr : e->d_xb; ef.bias = ld.b2; ef.pe = nullptr;
       ef.ln_g = (c.rezero || last) ? nullptr : e->layers[n_ + 1].ln_g[0];
       ef.ln_b = (c.rezero || last) ? nullptr : e->layers[n_ + 1].ln_b[0];
       ef.has_xold = 1; ef.L = Lw;
-      if (!fused) {
-        RowEpi ea{};
-        ea.x = e->d_x; ea.xb = e->d_xb; ea.bias = nullptr; ea.pe = nullptr;
-        ea.ln_g = c.rezero ? nullptr : ld.ln_g[1];
-        ea.ln_b = c.rezero ? nullptr : ld.ln_b[1];
-        ea.has_xold = 1; ea.L = Lw;
-        pbegin(1);
-        launch_gemm_row(e->d_att, ld.wo, kDP / 16, T, ea, st);
-        pend();
-        ++launches;
-        snap();
-      }
       pbegin(4);
-      if (fused)
-        launch_ffn_pair(e->d_att, ld.wffn2, ld.b1, c.filter_size, T, ef, st, ld.wo2,
-                        c.rezero ? nullptr : ld.ln_g[1], c.rezero ? nullptr : ld.ln_b[1]);
-      else if (e->ffn_pair)
-        launch_ffn_pair(e->d_xb, ld.wffn2, ld.b1, c.filter_size, T, ef, st);
-      else
-        launch_ffn(e->d_xb, ld.wffn, ld.b1, c.filter_size, T, ef, st);
+      launch_ffn_up(e->d_xb, ld.w1, ld.b1, c.filter_size, T, e->d_hid, st);
+      launch_gemm_row(e->d_hid, ld.w2, c.filter_size / 16, c.filter_size / 16, T, ef, st);
       pend();
       if (e->profile) e->prof_ffn_tokens += (long long)bw * L;   // valid tokens (layout padding is not algorithmic work)
-      if (!fused) snap();
-      e->fused_last = fused;
-      launches += 3;
+      snap();
+      launches += 5;
     }
-    const bool head_done = use_stack && e->fuse_head;
-    if (!head_done) {
-      pbegin(5);
-      launch_head(make_head(), T, st);
-      pend();
-      ++launches;
-    }
+    pbegin(5);
+    launch_head(make_head(), T, st);
+    pend();
+    ++launches;
     e->last_chunk_tokens = M;
   }
   CU(e, cudaEventRecord(sl.ev1, st));
@@ -1232,10 +1004,9 @@ int dcb_get_profile(dcb_engine* e, float* ffn_ms_total, int32_t* ffn_launches, i
   return DCB_OK;
 }
 
-int dcb_get_profile_kernels(dcb_engine* e, float* ms6, int32_t* n6, int32_t* fused_oproj) {
-  if (!e || !ms6 || !n6 || !fused_oproj) return DCB_ERR_INVALID;
+int dcb_get_profile_kernels(dcb_engine* e, float* ms6, int32_t* n6) {
+  if (!e || !ms6 || !n6) return DCB_ERR_INVALID;
   for (int i = 0; i < 6; ++i) { ms6[i] = e->prof_ms[i]; n6[i] = e->prof_n[i]; }
-  *fused_oproj = e->stack_last ? 2 : (e->fused_last ? 1 : 0);   // 2: whole stack in one kernel
   return DCB_OK;
 }
 
@@ -1470,9 +1241,6 @@ int dcb_fill_skipped(dcb_engine* e, const uint8_t* ccs_ids, const int16_t* ccs_b
   return DCB_OK;
 }
 
-int dcb_debug_trace(uint64_t* out, int32_t n) {
-  return read_ffn_trace(reinterpret_cast<unsigned long long*>(out), n) ? DCB_ERR_CUDA : DCB_OK;
-}
 
 int dcb_alloc_host(size_t bytes, void** out) {
   if (!out) return DCB_ERR_INVALID;

@@ -1,4 +1,4 @@
-// Per-token epilogue shared by head_kernel, the fused tail of stack_pair_kernel and the strict-fp32 head.
+// Per-token epilogue shared by head_kernel and the strict-fp32 head.
 #pragma once
 #include <math.h>
 
@@ -7,7 +7,7 @@
 namespace dcb {
 
 // logits (+ fc1 bias) -> softmax -> argmax -> Phred -> calibration -> cap / round -> ASCII, for one token
-// (networks.py:238, quick_inference.py:377-414).  Shared by head_kernel and the fused tail of stack_pair_kernel.
+// (networks.py:238, quick_inference.py:377-414).
 __device__ __forceinline__ void head_finish(const HeadParams& p, float (&lg)[kVocab], size_t oidx) {
   float mx = -INFINITY;
 #pragma unroll

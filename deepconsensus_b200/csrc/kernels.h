@@ -9,48 +9,25 @@ namespace dcb {
 cudaError_t kernels_init();
 
 size_t embed_smem_bytes(int R, int echunks, int table_elems);
-void launch_embed(const float* rows, int R, int L, int Lw, int M, int ntiles, int echunks,
+// `packed` != null: the rows are read from packed input rows (include/dcb200.h) instead of `rows`.
+void launch_embed(const float* rows, const uint8_t* packed, const PackedLayout& pl, int R, int L, int Lw, int M, int ntiles, int echunks,
                   const EmbedCol* cols, const EmbedRow* rowmeta, const __nv_bfloat16* tables,
                   int table_elems, __nv_bfloat16* emb, int* status, cudaStream_t st);
-// D = A * B^T with the 288-wide row epilogue (condenser + pos-enc, attention out-proj).
-void launch_gemm_row(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int ksteps, int ntiles,
+// D = A * B^T with the 288-wide row epilogue (condenser + pos-enc, attention out-proj, FFN down-projection).
+// b_ksteps == 2 * a_ksteps: b_img holds split-bf16 weights [W_hi; W_lo] along K (kernels.cu, gemm_kernel).
+void launch_gemm_row(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int a_ksteps, int b_ksteps, int ntiles,
                      const RowEpi& epi, cudaStream_t st);
-// fused q/k/v projection: A [tile][36][128][8] -> qkv image [tile][108][128][8]
+// fused q/k/v projection: A [tile][36][128][8] -> qkv image [tile][108][128][8]; b_img: kQKVN / kQKVGroup groups of
+// split-bf16 weights [72][kQKVGroup][8] (hi chunks, then lo chunks)
 void launch_gemm_qkv(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int ntiles,
                      __nv_bfloat16* qkv_img, cudaStream_t st);
-// fused embedding + condenser (+pos-enc, residual image, next operand); false if it does not fit smem
-size_t embed_condense_smem_bytes(int R, int echunks, int table_elems, int packed_stride);
-// `packed` != null: read the packed rows (include/dcb200.h) instead of `rows`; only when embed_condense_reads_packed().
-bool embed_condense_reads_packed(int L, int Lw);
-bool launch_embed_condense(const float* rows, const uint8_t* packed, const PackedLayout& pl, int R, int L, int Lw, int M,
-                           int ntiles, int echunks, const EmbedCol* cols,
-                           const EmbedRow* rowmeta, const __nv_bfloat16* tables, int table_elems,
-                           const __nv_bfloat16* wc_img, const RowEpi& epi, int* status, cudaStream_t st);
+// FFN up-projection: hid = relu(A W1 + b1) as a bf16 operand image [tile][ff/8][128][8]; w1_img: ff / kFFChunk groups
+// of [36][kFFChunk][8]
+void launch_ffn_up(const __nv_bfloat16* a_img, const __nv_bfloat16* w1_img, const float* b1, int ff, int ntiles,
+                   __nv_bfloat16* hid_img, cudaStream_t st);
 void launch_unpack_rows(const uint8_t* packed, const PackedLayout& pl, int nwindows, float* rows, cudaStream_t st);
-// two-tiles-per-weight-pass QKV projection; b_img: 9 groups x [36][96][8]
-void launch_qkv2(const __nv_bfloat16* a_img, const uint8_t* b_img, int ntiles, __nv_bfloat16* qkv_img,
-                 cudaStream_t st);
-// fused QKV projection + banded attention on window-aligned tiles (Lw == 128); w_img: per (head, rank)
-// [18 k-steps][2][216][8] with rows = [q|k|v] halves
-void launch_qkv_attn(const __nv_bfloat16* a_img, const uint8_t* w_img, int ntiles, int L, int win,
-                     __nv_bfloat16* att, cudaStream_t st);
 void launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* att, int L, int Lw, int win, int nwindows,
                       cudaStream_t st);
-// CTA-pair (cta_group::2) version; w2img is the per-rank half-chunk weight image.
-// With wo2img != null the attention out-projection (+ residual, + pre-norm `mid_ln_*` or identity) is
-// fused in front: a_img is then the attention operand image and epi.x the residual before the
-// attention sub-layer.
-void launch_ffn_pair(const __nv_bfloat16* a_img, const uint8_t* w2img, const float* b1, int ff, int ntiles,
-                     const RowEpi& epi, cudaStream_t st, const uint8_t* wo2img = nullptr,
-                     const float* mid_ln_g = nullptr, const float* mid_ln_b = nullptr);
-void launch_ffn(const __nv_bfloat16* a_img, const uint8_t* w_img, const float* b1, int ff, int ntiles,
-                const RowEpi& epi, cudaStream_t st);
-// The whole encoder stack in one launch (window-aligned tiles, attn_win_size in [1,16]): x is the fp32 residual
-// image written by the embedding kernel.  hp.bases != null: the head (final LayerNorm, fc1, softmax, argmax, Phred,
-// calibration, ASCII) runs in the kernel's tail and x is not written back; otherwise x returns the output of the last
-// layer for launch_head.
-void launch_stack(float* x, int ntiles, int L, int win, const StackParams& p, const HeadParams& hp, cudaStream_t st);
-int read_ffn_trace(unsigned long long* out, int n);
 void launch_head(const HeadParams& p, int ntiles, cudaStream_t st);
 // per-read window concatenation + gap compaction; read z = windows [zmw_start[z], zmw_start[z+1]) (device pointers)
 void launch_stitch(const uint8_t* bases, const uint8_t* quals, int L, const int32_t* zmw_start, int n_zmw,

@@ -1,4 +1,4 @@
-// Post-model stage of the path on the device (SURVEY.md section 8(f)2): what `stitch_utils.stitch_to_fastq` and the
+// Post-model stage of the path on the device : what `stitch_utils.stitch_to_fastq` and the
 // skip branch of `inference_on_n_zmws` do per read / per window after the model, as integer / byte kernels.
 //
 //   read_outcome_kernel   per read: missing-window check of get_full_sequence (stitch_utils.py:60-78), only-gaps check,

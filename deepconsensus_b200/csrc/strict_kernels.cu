@@ -3,12 +3,12 @@
 // float32 and every Keras layer below runs in float32).  Selected per engine (dcb_config.precision =
 // DCB_PRECISION_FP32) or per call (DCB_STRICT_FP32).
 //
-// What it is for: the default path rounds tensor-core operands to bf16 (DESIGN.md section 4), which moves logits by
+// What it is for: the default path rounds tensor-core operands to bf16, which moves logits by
 // 0.02-0.1 and flips the argmax at near-ties.  This path differs from the reference's float32 graph only by summation
 // order (measured ~1e-5 on logits), so it produces identical bases wherever the float32 top-2 margin exceeds 1e-3 and
 // is the on-device yardstick the default path is compared with at full batch sizes (bench.py "parity", tests).
 //
-// It runs on the CUDA cores (the tensor cores have no float32-operand mode: kind::tf32 keeps 10 mantissa bits), as
+// It runs on the CUDA cores (the tensor cores have no float32-operand mode: tf32 keeps 10 mantissa bits), as
 // plain global-memory kernels, row-major [tokens, features] activations, windows packed back to back:
 //
 //   strict_embed_kernel     format_rows clip + id + gather + sqrt(width) scale + zero-at-id-0 + concat

@@ -8,7 +8,7 @@
   * `model.forward(rows)` -> base / quality characters straight from the device epilogue
     (what quick_inference.py:377-414 computes on the host).
 
-There is no CPU fallback: if the CUDA library is missing or no sm_100 GPU is present,
+There is no CPU fallback: if the CUDA library is missing or no sm_90 GPU is present,
 construction raises.
 """
 from __future__ import annotations
@@ -85,7 +85,7 @@ ABI_SYMBOLS = (
     "dcb_synchronize", "dcb_last_error", "dcb_version", "dcb_destroy",
 )
 # include/dcb200_debug.h: developer / test hooks, not part of the drop-in boundary
-DEBUG_SYMBOLS = ("dcb_set_debug", "dcb_debug_residual", "dcb_debug_trace")
+DEBUG_SYMBOLS = ("dcb_set_debug", "dcb_debug_residual")
 
 
 def library_path() -> str:
@@ -105,7 +105,7 @@ _dev_lib = None
 
 def load_dev_library() -> ctypes.CDLL:
   """libdcb200_dev.so: the same sources built with -DDCB_DEV_SWITCHES, where DCB_* environment variables select the
-  measured alternative kernel paths (tests and scripts only; pass as B200Model(..., library=...))."""
+  alternative token layout and chunking (tests and scripts only; pass as B200Model(..., library=...))."""
   global _dev_lib
   if _dev_lib is None:
     _dev_lib = _load(os.path.join(os.path.dirname(_LIB_PATH), "libdcb200_dev.so"))
@@ -140,8 +140,7 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_set_profile.argtypes = [vp, i32]
   lib.dcb_get_profile.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(i32),
                                   ctypes.POINTER(ctypes.c_int64)]
-  lib.dcb_get_profile_kernels.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(i32),
-                                          ctypes.POINTER(i32)]
+  lib.dcb_get_profile_kernels.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(i32)]
   lib.dcb_debug_residual.argtypes = [vp, i32, vp, ctypes.c_int64]
   lib.dcb_alloc_host.argtypes = [ctypes.c_size_t, ctypes.POINTER(vp)]
   lib.dcb_free_host.argtypes = [vp]
@@ -205,7 +204,7 @@ class _Prediction:
 
 
 class B200Model:
-  """The encoder-only learned-values transformer on one B200, behind the C-ABI."""
+  """The encoder-only learned-values transformer on one H100, behind the C-ABI."""
 
   def __init__(self, params: params_lib.Params, weights: weights_lib.Weights, max_batch: int = 1024,
                device: int = 0, max_base_quality: int = 93,
@@ -305,7 +304,7 @@ class B200Model:
     self.last_ms, self.last_launches = ms, launches
     return out
 
-  # -- packed input rows (include/dcb200.h "packed input rows"; SURVEY.md section 8(f)1) -------------------------
+  # -- packed input rows (include/dcb200.h "packed input rows")1) -------------------------
   @property
   def packed_window_bytes(self) -> int:
     return packed_window_bytes(self.params)
@@ -592,11 +591,10 @@ class B200Model:
     ms, n, tok = ctypes.c_float(), ctypes.c_int32(), ctypes.c_int64()
     self._check(self._lib.dcb_get_profile(self._handle, ctypes.byref(ms), ctypes.byref(n),
                                           ctypes.byref(tok)))
-    ms6, n6, fused = (ctypes.c_float * 6)(), (ctypes.c_int32 * 6)(), ctypes.c_int32()
-    self._check(self._lib.dcb_get_profile_kernels(self._handle, ms6, n6, ctypes.byref(fused)))
+    ms6, n6 = (ctypes.c_float * 6)(), (ctypes.c_int32 * 6)()
+    self._check(self._lib.dcb_get_profile_kernels(self._handle, ms6, n6))
     names = ("embed", "row_gemm", "qkv_gemm", "attention", "ffn", "head")
     return dict(ffn_ms_total=float(ms.value), ffn_launches=int(n.value), ffn_tokens=int(tok.value),
-                fused_oproj=int(fused.value),   # 0: separate out-proj, 1: fused into the FFN kernel, 2: whole stack in one kernel
                 kernels={k: dict(ms=float(ms6[i]), launches=int(n6[i])) for i, k in enumerate(names)})
 
   def set_debug(self, enabled: bool = True) -> None:

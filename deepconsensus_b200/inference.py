@@ -315,7 +315,7 @@ def _as_str(x) -> str:
 
 
 def load_weights_npz(path: str) -> weights_lib.Weights:
-  """Variables exported as an .npz keyed by the checkpoint variable names (SURVEY.md Appendix B)."""
+  """Variables exported as an .npz keyed by the checkpoint variable names."""
   with np.load(path) as z:
     return {k: z[k] for k in z.files}
 

@@ -1,5 +1,5 @@
 """Work split for multi-GPU runs: windows are independent units, so a ZMW batch is sharded across
-ranks with no data-path collective (SURVEY.md section 8e).
+ranks with no data-path collective.
 
 Shards are ZMW-granular (all windows of a molecule stay on one rank so `stitch_to_fastq`, which
 runs per ZMW after the model -- quick_inference.py:721-736 -- needs no cross-rank merge) and assigned
@@ -46,7 +46,7 @@ def reduce_counters(counters: Dict[str, int], group=None) -> Dict[str, int]:
 class ScatterFeeder:
   """BASELINE configs[3]: ONE reader rank holds the packed rows of a whole step and deals one chunk to every rank
   (itself included) -- grouped point-to-point sends / receives, i.e. ncclGroupStart; ncclSend(chunk_r -> r) for all r;
-  ncclRecv; ncclGroupEnd (SURVEY.md section 8e) -- and collects every rank's base / quality characters the same way.
+  ncclRecv; ncclGroupEnd -- and collects every rank's base / quality characters the same way.
 
   Double-buffered: `scatter(step)` posts the transfers of step k+1 asynchronously while the caller scores step k out of
   the other buffer; `wait()` blocks the host until the posted transfers have landed (the engine runs on its own

@@ -54,7 +54,7 @@ def compare(test: Dict[str, np.ndarray], ref: Dict[str, np.ndarray], margin: flo
 
 
 def summary(stats: Dict[str, float], digits: int = 4) -> Dict[str, float]:
-  """The four numbers BASELINE.md section 3.4 asks to travel with every throughput number (+ their context)."""
+  """The four parity numbers that travel with every throughput number (+ their context)."""
   keys = ("bases_identical_pct", "qv_exact_pct", "max_dq", "max_logit_err", "rms_logit_err", "positions",
           "base_mismatches", "base_mismatches_outside_margin", "largest_margin_of_a_mismatch", "margin", "expected_flips")
   return {k: (round(v, digits) if isinstance(v, float) else v) for k, v in stats.items() if k in keys}

@@ -2,7 +2,7 @@
 
 Layout and value ranges follow the reference's feature construction
 (pre_lib.py:704-744; row order data_providers.py:81-113) and the statistics of the
-real fixture windows (SURVEY.md Appendix D / section 8d):
+real fixture windows:
 
   * bases / ccs rows: ids 0..4 (' ATCG'), gaps where the alignment has none;
   * pw / ip rows: small integers (geometric), 0 wherever the base is a gap
@@ -66,8 +66,7 @@ def mean_drift_weights(params: params_lib.Params, weights, w2_offset: float = 0.
                        wo_offset: float = 0.2):
   """A copy of `weights` whose sub-layer outputs carry a large common-mode component (a constant added to the attention
   output kernel, the FFN output kernel and the FFN output bias of every layer): the residual rows' mean runs away from
-  zero while their spread stays put.  LayerNorm removes it in exact arithmetic; an engine that rounds operands around a
-  stale mean does not (tests of the stack kernel's re-centring guard)."""
+  zero while their spread stays put.  LayerNorm removes it in exact arithmetic; the engine's fp32 LayerNorm must too."""
   out = dict(weights)
   for n in range(params.num_hidden_layers):
     pre = "model/encoder_stack/layers/%d" % n

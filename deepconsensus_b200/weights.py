@@ -2,7 +2,7 @@
 
 Names and shapes are those of the TF object-graph checkpoint the reference
 restores in `initialize_model` (quick_inference.py:515-529); the list was read
-from `testdata/model/checkpoint-1.index` (SURVEY.md Appendix B).  A weight set
+from `testdata/model/checkpoint-1.index`.  A weight set
 here is a plain `dict[str, np.ndarray(float32)]` keyed by those names (without
 the `/.ATTRIBUTES/VARIABLE_VALUE` suffix).
 

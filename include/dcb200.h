@@ -1,4 +1,4 @@
-/* dcb200 -- C ABI of the B200-native DeepConsensus model path.
+/* dcb200 -- C ABI of the H100-native (sm_90a) DeepConsensus model path.
  *
  * This is the drop-in boundary for the one hot path of google/deepconsensus (v1.2.0):
  *
@@ -80,7 +80,7 @@ typedef struct dcb_config {
 #define DCB_PRECISION_BF16 0
 #define DCB_PRECISION_FP32 1
 
-/* A named host tensor in the reference checkpoint's layout (SURVEY.md Appendix B), e.g.
+/* A named host tensor in the reference checkpoint's layout, e.g.
  * "model/encoder_stack/layers/0/0/layer/query_dense_layer/kernel" float32 [280,2,140]. */
 typedef struct dcb_tensor {
   const char* name;
@@ -112,7 +112,7 @@ int dcb_load_weights(dcb_engine* e, const dcb_tensor* tensors, int32_t n);
 int dcb_forward(dcb_engine* e, const float* rows, int32_t batch, uint32_t flags,
                 uint8_t* bases_out, uint8_t* quals_out, float* probs_out, float* logits_out);
 
-/* ---- packed input rows (SURVEY.md section 8(f)1: the feature-construction side of the path) --------------------------
+/* ---- packed input rows (the feature-construction side of the path) ----------------------------------------------------
  * The float32 [B, R, L] rows of quick_inference.py:363 hold small integers: bases / ccs in 0..4, pw / ip from uint8
  * BAM tags (pre_lib.py:221-226,704-744), strand in 0..2, ccs_bq in -1..93, plus four float SN values per window that
  * extract_features repeats along L (pre_lib.py:741-742).  The packed form keeps exactly that information in
@@ -164,7 +164,7 @@ int dcb_stitch(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, int32_
                const int32_t* zmw_start, int32_t n_zmw, uint32_t flags,
                uint8_t* seq_out, uint8_t* qual_out, int32_t* len_out);
 
-/* ---- the rest of the post-model stage on the device (SURVEY.md section 8(f)2) ------------------------------------------
+/* ---- the rest of the post-model stage on the device --------------------------------------------------------------------
  * dcb_stitch_fastq = stitch_utils.stitch_to_fastq for a batch of reads (stitch_utils.py:131-189): dcb_stitch, then per
  * read the missing-window check of get_full_sequence (window i must not start beyond i * L, stitch_utils.py:60-78), the
  * only-gaps check, the quality filter round(avg_phred(quals), 5) >= min_quality (utils.py:88-106,
@@ -208,7 +208,7 @@ int dcb_fill_skipped(dcb_engine* e, const uint8_t* ccs_ids, const int16_t* ccs_b
                      int32_t L, int32_t calibration_enabled, double calibration_threshold, double calibration_w,
                      double calibration_b, uint32_t flags, uint8_t* bases, uint8_t* quals);
 
-/* ---- feature construction from BAM (SURVEY.md section 8(f)3; host C++, htslib-free, needs no GPU) -----------------------
+/* ---- feature construction from BAM (host C++, htslib-free, needs no GPU) -----------------------------------------------
  * What `deepconsensus run` does in front of the model: stream the subreads-to-CCS BAM ZMW by ZMW (SubreadGrouper,
  * pre_lib.py:50-91), expand / clip / indent every subread (expand_clip_indent with trim_insertions, :1061-1239), fetch
  * the CCS read (:966-998,1322-1330), space all reads out (space_out_subreads, :1242-1276), cut windows of max_length
@@ -250,15 +250,14 @@ int dcb_last_forward_ms(dcb_engine* e, float* ms);
 /* Number of engine kernels launched by the last dcb_forward. */
 int dcb_last_forward_launches(dcb_engine* e, int32_t* n);
 
-/* Per-kernel timing of the dominant kernel (the fused FFN): when enabled, every ffn_kernel
- * launch is bracketed by CUDA events on the engine's stream; dcb_get_profile returns the
- * accumulated device time, launch count and tokens processed since dcb_set_profile. */
+/* Per-kernel timing of the dominant stage (the FFN GEMMs): when enabled, every launch is bracketed by CUDA events on the
+ * engine's stream; dcb_get_profile returns the FFN stages' accumulated device time, count and tokens processed since
+ * dcb_set_profile. */
 int dcb_set_profile(dcb_engine* e, int32_t enabled);
 int dcb_get_profile(dcb_engine* e, float* ffn_ms_total, int32_t* ffn_launches, int64_t* ffn_tokens);
 /* Device time (ms) and launch count per kernel class since dcb_set_profile: [0] embed, [1] row GEMM
- * (condenser / unfused out-proj), [2] QKV GEMM, [3] attention, [4] FFN (+ fused out-proj), [5] head;
- * *fused_oproj = 1 when the attention out-projection runs inside the FFN kernel. */
-int dcb_get_profile_kernels(dcb_engine* e, float* ms6, int32_t* n6, int32_t* fused_oproj);
+ * (condenser / out-projection), [2] QKV GEMM, [3] attention, [4] FFN, [5] head. */
+int dcb_get_profile_kernels(dcb_engine* e, float* ms6, int32_t* n6);
 
 /* Pinned host memory helpers (for callers that want async H2D/D2H). */
 int dcb_alloc_host(size_t bytes, void** out);

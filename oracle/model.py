@@ -8,7 +8,7 @@ may import this package; the product (`deepconsensus_b200/`) never does.
 PARITY STATUS -- pinned against the reference's own model code, not against TensorFlow's kernels:
 the reference cannot be imported as-is in this image (tensorflow, tf-models-official, ml_collections,
 pysam absent; no network), the bundled checkpoints ship without their data shard and the reference's
-tests hold no numeric golden for the transformer output (SURVEY.md section 8c).  So the pin is:
+tests hold no numeric golden for the transformer output.  So the pin is:
   * tests/golden/ref_model_*.npz -- outputs of the UNMODIFIED reference files networks.py,
     encoder_stack.py, attention_layer.py, ffn_layer.py, data_providers.format_rows, model_configs.get_config
     and model_utils.modify_params, executed from /root/reference on a NumPy stand-in for the TF primitives
@@ -28,7 +28,9 @@ Two arithmetic modes:
   * emulate=None   : float32 everywhere, op order of the reference (the oracle proper).
   * emulate="bf16" : identical graph, but operands of every tensor-core contraction are
                      rounded to bfloat16 at exactly the points the CUDA engine rounds
-                     them (DESIGN.md "precision policy"); accumulation stays fp32.
+                     them; accumulation stays fp32.  The condenser, q/k/v and out-projection
+                     weights are split-bf16 (hi + lo) as in the engine; LayerNorm runs in fp32
+                     and its output is rounded as the next contraction's operand.
                      Used to separate kernel bugs from the documented bf16 rounding.
 """
 from __future__ import annotations
@@ -59,11 +61,15 @@ def _hi_lo(x: torch.Tensor):
   return hi, _bf16(x - hi)
 
 
-def _mm(a: torch.Tensor, b: torch.Tensor, emulate: Optional[str]) -> torch.Tensor:
-  """a @ b with the engine's operand rounding: bf16 (1 product) or bf16x3 split (strict)."""
+def _mm(a: torch.Tensor, b: torch.Tensor, emulate: Optional[str], split_b: bool = False) -> torch.Tensor:
+  """a @ b with the engine's operand rounding: bf16 (1 product; split_b: the weights as a bf16 hi + lo pair, 2 products)
+  or bf16x3 split (strict)."""
   if emulate is None:
     return a @ b
   if emulate == "bf16":
+    if split_b:
+      bh, bl = _hi_lo(b)
+      return _bf16(a) @ bh + _bf16(a) @ bl
     return _bf16(a) @ _bf16(b)
   if emulate == "bf16x3":
     ah, al = _hi_lo(a)
@@ -151,55 +157,8 @@ def band_mask(length: int, attn_win_size: Optional[int]) -> torch.Tensor:
   return (idx[:, None] - idx[None, :]).abs() <= attn_win_size
 
 
-class DeferredLN:
-  """emulate="bf16", pre-LayerNorm models: the engine's deferred normalisation (stack_kernel.cuh, row_pass).
-
-  The tensor-core operand is bf16(x - shift) with shift = the row's mean at the previous sub-layer (+ the mean of a bias
-  that joined since; the exact mean for the first one, and for any row whose mean moved by more than its standard deviation); gamma is folded into the weight rows before rounding; the rank-1 terms -(mean - shift) * colsum and
-  (beta @ W + bias) / rstd ride in the operand's eight padding columns as bf16 hi / lo pairs; the accumulator is
-  multiplied by rstd when it is read.
-  """
-
-  guard = True     # tests switch the re-centring guard off to show what it protects against
-
-  def __init__(self, h2: torch.Tensor, shift: Optional[torch.Tensor], gamma: torch.Tensor, beta: torch.Tensor):
-    mean = h2.mean(-1, keepdim=True)
-    self.shift = mean if shift is None else shift
-
-    def stats():
-      d = h2 - self.shift
-      dmean = d.mean(-1, keepdim=True)
-      return d, dmean, ((d * d).mean(-1, keepdim=True) - dmean * dmean).clamp_min(0.0)
-    self.d, self.dmean, var = stats()
-    far = self.dmean * self.dmean > var          # the row's mean moved by more than its standard deviation: the engine
-    if self.guard and bool(far.any()):           # sweeps again with those rows centred on their exact mean
-      self.shift = torch.where(far, self.shift + self.dmean, self.shift)
-      self.d, self.dmean, var = stats()
-    self.sd = torch.sqrt(var + 1e-6)
-    self.next_shift = self.shift + self.dmean
-    self.gamma, self.beta = gamma, beta
-
-  @staticmethod
-  def _split(x: torch.Tensor):
-    hi = _bf16(x)
-    return hi, _bf16(x - hi)
-
-  def mm(self, wmat: torch.Tensor, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
-    wf = _bf16(self.gamma[:, None] * wmat)
-    bw = self.beta @ wmat
-    if bias is not None:
-      bw = bw + bias
-    ch, cl = self._split(wf.sum(0)[None])
-    bh, bl = self._split(bw[None])
-    dh, dl = self._split(-self.dmean)
-    ih, il = self._split(self.sd)
-    acc = _bf16(self.d) @ wf + (dh + dl) * (ch + cl) + (ih + il) * (bh + bl)
-    return acc / self.sd
-
-
 def attention(y: torch.Tensor, pre: str, params: params_lib.Params, w: weights_lib.Weights,
-              emulate: Optional[str], gain: float, collect: Optional[dict],
-              dln: Optional[DeferredLN] = None) -> torch.Tensor:
+              emulate: Optional[str], gain: float, collect: Optional[dict]) -> torch.Tensor:
   """`Attention.call` (attention_layer.py:169-221) on y [B, L, d]."""
   nh = params.num_heads
   d = params.hidden_size
@@ -211,13 +170,11 @@ def attention(y: torch.Tensor, pre: str, params: params_lib.Params, w: weights_l
   wo = _t(w[pre + "/output_dense_layer/kernel"]).reshape(d, d)
   scale = dh ** -0.5
   y2 = y.reshape(B * L, d)
-  if dln is not None:
-    q, k, v = _bf16(dln.mm(wq * scale)), _bf16(dln.mm(wk)), _bf16(dln.mm(wv))
-  elif emulate:
+  if emulate:
     # engine folds the query scale into Wq and the ReZero gain into Wo before rounding
-    q = _mm(y2, wq * scale, emulate)
-    k = _mm(y2, wk, emulate)
-    v = _mm(y2, wv, emulate)
+    q = _mm(y2, wq * scale, emulate, split_b=True)
+    k = _mm(y2, wk, emulate, split_b=True)
+    v = _mm(y2, wv, emulate, split_b=True)
     if emulate == "bf16":
       q, k, v = _bf16(q), _bf16(k), _bf16(v)   # stored as bf16 between kernels
   else:
@@ -236,17 +193,14 @@ def attention(y: torch.Tensor, pre: str, params: params_lib.Params, w: weights_l
     collect.setdefault("attention_scores", []).append(weights.numpy())
   o = weights @ v                                  # [B, N, F, H]
   o = o.permute(0, 2, 1, 3).reshape(B * L, d)
-  if emulate == "bf16":
-    out = _bf16(o) @ _bf16(wo * gain)
-  elif emulate == "bf16x3":
-    out = _mm(o, wo * gain, emulate)
+  if emulate:
+    out = _mm(o, wo * gain, emulate, split_b=True)
   else:
     out = o @ wo
   return out.reshape(B, L, d)
 
 
-def ffn(y: torch.Tensor, pre: str, w: weights_lib.Weights, emulate: Optional[str],
-        gain: float, dln: Optional[DeferredLN] = None) -> torch.Tensor:
+def ffn(y: torch.Tensor, pre: str, w: weights_lib.Weights, emulate: Optional[str], gain: float) -> torch.Tensor:
   """`FeedForwardNetwork.call`: relu(y W1 + b1) W2 + b2 (ffn_layer.py:83-86)."""
   B, L, d = y.shape
   w1 = _t(w[pre + "/filter_dense_layer/kernel"])
@@ -254,12 +208,7 @@ def ffn(y: torch.Tensor, pre: str, w: weights_lib.Weights, emulate: Optional[str
   w2 = _t(w[pre + "/output_dense_layer/kernel"])
   b2 = _t(w[pre + "/output_dense_layer/bias"])
   y2 = y.reshape(B * L, d)
-  if dln is not None:
-    h = torch.relu(dln.mm(w1, b1))
-    out = _mm(h, w2 * gain, emulate) + b2 * gain
-  elif emulate:
-    if emulate == "bf16":
-      b1 = sum(DeferredLN._split(b1))       # the engine adds b1 inside the GEMM, as a bf16 hi / lo pair
+  if emulate:
     h = torch.relu(_mm(y2, w1, emulate) + b1)
     out = _mm(h, w2 * gain, emulate) + b2 * gain
   else:
@@ -290,14 +239,13 @@ def forward(rows: np.ndarray, params: params_lib.Params, w: weights_lib.Weights,
     e = embed(x, params, w, emulate)                                # [B, L, E]
     if params.condense_transformer_input:
       wc = _t(w["model/transformer_input_condenser/kernel"])
-      h = _mm(e.reshape(B * L, -1), wc, emulate).reshape(B, L, d)
+      h = _mm(e.reshape(B * L, -1), wc, emulate, split_b=True).reshape(B, L, d)
     else:
       h = e
     if params.add_pos_encoding:
       h = h + _t(positional_encoding(L, d))[None]
     if inter is not None:
       inter["embedded"] = h.numpy().copy()
-    shift = None
     for n in range(params.num_hidden_layers):
       pre = "model/encoder_stack/layers/%d" % n
       for sub, fn in ((0, "attn"), (1, "ffn")):
@@ -307,17 +255,11 @@ def forward(rows: np.ndarray, params: params_lib.Params, w: weights_lib.Weights,
         else:
           y = layer_norm(h, _t(w[spre + "/layer_norm/gamma"]), _t(w[spre + "/layer_norm/beta"]))
           alpha = 1.0
-        dln = None
-        if emulate == "bf16" and not params.rezero:
-          dln = DeferredLN(h.reshape(B * L, d), shift, _t(w[spre + "/layer_norm/gamma"]), _t(w[spre + "/layer_norm/beta"]))
-          shift = dln.next_shift
-          if fn == "ffn":      # the FFN's output bias joins the residual at the next row pass: the shift moves by its mean
-            shift = shift + _t(w[spre + "/layer/output_dense_layer/bias"]).mean()
         gain = alpha if emulate else 1.0     # engine folds alpha into Wo / W2 / b2
         if fn == "attn":
-          out = attention(y, spre + "/layer", params, w, emulate, gain, inter, dln)
+          out = attention(y, spre + "/layer", params, w, emulate, gain, inter)
         else:
-          out = ffn(y, spre + "/layer", w, emulate, gain, dln)
+          out = ffn(y, spre + "/layer", w, emulate, gain)
         if emulate:
           h = h + out
         else:

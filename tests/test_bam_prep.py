@@ -1,4 +1,4 @@
-"""Feature construction from BAM (csrc/bam_prep.cpp, deepconsensus_b200/preprocess.py; SURVEY.md section 8(f)3) -- no GPU.
+"""Feature construction from BAM (csrc/bam_prep.cpp, deepconsensus_b200/preprocess.py)3) -- no GPU.
 
 THE pin: tests/golden/human_1m/{subreads_to_ccs,ccs}.bam are byte copies of the reference's BAM fixtures and
 inference_digest.json is a digest of the 1 593 examples the reference's own `deepconsensus preprocess` wrote from them

@@ -10,7 +10,7 @@ reference's own arithmetic; differs from the oracle / the reference-code goldens
   * quality characters within +-1 everywhere (a 1e-5 probability change can cross a rounding boundary of the integer
     Phred score), exact on >= STRICT_QV_EXACT of the positions.
 
-DEFAULT (bf16 tensor-core operands, fp32 accumulation; DESIGN.md section 4): the operand rounding moves logits by
+DEFAULT (bf16 tensor-core operands, fp32 accumulation): the operand rounding moves logits by
 0.02-0.1 on these random-weight models (gates = ~1.2x the largest value measured over all cases):
   * max |logit - oracle_fp32| <= LOGIT_TOL_FP32, RMS <= LOGIT_RMS_FP32, |logit - oracle_bf16| <= LOGIT_TOL_EMU,
   * bases identical on >= BASES_MIN of ALL positions and on every position with fp32 margin > MARGIN,
@@ -127,10 +127,8 @@ def test_layernorm_bq_5_layers_L100(engine_mod):
 
 
 def test_prelayernorm_rows_whose_mean_runs_away(engine_mod):
-  """Deferred LayerNorm of the stack kernel (operands rounded around the row's previous mean): sub-layer outputs with a
-  large common-mode component move the mean by many standard deviations per sub-layer.  The kernel's guard re-centres
-  those rows; without it the logit error is 0.09 on this case (oracle emulation with the guard off,
-  tests/test_oracle_model.py), with it the usual 0.02-0.03."""
+  """Pre-LayerNorm rows whose sub-layer outputs carry a large common-mode component move the mean by many standard
+  deviations per sub-layer; the row epilogue's LayerNorm must still normalise them to the usual parity gates."""
   p = params_lib.synthetic_params(20, 100, use_ccs_bq=True, num_hidden_layers=3, rezero=False)
   w = synthetic.mean_drift_weights(p, weights_lib.init_weights(p, seed=5))
   rows = synthetic.make_rows(p, 6, seed=6)
@@ -305,7 +303,7 @@ def test_run_model_and_stitch_merges_skipped_windows(engine_mod, golden_dir):
 
 @pytest.mark.parametrize("ccs_cal,min_q,min_len", [("skip", 0, 0), ("0,1.1,-0.5", 20, 0), ("30,0.9,2.0", 0, 450)])
 def test_device_post_model_stage_equals_reference_flow(engine_mod, golden_dir, ccs_cal, min_q, min_len):
-  """SURVEY.md 8(f)2 on the device: skip decision (dcb_skip_mask), process_skipped_window (dcb_fill_skipped), sort,
+  """The post-model stage on the device: skip decision (dcb_skip_mask), process_skipped_window (dcb_fill_skipped), sort,
   stitch + filters + FASTQ bytes (dcb_stitch_fastq) == the reference flow on per-window Python objects
   (split_skipped_windows -> run_model_on_examples -> sorted -> stitch_to_fastq), read for read, counter for counter."""
   import itertools
@@ -453,8 +451,8 @@ def test_pipeline_survives_errors_and_mixed_use(engine_mod):
 
 @pytest.mark.parametrize("P,L,bq,layers", [(20, 120, False, 2), (20, 100, True, 2), (32, 200, False, 1), (5, 40, True, 1)])
 def test_packed_rows_give_bit_identical_results(engine_mod, P, L, bq, layers):
-  """dcb_forward_packed (SURVEY.md 8(f)1): packed rows read inside the embedding kernel (L <= 128) or unpacked on the
-  device (L = 200, strict path) -> exactly the outputs of dcb_forward on the float32 rows, ~5.5x fewer H2D bytes."""
+  """dcb_forward_packed: packed rows read directly by the embedding kernel (unpacked on the device for the strict path)
+  -> exactly the outputs of dcb_forward on the float32 rows, ~5.5x fewer H2D bytes."""
   p = params_lib.synthetic_params(P, L, use_ccs_bq=bq, num_hidden_layers=layers)
   w = weights_lib.init_weights(p, seed=80 + L)
   rows = synthetic.make_rows(p, 23, seed=81 + L)
@@ -514,22 +512,19 @@ def test_initialize_model_from_a_tf_checkpoint(engine_mod, tmp_path):
 
 
 def test_unfused_fallback_paths_agree_with_fused(engine_mod):
-  """DCB_STACK / DCB_FUSE_HEAD / DCB_FUSE_OPROJ / DCB_FUSE_EMBED / DCB_FUSE_QA / DCB_ALIGN / DCB_FFN_PAIR select measured
-  alternatives of the same math.  They exist only in the developer build (libdcb200_dev.so, -DDCB_DEV_SWITCHES) and
-  are read when an engine is created; the product library ignores the environment (checked first)."""
+  """DCB_ALIGN / DCB_CHUNK_TILES select alternative token layouts and chunkings of the same math.  They exist only in
+  the developer build (libdcb200_dev.so, -DDCB_DEV_SWITCHES) and are read when an engine is created; the product
+  library ignores the environment (checked first)."""
   p = params_lib.synthetic_params(20, 120, num_hidden_layers=2)
   w = weights_lib.init_weights(p, seed=21)
   rows = synthetic.make_rows(p, 5, seed=22)
   ref = omodel.forward(rows, p, w)["logits"]
   dev = engine_mod.load_dev_library()
+  one_chunk = 3 + 5 * p.num_hidden_layers                          # embed, condenser, 5 per layer, head
   outs = {}
-  for name, env in (("fused", {}),                                     # default: whole stack in one kernel
-                    ("per_layer", {"DCB_STACK": "0"}),                  # QKV+attention and out-proj+FFN kernels per layer
-                    ("separate_head", {"DCB_FUSE_HEAD": "0"}),          # head_kernel after the stack instead of its fused tail
-                    ("unfused", {"DCB_FUSE_OPROJ": "0", "DCB_FUSE_EMBED": "0", "DCB_FUSE_QA": "0"}),
-                    ("packed", {"DCB_ALIGN": "0"}),                     # windows packed back to back, separate QKV / attention
-                    ("single_cta", {"DCB_FFN_PAIR": "0", "DCB_FUSE_QA": "0"}),
-                    ("qkv2", {"DCB_FUSE_QA": "0", "DCB_QKV2": "1"})):
+  for name, env in (("default", {}),                                   # one window per 128-token tile, one chunk
+                    ("packed", {"DCB_ALIGN": "0"}),                     # windows packed back to back across tiles
+                    ("chunked", {"DCB_CHUNK_TILES": "1"})):             # one tile (one window) per chunk
     old = {k: os.environ.get(k) for k in env}
     os.environ.update(env)
     try:
@@ -537,10 +532,11 @@ def test_unfused_fallback_paths_agree_with_fused(engine_mod):
       outs[name] = model.forward(rows, want_logits=True)["logits"]
       launches = model.last_launches
       model.close()
-      if name == "per_layer":
+      if name == "chunked":
+        assert launches == rows.shape[0] * one_chunk
         prod = engine_mod.B200Model(p, w, max_batch=8)              # product library: the switch is ignored
         prod.forward(rows)
-        assert prod.last_launches == 2 and launches > 2
+        assert prod.last_launches == one_chunk
         prod.close()
     finally:
       for k, v in old.items():
@@ -549,11 +545,8 @@ def test_unfused_fallback_paths_agree_with_fused(engine_mod):
         else:
           os.environ[k] = v
     assert np.abs(outs[name] - ref).max() <= LOGIT_TOL_FP32, name
-  assert np.abs(outs["fused"] - outs["per_layer"]).max() < 0.05
-  assert np.abs(outs["fused"] - outs["separate_head"]).max() < 1e-3
-  assert np.abs(outs["fused"] - outs["unfused"]).max() < 0.05
-  assert np.abs(outs["fused"] - outs["packed"]).max() < 0.05
-  assert np.abs(outs["qkv2"] - outs["unfused"]).max() < 0.05
+  assert np.array_equal(outs["default"], outs["chunked"])
+  assert np.abs(outs["default"] - outs["packed"]).max() < 0.05
 
 
 @pytest.mark.parametrize("name", ["rezero_p20", "layernorm_p20", "rezero_p20_bq", "layernorm_p20_bq", "rezero_p5_win3",
@@ -729,8 +722,8 @@ def test_full_size_properties_c2_batch_1024(engine_mod):
 @pytest.mark.parametrize("layers,ff,rezero,win,L,B", [
     (1, 128, True, 12, 120, 3),      # one layer, one hidden chunk: the FFN stage program never reaches the tail slots
     (3, 640, False, 16, 128, 4),     # pre-LN, band at the two-pass limit, window exactly one tile
-    (8, 256, True, 1, 64, 5),        # deepest stack the one-kernel path takes, narrowest band, short windows
-    (9, 256, True, 12, 100, 2),      # deeper than kMaxLayers: falls back to the per-layer kernels
+    (8, 256, True, 1, 64, 5),        # deep stack, narrowest band, short windows
+    (9, 256, True, 12, 100, 2),      # deeper still
 ])
 def test_stack_kernel_corner_shapes(engine_mod, layers, ff, rezero, win, L, B):
   p = params_lib.synthetic_params(20, L, num_hidden_layers=layers, rezero=rezero, attn_win_size=win)
@@ -741,11 +734,10 @@ def test_stack_kernel_corner_shapes(engine_mod, layers, ff, rezero, win, L, B):
   out = model.forward(rows, want_logits=True)
   launches = model.last_launches
   model.close()
-  assert launches == (2 if layers <= 8 else 2 + 2 * layers)
+  assert launches == 3 + 5 * layers                 # embed, condenser, 5 per layer, head
   ref = omodel.forward(rows, p, w)
   assert np.isfinite(out["logits"]).all()
-  # these are structural tests of the kernel's stage programs; the bf16 rounding error grows with depth (measured
-  # 0.22 at 8 layers with the narrowest band), so the 8- and 9-layer cases get a proportionally wider gate
+  # the bf16 rounding error grows with depth, so the 8- and 9-layer cases get a proportionally wider gate
   assert np.abs(out["logits"] - ref["logits"]).max() <= (LOGIT_TOL_FP32 if layers <= 6 else 0.30)
 
 
@@ -757,15 +749,15 @@ def test_stack_kernel_corner_shapes(engine_mod, layers, ff, rezero, win, L, B):
     (136, 8, False, 1, 1),       # single window
 ])
 def test_wide_windows_on_the_one_kernel_stack(engine_mod, L, win, rezero, layers, B):
-  """128 < L <= 256: one window per CTA pair (Lw = 256), the attention band crosses the pair through remote
-  shared-memory fragment loads.  Same two launches as the L <= 128 path; parity gates as everywhere else."""
+  """128 < L <= 256: windows are packed back to back, so a window and its attention band cross 128-token tiles.  Same
+  launch sequence as the L <= 128 path; parity gates as everywhere else."""
   p = params_lib.synthetic_params(20, L, num_hidden_layers=layers, rezero=rezero, attn_win_size=win)
   w = weights_lib.init_weights(p, seed=400 + L)
   rows = synthetic.make_rows(p, B, seed=401 + L)
   cal = calibration.parse_calibration_string(CAL)
   model = engine_mod.B200Model(p, w, max_batch=B, calibration=cal)
   out = model.forward(rows, want_probs=True, want_logits=True)
-  assert model.last_launches == 2
+  assert model.last_launches == 3 + 5 * layers
   again = model.forward(rows, want_logits=True)
   assert np.array_equal(out["logits"], again["logits"])
   one = model.forward(rows[B - 1:], want_logits=True)
@@ -777,7 +769,7 @@ def test_wide_windows_on_the_one_kernel_stack(engine_mod, L, win, rezero, layers
   _assert_strict(strict, refd)
   _assert_default(out, refd)
   _epilogue_exact(out, cal)
-  # the positions next to the cut (112..143) are the ones that use the partner's rows: check them on their own
+  # the positions next to the first tile boundary (112..143) attend across it: check them on their own
   cut = slice(112, min(L, 144))
   assert np.abs(out["logits"][:, cut] - ref["logits"][:, cut]).max() <= LOGIT_TOL_FP32
 

@@ -129,7 +129,7 @@ def test_get_indices():
 
 
 def test_params_json_fixture_roundtrip(tmp_path):
-  # the keys the reference fixture testdata/model/params.json carries for the path (SURVEY.md Appendix C)
+  # the keys the reference fixture testdata/model/params.json carries for the path
   fixture = dict(model_name="transformer_learn_values", max_passes=20, max_length=100, use_ccs_bq=False,
                  per_base_hidden_size=8, pw_hidden_size=8, ip_hidden_size=8, strand_hidden_size=2, sn_hidden_size=8,
                  ccs_bq_hidden_size=8, condense_transformer_input=True, transformer_input_size=280, hidden_size=280,
@@ -141,7 +141,7 @@ def test_params_json_fixture_roundtrip(tmp_path):
   params_lib.modify_params(p)
   assert p.hidden_size == 280 and p.num_heads == 2 and p.filter_size == 2048
   assert params_lib.embedded_width(p) == 560
-  assert weights.count_params(p) == 8943775                             # SURVEY.md Appendix B/E
+  assert weights.count_params(p) == 8943775                           
 
 
 def test_config_derived_hidden_sizes():

@@ -1,4 +1,4 @@
-"""Packed input rows (include/dcb200.h "packed input rows"; SURVEY.md section 8(f)1) -- host side, no GPU.
+"""Packed input rows (include/dcb200.h "packed input rows")1) -- host side, no GPU.
 
 dcb_pack_rows must keep exactly the information the model path reads: unpacking gives back the rows
 `format_rows` + `tf.cast(int32)` would produce (data_providers.py:151-162, networks.py:457-507), except SN which
