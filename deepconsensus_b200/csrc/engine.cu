@@ -99,7 +99,9 @@ struct dcb_engine {
   // post-model stage scratch (dcb_stitch_fastq / dcb_skip_mask / dcb_fill_skipped), grown on demand
   double* d_p10 = nullptr;           // 10^(-q/10), q = 0..255 (host libm pow, as NumPy)
   struct Scratch { void* p = nullptr; size_t cap = 0; } sc_pos, sc_names, sc_nameoff, sc_outcome, sc_avg, sc_recoff, sc_fastq,
-      sc_bq, sc_mask, sc_ids, sc_dst, sc_tmpb, sc_tmpq;
+      sc_bq, sc_mask, sc_ids, sc_dst, sc_tmpb, sc_tmpq,
+      sc_ev_probs, sc_ev_in, sc_ev_out;   // dcb_evaluate: host probs, labels | ccs ids, loss | counts | flags
+  cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;
   float* d_dbg = nullptr;  // [stages][chunk_tiles * x_image]
   // strict-fp32 path (strict_kernels.cu): float32 copies of every variable in the reference's own shapes, and a
   // row-major workspace allocated on the first strict call
@@ -320,8 +322,11 @@ void dcb_destroy(dcb_engine* e) {
   if (e->d_st_start) cudaFree(e->d_st_start);
   if (e->d_st_len) cudaFree(e->d_st_len);
   for (dcb_engine::Scratch* sc : {&e->sc_pos, &e->sc_names, &e->sc_nameoff, &e->sc_outcome, &e->sc_avg, &e->sc_recoff,
-                                  &e->sc_fastq, &e->sc_bq, &e->sc_mask, &e->sc_ids, &e->sc_dst, &e->sc_tmpb, &e->sc_tmpq})
+                                  &e->sc_fastq, &e->sc_bq, &e->sc_mask, &e->sc_ids, &e->sc_dst, &e->sc_tmpb, &e->sc_tmpq,
+                                  &e->sc_ev_probs, &e->sc_ev_in, &e->sc_ev_out})
     if (sc->p) cudaFree(sc->p);
+  if (e->ev_eval0) cudaEventDestroy(e->ev_eval0);
+  if (e->ev_eval1) cudaEventDestroy(e->ev_eval1);
   for (auto& sl : e->slots)
     for (auto& pr : sl.prof_events) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
   if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
@@ -1238,6 +1243,59 @@ int dcb_fill_skipped(dcb_engine* e, const uint8_t* ccs_ids, const int16_t* ccs_b
   }
   CU(e, cudaGetLastError());
   if (status & 1) return fail(e, DCB_ERR_INPUT_RANGE, "dcb_fill_skipped: CCS base id outside 0..4 (clamped)");
+  return DCB_OK;
+}
+
+int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const uint8_t* ccs_ids, int32_t batch,
+                 int32_t L, double del_cost, double loss_reg, int32_t band_width, uint32_t flags, float* loss_out,
+                 uint8_t* exact_out, int32_t* pred_counts, int32_t* ccs_counts, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  if (band_width >= 0)
+    return fail(e, DCB_ERR_INVALID, "dcb_evaluate: the banded alignment loss (band_width=%d) is not supported; "
+                "pass DCB_BAND_WIDTH_NONE (params.band_width None, as the released models are trained)", band_width);
+  if (batch < 0 || L <= 0 || L > 256) return fail(e, DCB_ERR_INVALID, "dcb_evaluate: need batch >= 0 and 0 < L <= 256");
+  if (!(del_cost == del_cost)) return fail(e, DCB_ERR_INVALID, "dcb_evaluate: del_cost is NaN");
+  if (ms_out) *ms_out = 0.f;
+  if (batch == 0) return DCB_OK;
+  if (!probs || !labels || !ccs_ids || !loss_out || !exact_out || !pred_counts || !ccs_counts)
+    return fail(e, DCB_ERR_INVALID, "dcb_evaluate: null pointer");
+  const size_t ntok = (size_t)batch * L;
+  for (size_t i = 0; i < ntok; ++i)
+    if (labels[i] > 4) return fail(e, DCB_ERR_INVALID, "dcb_evaluate: label id %d outside 0..4 at window %zu", labels[i], i / L);
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  const bool probs_dev = flags & DCB_ROWS_ON_DEVICE;
+  const size_t out_bytes = (size_t)batch * (sizeof(float) + 10 * sizeof(int32_t) + 1);
+  int rc;
+  if ((rc = ensure(e, e->sc_ev_in, 2 * ntok)) || (rc = ensure(e, e->sc_ev_out, out_bytes)) ||
+      (!probs_dev && (rc = ensure(e, e->sc_ev_probs, ntok * kVocab * sizeof(float)))))
+    return rc;
+  if (!e->ev_eval0) CU(e, cudaEventCreate(&e->ev_eval0));
+  if (!e->ev_eval1) CU(e, cudaEventCreate(&e->ev_eval1));
+  uint8_t* d_in = static_cast<uint8_t*>(e->sc_ev_in.p);
+  const float* d_probs = probs;
+  if (!probs_dev) {
+    CU(e, cudaMemcpyAsync(e->sc_ev_probs.p, probs, ntok * kVocab * sizeof(float), cudaMemcpyHostToDevice, st));
+    d_probs = static_cast<const float*>(e->sc_ev_probs.p);
+  }
+  CU(e, cudaMemcpyAsync(d_in, labels, ntok, cudaMemcpyHostToDevice, st));
+  CU(e, cudaMemcpyAsync(d_in + ntok, ccs_ids, ntok, cudaMemcpyHostToDevice, st));
+  float* d_loss = static_cast<float*>(e->sc_ev_out.p);
+  int32_t* d_pred = reinterpret_cast<int32_t*>(d_loss + batch);
+  int32_t* d_ccs = d_pred + (size_t)batch * 5;
+  uint8_t* d_exact = reinterpret_cast<uint8_t*>(d_ccs + (size_t)batch * 5);
+  const bool hard = !(loss_reg > 0.0);
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  CU(e, launch_evaluate(d_probs, d_in, d_in + ntok, batch, L, (float)del_cost, hard ? 1.f : (float)loss_reg, hard ? 1 : 0,
+                        d_loss, d_exact, d_pred, d_ccs, st));
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  CU(e, cudaMemcpyAsync(loss_out, d_loss, (size_t)batch * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CU(e, cudaMemcpyAsync(pred_counts, d_pred, (size_t)batch * 5 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CU(e, cudaMemcpyAsync(ccs_counts, d_ccs, (size_t)batch * 5 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CU(e, cudaMemcpyAsync(exact_out, d_exact, (size_t)batch, cudaMemcpyDeviceToHost, st));
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
   return DCB_OK;
 }
 

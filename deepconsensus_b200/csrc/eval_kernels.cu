@@ -1,0 +1,256 @@
+// Evaluation of a batch of labelled windows on the device: what `model.evaluate` computes per window in the reference's
+// model_inference.py, plus the identity the training loop reports (models/losses_and_metrics.py).
+//
+//   align_loss_kernel       AlignmentLoss.eval with width=None (losses_and_metrics.py:306-411,549-595), one CTA per
+//                           window: the label is left-shifted (:92-115), y_pred renormalised to sum to 1, the
+//                           xentropy substitution / insertion costs (clip at 1e-7) are formed on the fly from a
+//                           per-position table of -log(p) in shared memory, and the (L+1)^2 dynamic program sweeps
+//                           anti-diagonals through three rotating shared-memory rows.  Soft-min
+//                           -reg * logsumexp(-t / reg) with the max subtracted (tf.reduce_logsumexp), or the hard min.
+//                           float32 throughout, as the reference.
+//   align_identity_kernel   AlignmentMetric.alignment (:704-1043), one CTA per (window, sequence): blockIdx.y = 0 aligns
+//                           the argmax-decoded prediction, 1 the window's CCS row (get_batch_identity_ccs_pred,
+//                           :1061-1098).  Affine-gap Needleman-Wunsch (match +2, mismatch -5, gap open 9, extend 4) with
+//                           the reference's first-max tie-breaking in the order [match, ins, del]; the three argmax
+//                           directions of every cell are kept as one byte in shared memory ((L+1)^2 bytes, 66 KB at
+//                           L = 256) and one thread walks the traceback, counting the trans_enc edges 1-5.  The y = 0
+//                           CTA also writes PerExampleAccuracy's exact-match flag (:43-65).
+// Results are deterministic: every reduction is a fixed-order loop, no atomics.
+#include <cuda_runtime.h>
+#include <math.h>
+#include <stdint.h>
+
+#include "kernels.h"
+
+namespace dcb {
+
+namespace {
+
+constexpr int kEvalThreads = 256;
+constexpr int kEvalMaxL = 256;
+constexpr float kInf = 1e9f;
+constexpr float kEps = 1e-7f;
+constexpr float kOneMinusEps = (float)(1.0 - 1e-7);   // Python's 1 - eps, then float32, as tf.clip_by_value sees it
+
+// Left shift (left_shift_sequence): non-gap ids in order, then gaps.  One thread; L <= 256.  Returns the non-gap count.
+__device__ int left_shift_serial(const uint8_t* in, uint8_t* out, int L) {
+  int n = 0;
+  for (int i = 0; i < L; ++i)
+    if (in[i] != 0) out[n++] = in[i];
+  for (int i = n; i < L; ++i) out[i] = 0;
+  return n;
+}
+
+__device__ __forceinline__ int argmax5(const float* p) {
+  int best = 0;
+  for (int t = 1; t < kVocab; ++t)
+    if (p[t] > p[best]) best = t;
+  return best;
+}
+
+__device__ __forceinline__ float softmin3(float a, float b, float c, float reg, bool hard) {
+  if (hard) return fminf(fminf(a, b), c);
+  const float x0 = -a / reg, x1 = -b / reg, x2 = -c / reg;
+  float mx = fmaxf(fmaxf(x0, x1), x2);
+  if (!isfinite(mx)) mx = 0.f;
+  float s = expf(__fsub_rn(x0, mx));
+  s = __fadd_rn(s, expf(__fsub_rn(x1, mx)));
+  s = __fadd_rn(s, expf(__fsub_rn(x2, mx)));
+  return __fmul_rn(-reg, __fadd_rn(logf(s), mx));
+}
+
+}  // namespace
+
+__global__ void __launch_bounds__(kEvalThreads)
+align_loss_kernel(const float* __restrict__ probs, const uint8_t* __restrict__ labels, int L, float del_cost, float reg,
+                  int hard, float* __restrict__ loss_out) {
+  __shared__ float s_lp[kEvalMaxL * kVocab];     // -log(clip(p / sum p)) per position and token
+  __shared__ float s_v[3][kEvalMaxL + 1];        // anti-diagonals k-2, k-1, k (rotating)
+  __shared__ uint8_t s_lab_in[kEvalMaxL], s_lab[kEvalMaxL];
+  __shared__ int s_len;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int m = L, n = L;
+  const float* p = probs + (size_t)b * L * kVocab;
+  for (int j = tid; j < L; j += blockDim.x) {
+    float q[kVocab];
+    for (int t = 0; t < kVocab; ++t) q[t] = p[j * kVocab + t];
+    float tot = q[0];
+    for (int t = 1; t < kVocab; ++t) tot = __fadd_rn(tot, q[t]);
+    for (int t = 0; t < kVocab; ++t) s_lp[j * kVocab + t] = -logf(fminf(fmaxf(q[t] / tot, kEps), kOneMinusEps));
+    s_lab_in[j] = labels[(size_t)b * L + j];
+  }
+  __syncthreads();
+  if (tid == 0) s_len = left_shift_serial(s_lab_in, s_lab, L);
+  for (int i = tid; i <= m; i += blockDim.x) {   // anti-diagonals 0 and 1
+    s_v[0][i] = i == 0 ? 0.f : kInf;
+    s_v[1][i] = i == 0 ? s_lp[0 * kVocab + 0] : (i == 1 ? del_cost : kInf);
+  }
+  __syncthreads();
+  const int seq_len = s_len, k_end = seq_len + n;
+  const bool hard_min = hard != 0;
+  for (int k = 2; k <= k_end; ++k) {
+    const float* v2 = s_v[(k - 2) % 3];
+    const float* v1 = s_v[(k - 1) % 3];
+    float* v0 = s_v[k % 3];
+    for (int i = tid; i <= m; i += blockDim.x) {
+      const int j = k - i;
+      float v;
+      if (j < 0 || j > n) {
+        v = kInf;
+      } else if (i == 0) {
+        v = __fadd_rn(v1[0], k - 1 < n ? s_lp[(k - 1) * kVocab + 0] : 0.f);   // insertion along the first row
+      } else {
+        const bool jin = j - 1 >= 0 && j - 1 < n;                           // cost tables are 0 outside (wavefrontify)
+        const float om = __fadd_rn(v2[i - 1], jin ? s_lp[(j - 1) * kVocab + s_lab[i - 1]] : 0.f);
+        const float oi = __fadd_rn(v1[i], jin ? s_lp[(j - 1) * kVocab + 0] : 0.f);
+        const float od = __fadd_rn(v1[i - 1], del_cost);
+        v = softmin3(om, oi, od, reg, hard_min);
+      }
+      v0[i] = v;
+    }
+    __syncthreads();
+  }
+  if (tid == 0) loss_out[b] = k_end >= 2 ? s_v[k_end % 3][seq_len] : kInf;
+}
+
+// Directions byte of a cell: bits 0-1 match-state argmax (0..2), bit 2 insert-state argmax (0..1), bits 3-4 delete-state
+// argmax (0..2).
+__global__ void __launch_bounds__(kEvalThreads)
+align_identity_kernel(const float* __restrict__ probs, const uint8_t* __restrict__ labels,
+                      const uint8_t* __restrict__ ccs_ids, int L, int32_t* __restrict__ pred_counts,
+                      int32_t* __restrict__ ccs_counts, uint8_t* __restrict__ exact_out) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  const int b = blockIdx.x, which = blockIdx.y, tid = threadIdx.x;
+  const int m = L, n = L, W = L + 1;
+  float* s_v = reinterpret_cast<float*>(smem);                       // [3 rotating][3 states][L + 1]
+  uint8_t* s_y_in = smem + 9 * W * sizeof(float);
+  uint8_t* s_x_in = s_y_in + L;
+  uint8_t* s_y = s_x_in + L;
+  uint8_t* s_x = s_y + L;
+  uint8_t* s_dir = s_x + L;                                          // [L + 1][L + 1]
+  __shared__ int s_tl, s_pl;
+  for (int j = tid; j < L; j += blockDim.x) {
+    s_y_in[j] = labels[(size_t)b * L + j];
+    if (which == 0) {
+      s_x_in[j] = (uint8_t)argmax5(probs + ((size_t)b * L + j) * kVocab);
+    } else {
+      const uint8_t c = ccs_ids[(size_t)b * L + j];
+      s_x_in[j] = c < kVocab ? c : 0;          // one_hot of an id outside the vocabulary is all zeros: argmax 0
+    }
+  }
+  __syncthreads();
+  if (tid == 0) s_tl = left_shift_serial(s_y_in, s_y, L);
+  if (tid == 32) s_pl = left_shift_serial(s_x_in, s_x, L);
+  __syncthreads();
+  if (which == 0) {   // PerExampleAccuracy: all L left-shifted positions equal
+    int eq = 1;
+    for (int j = tid; j < L; j += blockDim.x) eq &= s_y[j] == s_x[j];
+    eq = __syncthreads_and(eq);
+    if (tid == 0) exact_out[b] = (uint8_t)eq;
+  }
+  const int tl = s_tl, pl = s_pl, k_end = tl + pl;
+  const float NEG = -kInf, GO = 9.f, GE = 4.f;
+  auto V = [&](int k, int s, int i) -> float& { return s_v[((k % 3) * 3 + s) * W + i]; };
+  for (int i = tid; i <= m; i += blockDim.x) {   // anti-diagonals 0 and 1
+    V(0, 0, i) = i == 0 ? 0.f : NEG;
+    V(0, 1, i) = NEG;
+    V(0, 2, i) = NEG;
+    V(1, 0, i) = NEG;
+    V(1, 1, i) = i == 0 ? -GO : NEG;
+    V(1, 2, i) = i == 1 ? -GO : NEG;
+  }
+  if (tid == 0) {
+    if (n >= 1) s_dir[0 * W + 1] = 0;          // (0,1): insert opened from the match state
+    if (m >= 1) s_dir[1 * W + 0] = 0;          // (1,0): delete opened from the match state
+  }
+  __syncthreads();
+  for (int k = 2; k <= k_end; ++k) {
+    for (int i = tid; i <= m; i += blockDim.x) {
+      const int j = k - i;
+      float vm = NEG, vi, vd = NEG;
+      int dm = 0, di, dd = 0;
+      // insert state: from (i, j-1) in states [match, ins]
+      {
+        const float a = V(k - 1, 0, i) - GO, c = V(k - 1, 1, i) - GE;
+        vi = a; di = 0;
+        if (c > vi) { vi = c; di = 1; }
+      }
+      if (i >= 1) {
+        const float sub = (j - 1 >= 0 && j - 1 < n) ? (s_y[i - 1] == s_x[j - 1] ? 2.f : -5.f) : 0.f;
+        vm = V(k - 2, 0, i - 1) + sub;
+        for (int s = 1; s < 3; ++s) {
+          const float t = V(k - 2, s, i - 1) + sub;
+          if (t > vm) { vm = t; dm = s; }
+        }
+        vd = V(k - 1, 0, i - 1) - GO;
+        float t = V(k - 1, 1, i - 1) - GO;
+        if (t > vd) { vd = t; dd = 1; }
+        t = V(k - 1, 2, i - 1) - GE;
+        if (t > vd) { vd = t; dd = 2; }
+      }
+      const bool valid = j >= 0 && j <= n;
+      V(k, 0, i) = valid ? vm : NEG;
+      V(k, 1, i) = valid ? vi : NEG;
+      V(k, 2, i) = valid ? vd : NEG;
+      if (valid) s_dir[i * W + j] = (uint8_t)(dm | (di << 2) | (dd << 3));
+    }
+    __syncthreads();
+  }
+  if (tid != 0) return;
+  // optimal final state at (tl, pl): first maximum over [match, ins, del]
+  int s = -1;
+  if (k_end >= 1) {
+    s = 0;
+    float best = V(k_end, 0, tl);
+    for (int t = 1; t < 3; ++t)
+      if (V(k_end, t, tl) > best) { best = V(k_end, t, tl); s = t; }
+  }
+  const int steps_k[3] = {-2, -1, -1}, steps_i[3] = {-1, 0, -1};
+  const int trans_enc[3][3] = {{1, 1, 1}, {2, 3, 2}, {4, 4, 5}};
+  int k_opt = k_end, i_opt = tl;
+  int nm = 0, ni = 0, nd = 0, nc = 0;
+  for (int it = 0; it <= m + n && s != -1; ++it) {
+    const int ss = s > 0 ? s : 0, si = i_opt > 0 ? i_opt : 0;
+    const int j_opt = k_opt - si;
+    int s_n;
+    if (si == 0 && j_opt == 0) {
+      s_n = ss == 0 ? -1 : -2;                 // the start cell: match state ends the walk
+    } else {
+      const uint8_t d = s_dir[si * W + j_opt];
+      s_n = ss == 0 ? (d & 3) : (ss == 1 ? ((d >> 2) & 1) : ((d >> 3) & 3));
+    }
+    if (s_n == -1) break;
+    const int edge = trans_enc[ss][s_n > 0 ? s_n : 0];
+    if (edge == 1) {
+      ++nm;
+      if (i_opt >= 1 && j_opt >= 1 && s_y[i_opt - 1] == s_x[j_opt - 1]) ++nc;
+    } else if (edge <= 3) {
+      ++ni;
+    } else {
+      ++nd;
+    }
+    k_opt += steps_k[ss];
+    i_opt += steps_i[ss];
+    s = s_n;
+  }
+  int32_t* out = (which == 0 ? pred_counts : ccs_counts) + (size_t)b * 5;
+  out[0] = nm; out[1] = ni; out[2] = nd; out[3] = nc; out[4] = nm + ni + nd;
+}
+
+size_t eval_identity_smem_bytes(int L) {
+  return (size_t)9 * (L + 1) * sizeof(float) + 4 * (size_t)L + (size_t)(L + 1) * (L + 1);
+}
+
+cudaError_t launch_evaluate(const float* probs, const uint8_t* labels, const uint8_t* ccs_ids, int B, int L,
+                            float del_cost, float loss_reg, int hard_min, float* loss, uint8_t* exact,
+                            int32_t* pred_counts, int32_t* ccs_counts, cudaStream_t st) {
+  if (B <= 0) return cudaSuccess;
+  align_loss_kernel<<<B, kEvalThreads, 0, st>>>(probs, labels, L, del_cost, loss_reg, hard_min, loss);
+  const size_t smem = eval_identity_smem_bytes(L);
+  cudaError_t err = cudaFuncSetAttribute(align_identity_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (err != cudaSuccess) return err;
+  align_identity_kernel<<<dim3(B, 2), kEvalThreads, smem, st>>>(probs, labels, ccs_ids, L, pred_counts, ccs_counts, exact);
+  return cudaGetLastError();
+}
+
+}  // namespace dcb

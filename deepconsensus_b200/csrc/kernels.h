@@ -47,6 +47,12 @@ void launch_fill_skipped(const uint8_t* ccs_ids, const int16_t* ccs_bq, const in
                          double thr, double cw, double cb, int max_q, uint8_t* bases, uint8_t* quals, int* status,
                          cudaStream_t st);
 
+// ---- evaluation on labelled windows (eval_kernels.cu): alignment loss, exact-match flag, alignment counts [B][5] of
+// the prediction and of the CCS row.  hard_min != 0: loss_reg None.  All pointers are device pointers.
+cudaError_t launch_evaluate(const float* probs, const uint8_t* labels, const uint8_t* ccs_ids, int B, int L,
+                            float del_cost, float loss_reg, int hard_min, float* loss, uint8_t* exact,
+                            int32_t* pred_counts, int32_t* ccs_counts, cudaStream_t st);
+
 // ---- strict-fp32 path (strict_kernels.cu): row-major float32 activations, windows packed back to back
 void launch_strict_embed(const float* rows, int R, int L, int E, int nwindows, const StrictEmbedRow* meta,
                          const float* tables, float* emb, int* status, cudaStream_t st);

@@ -37,6 +37,9 @@ DCB_PRECISION_FP32 = 1
 # per-read outcome codes of dcb_stitch_fastq (the OutcomeCounter field the reference would bump)
 DCB_READ_OK, DCB_READ_EMPTY, DCB_READ_ONLY_GAPS, DCB_READ_LOW_QUALITY, DCB_READ_TOO_SHORT = 0, 1, 2, 3, 4
 DCB_READ_BORDERLINE = 0x80
+DCB_BAND_WIDTH_NONE = -1
+# columns of dcb_evaluate's per-window alignment counts (AlignmentMetric.alignment's metric_values)
+EVAL_COUNT_KEYS = ("num_matches", "num_insertions", "num_deletions", "num_correct_matches", "alignment_length")
 
 
 class DcbError(RuntimeError):
@@ -77,7 +80,7 @@ class DcbTensor(ctypes.Structure):
 ABI_SYMBOLS = (
     "dcb_create", "dcb_load_weights", "dcb_forward", "dcb_submit", "dcb_wait", "dcb_stitch", "dcb_last_forward_ms",
     "dcb_packed_window_bytes", "dcb_pack_rows", "dcb_forward_packed", "dcb_submit_packed",
-    "dcb_stitch_fastq", "dcb_skip_mask", "dcb_fill_skipped",
+    "dcb_stitch_fastq", "dcb_skip_mask", "dcb_fill_skipped", "dcb_evaluate",
     "dcb_prep_open", "dcb_prep_set_threads", "dcb_prep_next_zmw", "dcb_prep_get_windows", "dcb_prep_ccs_header", "dcb_prep_close",
     "dcb_prep_last_error", "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
     "dcb_last_forward_launches", "dcb_set_profile", "dcb_get_profile", "dcb_get_profile_kernels", "dcb_alloc_host",
@@ -134,6 +137,8 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_stitch_fastq.argtypes = [vp, vp, vp, i32, i32, vp, i32, vp, vp, vp, f64, i32, u32, vp, ctypes.c_int64, vp, vp, vp]
   lib.dcb_skip_mask.argtypes = [vp, vp, i32, i32, f64, vp, vp]
   lib.dcb_fill_skipped.argtypes = [vp, vp, vp, vp, i32, i32, i32, f64, f64, f64, u32, vp, vp]
+  lib.dcb_evaluate.argtypes = [vp, vp, vp, vp, i32, i32, f64, f64, i32, u32, vp, vp, vp, vp,
+                               ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_launches.argtypes = [vp, ctypes.POINTER(i32)]
   lib.dcb_set_debug.argtypes = [vp, i32]
@@ -569,6 +574,100 @@ class B200Model:
                                      zs.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), int(zs.shape[0]) - 1, flags,
                                      ctypes.c_void_p(seq_ptr), ctypes.c_void_p(qual_ptr), ctypes.c_void_p(len_ptr)))
 
+  # -- evaluation of labelled windows (include/dcb200.h "evaluation of labelled windows") -------------------------
+  def _eval_args(self, del_cost, loss_reg, band_width):
+    p = self.params
+    del_cost = float(p.get("del_cost", 10.0) if del_cost is None else del_cost)
+    loss_reg = p.get("loss_reg", 0.1) if loss_reg == "params" else loss_reg
+    band_width = p.get("band_width") if band_width == "params" else band_width
+    return (del_cost, 0.0 if loss_reg is None else float(loss_reg),
+            DCB_BAND_WIDTH_NONE if band_width is None else int(band_width))
+
+  def evaluate_windows(self, probs, labels: np.ndarray, ccs_ids: np.ndarray, del_cost: Optional[float] = None,
+                       loss_reg: Any = "params", band_width: Any = "params", on_device: bool = False,
+                       batch: Optional[int] = None) -> Dict[str, Any]:
+    """dcb_evaluate: per-window AlignmentLoss, PerExampleAccuracy flag and AlignmentMetric counts of the prediction and
+    of the CCS row.  probs float32 [B, L, 5] (host array, or a device address with on_device=True and `batch`);
+    labels / ccs_ids uint8 [B, L].  del_cost / loss_reg / band_width default to params.json's (loss_reg=None: hard
+    min; band_width set: DcbError -1).  Returns loss float32 [B], exact uint8 [B], pred_counts / ccs_counts int32
+    [B, 5] (columns EVAL_COUNT_KEYS) and ms, the device time of the evaluation kernels."""
+    labels = np.ascontiguousarray(labels, dtype=np.uint8)
+    ccs = np.ascontiguousarray(ccs_ids, dtype=np.uint8)
+    if labels.ndim != 2 or ccs.shape != labels.shape:
+      raise ValueError("labels and ccs_ids must both be uint8 [B, L]")
+    B, L = labels.shape
+    if on_device:
+      if batch is None or int(batch) != B:
+        raise ValueError("evaluate_windows(on_device=True) needs batch == labels.shape[0]")
+      p_ptr, flags = ctypes.c_void_p(int(probs)), DCB_ROWS_ON_DEVICE
+    else:
+      probs = np.ascontiguousarray(probs, dtype=np.float32)
+      if probs.shape != (B, L, 5):
+        raise ValueError("probs must be float32 [%d, %d, 5], got %s" % (B, L, probs.shape))
+      p_ptr, flags = probs.ctypes.data_as(ctypes.c_void_p), 0
+    dc, reg, bw = self._eval_args(del_cost, loss_reg, band_width)
+    out = dict(loss=np.zeros(B, np.float32), exact=np.zeros(B, np.uint8), pred_counts=np.zeros((B, 5), np.int32),
+               ccs_counts=np.zeros((B, 5), np.int32))
+    ms = ctypes.c_float()
+    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    self._check(self._lib.dcb_evaluate(self._handle, p_ptr, vp(labels), vp(ccs), B, L, dc, reg, bw, flags,
+                                       vp(out["loss"]), vp(out["exact"]), vp(out["pred_counts"]),
+                                       vp(out["ccs_counts"]), ctypes.byref(ms)))
+    out["ms"] = float(ms.value)
+    return out
+
+  def ccs_ids(self, rows_or_packed: np.ndarray) -> np.ndarray:
+    """The CCS row of every window as ids uint8 [B, L] (model_utils.get_ccs_from_example: row 4 * max_passes)."""
+    return ccs_ids_from_input(self.params, rows_or_packed)
+
+  def evaluate(self, rows_or_packed: np.ndarray, labels: np.ndarray, strict: Optional[bool] = None,
+               del_cost: Optional[float] = None, loss_reg: Any = "params", band_width: Any = "params",
+               strict_input: bool = True) -> Dict[str, Any]:
+    """Forward + evaluation of labelled windows: float32 rows [B, R, L(,1)] or packed rows uint8 [B, packed bytes],
+    labels uint8 [B, L].  The forward writes its probabilities to device memory and dcb_evaluate reads them there;
+    they never come back to the host.  Returns evaluate_windows()'s dict (concatenated over max_batch chunks) plus
+    forward_ms / eval_ms, the summed device times."""
+    x = np.asarray(rows_or_packed)
+    packed = x.dtype == np.uint8 and x.ndim == 2
+    if packed:
+      x = np.ascontiguousarray(x)
+      if x.shape[1] != self.packed_window_bytes:
+        raise ValueError("packed rows must be uint8 [B, %d]" % self.packed_window_bytes)
+    else:
+      x = self._rows3(x)
+    B, L = x.shape[0], self.max_length
+    labels = np.ascontiguousarray(labels, dtype=np.uint8)
+    if labels.shape != (B, L):
+      raise ValueError("labels must be uint8 [%d, %d]" % (B, L))
+    ccs = self.ccs_ids(x)
+    mb = min(self.max_batch, max(B, 1))
+    d_probs = self.alloc_device(mb * L * 5 * 4)
+    d_bq = self.alloc_device(2 * mb * L)
+    parts = []
+    fwd_ms = eval_ms = 0.0
+    try:
+      fn = self._lib.dcb_forward_packed if packed else self._lib.dcb_forward
+      for b0 in range(0, B, mb):
+        b1 = min(B, b0 + mb)
+        rc = fn(self._handle, x[b0:b1].ctypes.data_as(ctypes.c_void_p), b1 - b0,
+                DCB_OUT_ON_DEVICE | self._precision_flag(strict), ctypes.c_void_p(d_bq),
+                ctypes.c_void_p(d_bq + mb * L), ctypes.c_void_p(d_probs), None)
+        self._check(rc, tolerate=() if strict_input else (-5,))
+        fwd_ms += self.last_forward_ms()
+        r = self.evaluate_windows(d_probs, labels[b0:b1], ccs[b0:b1], del_cost, loss_reg, band_width, on_device=True,
+                                  batch=b1 - b0)
+        eval_ms += r.pop("ms")
+        parts.append(r)
+    finally:
+      self.free_device(d_probs)
+      self.free_device(d_bq)
+    if not parts:
+      parts = [dict(loss=np.zeros(0, np.float32), exact=np.zeros(0, np.uint8), pred_counts=np.zeros((0, 5), np.int32),
+                    ccs_counts=np.zeros((0, 5), np.int32))]
+    out = {k: np.concatenate([p_[k] for p_ in parts]) for k in parts[0]}
+    out["forward_ms"], out["eval_ms"] = fwd_ms, eval_ms
+    return out
+
   def predict(self, rows: np.ndarray) -> _Prediction:
     """Softmax output [B, L, 5], shaped like `EncoderOnlyTransformer.predict` (networks.py:357-365)."""
     return _Prediction(self.forward(rows, want_probs=True)["probs"])
@@ -699,6 +798,20 @@ def unpack_rows(params: params_lib.Params, packed: np.ndarray) -> np.ndarray:
   sn = np.ascontiguousarray(packed[:, sn_off:sn_off + 16]).view(np.float32)
   rows[:, R - 4:] = sn[:, :, None]
   return rows
+
+
+def ccs_ids_from_input(params: params_lib.Params, rows_or_packed: np.ndarray) -> np.ndarray:
+  """The CCS row (row 4 * max_passes, data_providers.get_indices) of float32 rows [B, R, L(,1)] or packed rows
+  [B, packed bytes] as uint8 ids [B, L]; values outside 0..4 become 0, the id their all-zero one-hot row decodes to."""
+  x = np.asarray(rows_or_packed)
+  P, L = int(params.max_passes), int(params.max_length)
+  if x.dtype == np.uint8 and x.ndim == 2:
+    return np.ascontiguousarray(x[:, 3 * P * L:(3 * P + 1) * L])   # dcb_pack_rows rejects ccs ids outside 0..4
+  if x.ndim == 4:
+    x = x[..., 0]
+  c = x[:, 4 * P, :]
+  ok = (c >= 0) & (c <= 4)
+  return np.where(ok, np.trunc(np.where(ok, c, 0)), 0).astype(np.uint8)
 
 
 def alloc_pinned(nbytes: int) -> Tuple[int, np.ndarray]:

@@ -208,6 +208,35 @@ int dcb_fill_skipped(dcb_engine* e, const uint8_t* ccs_ids, const int16_t* ccs_b
                      int32_t L, int32_t calibration_enabled, double calibration_threshold, double calibration_w,
                      double calibration_b, uint32_t flags, uint8_t* bases, uint8_t* quals);
 
+/* ---- evaluation of labelled windows ---------------------------------------------------------------------------------
+ * What model_inference.py (models/model_inference.py:79-120 -> model_utils.run_inference_and_write_results,
+ * model_utils.py:379-421) has `model.evaluate` compute per window, and the identity of the training loop's metrics
+ * (model_utils.get_deepconsensus_metrics, model_utils.py:69-96), for a batch of B windows of length L <= 256:
+ *   loss_out [B]         AlignmentLoss.eval with width=None (losses_and_metrics.py:306-411,549-595): label left-shifted
+ *                        (:92-115), probs renormalised to sum to 1, xentropy substitution / insertion costs clipped at
+ *                        1e-7 (:123-143,191-207), constant del_cost, soft-min -loss_reg * logsumexp(-t / loss_reg) --
+ *                        or the hard min when loss_reg <= 0 (params.loss_reg None) -- read at anti-diagonal
+ *                        seq_len + L, row seq_len.  float32, as the reference.
+ *   exact_out [B]        PerExampleAccuracy (losses_and_metrics.py:37-65): 1 when the left-shifted argmax prediction
+ *                        equals the left-shifted label at all L positions.
+ *   pred_counts [B][5]   AlignmentMetric.alignment (losses_and_metrics.py:704-1043) of the label against the
+ *                        argmax-decoded prediction: num_matches, num_insertions, num_deletions, num_correct_matches,
+ *                        alignment_length (affine gaps: match +2, mismatch -5, open 5+4, extend 4; ties go to the
+ *                        first of [match, ins, del]).
+ *   ccs_counts [B][5]    the same against the window's CCS row (get_batch_identity_ccs_pred,
+ *                        losses_and_metrics.py:1061-1098; the row is model_utils.get_ccs_from_example,
+ *                        model_utils.py:128-139, i.e. row 4 * max_passes of data_providers.get_indices).
+ * probs float32 [B, L, 5]: a host array, or with DCB_ROWS_ON_DEVICE a device array (e.g. the DCB_OUT_ON_DEVICE probs_out
+ * of dcb_forward / dcb_forward_packed, so that the probabilities never leave the GPU).  labels / ccs_ids: host u8 [B, L],
+ * ids 0..4 over ' ATCG' (labels outside 0..4 are DCB_ERR_INVALID; a CCS id outside 0..4 counts as a gap, as its
+ * all-zero one-hot row decodes).  band_width >= 0 (the banded AlignmentLoss, params.band_width set) is DCB_ERR_INVALID;
+ * pass DCB_BAND_WIDTH_NONE.  Outputs are host arrays; ms_out (nullable) receives the device time of the evaluation
+ * kernels.  Deterministic: repeated calls give identical bits. */
+#define DCB_BAND_WIDTH_NONE (-1)
+int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const uint8_t* ccs_ids, int32_t batch,
+                 int32_t L, double del_cost, double loss_reg, int32_t band_width, uint32_t flags, float* loss_out,
+                 uint8_t* exact_out, int32_t* pred_counts, int32_t* ccs_counts, float* ms_out);
+
 /* ---- feature construction from BAM (host C++, htslib-free, needs no GPU) -----------------------------------------------
  * What `deepconsensus run` does in front of the model: stream the subreads-to-CCS BAM ZMW by ZMW (SubreadGrouper,
  * pre_lib.py:50-91), expand / clip / indent every subread (expand_clip_indent with trim_insertions, :1061-1239), fetch

@@ -323,3 +323,224 @@ def install():
     setattr(pysam, n, i)
   sys.modules["pysam"] = pysam
   return tf
+
+
+# --------------------------------------------------------------------------- ops of models/losses_and_metrics.py
+# Used only by scripts/make_loss_golden.py.  Reductions over small float axes are summed in order, left to right, as
+# Eigen's inner-dimension reducer does below its packet size; reduce_logsumexp follows tf.math.reduce_logsumexp
+# (max subtracted, replaced by 0 where it is not finite).
+def _np_dtype(dtype):
+  if dtype is None:
+    return None
+  name = getattr(dtype, "name", None) or str(dtype)
+  return np.dtype({"float32": "float32", "float64": "float64", "int32": "int32", "int64": "int64",
+                   "bool": "bool"}[name])
+
+
+def _cast_any(x, dtype):
+  x, dt = np.asarray(x), _np_dtype(dtype)
+  if dt.kind in "iu" and x.dtype.kind == "f":
+    x = np.trunc(x)
+  return _t(x.astype(dt))
+
+
+def _fold_sum(x, axis):
+  x = np.asarray(x)
+  if x.dtype.kind != "f":
+    return x.sum(axis=axis)
+  x = np.moveaxis(x, axis, 0)
+  acc = np.zeros(x.shape[1:], x.dtype)
+  for t in range(x.shape[0]):
+    acc = (acc + x[t]).astype(x.dtype)
+  return acc
+
+
+def _reduce_sum(x, axis=None, keepdims=False):
+  x = np.asarray(x)
+  if axis is None:
+    out = _fold_sum(x.reshape(-1), 0)
+  else:
+    axes = [axis] if np.isscalar(axis) else list(axis)
+    out = x
+    for a in sorted([a % x.ndim for a in axes], reverse=True):
+      out = _fold_sum(out, a)
+    if keepdims:
+      for a in sorted(a % x.ndim for a in axes):
+        out = np.expand_dims(out, a)
+  return _t(np.asarray(out))
+
+
+def _reduce_logsumexp(x, axis):
+  x = np.asarray(x)
+  raw = x.max(axis=axis, keepdims=True)
+  m = np.where(np.isfinite(raw), raw, np.zeros_like(raw))
+  s = _fold_sum(np.exp(x - m), axis % x.ndim)
+  return _t((np.log(s) + np.squeeze(m, axis)).astype(x.dtype))
+
+
+def _tf_slice(x, begin, size):
+  x = np.asarray(x)
+  idx = tuple(slice(int(b), None if int(s) == -1 else int(b) + int(s)) for b, s in zip(begin, size))
+  return _t(x[idx])
+
+
+def _gather(params, indices, axis=None, batch_dims=0):
+  params, indices = np.asarray(params), np.asarray(indices)
+  if batch_dims:
+    assert params.ndim == 2 and indices.ndim == 2, "only the [B, L] batch gather of left_shift_sequence"
+    return _t(np.take_along_axis(params, indices, axis=1))
+  return _t(np.take(params, indices, axis=axis or 0))
+
+
+def _gather_nd(params, indices):
+  params, indices = np.asarray(params), np.asarray(indices)
+  return _t(params[tuple(np.moveaxis(indices, -1, 0))])
+
+
+def _scatter_nd(indices, updates, shape):
+  out = np.zeros([int(s) for s in shape], np.asarray(updates).dtype)
+  np.add.at(out, tuple(np.moveaxis(np.asarray(indices), -1, 0)), np.asarray(updates))
+  return _t(out)
+
+
+def _fill(dims, value):
+  v = np.asarray(value)
+  dt = np.int32 if v.dtype.kind in "iu" else v.dtype
+  return _t(np.full([int(d) for d in np.atleast_1d(dims)], v, dt))
+
+
+def _pad(x, paddings, constant_values=0):
+  x = np.asarray(x)
+  return _t(np.pad(x, [(int(a), int(b)) for a, b in paddings], constant_values=np.asarray(constant_values, x.dtype)))
+
+
+def _one_hot(indices, depth, dtype=None):
+  idx = np.asarray(indices).astype(np.int64)
+  ok = (idx >= 0) & (idx < depth)
+  out = (np.arange(depth) == np.where(ok, idx, -1)[..., None]).astype(_np_dtype(dtype) or np.float32)
+  return _t(out)
+
+
+def _xlogy(x, y):
+  x, y = np.asarray(x), np.asarray(y)
+  with np.errstate(divide="ignore", invalid="ignore"):
+    return _t(np.where(x == 0, np.zeros_like(x * y), x * np.log(y)).astype(np.result_type(x, y)))
+
+
+class _TensorArray:
+  def __init__(self, dtype, size=0, clear_after_read=True, **kw):
+    self._items = {}
+
+  def write(self, i, v):
+    self._items[int(i)] = np.asarray(v)
+    return self
+
+  def read(self, i):
+    return _t(self._items[int(i)])
+
+  def stack(self):
+    return _t(np.stack([self._items[i] for i in sorted(self._items)]))
+
+
+class _Loss:
+  def __init__(self, reduction=None, name=None):
+    self.reduction = reduction
+
+  def __call__(self, y_true, y_pred):
+    return _t(np.asarray(self.call(y_true, y_pred)).mean(dtype=np.float32))
+
+
+class _Weight:
+  def __init__(self):
+    self.value = np.float32(0)
+
+  def assign_add(self, v):
+    self.value = np.float32(self.value + np.float32(v))
+
+  def assign(self, v):
+    self.value = np.float32(v)
+
+  def __array__(self, dtype=None, copy=None):
+    return np.asarray(self.value, dtype=dtype)
+
+
+class _Metric:
+  def __init__(self, name=None, **kw):
+    self.name = name
+
+  def add_weight(self, name=None, shape=None, initializer=None):
+    return _Weight()
+
+
+class _Mean(_Metric):
+  def __init__(self, name=None, **kw):
+    super().__init__(name)
+    self.reset_states()
+
+  def update_state(self, values, sample_weight=None):
+    v = np.asarray(values, np.float64).reshape(-1)
+    self._sum += v.sum()
+    self._n += v.size
+
+  def result(self):
+    return _t(np.float32(self._sum / self._n if self._n else 0.0))
+
+  def reset_states(self):
+    self._sum, self._n = 0.0, 0
+
+
+class _Accuracy(_Mean):
+  def update_state(self, y_true, y_pred, sample_weight=None):
+    super().update_state(np.asarray(y_true) == np.asarray(y_pred))
+
+
+def install_losses_ops(tf):
+  """Adds what losses_and_metrics.py (and dc_constants.py) use to the stand-in installed by install()."""
+  tf.bool = "bool"
+  tf.newaxis = None
+  tf.cast = _cast_any
+  tf.shape = lambda x: np.array(np.shape(x), np.int32)
+  tf.range = lambda *a, dtype=None: _t(np.arange(*[int(v) for v in a], dtype=_np_dtype(dtype) or np.int32))
+  tf.broadcast_to = lambda x, shape: _t(np.broadcast_to(np.asarray(x), [int(s) for s in shape]))
+  tf.sort = lambda x, axis=-1: _t(np.sort(np.asarray(x), axis=axis))
+  tf.where = lambda c, a, b: _t(np.where(np.asarray(c), np.asarray(a), np.asarray(b)))
+  tf.gather, tf.gather_nd, tf.scatter_nd = _gather, _gather_nd, _scatter_nd
+  tf.reduce_sum = _reduce_sum
+  tf.reduce_min = lambda x, axis=None: _t(np.asarray(x).min(axis=axis))
+  tf.reduce_max = lambda x, axis=None: _t(np.asarray(x).max(axis=axis))
+  tf.reduce_logsumexp = _reduce_logsumexp
+  tf.argmax = lambda x, axis=None, output_type=None: _t(
+      np.asarray(x).argmax(axis=-1 if axis is None else axis).astype(_np_dtype(output_type) or np.int64))
+  tf.one_hot = _one_hot
+  tf.convert_to_tensor = lambda x, dtype=None, **kw: _t(np.asarray(x, dtype=_np_dtype(dtype)))
+  tf.constant = lambda x, dtype=None: _t(np.asarray(x, dtype=_np_dtype(dtype)))
+  tf.clip_by_value = lambda x, lo, hi: _t(np.clip(np.asarray(x), np.asarray(lo, np.asarray(x).dtype),
+                                                  np.asarray(hi, np.asarray(x).dtype)))
+  tf.expand_dims = lambda x, axis: _t(np.expand_dims(np.asarray(x), axis))
+  tf.squeeze = lambda x, axis=None: _t(np.squeeze(np.asarray(x), tuple(axis) if isinstance(axis, list) else axis))
+  tf.slice = _tf_slice
+  tf.pad = _pad
+  tf.transpose = lambda x, perm=None: _t(np.transpose(np.asarray(x), perm))
+  tf.fill = _fill
+  tf.concat = lambda xs, axis: _t(np.concatenate([np.asarray(x) for x in xs], axis=axis))
+  tf.stack = lambda xs, axis=0: _t(np.stack([np.asarray(x) for x in xs], axis=axis))
+  tf.roll = lambda x, shift, axis: _t(np.roll(np.asarray(x), shift, axis))
+  tf.reshape = lambda x, s: _t(np.reshape(np.asarray(x), [int(v) for v in s]))
+  tf.maximum = lambda a, b: _t(np.maximum(a, b))
+  tf.logical_and = lambda a, b: _t(np.logical_and(a, b))
+  tf.logical_or = lambda a, b: _t(np.logical_or(a, b))
+  tf.logical_not = lambda a: _t(np.logical_not(a))
+  tf.equal = lambda a, b: _t(np.equal(a, b))
+  tf.ones_like = lambda x: _t(np.ones_like(np.asarray(x)))
+  tf.zeros = lambda shape, dtype=None: _t(np.zeros(shape, _np_dtype(dtype) or np.float32))
+  tf.TensorArray = _TensorArray
+  tf.debugging = _NS(assert_equal=lambda x, y, message=None: None)
+  tf.math = _NS(log=lambda x: _t(np.log(np.asarray(x))), xlogy=_xlogy,
+                count_nonzero=lambda x, axis=None: _t(np.count_nonzero(np.asarray(x), axis=axis)),
+                divide_no_nan=lambda a, b: _t(np.float32(0) if float(np.asarray(b)) == 0 else
+                                              np.float32(np.asarray(a) / np.asarray(b))))
+  tf.keras.losses = _NS(Loss=_Loss, Reduction=_NS(AUTO="auto", NONE="none", SUM="sum"))
+  tf.keras.metrics = _NS(Metric=_Metric, Mean=_Mean, Accuracy=_Accuracy)
+  tf.metrics = tf.keras.metrics
+  sys.modules["tensorflow.compat.v2"].__dict__.update(tf.__dict__)
+  return tf
