@@ -8,6 +8,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <functional>
 #include <map>
 #include <string>
@@ -100,7 +101,8 @@ struct dcb_engine {
   double* d_p10 = nullptr;           // 10^(-q/10), q = 0..255 (host libm pow, as NumPy)
   struct Scratch { void* p = nullptr; size_t cap = 0; } sc_pos, sc_names, sc_nameoff, sc_outcome, sc_avg, sc_recoff, sc_fastq,
       sc_bq, sc_mask, sc_ids, sc_dst, sc_tmpb, sc_tmpq,
-      sc_ev_probs, sc_ev_in, sc_ev_out;   // dcb_evaluate: host probs, labels | ccs ids, loss | counts | flags
+      sc_ev_probs, sc_ev_in, sc_ev_out,   // dcb_evaluate: host probs, labels | ccs ids, loss | counts | flags
+      sc_ds_in, sc_ds_out;                // dcb_distill_loss: host teacher | student logits, loss
   cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;
   float* d_dbg = nullptr;  // [stages][chunk_tiles * x_image]
   // strict-fp32 path (strict_kernels.cu): float32 copies of every variable in the reference's own shapes, and a
@@ -323,7 +325,7 @@ void dcb_destroy(dcb_engine* e) {
   if (e->d_st_len) cudaFree(e->d_st_len);
   for (dcb_engine::Scratch* sc : {&e->sc_pos, &e->sc_names, &e->sc_nameoff, &e->sc_outcome, &e->sc_avg, &e->sc_recoff,
                                   &e->sc_fastq, &e->sc_bq, &e->sc_mask, &e->sc_ids, &e->sc_dst, &e->sc_tmpb, &e->sc_tmpq,
-                                  &e->sc_ev_probs, &e->sc_ev_in, &e->sc_ev_out})
+                                  &e->sc_ev_probs, &e->sc_ev_in, &e->sc_ev_out, &e->sc_ds_in, &e->sc_ds_out})
     if (sc->p) cudaFree(sc->p);
   if (e->ev_eval0) cudaEventDestroy(e->ev_eval0);
   if (e->ev_eval1) cudaEventDestroy(e->ev_eval1);
@@ -1293,6 +1295,52 @@ int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const
   CU(e, cudaMemcpyAsync(pred_counts, d_pred, (size_t)batch * 5 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CU(e, cudaMemcpyAsync(ccs_counts, d_ccs, (size_t)batch * 5 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CU(e, cudaMemcpyAsync(exact_out, d_exact, (size_t)batch, cudaMemcpyDeviceToHost, st));
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  return DCB_OK;
+}
+
+int dcb_distill_loss(dcb_engine* e, const float* teacher_logits, const float* student_logits, int32_t batch,
+                     int32_t L, double temperature, int32_t logit_loss, uint32_t flags, float* loss_out,
+                     float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  if (batch < 0 || L <= 0 || L > 256)
+    return fail(e, DCB_ERR_INVALID, "dcb_distill_loss: need batch >= 0 and 0 < L <= 256 (batch=%d, L=%d)", batch, L);
+  const float t32 = (float)temperature;   // the logits are divided in float32, as tf divides a float32 tensor
+  if (!std::isfinite(temperature) || !(temperature > 0.0) || !std::isfinite(t32) || !(t32 > 0.f))
+    return fail(e, DCB_ERR_INVALID, "dcb_distill_loss: temperature must be finite and > 0 in float32 (got %g)",
+                temperature);
+  if (logit_loss != DCB_LOGIT_LOSS_MSE && logit_loss != DCB_LOGIT_LOSS_KL)
+    return fail(e, DCB_ERR_INVALID, "dcb_distill_loss: unknown logit loss id %d (DCB_LOGIT_LOSS_MSE = %d, "
+                "DCB_LOGIT_LOSS_KL = %d)", logit_loss, DCB_LOGIT_LOSS_MSE, DCB_LOGIT_LOSS_KL);
+  if (ms_out) *ms_out = 0.f;
+  if (batch == 0) return DCB_OK;
+  if (!teacher_logits || !student_logits || !loss_out)
+    return fail(e, DCB_ERR_INVALID, "dcb_distill_loss: null pointer");
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  const size_t nlog = (size_t)batch * L * kVocab;
+  int rc;
+  if ((rc = ensure(e, e->sc_ds_out, (size_t)batch * sizeof(float))) ||
+      (!(flags & DCB_ROWS_ON_DEVICE) && (rc = ensure(e, e->sc_ds_in, 2 * nlog * sizeof(float)))))
+    return rc;
+  if (!e->ev_eval0) CU(e, cudaEventCreate(&e->ev_eval0));
+  if (!e->ev_eval1) CU(e, cudaEventCreate(&e->ev_eval1));
+  const float* d_teacher = teacher_logits;
+  const float* d_student = student_logits;
+  if (!(flags & DCB_ROWS_ON_DEVICE)) {
+    float* d_in = static_cast<float*>(e->sc_ds_in.p);
+    CU(e, cudaMemcpyAsync(d_in, teacher_logits, nlog * sizeof(float), cudaMemcpyHostToDevice, st));
+    CU(e, cudaMemcpyAsync(d_in + nlog, student_logits, nlog * sizeof(float), cudaMemcpyHostToDevice, st));
+    d_teacher = d_in;
+    d_student = d_in + nlog;
+  }
+  float* d_loss = static_cast<float*>(e->sc_ds_out.p);
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  CU(e, launch_distill_loss(d_teacher, d_student, batch, L, t32, logit_loss, d_loss, st));
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  CU(e, cudaMemcpyAsync(loss_out, d_loss, (size_t)batch * sizeof(float), cudaMemcpyDeviceToHost, st));
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));

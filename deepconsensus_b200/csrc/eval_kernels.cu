@@ -15,6 +15,9 @@
 //                           directions of every cell are kept as one byte in shared memory ((L+1)^2 bytes, 66 KB at
 //                           L = 256) and one thread walks the traceback, counting the trans_enc edges 1-5.  The y = 0
 //                           CTA also writes PerExampleAccuracy's exact-match flag (:43-65).
+//   distill_loss_kernel     DistillationLoss.call (:1170-1213) on teacher and student logits, one warp per window: the
+//                           temperature-scaled softmax of both, the Keras logit loss (mean squared error or KL
+//                           divergence) per position, the mean over the window.
 // Results are deterministic: every reduction is a fixed-order loop, no atomics.
 #include <cuda_runtime.h>
 #include <math.h>
@@ -31,6 +34,8 @@ constexpr int kEvalMaxL = 256;
 constexpr float kInf = 1e9f;
 constexpr float kEps = 1e-7f;
 constexpr float kOneMinusEps = (float)(1.0 - 1e-7);   // Python's 1 - eps, then float32, as tf.clip_by_value sees it
+constexpr int kDistillWarps = 4;                       // windows (one warp each) per CTA of distill_loss_kernel
+constexpr int kLogitLossKL = 1;                        // DCB_LOGIT_LOSS_KL (include/dcb200.h); 0 is MSE
 
 // Left shift (left_shift_sequence): non-gap ids in order, then gaps.  One thread; L <= 256.  Returns the non-gap count.
 __device__ int left_shift_serial(const uint8_t* in, uint8_t* out, int L) {
@@ -235,6 +240,71 @@ align_identity_kernel(const float* __restrict__ probs, const uint8_t* __restrict
   }
   int32_t* out = (which == 0 ? pred_counts : ccs_counts) + (size_t)b * 5;
   out[0] = nm; out[1] = ni; out[2] = nd; out[3] = nc; out[4] = nm + ni + nd;
+}
+
+// DistillationLoss.call (losses_and_metrics.py:1170-1213), one warp per window, lanes over positions.  Per position
+// t = softmax(teacher / T), s = softmax(student / T) as tf.nn.softmax computes them (divide by T, subtract the max,
+// exp, sum in order, divide), then the Keras logit loss with the teacher as y_true:
+//   DCB_LOGIT_LOSS_MSE  mean_c (s_c - t_c)^2                                   (sum in order, / 5)
+//   DCB_LOGIT_LOSS_KL   sum_c t_c * log(t_c / s_c), both clipped to [1e-7, 1]  (sum in order)
+// and the mean over all L positions, padding included (reduce_mean(loss, axis=-1)).  Lane i sums positions i, i + 32,
+// ... in order; the 32 partial sums are combined by a fixed shuffle-down tree (offsets 16, 8, 4, 2, 1), so every call
+// gives the same bits.  Every float operation is an explicit _rn intrinsic: nothing is contracted into an FMA, and
+// identical teacher and student logits give exactly 0.
+__device__ __forceinline__ void softmax5_scaled(const float* __restrict__ logits, float temperature, float* p) {
+  float x[kVocab];
+  for (int c = 0; c < kVocab; ++c) x[c] = __fdiv_rn(logits[c], temperature);
+  float mx = x[0];
+  for (int c = 1; c < kVocab; ++c) mx = fmaxf(mx, x[c]);
+  for (int c = 0; c < kVocab; ++c) x[c] = expf(__fsub_rn(x[c], mx));
+  float sum = x[0];
+  for (int c = 1; c < kVocab; ++c) sum = __fadd_rn(sum, x[c]);
+  for (int c = 0; c < kVocab; ++c) p[c] = __fdiv_rn(x[c], sum);
+}
+
+__global__ void __launch_bounds__(kDistillWarps * 32)
+distill_loss_kernel(const float* __restrict__ teacher, const float* __restrict__ student, int B, int L,
+                    float temperature, int logit_loss, float* __restrict__ loss_out) {
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * kDistillWarps + (threadIdx.x >> 5);
+  if (b >= B) return;                                      // whole warps retire together
+  const float* tw = teacher + (size_t)b * L * kVocab;
+  const float* sw = student + (size_t)b * L * kVocab;
+  float acc = 0.f;
+  for (int j = lane; j < L; j += 32) {
+    float tl[kVocab], sl[kVocab], t[kVocab], s[kVocab];
+    for (int c = 0; c < kVocab; ++c) {
+      tl[c] = __ldg(tw + j * kVocab + c);
+      sl[c] = __ldg(sw + j * kVocab + c);
+    }
+    softmax5_scaled(tl, temperature, t);
+    softmax5_scaled(sl, temperature, s);
+    float v = 0.f;
+    if (logit_loss == kLogitLossKL) {
+      for (int c = 0; c < kVocab; ++c) {
+        const float tc = fminf(fmaxf(t[c], kEps), 1.f), sc = fminf(fmaxf(s[c], kEps), 1.f);
+        const float term = __fmul_rn(tc, logf(__fdiv_rn(tc, sc)));
+        v = c == 0 ? term : __fadd_rn(v, term);
+      }
+    } else {
+      for (int c = 0; c < kVocab; ++c) {
+        const float d = __fsub_rn(s[c], t[c]);
+        v = c == 0 ? __fmul_rn(d, d) : __fadd_rn(v, __fmul_rn(d, d));
+      }
+      v = __fdiv_rn(v, (float)kVocab);
+    }
+    acc = j == lane ? v : __fadd_rn(acc, v);
+  }
+  for (int off = 16; off > 0; off >>= 1) acc = __fadd_rn(acc, __shfl_down_sync(0xffffffffu, acc, off));
+  if (lane == 0) loss_out[b] = __fdiv_rn(acc, (float)L);
+}
+
+cudaError_t launch_distill_loss(const float* teacher, const float* student, int B, int L, float temperature,
+                                int logit_loss, float* loss, cudaStream_t st) {
+  if (B <= 0) return cudaSuccess;
+  distill_loss_kernel<<<(B + kDistillWarps - 1) / kDistillWarps, kDistillWarps * 32, 0, st>>>(
+      teacher, student, B, L, temperature, logit_loss, loss);
+  return cudaGetLastError();
 }
 
 size_t eval_identity_smem_bytes(int L) {

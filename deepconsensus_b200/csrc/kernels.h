@@ -52,6 +52,10 @@ void launch_fill_skipped(const uint8_t* ccs_ids, const int16_t* ccs_bq, const in
 cudaError_t launch_evaluate(const float* probs, const uint8_t* labels, const uint8_t* ccs_ids, int B, int L,
                             float del_cost, float loss_reg, int hard_min, float* loss, uint8_t* exact,
                             int32_t* pred_counts, int32_t* ccs_counts, cudaStream_t st);
+// DistillationLoss per window from teacher / student logits [B, L, 5]; logit_loss 0 = mean squared error, 1 = KL
+// divergence (DCB_LOGIT_LOSS_*).  Device pointers.
+cudaError_t launch_distill_loss(const float* teacher, const float* student, int B, int L, float temperature,
+                                int logit_loss, float* loss, cudaStream_t st);
 
 // ---- strict-fp32 path (strict_kernels.cu): row-major float32 activations, windows packed back to back
 void launch_strict_embed(const float* rows, int R, int L, int E, int nwindows, const StrictEmbedRow* meta,

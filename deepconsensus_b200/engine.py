@@ -38,6 +38,11 @@ DCB_PRECISION_FP32 = 1
 DCB_READ_OK, DCB_READ_EMPTY, DCB_READ_ONLY_GAPS, DCB_READ_LOW_QUALITY, DCB_READ_TOO_SHORT = 0, 1, 2, 3, 4
 DCB_READ_BORDERLINE = 0x80
 DCB_BAND_WIDTH_NONE = -1
+DCB_LOGIT_LOSS_MSE, DCB_LOGIT_LOSS_KL = 0, 1
+# Keras loss identifiers (tf.keras.losses.get) of the two logit losses DistillationLoss is used with
+LOGIT_LOSS_IDS = {"mean_squared_error": DCB_LOGIT_LOSS_MSE, "mse": DCB_LOGIT_LOSS_MSE, "MSE": DCB_LOGIT_LOSS_MSE,
+                  "kl_divergence": DCB_LOGIT_LOSS_KL, "kullback_leibler_divergence": DCB_LOGIT_LOSS_KL,
+                  "kld": DCB_LOGIT_LOSS_KL, "KLD": DCB_LOGIT_LOSS_KL}
 # columns of dcb_evaluate's per-window alignment counts (AlignmentMetric.alignment's metric_values)
 EVAL_COUNT_KEYS = ("num_matches", "num_insertions", "num_deletions", "num_correct_matches", "alignment_length")
 
@@ -80,7 +85,7 @@ class DcbTensor(ctypes.Structure):
 ABI_SYMBOLS = (
     "dcb_create", "dcb_load_weights", "dcb_forward", "dcb_submit", "dcb_wait", "dcb_stitch", "dcb_last_forward_ms",
     "dcb_packed_window_bytes", "dcb_pack_rows", "dcb_forward_packed", "dcb_submit_packed",
-    "dcb_stitch_fastq", "dcb_skip_mask", "dcb_fill_skipped", "dcb_evaluate",
+    "dcb_stitch_fastq", "dcb_skip_mask", "dcb_fill_skipped", "dcb_evaluate", "dcb_distill_loss",
     "dcb_prep_open", "dcb_prep_set_threads", "dcb_prep_next_zmw", "dcb_prep_get_windows", "dcb_prep_ccs_header", "dcb_prep_close",
     "dcb_prep_last_error", "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
     "dcb_last_forward_launches", "dcb_set_profile", "dcb_get_profile", "dcb_get_profile_kernels", "dcb_alloc_host",
@@ -139,6 +144,7 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_fill_skipped.argtypes = [vp, vp, vp, vp, i32, i32, i32, f64, f64, f64, u32, vp, vp]
   lib.dcb_evaluate.argtypes = [vp, vp, vp, vp, i32, i32, f64, f64, i32, u32, vp, vp, vp, vp,
                                ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_distill_loss.argtypes = [vp, vp, vp, i32, i32, f64, i32, u32, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_launches.argtypes = [vp, ctypes.POINTER(i32)]
   lib.dcb_set_debug.argtypes = [vp, i32]
@@ -616,6 +622,33 @@ class B200Model:
     out["ms"] = float(ms.value)
     return out
 
+  def distill_loss(self, teacher_logits, student_logits, temperature: float = 1.0, logit_loss: Any = "kl_divergence",
+                   on_device: bool = False, batch: Optional[int] = None,
+                   length: Optional[int] = None) -> Dict[str, Any]:
+    """dcb_distill_loss: per-window DistillationLoss between teacher and student logits float32 [B, L, 5] (host arrays,
+    or device addresses with on_device=True, `batch` and optionally `length`, default max_length).  logit_loss is a
+    Keras identifier (LOGIT_LOSS_IDS) or a DCB_LOGIT_LOSS_* id.  Returns loss float32 [B] and ms, the kernel's device
+    time."""
+    lid = logit_loss_id(logit_loss)
+    if on_device:
+      if batch is None:
+        raise ValueError("distill_loss(on_device=True) needs batch")
+      B, L = int(batch), int(length) if length is not None else self.max_length
+      t_ptr, s_ptr, flags = ctypes.c_void_p(int(teacher_logits)), ctypes.c_void_p(int(student_logits)), DCB_ROWS_ON_DEVICE
+    else:
+      teacher = np.ascontiguousarray(teacher_logits, dtype=np.float32)
+      student = np.ascontiguousarray(student_logits, dtype=np.float32)
+      if teacher.ndim != 3 or teacher.shape[2] != 5 or student.shape != teacher.shape:
+        raise ValueError("teacher and student logits must both be float32 [B, L, 5], got %s and %s" %
+                         (teacher.shape, student.shape))
+      B, L = teacher.shape[:2]
+      t_ptr, s_ptr, flags = teacher.ctypes.data_as(ctypes.c_void_p), student.ctypes.data_as(ctypes.c_void_p), 0
+    loss = np.zeros(B, np.float32)
+    ms = ctypes.c_float()
+    self._check(self._lib.dcb_distill_loss(self._handle, t_ptr, s_ptr, B, L, float(temperature), lid, flags,
+                                           loss.ctypes.data_as(ctypes.c_void_p), ctypes.byref(ms)))
+    return dict(loss=loss, ms=float(ms.value))
+
   def ccs_ids(self, rows_or_packed: np.ndarray) -> np.ndarray:
     """The CCS row of every window as ids uint8 [B, L] (model_utils.get_ccs_from_example: row 4 * max_passes)."""
     return ccs_ids_from_input(self.params, rows_or_packed)
@@ -812,6 +845,15 @@ def ccs_ids_from_input(params: params_lib.Params, rows_or_packed: np.ndarray) ->
   c = x[:, 4 * P, :]
   ok = (c >= 0) & (c <= 4)
   return np.where(ok, np.trunc(np.where(ok, c, 0)), 0).astype(np.uint8)
+
+
+def logit_loss_id(identifier: Any) -> int:
+  """params.logit_loss_identifier (a tf.keras.losses.get identifier) -> DCB_LOGIT_LOSS_*; an int id passes through."""
+  if isinstance(identifier, (int, np.integer)) and not isinstance(identifier, bool):
+    return int(identifier)
+  if identifier not in LOGIT_LOSS_IDS:
+    raise ValueError("logit loss %r is not supported: use one of %s" % (identifier, ", ".join(LOGIT_LOSS_IDS)))
+  return LOGIT_LOSS_IDS[identifier]
 
 
 def alloc_pinned(nbytes: int) -> Tuple[int, np.ndarray]:

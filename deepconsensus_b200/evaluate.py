@@ -19,6 +19,18 @@ of model_utils.get_deepconsensus_metrics):
     (drop_remainder=False), averaged over batches; identity_ccs the same for the CCS rows;
   * yield_over_ccs: divide_no_nan(#batches with identity >= 0.997, #batches with CCS identity >= 0.997).
 `--limit N` takes the first N batches, as the reference's get_dataset applies ds.take(limit) after batching.
+
+Distilled students (the reference's model_distillation.py): `--teacher_model_dir CKPT` (with `--teacher_random_weights
+SEED` the counterpart of `--random_weights`) builds the teacher as a second engine on the same device and precision,
+from its own params.json; its inputs (max_passes, max_length, use_ccs_bq, the embedding widths and the *_MAX clips) must
+be the student's.  Both forwards leave their logits in device memory, dcb_distill_loss compares them there, and
+`eval_metrics.json` gains a "distillation" entry per dataset with what the distillation loop's eval step reports
+(model_distillation.py:242-270,320-349): per example student_alpha * AlignmentLoss + distill_alpha * DistillationLoss,
+per batch their sum / batch_size (tf.nn.compute_average_loss), `loss` (eval/loss) the mean over batches, the same for
+`student_loss` and `distill_loss` alone, and the accuracy, identity and yield metrics -- all over FULL batches only, as
+create_input_fn batches with drop_remainder=True and get_step_counts counts n // batch_size steps.  distill_alpha,
+student_alpha, temperature and logit_loss_identifier come from the student's params.json (defaults: the
+transformer_learn_values_distill config).  `inference.csv` and the other entries stay the student-only numbers.
 """
 from __future__ import annotations
 
@@ -64,6 +76,51 @@ def aggregate(loss: np.ndarray, exact: np.ndarray, pred_counts: np.ndarray, ccs_
               yield_over_ccs=dc / cc if cc else 0.0,
               batch_identity_pred=ident, batch_identity_ccs=ident_ccs,
               n_windows=n, n_batches=len(ident), batch_size=int(batch_size))
+
+
+# the inputs both models of a distillation pair must agree on: the rows they read and how they embed them
+TEACHER_INPUT_KEYS = ("max_passes", "max_length", "use_ccs_bq", "per_base_hidden_size", "pw_hidden_size",
+                      "ip_hidden_size", "strand_hidden_size", "ccs_bq_hidden_size", "sn_hidden_size", "PW_MAX",
+                      "IP_MAX", "SN_MAX", "CCS_BQ_MAX", "STRAND_MAX")
+DISTILL_KEYS = ("distill_alpha", "student_alpha", "temperature", "logit_loss_identifier")
+
+
+def distill_settings(params: params_lib.Params) -> Dict[str, Any]:
+  """The distillation loss parameters of a student's params.json, defaulting to the transformer_learn_values_distill
+  config's (model_configs.py:155-190)."""
+  defaults = params_lib.get_config("transformer_learn_values_distill+custom")
+  return {k: params[k] if params.get(k) is not None else defaults[k] for k in DISTILL_KEYS}
+
+
+def check_teacher_inputs(student: params_lib.Params, teacher: params_lib.Params) -> None:
+  """Raises ValueError naming the first input key on which the teacher's params.json differs from the student's."""
+  for k in TEACHER_INPUT_KEYS:
+    if student.get(k) != teacher.get(k):
+      raise ValueError("teacher params.%s=%r differs from the student's %r: both models must read the same windows" %
+                       (k, teacher.get(k), student.get(k)))
+
+
+def aggregate_distillation(student_loss: np.ndarray, distill_loss: np.ndarray, exact: np.ndarray,
+                           pred_counts: np.ndarray, ccs_counts: np.ndarray, batch_size: int, student_alpha: float,
+                           distill_alpha: float) -> Dict[str, Any]:
+  """Per-window values -> what the distillation loop's eval step reports, over the full batches only (module
+  docstring).  The losses are computed in float32, as the loop computes them, with sums taken left to right."""
+  f32 = np.float32
+  n_batches = int(student_loss.shape[0]) // batch_size
+  n = n_batches * batch_size
+  sl, dl = np.asarray(student_loss[:n], f32), np.asarray(distill_loss[:n], f32)
+  per_example = ((f32(student_alpha) * sl).astype(f32) + (f32(distill_alpha) * dl).astype(f32)).astype(f32)
+  out = dict(aggregate(sl, exact[:n], pred_counts[:n], ccs_counts[:n], batch_size))
+  for key, v in (("loss", per_example), ("student_loss", sl), ("distill_loss", dl)):
+    total = f32(0)                                     # tf.keras.metrics.Mean over the per-batch losses
+    for b in range(n_batches):
+      s = f32(0)
+      for x in v[b * batch_size:(b + 1) * batch_size]:
+        s = f32(s + x)
+      total = f32(total + f32(s / f32(batch_size)))     # tf.nn.compute_average_loss
+    out[key] = float(f32(total / f32(n_batches))) if n_batches else 0.0
+  out.update(student_alpha=float(student_alpha), distill_alpha=float(distill_alpha))
+  return out
 
 
 def write_inference_csv(path: str, rows: Sequence[Tuple[str, float, float]]) -> None:
@@ -124,12 +181,105 @@ def evaluate_rows(model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndar
   return out
 
 
+def evaluate_rows_distill(student: engine_lib.B200Model, teacher: engine_lib.B200Model, rows: np.ndarray,
+                          labels: np.ndarray, chunk: int, temperature: float, logit_loss: str) -> Dict[str, Any]:
+  """evaluate_rows() for a student and its teacher: per chunk both engines run their forward from the same pinned rows
+  through dcb_submit (device probabilities and logits, two batches in flight per engine); once both tickets are done,
+  dcb_evaluate reads the student's probabilities and dcb_distill_loss the two logits buffers, all on the device.  Adds
+  distill_loss float32 [N] and the teacher's forward and the distillation kernel's device times."""
+  N, L = rows.shape[0], student.max_length
+  ccs = student.ccs_ids(rows)
+  logit_bytes = chunk * L * 5 * 4
+  d_probs = [student.alloc_device(logit_bytes) for _ in range(2)]
+  d_logits_s = [student.alloc_device(logit_bytes) for _ in range(2)]
+  d_bq_s = [student.alloc_device(2 * chunk * L) for _ in range(2)]
+  d_logits_t = [teacher.alloc_device(logit_bytes) for _ in range(2)]
+  d_bq_t = [teacher.alloc_device(2 * chunk * L) for _ in range(2)]
+  parts: List[Dict[str, np.ndarray]] = []
+  times = dict(forward_ms=0.0, teacher_forward_ms=0.0, eval_ms=0.0, distill_ms=0.0)
+
+  in_flight = {id(student): [], id(teacher): []}      # tickets submitted and not yet waited for, per engine
+
+  def wait(m):
+    m.wait_raw(in_flight[id(m)].pop(0))
+
+  def finish(slot, b0, b1):
+    wait(student)
+    times["forward_ms"] += student.last_forward_ms()
+    wait(teacher)
+    times["teacher_forward_ms"] += teacher.last_forward_ms()
+    r = student.evaluate_windows(d_probs[slot], labels[b0:b1], ccs[b0:b1], on_device=True, batch=b1 - b0)
+    times["eval_ms"] += r.pop("ms")
+    d = student.distill_loss(d_logits_t[slot], d_logits_s[slot], temperature, logit_loss, on_device=True,
+                             batch=b1 - b0, length=L)
+    times["distill_ms"] += d["ms"]
+    r["distill_loss"] = d["loss"]
+    parts.append(r)
+
+  pending = None
+  try:
+    for i, b0 in enumerate(range(0, N, chunk)):
+      b1, slot = min(N, b0 + chunk), i % 2
+      staging = student.staging_rows(slot)
+      staging[:b1 - b0] = rows[b0:b1]
+      out_flag = engine_lib.DCB_OUT_ON_DEVICE
+      in_flight[id(student)].append(student.submit_raw(staging.ctypes.data, b1 - b0, out_flag, d_bq_s[slot],
+                                                       d_bq_s[slot] + chunk * L, probs_ptr=d_probs[slot],
+                                                       logits_ptr=d_logits_s[slot]))
+      in_flight[id(teacher)].append(teacher.submit_raw(staging.ctypes.data, b1 - b0, out_flag, d_bq_t[slot],
+                                                       d_bq_t[slot] + chunk * L, logits_ptr=d_logits_t[slot]))
+      prev, pending = pending, (slot, b0, b1)
+      if prev is not None:
+        finish(*prev)
+    if pending is not None:
+      prev, pending = pending, None
+      finish(*prev)
+  finally:
+    for m in (student, teacher):
+      while in_flight[id(m)]:
+        try:
+          wait(m)
+        except engine_lib.DcbError:
+          pass
+    for p in d_probs + d_logits_s + d_bq_s:
+      student.free_device(p)
+    for p in d_logits_t + d_bq_t:
+      teacher.free_device(p)
+  if not parts:
+    parts = [dict(loss=np.zeros(0, np.float32), exact=np.zeros(0, np.uint8), pred_counts=np.zeros((0, 5), np.int32),
+                  ccs_counts=np.zeros((0, 5), np.int32), distill_loss=np.zeros(0, np.float32))]
+  out = {k: np.concatenate([p[k] for p in parts]) for k in parts[0]}
+  out.update(times)
+  return out
+
+
+def _load_teacher(teacher_model_dir: str, options: inference.InferenceOptions, random_weights: Optional[int],
+                  device: int, precision: str) -> engine_lib.B200Model:
+  """The teacher engine: its own params.json (layer count and filter size may differ), the student's options."""
+  tparams = params_lib.read_params_from_json(teacher_model_dir)
+  weights = None
+  if random_weights is not None:
+    params_lib.modify_params(tparams, max_length=options.max_length)
+    weights = weights_lib.init_weights(tparams, seed=random_weights)
+  model, _ = inference.initialize_model(teacher_model_dir, tparams, options, weights=weights, device=device,
+                                        precision=precision)
+  return model
+
+
 def run(checkpoint: str, eval_path: Sequence[str], out_dir: str, limit: int = -1, batch_size: Optional[int] = None,
         precision: str = "bf16", random_weights: Optional[int] = None, device: int = 0,
-        chunk: int = 1024) -> Dict[str, Any]:
+        chunk: int = 1024, teacher_model_dir: Optional[str] = None,
+        teacher_random_weights: Optional[int] = None) -> Dict[str, Any]:
   params = params_lib.read_params_from_json(checkpoint)
   if params.get("band_width") is not None:
     raise ValueError("params.band_width=%s: the banded alignment loss is not supported" % params.band_width)
+  distill = None
+  if teacher_random_weights is not None and teacher_model_dir is None:
+    raise ValueError("--teacher_random_weights needs --teacher_model_dir")
+  if teacher_model_dir is not None:
+    distill = distill_settings(params)
+    engine_lib.logit_loss_id(distill["logit_loss_identifier"])      # an unsupported identifier fails before any work
+    check_teacher_inputs(params, params_lib.read_params_from_json(teacher_model_dir))
   bs = int(batch_size or params.get("batch_size", 1))
   options = inference.InferenceOptions(
       max_length=int(params.max_length), example_height=params_lib.get_total_rows(params.max_passes, params.use_ccs_bq),
@@ -142,6 +292,13 @@ def run(checkpoint: str, eval_path: Sequence[str], out_dir: str, limit: int = -1
     weights = weights_lib.init_weights(params, seed=random_weights)
   model, params = inference.initialize_model(checkpoint, params, options, weights=weights, device=device,
                                              precision=precision)
+  teacher = None
+  if distill is not None:
+    try:
+      teacher = _load_teacher(teacher_model_dir, options, teacher_random_weights, device, precision)
+    except BaseException:
+      model.close()
+      raise
   os.makedirs(out_dir, exist_ok=True)
   csv_rows, metrics = [], {}
   try:
@@ -153,14 +310,28 @@ def run(checkpoint: str, eval_path: Sequence[str], out_dir: str, limit: int = -1
         raise ValueError("%s: windows of shape %s, the checkpoint's params expect [%d, %d]" %
                          (path, rows.shape[1:], model.total_rows, model.max_length))
       t1 = time.time()
-      per = evaluate_rows(model, rows, labels, chunk)
+      if teacher is None:
+        per = evaluate_rows(model, rows, labels, chunk)
+      else:
+        per = evaluate_rows_distill(model, teacher, rows, labels, chunk, float(distill["temperature"]),
+                                    distill["logit_loss_identifier"])
       agg = aggregate(per["loss"], per["exact"], per["pred_counts"], per["ccs_counts"], bs)
       agg.update(precision=precision, forward_ms=per["forward_ms"], eval_ms=per["eval_ms"],
                  seconds_read=t1 - t0, seconds_model_and_eval=time.time() - t1)
+      if teacher is not None:
+        dist = aggregate_distillation(per["loss"], per["distill_loss"], per["exact"], per["pred_counts"],
+                                      per["ccs_counts"], bs, float(distill["student_alpha"]),
+                                      float(distill["distill_alpha"]))
+        dist.update(temperature=float(distill["temperature"]), logit_loss=distill["logit_loss_identifier"],
+                    student_forward_ms=per["forward_ms"], teacher_forward_ms=per["teacher_forward_ms"],
+                    eval_ms=per["eval_ms"], distill_ms=per["distill_ms"])
+        agg["distillation"] = dist
       csv_rows.append((path, agg["loss"], agg["per_example_accuracy"]))
       metrics[path] = agg
   finally:
     model.close()
+    if teacher is not None:
+      teacher.close()
   write_inference_csv(os.path.join(out_dir, "inference.csv"), csv_rows)
   with open(os.path.join(out_dir, "eval_metrics.json"), "w") as f:
     json.dump(metrics, f, indent=1)
@@ -177,6 +348,9 @@ def main(argv: Optional[List[str]] = None) -> None:
   ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
   ap.add_argument("--random_weights", type=int, default=None)
   ap.add_argument("--device", type=int, default=0)
+  ap.add_argument("--teacher_model_dir", default=None,
+                  help="checkpoint of the teacher of a distilled student: adds the distillation losses")
+  ap.add_argument("--teacher_random_weights", type=int, default=None)
   a = ap.parse_args(argv)
   m = run(**vars(a))
   print(json.dumps({p: {k: v for k, v in r.items() if not k.startswith("batch_identity")} for p, r in m.items()}))

@@ -139,9 +139,14 @@ def get_config(config_name: Optional[str] = None) -> Params:
   elif model_cfg == "transformer_learn_values":
     _set_learn_values(p)
   elif model_cfg == "transformer_learn_values_distill":
-    _set_learn_values(p)             # model_configs.py:150-177
+    _set_learn_values(p)             # model_configs.py:150-190
     p.model_name = "transformer_learn_values_distill"
     p.num_hidden_layers, p.filter_size = 5, 2048
+    p.layer_postprocess_dropout, p.attention_dropout, p.relu_dropout = 0.0, 0.1, 0.0
+    p.init_encoder_stack = p.init_nonencoder_layers = True
+    p.teacher_encoder_layers, p.student_encoder_layers = [1, 2, 3, 4, 5], [0, 1, 2, 3, 4]
+    p.distill_alpha, p.student_alpha, p.temperature = 1.0e5, 1.0, 1.0
+    p.logit_loss_identifier = "mean_squared_error"
   else:
     raise ValueError("Unknown model_config_name: %s" % model_cfg)
   if data_cfg in ("test", "custom"):

@@ -237,6 +237,28 @@ int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const
                  int32_t L, double del_cost, double loss_reg, int32_t band_width, uint32_t flags, float* loss_out,
                  uint8_t* exact_out, int32_t* pred_counts, int32_t* ccs_counts, float* ms_out);
 
+/* The distillation term of a distilled student's loss: DistillationLoss.call (losses_and_metrics.py:1170-1213), which
+ * the distillation loop's eval step adds to the student's AlignmentLoss (model_distillation.py:242-270,320-349:
+ * per example student_alpha * AlignmentLoss + distill_alpha * DistillationLoss).  For a batch of B windows of length
+ * L <= 256, teacher_logits / student_logits float32 [B, L, 5]:
+ *   t = softmax(teacher / T), s = softmax(student / T) over the 5 classes (tf.nn.softmax: divide by T, subtract the
+ *   max, exp, sum, divide), then per position the Keras logit loss with the teacher as y_true --
+ *     DCB_LOGIT_LOSS_MSE  mean_squared_error: mean_c (s_c - t_c)^2 (the transformer_learn_values_distill default,
+ *                         model_configs.py:150-190)
+ *     DCB_LOGIT_LOSS_KL   kl_divergence: both clipped to [1e-7, 1], sum_c t_c * log(t_c / s_c) (DistillationLoss's
+ *                         own default)
+ *   and loss_out[b] = the mean over all L positions, padding included.  float32 throughout.
+ * Both logits arrays are host arrays, or with DCB_ROWS_ON_DEVICE device arrays (e.g. the DCB_OUT_ON_DEVICE logits_out of
+ * two engines on the same device, a teacher and a student, once both forwards have been waited for).  loss_out is a
+ * host array; ms_out (nullable) receives the kernel's device time.  DCB_ERR_INVALID for batch < 0, L outside 1..256, a
+ * temperature that is not finite and > 0 (in float32), an unknown logit-loss id, or a null pointer with batch > 0;
+ * batch == 0 does nothing.  Deterministic: repeated calls, and host vs device inputs, give identical bits. */
+#define DCB_LOGIT_LOSS_MSE 0
+#define DCB_LOGIT_LOSS_KL 1
+int dcb_distill_loss(dcb_engine* e, const float* teacher_logits, const float* student_logits, int32_t batch,
+                     int32_t L, double temperature, int32_t logit_loss, uint32_t flags, float* loss_out,
+                     float* ms_out);
+
 /* ---- feature construction from BAM (host C++, htslib-free, needs no GPU) -----------------------------------------------
  * What `deepconsensus run` does in front of the model: stream the subreads-to-CCS BAM ZMW by ZMW (SubreadGrouper,
  * pre_lib.py:50-91), expand / clip / indent every subread (expand_clip_indent with trim_insertions, :1061-1239), fetch

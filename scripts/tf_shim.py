@@ -306,6 +306,7 @@ def install():
   cd_mod.ConfigDict = cd_mod.FrozenConfigDict = ConfigDict
   cd_pkg.config_dict = cd_mod
   cd_pkg.ConfigDict = cd_pkg.FrozenConfigDict = ConfigDict
+  cd_pkg.placeholder = lambda field_type, required=False: None    # model_configs.get_config's unset fields
   mlc.config_dict = cd_pkg
   sys.modules.update({"ml_collections": mlc, "ml_collections.config_dict": cd_pkg,
                       "ml_collections.config_dict.config_dict": cd_mod})
@@ -326,8 +327,8 @@ def install():
 
 
 # --------------------------------------------------------------------------- ops of models/losses_and_metrics.py
-# Used only by scripts/make_loss_golden.py.  Reductions over small float axes are summed in order, left to right, as
-# Eigen's inner-dimension reducer does below its packet size; reduce_logsumexp follows tf.math.reduce_logsumexp
+# Used only by scripts/make_loss_golden.py and scripts/make_distill_golden.py.  Reductions over small float axes are
+# summed in order, left to right, as Eigen's inner-dimension reducer does below its packet size; reduce_logsumexp follows tf.math.reduce_logsumexp
 # (max subtracted, replaced by 0 where it is not finite).
 def _np_dtype(dtype):
   if dtype is None:
@@ -425,6 +426,52 @@ def _xlogy(x, y):
   x, y = np.asarray(x), np.asarray(y)
   with np.errstate(divide="ignore", invalid="ignore"):
     return _t(np.where(x == 0, np.zeros_like(x * y), x * np.log(y)).astype(np.result_type(x, y)))
+
+
+def _softmax_folded(x, axis=-1, name=None):
+  """tf.nn.softmax: subtract the max, exp, sum (in order), divide."""
+  x = np.asarray(x)
+  e = np.exp(x - x.max(axis, keepdims=True))
+  return _t((e / np.expand_dims(_fold_sum(e, axis % x.ndim), axis)).astype(x.dtype))
+
+
+def _reduce_mean(x, axis=None):
+  """tf.math.reduce_mean: the in-order sum divided by the element count, in the input's dtype."""
+  x = np.asarray(x)
+  n = x.size if axis is None else x.shape[axis]
+  return _t((np.asarray(_reduce_sum(x, axis)) / x.dtype.type(n)).astype(x.dtype))
+
+
+# The two Keras logit losses DistillationLoss is used with (Keras is not part of the reference tree; restated from the
+# documented semantics of keras/losses.py, Keras 2.x): y_true is the first argument.
+def _mean_squared_error(y_true, y_pred):
+  y_true, y_pred = np.asarray(y_true), np.asarray(y_pred)
+  return _reduce_mean(np.square(y_pred - y_true), axis=-1)
+
+
+_KERAS_EPSILON = 1e-7          # keras.backend.epsilon()
+
+
+def _kl_divergence(y_true, y_pred):
+  y_true, y_pred = np.asarray(y_true), np.asarray(y_pred)
+  dt = y_true.dtype.type
+  y_true = np.clip(y_true, dt(_KERAS_EPSILON), dt(1))
+  y_pred = np.clip(y_pred, dt(_KERAS_EPSILON), dt(1))
+  return _reduce_sum(y_true * np.log(y_true / y_pred), axis=-1)
+
+
+_KERAS_LOSSES = {"mean_squared_error": _mean_squared_error, "mse": _mean_squared_error, "MSE": _mean_squared_error,
+                 "kl_divergence": _kl_divergence, "kullback_leibler_divergence": _kl_divergence,
+                 "kld": _kl_divergence, "KLD": _kl_divergence}
+
+
+def _keras_losses_get(identifier):
+  """tf.keras.losses.get for the identifiers above (callables pass through)."""
+  if callable(identifier):
+    return identifier
+  if identifier not in _KERAS_LOSSES:
+    raise ValueError("Unknown loss function: %r" % (identifier,))
+  return _KERAS_LOSSES[identifier]
 
 
 class _TensorArray:
@@ -538,8 +585,10 @@ def install_losses_ops(tf):
   tf.math = _NS(log=lambda x: _t(np.log(np.asarray(x))), xlogy=_xlogy,
                 count_nonzero=lambda x, axis=None: _t(np.count_nonzero(np.asarray(x), axis=axis)),
                 divide_no_nan=lambda a, b: _t(np.float32(0) if float(np.asarray(b)) == 0 else
-                                              np.float32(np.asarray(a) / np.asarray(b))))
-  tf.keras.losses = _NS(Loss=_Loss, Reduction=_NS(AUTO="auto", NONE="none", SUM="sum"))
+                                              np.float32(np.asarray(a) / np.asarray(b))),
+                reduce_mean=_reduce_mean)
+  tf.nn.softmax = _softmax_folded
+  tf.keras.losses = _NS(Loss=_Loss, Reduction=_NS(AUTO="auto", NONE="none", SUM="sum"), get=_keras_losses_get)
   tf.keras.metrics = _NS(Metric=_Metric, Mean=_Mean, Accuracy=_Accuracy)
   tf.metrics = tf.keras.metrics
   sys.modules["tensorflow.compat.v2"].__dict__.update(tf.__dict__)
