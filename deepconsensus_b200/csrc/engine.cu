@@ -105,6 +105,7 @@ struct dcb_engine {
       sc_ds_in, sc_ds_out;                // dcb_distill_loss: host teacher | student logits, loss
   cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;
   float* d_dbg = nullptr;  // [stages][chunk_tiles * x_image]
+  __nv_bfloat16* d_dbg_op = nullptr;   // bf16 operand images per stage (dbg_operand_slot)
   // strict-fp32 path (strict_kernels.cu): float32 copies of every variable in the reference's own shapes, and a
   // row-major workspace allocated on the first strict call
   struct StrictLayer {
@@ -671,6 +672,35 @@ static int strict_forward_chunk(dcb_engine* e, const float* rows_chunk, int bw, 
   return launches;
 }
 
+// Where the debug capture keeps bf16 operand image `which` (DCB_DEBUG_*) of stage `stage`: element offset into d_dbg_op
+// per tile row of 128 tokens and the image width.  Per stage the images are stored back to back, each chunk_tiles
+// tiles long.  Returns false for a pair that is not captured.
+//   stage 0     : EMBED (Epad), XB (layer 0's q/k/v operand)
+//   stage 1 + 2n: QKV (864), ATT (288), XB (the FFN's operand)
+//   stage 2 + 2n: HID (ff), XB (layer n + 1's q/k/v operand; not after the last layer)
+static bool dbg_operand_slot(const dcb_engine* e, int stage, int which, size_t* off_cols, int* width) {
+  const int layers = e->cfg.num_hidden_layers, ff = e->cfg.filter_size;
+  if (stage < 0 || stage > 2 * layers) return false;
+  size_t cols = 0;
+  for (int s = 0; s < stage; ++s) cols += s == 0 ? e->Epad + kDP : (s & 1) ? kQKVN + 2 * kDP : ff + kDP;
+  int w = -1;
+  if (stage == 0) {
+    if (which == DCB_DEBUG_EMBED) w = e->Epad;
+    else if (which == DCB_DEBUG_XB) { cols += e->Epad; w = kDP; }
+  } else if (stage & 1) {
+    if (which == DCB_DEBUG_QKV) w = kQKVN;
+    else if (which == DCB_DEBUG_ATT) { cols += kQKVN; w = kDP; }
+    else if (which == DCB_DEBUG_XB) { cols += kQKVN + kDP; w = kDP; }
+  } else {
+    if (which == DCB_DEBUG_HID) w = ff;
+    else if (which == DCB_DEBUG_XB && stage < 2 * layers) { cols += ff; w = kDP; }
+  }
+  if (w < 0) return false;
+  *off_cols = cols;
+  *width = w;
+  return true;
+}
+
 int dcb_set_debug(dcb_engine* e, int32_t enabled) {
   if (!e) return DCB_ERR_INVALID;
   e->debug = enabled != 0;
@@ -678,6 +708,11 @@ int dcb_set_debug(dcb_engine* e, int32_t enabled) {
     CU(e, cudaSetDevice(e->cfg.device));
     const size_t stages = 1 + 2 * (size_t)e->cfg.num_hidden_layers;
     int rc = dev_alloc(e, &e->d_dbg, stages * e->chunk_tiles * x_image_elems());
+    if (rc) return rc;
+    size_t cols = 0;
+    int w = 0;
+    dbg_operand_slot(e, (int)stages - 1, DCB_DEBUG_HID, &cols, &w);   // the last stage holds HID only
+    rc = dev_alloc(e, &e->d_dbg_op, (cols + w) * e->chunk_tiles * kTileM);
     if (rc) return rc;
   }
   return DCB_OK;
@@ -790,7 +825,18 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
     const float* rows_chunk = rows_base + (size_t)w0 * R * L;
     int stage = 0;
     auto snap = [&]() {
-      if (e->debug) cudaMemcpyAsync(e->d_dbg + (size_t)stage * e->chunk_tiles * ximg, e->d_x, (size_t)T * ximg * sizeof(float), cudaMemcpyDeviceToDevice, st);
+      if (e->debug) {
+        cudaMemcpyAsync(e->d_dbg + (size_t)stage * e->chunk_tiles * ximg, e->d_x, (size_t)T * ximg * sizeof(float), cudaMemcpyDeviceToDevice, st);
+        // the bf16 operand images the launches since the previous snapshot wrote (stream-ordered copies only)
+        const __nv_bfloat16* src[5] = {e->d_embqkv, e->d_xb, e->d_embqkv, e->d_att, e->d_hid};   // DCB_DEBUG_* order
+        for (int which = 0; which < 5; ++which) {
+          size_t cols = 0;
+          int w = 0;
+          if (dbg_operand_slot(e, stage, which, &cols, &w))
+            cudaMemcpyAsync(e->d_dbg_op + cols * e->chunk_tiles * kTileM, src[which], (size_t)T * kTileM * w * sizeof(__nv_bfloat16),
+                            cudaMemcpyDeviceToDevice, st);
+        }
+      }
       ++stage;
     };
     auto make_head = [&]() {
@@ -1034,6 +1080,30 @@ int dcb_debug_residual(dcb_engine* e, int32_t stage, float* out, int64_t out_ele
     const int tile = tl / kTileM, r = tl % kTileM;
     for (int col = 0; col < kD; ++col)
       out[(size_t)t * kD + col] = img[(((size_t)tile * kXChunks + col / 4) * kTileM + r) * 4 + col % 4];
+  }
+  return DCB_OK;
+}
+
+int dcb_debug_operand(dcb_engine* e, int32_t stage, int32_t which, uint16_t* out, int64_t out_elems) {
+  if (!e || !out) return DCB_ERR_INVALID;
+  if (!e->debug || !e->d_dbg_op) return fail(e, DCB_ERR_STATE, "debug capture not enabled");
+  size_t cols = 0;
+  int w = 0;
+  if (!dbg_operand_slot(e, stage, which, &cols, &w))
+    return fail(e, DCB_ERR_INVALID, "operand %d is not captured at stage %d", which, stage);
+  const int Mlay = e->last_chunk_tokens;               // tokens in the layout
+  const int M = Mlay / e->Lw * e->L;                   // valid tokens
+  if (out_elems < (int64_t)M * w) return fail(e, DCB_ERR_INVALID, "output too small: need %lld", (long long)M * w);
+  CU(e, cudaSetDevice(e->cfg.device));
+  const int T = (Mlay + kTileM - 1) / kTileM;
+  std::vector<uint16_t> img((size_t)T * kTileM * w);
+  CU(e, cudaMemcpy(img.data(), e->d_dbg_op + cols * e->chunk_tiles * kTileM, img.size() * sizeof(uint16_t), cudaMemcpyDeviceToHost));
+  const int chunks = w / 8;
+  for (int t = 0; t < M; ++t) {
+    const int tl = t / e->L * e->Lw + t % e->L;        // position of valid token t in the layout
+    const int tile = tl / kTileM, r = tl % kTileM;
+    for (int col = 0; col < w; ++col)
+      out[(size_t)t * w + col] = img[(((size_t)tile * chunks + col / 8) * kTileM + r) * 8 + col % 8];
   }
   return DCB_OK;
 }

@@ -93,7 +93,9 @@ ABI_SYMBOLS = (
     "dcb_synchronize", "dcb_last_error", "dcb_version", "dcb_destroy",
 )
 # include/dcb200_debug.h: developer / test hooks, not part of the drop-in boundary
-DEBUG_SYMBOLS = ("dcb_set_debug", "dcb_debug_residual")
+DEBUG_SYMBOLS = ("dcb_set_debug", "dcb_debug_residual", "dcb_debug_operand")
+# dcb_debug_operand's image ids (DCB_DEBUG_*)
+DEBUG_OPERANDS = {"embed": 0, "xb": 1, "qkv": 2, "att": 3, "hid": 4}
 
 
 def library_path() -> str:
@@ -153,6 +155,7 @@ def _load(path: str) -> ctypes.CDLL:
                                   ctypes.POINTER(ctypes.c_int64)]
   lib.dcb_get_profile_kernels.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(i32)]
   lib.dcb_debug_residual.argtypes = [vp, i32, vp, ctypes.c_int64]
+  lib.dcb_debug_operand.argtypes = [vp, i32, i32, vp, ctypes.c_int64]
   lib.dcb_alloc_host.argtypes = [ctypes.c_size_t, ctypes.POINTER(vp)]
   lib.dcb_free_host.argtypes = [vp]
   lib.dcb_alloc_device.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(vp)]
@@ -736,6 +739,16 @@ class B200Model:
     out = np.empty((tokens, 280), np.float32)
     self._check(self._lib.dcb_debug_residual(self._handle, stage, out.ctypes.data_as(ctypes.c_void_p),
                                              out.size))
+    return out
+
+  def debug_operand(self, stage: int, which: str, tokens: int) -> np.ndarray:
+    """dcb_debug_operand: bf16 operand image `which` (a DEBUG_OPERANDS key) captured at `stage`, as raw bf16 bits
+    uint16 [tokens, width] at the image's padded width."""
+    width = {"embed": (params_lib.embedded_width(self.params) + 15) // 16 * 16, "xb": 288, "qkv": 864, "att": 288,
+             "hid": int(self.params.filter_size)}[which]
+    out = np.empty((tokens, width), np.uint16)
+    self._check(self._lib.dcb_debug_operand(self._handle, stage, DEBUG_OPERANDS[which],
+                                            out.ctypes.data_as(ctypes.c_void_p), out.size))
     return out
 
   # -- raw device / pinned buffers (bench, multi-GPU driver) ----------------------------------

@@ -15,6 +15,21 @@ extern "C" {
 int dcb_set_debug(dcb_engine* e, int32_t enabled);
 int dcb_debug_residual(dcb_engine* e, int32_t stage, float* out, int64_t out_elems);
 
+/* Debug/test hook: copy bf16 operand image `which` as captured at stage `stage` (numbered as for
+ * dcb_debug_residual) of the LAST chunk of the last forward into out [tokens, width] as raw bf16 bits,
+ * token-major, at the image's full padded width (padding columns included):
+ *   DCB_DEBUG_EMBED  stage 0       the concatenated embeddings (width = E rounded up to 16)
+ *   DCB_DEBUG_XB     stage 0       layer 0's q/k/v operand (288)
+ *                    stage 1+2n    layer n's FFN operand (288)
+ *                    stage 2+2n    layer n+1's q/k/v operand (288; not after the last layer)
+ *   DCB_DEBUG_QKV    stage 1+2n    q/k/v of layer n (864: q_h0 q_h1 k_h0 k_h1 v_h0 v_h1, 144 each)
+ *   DCB_DEBUG_ATT    stage 1+2n    attention output of layer n (288: two heads of 144)
+ *   DCB_DEBUG_HID    stage 2+2n    ReLU hidden activation of layer n (filter_size)
+ * Capture is a stream-ordered device copy at the same points as the residual's.  Requires
+ * dcb_set_debug(e, 1). */
+enum { DCB_DEBUG_EMBED = 0, DCB_DEBUG_XB = 1, DCB_DEBUG_QKV = 2, DCB_DEBUG_ATT = 3, DCB_DEBUG_HID = 4 };
+int dcb_debug_operand(dcb_engine* e, int32_t stage, int32_t which, uint16_t* out, int64_t out_elems);
+
 #ifdef __cplusplus
 }
 #endif

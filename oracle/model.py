@@ -177,6 +177,8 @@ def attention(y: torch.Tensor, pre: str, params: params_lib.Params, w: weights_l
     v = _mm(y2, wv, emulate, split_b=True)
     if emulate == "bf16":
       q, k, v = _bf16(q), _bf16(k), _bf16(v)   # stored as bf16 between kernels
+      if collect is not None:
+        collect.setdefault("qkv", []).append(torch.stack([q, k, v]).reshape(3, B, L, d).numpy())
   else:
     q = (y2 @ wq) * scale
     k = y2 @ wk
@@ -193,6 +195,8 @@ def attention(y: torch.Tensor, pre: str, params: params_lib.Params, w: weights_l
     collect.setdefault("attention_scores", []).append(weights.numpy())
   o = weights @ v                                  # [B, N, F, H]
   o = o.permute(0, 2, 1, 3).reshape(B * L, d)
+  if emulate == "bf16" and collect is not None:
+    collect.setdefault("att", []).append(_bf16(o).reshape(B, L, d).numpy())
   if emulate:
     out = _mm(o, wo * gain, emulate, split_b=True)
   else:
@@ -200,7 +204,8 @@ def attention(y: torch.Tensor, pre: str, params: params_lib.Params, w: weights_l
   return out.reshape(B, L, d)
 
 
-def ffn(y: torch.Tensor, pre: str, w: weights_lib.Weights, emulate: Optional[str], gain: float) -> torch.Tensor:
+def ffn(y: torch.Tensor, pre: str, w: weights_lib.Weights, emulate: Optional[str], gain: float,
+        collect: Optional[dict] = None) -> torch.Tensor:
   """`FeedForwardNetwork.call`: relu(y W1 + b1) W2 + b2 (ffn_layer.py:83-86)."""
   B, L, d = y.shape
   w1 = _t(w[pre + "/filter_dense_layer/kernel"])
@@ -210,6 +215,8 @@ def ffn(y: torch.Tensor, pre: str, w: weights_lib.Weights, emulate: Optional[str
   y2 = y.reshape(B * L, d)
   if emulate:
     h = torch.relu(_mm(y2, w1, emulate) + b1)
+    if emulate == "bf16" and collect is not None:
+      collect.setdefault("hid", []).append(_bf16(h).reshape(B, L, -1).numpy())
     out = _mm(h, w2 * gain, emulate) + b2 * gain
   else:
     h = torch.relu(y2 @ w1 + b1)
@@ -224,6 +231,10 @@ def forward(rows: np.ndarray, params: params_lib.Params, w: weights_lib.Weights,
 
   `format_rows` (host clip) + `EncoderOnlyTransformer.call` (networks.py:221-239):
   squeeze/transpose (:268-273), encode (:436-520, :286-345), softmax (:238).
+
+  return_intermediates: the residual after every stage ("embedded", "attn_n", "ffn_n"), the attention scores and,
+  with emulate="bf16", the operands the engine stores as bf16 ("emb", per sub-layer "xb", per layer "qkv" [3, B, L, d],
+  "att", "hid"), for the stage references of oracle/stages.py.
   """
   rows = np.asarray(rows, dtype=np.float32)
   if rows.ndim == 4:
@@ -237,6 +248,8 @@ def forward(rows: np.ndarray, params: params_lib.Params, w: weights_lib.Weights,
   with torch.no_grad():
     x = _t(rows).permute(0, 2, 1).contiguous()                      # [B, L, R]
     e = embed(x, params, w, emulate)                                # [B, L, E]
+    if inter is not None and emulate == "bf16":
+      inter["emb"] = e.numpy().copy()
     if params.condense_transformer_input:
       wc = _t(w["model/transformer_input_condenser/kernel"])
       h = _mm(e.reshape(B * L, -1), wc, emulate, split_b=True).reshape(B, L, d)
@@ -256,10 +269,12 @@ def forward(rows: np.ndarray, params: params_lib.Params, w: weights_lib.Weights,
           y = layer_norm(h, _t(w[spre + "/layer_norm/gamma"]), _t(w[spre + "/layer_norm/beta"]))
           alpha = 1.0
         gain = alpha if emulate else 1.0     # engine folds alpha into Wo / W2 / b2
+        if inter is not None and emulate == "bf16":
+          inter.setdefault("xb", []).append(_bf16(y).numpy())   # the sub-layer's bf16 GEMM operand
         if fn == "attn":
           out = attention(y, spre + "/layer", params, w, emulate, gain, inter)
         else:
-          out = ffn(y, spre + "/layer", w, emulate, gain)
+          out = ffn(y, spre + "/layer", w, emulate, gain, inter)
         if emulate:
           h = h + out
         else:
