@@ -102,7 +102,8 @@ struct dcb_engine {
   struct Scratch { void* p = nullptr; size_t cap = 0; } sc_pos, sc_names, sc_nameoff, sc_outcome, sc_avg, sc_recoff, sc_fastq,
       sc_bq, sc_mask, sc_ids, sc_dst, sc_tmpb, sc_tmpq,
       sc_ev_probs, sc_ev_in, sc_ev_out,   // dcb_evaluate: host probs, labels | ccs ids, loss | counts | flags
-      sc_ds_in, sc_ds_out;                // dcb_distill_loss: host teacher | student logits, loss
+      sc_ds_in, sc_ds_out,                // dcb_distill_loss: host teacher | student logits, loss
+      sc_he_in, sc_he_out;                // dcb_debug_head_epilogue: logits + zero bias | probs, bases, quals
   cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;
   float* d_dbg = nullptr;  // [stages][chunk_tiles * x_image]
   __nv_bfloat16* d_dbg_op = nullptr;   // bf16 operand images per stage (dbg_operand_slot)
@@ -134,6 +135,14 @@ int fail(dcb_engine* e, int code, const char* fmt, ...) {
   va_end(ap);
   if (e) e->err = buf; else g_create_error = buf;
   return code;
+}
+
+// the head epilogue's calibration and cap, from the configuration
+void set_head_quality(HeadParams& hp, const dcb_config& c) {
+  hp.calib_enabled = c.calibration_enabled;
+  hp.calib_thr = (float)c.calibration_threshold; hp.calib_w = (float)c.calibration_w; hp.calib_b = (float)c.calibration_b;
+  hp.calib_thr64 = c.calibration_threshold; hp.calib_w64 = c.calibration_w; hp.calib_b64 = c.calibration_b;
+  hp.max_q = (float)c.max_base_quality;
 }
 
 #define CU(e, call)                                                                     \
@@ -326,7 +335,8 @@ void dcb_destroy(dcb_engine* e) {
   if (e->d_st_len) cudaFree(e->d_st_len);
   for (dcb_engine::Scratch* sc : {&e->sc_pos, &e->sc_names, &e->sc_nameoff, &e->sc_outcome, &e->sc_avg, &e->sc_recoff,
                                   &e->sc_fastq, &e->sc_bq, &e->sc_mask, &e->sc_ids, &e->sc_dst, &e->sc_tmpb, &e->sc_tmpq,
-                                  &e->sc_ev_probs, &e->sc_ev_in, &e->sc_ev_out, &e->sc_ds_in, &e->sc_ds_out})
+                                  &e->sc_ev_probs, &e->sc_ev_in, &e->sc_ev_out, &e->sc_ds_in, &e->sc_ds_out,
+                                  &e->sc_he_in, &e->sc_he_out})
     if (sc->p) cudaFree(sc->p);
   if (e->ev_eval0) cudaEventDestroy(e->ev_eval0);
   if (e->ev_eval1) cudaEventDestroy(e->ev_eval1);
@@ -805,10 +815,7 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
     hp.quals = (out_dev ? quals_out : sl.d_quals) + t0;
     hp.probs = probs_out ? ((out_dev ? probs_out : sl.d_probs) + t0 * kVocab) : nullptr;
     hp.logits = logits_out ? ((out_dev ? logits_out : sl.d_logits) + t0 * kVocab) : nullptr;
-    hp.calib_enabled = c.calibration_enabled;
-    hp.calib_thr = (float)c.calibration_threshold; hp.calib_w = (float)c.calibration_w; hp.calib_b = (float)c.calibration_b;
-    hp.calib_thr64 = c.calibration_threshold; hp.calib_w64 = c.calibration_w; hp.calib_b64 = c.calibration_b;
-    hp.max_q = (float)c.max_base_quality;
+    set_head_quality(hp, c);
     return hp;
   };
   if (strict) {
@@ -1315,6 +1322,41 @@ int dcb_fill_skipped(dcb_engine* e, const uint8_t* ccs_ids, const int16_t* ccs_b
   }
   CU(e, cudaGetLastError());
   if (status & 1) return fail(e, DCB_ERR_INPUT_RANGE, "dcb_fill_skipped: CCS base id outside 0..4 (clamped)");
+  return DCB_OK;
+}
+
+int dcb_debug_head_epilogue(dcb_engine* e, const float* logits, int64_t n, uint8_t* bases, uint8_t* quals, float* probs) {
+  if (!e || !logits || !bases || !quals) return DCB_ERR_INVALID;
+  if (n < 0) return fail(e, DCB_ERR_INVALID, "dcb_debug_head_epilogue: negative token count");
+  if (n == 0) return DCB_OK;
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  const int64_t chunk = std::min<int64_t>(n, 1 << 20);
+  int rc;
+  // in: [8] zero fc1 bias, then the chunk's logits; out: probs, then bases and quals
+  if ((rc = ensure(e, e->sc_he_in, (8 + (size_t)chunk * kVocab) * sizeof(float))) ||
+      (rc = ensure(e, e->sc_he_out, (size_t)chunk * (kVocab * sizeof(float) + 2))))
+    return rc;
+  float* d_bias = static_cast<float*>(e->sc_he_in.p);
+  float* d_logits = d_bias + 8;
+  float* d_probs = static_cast<float*>(e->sc_he_out.p);
+  uint8_t* d_bases = reinterpret_cast<uint8_t*>(d_probs + (size_t)chunk * kVocab);
+  uint8_t* d_quals = d_bases + chunk;
+  CU(e, cudaMemsetAsync(d_bias, 0, 8 * sizeof(float), st));
+  HeadParams hp{};
+  hp.bfc = d_bias;
+  set_head_quality(hp, e->cfg);
+  hp.bases = d_bases; hp.quals = d_quals; hp.probs = probs ? d_probs : nullptr;
+  for (int64_t t0 = 0; t0 < n; t0 += chunk) {
+    const int m = (int)std::min<int64_t>(chunk, n - t0);
+    CU(e, cudaMemcpyAsync(d_logits, logits + t0 * kVocab, (size_t)m * kVocab * sizeof(float), cudaMemcpyHostToDevice, st));
+    launch_head_epilogue(d_logits, m, hp, st);
+    CU(e, cudaMemcpyAsync(bases + t0, d_bases, (size_t)m, cudaMemcpyDeviceToHost, st));
+    CU(e, cudaMemcpyAsync(quals + t0, d_quals, (size_t)m, cudaMemcpyDeviceToHost, st));
+    if (probs) CU(e, cudaMemcpyAsync(probs + t0 * kVocab, d_probs, (size_t)m * kVocab * sizeof(float), cudaMemcpyDeviceToHost, st));
+    CU(e, cudaStreamSynchronize(st));   // pageable host buffers: the next chunk reuses the scratch
+  }
+  CU(e, cudaGetLastError());
   return DCB_OK;
 }
 

@@ -3,6 +3,7 @@
 #include <math.h>
 
 #include "common.h"
+#include "quality.cuh"
 
 namespace dcb {
 
@@ -28,20 +29,8 @@ __device__ __forceinline__ void head_finish(const HeadParams& p, float (&lg)[kVo
   // float32 log10, correctly rounded (double log10 rounded once): NumPy's float32 log10 is the platform libm's / SVML's
   // (<= 1 ulp, not always correctly rounded), so "the same float32 value as the reference" is only defined up to
   // that ulp; the correctly rounded value is the one every such library approximates.  err == 0 -> +inf.
-  float qf = -10.f * (float)log10((double)err);
-  int qi;
-  if (p.calib_enabled && p.calib_thr != 0.f) {
-    // np.where branch of calibrate_quality_scores (calibration_lib.py:93-99): the comparison `quality_scores >
-    // threshold` is float32 array vs Python scalar -> evaluated in float32; the selected w / b arrays are float64, so
-    // the multiply-add promotes to float64
-    const double qd = (double)qf;
-    const bool above = qf > p.calib_thr;
-    const double qc = qd * (above ? p.calib_w64 : 1.0) + (above ? p.calib_b64 : 0.0);
-    qi = (int)rint(fmin(qc, (double)p.max_q));
-  } else {
-    if (p.calib_enabled) qf = qf * p.calib_w + p.calib_b;    // float32 path (threshold == 0)
-    qi = (int)rintf(fminf(qf, p.max_q));                     // np.round: half to even
-  }
+  const float qf = -10.f * (float)log10((double)err);
+  int qi = head_quality(p, qf);                              // calibration, cap, round (quality.cuh)
   qi = qi < 0 ? 0 : qi;
   const char vocab[kVocab] = {' ', 'A', 'T', 'C', 'G'};
   p.bases[oidx] = (uint8_t)vocab[arg];

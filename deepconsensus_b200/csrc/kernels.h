@@ -46,6 +46,8 @@ void launch_skip_mask(const int16_t* ccs_bq, int n_windows, int L, const double*
 void launch_fill_skipped(const uint8_t* ccs_ids, const int16_t* ccs_bq, const int32_t* dst, int k, int L, int calib_enabled,
                          double thr, double cw, double cb, int max_q, uint8_t* bases, uint8_t* quals, int* status,
                          cudaStream_t st);
+// head_finish on final logits [n][5] (device pointer) into p.bases / p.quals / p.probs (dcb_debug_head_epilogue)
+void launch_head_epilogue(const float* logits, int n, const HeadParams& p, cudaStream_t st);
 
 // ---- evaluation on labelled windows (eval_kernels.cu): alignment loss, exact-match flag, alignment counts [B][5] of
 // the prediction and of the CCS row.  hard_min != 0: loss_reg None.  All pointers are device pointers.

@@ -21,6 +21,7 @@
 #include <stdint.h>
 
 #include "../../include/dcb200.h"
+#include "head_finish.cuh"
 #include "kernels.h"
 
 namespace dcb {
@@ -153,22 +154,26 @@ fill_skipped_kernel(const uint8_t* __restrict__ ccs_ids, const int16_t* __restri
     const int j = (int)(i / L), l = (int)(i - (long long)j * L);
     int id = ccs_ids[i];
     if (id > 4) { atomicOr(status, 1); id = 4; }
-    const int qraw = ccs_bq[i];
-    int qi;
-    if (calib_enabled) {
-      // calibrate_quality_scores on an integer array: float64 throughout (calibration_lib.py:89-99)
-      double qd = (double)qraw;
-      if (thr == 0.0) qd = qd * cw + cb;
-      else { const bool above = qd > thr; qd = qd * (above ? cw : 1.0) + (above ? cb : 0.0); }
-      qd = fmin(qd, (double)max_q);                    // np.minimum
-      qi = (int)qd;                                     // astype(int32): truncation
-    } else {
-      qi = qraw < max_q ? qraw : max_q;
-    }
+    const int qi = ccs_quality(ccs_bq[i], calib_enabled, thr, cw, cb, max_q);   // quality.cuh
     const size_t o = (size_t)dst[j] * L + l;
     bases[o] = (uint8_t)vocab[id];
     quals[o] = (uint8_t)(qi + 33);                      // quality_scores_to_string (utils.py:60-62)
   }
+}
+
+// dcb_debug_head_epilogue: head_finish on caller-supplied final logits [n][5], one thread per token
+__global__ void __launch_bounds__(256)
+head_epilogue_kernel(const float* __restrict__ logits, int n, HeadParams p) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  float lg[kVocab];
+#pragma unroll
+  for (int j = 0; j < kVocab; ++j) lg[j] = logits[(size_t)t * kVocab + j];
+  head_finish(p, lg, (size_t)t);
+}
+
+void launch_head_epilogue(const float* logits, int n, const HeadParams& p, cudaStream_t st) {
+  if (n > 0) head_epilogue_kernel<<<(n + 255) / 256, 256, 0, st>>>(logits, n, p);
 }
 
 void launch_read_outcome(const uint8_t* qual, const int32_t* len, const int32_t* zmw_start, const int32_t* window_pos,

@@ -93,7 +93,7 @@ ABI_SYMBOLS = (
     "dcb_synchronize", "dcb_last_error", "dcb_version", "dcb_destroy",
 )
 # include/dcb200_debug.h: developer / test hooks, not part of the drop-in boundary
-DEBUG_SYMBOLS = ("dcb_set_debug", "dcb_debug_residual", "dcb_debug_operand")
+DEBUG_SYMBOLS = ("dcb_set_debug", "dcb_debug_residual", "dcb_debug_operand", "dcb_debug_head_epilogue")
 # dcb_debug_operand's image ids (DCB_DEBUG_*)
 DEBUG_OPERANDS = {"embed": 0, "xb": 1, "qkv": 2, "att": 3, "hid": 4}
 
@@ -156,6 +156,7 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_get_profile_kernels.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(i32)]
   lib.dcb_debug_residual.argtypes = [vp, i32, vp, ctypes.c_int64]
   lib.dcb_debug_operand.argtypes = [vp, i32, i32, vp, ctypes.c_int64]
+  lib.dcb_debug_head_epilogue.argtypes = [vp, vp, ctypes.c_int64, vp, vp, vp]
   lib.dcb_alloc_host.argtypes = [ctypes.c_size_t, ctypes.POINTER(vp)]
   lib.dcb_free_host.argtypes = [vp]
   lib.dcb_alloc_device.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(vp)]
@@ -750,6 +751,19 @@ class B200Model:
     self._check(self._lib.dcb_debug_operand(self._handle, stage, DEBUG_OPERANDS[which],
                                             out.ctypes.data_as(ctypes.c_void_p), out.size))
     return out
+
+  def debug_head_epilogue(self, logits: np.ndarray) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """dcb_debug_head_epilogue: the head's per-token epilogue (softmax .. ASCII, with this engine's calibration and
+    max_base_quality) on final logits float32 [n, 5], no fc1 bias added.  Returns (bases uint8 [n], quals uint8 [n],
+    probs float32 [n, 5])."""
+    lg = np.ascontiguousarray(logits, dtype=np.float32)
+    if lg.ndim != 2 or lg.shape[1] != 5:
+      raise ValueError("debug_head_epilogue: logits must be [n, 5]")
+    n = int(lg.shape[0])
+    bases, quals, probs = np.empty(n, np.uint8), np.empty(n, np.uint8), np.empty((n, 5), np.float32)
+    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    self._check(self._lib.dcb_debug_head_epilogue(self._handle, vp(lg), n, vp(bases), vp(quals), vp(probs)))
+    return bases, quals, probs
 
   # -- raw device / pinned buffers (bench, multi-GPU driver) ----------------------------------
   def alloc_device(self, nbytes: int) -> int:

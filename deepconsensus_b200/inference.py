@@ -208,6 +208,16 @@ def run_model_and_stitch(feature_dicts: List[Dict[str, Any]], model: engine_lib.
                                           options.min_length, outcome_counter)
 
 
+def skip_decisions(model: engine_lib.B200Model, ccs_bq: np.ndarray, skip_windows_above: float) -> np.ndarray:
+  """avg_phred(ccs_base_quality_scores) > skip_windows_above for every window of int16 [n, L] (quick_inference.py:
+  663-672), decided by dcb_skip_mask; windows within 1e-7 of the threshold are re-decided with the reference's NumPy
+  expression.  Returns bool [n]."""
+  mask, _ = model.skip_mask(ccs_bq, skip_windows_above)
+  for i in np.nonzero(mask == 2)[0]:
+    mask[i] = utils.avg_phred(ccs_bq[i].astype(np.int64)) > skip_windows_above
+  return mask.astype(bool)
+
+
 def inference_on_zmw_windows(feature_dicts_for_zmws: Iterable[Iterable[Dict[str, Any]]], model: engine_lib.B200Model,
                              model_params: params_lib.Params, options: InferenceOptions,
                              outcome_counter: stitch_utils.OutcomeCounter) -> List[Optional[str]]:
@@ -233,10 +243,7 @@ def inference_on_zmw_windows(feature_dicts_for_zmws: Iterable[Iterable[Dict[str,
   bq = np.stack([np.asarray(w["ccs_base_quality_scores"]) for w in windows]).astype(np.int16)
   skip = np.array([bool(w.get("overflow", False)) for w in windows])
   if options.skip_windows_above:
-    mask, _ = model.skip_mask(bq, options.skip_windows_above)
-    for i in np.nonzero(mask == 2)[0]:                       # within 1e-7 of the threshold: the reference's expression
-      mask[i] = utils.avg_phred(windows[i]["ccs_base_quality_scores"]) > options.skip_windows_above
-    skip |= mask.astype(bool)
+    skip |= skip_decisions(model, bq, options.skip_windows_above)
   order = sorted(range(n), key=lambda i: (names[i], positions[i]))          # quick_inference.py:721-728
   dest = np.empty(n, np.int32)
   dest[order] = np.arange(n, dtype=np.int32)
@@ -283,10 +290,7 @@ def inference_on_packed_zmws(zmws: List[Dict[str, Any]], model: engine_lib.B200M
   names_z = [z["name"] for z in zmws]
   n = len(pos)
   if options.skip_windows_above:
-    mask, _ = model.skip_mask(bq, options.skip_windows_above)
-    for i in np.nonzero(mask == 2)[0]:
-      mask[i] = utils.avg_phred(bq[i].astype(np.int64)) > options.skip_windows_above
-    skip |= mask.astype(bool)
+    skip |= skip_decisions(model, bq, options.skip_windows_above)
   # sort by (name, window_pos): ZMW order by name, windows inside a ZMW by position (quick_inference.py:721-728)
   zorder = sorted(range(len(zmws)), key=lambda k: names_z[k])
   starts = np.concatenate([[0], np.cumsum(counts)])

@@ -30,6 +30,14 @@ int dcb_debug_residual(dcb_engine* e, int32_t stage, float* out, int64_t out_ele
 enum { DCB_DEBUG_EMBED = 0, DCB_DEBUG_XB = 1, DCB_DEBUG_QKV = 2, DCB_DEBUG_ATT = 3, DCB_DEBUG_HID = 4 };
 int dcb_debug_operand(dcb_engine* e, int32_t stage, int32_t which, uint16_t* out, int64_t out_elems);
 
+/* Debug/test hook: the model head's per-token epilogue (softmax, argmax, Phred, calibration, cap, round, ASCII) on
+ * caller-supplied final logits, one token per row: logits [n, 5] float32 -> bases [n] (' ATCG'), quals [n]
+ * (Phred+33) and probs [n, 5] (nullable), all host arrays.  The logits are taken as they are: no fc1 bias is added
+ * (the epilogue runs with a zero bias).  Uses the engine's calibration and max_base_quality; needs no forward and no
+ * dcb_set_debug.  Any n >= 0 (processed in chunks through device scratch).  DCB_ERR_INVALID for a null pointer or
+ * n < 0. */
+int dcb_debug_head_epilogue(dcb_engine* e, const float* logits, int64_t n, uint8_t* bases, uint8_t* quals, float* probs);
+
 #ifdef __cplusplus
 }
 #endif

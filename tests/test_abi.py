@@ -64,6 +64,20 @@ def test_no_cpu_fallback_without_gpu():
     engine.B200Model(p, weights_lib.init_weights(p), max_batch=2)
 
 
+def test_destroy_frees_every_scratch_buffer():
+  """The grow-on-demand device scratch (dcb_engine::Scratch) has no destructor: dcb_destroy frees it from an explicit
+  list, which must name every buffer the engine declares."""
+  src = open(os.path.join(ROOT, "deepconsensus_b200", "csrc", "engine.cu")).read()
+  decl = src[src.index("struct Scratch {"):]
+  decl = decl[decl.index("}") + 1:]
+  decl = re.sub(r"//[^\n]*", "", decl[:decl.index(";")])
+  declared = set(re.findall(r"\b(sc_\w+)", decl))
+  destroy = src[src.index("void dcb_destroy("):]
+  loop = destroy[destroy.index("for (dcb_engine::Scratch* sc :"):]
+  freed = set(re.findall(r"&e->(sc_\w+)", loop[:loop.index("})")]))
+  assert len(declared) >= 20 and declared == freed, declared ^ freed
+
+
 def test_product_code_never_imports_oracle():
   pkg = os.path.join(ROOT, "deepconsensus_b200")
   for dirpath, _, files in os.walk(pkg):
