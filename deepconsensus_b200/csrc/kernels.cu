@@ -106,9 +106,13 @@ embed_rows_kernel(const float* __restrict__ rows, const uint8_t* __restrict__ pa
 // 64-127, accumulators in registers); one thread of warpgroup 2 streams operands into shared memory with bulk copies
 // (TMA) that complete on mbarriers.  setmaxnreg moves the producer warpgroup's registers to the consumers.
 //
-// kAres (the K = 288 projections with several n-groups: fused QKV, FFN up-projection): the A tile is loaded once and
-// stays resident while every n-group of that tile streams its B k-steps through the stage ring.  Otherwise (the row
-// epilogue GEMMs, one n-group covering all 288 columns, K up to 2048) A and B k-steps stream together.
+// kAres (the K = 288 projections with several n-groups: fused QKV, FFN up-projection): a work item is a pair of
+// consecutive tiles (2i, 2i + 1).  Both A tiles are loaded once and stay resident while every n-group streams its B
+// k-steps through the stage ring; warpgroup w owns tile 2i + w and issues two m64 wgmmas (tile rows 0-63, 64-127) per B
+// k-step, so every weight byte that crosses from L2 feeds 256 tokens.  An odd tile count leaves the last pair with one
+// tile: the other warpgroup then waits and arrives on every barrier like its partner but issues no wgmma and stores
+// nothing.  Otherwise (the row epilogue GEMMs, one n-group covering all 288 columns, K up to 2048) warpgroup w owns tile
+// rows [64 w, 64 w + 64) of one tile, and A and B k-steps stream together.
 //
 // Split-bf16 weights: the B image may hold K twice as [W_hi; W_lo] (b_ksteps = 2 * a_ksteps, W_lo = bf16(W - W_hi));
 // the A k-steps are then read twice, so the accumulator sums A W_hi + A W_lo and the weights carry ~16 mantissa bits.
@@ -126,7 +130,9 @@ struct GemmCfg {
   static constexpr int kBBytesPerK = 2 * kNI * 16;
   static constexpr int kStageBytes = kSK * ((kAres ? 0 : kABytesPerK) + kBBytesPerK);
   static constexpr int kStages = 4;
-  static constexpr int kAresBytes = kAres ? (kDP / 16) * kABytesPerK : 0;   // resident A: K = 288
+  static constexpr int kMH = kAres ? 2 : 1;                       // m64 row blocks per consumer warpgroup
+  static constexpr int kATileBytes = (kDP / 16) * kABytesPerK;    // kAres: one resident A tile, K = 288
+  static constexpr int kAresBytes = kAres ? 2 * kATileBytes : 0;  // kAres: the item's two tiles
   static constexpr int kThreads = 384;                            // 2 consumer warpgroups + 1 producer warpgroup
   static constexpr int kVecBytes = kAres ? 0 : 3 * kDP * 4;       // row epilogue: bias, LayerNorm gamma, beta (fp32)
   static constexpr int kSmemBytes = kAresBytes + kStages * kStageBytes + 256 + kVecBytes;
@@ -182,8 +188,8 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
   }
   __syncthreads();
 
-  // kAres: a work item is a tile (its n-groups run back to back on the resident A); otherwise a (tile, n-group) pair
-  const int nitems = kAres ? ntiles : ntiles * ngroups;
+  // kAres: a work item is a tile pair (its n-groups run back to back on the resident A); otherwise a (tile, n-group) pair
+  const int nitems = kAres ? (ntiles + 1) / 2 : ntiles * ngroups;
   const int gper = kAres ? ngroups : 1;
   const int kstages = ksteps / Cfg::kSK;   // ksteps % kSK == 0 (launchers): every stage holds exactly kSK k-steps, so
                                            // its wgmma run is straight-line code with no register moves in between
@@ -196,12 +202,13 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
     if (warp == 8 && lane == 0) {
       uint32_t slot = 0, phase = 0, it = 0;
       for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++it) {
-        const int tile = kAres ? item : item / ngroups;
+        const int tile = kAres ? 2 * item : item / ngroups;
         const uint8_t* a_src = reinterpret_cast<const uint8_t*>(a_img) + tile * a_tile_bytes;
-        if constexpr (kAres) {
+        if constexpr (kAres) {   // the pair's A images are contiguous: one copy of one or two tiles
+          const uint32_t a_bytes = (uint32_t)((tile + 1 < ntiles ? 2 : 1) * a_tile_bytes);
           mbar_wait(a_empty, (it & 1) ^ 1);
-          mbar_arrive_expect_tx(a_full, (uint32_t)a_tile_bytes);
-          bulk_g2s(a_res, a_src, (uint32_t)a_tile_bytes, a_full);
+          mbar_arrive_expect_tx(a_full, a_bytes);
+          bulk_g2s(a_res, a_src, a_bytes, a_full);
         }
         for (int gi = 0; gi < gper; ++gi) {
           const int grp = kAres ? gi : item % ngroups;
@@ -231,14 +238,28 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
 
   // --------------------------------------------------------------- consumers (2 warpgroups)
   setmaxnreg_inc<232>();
-  const int wg = warp >> 2;                                   // tile rows [64 wg, 64 wg + 64)
+  const int wg = warp >> 2;
   const int g = lane >> 2, q = lane & 3;
-  const int row0 = wg * 64 + (warp & 3) * 16 + g;             // this thread's accumulator rows: row0 and row0 + 8
-  float acc[NCH][BN / 2];
+  // this thread's accumulator rows in its tile: row0 + 64 mh and row0 + 64 mh + 8 for m64 block mh < kMH
+  const int row0 = (kAres ? 0 : wg * 64) + (warp & 3) * 16 + g;
+  float accm[Cfg::kMH][NCH][BN / 2];
   uint32_t slot = 0, phase = 0, it = 0;
   for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++it) {
-    const int tile = kAres ? item : item / ngroups;
-    if constexpr (kAres) mbar_wait(a_full, it & 1);
+    const int tile = kAres ? 2 * item + wg : item / ngroups;
+    if constexpr (kAres) {
+      mbar_wait(a_full, it & 1);
+      if (tile >= ntiles) {
+        // the pair has one tile: step through the same barrier phases as the partner warpgroup without MMAs or stores
+        // (waiting on `full` keeps these arrivals from running ahead into the slot's next phase)
+        for (int s = 0; s < gper * kstages; ++s) {
+          mbar_wait(&full[slot], phase);
+          mbar_arrive(&empty[slot]);
+          if (++slot == Cfg::kStages) { slot = 0; phase ^= 1; }
+        }
+        mbar_arrive(a_empty);
+        continue;
+      }
+    }
     for (int gi = 0; gi < gper; ++gi) {
       const int grp = kAres ? gi : item % ngroups;
       uint32_t prev = 0;
@@ -247,22 +268,30 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
         const uint32_t st = smem_u32(stage_base + slot * Cfg::kStageBytes);
         const uint32_t sb = kAres ? st : st + Cfg::kSK * Cfg::kABytesPerK;
 #pragma unroll
-        for (int j = 0; j < NCH; ++j) wgmma_fence_regs(acc[j]);
+        for (int mh = 0; mh < Cfg::kMH; ++mh)
+#pragma unroll
+          for (int j = 0; j < NCH; ++j) wgmma_fence_regs(accm[mh][j]);
         wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < Cfg::kSK; ++kk) {
-          const uint32_t sa = kAres ? smem_u32(a_res) + ((s * Cfg::kSK + kk) % a_ksteps) * Cfg::kABytesPerK
+          const uint32_t sa = kAres ? smem_u32(a_res) + wg * Cfg::kATileBytes +
+                                          ((s * Cfg::kSK + kk) % a_ksteps) * Cfg::kABytesPerK
                                     : st + kk * Cfg::kABytesPerK;
-          const uint64_t adesc = make_kc16_desc(sa + wg * 64 * 16, kTileM * 16, 128);
 #pragma unroll
-          for (int j = 0; j < NCH; ++j) {
-            const uint64_t bdesc = make_kc16_desc(sb + kk * Cfg::kBBytesPerK + j * BN * 16, Cfg::kNI * 16, 128);
-            wgmma_bn<BN>(acc[j], adesc, bdesc, (s | kk) != 0);
+          for (int mh = 0; mh < Cfg::kMH; ++mh) {
+            const uint64_t adesc = make_kc16_desc(sa + (kAres ? 64 * mh : 64 * wg) * 16, kTileM * 16, 128);
+#pragma unroll
+            for (int j = 0; j < NCH; ++j) {
+              const uint64_t bdesc = make_kc16_desc(sb + kk * Cfg::kBBytesPerK + j * BN * 16, Cfg::kNI * 16, 128);
+              wgmma_bn<BN>(accm[mh][j], adesc, bdesc, (s | kk) != 0);
+            }
           }
         }
         wgmma_commit();
 #pragma unroll
-        for (int j = 0; j < NCH; ++j) wgmma_fence_regs(acc[j]);
+        for (int mh = 0; mh < Cfg::kMH; ++mh)
+#pragma unroll
+          for (int j = 0; j < NCH; ++j) wgmma_fence_regs(accm[mh][j]);
         // the previous stage's MMAs are complete once at most this stage's group is in flight: hand it back
         wgmma_wait<1>();
         if (s > 0) mbar_arrive(&empty[prev]);
@@ -271,7 +300,9 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
       }
       wgmma_wait<0>();
 #pragma unroll
-      for (int j = 0; j < NCH; ++j) wgmma_fence_regs(acc[j]);
+      for (int mh = 0; mh < Cfg::kMH; ++mh)
+#pragma unroll
+        for (int j = 0; j < NCH; ++j) wgmma_fence_regs(accm[mh][j]);
       mbar_arrive(&empty[prev]);
       if (kAres && gi + 1 == gper) mbar_arrive(a_empty);   // the last group's MMAs have read A
 
@@ -279,23 +310,26 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
       if constexpr (EPI == EPI_QKV || EPI == EPI_RELU) {
         __nv_bfloat16* obase = out_img + (size_t)tile * kTileM * out_chunks * 8;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = row0 + 8 * h;
+        for (int mh = 0; mh < Cfg::kMH; ++mh)
 #pragma unroll
-          for (int j = 0; j < NCH; ++j)
+          for (int h = 0; h < 2; ++h) {
+            const int row = row0 + 64 * mh + 8 * h;
 #pragma unroll
-            for (int jj = 0; jj < BN / 8; ++jj) {
-              const int col = grp * Cfg::kNI + j * BN + jj * 8 + 2 * q;
-              float v0 = acc[j][jj * 4 + 2 * h], v1 = acc[j][jj * 4 + 2 * h + 1];
-              if constexpr (EPI == EPI_RELU) {
-                v0 = fmaxf(v0 + __ldg(out_bias + col), 0.f);
-                v1 = fmaxf(v1 + __ldg(out_bias + col + 1), 0.f);
+            for (int j = 0; j < NCH; ++j)
+#pragma unroll
+              for (int jj = 0; jj < BN / 8; ++jj) {
+                const int col = grp * Cfg::kNI + j * BN + jj * 8 + 2 * q;
+                float v0 = accm[mh][j][jj * 4 + 2 * h], v1 = accm[mh][j][jj * 4 + 2 * h + 1];
+                if constexpr (EPI == EPI_RELU) {
+                  v0 = fmaxf(v0 + __ldg(out_bias + col), 0.f);
+                  v1 = fmaxf(v1 + __ldg(out_bias + col + 1), 0.f);
+                }
+                *reinterpret_cast<uint32_t*>(obase + ((size_t)(col >> 3) * kTileM + row) * 8 + (col & 7)) =
+                    pack_bf16x2(v0, v1);
               }
-              *reinterpret_cast<uint32_t*>(obase + ((size_t)(col >> 3) * kTileM + row) * 8 + (col & 7)) =
-                  pack_bf16x2(v0, v1);
-            }
-        }
+          }
       } else {
+        float (&acc)[NCH][BN / 2] = accm[0];   // one m64 block per warpgroup
         // x is updated in place, so the compiler keeps each x_old load behind every store that precedes it in source
         // order.  Each pass (row half h, accumulator chunk j) therefore issues all of its global loads before its first
         // store: four batches of 18 loads per tile instead of a load -> store round trip per fragment.  The per-column
@@ -735,7 +769,8 @@ void launch_gemm_row(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int
 void launch_gemm_qkv(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int ntiles,
                      __nv_bfloat16* qkv_img, cudaStream_t st) {
   using Cfg = GemmCfg<kNC, 1, true>;
-  const int grid = ntiles < num_sms() ? ntiles : num_sms();
+  const int npairs = (ntiles + 1) / 2;
+  const int grid = npairs < num_sms() ? npairs : num_sms();
   RowEpi none{};
   gemm_kernel<kNC, 1, EPI_QKV, true><<<grid, Cfg::kThreads, Cfg::kSmemBytes, st>>>(
       a_img, b_img, kDP / 16, 2 * (kDP / 16), ntiles, kQKVN / kQKVGroup, qkv_img, kQKVN / 8, nullptr, none);
@@ -744,7 +779,8 @@ void launch_gemm_qkv(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int
 void launch_ffn_up(const __nv_bfloat16* a_img, const __nv_bfloat16* w1_img, const float* b1, int ff, int ntiles,
                    __nv_bfloat16* hid_img, cudaStream_t st) {
   using Cfg = GemmCfg<kFFChunk, 1, true>;
-  const int grid = ntiles < num_sms() ? ntiles : num_sms();
+  const int npairs = (ntiles + 1) / 2;
+  const int grid = npairs < num_sms() ? npairs : num_sms();
   RowEpi none{};
   gemm_kernel<kFFChunk, 1, EPI_RELU, true><<<grid, Cfg::kThreads, Cfg::kSmemBytes, st>>>(
       a_img, w1_img, kDP / 16, kDP / 16, ntiles, ff / kFFChunk, hid_img, ff / 8, b1, none);
