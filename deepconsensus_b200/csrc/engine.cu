@@ -103,6 +103,7 @@ struct dcb_engine {
       sc_bq, sc_mask, sc_ids, sc_dst, sc_tmpb, sc_tmpq,
       sc_ev_probs, sc_ev_in, sc_ev_out,   // dcb_evaluate: host probs, labels | ccs ids, loss | counts | flags
       sc_ds_in, sc_ds_out,                // dcb_distill_loss: host teacher | student logits, loss
+      sc_lg_in, sc_lg_out, sc_lg_dp,      // dcb_alignment_loss_grad: host probs | labels, loss | grad | matches, DP tables
       sc_he_in, sc_he_out;                // dcb_debug_head_epilogue: logits + zero bias | probs, bases, quals
   cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;
   float* d_dbg = nullptr;  // [stages][chunk_tiles * x_image]
@@ -336,7 +337,7 @@ void dcb_destroy(dcb_engine* e) {
   for (dcb_engine::Scratch* sc : {&e->sc_pos, &e->sc_names, &e->sc_nameoff, &e->sc_outcome, &e->sc_avg, &e->sc_recoff,
                                   &e->sc_fastq, &e->sc_bq, &e->sc_mask, &e->sc_ids, &e->sc_dst, &e->sc_tmpb, &e->sc_tmpq,
                                   &e->sc_ev_probs, &e->sc_ev_in, &e->sc_ev_out, &e->sc_ds_in, &e->sc_ds_out,
-                                  &e->sc_he_in, &e->sc_he_out})
+                                  &e->sc_lg_in, &e->sc_lg_out, &e->sc_lg_dp, &e->sc_he_in, &e->sc_he_out})
     if (sc->p) cudaFree(sc->p);
   if (e->ev_eval0) cudaEventDestroy(e->ev_eval0);
   if (e->ev_eval1) cudaEventDestroy(e->ev_eval1);
@@ -1453,6 +1454,76 @@ int dcb_distill_loss(dcb_engine* e, const float* teacher_logits, const float* st
   CU(e, launch_distill_loss(d_teacher, d_student, batch, L, t32, logit_loss, d_loss, st));
   CU(e, cudaEventRecord(e->ev_eval1, st));
   CU(e, cudaMemcpyAsync(loss_out, d_loss, (size_t)batch * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  return DCB_OK;
+}
+
+int dcb_alignment_loss_grad(dcb_engine* e, const float* probs, const uint8_t* labels, int32_t batch, int32_t L,
+                            double del_cost, double loss_reg, int32_t band_width, uint32_t flags, float* loss_out,
+                            float* grad_out, float* matches_out, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  if (band_width >= 0)
+    return fail(e, DCB_ERR_INVALID, "dcb_alignment_loss_grad: the banded alignment loss (band_width=%d) is not "
+                "supported; pass DCB_BAND_WIDTH_NONE", band_width);
+  if (batch < 0 || L <= 0 || L > 256)
+    return fail(e, DCB_ERR_INVALID, "dcb_alignment_loss_grad: need batch >= 0 and 0 < L <= 256 (batch=%d, L=%d)", batch, L);
+  if (!(del_cost == del_cost)) return fail(e, DCB_ERR_INVALID, "dcb_alignment_loss_grad: del_cost is NaN");
+  if (ms_out) *ms_out = 0.f;
+  if (batch == 0) return DCB_OK;
+  if (!probs || !labels || !loss_out) return fail(e, DCB_ERR_INVALID, "dcb_alignment_loss_grad: null pointer");
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  const bool in_dev = flags & DCB_ROWS_ON_DEVICE, out_dev = flags & DCB_OUT_ON_DEVICE;
+  const size_t ntok = (size_t)batch * L, np = ntok * kVocab * sizeof(float);
+  const uint8_t* hl = labels;
+  std::vector<uint8_t> lab_copy;
+  if (in_dev) {   // the label check reads them on the host
+    lab_copy.resize(ntok);
+    CU(e, cudaMemcpyAsync(lab_copy.data(), labels, ntok, cudaMemcpyDeviceToHost, st));
+    CU(e, cudaStreamSynchronize(st));
+    hl = lab_copy.data();
+  }
+  for (size_t i = 0; i < ntok; ++i)
+    if (hl[i] > 4)
+      return fail(e, DCB_ERR_INVALID, "dcb_alignment_loss_grad: label id %d outside 0..4 at window %zu", hl[i], i / L);
+  int ctas = 0;
+  CU(e, loss_grad_grid(batch, &ctas));
+  // host outputs go through scratch: loss [B] | grad [B, L, 5] | matches [B, L, L]
+  const size_t n_grad = grad_out ? ntok * kVocab : 0, n_match = matches_out ? ntok * L : 0;
+  int rc;
+  if ((rc = ensure(e, e->sc_lg_dp, loss_grad_table_bytes(L, ctas))) ||
+      (!in_dev && (rc = ensure(e, e->sc_lg_in, np + ntok))) ||
+      (!out_dev && (rc = ensure(e, e->sc_lg_out, ((size_t)batch + n_grad + n_match) * sizeof(float)))))
+    return rc;
+  if (!e->ev_eval0) CU(e, cudaEventCreate(&e->ev_eval0));
+  if (!e->ev_eval1) CU(e, cudaEventCreate(&e->ev_eval1));
+  const float* d_probs = probs;
+  const uint8_t* d_labels = labels;
+  if (!in_dev) {
+    float* d_in = static_cast<float*>(e->sc_lg_in.p);
+    CU(e, cudaMemcpyAsync(d_in, probs, np, cudaMemcpyHostToDevice, st));
+    CU(e, cudaMemcpyAsync(d_in + ntok * kVocab, labels, ntok, cudaMemcpyHostToDevice, st));
+    d_probs = d_in;
+    d_labels = reinterpret_cast<const uint8_t*>(d_in + ntok * kVocab);
+  }
+  float *d_loss = loss_out, *d_grad = grad_out, *d_match = matches_out;
+  if (!out_dev) {
+    d_loss = static_cast<float*>(e->sc_lg_out.p);
+    d_grad = grad_out ? d_loss + batch : nullptr;
+    d_match = matches_out ? d_loss + batch + n_grad : nullptr;
+  }
+  const bool hard = !(loss_reg > 0.0);
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  CU(e, launch_loss_grad(d_probs, d_labels, batch, L, (float)del_cost, hard ? 1.f : (float)loss_reg, hard ? 1 : 0,
+                         static_cast<float*>(e->sc_lg_dp.p), ctas, d_loss, d_grad, d_match, st));
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  if (!out_dev) {
+    CU(e, cudaMemcpyAsync(loss_out, d_loss, (size_t)batch * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (grad_out) CU(e, cudaMemcpyAsync(grad_out, d_grad, n_grad * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (matches_out) CU(e, cudaMemcpyAsync(matches_out, d_match, n_match * sizeof(float), cudaMemcpyDeviceToHost, st));
+  }
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));

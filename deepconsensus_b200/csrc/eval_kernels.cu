@@ -8,6 +8,10 @@
 //                           anti-diagonals through three rotating shared-memory rows.  Soft-min
 //                           -reg * logsumexp(-t / reg) with the max subtracted (tf.reduce_logsumexp), or the hard min.
 //                           float32 throughout, as the reference.
+//   align_loss_grad_kernel  the same loss (identical bits) plus its gradient: AlignmentLoss.eval(return_matches=True)
+//                           and d loss / d y_pred as TensorFlow's tape computes them.  Persistent grid, one window per
+//                           CTA at a time; the whole DP table in a per-CTA slice of device scratch, then a reverse
+//                           anti-diagonal sweep.
 //   align_identity_kernel   AlignmentMetric.alignment (:704-1043), one CTA per (window, sequence): blockIdx.y = 0 aligns
 //                           the argmax-decoded prediction, 1 the window's CCS row (get_batch_identity_ccs_pred,
 //                           :1061-1098).  Affine-gap Needleman-Wunsch (match +2, mismatch -5, gap open 9, extend 4) with
@@ -23,6 +27,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include <algorithm>
+
 #include "kernels.h"
 
 namespace dcb {
@@ -36,6 +42,9 @@ constexpr float kEps = 1e-7f;
 constexpr float kOneMinusEps = (float)(1.0 - 1e-7);   // Python's 1 - eps, then float32, as tf.clip_by_value sees it
 constexpr int kDistillWarps = 4;                       // windows (one warp each) per CTA of distill_loss_kernel
 constexpr int kLogitLossKL = 1;                        // DCB_LOGIT_LOSS_KL (include/dcb200.h); 0 is MSE
+// Resident CTAs per SM of align_loss_grad_kernel's persistent grid: each holds an (L + 1)^2 float table in device
+// scratch (41 KB at L = 100, 264 KB at L = 256), so 4 per SM keeps the L = 100 tables of the whole grid within L2.
+constexpr int kLossGradCtasPerSm = 4;
 
 // Left shift (left_shift_sequence): non-gap ids in order, then gaps.  One thread; L <= 256.  Returns the non-gap count.
 __device__ int left_shift_serial(const uint8_t* in, uint8_t* out, int L) {
@@ -64,6 +73,46 @@ __device__ __forceinline__ float softmin3(float a, float b, float c, float reg, 
   return __fmul_rn(-reg, __fadd_rn(logf(s), mx));
 }
 
+// The gradient of softmin3 with respect to its three arguments, as TensorFlow differentiates the two minops: for the
+// soft min the softmax of -t / reg with the (stop-gradient) max subtracted, for the hard min tf.reduce_min's
+// indicator / count, which splits equally among exactly tied minima.  An argument far above the others (1e9, "inf")
+// gets weight 0: its exp underflows, or it is not the minimum.
+__device__ __forceinline__ void softmin3_weights(float a, float b, float c, float reg, bool hard, float* w) {
+  if (hard) {
+    const float mn = fminf(fminf(a, b), c);
+    const float ia = a == mn ? 1.f : 0.f, ib = b == mn ? 1.f : 0.f, ic = c == mn ? 1.f : 0.f;
+    const float cnt = __fadd_rn(__fadd_rn(ia, ib), ic);
+    w[0] = __fdiv_rn(ia, cnt); w[1] = __fdiv_rn(ib, cnt); w[2] = __fdiv_rn(ic, cnt);
+    return;
+  }
+  const float x0 = -a / reg, x1 = -b / reg, x2 = -c / reg;
+  float mx = fmaxf(fmaxf(x0, x1), x2);
+  if (!isfinite(mx)) mx = 0.f;
+  const float e0 = expf(__fsub_rn(x0, mx)), e1 = expf(__fsub_rn(x1, mx)), e2 = expf(__fsub_rn(x2, mx));
+  const float s = __fadd_rn(__fadd_rn(e0, e1), e2);
+  w[0] = __fdiv_rn(e0, s); w[1] = __fdiv_rn(e1, s); w[2] = __fdiv_rn(e2, s);
+}
+
+// One interior cell of the alignment DP (i >= 1): the match, insertion and deletion candidates from the three
+// predecessor values and the position's -log costs, then the soft / hard min.  Shared by the loss and gradient kernels
+// so that both compute identical bits.
+__device__ __forceinline__ float align_cell(float v_diag, float v_left, float v_up, float lp_sub, float lp_ins,
+                                            float del_cost, float reg, bool hard) {
+  const float om = __fadd_rn(v_diag, lp_sub);
+  const float oi = __fadd_rn(v_left, lp_ins);
+  const float od = __fadd_rn(v_up, del_cost);
+  return softmin3(om, oi, od, reg, hard);
+}
+
+// -log(clip(p / sum p, 1e-7, 1 - 1e-7)) of one position (xentropy_subs_cost_fn / xentropy_ins_cost_fn).
+__device__ __forceinline__ void neg_log_probs(const float* p, float* lp) {
+  float q[kVocab];
+  for (int t = 0; t < kVocab; ++t) q[t] = p[t];
+  float tot = q[0];
+  for (int t = 1; t < kVocab; ++t) tot = __fadd_rn(tot, q[t]);
+  for (int t = 0; t < kVocab; ++t) lp[t] = -logf(fminf(fmaxf(q[t] / tot, kEps), kOneMinusEps));
+}
+
 }  // namespace
 
 __global__ void __launch_bounds__(kEvalThreads)
@@ -77,11 +126,7 @@ align_loss_kernel(const float* __restrict__ probs, const uint8_t* __restrict__ l
   const int m = L, n = L;
   const float* p = probs + (size_t)b * L * kVocab;
   for (int j = tid; j < L; j += blockDim.x) {
-    float q[kVocab];
-    for (int t = 0; t < kVocab; ++t) q[t] = p[j * kVocab + t];
-    float tot = q[0];
-    for (int t = 1; t < kVocab; ++t) tot = __fadd_rn(tot, q[t]);
-    for (int t = 0; t < kVocab; ++t) s_lp[j * kVocab + t] = -logf(fminf(fmaxf(q[t] / tot, kEps), kOneMinusEps));
+    neg_log_probs(p + j * kVocab, s_lp + j * kVocab);
     s_lab_in[j] = labels[(size_t)b * L + j];
   }
   __syncthreads();
@@ -106,16 +151,139 @@ align_loss_kernel(const float* __restrict__ probs, const uint8_t* __restrict__ l
         v = __fadd_rn(v1[0], k - 1 < n ? s_lp[(k - 1) * kVocab + 0] : 0.f);   // insertion along the first row
       } else {
         const bool jin = j - 1 >= 0 && j - 1 < n;                           // cost tables are 0 outside (wavefrontify)
-        const float om = __fadd_rn(v2[i - 1], jin ? s_lp[(j - 1) * kVocab + s_lab[i - 1]] : 0.f);
-        const float oi = __fadd_rn(v1[i], jin ? s_lp[(j - 1) * kVocab + 0] : 0.f);
-        const float od = __fadd_rn(v1[i - 1], del_cost);
-        v = softmin3(om, oi, od, reg, hard_min);
+        v = align_cell(v2[i - 1], v1[i], v1[i - 1], jin ? s_lp[(j - 1) * kVocab + s_lab[i - 1]] : 0.f,
+                       jin ? s_lp[(j - 1) * kVocab + 0] : 0.f, del_cost, reg, hard_min);
       }
       v0[i] = v;
     }
     __syncthreads();
   }
   if (tid == 0) loss_out[b] = k_end >= 2 ? s_v[k_end % 3][seq_len] : kInf;
+}
+
+// Offset of cell (i, k - i) in a window's (L + 1)^2 table stored by anti-diagonal: diagonal k holds rows
+// max(0, k - L) .. min(L, k), contiguously.
+__device__ __forceinline__ int diag_cell(int k, int i, int L) {
+  if (k <= L) return k * (k + 1) / 2 + i;
+  const int d = k - L - 1;
+  return (L + 1) * (L + 2) / 2 + d * (L + 1) - d * (d + 1) / 2 + (i - (k - L));
+}
+
+// AlignmentLoss.eval(return_matches=True) and the gradient of the loss with respect to y_pred, one CTA per window in a
+// persistent grid.  The forward is align_loss_kernel's, cell for cell (align_cell), over rows 0..seq_len (rows below
+// do not reach the result), but every value is kept: in `table`, this CTA's (L + 1)^2 floats of device scratch, laid
+// out by anti-diagonal.  The backward sweeps the anti-diagonals in reverse from (seq_len, L) with adjoint 1.  Each cell
+// pulls its adjoint E from the messages its successors left in shared memory, rebuilds its own three candidates and
+// their weights (softmin3_weights), and leaves E * weight for each predecessor.  E * w_match is matches[i-1][j-1];
+// E * w_match and E * w_ins accumulate into dL/dlp[j-1][label] and dL/dlp[j-1][0].  An anti-diagonal has one cell per
+// column, so these sums have one writer per step and a fixed order: no atomics, identical bits on every call.
+// Row 0 is the chain V[0][j] = V[0][j-1] + ins[j-1]; column 0 only carries deletions and reaches no cost.  Finally
+// dL/dq = -dL/dlp / q inside the clip range (0 outside; the bounds pass), and through q = p / sum p,
+// dL/dp_s = (dL/dq_s - sum_t dL/dq_t q_t) / sum p.
+__global__ void __launch_bounds__(kEvalThreads)
+align_loss_grad_kernel(const float* __restrict__ probs, const uint8_t* __restrict__ labels, int B, int L,
+                       float del_cost, float reg, int hard, float* __restrict__ tables, float* __restrict__ loss_out,
+                       float* __restrict__ grad_out, float* __restrict__ matches_out) {
+  __shared__ float s_lp[kEvalMaxL * kVocab];     // -log(clip(p / sum p))
+  __shared__ float s_g[kEvalMaxL * kVocab];      // dL / d s_lp
+  __shared__ float s_msg[3][3][kEvalMaxL + 1];   // [diagonal k mod 3][match, ins, del][row]: E * weight
+  __shared__ uint8_t s_lab_in[kEvalMaxL], s_lab[kEvalMaxL];
+  __shared__ int s_len;
+  const int tid = threadIdx.x, n = L;
+  const bool hard_min = hard != 0;
+  float* V = tables + (size_t)blockIdx.x * (L + 1) * (L + 1);
+  for (int b = blockIdx.x; b < B; b += gridDim.x) {
+    const float* p = probs + (size_t)b * L * kVocab;
+    for (int j = tid; j < L; j += blockDim.x) {
+      neg_log_probs(p + j * kVocab, s_lp + j * kVocab);
+      for (int t = 0; t < kVocab; ++t) s_g[j * kVocab + t] = 0.f;
+      s_lab_in[j] = labels[(size_t)b * L + j];
+    }
+    __syncthreads();
+    if (tid == 0) s_len = left_shift_serial(s_lab_in, s_lab, L);
+    __syncthreads();
+    const int seq_len = s_len, k_end = seq_len + n;
+    float* mt = matches_out ? matches_out + (size_t)b * L * L : nullptr;
+    if (mt)   // label rows at or beyond seq_len are never aligned
+      for (int x = seq_len * L + tid; x < L * L; x += blockDim.x) mt[x] = 0.f;
+    // forward: every cell of rows 0..seq_len
+    for (int k = 0; k <= k_end; ++k) {
+      const int ilo = max(0, k - n), ihi = min(seq_len, k);
+      for (int i = ilo + tid; i <= ihi; i += blockDim.x) {
+        const int j = k - i;
+        float v;
+        if (k == 0) {
+          v = 0.f;
+        } else if (i == 0) {
+          v = __fadd_rn(V[diag_cell(k - 1, 0, L)], s_lp[(j - 1) * kVocab + 0]);
+        } else if (k == 1) {
+          v = del_cost;                                    // (1, 0): the recursion's initial value
+        } else if (j == 0) {
+          v = align_cell(kInf, kInf, V[diag_cell(k - 1, i - 1, L)], 0.f, 0.f, del_cost, reg, hard_min);
+        } else {
+          v = align_cell(V[diag_cell(k - 2, i - 1, L)], V[diag_cell(k - 1, i, L)], V[diag_cell(k - 1, i - 1, L)],
+                         s_lp[(j - 1) * kVocab + s_lab[i - 1]], s_lp[(j - 1) * kVocab + 0], del_cost, reg, hard_min);
+        }
+        V[diag_cell(k, i, L)] = v;
+      }
+      __syncthreads();
+    }
+    if (tid == 0) loss_out[b] = k_end >= 2 ? V[diag_cell(k_end, seq_len, L)] : kInf;
+    // backward (the reference's recursion starts at k = 2: with k_end < 2 the loss is the constant inf)
+    for (int k = k_end; k >= 1 && k_end >= 2; --k) {
+      const int ilo = max(0, k - n), ihi = min(seq_len, k);
+      float(*out)[kEvalMaxL + 1] = s_msg[k % 3];
+      const float(*m1)[kEvalMaxL + 1] = s_msg[(k + 1) % 3];
+      const float(*m2)[kEvalMaxL + 1] = s_msg[(k + 2) % 3];
+      for (int i = ilo + tid; i <= ihi; i += blockDim.x) {
+        const int j = k - i;
+        float e;
+        if (k == k_end) {
+          e = 1.f;                                         // the diagonal holds (seq_len, L) only
+        } else {
+          e = 0.f;
+          if (i + 1 <= seq_len && j + 1 <= n) e = __fadd_rn(e, m2[0][i + 1]);   // (i+1, j+1) matched (i, j)
+          if (j + 1 <= n) e = __fadd_rn(e, m1[1][i]);                          // (i, j+1) inserted after it
+          if (i + 1 <= seq_len) e = __fadd_rn(e, m1[2][i + 1]);                // (i+1, j) deleted after it
+        }
+        float wm = 0.f, wi = 0.f, wd = 0.f;
+        if (i == 0) {
+          wi = e;
+          s_g[(j - 1) * kVocab + 0] = __fadd_rn(s_g[(j - 1) * kVocab + 0], e);
+        } else if (j >= 1) {
+          const float lp_sub = s_lp[(j - 1) * kVocab + s_lab[i - 1]], lp_ins = s_lp[(j - 1) * kVocab + 0];
+          float w[3];
+          softmin3_weights(__fadd_rn(V[diag_cell(k - 2, i - 1, L)], lp_sub),
+                           __fadd_rn(V[diag_cell(k - 1, i, L)], lp_ins),
+                           __fadd_rn(V[diag_cell(k - 1, i - 1, L)], del_cost), reg, hard_min, w);
+          wm = __fmul_rn(e, w[0]); wi = __fmul_rn(e, w[1]); wd = __fmul_rn(e, w[2]);
+          float* g = s_g + (j - 1) * kVocab;
+          g[s_lab[i - 1]] = __fadd_rn(g[s_lab[i - 1]], wm);
+          g[0] = __fadd_rn(g[0], wi);
+          if (mt) mt[(size_t)(i - 1) * L + (j - 1)] = wm;
+        }
+        out[0][i] = wm; out[1][i] = wi; out[2][i] = wd;
+      }
+      __syncthreads();
+    }
+    if (grad_out) {
+      float* gp = grad_out + (size_t)b * L * kVocab;
+      for (int j = tid; j < L; j += blockDim.x) {
+        float q[kVocab], gq[kVocab];
+        for (int t = 0; t < kVocab; ++t) q[t] = p[j * kVocab + t];
+        float tot = q[0];
+        for (int t = 1; t < kVocab; ++t) tot = __fadd_rn(tot, q[t]);
+        for (int t = 0; t < kVocab; ++t) {
+          q[t] = q[t] / tot;
+          gq[t] = q[t] >= kEps && q[t] <= kOneMinusEps ? -__fdiv_rn(s_g[j * kVocab + t], q[t]) : 0.f;
+        }
+        float dot = __fmul_rn(gq[0], q[0]);
+        for (int t = 1; t < kVocab; ++t) dot = __fadd_rn(dot, __fmul_rn(gq[t], q[t]));
+        for (int t = 0; t < kVocab; ++t) gp[j * kVocab + t] = __fdiv_rn(__fsub_rn(gq[t], dot), tot);
+      }
+    }
+    __syncthreads();   // shared buffers are reused by the next window
+  }
 }
 
 // Directions byte of a cell: bits 0-1 match-state argmax (0..2), bit 2 insert-state argmax (0..1), bits 3-4 delete-state
@@ -320,6 +488,29 @@ cudaError_t launch_evaluate(const float* probs, const uint8_t* labels, const uin
   cudaError_t err = cudaFuncSetAttribute(align_identity_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (err != cudaSuccess) return err;
   align_identity_kernel<<<dim3(B, 2), kEvalThreads, smem, st>>>(probs, labels, ccs_ids, L, pred_counts, ccs_counts, exact);
+  return cudaGetLastError();
+}
+
+cudaError_t loss_grad_grid(int B, int* ctas) {
+  int dev = 0, sms = 0, per_sm = 0;
+  cudaError_t err = cudaGetDevice(&dev);
+  if (err == cudaSuccess) err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (err == cudaSuccess)
+    err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, align_loss_grad_kernel, kEvalThreads, 0);
+  if (err != cudaSuccess) return err;
+  const int resident = sms * std::max(1, std::min(per_sm, kLossGradCtasPerSm));
+  *ctas = std::max(1, std::min(B, resident));
+  return cudaSuccess;
+}
+
+size_t loss_grad_table_bytes(int L, int ctas) { return (size_t)ctas * (L + 1) * (L + 1) * sizeof(float); }
+
+cudaError_t launch_loss_grad(const float* probs, const uint8_t* labels, int B, int L, float del_cost, float loss_reg,
+                             int hard_min, float* tables, int ctas, float* loss, float* grad, float* matches,
+                             cudaStream_t st) {
+  if (B <= 0) return cudaSuccess;
+  align_loss_grad_kernel<<<ctas, kEvalThreads, 0, st>>>(probs, labels, B, L, del_cost, loss_reg, hard_min, tables, loss,
+                                                        grad, matches);
   return cudaGetLastError();
 }
 

@@ -54,6 +54,14 @@ void launch_head_epilogue(const float* logits, int n, const HeadParams& p, cudaS
 cudaError_t launch_evaluate(const float* probs, const uint8_t* labels, const uint8_t* ccs_ids, int B, int L,
                             float del_cost, float loss_reg, int hard_min, float* loss, uint8_t* exact,
                             int32_t* pred_counts, int32_t* ccs_counts, cudaStream_t st);
+// AlignmentLoss per window with its gradient: loss [B], d loss / d probs [B, L, 5] and the soft alignment matches
+// [B, L, L] (both nullable).  `tables` is loss_grad_table_bytes(L, ctas) of device scratch, ctas from loss_grad_grid(B)
+// (persistent grid on the current device).  Device pointers.
+cudaError_t loss_grad_grid(int B, int* ctas);
+size_t loss_grad_table_bytes(int L, int ctas);
+cudaError_t launch_loss_grad(const float* probs, const uint8_t* labels, int B, int L, float del_cost, float loss_reg,
+                             int hard_min, float* tables, int ctas, float* loss, float* grad, float* matches,
+                             cudaStream_t st);
 // DistillationLoss per window from teacher / student logits [B, L, 5]; logit_loss 0 = mean squared error, 1 = KL
 // divergence (DCB_LOGIT_LOSS_*).  Device pointers.
 cudaError_t launch_distill_loss(const float* teacher, const float* student, int B, int L, float temperature,

@@ -86,7 +86,7 @@ ABI_SYMBOLS = (
     "dcb_create", "dcb_load_weights", "dcb_forward", "dcb_submit", "dcb_wait", "dcb_stitch", "dcb_last_forward_ms",
     "dcb_packed_window_bytes", "dcb_pack_rows", "dcb_forward_packed", "dcb_submit_packed",
     "dcb_stitch_fastq", "dcb_skip_mask", "dcb_fill_skipped", "dcb_evaluate", "dcb_distill_loss",
-    "dcb_prep_open", "dcb_prep_set_threads", "dcb_prep_next_zmw", "dcb_prep_get_windows", "dcb_prep_ccs_header", "dcb_prep_close",
+    "dcb_alignment_loss_grad", "dcb_prep_open", "dcb_prep_set_threads", "dcb_prep_next_zmw", "dcb_prep_get_windows", "dcb_prep_ccs_header", "dcb_prep_close",
     "dcb_prep_last_error", "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
     "dcb_last_forward_launches", "dcb_set_profile", "dcb_get_profile", "dcb_get_profile_kernels", "dcb_alloc_host",
     "dcb_free_host", "dcb_alloc_device", "dcb_free_device", "dcb_memcpy_h2d", "dcb_memcpy_d2h",
@@ -147,6 +147,8 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_evaluate.argtypes = [vp, vp, vp, vp, i32, i32, f64, f64, i32, u32, vp, vp, vp, vp,
                                ctypes.POINTER(ctypes.c_float)]
   lib.dcb_distill_loss.argtypes = [vp, vp, vp, i32, i32, f64, i32, u32, vp, ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_alignment_loss_grad.argtypes = [vp, vp, vp, i32, i32, f64, f64, i32, u32, vp, vp, vp,
+                                          ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_launches.argtypes = [vp, ctypes.POINTER(i32)]
   lib.dcb_set_debug.argtypes = [vp, i32]
@@ -232,6 +234,7 @@ class B200Model:
     self._handle = ctypes.c_void_p()
     self.params = params
     self.max_batch = max_batch
+    self.device = int(device)
     self.max_length = int(params.max_length)
     self.total_rows = params_lib.get_total_rows(params.max_passes, params.use_ccs_bq)
     cfg = make_config(params, max_batch, device, max_base_quality, calibration, chunk_tiles, precision)
@@ -652,6 +655,51 @@ class B200Model:
     self._check(self._lib.dcb_distill_loss(self._handle, t_ptr, s_ptr, B, L, float(temperature), lid, flags,
                                            loss.ctypes.data_as(ctypes.c_void_p), ctypes.byref(ms)))
     return dict(loss=loss, ms=float(ms.value))
+
+  def alignment_loss_grad(self, probs, labels, del_cost: Optional[float] = None, loss_reg: Any = "params",
+                          band_width: Any = "params", want_grad: bool = True, want_matches: bool = False,
+                          on_device: bool = False, batch: Optional[int] = None, length: Optional[int] = None,
+                          out: Optional[Dict[str, int]] = None) -> Dict[str, Any]:
+    """dcb_alignment_loss_grad: per-window AlignmentLoss, its gradient with respect to probs and the soft alignment
+    matches (AlignmentLoss.eval(return_matches=True)).  probs float32 [B, L, 5] and labels uint8 [B, L] are host arrays,
+    or device addresses with on_device=True, `batch` and optionally `length` (default max_length).  del_cost / loss_reg
+    / band_width default to params.json's, as in evaluate_windows.  Returns loss float32 [B], grad float32 [B, L, 5]
+    (None unless want_grad), matches float32 [B, L, L] (None unless want_matches) and ms, the kernel's device time.
+    With `out`, a dict of device addresses for "loss" and, as wanted, "grad" / "matches", the results are written
+    there instead and returned as None."""
+    if on_device:
+      if batch is None:
+        raise ValueError("alignment_loss_grad(on_device=True) needs batch")
+      B, L = int(batch), int(length) if length is not None else self.max_length
+      p_ptr, l_ptr, flags = ctypes.c_void_p(int(probs)), ctypes.c_void_p(int(labels)), DCB_ROWS_ON_DEVICE
+    else:
+      labels = np.ascontiguousarray(labels, dtype=np.uint8)
+      if labels.ndim != 2:
+        raise ValueError("labels must be uint8 [B, L], got %s" % (labels.shape,))
+      B, L = labels.shape
+      probs = np.ascontiguousarray(probs, dtype=np.float32)
+      if probs.shape != (B, L, 5):
+        raise ValueError("probs must be float32 [%d, %d, 5], got %s" % (B, L, probs.shape))
+      p_ptr, l_ptr, flags = probs.ctypes.data_as(ctypes.c_void_p), labels.ctypes.data_as(ctypes.c_void_p), 0
+    dc, reg, bw = self._eval_args(del_cost, loss_reg, band_width)
+    res: Dict[str, Any] = dict(loss=None, grad=None, matches=None)
+    if out is not None:
+      flags |= DCB_OUT_ON_DEVICE
+      ptrs = [ctypes.c_void_p(int(out["loss"])),
+              ctypes.c_void_p(int(out["grad"])) if want_grad else None,
+              ctypes.c_void_p(int(out["matches"])) if want_matches else None]
+    else:
+      res["loss"] = np.zeros(B, np.float32)
+      if want_grad:
+        res["grad"] = np.zeros((B, L, 5), np.float32)
+      if want_matches:
+        res["matches"] = np.zeros((B, L, L), np.float32)
+      ptrs = [None if res[k] is None else res[k].ctypes.data_as(ctypes.c_void_p) for k in ("loss", "grad", "matches")]
+    ms = ctypes.c_float()
+    self._check(self._lib.dcb_alignment_loss_grad(self._handle, p_ptr, l_ptr, B, L, dc, reg, bw, flags, *ptrs,
+                                                  ctypes.byref(ms)))
+    res["ms"] = float(ms.value)
+    return res
 
   def ccs_ids(self, rows_or_packed: np.ndarray) -> np.ndarray:
     """The CCS row of every window as ids uint8 [B, L] (model_utils.get_ccs_from_example: row 4 * max_passes)."""

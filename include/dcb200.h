@@ -237,6 +237,28 @@ int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const
                  int32_t L, double del_cost, double loss_reg, int32_t band_width, uint32_t flags, float* loss_out,
                  uint8_t* exact_out, int32_t* pred_counts, int32_t* ccs_counts, float* ms_out);
 
+/* The gradient of the alignment loss, for training: AlignmentLoss.eval(return_matches=True)
+ * (losses_and_metrics.py:549-595, width=None) and the gradient the training loop's tape takes of the per-window loss
+ * with respect to y_pred (model_train_custom_loop.py, model_distillation.py).  For B windows of length L <= 256, probs
+ * float32 [B, L, 5] and labels u8 [B, L] (ids 0..4 over ' ATCG'):
+ *   loss_out [B]            the loss, bitwise equal to dcb_evaluate's loss_out on the same arguments
+ *   grad_out [B, L, 5]      d loss[b] / d probs[b] (nullable): float32, with TensorFlow's gradient semantics -- the
+ *                           soft-min's gradient is softmax(-t / loss_reg), the hard min's splits equally among exactly
+ *                           tied minima, clip_by_value passes at its bounds and is zero outside, xlogy is zero where
+ *                           the one-hot label is zero, probs are renormalised to sum to 1 on the way in
+ *   matches_out [B, L, L]   d loss[b] / d substitution cost [i][j] (nullable): the soft alignment of left-shifted label
+ *                           position i to prediction position j; rows at or beyond the label's length are 0
+ * loss_reg <= 0 is the hard min (params.loss_reg None); band_width >= 0 is DCB_ERR_INVALID (pass DCB_BAND_WIDTH_NONE).
+ * probs / labels are host arrays, or device arrays with DCB_ROWS_ON_DEVICE; outputs are host arrays, or device arrays
+ * with DCB_OUT_ON_DEVICE.  The engine keeps every DP cell of each window in device scratch it grows on demand ((L + 1)^2
+ * floats per resident CTA).  ms_out (nullable) receives the kernel's device time.  Returns once the work on the engine's
+ * stream has finished.  DCB_ERR_INVALID for batch < 0, L outside 1..256, a label id above 4, or a null probs / labels /
+ * loss_out with batch > 0; batch == 0 does nothing.  Deterministic: no atomics; repeated calls, and host vs device
+ * pointers, give identical bits. */
+int dcb_alignment_loss_grad(dcb_engine* e, const float* probs, const uint8_t* labels, int32_t batch, int32_t L,
+                            double del_cost, double loss_reg, int32_t band_width, uint32_t flags, float* loss_out,
+                            float* grad_out, float* matches_out, float* ms_out);
+
 /* The distillation term of a distilled student's loss: DistillationLoss.call (losses_and_metrics.py:1170-1213), which
  * the distillation loop's eval step adds to the student's AlignmentLoss (model_distillation.py:242-270,320-349:
  * per example student_alpha * AlignmentLoss + distill_alpha * DistillationLoss).  For a batch of B windows of length
