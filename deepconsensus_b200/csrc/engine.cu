@@ -24,15 +24,44 @@ namespace {
 
 thread_local std::string g_create_error;
 
+// One embedding table of the checkpoint (networks.py:375-421) and its element offset in the table blob.  The blob's
+// tables start 16-byte aligned as bf16 (the embed kernel's width-8 fast path); the float32 blob uses the same offsets.
+struct EmbedTable {
+  const char* layer;
+  int vocab, width, off;
+};
+
 struct LayerDev {
   __nv_bfloat16* wqkv = nullptr;  // 6 groups x split-bf16 [72][144][8]: q_h0, q_h1, k_h0, k_h1, v_h0, v_h1
   __nv_bfloat16* wo = nullptr;    // split-bf16 [72][288][8]
   __nv_bfloat16* w1 = nullptr;    // ff / kFFChunk groups x [36][kFFChunk][8]
   __nv_bfloat16* w2 = nullptr;    // [ff/8][288][8] (ReZero alpha folded in)
-  float* b1 = nullptr;            // [ff]
+  float* b1 = nullptr;            // [ff] (both paths)
   float* b2 = nullptr;            // [288] (gain folded)
-  float* ln_g[2] = {nullptr, nullptr};  // pre-norm gamma/beta of the attention / FFN sub-layer
+  float* ln_g[2] = {nullptr, nullptr};  // [288] pre-norm gamma/beta of the attention / FFN sub-layer (both paths)
   float* ln_b[2] = {nullptr, nullptr};
+  struct {   // strict-fp32 path (strict_kernels.cu): float32 in the reference's own shapes
+    float *wq = nullptr, *wk = nullptr, *wv = nullptr, *wo = nullptr, *w1 = nullptr, *w2 = nullptr, *b2 = nullptr;
+    float alpha[2] = {1.f, 1.f};
+  } strict;
+};
+
+// The device copy of one checkpoint.  dcb_load_weights builds a complete new set before it frees the previous one.
+struct Weights {
+  EmbedCol* cols = nullptr;
+  EmbedRow* rowmeta = nullptr;
+  __nv_bfloat16* tables = nullptr;
+  __nv_bfloat16* wc = nullptr;   // split-bf16 condenser [2 Epad / 8][288][8]
+  float* pe = nullptr;           // positional table [Lw][288]
+  float* pe_img = nullptr;       // same table in residual-image order (window-aligned layout only)
+  std::vector<LayerDev> layers;
+  float *fln_g = nullptr, *fln_b = nullptr, *wfc = nullptr, *bfc = nullptr;   // final LayerNorm [288], fc1 (both paths)
+  float *head_gw8 = nullptr, *head_ab = nullptr;   // head_kernel: gamma * Wfc (padded to 8) and the A / B sums
+  struct {   // strict-fp32 path
+    StrictEmbedRow* embed = nullptr;
+    float *tables = nullptr, *wc = nullptr, *pe = nullptr;   // pe: [L][280]
+  } strict;
+  std::vector<void*> owned;
 };
 
 }  // namespace
@@ -76,17 +105,11 @@ struct dcb_engine {
   float last_ms = 0.f;
   int last_launches = 0;
   int last_chunk_tokens = 0;
-  // model
-  EmbedCol* d_cols = nullptr;
-  EmbedRow* d_rowmeta = nullptr;
+  // model: the embedding layout follows from the configuration (dcb_create), the weights from the checkpoint
+  std::vector<EmbedTable> tables;
+  std::vector<StrictEmbedRow> embed;   // per input row, in concat order; table_off into the table blob
   int table_elems = 0;
-  __nv_bfloat16* d_tables = nullptr;
-  __nv_bfloat16* d_wc = nullptr;   // split-bf16 condenser [2 Epad / 8][288][8]
-  float* d_pe = nullptr;
-  float* d_pe_img = nullptr;   // same table in residual-image order (window-aligned layout only)
-  std::vector<LayerDev> layers;
-  float *d_fln_g = nullptr, *d_fln_b = nullptr, *d_wfc = nullptr, *d_bfc = nullptr;
-  float *d_head_gw8 = nullptr, *d_head_ab = nullptr;   // head_kernel: gamma * Wfc (padded to 8) and the A / B sums
+  Weights w;
   // workspace
   __nv_bfloat16* d_embqkv = nullptr;
   float* d_x = nullptr;
@@ -108,22 +131,12 @@ struct dcb_engine {
   cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;
   float* d_dbg = nullptr;  // [stages][chunk_tiles * x_image]
   __nv_bfloat16* d_dbg_op = nullptr;   // bf16 operand images per stage (dbg_operand_slot)
-  // strict-fp32 path (strict_kernels.cu): float32 copies of every variable in the reference's own shapes, and a
-  // row-major workspace allocated on the first strict call
-  struct StrictLayer {
-    float *wq = nullptr, *wk = nullptr, *wv = nullptr, *wo = nullptr, *w1 = nullptr, *b1 = nullptr, *w2 = nullptr, *b2 = nullptr;
-    float *ln_g[2] = {nullptr, nullptr}, *ln_b[2] = {nullptr, nullptr};
-    float alpha[2] = {1.f, 1.f};
-  };
+  // strict-fp32 path (strict_kernels.cu): row-major workspace, allocated on the first strict call
   struct Strict {
-    StrictEmbedRow* meta = nullptr;
-    float *tables = nullptr, *wc = nullptr, *pe = nullptr;
-    float *fln_g = nullptr, *fln_b = nullptr;
-    std::vector<StrictLayer> layers;
     float *emb = nullptr, *x = nullptr, *y = nullptr, *q = nullptr, *k = nullptr, *v = nullptr, *att = nullptr, *hid = nullptr;
     int chunk_windows = 0;
   } strict;
-  std::vector<void*> owned;
+  std::vector<void*> owned;   // workspace
 };
 
 namespace {
@@ -154,17 +167,23 @@ void set_head_quality(HeadParams& hp, const dcb_config& c) {
                   __FILE__, __LINE__);                                                  \
   } while (0)
 
+// n zeroed elements, freed with the allocations in `owned` (the engine's workspace or one weight set)
 template <typename T>
-int dev_alloc(dcb_engine* e, T** p, size_t n) {
+int dev_alloc(dcb_engine* e, std::vector<void*>& owned, T** p, size_t n) {
   CU(e, cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)));
+  owned.push_back(*p);
   CU(e, cudaMemset(*p, 0, n * sizeof(T)));
-  e->owned.push_back(*p);
   return DCB_OK;
 }
 
 template <typename T>
-int upload(dcb_engine* e, T** p, const std::vector<T>& h) {
-  int rc = dev_alloc(e, p, h.size());
+int dev_alloc(dcb_engine* e, T** p, size_t n) {
+  return dev_alloc(e, e->owned, p, n);
+}
+
+template <typename T>
+int upload(dcb_engine* e, std::vector<void*>& owned, T** p, const std::vector<T>& h) {
+  int rc = dev_alloc(e, owned, p, h.size());
   if (rc) return rc;
   CU(e, cudaMemcpy(*p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
   return DCB_OK;
@@ -192,31 +211,235 @@ std::vector<__nv_bfloat16> pack_b_split(int kpad, int n, const std::function<flo
   return img;
 }
 
-struct TensorMap {
-  std::map<std::string, const dcb_tensor*> m;
-  dcb_engine* e;
-  const float* get(const std::string& name, std::initializer_list<int64_t> shape, int* rc) {
-    auto it = m.find(name);
-    if (it == m.end()) {
-      *rc = fail(e, DCB_ERR_WEIGHTS, "missing variable %s", name.c_str());
-      return nullptr;
-    }
-    const dcb_tensor* t = it->second;
-    bool ok = t->ndim == (int)shape.size() && t->data != nullptr;
-    int i = 0;
-    for (int64_t s : shape) { if (ok && t->shape[i] != s) ok = false; ++i; }
-    if (!ok) {
-      *rc = fail(e, DCB_ERR_WEIGHTS, "variable %s has the wrong shape/ndim", name.c_str());
-      return nullptr;
-    }
-    return t->data;
-  }
-};
-
 std::vector<float> pad288(const float* src, float scale = 1.f) {
   std::vector<float> v(kDP, 0.f);
   for (int i = 0; i < kD; ++i) v[i] = src[i] * scale;
   return v;
+}
+
+// The checkpoint's variables, each looked up and shape-checked once: host pointers into the caller's tensors.
+struct Checkpoint {
+  struct Layer {
+    float alpha[2] = {1.f, 1.f};   // ReZero
+    const float *ln_g[2] = {}, *ln_b[2] = {};   // pre-LN
+    const float *wq, *wk, *wv, *wo, *w1, *b1, *w2, *b2;
+  };
+  std::vector<const float*> tables;   // per dcb_engine::tables entry
+  const float* wc;
+  std::vector<Layer> layers;
+  const float *fln_g, *fln_b, *wfc, *bfc;
+};
+
+int read_checkpoint(dcb_engine* e, const dcb_tensor* tensors, int n, Checkpoint* ck) {
+  std::map<std::string, const dcb_tensor*> m;
+  for (int i = 0; i < n; ++i)
+    if (tensors[i].name) m[tensors[i].name] = &tensors[i];
+  int rc = DCB_OK;   // the first failure: later lookups are skipped, so its message is the one reported
+  auto get = [&](const std::string& name, std::initializer_list<int64_t> shape) -> const float* {
+    if (rc) return nullptr;
+    auto it = m.find(name);
+    if (it == m.end()) { rc = fail(e, DCB_ERR_WEIGHTS, "missing variable %s", name.c_str()); return nullptr; }
+    const dcb_tensor* t = it->second;
+    bool ok = t->ndim == (int)shape.size() && t->data != nullptr;
+    int i = 0;
+    for (int64_t s : shape) { if (ok && t->shape[i] != s) ok = false; ++i; }
+    if (!ok) { rc = fail(e, DCB_ERR_WEIGHTS, "variable %s has the wrong shape/ndim", name.c_str()); return nullptr; }
+    return t->data;
+  };
+  const dcb_config& c = e->cfg;
+  const int ff = c.filter_size;
+  for (const EmbedTable& tb : e->tables)
+    ck->tables.push_back(get(std::string("model/") + tb.layer + "/embeddings", {tb.vocab, tb.width}));
+  ck->wc = get("model/transformer_input_condenser/kernel", {e->E, kD});
+  ck->layers.resize(c.num_hidden_layers);
+  for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
+    Checkpoint::Layer& l = ck->layers[n_];
+    const std::string pre = "model/encoder_stack/layers/" + std::to_string(n_);
+    const std::string P0 = pre + "/0", P1 = pre + "/1";
+    for (int s = 0; s < 2; ++s) {
+      const std::string& P = s ? P1 : P0;
+      if (c.rezero) {
+        if (const float* a = get(P + "/alpha", {})) l.alpha[s] = *a;
+      } else {
+        l.ln_g[s] = get(P + "/layer_norm/gamma", {kD});
+        l.ln_b[s] = get(P + "/layer_norm/beta", {kD});
+      }
+    }
+    l.wq = get(P0 + "/layer/query_dense_layer/kernel", {kD, kHeads, kDH});
+    l.wk = get(P0 + "/layer/key_dense_layer/kernel", {kD, kHeads, kDH});
+    l.wv = get(P0 + "/layer/value_dense_layer/kernel", {kD, kHeads, kDH});
+    l.wo = get(P0 + "/layer/output_dense_layer/kernel", {kHeads, kDH, kD});
+    l.w1 = get(P1 + "/layer/filter_dense_layer/kernel", {kD, ff});
+    l.b1 = get(P1 + "/layer/filter_dense_layer/bias", {ff});
+    l.w2 = get(P1 + "/layer/output_dense_layer/kernel", {ff, kD});
+    l.b2 = get(P1 + "/layer/output_dense_layer/bias", {kD});
+  }
+  ck->fln_g = get("model/encoder_stack/output_normalization/gamma", {kD});
+  ck->fln_b = get("model/encoder_stack/output_normalization/beta", {kD});
+  ck->wfc = get("model/fc1/kernel", {kD, kVocab});
+  ck->bfc = get("model/fc1/bias", {kVocab});
+  return rc;
+}
+
+void free_weights(Weights& w) {
+  for (void* p : w.owned) cudaFree(p);
+  w = Weights();
+}
+
+// Both paths' device weights from a validated checkpoint, allocated in w->owned.
+int upload_weights(dcb_engine* e, const Checkpoint& ck, Weights* w) {
+  const dcb_config& c = e->cfg;
+  int rc = DCB_OK;   // the first failure: later uploads are skipped
+  auto up = [&](auto** p, const auto& h) { if (!rc) rc = upload(e, w->owned, p, h); };
+  auto copy = [&](float** p, const float* src, size_t n) { up(p, std::vector<float>(src, src + n)); };
+
+  // ---- embedding tables (networks.py:375-421), pre-scaled by sqrt(width), row 0 zeroed
+  //      (ModifiedOnDeviceEmbedding, networks.py:42-63); the bf16 blob is the float32 blob rounded
+  std::vector<float> blob(e->table_elems, 0.f);
+  for (size_t t = 0; t < e->tables.size(); ++t) {
+    const EmbedTable& tb = e->tables[t];
+    const float scale = sqrtf((float)tb.width);
+    for (int i = tb.width; i < tb.vocab * tb.width; ++i) blob[tb.off + i] = ck.tables[t][i] * scale;
+  }
+  std::vector<__nv_bfloat16> blob16(blob.size());
+  for (size_t i = 0; i < blob.size(); ++i) blob16[i] = __float2bfloat16(blob[i]);
+  // ---- the embed kernel's per-row id rules and per-column gather descriptors (columns E..Epad: src_row -1)
+  std::vector<EmbedRow> rowmeta;
+  std::vector<EmbedCol> cols(e->Epad, EmbedCol{-1, 0, 0, 0, 0, 0, 0.f});
+  for (int r = 0; r < e->R; ++r) {
+    const StrictEmbedRow& m = e->embed[r];
+    rowmeta.push_back(EmbedRow{m.clip_hi, m.shift, m.vocab});
+    for (int j = 0; j < m.width; ++j)
+      cols[m.col0 + j] = EmbedCol{(int16_t)r, (int16_t)m.width, (int16_t)j, (int16_t)m.shift, m.table_off, m.vocab, m.clip_hi};
+  }
+  up(&w->tables, blob16);
+  up(&w->rowmeta, rowmeta);
+  up(&w->cols, cols);
+  up(&w->strict.tables, blob);
+  up(&w->strict.embed, e->embed);
+  // ---- condenser (networks.py:426-434): B image [Epad/8][288][8]
+  {
+    const int E = e->E;
+    auto img = pack_b_split(e->Epad, kDP, [&](int k, int nn) { return (k < E && nn < kD) ? ck.wc[(size_t)k * kD + nn] : 0.f; });
+    up(&w->wc, img);
+    copy(&w->strict.wc, ck.wc, (size_t)E * kD);
+  }
+  // ---- positional encoding table [Lw][288] (tf-models RelativePositionEmbedding; networks.py:301-323)
+  {
+    std::vector<float> pe((size_t)e->Lw * kDP, 0.f);
+    if (c.add_pos_encoding) {
+      const int nt = kD / 2;
+      const float inc = (float)(log(1e4 / 1.0) / (double)(nt - 1));
+      for (int l = 0; l < e->L; ++l)
+        for (int k = 0; k < nt; ++k) {
+          const float inv = expf((float)k * -inc);
+          const float sc = (float)l * inv;
+          pe[(size_t)l * kDP + k] = sinf(sc);
+          pe[(size_t)l * kDP + nt + k] = cosf(sc);
+        }
+    }
+    up(&w->pe, pe);
+    if (e->Lw == kTileM) {
+      // window-aligned layout: every tile sees positions 0..127, so the table can also be laid out like the residual
+      // image [72][128][4] -- a warp of the row epilogue then reads 512 contiguous bytes instead of 32 scattered rows
+      std::vector<float> img((size_t)kTileM * kDP, 0.f);
+      for (int l = 0; l < kTileM; ++l)
+        for (int col = 0; col < kDP; ++col) img[((size_t)(col / 4) * kTileM + l) * 4 + (col & 3)] = pe[(size_t)l * kDP + col];
+      up(&w->pe_img, img);
+    }
+    std::vector<float> pe_strict((size_t)e->L * kD);   // the strict GEMM epilogue reads [L][280]
+    for (int l = 0; l < e->L; ++l) std::copy_n(&pe[(size_t)l * kDP], kD, &pe_strict[(size_t)l * kD]);
+    up(&w->strict.pe, pe_strict);
+  }
+  // ---- encoder layers
+  const int ff = c.filter_size;
+  w->layers.assign(c.num_hidden_layers, LayerDev());
+  for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
+    LayerDev& ld = w->layers[n_];
+    const Checkpoint::Layer& l = ck.layers[n_];
+    const float alpha0 = l.alpha[0], alpha1 = l.alpha[1];
+    for (int s = 0; s < 2 && !c.rezero; ++s) {
+      up(&ld.ln_g[s], pad288(l.ln_g[s]));
+      up(&ld.ln_b[s], pad288(l.ln_b[s]));
+    }
+    const float qscale = 1.0f / sqrtf((float)kDH);  // query *= depth**-0.5 (attention_layer.py:196-197)
+    {
+      // kQKVN / kQKVGroup n-groups of 288 columns: [q_h0 q_h1 | k_h0 k_h1 | v_h0 v_h1], each slot 144 wide (140 + 4 zero)
+      std::vector<__nv_bfloat16> img;
+      for (int grp = 0; grp < kQKVN / kQKVGroup; ++grp) {
+        auto part = pack_b_split(kDP, kQKVGroup, [&](int k, int nn) {
+          const int colg = grp * kQKVGroup + nn;
+          const int slot = colg / kDHP, dd = colg % kDHP;
+          if (k >= kD || dd >= kDH) return 0.f;
+          const int proj = slot / kHeads, head = slot % kHeads;
+          const float* wp = proj == 0 ? l.wq : (proj == 1 ? l.wk : l.wv);
+          const float v = wp[((size_t)k * kHeads + head) * kDH + dd];
+          return proj == 0 ? v * qscale : v;
+        });
+        img.insert(img.end(), part.begin(), part.end());
+      }
+      up(&ld.wqkv, img);
+    }
+    {
+      // out-proj: K index = head*144 + dd, N = e; ReZero alpha folded in (encoder_stack.py:88-90)
+      auto img = pack_b_split(kDP, kDP, [&](int k, int nn) {
+        const int head = k / kDHP, dd = k % kDHP;
+        if (dd >= kDH || nn >= kD) return 0.f;
+        return l.wo[((size_t)head * kDH + dd) * kD + nn] * alpha0;
+      });
+      up(&ld.wo, img);
+    }
+    {
+      // W1 in n-groups of kFFChunk hidden units, W2 as one [ff/8][288][8] image (ReZero alpha folded in)
+      const int gw = kFFChunk;
+      std::vector<__nv_bfloat16> img;
+      img.reserve((size_t)ff * kDP);
+      for (int grp = 0; grp < ff / gw; ++grp) {
+        auto part = pack_b(kDP, gw, [&](int k, int nn) { return k < kD ? l.w1[(size_t)k * ff + grp * gw + nn] : 0.f; });
+        img.insert(img.end(), part.begin(), part.end());
+      }
+      up(&ld.w1, img);
+      auto img2 = pack_b(ff, kDP, [&](int k, int nn) { return nn < kD ? l.w2[(size_t)k * kD + nn] * alpha1 : 0.f; });
+      up(&ld.w2, img2);
+    }
+    copy(&ld.b1, l.b1, ff);
+    up(&ld.b2, pad288(l.b2, alpha1));
+    // the strict path: every matrix once more as float32, in the reference's own shapes
+    ld.strict.alpha[0] = alpha0;
+    ld.strict.alpha[1] = alpha1;
+    copy(&ld.strict.wq, l.wq, (size_t)kD * kD);
+    copy(&ld.strict.wk, l.wk, (size_t)kD * kD);
+    copy(&ld.strict.wv, l.wv, (size_t)kD * kD);
+    copy(&ld.strict.wo, l.wo, (size_t)kD * kD);
+    copy(&ld.strict.w1, l.w1, (size_t)kD * ff);
+    copy(&ld.strict.w2, l.w2, (size_t)ff * kD);
+    copy(&ld.strict.b2, l.b2, kD);
+  }
+  // ---- head
+  up(&w->fln_g, pad288(ck.fln_g));
+  up(&w->fln_b, pad288(ck.fln_b));
+  copy(&w->wfc, ck.wfc, kD * kVocab);
+  copy(&w->bfc, ck.bfc, kVocab);
+  {
+    // head_kernel folds the final LayerNorm into the fc1 sums (one pass over the row): logits_j = rstd * (sum_c y_c g_c W_cj
+    // - mean_y * A_j) + B_j + bfc_j.  The products are formed here once, in float32.
+    const float *g = ck.fln_g, *b = ck.fln_b, *wf = ck.wfc;
+    std::vector<float> gw8((size_t)kD * 8, 0.f), ab(16, 0.f);
+    for (int cc = 0; cc < kD; ++cc)
+      for (int j = 0; j < kVocab; ++j) gw8[(size_t)cc * 8 + j] = g[cc] * wf[cc * kVocab + j];
+    for (int j = 0; j < kVocab; ++j) {
+      float a = 0.f, bsum = 0.f;
+      for (int cc = 0; cc < kD; ++cc) { a += g[cc] * wf[cc * kVocab + j]; bsum += b[cc] * wf[cc * kVocab + j]; }
+      ab[j] = a; ab[8 + j] = bsum;
+    }
+    up(&w->head_gw8, gw8);
+    up(&w->head_ab, ab);
+  }
+  if (rc) return rc;
+  // the uploads have landed before any kernel on the engine's (non-blocking) streams reads them, and no kernel still
+  // reads the previous set when the caller frees it
+  CU(e, cudaDeviceSynchronize());
+  return DCB_OK;
 }
 
 }  // namespace
@@ -271,10 +494,32 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
   if (align && e->L <= kTileM) e->Lw = kTileM;
   e->R = 4 * cfg->max_passes + (cfg->use_ccs_bq ? 6 : 5);  // data_providers.py:61-78
   e->pl = make_packed_layout(cfg->max_passes, cfg->max_length, cfg->use_ccs_bq ? 1 : 0);
-  e->E = cfg->max_passes * (cfg->per_base_hidden_size + cfg->pw_hidden_size + cfg->ip_hidden_size +
-                            cfg->strand_hidden_size) +
-         cfg->per_base_hidden_size + (cfg->use_ccs_bq ? cfg->ccs_bq_hidden_size : 0) +
-         4 * cfg->sn_hidden_size;
+  {
+    // the embedding in concat order (networks.py:457-506): each table once in the blob, then each input row with its
+    // table, clip (data_providers.py:151-162), id shift and first column; E is the sum of the rows' widths
+    auto table = [&](const char* layer, int vocab, int width) {
+      const int off = (e->table_elems + 7) / 8 * 8;
+      e->tables.push_back(EmbedTable{layer, vocab, width, off});
+      e->table_elems = off + vocab * width;
+      return e->tables.back();
+    };
+    auto rows = [&](const EmbedTable& tb, int n, float clip, int shift) {
+      for (int r = 0; r < n; ++r) {
+        e->embed.push_back(StrictEmbedRow{clip, shift, tb.vocab, tb.width, e->E, tb.off});
+        e->E += tb.width;
+      }
+    };
+    const int P = cfg->max_passes;
+    const EmbedTable bases = table("bases_embedding_layer", kVocab, cfg->per_base_hidden_size);
+    rows(bases, P, 0.f, 0);
+    rows(table("pw_embedding_layer", cfg->pw_max + 1, cfg->pw_hidden_size), P, (float)cfg->pw_max, 0);
+    rows(table("ip_embedding_layer", cfg->ip_max + 1, cfg->ip_hidden_size), P, (float)cfg->ip_max, 0);
+    rows(table("strand_embedding_layer", cfg->strand_max + 1, cfg->strand_hidden_size), P, 0.f, 0);
+    rows(bases, 1, 0.f, 0);                                                  // ccs shares the bases table (networks.py:485-489)
+    if (cfg->use_ccs_bq)                                                     // +1 shift (networks.py:495)
+      rows(table("ccs_base_quality_scores_embedding_layer", cfg->ccs_bq_max, cfg->ccs_bq_hidden_size), 1, 0.f, 1);
+    rows(table("sn_embedding_layer", cfg->sn_max + 1, cfg->sn_hidden_size), 4, (float)cfg->sn_max, 0);
+  }
   e->Epad = (e->E + 15) / 16 * 16;
   e->echunks = e->Epad / 8;
   if (ct <= 0) ct = 8 * e->num_sms;   // measured: larger chunks win (kernels are not DRAM-bound)
@@ -300,7 +545,7 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
   {
     std::vector<double> p10(256);
     for (int q = 0; q < 256; ++q) p10[q] = pow(10.0, (double)q / -10.0);    // utils.py:103: 10 ** (q / -10.0)
-    TRY(upload(e, &e->d_p10, p10));
+    TRY(upload(e, e->owned, &e->d_p10, p10));
   }
   const size_t T = e->chunk_tiles;
   for (auto& sl : e->slots) {
@@ -330,6 +575,7 @@ void dcb_destroy(dcb_engine* e) {
   if (e->stream) cudaStreamSynchronize(e->stream);
   if (e->out_stream) cudaStreamSynchronize(e->out_stream);
   for (void* p : e->owned) cudaFree(p);
+  free_weights(e->w);
   if (e->d_st_in) cudaFree(e->d_st_in);
   if (e->d_st_out) cudaFree(e->d_st_out);
   if (e->d_st_start) cudaFree(e->d_st_start);
@@ -360,285 +606,20 @@ void dcb_destroy(dcb_engine* e) {
 int dcb_load_weights(dcb_engine* e, const dcb_tensor* tensors, int32_t n) {
   if (!e || !tensors) return fail(e, DCB_ERR_INVALID, "null argument");
   CU(e, cudaSetDevice(e->cfg.device));
-  const dcb_config& c = e->cfg;
-  TensorMap tm;
-  tm.e = e;
-  for (int i = 0; i < n; ++i)
-    if (tensors[i].name) tm.m[tensors[i].name] = &tensors[i];
-  int rc = DCB_OK;
-
-  // ---- embedding tables (networks.py:375-421), pre-scaled by sqrt(width), row 0 zeroed
-  //      (ModifiedOnDeviceEmbedding, networks.py:42-63)
-  struct Tab { const char* layer; int vocab, width; int off; const float* data; };
-  std::vector<Tab> tabs = {
-      {"bases_embedding_layer", kVocab, c.per_base_hidden_size, 0, nullptr},
-      {"pw_embedding_layer", c.pw_max + 1, c.pw_hidden_size, 0, nullptr},
-      {"ip_embedding_layer", c.ip_max + 1, c.ip_hidden_size, 0, nullptr},
-      {"strand_embedding_layer", c.strand_max + 1, c.strand_hidden_size, 0, nullptr},
-      {"ccs_base_quality_scores_embedding_layer", c.ccs_bq_max, c.ccs_bq_hidden_size, 0, nullptr},
-      {"sn_embedding_layer", c.sn_max + 1, c.sn_hidden_size, 0, nullptr},
-  };
-  std::vector<__nv_bfloat16> blob;
-  for (size_t t = 0; t < tabs.size(); ++t) {
-    if (t == 4 && !c.use_ccs_bq) continue;
-    Tab& tb = tabs[t];
-    tb.data = tm.get(std::string("model/") + tb.layer + "/embeddings", {tb.vocab, tb.width}, &rc);
-    if (rc) return rc;
-    while (blob.size() % 8) blob.push_back(__float2bfloat16(0.f));   // 16-byte aligned table rows (width-8 fast path)
-    tb.off = (int)blob.size();
-    const float scale = sqrtf((float)tb.width);
-    for (int v = 0; v < tb.vocab; ++v)
-      for (int j = 0; j < tb.width; ++j)
-        blob.push_back(__float2bfloat16(v == 0 ? 0.f : tb.data[v * tb.width + j] * scale));
+  if (embed_smem_bytes(e->R, e->echunks, e->table_elems) > 160 * 1024)
+    return fail(e, DCB_ERR_INVALID, "embedding tables + ids do not fit the embed kernel's shared memory");
+  // every variable is checked before the first allocation, and the previous weights stay in use until the new set is
+  // complete: a failed load changes nothing
+  Checkpoint ck;
+  int rc = read_checkpoint(e, tensors, n, &ck);
+  if (rc) return rc;
+  Weights w;
+  if ((rc = upload_weights(e, ck, &w))) {
+    free_weights(w);
+    return rc;
   }
-  // ---- per-column gather descriptors in concat order (networks.py:457-506)
-  std::vector<EmbedCol> cols(e->Epad);
-  for (auto& cc : cols) { cc = EmbedCol{}; cc.src_row = -1; }
-  {
-    const int P = c.max_passes;
-    int eoff = 0;
-    auto add_rows = [&](int tab, int row0, int nrows, float clip, int shift) {
-      for (int r = 0; r < nrows; ++r)
-        for (int j = 0; j < tabs[tab].width; ++j) {
-          EmbedCol& cc = cols[eoff++];
-          cc.src_row = (int16_t)(row0 + r);
-          cc.width = (int16_t)tabs[tab].width;
-          cc.col = (int16_t)j;
-          cc.shift = (int16_t)shift;
-          cc.table_off = tabs[tab].off;
-          cc.vocab = tabs[tab].vocab;
-          cc.clip_hi = clip;
-        }
-    };
-    add_rows(0, 0, P, 0.f, 0);                                  // bases
-    add_rows(1, P, P, (float)c.pw_max, 0);                      // pw   (clip: data_providers.py:151-154)
-    add_rows(2, 2 * P, P, (float)c.ip_max, 0);                  // ip   (:155-158)
-    add_rows(3, 3 * P, P, 0.f, 0);                              // strand
-    add_rows(0, 4 * P, 1, 0.f, 0);                              // ccs shares the bases table (networks.py:485-489)
-    int next = 4 * P + 1;
-    if (c.use_ccs_bq) { add_rows(4, next, 1, 0.f, 1); ++next; }  // +1 shift (networks.py:495)
-    add_rows(5, next, 4, (float)c.sn_max, 0);                   // sn   (:159-162)
-    if (eoff != e->E) return fail(e, DCB_ERR_INVALID, "internal: embedding width %d != %d", eoff, e->E);
-  }
-  {
-    std::vector<EmbedRow> meta(e->R, EmbedRow{0.f, 0, 1});
-    for (const EmbedCol& cc : cols)
-      if (cc.src_row >= 0) meta[cc.src_row] = EmbedRow{cc.clip_hi, cc.shift, cc.vocab};
-    if ((rc = upload(e, &e->d_rowmeta, meta))) return rc;
-    e->table_elems = (int)blob.size();
-    if (embed_smem_bytes(e->R, e->echunks, e->table_elems) > 160 * 1024)
-      return fail(e, DCB_ERR_INVALID, "embedding tables + ids do not fit the embed kernel's shared memory");
-  }
-  if ((rc = upload(e, &e->d_tables, blob))) return rc;
-  if ((rc = upload(e, &e->d_cols, cols))) return rc;
-
-  // ---- condenser (networks.py:426-434): B image [Epad/8][288][8]
-  {
-    const float* wc = tm.get("model/transformer_input_condenser/kernel", {e->E, kD}, &rc);
-    if (rc) return rc;
-    const int E = e->E;
-    auto img = pack_b_split(e->Epad, kDP, [&](int k, int nn) { return (k < E && nn < kD) ? wc[(size_t)k * kD + nn] : 0.f; });
-    if ((rc = upload(e, &e->d_wc, img))) return rc;
-  }
-  // ---- positional encoding table [L][288] (tf-models RelativePositionEmbedding; networks.py:301-323)
-  {
-    std::vector<float> pe((size_t)e->Lw * kDP, 0.f);
-    if (c.add_pos_encoding) {
-      const int nt = kD / 2;
-      const float inc = (float)(log(1e4 / 1.0) / (double)(nt - 1));
-      for (int l = 0; l < e->L; ++l)
-        for (int k = 0; k < nt; ++k) {
-          const float inv = expf((float)k * -inc);
-          const float sc = (float)l * inv;
-          pe[(size_t)l * kDP + k] = sinf(sc);
-          pe[(size_t)l * kDP + nt + k] = cosf(sc);
-        }
-    }
-    if ((rc = upload(e, &e->d_pe, pe))) return rc;
-    if (e->Lw == kTileM) {
-      // window-aligned layout: every tile sees positions 0..127, so the table can also be laid out like the residual
-      // image [72][128][4] -- a warp of the row epilogue then reads 512 contiguous bytes instead of 32 scattered rows
-      std::vector<float> img((size_t)kTileM * kDP, 0.f);
-      for (int l = 0; l < kTileM; ++l)
-        for (int col = 0; col < kDP; ++col) img[((size_t)(col / 4) * kTileM + l) * 4 + (col & 3)] = pe[(size_t)l * kDP + col];
-      if ((rc = upload(e, &e->d_pe_img, img))) return rc;
-    }
-  }
-  // ---- encoder layers
-  const int ff = c.filter_size;
-  e->layers.assign(c.num_hidden_layers, LayerDev());
-  for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
-    LayerDev& ld = e->layers[n_];
-    char pre[128];
-    snprintf(pre, sizeof pre, "model/encoder_stack/layers/%d", n_);
-    const std::string P0 = std::string(pre) + "/0", P1 = std::string(pre) + "/1";
-    float alpha0 = 1.f, alpha1 = 1.f;
-    if (c.rezero) {
-      const float* a0 = tm.get(P0 + "/alpha", std::initializer_list<int64_t>{}, &rc); if (rc) return rc;
-      const float* a1 = tm.get(P1 + "/alpha", std::initializer_list<int64_t>{}, &rc); if (rc) return rc;
-      alpha0 = *a0; alpha1 = *a1;
-    } else {
-      for (int s = 0; s < 2; ++s) {
-        const std::string P = s ? P1 : P0;
-        const float* g = tm.get(P + "/layer_norm/gamma", {kD}, &rc); if (rc) return rc;
-        const float* b = tm.get(P + "/layer_norm/beta", {kD}, &rc); if (rc) return rc;
-        if ((rc = upload(e, &ld.ln_g[s], pad288(g)))) return rc;
-        if ((rc = upload(e, &ld.ln_b[s], pad288(b)))) return rc;
-      }
-    }
-    const float* wq = tm.get(P0 + "/layer/query_dense_layer/kernel", {kD, kHeads, kDH}, &rc); if (rc) return rc;
-    const float* wk = tm.get(P0 + "/layer/key_dense_layer/kernel", {kD, kHeads, kDH}, &rc); if (rc) return rc;
-    const float* wv = tm.get(P0 + "/layer/value_dense_layer/kernel", {kD, kHeads, kDH}, &rc); if (rc) return rc;
-    const float* wo = tm.get(P0 + "/layer/output_dense_layer/kernel", {kHeads, kDH, kD}, &rc); if (rc) return rc;
-    const float qscale = 1.0f / sqrtf((float)kDH);  // query *= depth**-0.5 (attention_layer.py:196-197)
-    {
-      // kQKVN / kQKVGroup n-groups of 288 columns: [q_h0 q_h1 | k_h0 k_h1 | v_h0 v_h1], each slot 144 wide (140 + 4 zero)
-      std::vector<__nv_bfloat16> img;
-      for (int grp = 0; grp < kQKVN / kQKVGroup; ++grp) {
-        auto part = pack_b_split(kDP, kQKVGroup, [&](int k, int nn) {
-          const int colg = grp * kQKVGroup + nn;
-          const int slot = colg / kDHP, dd = colg % kDHP;
-          if (k >= kD || dd >= kDH) return 0.f;
-          const int proj = slot / kHeads, head = slot % kHeads;
-          const float* w = proj == 0 ? wq : (proj == 1 ? wk : wv);
-          const float v = w[((size_t)k * kHeads + head) * kDH + dd];
-          return proj == 0 ? v * qscale : v;
-        });
-        img.insert(img.end(), part.begin(), part.end());
-      }
-      if ((rc = upload(e, &ld.wqkv, img))) return rc;
-    }
-    {
-      // out-proj: K index = head*144 + dd, N = e; ReZero alpha folded in (encoder_stack.py:88-90)
-      auto img = pack_b_split(kDP, kDP, [&](int k, int nn) {
-        const int head = k / kDHP, dd = k % kDHP;
-        if (dd >= kDH || nn >= kD) return 0.f;
-        return wo[((size_t)head * kDH + dd) * kD + nn] * alpha0;
-      });
-      if ((rc = upload(e, &ld.wo, img))) return rc;
-    }
-    const float* w1 = tm.get(P1 + "/layer/filter_dense_layer/kernel", {kD, ff}, &rc); if (rc) return rc;
-    const float* b1 = tm.get(P1 + "/layer/filter_dense_layer/bias", {ff}, &rc); if (rc) return rc;
-    const float* w2 = tm.get(P1 + "/layer/output_dense_layer/kernel", {ff, kD}, &rc); if (rc) return rc;
-    const float* b2 = tm.get(P1 + "/layer/output_dense_layer/bias", {kD}, &rc); if (rc) return rc;
-    {
-      // W1 in n-groups of kFFChunk hidden units, W2 as one [ff/8][288][8] image (ReZero alpha folded in)
-      const int gw = kFFChunk;
-      std::vector<__nv_bfloat16> img;
-      img.reserve((size_t)ff * kDP);
-      for (int grp = 0; grp < ff / gw; ++grp) {
-        auto part = pack_b(kDP, gw, [&](int k, int nn) { return k < kD ? w1[(size_t)k * ff + grp * gw + nn] : 0.f; });
-        img.insert(img.end(), part.begin(), part.end());
-      }
-      if ((rc = upload(e, &ld.w1, img))) return rc;
-      auto img2 = pack_b(ff, kDP, [&](int k, int nn) { return nn < kD ? w2[(size_t)k * kD + nn] * alpha1 : 0.f; });
-      if ((rc = upload(e, &ld.w2, img2))) return rc;
-    }
-    if ((rc = upload(e, &ld.b1, std::vector<float>(b1, b1 + ff)))) return rc;
-    if ((rc = upload(e, &ld.b2, pad288(b2, alpha1)))) return rc;
-  }
-  // ---- head
-  {
-    const float* g = tm.get("model/encoder_stack/output_normalization/gamma", {kD}, &rc); if (rc) return rc;
-    const float* b = tm.get("model/encoder_stack/output_normalization/beta", {kD}, &rc); if (rc) return rc;
-    const float* w = tm.get("model/fc1/kernel", {kD, kVocab}, &rc); if (rc) return rc;
-    const float* bb = tm.get("model/fc1/bias", {kVocab}, &rc); if (rc) return rc;
-    if ((rc = upload(e, &e->d_fln_g, pad288(g)))) return rc;
-    if ((rc = upload(e, &e->d_fln_b, pad288(b)))) return rc;
-    if ((rc = upload(e, &e->d_wfc, std::vector<float>(w, w + kD * kVocab)))) return rc;
-    if ((rc = upload(e, &e->d_bfc, std::vector<float>(bb, bb + kVocab)))) return rc;
-    // head_kernel folds the final LayerNorm into the fc1 sums (one pass over the row): logits_j = rstd * (sum_c y_c g_c W_cj
-    // - mean_y * A_j) + B_j + bfc_j.  The products are formed here once, in float32.
-    std::vector<float> gw8((size_t)kD * 8, 0.f), ab(16, 0.f);
-    for (int cc = 0; cc < kD; ++cc)
-      for (int j = 0; j < kVocab; ++j) gw8[(size_t)cc * 8 + j] = g[cc] * w[cc * kVocab + j];
-    for (int j = 0; j < kVocab; ++j) {
-      float a = 0.f, bsum = 0.f;
-      for (int cc = 0; cc < kD; ++cc) { a += g[cc] * w[cc * kVocab + j]; bsum += b[cc] * w[cc * kVocab + j]; }
-      ab[j] = a; ab[8 + j] = bsum;
-    }
-    if ((rc = upload(e, &e->d_head_gw8, gw8))) return rc;
-    if ((rc = upload(e, &e->d_head_ab, ab))) return rc;
-  }
-  // ---- strict-fp32 path: every variable once more as float32, in the reference's own shapes
-  {
-    dcb_engine::Strict& S = e->strict;
-    std::vector<float> fblob;
-    std::vector<int> foff(tabs.size(), 0);
-    for (size_t t = 0; t < tabs.size(); ++t) {
-      if (t == 4 && !c.use_ccs_bq) continue;
-      const Tab& tb = tabs[t];
-      foff[t] = (int)fblob.size();
-      const float scale = sqrtf((float)tb.width);          // networks.py:54
-      for (int v = 0; v < tb.vocab; ++v)
-        for (int j = 0; j < tb.width; ++j) fblob.push_back(v == 0 ? 0.f : tb.data[v * tb.width + j] * scale);   // :58-63
-    }
-    std::vector<StrictEmbedRow> meta(e->R);
-    {
-      const int P = c.max_passes;
-      int col = 0, row = 0;
-      auto add = [&](int tab, int nrows, float clip, int shift) {
-        for (int r = 0; r < nrows; ++r) {
-          meta[row++] = StrictEmbedRow{clip, shift, tabs[tab].vocab, tabs[tab].width, col, foff[tab]};
-          col += tabs[tab].width;
-        }
-      };
-      add(0, P, 0.f, 0); add(1, P, (float)c.pw_max, 0); add(2, P, (float)c.ip_max, 0); add(3, P, 0.f, 0);
-      add(0, 1, 0.f, 0);
-      if (c.use_ccs_bq) add(4, 1, 0.f, 1);
-      add(5, 4, (float)c.sn_max, 0);
-      if (row != e->R || col != e->E) return fail(e, DCB_ERR_INVALID, "internal: strict embedding layout %d/%d", row, col);
-    }
-    if ((rc = upload(e, &S.meta, meta))) return rc;
-    if ((rc = upload(e, &S.tables, fblob))) return rc;
-    const float* wc = tm.get("model/transformer_input_condenser/kernel", {e->E, kD}, &rc); if (rc) return rc;
-    if ((rc = upload(e, &S.wc, std::vector<float>(wc, wc + (size_t)e->E * kD)))) return rc;
-    {
-      std::vector<float> pe((size_t)e->L * kD, 0.f);
-      if (c.add_pos_encoding) {
-        const int nt = kD / 2;
-        const float inc = (float)(log(1e4 / 1.0) / (double)(nt - 1));
-        for (int l = 0; l < e->L; ++l)
-          for (int k = 0; k < nt; ++k) {
-            const float sc = (float)l * expf((float)k * -inc);
-            pe[(size_t)l * kD + k] = sinf(sc);
-            pe[(size_t)l * kD + nt + k] = cosf(sc);
-          }
-      }
-      if ((rc = upload(e, &S.pe, pe))) return rc;
-    }
-    S.layers.assign(c.num_hidden_layers, dcb_engine::StrictLayer());
-    for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
-      dcb_engine::StrictLayer& sl = S.layers[n_];
-      char pre[128];
-      snprintf(pre, sizeof pre, "model/encoder_stack/layers/%d", n_);
-      const std::string P0 = std::string(pre) + "/0", P1 = std::string(pre) + "/1";
-      auto up = [&](float** dst, const std::string& name, std::initializer_list<int64_t> shape, size_t count) {
-        const float* src = tm.get(name, shape, &rc);
-        if (rc) return rc;
-        return rc = upload(e, dst, std::vector<float>(src, src + count));
-      };
-      if (c.rezero) {
-        sl.alpha[0] = *tm.get(P0 + "/alpha", std::initializer_list<int64_t>{}, &rc); if (rc) return rc;
-        sl.alpha[1] = *tm.get(P1 + "/alpha", std::initializer_list<int64_t>{}, &rc); if (rc) return rc;
-      } else {
-        for (int sidx = 0; sidx < 2; ++sidx) {
-          const std::string PP = sidx ? P1 : P0;
-          if (up(&sl.ln_g[sidx], PP + "/layer_norm/gamma", {kD}, kD)) return rc;
-          if (up(&sl.ln_b[sidx], PP + "/layer_norm/beta", {kD}, kD)) return rc;
-        }
-      }
-      if (up(&sl.wq, P0 + "/layer/query_dense_layer/kernel", {kD, kHeads, kDH}, (size_t)kD * kD)) return rc;
-      if (up(&sl.wk, P0 + "/layer/key_dense_layer/kernel", {kD, kHeads, kDH}, (size_t)kD * kD)) return rc;
-      if (up(&sl.wv, P0 + "/layer/value_dense_layer/kernel", {kD, kHeads, kDH}, (size_t)kD * kD)) return rc;
-      if (up(&sl.wo, P0 + "/layer/output_dense_layer/kernel", {kHeads, kDH, kD}, (size_t)kD * kD)) return rc;
-      if (up(&sl.w1, P1 + "/layer/filter_dense_layer/kernel", {kD, ff}, (size_t)kD * ff)) return rc;
-      if (up(&sl.b1, P1 + "/layer/filter_dense_layer/bias", {ff}, (size_t)ff)) return rc;
-      if (up(&sl.w2, P1 + "/layer/output_dense_layer/kernel", {ff, kD}, (size_t)ff * kD)) return rc;
-      if (up(&sl.b2, P1 + "/layer/output_dense_layer/bias", {kD}, (size_t)kD)) return rc;
-    }
-  }
-  CU(e, cudaDeviceSynchronize());
+  free_weights(e->w);
+  e->w = std::move(w);
   e->weights_loaded = true;
   return DCB_OK;
 }
@@ -648,33 +629,34 @@ static int strict_forward_chunk(dcb_engine* e, const float* rows_chunk, int bw, 
                                 cudaStream_t st) {
   const dcb_config& c = e->cfg;
   dcb_engine::Strict& S = e->strict;
+  const Weights& W = e->w;
   const int L = e->L, M = bw * L, ff = c.filter_size;
   int launches = 0;
-  launch_strict_embed(rows_chunk, e->R, L, e->E, bw, S.meta, S.tables, S.emb, d_status, st); ++launches;
+  launch_strict_embed(rows_chunk, e->R, L, e->E, bw, W.strict.embed, W.strict.tables, S.emb, d_status, st); ++launches;
   {
     StrictEpi ep;
-    if (c.add_pos_encoding) { ep.pe = S.pe; ep.pe_L = L; }
-    launch_strict_gemm(S.emb, S.wc, S.x, M, kD, e->E, ep, st); ++launches;            // networks.py:509-516, :319-323
+    if (c.add_pos_encoding) { ep.pe = W.strict.pe; ep.pe_L = L; }
+    launch_strict_gemm(S.emb, W.strict.wc, S.x, M, kD, e->E, ep, st); ++launches;            // networks.py:509-516, :319-323
   }
   const float qscale = 1.0f / sqrtf((float)kDH);                                       // attention_layer.py:196-197
   for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
-    const dcb_engine::StrictLayer& sl = S.layers[n_];
+    const LayerDev& ld = W.layers[n_];
     const float* yin = S.x;
-    if (!c.rezero) { launch_strict_layernorm(S.x, S.y, M, sl.ln_g[0], sl.ln_b[0], st); ++launches; yin = S.y; }
+    if (!c.rezero) { launch_strict_layernorm(S.x, S.y, M, ld.ln_g[0], ld.ln_b[0], st); ++launches; yin = S.y; }
     StrictEpi eq; eq.scale = qscale;
-    launch_strict_gemm(yin, sl.wq, S.q, M, kD, kD, eq, st);
-    launch_strict_gemm(yin, sl.wk, S.k, M, kD, kD, StrictEpi(), st);
-    launch_strict_gemm(yin, sl.wv, S.v, M, kD, kD, StrictEpi(), st);
+    launch_strict_gemm(yin, ld.strict.wq, S.q, M, kD, kD, eq, st);
+    launch_strict_gemm(yin, ld.strict.wk, S.k, M, kD, kD, StrictEpi(), st);
+    launch_strict_gemm(yin, ld.strict.wv, S.v, M, kD, kD, StrictEpi(), st);
     launch_strict_attention(S.q, S.k, S.v, S.att, bw, L, c.attn_win_size, st);
-    StrictEpi eo; eo.residual = S.x; eo.scale = c.rezero ? sl.alpha[0] : 1.f;         // encoder_stack.py:88-92
-    launch_strict_gemm(S.att, sl.wo, S.x, M, kD, kD, eo, st);
+    StrictEpi eo; eo.residual = S.x; eo.scale = c.rezero ? ld.strict.alpha[0] : 1.f;         // encoder_stack.py:88-92
+    launch_strict_gemm(S.att, ld.strict.wo, S.x, M, kD, kD, eo, st);
     launches += 5;
     yin = S.x;
-    if (!c.rezero) { launch_strict_layernorm(S.x, S.y, M, sl.ln_g[1], sl.ln_b[1], st); ++launches; yin = S.y; }
-    StrictEpi e1; e1.bias = sl.b1; e1.relu = 1;                                        // ffn_layer.py:83-86
-    launch_strict_gemm(yin, sl.w1, S.hid, M, ff, kD, e1, st);
-    StrictEpi e2; e2.bias = sl.b2; e2.residual = S.x; e2.scale = c.rezero ? sl.alpha[1] : 1.f;
-    launch_strict_gemm(S.hid, sl.w2, S.x, M, kD, ff, e2, st);
+    if (!c.rezero) { launch_strict_layernorm(S.x, S.y, M, ld.ln_g[1], ld.ln_b[1], st); ++launches; yin = S.y; }
+    StrictEpi e1; e1.bias = ld.b1; e1.relu = 1;                                        // ffn_layer.py:83-86
+    launch_strict_gemm(yin, ld.strict.w1, S.hid, M, ff, kD, e1, st);
+    StrictEpi e2; e2.bias = ld.strict.b2; e2.residual = S.x; e2.scale = c.rezero ? ld.strict.alpha[1] : 1.f;
+    launch_strict_gemm(S.hid, ld.strict.w2, S.x, M, kD, ff, e2, st);
     launches += 2;
   }
   HeadParams h = hp;
@@ -809,8 +791,8 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
   };
   auto make_head_at = [&](int w0) {
     HeadParams hp{};
-    hp.x = e->d_x; hp.ln_g = e->d_fln_g; hp.ln_b = e->d_fln_b; hp.wfc = e->d_wfc; hp.bfc = e->d_bfc;
-    hp.gw8 = e->d_head_gw8; hp.ab = e->d_head_ab;
+    hp.x = e->d_x; hp.ln_g = e->w.fln_g; hp.ln_b = e->w.fln_b; hp.wfc = e->w.wfc; hp.bfc = e->w.bfc;
+    hp.gw8 = e->w.head_gw8; hp.ab = e->w.head_ab;
     const size_t t0 = (size_t)w0 * L;
     hp.bases = (out_dev ? bases_out : sl.d_bases) + t0;
     hp.quals = (out_dev ? quals_out : sl.d_quals) + t0;
@@ -855,23 +837,23 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
     {
       RowEpi epi{};
       epi.x = e->d_x; epi.xb = e->d_xb; epi.bias = nullptr;
-      epi.pe = c.add_pos_encoding ? e->d_pe : nullptr;
-      epi.pe_img = c.add_pos_encoding ? e->d_pe_img : nullptr;
-      epi.ln_g = c.rezero ? nullptr : e->layers[0].ln_g[0];
-      epi.ln_b = c.rezero ? nullptr : e->layers[0].ln_b[0];
+      epi.pe = c.add_pos_encoding ? e->w.pe : nullptr;
+      epi.pe_img = c.add_pos_encoding ? e->w.pe_img : nullptr;
+      epi.ln_g = c.rezero ? nullptr : e->w.layers[0].ln_g[0];
+      epi.ln_b = c.rezero ? nullptr : e->w.layers[0].ln_b[0];
       epi.has_xold = 0; epi.L = Lw;
       pbegin(0);
       launch_embed(packed_base ? nullptr : rows_chunk, packed_base ? packed_base + (size_t)w0 * e->pl.stride : nullptr, e->pl,
-                   R, L, Lw, M, T, e->echunks, e->d_cols, e->d_rowmeta, e->d_tables, e->table_elems, e->d_embqkv, sl.d_status, st);
+                   R, L, Lw, M, T, e->echunks, e->w.cols, e->w.rowmeta, e->w.tables, e->table_elems, e->d_embqkv, sl.d_status, st);
       pend();
       pbegin(1);
-      launch_gemm_row(e->d_embqkv, e->d_wc, e->Epad / 16, 2 * (e->Epad / 16), T, epi, st);
+      launch_gemm_row(e->d_embqkv, e->w.wc, e->Epad / 16, 2 * (e->Epad / 16), T, epi, st);
       pend();
       launches += 2;
       snap();
     }
     for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
-      const LayerDev& ld = e->layers[n_];
+      const LayerDev& ld = e->w.layers[n_];
       const bool last = n_ + 1 == c.num_hidden_layers;
       pbegin(2);
       launch_gemm_qkv(e->d_xb, ld.wqkv, T, e->d_embqkv, st);
@@ -892,8 +874,8 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
       // FFN: hidden = relu(xb W1 + b1), then hidden W2 + b2 + residual; xb = the next layer's input
       RowEpi ef{};
       ef.x = e->d_x; ef.xb = last ? nullptr : e->d_xb; ef.bias = ld.b2; ef.pe = nullptr;
-      ef.ln_g = (c.rezero || last) ? nullptr : e->layers[n_ + 1].ln_g[0];
-      ef.ln_b = (c.rezero || last) ? nullptr : e->layers[n_ + 1].ln_b[0];
+      ef.ln_g = (c.rezero || last) ? nullptr : e->w.layers[n_ + 1].ln_g[0];
+      ef.ln_b = (c.rezero || last) ? nullptr : e->w.layers[n_ + 1].ln_b[0];
       ef.has_xold = 1; ef.L = Lw;
       pbegin(4);
       launch_ffn_up(e->d_xb, ld.w1, ld.b1, c.filter_size, T, e->d_hid, st);

@@ -511,6 +511,37 @@ def test_initialize_model_from_a_tf_checkpoint(engine_mod, tmp_path):
     inference.initialize_model(str(tmp_path / "checkpoint-5"), p.copy(), opts)
 
 
+def test_failed_weight_load_keeps_the_previous_weights(engine_mod, monkeypatch):
+  """dcb_load_weights checks every variable before it touches the device and replaces the weights as one unit: a
+  checkpoint missing its last variable is refused and the engine keeps computing with the previous one; a complete
+  reload then gives exactly what a fresh engine built with the new checkpoint gives, on both paths."""
+  p = params_lib.synthetic_params(20, 100, use_ccs_bq=True, num_hidden_layers=2, rezero=False)
+  wa, wb = weights_lib.init_weights(p, seed=61), weights_lib.init_weights(p, seed=62)
+  rows = synthetic.make_rows(p, 6, seed=63)
+  model = engine_mod.B200Model(p, wa, max_batch=6)
+  first = [model.forward(rows, want_logits=True, strict=s) for s in (False, True)]
+  partial = {k: v for k, v in wb.items() if k != "model/fc1/bias"}
+  with monkeypatch.context() as mp:
+    mp.setattr(weights_lib, "check_weights", lambda *a, **k: None)     # the engine's own check, not the Python one
+    with pytest.raises(engine_mod.DcbError, match="missing variable model/fc1/bias") as ei:
+      model.load_weights(partial)
+  assert ei.value.code == -3
+  for s, want in zip((False, True), first):
+    got = model.forward(rows, want_logits=True, strict=s)
+    for k in ("bases", "quals", "logits"):
+      assert np.array_equal(got[k], want[k]), (s, k)
+  model.load_weights(wb)
+  fresh = engine_mod.B200Model(p, wb, max_batch=6)
+  for s, old in zip((False, True), first):
+    got = model.forward(rows, want_logits=True, strict=s)
+    want = fresh.forward(rows, want_logits=True, strict=s)
+    assert not np.array_equal(got["logits"], old["logits"])
+    for k in ("bases", "quals", "logits"):
+      assert np.array_equal(got[k], want[k]), (s, k)
+  fresh.close()
+  model.close()
+
+
 def test_unfused_fallback_paths_agree_with_fused(engine_mod):
   """DCB_ALIGN / DCB_CHUNK_TILES select alternative token layouts and chunkings of the same math.  They exist only in
   the developer build (libdcb200_dev.so, -DDCB_DEV_SWITCHES) and are read when an engine is created; the product
