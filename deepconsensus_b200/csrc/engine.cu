@@ -11,6 +11,7 @@
 #include <cmath>
 #include <functional>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -24,6 +25,37 @@ namespace {
 
 thread_local std::string g_create_error;
 
+// Device memory of `cap` elements that the engine owns: freed by the destructor.  Every device allocation the engine
+// makes for itself lives in one of these (allocated by alloc() or ensure() below).
+template <typename T>
+struct DevBuf {
+  T* p = nullptr;
+  size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    if (this != &o) { reset(); std::swap(p, o.p); std::swap(cap, o.cap); }
+    return *this;
+  }
+  ~DevBuf() { reset(); }
+  operator T*() const { return p; }
+  void reset() {
+    if (p) cudaFree(p);
+    p = nullptr;
+    cap = 0;
+  }
+  // a new block of n elements in place of the old one (contents undefined)
+  cudaError_t reallocate(size_t n) {
+    reset();
+    const cudaError_t st = cudaMalloc(reinterpret_cast<void**>(&p), n * sizeof(T));
+    if (st == cudaSuccess) cap = n;
+    else p = nullptr;
+    return st;
+  }
+};
+
 // One embedding table of the checkpoint (networks.py:375-421) and its element offset in the table blob.  The blob's
 // tables start 16-byte aligned as bf16 (the embed kernel's width-8 fast path); the float32 blob uses the same offsets.
 struct EmbedTable {
@@ -32,37 +64,38 @@ struct EmbedTable {
 };
 
 struct LayerDev {
-  __nv_bfloat16* wqkv = nullptr;  // 6 groups x split-bf16 [72][144][8]: q_h0, q_h1, k_h0, k_h1, v_h0, v_h1
-  __nv_bfloat16* wo = nullptr;    // split-bf16 [72][288][8]
-  __nv_bfloat16* w1 = nullptr;    // ff / kFFChunk groups x [36][kFFChunk][8]
-  __nv_bfloat16* w2 = nullptr;    // [ff/8][288][8] (ReZero alpha folded in)
-  float* b1 = nullptr;            // [ff] (both paths)
-  float* b2 = nullptr;            // [288] (gain folded)
-  float* ln_g[2] = {nullptr, nullptr};  // [288] pre-norm gamma/beta of the attention / FFN sub-layer (both paths)
-  float* ln_b[2] = {nullptr, nullptr};
+  DevBuf<__nv_bfloat16> wqkv;   // 6 groups x split-bf16 [72][144][8]: q_h0, q_h1, k_h0, k_h1, v_h0, v_h1
+  DevBuf<__nv_bfloat16> wo;     // split-bf16 [72][288][8]
+  DevBuf<__nv_bfloat16> w1;     // ff / kFFChunk groups x [36][kFFChunk][8]
+  DevBuf<__nv_bfloat16> w2;     // [ff/8][288][8] (ReZero alpha folded in)
+  DevBuf<float> b1;             // [ff] (both paths)
+  DevBuf<float> b2;             // [288] (gain folded)
+  DevBuf<float> ln_g[2], ln_b[2];   // [288] pre-norm gamma/beta of the attention / FFN sub-layer (both paths)
   struct {   // strict-fp32 path (strict_kernels.cu): float32 in the reference's own shapes
-    float *wq = nullptr, *wk = nullptr, *wv = nullptr, *wo = nullptr, *w1 = nullptr, *w2 = nullptr, *b2 = nullptr;
+    DevBuf<float> wq, wk, wv, wo, w1, w2, b2;
     float alpha[2] = {1.f, 1.f};
   } strict;
 };
 
 // The device copy of one checkpoint.  dcb_load_weights builds a complete new set before it frees the previous one.
 struct Weights {
-  EmbedCol* cols = nullptr;
-  EmbedRow* rowmeta = nullptr;
-  __nv_bfloat16* tables = nullptr;
-  __nv_bfloat16* wc = nullptr;   // split-bf16 condenser [2 Epad / 8][288][8]
-  float* pe = nullptr;           // positional table [Lw][288]
-  float* pe_img = nullptr;       // same table in residual-image order (window-aligned layout only)
+  DevBuf<EmbedCol> cols;
+  DevBuf<EmbedRow> rowmeta;
+  DevBuf<__nv_bfloat16> tables;
+  DevBuf<__nv_bfloat16> wc;   // split-bf16 condenser [2 Epad / 8][288][8]
+  DevBuf<float> pe;           // positional table [Lw][288]
+  DevBuf<float> pe_img;       // same table in residual-image order (window-aligned layout only)
   std::vector<LayerDev> layers;
-  float *fln_g = nullptr, *fln_b = nullptr, *wfc = nullptr, *bfc = nullptr;   // final LayerNorm [288], fc1 (both paths)
-  float *head_gw8 = nullptr, *head_ab = nullptr;   // head_kernel: gamma * Wfc (padded to 8) and the A / B sums
+  DevBuf<float> fln_g, fln_b, wfc, bfc;   // final LayerNorm [288], fc1 (both paths)
+  DevBuf<float> head_gw8, head_ab;        // head_kernel: gamma * Wfc (padded to 8) and the A / B sums
   struct {   // strict-fp32 path
-    StrictEmbedRow* embed = nullptr;
-    float *tables = nullptr, *wc = nullptr, *pe = nullptr;   // pe: [L][280]
+    DevBuf<StrictEmbedRow> embed;
+    DevBuf<float> tables, wc, pe;   // pe: [L][280]
   } strict;
-  std::vector<void*> owned;
 };
+
+// Kernel classes of the forward's profile, in dcb_get_profile_kernels' order.
+enum ProfKind { kProfEmbed, kProfRowGemm, kProfQkv, kProfAttention, kProfFfn, kProfHead, kProfKinds };
 
 }  // namespace
 
@@ -79,28 +112,26 @@ struct dcb_engine {
   // Two-deep submission pipeline (dcb_submit / dcb_wait): only the input rows and the status word are per slot; every
   // other buffer is reused in stream order.
   struct Slot {
-    float* d_rows = nullptr;
-    uint8_t* d_packed = nullptr;        // packed rows of a dcb_submit_packed call (allocated on first use)
-    uint8_t *d_bases = nullptr, *d_quals = nullptr;   // per slot: the results of batch i are copied out on `out_stream`
-    float *d_probs = nullptr, *d_logits = nullptr;    // while the kernels of batch i+1 already write the other slot's
-    int* d_status = nullptr;
+    DevBuf<float> d_rows;
+    DevBuf<uint8_t> d_packed;           // packed rows of a dcb_submit_packed call (allocated on first use)
+    DevBuf<uint8_t> d_bases, d_quals;   // per slot: the results of batch i are copied out on `out_stream`
+    DevBuf<float> d_probs, d_logits;    // while the kernels of batch i+1 already write the other slot's
+    DevBuf<int> d_status;
     int* h_status = nullptr;            // pinned
     cudaEvent_t rows_ready = nullptr, ev0 = nullptr, ev1 = nullptr, done = nullptr;
     bool busy = false, used = false;
     int64_t ticket = -1;
     int launches = 0;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events;  // around every launch when profiling
-    std::vector<int> prof_kind;                                    // kernel class of each event pair
+    std::vector<ProfKind> prof_kind;                               // kernel class of each event pair
     size_t prof_used = 0;
   } slots[2];
   int64_t next_ticket = 0;
   bool weights_loaded = false;
   bool debug = false;
   bool profile = false;
-  float prof_ms[6] = {0, 0, 0, 0, 0, 0};   // embed, gemm_row, qkv, attention, ffn, head
-  int prof_n[6] = {0, 0, 0, 0, 0, 0};
-  float prof_ffn_ms = 0.f;
-  int prof_ffn_launches = 0;
+  float prof_ms[kProfKinds] = {};   // per ProfKind
+  int prof_n[kProfKinds] = {};
   long long prof_ffn_tokens = 0;
   float last_ms = 0.f;
   int last_launches = 0;
@@ -111,32 +142,51 @@ struct dcb_engine {
   int table_elems = 0;
   Weights w;
   // workspace
-  __nv_bfloat16* d_embqkv = nullptr;
-  float* d_x = nullptr;
-  __nv_bfloat16* d_xb = nullptr;
-  __nv_bfloat16* d_att = nullptr;
-  __nv_bfloat16* d_hid = nullptr;   // FFN hidden activation, bf16 operand image [tile][ff/8][128][8]
-  // stitch scratch (grown on demand)
-  uint8_t *d_st_in = nullptr, *d_st_out = nullptr;   // [2][cap] each: bases|quals, seq|qual
-  int32_t *d_st_start = nullptr, *d_st_len = nullptr;
-  size_t st_cap = 0, st_zcap = 0;
-  // post-model stage scratch (dcb_stitch_fastq / dcb_skip_mask / dcb_fill_skipped), grown on demand
-  double* d_p10 = nullptr;           // 10^(-q/10), q = 0..255 (host libm pow, as NumPy)
-  struct Scratch { void* p = nullptr; size_t cap = 0; } sc_pos, sc_names, sc_nameoff, sc_outcome, sc_avg, sc_recoff, sc_fastq,
-      sc_bq, sc_mask, sc_ids, sc_dst, sc_tmpb, sc_tmpq,
-      sc_ev_probs, sc_ev_in, sc_ev_out,   // dcb_evaluate: host probs, labels | ccs ids, loss | counts | flags
-      sc_ds_in, sc_ds_out,                // dcb_distill_loss: host teacher | student logits, loss
-      sc_lg_in, sc_lg_out, sc_lg_dp,      // dcb_alignment_loss_grad: host probs | labels, loss | grad | matches, DP tables
-      sc_he_in, sc_he_out;                // dcb_debug_head_epilogue: logits + zero bias | probs, bases, quals
-  cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;
-  float* d_dbg = nullptr;  // [stages][chunk_tiles * x_image]
-  __nv_bfloat16* d_dbg_op = nullptr;   // bf16 operand images per stage (dbg_operand_slot)
+  DevBuf<__nv_bfloat16> d_embqkv;
+  DevBuf<float> d_x;
+  DevBuf<__nv_bfloat16> d_xb;
+  DevBuf<__nv_bfloat16> d_att;
+  DevBuf<__nv_bfloat16> d_hid;   // FFN hidden activation, bf16 operand image [tile][ff/8][128][8]
+  DevBuf<double> d_p10;          // 10^(-q/10), q = 0..255 (host libm pow, as NumPy)
+  DevBuf<float> d_dbg;           // [stages][chunk_tiles * x_image]
+  DevBuf<__nv_bfloat16> d_dbg_op;   // bf16 operand images per stage (dbg_operand_slot)
   // strict-fp32 path (strict_kernels.cu): row-major workspace, allocated on the first strict call
   struct Strict {
-    float *emb = nullptr, *x = nullptr, *y = nullptr, *q = nullptr, *k = nullptr, *v = nullptr, *att = nullptr, *hid = nullptr;
-    int chunk_windows = 0;
+    DevBuf<float> emb, x, y, q, k, v, att, hid;
+    int chunk_windows = 0;   // 0 until the workspace is allocated
   } strict;
-  std::vector<void*> owned;   // workspace
+  // Host-or-device staging of the entry points besides the forward, one buffer per array, grown on demand (ensure,
+  // stage_in, stage_out).  Every such call ends with a stream synchronisation, so the next one may reuse them.
+  struct {   // dcb_stitch, dcb_stitch_fastq
+    DevBuf<uint8_t> bases, quals, seq, qual, names, fastq;
+    DevBuf<int32_t> start, len, pos, name_off, outcome;
+    DevBuf<int64_t> rec_off;
+    DevBuf<double> avg_q;
+  } st;
+  struct { DevBuf<int16_t> bq; DevBuf<uint8_t> mask; DevBuf<double> avg; } sk;   // dcb_skip_mask
+  struct { DevBuf<uint8_t> ids, bases, quals; DevBuf<int16_t> bq; DevBuf<int32_t> dst; DevBuf<int> status; } fs;   // dcb_fill_skipped
+  struct { DevBuf<float> probs, loss; DevBuf<uint8_t> labels, ccs, exact; DevBuf<int32_t> pred, ccs_counts; } ev;   // dcb_evaluate
+  struct { DevBuf<float> teacher, student, loss; } ds;   // dcb_distill_loss
+  struct { DevBuf<float> probs, loss, grad, matches, dp; DevBuf<uint8_t> labels; } lg;   // dcb_alignment_loss_grad
+  struct { DevBuf<float> bias, logits, probs; DevBuf<uint8_t> bases, quals; } he;   // dcb_debug_head_epilogue
+  cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;   // around the kernel of dcb_evaluate / _distill_loss / _loss_grad
+
+  // Safe on a partly built engine.  The caller has made cfg.device current; the DevBuf members free themselves after
+  // the streams have drained.
+  ~dcb_engine() {
+    for (cudaStream_t s : {copy_stream, stream, out_stream})
+      if (s) cudaStreamSynchronize(s);
+    std::vector<cudaEvent_t> events = {ev_eval0, ev_eval1};
+    for (Slot& sl : slots) {
+      events.insert(events.end(), {sl.rows_ready, sl.ev0, sl.ev1, sl.done});
+      for (auto& pr : sl.prof_events) events.insert(events.end(), {pr.first, pr.second});
+      if (sl.h_status) cudaFreeHost(sl.h_status);
+    }
+    for (cudaEvent_t ev : events)
+      if (ev) cudaEventDestroy(ev);
+    for (cudaStream_t s : {copy_stream, out_stream, stream})
+      if (s) cudaStreamDestroy(s);
+  }
 };
 
 namespace {
@@ -167,25 +217,68 @@ void set_head_quality(HeadParams& hp, const dcb_config& c) {
                   __FILE__, __LINE__);                                                  \
   } while (0)
 
-// n zeroed elements, freed with the allocations in `owned` (the engine's workspace or one weight set)
+// n zeroed elements (the operand images' padding columns rely on the zeros).  cudaMemset runs on the legacy default
+// stream, which the engine's non-blocking streams do not wait for, so the fill completes before the buffer is used.
 template <typename T>
-int dev_alloc(dcb_engine* e, std::vector<void*>& owned, T** p, size_t n) {
-  CU(e, cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)));
-  owned.push_back(*p);
-  CU(e, cudaMemset(*p, 0, n * sizeof(T)));
+int alloc(dcb_engine* e, DevBuf<T>& b, size_t n) {
+  CU(e, b.reallocate(n));
+  CU(e, cudaMemset(b.p, 0, n * sizeof(T)));
+  CU(e, cudaStreamSynchronize(cudaStreamLegacy));
   return DCB_OK;
 }
 
 template <typename T>
-int dev_alloc(dcb_engine* e, T** p, size_t n) {
-  return dev_alloc(e, e->owned, p, n);
+int upload(dcb_engine* e, DevBuf<T>& b, const std::vector<T>& h) {
+  int rc = alloc(e, b, h.size());
+  if (rc) return rc;
+  CU(e, cudaMemcpy(b.p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
+  return DCB_OK;
+}
+
+// At least n elements, grown on demand; contents are not preserved.  A kernel on the compute stream may still read the
+// old block, so the stream drains before it is freed.
+template <typename T>
+int ensure(dcb_engine* e, DevBuf<T>& b, size_t n) {
+  if (n <= b.cap) return DCB_OK;
+  CU(e, cudaStreamSynchronize(e->stream));
+  CU(e, b.reallocate(n));
+  return DCB_OK;
+}
+
+// A host-or-device input of n elements: *d = src when the caller's array is on the device, else src copied into b on
+// the compute stream.
+template <typename T>
+int stage_in(dcb_engine* e, DevBuf<T>& b, const T* src, size_t n, bool on_device, const T** d) {
+  *d = src;
+  if (on_device) return DCB_OK;
+  int rc = ensure(e, b, n);
+  if (rc) return rc;
+  if (n) CU(e, cudaMemcpyAsync(b.p, src, n * sizeof(T), cudaMemcpyHostToDevice, e->stream));
+  *d = b.p;
+  return DCB_OK;
+}
+
+// A host-or-device output of n elements: the kernel writes `d`, and copy_out brings it to the caller's host array.
+template <typename T>
+struct Output {
+  T* d = nullptr;
+  T* host = nullptr;   // null when the kernel writes the caller's device array, or the caller wants no such output
+  size_t n = 0;
+};
+
+template <typename T>
+int stage_out(dcb_engine* e, DevBuf<T>& b, T* dst, size_t n, bool on_device, Output<T>* o) {
+  *o = Output<T>{dst, nullptr, n};
+  if (on_device || !dst) return DCB_OK;
+  int rc = ensure(e, b, n);
+  if (rc) return rc;
+  *o = Output<T>{b.p, dst, n};
+  return DCB_OK;
 }
 
 template <typename T>
-int upload(dcb_engine* e, std::vector<void*>& owned, T** p, const std::vector<T>& h) {
-  int rc = dev_alloc(e, owned, p, h.size());
-  if (rc) return rc;
-  CU(e, cudaMemcpy(*p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
+int copy_out(dcb_engine* e, const Output<T>& o) {
+  if (o.host && o.n) CU(e, cudaMemcpyAsync(o.host, o.d, o.n * sizeof(T), cudaMemcpyDeviceToHost, e->stream));
   return DCB_OK;
 }
 
@@ -281,17 +374,12 @@ int read_checkpoint(dcb_engine* e, const dcb_tensor* tensors, int n, Checkpoint*
   return rc;
 }
 
-void free_weights(Weights& w) {
-  for (void* p : w.owned) cudaFree(p);
-  w = Weights();
-}
-
-// Both paths' device weights from a validated checkpoint, allocated in w->owned.
+// Both paths' device weights from a validated checkpoint.
 int upload_weights(dcb_engine* e, const Checkpoint& ck, Weights* w) {
   const dcb_config& c = e->cfg;
   int rc = DCB_OK;   // the first failure: later uploads are skipped
-  auto up = [&](auto** p, const auto& h) { if (!rc) rc = upload(e, w->owned, p, h); };
-  auto copy = [&](float** p, const float* src, size_t n) { up(p, std::vector<float>(src, src + n)); };
+  auto up = [&](auto& b, const auto& h) { if (!rc) rc = upload(e, b, h); };
+  auto copy = [&](DevBuf<float>& b, const float* src, size_t n) { up(b, std::vector<float>(src, src + n)); };
 
   // ---- embedding tables (networks.py:375-421), pre-scaled by sqrt(width), row 0 zeroed
   //      (ModifiedOnDeviceEmbedding, networks.py:42-63); the bf16 blob is the float32 blob rounded
@@ -312,17 +400,17 @@ int upload_weights(dcb_engine* e, const Checkpoint& ck, Weights* w) {
     for (int j = 0; j < m.width; ++j)
       cols[m.col0 + j] = EmbedCol{(int16_t)r, (int16_t)m.width, (int16_t)j, (int16_t)m.shift, m.table_off, m.vocab, m.clip_hi};
   }
-  up(&w->tables, blob16);
-  up(&w->rowmeta, rowmeta);
-  up(&w->cols, cols);
-  up(&w->strict.tables, blob);
-  up(&w->strict.embed, e->embed);
+  up(w->tables, blob16);
+  up(w->rowmeta, rowmeta);
+  up(w->cols, cols);
+  up(w->strict.tables, blob);
+  up(w->strict.embed, e->embed);
   // ---- condenser (networks.py:426-434): B image [Epad/8][288][8]
   {
     const int E = e->E;
     auto img = pack_b_split(e->Epad, kDP, [&](int k, int nn) { return (k < E && nn < kD) ? ck.wc[(size_t)k * kD + nn] : 0.f; });
-    up(&w->wc, img);
-    copy(&w->strict.wc, ck.wc, (size_t)E * kD);
+    up(w->wc, img);
+    copy(w->strict.wc, ck.wc, (size_t)E * kD);
   }
   // ---- positional encoding table [Lw][288] (tf-models RelativePositionEmbedding; networks.py:301-323)
   {
@@ -338,29 +426,29 @@ int upload_weights(dcb_engine* e, const Checkpoint& ck, Weights* w) {
           pe[(size_t)l * kDP + nt + k] = cosf(sc);
         }
     }
-    up(&w->pe, pe);
+    up(w->pe, pe);
     if (e->Lw == kTileM) {
       // window-aligned layout: every tile sees positions 0..127, so the table can also be laid out like the residual
       // image [72][128][4] -- a warp of the row epilogue then reads 512 contiguous bytes instead of 32 scattered rows
       std::vector<float> img((size_t)kTileM * kDP, 0.f);
       for (int l = 0; l < kTileM; ++l)
         for (int col = 0; col < kDP; ++col) img[((size_t)(col / 4) * kTileM + l) * 4 + (col & 3)] = pe[(size_t)l * kDP + col];
-      up(&w->pe_img, img);
+      up(w->pe_img, img);
     }
     std::vector<float> pe_strict((size_t)e->L * kD);   // the strict GEMM epilogue reads [L][280]
     for (int l = 0; l < e->L; ++l) std::copy_n(&pe[(size_t)l * kDP], kD, &pe_strict[(size_t)l * kD]);
-    up(&w->strict.pe, pe_strict);
+    up(w->strict.pe, pe_strict);
   }
   // ---- encoder layers
   const int ff = c.filter_size;
-  w->layers.assign(c.num_hidden_layers, LayerDev());
+  w->layers.resize(c.num_hidden_layers);
   for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
     LayerDev& ld = w->layers[n_];
     const Checkpoint::Layer& l = ck.layers[n_];
     const float alpha0 = l.alpha[0], alpha1 = l.alpha[1];
     for (int s = 0; s < 2 && !c.rezero; ++s) {
-      up(&ld.ln_g[s], pad288(l.ln_g[s]));
-      up(&ld.ln_b[s], pad288(l.ln_b[s]));
+      up(ld.ln_g[s], pad288(l.ln_g[s]));
+      up(ld.ln_b[s], pad288(l.ln_b[s]));
     }
     const float qscale = 1.0f / sqrtf((float)kDH);  // query *= depth**-0.5 (attention_layer.py:196-197)
     {
@@ -378,7 +466,7 @@ int upload_weights(dcb_engine* e, const Checkpoint& ck, Weights* w) {
         });
         img.insert(img.end(), part.begin(), part.end());
       }
-      up(&ld.wqkv, img);
+      up(ld.wqkv, img);
     }
     {
       // out-proj: K index = head*144 + dd, N = e; ReZero alpha folded in (encoder_stack.py:88-90)
@@ -387,7 +475,7 @@ int upload_weights(dcb_engine* e, const Checkpoint& ck, Weights* w) {
         if (dd >= kDH || nn >= kD) return 0.f;
         return l.wo[((size_t)head * kDH + dd) * kD + nn] * alpha0;
       });
-      up(&ld.wo, img);
+      up(ld.wo, img);
     }
     {
       // W1 in n-groups of kFFChunk hidden units, W2 as one [ff/8][288][8] image (ReZero alpha folded in)
@@ -398,28 +486,28 @@ int upload_weights(dcb_engine* e, const Checkpoint& ck, Weights* w) {
         auto part = pack_b(kDP, gw, [&](int k, int nn) { return k < kD ? l.w1[(size_t)k * ff + grp * gw + nn] : 0.f; });
         img.insert(img.end(), part.begin(), part.end());
       }
-      up(&ld.w1, img);
+      up(ld.w1, img);
       auto img2 = pack_b(ff, kDP, [&](int k, int nn) { return nn < kD ? l.w2[(size_t)k * kD + nn] * alpha1 : 0.f; });
-      up(&ld.w2, img2);
+      up(ld.w2, img2);
     }
-    copy(&ld.b1, l.b1, ff);
-    up(&ld.b2, pad288(l.b2, alpha1));
+    copy(ld.b1, l.b1, ff);
+    up(ld.b2, pad288(l.b2, alpha1));
     // the strict path: every matrix once more as float32, in the reference's own shapes
     ld.strict.alpha[0] = alpha0;
     ld.strict.alpha[1] = alpha1;
-    copy(&ld.strict.wq, l.wq, (size_t)kD * kD);
-    copy(&ld.strict.wk, l.wk, (size_t)kD * kD);
-    copy(&ld.strict.wv, l.wv, (size_t)kD * kD);
-    copy(&ld.strict.wo, l.wo, (size_t)kD * kD);
-    copy(&ld.strict.w1, l.w1, (size_t)kD * ff);
-    copy(&ld.strict.w2, l.w2, (size_t)ff * kD);
-    copy(&ld.strict.b2, l.b2, kD);
+    copy(ld.strict.wq, l.wq, (size_t)kD * kD);
+    copy(ld.strict.wk, l.wk, (size_t)kD * kD);
+    copy(ld.strict.wv, l.wv, (size_t)kD * kD);
+    copy(ld.strict.wo, l.wo, (size_t)kD * kD);
+    copy(ld.strict.w1, l.w1, (size_t)kD * ff);
+    copy(ld.strict.w2, l.w2, (size_t)ff * kD);
+    copy(ld.strict.b2, l.b2, kD);
   }
   // ---- head
-  up(&w->fln_g, pad288(ck.fln_g));
-  up(&w->fln_b, pad288(ck.fln_b));
-  copy(&w->wfc, ck.wfc, kD * kVocab);
-  copy(&w->bfc, ck.bfc, kVocab);
+  up(w->fln_g, pad288(ck.fln_g));
+  up(w->fln_b, pad288(ck.fln_b));
+  copy(w->wfc, ck.wfc, kD * kVocab);
+  copy(w->bfc, ck.bfc, kVocab);
   {
     // head_kernel folds the final LayerNorm into the fc1 sums (one pass over the row): logits_j = rstd * (sum_c y_c g_c W_cj
     // - mean_y * A_j) + B_j + bfc_j.  The products are formed here once, in float32.
@@ -432,8 +520,8 @@ int upload_weights(dcb_engine* e, const Checkpoint& ck, Weights* w) {
       for (int cc = 0; cc < kD; ++cc) { a += g[cc] * wf[cc * kVocab + j]; bsum += b[cc] * wf[cc * kVocab + j]; }
       ab[j] = a; ab[8 + j] = bsum;
     }
-    up(&w->head_gw8, gw8);
-    up(&w->head_ab, ab);
+    up(w->head_gw8, gw8);
+    up(w->head_ab, ab);
   }
   if (rc) return rc;
   // the uploads have landed before any kernel on the engine's (non-blocking) streams reads them, and no kernel still
@@ -476,7 +564,8 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
     return fail(nullptr, DCB_ERR_CUDA, "device %d is not an sm_90 GPU (compute capability %d.%d)", cfg->device,
                 prop.major, prop.minor);
 
-  dcb_engine* e = new dcb_engine();
+  std::unique_ptr<dcb_engine> eng(new dcb_engine());
+  dcb_engine* e = eng.get();
   e->cfg = *cfg;
   e->num_sms = prop.multiProcessorCount;
   e->L = cfg->max_length;
@@ -527,79 +616,50 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
   e->chunk_windows = std::max(1, std::min(cfg->max_batch, ct * kTileM / e->Lw));
   e->chunk_tiles = std::min(max_tiles, (e->chunk_windows * e->Lw + kTileM - 1) / kTileM);
 
-  auto bail = [&](int rc) { std::string m = e->err; dcb_destroy(e); g_create_error = m; return rc; };
-#define TRY(x) do { int _rc = (x); if (_rc) return bail(_rc); } while (0)
-#define CUC(call) do { cudaError_t _s = (call); if (_s != cudaSuccess) { fail(e, DCB_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(_s)); return bail(DCB_ERR_CUDA); } } while (0)
-  CUC(cudaSetDevice(cfg->device));
-  CUC(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
-  CUC(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-  CUC(cudaStreamCreateWithFlags(&e->out_stream, cudaStreamNonBlocking));
-  for (auto& sl : e->slots) {
-    CUC(cudaEventCreateWithFlags(&sl.rows_ready, cudaEventDisableTiming));
-    CUC(cudaEventCreate(&sl.ev0));
-    CUC(cudaEventCreate(&sl.ev1));
-    CUC(cudaEventCreateWithFlags(&sl.done, cudaEventDisableTiming));
-    CUC(cudaMallocHost(reinterpret_cast<void**>(&sl.h_status), sizeof(int)));
-  }
-  CUC(kernels_init());
-  {
+  // on failure the engine's destructor releases what was built, and its message becomes the create error
+  const int rc = [&]() -> int {
+    CU(e, cudaSetDevice(cfg->device));
+    CU(e, cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
+    CU(e, cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
+    CU(e, cudaStreamCreateWithFlags(&e->out_stream, cudaStreamNonBlocking));
+    for (auto& sl : e->slots) {
+      CU(e, cudaEventCreateWithFlags(&sl.rows_ready, cudaEventDisableTiming));
+      CU(e, cudaEventCreate(&sl.ev0));
+      CU(e, cudaEventCreate(&sl.ev1));
+      CU(e, cudaEventCreateWithFlags(&sl.done, cudaEventDisableTiming));
+      CU(e, cudaMallocHost(reinterpret_cast<void**>(&sl.h_status), sizeof(int)));
+    }
+    CU(e, cudaEventCreate(&e->ev_eval0));
+    CU(e, cudaEventCreate(&e->ev_eval1));
+    CU(e, kernels_init());
     std::vector<double> p10(256);
     for (int q = 0; q < 256; ++q) p10[q] = pow(10.0, (double)q / -10.0);    // utils.py:103: 10 ** (q / -10.0)
-    TRY(upload(e, e->owned, &e->d_p10, p10));
+    int rc = upload(e, e->d_p10, p10);
+    const size_t T = e->chunk_tiles, mtok = (size_t)cfg->max_batch * e->L;
+    for (auto& sl : e->slots) {
+      if (!rc) rc = alloc(e, sl.d_rows, (size_t)cfg->max_batch * e->R * e->L);
+      if (!rc) rc = alloc(e, sl.d_status, 1);
+      if (!rc) rc = alloc(e, sl.d_bases, mtok);
+      if (!rc) rc = alloc(e, sl.d_quals, mtok);
+    }
+    if (!rc) rc = alloc(e, e->d_embqkv, T * kTileM * (size_t)std::max(e->Epad, kQKVN));
+    if (!rc) rc = alloc(e, e->d_x, T * x_image_elems());
+    if (!rc) rc = alloc(e, e->d_xb, T * act_image_elems(kDP));
+    if (!rc) rc = alloc(e, e->d_att, T * act_image_elems(kDP));
+    if (!rc) rc = alloc(e, e->d_hid, T * act_image_elems(cfg->filter_size));
+    return rc;
+  }();
+  if (rc) {
+    g_create_error = e->err;
+    return rc;
   }
-  const size_t T = e->chunk_tiles;
-  for (auto& sl : e->slots) {
-    TRY(dev_alloc(e, &sl.d_rows, (size_t)cfg->max_batch * e->R * e->L));
-    TRY(dev_alloc(e, &sl.d_status, 1));
-  }
-  TRY(dev_alloc(e, &e->d_embqkv, T * kTileM * (size_t)std::max(e->Epad, kQKVN)));
-  TRY(dev_alloc(e, &e->d_x, T * x_image_elems()));
-  TRY(dev_alloc(e, &e->d_xb, T * act_image_elems(kDP)));
-  TRY(dev_alloc(e, &e->d_att, T * act_image_elems(kDP)));
-  TRY(dev_alloc(e, &e->d_hid, T * act_image_elems(cfg->filter_size)));
-  const size_t mtok = (size_t)cfg->max_batch * e->L;
-  for (auto& sl : e->slots) {
-    TRY(dev_alloc(e, &sl.d_bases, mtok));
-    TRY(dev_alloc(e, &sl.d_quals, mtok));
-  }
-#undef TRY
-#undef CUC
-  *out = e;
+  *out = eng.release();
   return DCB_OK;
 }
 
 void dcb_destroy(dcb_engine* e) {
   if (!e) return;
   cudaSetDevice(e->cfg.device);
-  if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
-  if (e->stream) cudaStreamSynchronize(e->stream);
-  if (e->out_stream) cudaStreamSynchronize(e->out_stream);
-  for (void* p : e->owned) cudaFree(p);
-  free_weights(e->w);
-  if (e->d_st_in) cudaFree(e->d_st_in);
-  if (e->d_st_out) cudaFree(e->d_st_out);
-  if (e->d_st_start) cudaFree(e->d_st_start);
-  if (e->d_st_len) cudaFree(e->d_st_len);
-  for (dcb_engine::Scratch* sc : {&e->sc_pos, &e->sc_names, &e->sc_nameoff, &e->sc_outcome, &e->sc_avg, &e->sc_recoff,
-                                  &e->sc_fastq, &e->sc_bq, &e->sc_mask, &e->sc_ids, &e->sc_dst, &e->sc_tmpb, &e->sc_tmpq,
-                                  &e->sc_ev_probs, &e->sc_ev_in, &e->sc_ev_out, &e->sc_ds_in, &e->sc_ds_out,
-                                  &e->sc_lg_in, &e->sc_lg_out, &e->sc_lg_dp, &e->sc_he_in, &e->sc_he_out})
-    if (sc->p) cudaFree(sc->p);
-  if (e->ev_eval0) cudaEventDestroy(e->ev_eval0);
-  if (e->ev_eval1) cudaEventDestroy(e->ev_eval1);
-  for (auto& sl : e->slots)
-    for (auto& pr : sl.prof_events) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
-  if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
-  for (auto& sl : e->slots) {
-    if (sl.rows_ready) cudaEventDestroy(sl.rows_ready);
-    if (sl.ev0) cudaEventDestroy(sl.ev0);
-    if (sl.ev1) cudaEventDestroy(sl.ev1);
-    if (sl.done) cudaEventDestroy(sl.done);
-    if (sl.h_status) cudaFreeHost(sl.h_status);
-  }
-  if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
-  if (e->out_stream) cudaStreamDestroy(e->out_stream);
-  if (e->stream) cudaStreamDestroy(e->stream);
   delete e;
 }
 
@@ -614,11 +674,7 @@ int dcb_load_weights(dcb_engine* e, const dcb_tensor* tensors, int32_t n) {
   int rc = read_checkpoint(e, tensors, n, &ck);
   if (rc) return rc;
   Weights w;
-  if ((rc = upload_weights(e, ck, &w))) {
-    free_weights(w);
-    return rc;
-  }
-  free_weights(e->w);
+  if ((rc = upload_weights(e, ck, &w))) return rc;
   e->w = std::move(w);
   e->weights_loaded = true;
   return DCB_OK;
@@ -700,12 +756,12 @@ int dcb_set_debug(dcb_engine* e, int32_t enabled) {
   if (e->debug && !e->d_dbg) {
     CU(e, cudaSetDevice(e->cfg.device));
     const size_t stages = 1 + 2 * (size_t)e->cfg.num_hidden_layers;
-    int rc = dev_alloc(e, &e->d_dbg, stages * e->chunk_tiles * x_image_elems());
+    int rc = alloc(e, e->d_dbg, stages * e->chunk_tiles * x_image_elems());
     if (rc) return rc;
     size_t cols = 0;
     int w = 0;
     dbg_operand_slot(e, (int)stages - 1, DCB_DEBUG_HID, &cols, &w);   // the last stage holds HID only
-    rc = dev_alloc(e, &e->d_dbg_op, (cols + w) * e->chunk_tiles * kTileM);
+    rc = alloc(e, e->d_dbg_op, (cols + w) * e->chunk_tiles * kTileM);
     if (rc) return rc;
   }
   return DCB_OK;
@@ -732,28 +788,29 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
   if (packed && (c.pw_max > 255 || c.ip_max > 255)) return fail(e, DCB_ERR_INVALID, "packed rows need PW_MAX, IP_MAX <= 255");
   const int L = e->L, R = e->R;
   const size_t mtok = (size_t)c.max_batch * L;
-  if (probs_out && !sl.d_probs) { int rc = dev_alloc(e, &sl.d_probs, mtok * kVocab); if (rc) return rc; }
-  if (logits_out && !sl.d_logits) { int rc = dev_alloc(e, &sl.d_logits, mtok * kVocab); if (rc) return rc; }
+  if (probs_out && !sl.d_probs) { int rc = alloc(e, sl.d_probs, mtok * kVocab); if (rc) return rc; }
+  if (logits_out && !sl.d_logits) { int rc = alloc(e, sl.d_logits, mtok * kVocab); if (rc) return rc; }
   const bool rows_dev = flags & DCB_ROWS_ON_DEVICE;
   const bool out_dev = flags & DCB_OUT_ON_DEVICE;
   if ((flags & DCB_STRICT_FP32) && (flags & DCB_FAST_BF16)) return fail(e, DCB_ERR_INVALID, "DCB_STRICT_FP32 and DCB_FAST_BF16 are exclusive");
   const bool strict = (flags & DCB_STRICT_FP32) || (c.precision == DCB_PRECISION_FP32 && !(flags & DCB_FAST_BF16));
   if (rows_dev && ((reinterpret_cast<uintptr_t>(rows) | reinterpret_cast<uintptr_t>(packed)) & 15))
     return fail(e, DCB_ERR_INVALID, "device-resident rows must be 16-byte aligned");
-  if (strict && !e->strict.emb) {
+  if (strict && !e->strict.chunk_windows) {
     // workspace of the strict path, on first use: ~16 k tokens per chunk
     dcb_engine::Strict& S = e->strict;
-    S.chunk_windows = std::max(1, std::min(c.max_batch, 16384 / L));
-    const size_t Mc = (size_t)S.chunk_windows * L;
-    int rc = 0;
-    if ((rc = dev_alloc(e, &S.emb, Mc * e->E)) || (rc = dev_alloc(e, &S.x, Mc * kD)) || (rc = dev_alloc(e, &S.y, Mc * kD)) ||
-        (rc = dev_alloc(e, &S.q, Mc * kD)) || (rc = dev_alloc(e, &S.k, Mc * kD)) || (rc = dev_alloc(e, &S.v, Mc * kD)) ||
-        (rc = dev_alloc(e, &S.att, Mc * kD)) || (rc = dev_alloc(e, &S.hid, Mc * c.filter_size)))
-      return rc;
+    const int cw = std::max(1, std::min(c.max_batch, 16384 / L));
+    const size_t Mc = (size_t)cw * L;
+    int rc = alloc(e, S.emb, Mc * e->E);
+    for (DevBuf<float>* b : {&S.x, &S.y, &S.q, &S.k, &S.v, &S.att})
+      if (!rc) rc = alloc(e, *b, Mc * kD);
+    if (!rc) rc = alloc(e, S.hid, Mc * c.filter_size);
+    if (rc) return rc;
+    S.chunk_windows = cw;
   }
   cudaStream_t st = e->stream;
   if (packed && !rows_dev && !sl.d_packed) {
-    int rc = dev_alloc(e, &sl.d_packed, (size_t)c.max_batch * e->pl.stride);
+    int rc = alloc(e, sl.d_packed, (size_t)c.max_batch * e->pl.stride);
     if (rc) return rc;
   }
   if (!rows_dev) {
@@ -773,7 +830,7 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
   int launches = (packed_base && strict) ? 1 : 0;
   const size_t ximg = x_image_elems();
   bool prof_err = false;
-  auto pbegin = [&](int kind) {
+  auto pbegin = [&](ProfKind kind) {
     if (!e->profile) return;
     if (sl.prof_used == sl.prof_events.size()) {
       cudaEvent_t a, b;
@@ -837,16 +894,16 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
     {
       RowEpi epi{};
       epi.x = e->d_x; epi.xb = e->d_xb; epi.bias = nullptr;
-      epi.pe = c.add_pos_encoding ? e->w.pe : nullptr;
-      epi.pe_img = c.add_pos_encoding ? e->w.pe_img : nullptr;
-      epi.ln_g = c.rezero ? nullptr : e->w.layers[0].ln_g[0];
-      epi.ln_b = c.rezero ? nullptr : e->w.layers[0].ln_b[0];
+      epi.pe = c.add_pos_encoding ? e->w.pe.p : nullptr;
+      epi.pe_img = c.add_pos_encoding ? e->w.pe_img.p : nullptr;
+      epi.ln_g = c.rezero ? nullptr : e->w.layers[0].ln_g[0].p;
+      epi.ln_b = c.rezero ? nullptr : e->w.layers[0].ln_b[0].p;
       epi.has_xold = 0; epi.L = Lw;
-      pbegin(0);
+      pbegin(kProfEmbed);
       launch_embed(packed_base ? nullptr : rows_chunk, packed_base ? packed_base + (size_t)w0 * e->pl.stride : nullptr, e->pl,
                    R, L, Lw, M, T, e->echunks, e->w.cols, e->w.rowmeta, e->w.tables, e->table_elems, e->d_embqkv, sl.d_status, st);
       pend();
-      pbegin(1);
+      pbegin(kProfRowGemm);
       launch_gemm_row(e->d_embqkv, e->w.wc, e->Epad / 16, 2 * (e->Epad / 16), T, epi, st);
       pend();
       launches += 2;
@@ -855,29 +912,29 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
     for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
       const LayerDev& ld = e->w.layers[n_];
       const bool last = n_ + 1 == c.num_hidden_layers;
-      pbegin(2);
+      pbegin(kProfQkv);
       launch_gemm_qkv(e->d_xb, ld.wqkv, T, e->d_embqkv, st);
       pend();
-      pbegin(3);
+      pbegin(kProfAttention);
       launch_attention(e->d_embqkv, e->d_att, L, Lw, c.attn_win_size, bw, st);
       pend();
       // attention out-projection + residual; xb = the FFN sub-layer's input (pre-LayerNorm or identity)
       RowEpi ea{};
       ea.x = e->d_x; ea.xb = e->d_xb; ea.bias = nullptr; ea.pe = nullptr;
-      ea.ln_g = c.rezero ? nullptr : ld.ln_g[1];
-      ea.ln_b = c.rezero ? nullptr : ld.ln_b[1];
+      ea.ln_g = c.rezero ? nullptr : ld.ln_g[1].p;
+      ea.ln_b = c.rezero ? nullptr : ld.ln_b[1].p;
       ea.has_xold = 1; ea.L = Lw;
-      pbegin(1);
+      pbegin(kProfRowGemm);
       launch_gemm_row(e->d_att, ld.wo, kDP / 16, 2 * (kDP / 16), T, ea, st);
       pend();
       snap();
       // FFN: hidden = relu(xb W1 + b1), then hidden W2 + b2 + residual; xb = the next layer's input
       RowEpi ef{};
-      ef.x = e->d_x; ef.xb = last ? nullptr : e->d_xb; ef.bias = ld.b2; ef.pe = nullptr;
-      ef.ln_g = (c.rezero || last) ? nullptr : e->w.layers[n_ + 1].ln_g[0];
-      ef.ln_b = (c.rezero || last) ? nullptr : e->w.layers[n_ + 1].ln_b[0];
+      ef.x = e->d_x; ef.xb = last ? nullptr : e->d_xb.p; ef.bias = ld.b2; ef.pe = nullptr;
+      ef.ln_g = (c.rezero || last) ? nullptr : e->w.layers[n_ + 1].ln_g[0].p;
+      ef.ln_b = (c.rezero || last) ? nullptr : e->w.layers[n_ + 1].ln_b[0].p;
       ef.has_xold = 1; ef.L = Lw;
-      pbegin(4);
+      pbegin(kProfFfn);
       launch_ffn_up(e->d_xb, ld.w1, ld.b1, c.filter_size, T, e->d_hid, st);
       launch_gemm_row(e->d_hid, ld.w2, c.filter_size / 16, c.filter_size / 16, T, ef, st);
       pend();
@@ -885,7 +942,7 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
       snap();
       launches += 5;
     }
-    pbegin(5);
+    pbegin(kProfHead);
     launch_head(make_head(), T, st);
     pend();
     ++launches;
@@ -997,10 +1054,9 @@ int dcb_wait(dcb_engine* e, int64_t ticket) {
     for (size_t i = 0; i < sl.prof_used; ++i) {
       float ms = 0.f;
       CU(e, cudaEventElapsedTime(&ms, sl.prof_events[i].first, sl.prof_events[i].second));
-      const int kind = sl.prof_kind[i];
+      const ProfKind kind = sl.prof_kind[i];
       e->prof_ms[kind] += ms;
       ++e->prof_n[kind];
-      if (kind == 4) { e->prof_ffn_ms += ms; ++e->prof_ffn_launches; }
     }
     sl.prof_used = 0;
   }
@@ -1031,25 +1087,23 @@ int dcb_last_forward_launches(dcb_engine* e, int32_t* n) {
 int dcb_set_profile(dcb_engine* e, int32_t enabled) {
   if (!e) return DCB_ERR_INVALID;
   e->profile = enabled != 0;
-  e->prof_ffn_ms = 0.f;
-  e->prof_ffn_launches = 0;
   e->prof_ffn_tokens = 0;
   for (auto& sl : e->slots) sl.prof_used = 0;
-  for (int i = 0; i < 6; ++i) { e->prof_ms[i] = 0.f; e->prof_n[i] = 0; }
+  for (int i = 0; i < kProfKinds; ++i) { e->prof_ms[i] = 0.f; e->prof_n[i] = 0; }
   return DCB_OK;
 }
 
 int dcb_get_profile(dcb_engine* e, float* ffn_ms_total, int32_t* ffn_launches, int64_t* ffn_tokens) {
   if (!e || !ffn_ms_total || !ffn_launches || !ffn_tokens) return DCB_ERR_INVALID;
-  *ffn_ms_total = e->prof_ffn_ms;
-  *ffn_launches = e->prof_ffn_launches;
+  *ffn_ms_total = e->prof_ms[kProfFfn];
+  *ffn_launches = e->prof_n[kProfFfn];
   *ffn_tokens = e->prof_ffn_tokens;
   return DCB_OK;
 }
 
 int dcb_get_profile_kernels(dcb_engine* e, float* ms6, int32_t* n6) {
   if (!e || !ms6 || !n6) return DCB_ERR_INVALID;
-  for (int i = 0; i < 6; ++i) { ms6[i] = e->prof_ms[i]; n6[i] = e->prof_n[i]; }
+  for (int i = 0; i < kProfKinds; ++i) { ms6[i] = e->prof_ms[i]; n6[i] = e->prof_n[i]; }
   return DCB_OK;
 }
 
@@ -1098,6 +1152,14 @@ int dcb_debug_operand(dcb_engine* e, int32_t stage, int32_t which, uint16_t* out
   return DCB_OK;
 }
 
+// read z is the windows [zmw_start[z], zmw_start[z + 1]) of n_windows
+static int check_zmw_start(dcb_engine* e, const int32_t* zmw_start, int n_zmw, int n_windows) {
+  if (zmw_start[0] < 0 || zmw_start[n_zmw] > n_windows) return fail(e, DCB_ERR_INVALID, "dcb_stitch: zmw_start outside [0, n_windows]");
+  for (int z = 0; z < n_zmw; ++z)
+    if (zmw_start[z + 1] < zmw_start[z]) return fail(e, DCB_ERR_INVALID, "dcb_stitch: zmw_start must be non-decreasing");
+  return DCB_OK;
+}
+
 int dcb_stitch(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, int32_t n_windows, int32_t L,
                const int32_t* zmw_start, int32_t n_zmw, uint32_t flags,
                uint8_t* seq_out, uint8_t* qual_out, int32_t* len_out) {
@@ -1105,66 +1167,27 @@ int dcb_stitch(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, int32_
   if (n_windows < 0 || L <= 0 || n_zmw < 0) return fail(e, DCB_ERR_INVALID, "dcb_stitch: negative size");
   if (n_zmw == 0 || n_windows == 0) return DCB_OK;
   if (!bases || !quals || !zmw_start || !seq_out || !qual_out || !len_out) return fail(e, DCB_ERR_INVALID, "dcb_stitch: null pointer");
-  if (zmw_start[0] < 0 || zmw_start[n_zmw] > n_windows) return fail(e, DCB_ERR_INVALID, "dcb_stitch: zmw_start outside [0, n_windows]");
-  for (int z = 0; z < n_zmw; ++z)
-    if (zmw_start[z + 1] < zmw_start[z]) return fail(e, DCB_ERR_INVALID, "dcb_stitch: zmw_start must be non-decreasing");
+  int rc = check_zmw_start(e, zmw_start, n_zmw, n_windows);
+  if (rc) return rc;
   CU(e, cudaSetDevice(e->cfg.device));
   const size_t nbytes = (size_t)n_windows * L;
   const bool in_dev = flags & DCB_ROWS_ON_DEVICE, out_dev = flags & DCB_OUT_ON_DEVICE;
-  cudaStream_t st = e->stream;
-  if (nbytes > e->st_cap) {
-    CU(e, cudaStreamSynchronize(st));
-    if (e->d_st_in) cudaFree(e->d_st_in);
-    if (e->d_st_out) cudaFree(e->d_st_out);
-    e->d_st_in = e->d_st_out = nullptr;
-    e->st_cap = 0;
-    CU(e, cudaMalloc(reinterpret_cast<void**>(&e->d_st_in), 2 * nbytes));
-    CU(e, cudaMalloc(reinterpret_cast<void**>(&e->d_st_out), 2 * nbytes));
-    e->st_cap = nbytes;
-  }
-  if ((size_t)n_zmw + 1 > e->st_zcap) {
-    CU(e, cudaStreamSynchronize(st));
-    if (e->d_st_start) cudaFree(e->d_st_start);
-    if (e->d_st_len) cudaFree(e->d_st_len);
-    e->d_st_start = e->d_st_len = nullptr;
-    e->st_zcap = 0;
-    CU(e, cudaMalloc(reinterpret_cast<void**>(&e->d_st_start), ((size_t)n_zmw + 1) * sizeof(int32_t)));
-    CU(e, cudaMalloc(reinterpret_cast<void**>(&e->d_st_len), ((size_t)n_zmw + 1) * sizeof(int32_t)));
-    e->st_zcap = (size_t)n_zmw + 1;
-  }
-  const uint8_t *db = bases, *dq = quals;
-  if (!in_dev) {
-    CU(e, cudaMemcpyAsync(e->d_st_in, bases, nbytes, cudaMemcpyHostToDevice, st));
-    CU(e, cudaMemcpyAsync(e->d_st_in + e->st_cap, quals, nbytes, cudaMemcpyHostToDevice, st));
-    db = e->d_st_in; dq = e->d_st_in + e->st_cap;
-  }
-  CU(e, cudaMemcpyAsync(e->d_st_start, zmw_start, ((size_t)n_zmw + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  uint8_t* ds = out_dev ? seq_out : e->d_st_out;
-  uint8_t* dqo = out_dev ? qual_out : e->d_st_out + e->st_cap;
-  int32_t* dl = out_dev ? len_out : e->d_st_len;
-  launch_stitch(db, dq, L, e->d_st_start, n_zmw, ds, dqo, dl, st);
-  if (!out_dev) {
-    CU(e, cudaMemcpyAsync(seq_out, ds, nbytes, cudaMemcpyDeviceToHost, st));
-    CU(e, cudaMemcpyAsync(qual_out, dqo, nbytes, cudaMemcpyDeviceToHost, st));
-    CU(e, cudaMemcpyAsync(len_out, dl, (size_t)n_zmw * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  }
-  CU(e, cudaStreamSynchronize(st));
+  const uint8_t *db, *dq;
+  const int32_t* d_start;
+  Output<uint8_t> seq, qual;
+  Output<int32_t> len;
+  if ((rc = stage_in(e, e->st.bases, bases, nbytes, in_dev, &db)) || (rc = stage_in(e, e->st.quals, quals, nbytes, in_dev, &dq)) ||
+      (rc = stage_in(e, e->st.start, zmw_start, (size_t)n_zmw + 1, false, &d_start)) ||
+      (rc = stage_out(e, e->st.seq, seq_out, nbytes, out_dev, &seq)) ||
+      (rc = stage_out(e, e->st.qual, qual_out, nbytes, out_dev, &qual)) ||
+      (rc = stage_out(e, e->st.len, len_out, (size_t)n_zmw, out_dev, &len)))
+    return rc;
+  launch_stitch(db, dq, L, d_start, n_zmw, seq.d, qual.d, len.d, e->stream);
+  if ((rc = copy_out(e, seq)) || (rc = copy_out(e, qual)) || (rc = copy_out(e, len))) return rc;
+  CU(e, cudaStreamSynchronize(e->stream));
   CU(e, cudaGetLastError());
   return DCB_OK;
 }
-
-namespace {
-// grow-on-demand device scratch; contents are not preserved
-int ensure(dcb_engine* e, dcb_engine::Scratch& sc, size_t bytes) {
-  if (bytes <= sc.cap) return DCB_OK;
-  CU(e, cudaStreamSynchronize(e->stream));
-  if (sc.p) cudaFree(sc.p);
-  sc.p = nullptr; sc.cap = 0;
-  CU(e, cudaMalloc(&sc.p, bytes));
-  sc.cap = bytes;
-  return DCB_OK;
-}
-}  // namespace
 
 int dcb_stitch_fastq(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, int32_t n_windows, int32_t L,
                      const int32_t* zmw_start, int32_t n_zmw, const int32_t* window_pos, const uint8_t* names,
@@ -1179,60 +1202,35 @@ int dcb_stitch_fastq(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, 
   if (name_off[0] != 0) return fail(e, DCB_ERR_INVALID, "dcb_stitch_fastq: name_off[0] must be 0");
   for (int z = 0; z < n_zmw; ++z)
     if (name_off[z + 1] < name_off[z]) return fail(e, DCB_ERR_INVALID, "dcb_stitch_fastq: name_off must be non-decreasing");
-  const size_t nbytes = (size_t)n_windows * L;
-  // stage 1: concatenation + gap compaction (dcb_stitch), results stay on the device
+  int rc = check_zmw_start(e, zmw_start, n_zmw, n_windows);
+  if (rc) return rc;
   CU(e, cudaSetDevice(e->cfg.device));
   cudaStream_t st = e->stream;
-  int rc;
-  // reuse dcb_stitch with device-side outputs into our own scratch
-  if ((rc = ensure(e, e->sc_tmpb, nbytes ? nbytes : 1)) || (rc = ensure(e, e->sc_tmpq, nbytes ? nbytes : 1)) ||
-      (rc = ensure(e, e->sc_dst, ((size_t)n_zmw + 1) * sizeof(int32_t))))
+  const size_t nbytes = (size_t)n_windows * L, nz = n_zmw;
+  const bool in_dev = flags & DCB_ROWS_ON_DEVICE;
+  const uint8_t *db, *dq, *d_names;
+  const int32_t *d_start, *d_pos, *d_name_off;
+  Output<int64_t> rec;
+  Output<int32_t> out;
+  Output<double> avg;
+  if ((rc = stage_in(e, e->st.bases, bases, nbytes, in_dev, &db)) || (rc = stage_in(e, e->st.quals, quals, nbytes, in_dev, &dq)) ||
+      (rc = stage_in(e, e->st.start, zmw_start, nz + 1, false, &d_start)) ||
+      (rc = stage_in(e, e->st.pos, window_pos, (size_t)n_windows, false, &d_pos)) ||
+      (rc = stage_in(e, e->st.names, names, (size_t)name_off[n_zmw], false, &d_names)) ||
+      (rc = stage_in(e, e->st.name_off, name_off, nz + 1, false, &d_name_off)) ||
+      (rc = ensure(e, e->st.seq, nbytes)) || (rc = ensure(e, e->st.qual, nbytes)) || (rc = ensure(e, e->st.len, nz)) ||
+      (rc = ensure(e, e->st.fastq, (size_t)fastq_cap)) || (rc = stage_out(e, e->st.rec_off, rec_off, nz + 1, false, &rec)) ||
+      (rc = stage_out(e, e->st.outcome, outcome, nz, false, &out)) || (rc = stage_out(e, e->st.avg_q, avg_q, nz, false, &avg)))
     return rc;
-  uint8_t* d_seq = static_cast<uint8_t*>(e->sc_tmpb.p);
-  uint8_t* d_qual = static_cast<uint8_t*>(e->sc_tmpq.p);
-  int32_t* d_len = static_cast<int32_t*>(e->sc_dst.p);
-  if (n_windows > 0) {
-    rc = dcb_stitch(e, bases, quals, n_windows, L, zmw_start, n_zmw, (flags & DCB_ROWS_ON_DEVICE) | DCB_OUT_ON_DEVICE, d_seq, d_qual, d_len);
-    if (rc) return rc;
-  } else {
-    CU(e, cudaMemsetAsync(d_len, 0, ((size_t)n_zmw + 1) * sizeof(int32_t), st));
-  }
-  const size_t names_bytes = (size_t)name_off[n_zmw];
-  const size_t cap = (size_t)fastq_cap;
-  if ((rc = ensure(e, e->sc_pos, (nbytes ? (size_t)n_windows : 1) * sizeof(int32_t))) ||
-      (rc = ensure(e, e->sc_names, names_bytes ? names_bytes : 1)) ||
-      (rc = ensure(e, e->sc_nameoff, ((size_t)n_zmw + 1) * sizeof(int32_t))) ||
-      (rc = ensure(e, e->sc_outcome, (size_t)n_zmw * sizeof(int32_t))) || (rc = ensure(e, e->sc_avg, (size_t)n_zmw * sizeof(double))) ||
-      (rc = ensure(e, e->sc_recoff, ((size_t)n_zmw + 1) * sizeof(int64_t))) || (rc = ensure(e, e->sc_fastq, cap ? cap : 1)))
-    return rc;
-  // dcb_stitch left zmw_start in its own scratch (d_st_start)
-  if (n_windows == 0) {
-    if ((size_t)n_zmw + 1 > e->st_zcap) {
-      if (e->d_st_start) cudaFree(e->d_st_start);
-      if (e->d_st_len) cudaFree(e->d_st_len);
-      e->d_st_start = e->d_st_len = nullptr; e->st_zcap = 0;
-      CU(e, cudaMalloc(reinterpret_cast<void**>(&e->d_st_start), ((size_t)n_zmw + 1) * sizeof(int32_t)));
-      CU(e, cudaMalloc(reinterpret_cast<void**>(&e->d_st_len), ((size_t)n_zmw + 1) * sizeof(int32_t)));
-      e->st_zcap = (size_t)n_zmw + 1;
-    }
-    CU(e, cudaMemcpyAsync(e->d_st_start, zmw_start, ((size_t)n_zmw + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  }
-  if (n_windows > 0) CU(e, cudaMemcpyAsync(e->sc_pos.p, window_pos, (size_t)n_windows * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  if (names_bytes) CU(e, cudaMemcpyAsync(e->sc_names.p, names, names_bytes, cudaMemcpyHostToDevice, st));
-  CU(e, cudaMemcpyAsync(e->sc_nameoff.p, name_off, ((size_t)n_zmw + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  int32_t* d_out = static_cast<int32_t*>(e->sc_outcome.p);
-  double* d_avg = static_cast<double*>(e->sc_avg.p);
-  int64_t* d_rec = static_cast<int64_t*>(e->sc_recoff.p);
-  launch_read_outcome(d_qual, d_len, e->d_st_start, static_cast<const int32_t*>(e->sc_pos.p), L, n_zmw, e->d_p10, min_quality,
-                      min_length, d_out, d_avg, st);
-  launch_fastq(d_seq, d_qual, d_len, e->d_st_start, L, n_zmw, d_out, static_cast<const uint8_t*>(e->sc_names.p),
-               static_cast<const int32_t*>(e->sc_nameoff.p), d_rec, static_cast<uint8_t*>(e->sc_fastq.p), fastq_cap, st);
-  CU(e, cudaMemcpyAsync(rec_off, d_rec, ((size_t)n_zmw + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-  CU(e, cudaMemcpyAsync(outcome, d_out, (size_t)n_zmw * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  CU(e, cudaMemcpyAsync(avg_q, d_avg, (size_t)n_zmw * sizeof(double), cudaMemcpyDeviceToHost, st));
+  // concatenation + gap compaction (with no windows, every read is empty), then the filters and the records
+  launch_stitch(db, dq, L, d_start, n_zmw, e->st.seq, e->st.qual, e->st.len, st);
+  launch_read_outcome(e->st.qual, e->st.len, d_start, d_pos, L, n_zmw, e->d_p10, min_quality, min_length, out.d, avg.d, st);
+  launch_fastq(e->st.seq, e->st.qual, e->st.len, d_start, L, n_zmw, out.d, d_names, d_name_off, rec.d, e->st.fastq,
+               fastq_cap, st);
+  if ((rc = copy_out(e, rec)) || (rc = copy_out(e, out)) || (rc = copy_out(e, avg))) return rc;
   CU(e, cudaStreamSynchronize(st));
   if (rec_off[n_zmw] > fastq_cap) return fail(e, DCB_ERR_INVALID, "dcb_stitch_fastq: fastq_out too small: need %lld bytes", (long long)rec_off[n_zmw]);
-  if (rec_off[n_zmw] > 0) CU(e, cudaMemcpy(fastq_out, e->sc_fastq.p, (size_t)rec_off[n_zmw], cudaMemcpyDeviceToHost));
+  if (rec_off[n_zmw] > 0) CU(e, cudaMemcpy(fastq_out, e->st.fastq, (size_t)rec_off[n_zmw], cudaMemcpyDeviceToHost));
   CU(e, cudaGetLastError());
   return DCB_OK;
 }
@@ -1244,18 +1242,17 @@ int dcb_skip_mask(dcb_engine* e, const int16_t* ccs_bq, int32_t n_windows, int32
   if (n_windows == 0) return DCB_OK;
   if (!ccs_bq || !mask_out) return fail(e, DCB_ERR_INVALID, "dcb_skip_mask: null pointer");
   CU(e, cudaSetDevice(e->cfg.device));
-  cudaStream_t st = e->stream;
-  const size_t n = (size_t)n_windows * L;
+  const int16_t* d_bq;
+  Output<uint8_t> mask;
+  Output<double> avg;
   int rc;
-  if ((rc = ensure(e, e->sc_bq, n * sizeof(int16_t))) || (rc = ensure(e, e->sc_mask, (size_t)n_windows)) ||
-      (rc = ensure(e, e->sc_avg, (size_t)n_windows * sizeof(double))))
+  if ((rc = stage_in(e, e->sk.bq, ccs_bq, (size_t)n_windows * L, false, &d_bq)) ||
+      (rc = stage_out(e, e->sk.mask, mask_out, (size_t)n_windows, false, &mask)) ||
+      (rc = stage_out(e, e->sk.avg, avg_out, (size_t)n_windows, false, &avg)))
     return rc;
-  CU(e, cudaMemcpyAsync(e->sc_bq.p, ccs_bq, n * sizeof(int16_t), cudaMemcpyHostToDevice, st));
-  launch_skip_mask(static_cast<const int16_t*>(e->sc_bq.p), n_windows, L, e->d_p10, skip_windows_above,
-                   static_cast<uint8_t*>(e->sc_mask.p), static_cast<double*>(e->sc_avg.p), st);
-  CU(e, cudaMemcpyAsync(mask_out, e->sc_mask.p, (size_t)n_windows, cudaMemcpyDeviceToHost, st));
-  if (avg_out) CU(e, cudaMemcpyAsync(avg_out, e->sc_avg.p, (size_t)n_windows * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CU(e, cudaStreamSynchronize(st));
+  launch_skip_mask(d_bq, n_windows, L, e->d_p10, skip_windows_above, mask.d, avg.d, e->stream);
+  if ((rc = copy_out(e, mask)) || (rc = copy_out(e, avg))) return rc;
+  CU(e, cudaStreamSynchronize(e->stream));
   CU(e, cudaGetLastError());
   return DCB_OK;
 }
@@ -1273,35 +1270,31 @@ int dcb_fill_skipped(dcb_engine* e, const uint8_t* ccs_ids, const int16_t* ccs_b
   cudaStream_t st = e->stream;
   const size_t n = (size_t)k * L;
   const bool out_dev = flags & DCB_OUT_ON_DEVICE;
-  int rc;
-  if ((rc = ensure(e, e->sc_ids, n)) || (rc = ensure(e, e->sc_bq, n * sizeof(int16_t))) ||
-      (rc = ensure(e, e->sc_dst, ((size_t)k + 1) * sizeof(int32_t))) || (rc = ensure(e, e->sc_mask, sizeof(int))))
-    return rc;
-  if (!out_dev && ((rc = ensure(e, e->sc_tmpb, n)) || (rc = ensure(e, e->sc_tmpq, n)))) return rc;
+  // host outputs: the kernel writes a dense [k, L] temporary, scattered into the caller's rows on the host below
   std::vector<int32_t> dst(dst_window, dst_window + k);
-  if (!out_dev) for (int j = 0; j < k; ++j) dst[j] = j;      // dense temporary, scattered on the host below
-  CU(e, cudaMemcpyAsync(e->sc_ids.p, ccs_ids, n, cudaMemcpyHostToDevice, st));
-  CU(e, cudaMemcpyAsync(e->sc_bq.p, ccs_bq, n * sizeof(int16_t), cudaMemcpyHostToDevice, st));
-  CU(e, cudaMemcpyAsync(e->sc_dst.p, dst.data(), (size_t)k * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  CU(e, cudaMemsetAsync(e->sc_mask.p, 0, sizeof(int), st));
-  uint8_t* db = out_dev ? bases : static_cast<uint8_t*>(e->sc_tmpb.p);
-  uint8_t* dq = out_dev ? quals : static_cast<uint8_t*>(e->sc_tmpq.p);
-  launch_fill_skipped(static_cast<const uint8_t*>(e->sc_ids.p), static_cast<const int16_t*>(e->sc_bq.p),
-                      static_cast<const int32_t*>(e->sc_dst.p), k, L, calibration_enabled, calibration_threshold,
-                      calibration_w, calibration_b, e->cfg.max_base_quality, db, dq, static_cast<int*>(e->sc_mask.p), st);
+  std::vector<uint8_t> hb(out_dev ? 0 : n), hq(out_dev ? 0 : n);
+  if (!out_dev) for (int j = 0; j < k; ++j) dst[j] = j;
+  const uint8_t* d_ids;
+  const int16_t* d_bq;
+  const int32_t* d_dst;
+  Output<uint8_t> ob, oq;
+  Output<int> ostatus;
   int status = 0;
-  CU(e, cudaMemcpyAsync(&status, e->sc_mask.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-  if (!out_dev) {
-    std::vector<uint8_t> hb(n), hq(n);
-    CU(e, cudaMemcpyAsync(hb.data(), db, n, cudaMemcpyDeviceToHost, st));
-    CU(e, cudaMemcpyAsync(hq.data(), dq, n, cudaMemcpyDeviceToHost, st));
-    CU(e, cudaStreamSynchronize(st));
-    for (int j = 0; j < k; ++j) {
-      memcpy(bases + (size_t)dst_window[j] * L, hb.data() + (size_t)j * L, L);
-      memcpy(quals + (size_t)dst_window[j] * L, hq.data() + (size_t)j * L, L);
-    }
-  } else {
-    CU(e, cudaStreamSynchronize(st));
+  int rc;
+  if ((rc = stage_in(e, e->fs.ids, ccs_ids, n, false, &d_ids)) || (rc = stage_in(e, e->fs.bq, ccs_bq, n, false, &d_bq)) ||
+      (rc = stage_in(e, e->fs.dst, dst.data(), (size_t)k, false, &d_dst)) ||
+      (rc = stage_out(e, e->fs.status, &status, 1, false, &ostatus)) ||
+      (rc = stage_out(e, e->fs.bases, out_dev ? bases : hb.data(), n, out_dev, &ob)) ||
+      (rc = stage_out(e, e->fs.quals, out_dev ? quals : hq.data(), n, out_dev, &oq)))
+    return rc;
+  CU(e, cudaMemsetAsync(ostatus.d, 0, sizeof(int), st));
+  launch_fill_skipped(d_ids, d_bq, d_dst, k, L, calibration_enabled, calibration_threshold, calibration_w, calibration_b,
+                      e->cfg.max_base_quality, ob.d, oq.d, ostatus.d, st);
+  if ((rc = copy_out(e, ostatus)) || (rc = copy_out(e, ob)) || (rc = copy_out(e, oq))) return rc;
+  CU(e, cudaStreamSynchronize(st));
+  for (int j = 0; j < k && !out_dev; ++j) {
+    memcpy(bases + (size_t)dst_window[j] * L, hb.data() + (size_t)j * L, L);
+    memcpy(quals + (size_t)dst_window[j] * L, hq.data() + (size_t)j * L, L);
   }
   CU(e, cudaGetLastError());
   if (status & 1) return fail(e, DCB_ERR_INPUT_RANGE, "dcb_fill_skipped: CCS base id outside 0..4 (clamped)");
@@ -1315,29 +1308,25 @@ int dcb_debug_head_epilogue(dcb_engine* e, const float* logits, int64_t n, uint8
   CU(e, cudaSetDevice(e->cfg.device));
   cudaStream_t st = e->stream;
   const int64_t chunk = std::min<int64_t>(n, 1 << 20);
-  int rc;
-  // in: [8] zero fc1 bias, then the chunk's logits; out: probs, then bases and quals
-  if ((rc = ensure(e, e->sc_he_in, (8 + (size_t)chunk * kVocab) * sizeof(float))) ||
-      (rc = ensure(e, e->sc_he_out, (size_t)chunk * (kVocab * sizeof(float) + 2))))
-    return rc;
-  float* d_bias = static_cast<float*>(e->sc_he_in.p);
-  float* d_logits = d_bias + 8;
-  float* d_probs = static_cast<float*>(e->sc_he_out.p);
-  uint8_t* d_bases = reinterpret_cast<uint8_t*>(d_probs + (size_t)chunk * kVocab);
-  uint8_t* d_quals = d_bases + chunk;
-  CU(e, cudaMemsetAsync(d_bias, 0, 8 * sizeof(float), st));
+  int rc = ensure(e, e->he.bias, 8);   // fc1 bias: zero
+  if (rc) return rc;
+  CU(e, cudaMemsetAsync(e->he.bias, 0, 8 * sizeof(float), st));
   HeadParams hp{};
-  hp.bfc = d_bias;
+  hp.bfc = e->he.bias;
   set_head_quality(hp, e->cfg);
-  hp.bases = d_bases; hp.quals = d_quals; hp.probs = probs ? d_probs : nullptr;
-  for (int64_t t0 = 0; t0 < n; t0 += chunk) {
-    const int m = (int)std::min<int64_t>(chunk, n - t0);
-    CU(e, cudaMemcpyAsync(d_logits, logits + t0 * kVocab, (size_t)m * kVocab * sizeof(float), cudaMemcpyHostToDevice, st));
-    launch_head_epilogue(d_logits, m, hp, st);
-    CU(e, cudaMemcpyAsync(bases + t0, d_bases, (size_t)m, cudaMemcpyDeviceToHost, st));
-    CU(e, cudaMemcpyAsync(quals + t0, d_quals, (size_t)m, cudaMemcpyDeviceToHost, st));
-    if (probs) CU(e, cudaMemcpyAsync(probs + t0 * kVocab, d_probs, (size_t)m * kVocab * sizeof(float), cudaMemcpyDeviceToHost, st));
-    CU(e, cudaStreamSynchronize(st));   // pageable host buffers: the next chunk reuses the scratch
+  for (int64_t t0 = 0; t0 < n; t0 += chunk) {   // the first chunk is the largest: the buffers grow once
+    const size_t m = (size_t)std::min<int64_t>(chunk, n - t0);
+    const float* d_logits;
+    Output<uint8_t> ob, oq;
+    Output<float> op;
+    if ((rc = stage_in(e, e->he.logits, logits + t0 * kVocab, m * kVocab, false, &d_logits)) ||
+        (rc = stage_out(e, e->he.bases, bases + t0, m, false, &ob)) || (rc = stage_out(e, e->he.quals, quals + t0, m, false, &oq)) ||
+        (rc = stage_out(e, e->he.probs, probs ? probs + t0 * kVocab : nullptr, m * kVocab, false, &op)))
+      return rc;
+    hp.bases = ob.d; hp.quals = oq.d; hp.probs = op.d;
+    launch_head_epilogue(d_logits, (int)m, hp, st);
+    if ((rc = copy_out(e, ob)) || (rc = copy_out(e, oq)) || (rc = copy_out(e, op))) return rc;
+    CU(e, cudaStreamSynchronize(st));   // pageable host buffers: the next chunk reuses the staging
   }
   CU(e, cudaGetLastError());
   return DCB_OK;
@@ -1361,35 +1350,25 @@ int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const
     if (labels[i] > 4) return fail(e, DCB_ERR_INVALID, "dcb_evaluate: label id %d outside 0..4 at window %zu", labels[i], i / L);
   CU(e, cudaSetDevice(e->cfg.device));
   cudaStream_t st = e->stream;
-  const bool probs_dev = flags & DCB_ROWS_ON_DEVICE;
-  const size_t out_bytes = (size_t)batch * (sizeof(float) + 10 * sizeof(int32_t) + 1);
+  const float* d_probs;
+  const uint8_t *d_labels, *d_ccs;
+  Output<float> loss;
+  Output<int32_t> pred, ccs;
+  Output<uint8_t> exact;
   int rc;
-  if ((rc = ensure(e, e->sc_ev_in, 2 * ntok)) || (rc = ensure(e, e->sc_ev_out, out_bytes)) ||
-      (!probs_dev && (rc = ensure(e, e->sc_ev_probs, ntok * kVocab * sizeof(float)))))
+  if ((rc = stage_in(e, e->ev.probs, probs, ntok * kVocab, flags & DCB_ROWS_ON_DEVICE, &d_probs)) ||
+      (rc = stage_in(e, e->ev.labels, labels, ntok, false, &d_labels)) || (rc = stage_in(e, e->ev.ccs, ccs_ids, ntok, false, &d_ccs)) ||
+      (rc = stage_out(e, e->ev.loss, loss_out, (size_t)batch, false, &loss)) ||
+      (rc = stage_out(e, e->ev.pred, pred_counts, (size_t)batch * 5, false, &pred)) ||
+      (rc = stage_out(e, e->ev.ccs_counts, ccs_counts, (size_t)batch * 5, false, &ccs)) ||
+      (rc = stage_out(e, e->ev.exact, exact_out, (size_t)batch, false, &exact)))
     return rc;
-  if (!e->ev_eval0) CU(e, cudaEventCreate(&e->ev_eval0));
-  if (!e->ev_eval1) CU(e, cudaEventCreate(&e->ev_eval1));
-  uint8_t* d_in = static_cast<uint8_t*>(e->sc_ev_in.p);
-  const float* d_probs = probs;
-  if (!probs_dev) {
-    CU(e, cudaMemcpyAsync(e->sc_ev_probs.p, probs, ntok * kVocab * sizeof(float), cudaMemcpyHostToDevice, st));
-    d_probs = static_cast<const float*>(e->sc_ev_probs.p);
-  }
-  CU(e, cudaMemcpyAsync(d_in, labels, ntok, cudaMemcpyHostToDevice, st));
-  CU(e, cudaMemcpyAsync(d_in + ntok, ccs_ids, ntok, cudaMemcpyHostToDevice, st));
-  float* d_loss = static_cast<float*>(e->sc_ev_out.p);
-  int32_t* d_pred = reinterpret_cast<int32_t*>(d_loss + batch);
-  int32_t* d_ccs = d_pred + (size_t)batch * 5;
-  uint8_t* d_exact = reinterpret_cast<uint8_t*>(d_ccs + (size_t)batch * 5);
   const bool hard = !(loss_reg > 0.0);
   CU(e, cudaEventRecord(e->ev_eval0, st));
-  CU(e, launch_evaluate(d_probs, d_in, d_in + ntok, batch, L, (float)del_cost, hard ? 1.f : (float)loss_reg, hard ? 1 : 0,
-                        d_loss, d_exact, d_pred, d_ccs, st));
+  CU(e, launch_evaluate(d_probs, d_labels, d_ccs, batch, L, (float)del_cost, hard ? 1.f : (float)loss_reg, hard ? 1 : 0,
+                        loss.d, exact.d, pred.d, ccs.d, st));
   CU(e, cudaEventRecord(e->ev_eval1, st));
-  CU(e, cudaMemcpyAsync(loss_out, d_loss, (size_t)batch * sizeof(float), cudaMemcpyDeviceToHost, st));
-  CU(e, cudaMemcpyAsync(pred_counts, d_pred, (size_t)batch * 5 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  CU(e, cudaMemcpyAsync(ccs_counts, d_ccs, (size_t)batch * 5 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  CU(e, cudaMemcpyAsync(exact_out, d_exact, (size_t)batch, cudaMemcpyDeviceToHost, st));
+  if ((rc = copy_out(e, loss)) || (rc = copy_out(e, pred)) || (rc = copy_out(e, ccs)) || (rc = copy_out(e, exact))) return rc;
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
@@ -1416,26 +1395,18 @@ int dcb_distill_loss(dcb_engine* e, const float* teacher_logits, const float* st
   CU(e, cudaSetDevice(e->cfg.device));
   cudaStream_t st = e->stream;
   const size_t nlog = (size_t)batch * L * kVocab;
+  const bool in_dev = flags & DCB_ROWS_ON_DEVICE;
+  const float *d_teacher, *d_student;
+  Output<float> loss;
   int rc;
-  if ((rc = ensure(e, e->sc_ds_out, (size_t)batch * sizeof(float))) ||
-      (!(flags & DCB_ROWS_ON_DEVICE) && (rc = ensure(e, e->sc_ds_in, 2 * nlog * sizeof(float)))))
+  if ((rc = stage_in(e, e->ds.teacher, teacher_logits, nlog, in_dev, &d_teacher)) ||
+      (rc = stage_in(e, e->ds.student, student_logits, nlog, in_dev, &d_student)) ||
+      (rc = stage_out(e, e->ds.loss, loss_out, (size_t)batch, false, &loss)))
     return rc;
-  if (!e->ev_eval0) CU(e, cudaEventCreate(&e->ev_eval0));
-  if (!e->ev_eval1) CU(e, cudaEventCreate(&e->ev_eval1));
-  const float* d_teacher = teacher_logits;
-  const float* d_student = student_logits;
-  if (!(flags & DCB_ROWS_ON_DEVICE)) {
-    float* d_in = static_cast<float*>(e->sc_ds_in.p);
-    CU(e, cudaMemcpyAsync(d_in, teacher_logits, nlog * sizeof(float), cudaMemcpyHostToDevice, st));
-    CU(e, cudaMemcpyAsync(d_in + nlog, student_logits, nlog * sizeof(float), cudaMemcpyHostToDevice, st));
-    d_teacher = d_in;
-    d_student = d_in + nlog;
-  }
-  float* d_loss = static_cast<float*>(e->sc_ds_out.p);
   CU(e, cudaEventRecord(e->ev_eval0, st));
-  CU(e, launch_distill_loss(d_teacher, d_student, batch, L, t32, logit_loss, d_loss, st));
+  CU(e, launch_distill_loss(d_teacher, d_student, batch, L, t32, logit_loss, loss.d, st));
   CU(e, cudaEventRecord(e->ev_eval1, st));
-  CU(e, cudaMemcpyAsync(loss_out, d_loss, (size_t)batch * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if ((rc = copy_out(e, loss))) return rc;
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
@@ -1458,7 +1429,7 @@ int dcb_alignment_loss_grad(dcb_engine* e, const float* probs, const uint8_t* la
   CU(e, cudaSetDevice(e->cfg.device));
   cudaStream_t st = e->stream;
   const bool in_dev = flags & DCB_ROWS_ON_DEVICE, out_dev = flags & DCB_OUT_ON_DEVICE;
-  const size_t ntok = (size_t)batch * L, np = ntok * kVocab * sizeof(float);
+  const size_t ntok = (size_t)batch * L;
   const uint8_t* hl = labels;
   std::vector<uint8_t> lab_copy;
   if (in_dev) {   // the label check reads them on the host
@@ -1472,46 +1443,28 @@ int dcb_alignment_loss_grad(dcb_engine* e, const float* probs, const uint8_t* la
       return fail(e, DCB_ERR_INVALID, "dcb_alignment_loss_grad: label id %d outside 0..4 at window %zu", hl[i], i / L);
   int ctas = 0;
   CU(e, loss_grad_grid(batch, &ctas));
-  // host outputs go through scratch: loss [B] | grad [B, L, 5] | matches [B, L, L]
-  const size_t n_grad = grad_out ? ntok * kVocab : 0, n_match = matches_out ? ntok * L : 0;
+  const float* d_probs;
+  const uint8_t* d_labels;
+  Output<float> loss, grad, match;
   int rc;
-  if ((rc = ensure(e, e->sc_lg_dp, loss_grad_table_bytes(L, ctas))) ||
-      (!in_dev && (rc = ensure(e, e->sc_lg_in, np + ntok))) ||
-      (!out_dev && (rc = ensure(e, e->sc_lg_out, ((size_t)batch + n_grad + n_match) * sizeof(float)))))
+  if ((rc = ensure(e, e->lg.dp, loss_grad_table_bytes(L, ctas) / sizeof(float))) ||
+      (rc = stage_in(e, e->lg.probs, probs, ntok * kVocab, in_dev, &d_probs)) ||
+      (rc = stage_in(e, e->lg.labels, labels, ntok, in_dev, &d_labels)) ||
+      (rc = stage_out(e, e->lg.loss, loss_out, (size_t)batch, out_dev, &loss)) ||
+      (rc = stage_out(e, e->lg.grad, grad_out, ntok * kVocab, out_dev, &grad)) ||
+      (rc = stage_out(e, e->lg.matches, matches_out, ntok * L, out_dev, &match)))
     return rc;
-  if (!e->ev_eval0) CU(e, cudaEventCreate(&e->ev_eval0));
-  if (!e->ev_eval1) CU(e, cudaEventCreate(&e->ev_eval1));
-  const float* d_probs = probs;
-  const uint8_t* d_labels = labels;
-  if (!in_dev) {
-    float* d_in = static_cast<float*>(e->sc_lg_in.p);
-    CU(e, cudaMemcpyAsync(d_in, probs, np, cudaMemcpyHostToDevice, st));
-    CU(e, cudaMemcpyAsync(d_in + ntok * kVocab, labels, ntok, cudaMemcpyHostToDevice, st));
-    d_probs = d_in;
-    d_labels = reinterpret_cast<const uint8_t*>(d_in + ntok * kVocab);
-  }
-  float *d_loss = loss_out, *d_grad = grad_out, *d_match = matches_out;
-  if (!out_dev) {
-    d_loss = static_cast<float*>(e->sc_lg_out.p);
-    d_grad = grad_out ? d_loss + batch : nullptr;
-    d_match = matches_out ? d_loss + batch + n_grad : nullptr;
-  }
   const bool hard = !(loss_reg > 0.0);
   CU(e, cudaEventRecord(e->ev_eval0, st));
   CU(e, launch_loss_grad(d_probs, d_labels, batch, L, (float)del_cost, hard ? 1.f : (float)loss_reg, hard ? 1 : 0,
-                         static_cast<float*>(e->sc_lg_dp.p), ctas, d_loss, d_grad, d_match, st));
+                         e->lg.dp, ctas, loss.d, grad.d, match.d, st));
   CU(e, cudaEventRecord(e->ev_eval1, st));
-  if (!out_dev) {
-    CU(e, cudaMemcpyAsync(loss_out, d_loss, (size_t)batch * sizeof(float), cudaMemcpyDeviceToHost, st));
-    if (grad_out) CU(e, cudaMemcpyAsync(grad_out, d_grad, n_grad * sizeof(float), cudaMemcpyDeviceToHost, st));
-    if (matches_out) CU(e, cudaMemcpyAsync(matches_out, d_match, n_match * sizeof(float), cudaMemcpyDeviceToHost, st));
-  }
+  if ((rc = copy_out(e, loss)) || (rc = copy_out(e, grad)) || (rc = copy_out(e, match))) return rc;
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
   return DCB_OK;
 }
-
 
 int dcb_alloc_host(size_t bytes, void** out) {
   if (!out) return DCB_ERR_INVALID;

@@ -64,18 +64,27 @@ def test_no_cpu_fallback_without_gpu():
     engine.B200Model(p, weights_lib.init_weights(p), max_batch=2)
 
 
-def test_destroy_frees_every_scratch_buffer():
-  """The grow-on-demand device scratch (dcb_engine::Scratch) has no destructor: dcb_destroy frees it from an explicit
-  list, which must name every buffer the engine declares."""
-  src = open(os.path.join(ROOT, "deepconsensus_b200", "csrc", "engine.cu")).read()
-  decl = src[src.index("struct Scratch {"):]
-  decl = decl[decl.index("}") + 1:]
-  decl = re.sub(r"//[^\n]*", "", decl[:decl.index(";")])
-  declared = set(re.findall(r"\b(sc_\w+)", decl))
-  destroy = src[src.index("void dcb_destroy("):]
-  loop = destroy[destroy.index("for (dcb_engine::Scratch* sc :"):]
-  freed = set(re.findall(r"&e->(sc_\w+)", loop[:loop.index("})")]))
-  assert len(declared) >= 20 and declared == freed, declared ^ freed
+def test_device_memory_is_owned_by_its_buffer_type():
+  """Every device allocation the engine makes for itself lives in a DevBuf, whose destructor frees it: cudaMalloc and
+  cudaFree appear only inside that type and in the caller-owned dcb_alloc_device / dcb_free_device."""
+  src = re.sub(r"//[^\n]*", "", open(os.path.join(ROOT, "deepconsensus_b200", "csrc", "engine.cu")).read())
+
+  def block(start):   # `start` through the end of the brace-balanced body that follows it
+    i = src.index(start)
+    depth = 0
+    for k in range(src.index("{", i), len(src)):
+      depth += {"{": 1, "}": -1}.get(src[k], 0)
+      if depth == 0:
+        return src[i:k + 1]
+
+  owners = {s: block(s) for s in ("struct DevBuf {", "int dcb_alloc_device(", "int dcb_free_device(")}
+  rest = src
+  for body in owners.values():
+    rest = rest.replace(body, "")
+  assert re.findall(r"\bcuda(?:Malloc|Free)\(", rest) == []
+  devbuf = owners["struct DevBuf {"]
+  assert "cudaMalloc(" in devbuf and re.search(r"~DevBuf\(\)\s*\{\s*reset\(\);", devbuf)
+  assert "cudaFree(" in devbuf[devbuf.index("void reset()"):]
 
 
 def test_product_code_never_imports_oracle():
