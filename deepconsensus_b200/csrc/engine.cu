@@ -785,7 +785,8 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
   if ((!rows && !packed) || !bases_out || !quals_out) return fail(e, DCB_ERR_INVALID, "null rows / output buffer");
   CU(e, cudaSetDevice(e->cfg.device));
   const dcb_config& c = e->cfg;
-  if (packed && (c.pw_max > 255 || c.ip_max > 255)) return fail(e, DCB_ERR_INVALID, "packed rows need PW_MAX, IP_MAX <= 255");
+  if (packed && (c.pw_max > 255 || c.ip_max > 255 || c.strand_max > 3 || c.ccs_bq_max > 256))
+    return fail(e, DCB_ERR_INVALID, "packed rows need PW_MAX, IP_MAX <= 255, STRAND_MAX <= 3 and CCS_BQ_MAX <= 256");
   const int L = e->L, R = e->R;
   const size_t mtok = (size_t)c.max_batch * L;
   if (probs_out && !sl.d_probs) { int rc = alloc(e, sl.d_probs, mtok * kVocab); if (rc) return rc; }
@@ -998,7 +999,9 @@ int dcb_pack_rows(const dcb_config* cfg, const float* rows, int32_t batch, uint8
     return fail(nullptr, DCB_ERR_INVALID, "dcb_pack_rows: bad argument");
   const dcb_config& c = *cfg;
   dcb_engine* e = nullptr;   // messages go to the engine-less error slot (dcb_last_error(NULL))
-  if (c.pw_max > 255 || c.ip_max > 255) return fail(e, DCB_ERR_INVALID, "packed rows need PW_MAX, IP_MAX <= 255");
+  // the format keeps pw / ip and the ccs_bq id (at most CCS_BQ_MAX - 1) in one byte each and strand in 2 bits
+  if (c.pw_max > 255 || c.ip_max > 255 || c.strand_max > 3 || c.ccs_bq_max > 256)
+    return fail(e, DCB_ERR_INVALID, "packed rows need PW_MAX, IP_MAX <= 255, STRAND_MAX <= 3 and CCS_BQ_MAX <= 256");
   const PackedLayout pl = make_packed_layout(c.max_passes, c.max_length, c.use_ccs_bq ? 1 : 0);
   const int P = pl.P, L = pl.L, R = pl.R;
   bool bad = false;

@@ -130,8 +130,9 @@ int dcb_forward(dcb_engine* e, const float* rows, int32_t batch, uint32_t flags,
  * dcb_pack_rows: host helper (needs no GPU and no engine -- it belongs to the producer of the rows; only max_passes,
  * max_length, use_ccs_bq and the *_max fields of `cfg` are read), float32 rows [B, R, L] -> packed.  Returns DCB_ERR_INPUT_RANGE (and still writes
  * clamped output) if a base / strand / ccs / ccs_bq value is outside its vocabulary -- the values TensorFlow's gather
- * would raise on -- or an SN row is not constant along L; DCB_ERR_INVALID if the configuration cannot be packed
- * (PW_MAX or IP_MAX above 255). */
+ * would raise on -- or an SN row is not constant along L; DCB_ERR_INVALID if the configuration cannot be packed:
+ * PW_MAX or IP_MAX above 255, STRAND_MAX above 3 (two bits) or CCS_BQ_MAX above 256 (its largest id, CCS_BQ_MAX - 1,
+ * must fit a byte).  The packed entry points refuse such an engine with DCB_ERR_INVALID too. */
 size_t dcb_packed_window_bytes(const dcb_config* cfg);
 int dcb_pack_rows(const dcb_config* cfg, const float* rows, int32_t batch, uint8_t* packed_out);
 /* dcb_forward / dcb_submit on packed rows (host pointer, or device pointer with DCB_ROWS_ON_DEVICE: 16-byte aligned). */

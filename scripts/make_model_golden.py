@@ -101,6 +101,27 @@ def count_variables(obj, seen=None):
   return n
 
 
+def clip_boundaries(rows, p):
+  """Puts values on every clip and id boundary of `p` into synthetic rows [B, R, L, 1] (in place): PW / IP at, just
+  above and far beyond their maxima and below 0, SN on both sides of SN_MAX and far above 255, ccs_bq on its largest
+  id, strand on its largest id."""
+  from deepconsensus_b200 import params as params_lib
+  (bases, pw, ip, strand, ccs, bq, sn) = params_lib.get_indices(p.max_passes, p.use_ccs_bq)
+  for lo_hi, mx in ((pw, p.PW_MAX), (ip, p.IP_MAX)):
+    for i, v in enumerate((mx, mx + 0.5, mx + 1, 300.0, -3.0, mx - 0.5)):
+      rows[i % rows.shape[0], lo_hi[0]:lo_hi[1], 10 * i:10 * i + 10, 0] = v
+  sn_values = ((p.SN_MAX - 0.5, p.SN_MAX, 1500.0, 255.5), (256.0, p.SN_MAX + 0.25, 0.0, 300.7),
+               (p.SN_MAX + 0.5, 511.9, -2.0, p.SN_MAX - 1))
+  for b, vals in enumerate(sn_values[:rows.shape[0]]):
+    rows[b, sn[0]:sn[1], :, 0] = np.array(vals, np.float32)[:, None]
+  rows[0, bq[0], :50, 0] = p.CCS_BQ_MAX - 2                  # id CCS_BQ_MAX - 1: the table's last row
+  rows[1, bq[0], 50:, 0] = p.CCS_BQ_MAX - 2.5                # truncation toward zero: the id below it
+  rows[2, bq[0], :, 0] = -1.0                                # id 0: the zero vector
+  rows[0, strand[0]:strand[1], :, 0] = (np.arange(strand[1] - strand[0]) % (p.STRAND_MAX + 1))[:, None]
+  rows[1, strand[0]:strand[1], :, 0] = p.STRAND_MAX
+  return rows
+
+
 CASES = [
     # name, config, overrides, window source, seed.  (The reference's testdata windows are 85 rows = no CCS-BQ row.)
     dict(name="rezero_p20", config="transformer_learn_values+test", over={}, src="real", n=6, seed=11),
@@ -119,6 +140,36 @@ CASES = [
     dict(name="c5_p32_l200_ln_bq", config="transformer_learn_values+test",
          over=dict(max_passes=32, use_ccs_bq=True, rezero=False, num_hidden_layers=5), src="synthetic", L=200, n=2,
          seed=18),
+    # Embedding layouts a params.json can describe besides the default one (tests/test_embedding_layouts.py says which
+    # embed / condenser paths each reaches).  E = embedded width, Epad = E rounded up to 16.
+    # E = 127, Epad 128; widths 6/5/3/1/4 put 3+ input rows in one 8-column chunk; no positional table.
+    dict(name="layout_narrow_nopos", config="transformer_learn_values+test",
+         over=dict(max_passes=7, per_base_hidden_size=6, pw_hidden_size=5, ip_hidden_size=3, strand_hidden_size=1,
+                   sn_hidden_size=4, PW_MAX=100, IP_MAX=60, SN_MAX=30, add_pos_encoding=False, num_hidden_layers=2),
+         src="synthetic", L=40, n=3, seed=21),
+    # E = 126 (2 padding columns); the ccs_bq and strand tables off their default widths; pre-LayerNorm.
+    dict(name="layout_bq5_strand3_ln", config="transformer_learn_values+test",
+         over=dict(max_passes=3, use_ccs_bq=True, ccs_bq_hidden_size=5, strand_hidden_size=3, rezero=False,
+                   num_hidden_layers=2),
+         src="synthetic", L=40, n=3, seed=22),
+    # E = Epad = 1136: 71 condenser k-steps (odd) and not one chunk on the width-8 fast path.
+    dict(name="layout_wide16_bq", config="transformer_learn_values+test",
+         over=dict(max_passes=20, use_ccs_bq=True, per_base_hidden_size=16, pw_hidden_size=16, ip_hidden_size=16,
+                   strand_hidden_size=4, ccs_bq_hidden_size=16, sn_hidden_size=16, num_hidden_layers=2),
+         src="synthetic", L=100, n=3, seed=23),
+    # E = 66, Epad 80 (14 padding columns, 5 k-steps); the window fills one 128-token tile exactly; no positional table.
+    dict(name="layout_p1_l128_nopos_ln", config="transformer_learn_values+test",
+         over=dict(max_passes=1, add_pos_encoding=False, rezero=False, num_hidden_layers=2),
+         src="synthetic", L=128, n=3, seed=24),
+    # E = 1704, Epad 1712 (107 k-steps); 261 input rows of ids in the embed kernel's shared memory.
+    dict(name="layout_p64", config="transformer_learn_values+test",
+         over=dict(max_passes=64, num_hidden_layers=1),
+         src="synthetic", L=100, n=3, seed=25),
+    # Clip maxima off their defaults, at the largest values packed rows hold; rows on every clip boundary.
+    dict(name="layout_clip_maxima_bq", config="transformer_learn_values+test",
+         over=dict(max_passes=20, use_ccs_bq=True, PW_MAX=255, IP_MAX=9, SN_MAX=1000, STRAND_MAX=3, CCS_BQ_MAX=256,
+                   num_hidden_layers=2),
+         src="synthetic", L=100, n=3, seed=26, edit=clip_boundaries),
 ]
 
 
@@ -151,6 +202,8 @@ def main():
     else:
       rows = synthetic.make_rows(mine, case["n"], seed=case["seed"])
       rows = rows.reshape(case["n"], mine.total_rows, max_length, 1).astype(np.float32)
+    if "edit" in case:
+      rows = case["edit"](rows, mine)
     assert rows.shape[1] == params.total_rows
 
     model = networks.EncoderOnlyLearnedValuesTransformer(params)

@@ -581,7 +581,9 @@ def test_unfused_fallback_paths_agree_with_fused(engine_mod):
 
 
 @pytest.mark.parametrize("name", ["rezero_p20", "layernorm_p20", "rezero_p20_bq", "layernorm_p20_bq", "rezero_p5_win3",
-                                  "c2_p20_l120", "c5_p32_l200", "c5_p32_l200_ln_bq"])
+                                  "c2_p20_l120", "c5_p32_l200", "c5_p32_l200_ln_bq",
+                                  "layout_narrow_nopos", "layout_bq5_strand3_ln", "layout_wide16_bq",
+                                  "layout_p1_l128_nopos_ln", "layout_p64", "layout_clip_maxima_bq"])
 def test_engine_against_reference_code_goldens(engine_mod, golden_dir, name):
   """CUDA paths vs outputs of the reference's OWN model code (tests/golden/ref_model_*.npz, generated by
   scripts/make_model_golden.py) -- no oracle in between.  Includes the BASELINE configs[1] (P=20, L=120) and

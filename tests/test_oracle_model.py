@@ -86,7 +86,9 @@ def test_postprocess_matches_quick_inference_semantics():
 # ffn_layer.py / data_providers.format_rows / model_configs / model_utils.modify_params on a NumPy stand-in for the
 # TF primitives (scripts/make_model_golden.py + scripts/tf_shim.py).  Weights are regenerated from the seed.
 REF_MODEL_CASES = ["rezero_p20", "layernorm_p20", "rezero_p20_bq", "layernorm_p20_bq", "rezero_p5_win3",
-                   "c2_p20_l120", "c5_p32_l200", "c5_p32_l200_ln_bq"]
+                   "c2_p20_l120", "c5_p32_l200", "c5_p32_l200_ln_bq",
+                   "layout_narrow_nopos", "layout_bq5_strand3_ln", "layout_wide16_bq",
+                   "layout_p1_l128_nopos_ln", "layout_p64", "layout_clip_maxima_bq"]
 
 
 def _load_ref_case(golden_dir, name):
