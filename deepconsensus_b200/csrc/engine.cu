@@ -166,7 +166,7 @@ struct dcb_engine {
   struct { DevBuf<int16_t> bq; DevBuf<uint8_t> mask; DevBuf<double> avg; } sk;   // dcb_skip_mask
   struct { DevBuf<uint8_t> ids, bases, quals; DevBuf<int16_t> bq; DevBuf<int32_t> dst; DevBuf<int> status; } fs;   // dcb_fill_skipped
   struct { DevBuf<float> probs, loss; DevBuf<uint8_t> labels, ccs, exact; DevBuf<int32_t> pred, ccs_counts; } ev;   // dcb_evaluate
-  struct { DevBuf<float> teacher, student, loss; } ds;   // dcb_distill_loss
+  struct { DevBuf<float> teacher, student, loss, grad; } ds;   // dcb_distill_loss, dcb_distill_loss_grad
   struct { DevBuf<float> probs, loss, grad, matches, dp; DevBuf<uint8_t> labels; } lg;   // dcb_alignment_loss_grad
   struct { DevBuf<float> bias, logits, probs; DevBuf<uint8_t> bases, quals; } he;   // dcb_debug_head_epilogue
   cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;   // around the kernel of dcb_evaluate / _distill_loss / _loss_grad
@@ -1378,19 +1378,25 @@ int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const
   return DCB_OK;
 }
 
+// The argument checks of dcb_distill_loss and dcb_distill_loss_grad (`fn` names the call in the message).
+static int check_distill_args(dcb_engine* e, const char* fn, int32_t batch, int32_t L, double temperature, int32_t logit_loss) {
+  if (batch < 0 || L <= 0 || L > 256)
+    return fail(e, DCB_ERR_INVALID, "%s: need batch >= 0 and 0 < L <= 256 (batch=%d, L=%d)", fn, batch, L);
+  const float t32 = (float)temperature;   // the logits are divided in float32, as tf divides a float32 tensor
+  if (!std::isfinite(temperature) || !(temperature > 0.0) || !std::isfinite(t32) || !(t32 > 0.f))
+    return fail(e, DCB_ERR_INVALID, "%s: temperature must be finite and > 0 in float32 (got %g)", fn, temperature);
+  if (logit_loss != DCB_LOGIT_LOSS_MSE && logit_loss != DCB_LOGIT_LOSS_KL)
+    return fail(e, DCB_ERR_INVALID, "%s: unknown logit loss id %d (DCB_LOGIT_LOSS_MSE = %d, DCB_LOGIT_LOSS_KL = %d)",
+                fn, logit_loss, DCB_LOGIT_LOSS_MSE, DCB_LOGIT_LOSS_KL);
+  return DCB_OK;
+}
+
 int dcb_distill_loss(dcb_engine* e, const float* teacher_logits, const float* student_logits, int32_t batch,
                      int32_t L, double temperature, int32_t logit_loss, uint32_t flags, float* loss_out,
                      float* ms_out) {
   if (!e) return DCB_ERR_INVALID;
-  if (batch < 0 || L <= 0 || L > 256)
-    return fail(e, DCB_ERR_INVALID, "dcb_distill_loss: need batch >= 0 and 0 < L <= 256 (batch=%d, L=%d)", batch, L);
-  const float t32 = (float)temperature;   // the logits are divided in float32, as tf divides a float32 tensor
-  if (!std::isfinite(temperature) || !(temperature > 0.0) || !std::isfinite(t32) || !(t32 > 0.f))
-    return fail(e, DCB_ERR_INVALID, "dcb_distill_loss: temperature must be finite and > 0 in float32 (got %g)",
-                temperature);
-  if (logit_loss != DCB_LOGIT_LOSS_MSE && logit_loss != DCB_LOGIT_LOSS_KL)
-    return fail(e, DCB_ERR_INVALID, "dcb_distill_loss: unknown logit loss id %d (DCB_LOGIT_LOSS_MSE = %d, "
-                "DCB_LOGIT_LOSS_KL = %d)", logit_loss, DCB_LOGIT_LOSS_MSE, DCB_LOGIT_LOSS_KL);
+  int rc = check_distill_args(e, "dcb_distill_loss", batch, L, temperature, logit_loss);
+  if (rc) return rc;
   if (ms_out) *ms_out = 0.f;
   if (batch == 0) return DCB_OK;
   if (!teacher_logits || !student_logits || !loss_out)
@@ -1401,15 +1407,45 @@ int dcb_distill_loss(dcb_engine* e, const float* teacher_logits, const float* st
   const bool in_dev = flags & DCB_ROWS_ON_DEVICE;
   const float *d_teacher, *d_student;
   Output<float> loss;
-  int rc;
   if ((rc = stage_in(e, e->ds.teacher, teacher_logits, nlog, in_dev, &d_teacher)) ||
       (rc = stage_in(e, e->ds.student, student_logits, nlog, in_dev, &d_student)) ||
       (rc = stage_out(e, e->ds.loss, loss_out, (size_t)batch, false, &loss)))
     return rc;
   CU(e, cudaEventRecord(e->ev_eval0, st));
-  CU(e, launch_distill_loss(d_teacher, d_student, batch, L, t32, logit_loss, loss.d, st));
+  CU(e, launch_distill_loss(d_teacher, d_student, batch, L, (float)temperature, logit_loss, loss.d, st));
   CU(e, cudaEventRecord(e->ev_eval1, st));
   if ((rc = copy_out(e, loss))) return rc;
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  return DCB_OK;
+}
+
+int dcb_distill_loss_grad(dcb_engine* e, const float* teacher_logits, const float* student_logits, int32_t batch,
+                          int32_t L, double temperature, int32_t logit_loss, uint32_t flags, float* loss_out,
+                          float* grad_out, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  int rc = check_distill_args(e, "dcb_distill_loss_grad", batch, L, temperature, logit_loss);
+  if (rc) return rc;
+  if (ms_out) *ms_out = 0.f;
+  if (batch == 0) return DCB_OK;
+  if (!teacher_logits || !student_logits || !loss_out)
+    return fail(e, DCB_ERR_INVALID, "dcb_distill_loss_grad: null pointer");
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  const size_t nlog = (size_t)batch * L * kVocab;
+  const bool in_dev = flags & DCB_ROWS_ON_DEVICE, out_dev = flags & DCB_OUT_ON_DEVICE;
+  const float *d_teacher, *d_student;
+  Output<float> loss, grad;
+  if ((rc = stage_in(e, e->ds.teacher, teacher_logits, nlog, in_dev, &d_teacher)) ||
+      (rc = stage_in(e, e->ds.student, student_logits, nlog, in_dev, &d_student)) ||
+      (rc = stage_out(e, e->ds.loss, loss_out, (size_t)batch, out_dev, &loss)) ||
+      (rc = stage_out(e, e->ds.grad, grad_out, nlog, out_dev, &grad)))
+    return rc;
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  CU(e, launch_distill_loss_grad(d_teacher, d_student, batch, L, (float)temperature, logit_loss, loss.d, grad.d, st));
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  if ((rc = copy_out(e, loss)) || (rc = copy_out(e, grad))) return rc;
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));

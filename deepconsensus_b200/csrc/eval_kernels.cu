@@ -21,7 +21,8 @@
 //                           CTA also writes PerExampleAccuracy's exact-match flag (:43-65).
 //   distill_loss_kernel     DistillationLoss.call (:1170-1213) on teacher and student logits, one warp per window: the
 //                           temperature-scaled softmax of both, the Keras logit loss (mean squared error or KL
-//                           divergence) per position, the mean over the window.
+//                           divergence) per position, the mean over the window.  A compile-time variant also writes
+//                           the gradient with respect to the student's logits (same loss bits).
 // Results are deterministic: every reduction is a fixed-order loop, no atomics.
 #include <cuda_runtime.h>
 #include <math.h>
@@ -430,17 +431,29 @@ __device__ __forceinline__ void softmax5_scaled(const float* __restrict__ logits
   for (int c = 0; c < kVocab; ++c) p[c] = __fdiv_rn(x[c], sum);
 }
 
+//
+// kGrad adds d loss[b] / d student[b] (grad_out [B, L, 5]) with TensorFlow's gradient semantics, the teacher held
+// constant; the loss arithmetic is the same code, so both variants give the same loss bits.  Per position, with
+// inv_L = 1 / L (reduce_mean over the window):
+//   MSE  g_c = (2 (s_c - t_c) / 5) * inv_L
+//   KL   g_c = (-t'_c / s'_c) * inv_L where s_c lies in [1e-7, 1], else 0 (clip_by_value passes at its bounds and
+//        blocks outside them); t', s' the clipped probabilities
+// then the softmax backward and the division by T in front of it:
+//   grad_c = ((g_c - sum_c' g_c' s_c') * s_c) / T        (the sum in class order)
+// Each position is one lane's work, so the gradient needs no reduction at all.
+template <bool kGrad>
 __global__ void __launch_bounds__(kDistillWarps * 32)
 distill_loss_kernel(const float* __restrict__ teacher, const float* __restrict__ student, int B, int L,
-                    float temperature, int logit_loss, float* __restrict__ loss_out) {
+                    float temperature, int logit_loss, float* __restrict__ loss_out, float* __restrict__ grad_out) {
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * kDistillWarps + (threadIdx.x >> 5);
   if (b >= B) return;                                      // whole warps retire together
   const float* tw = teacher + (size_t)b * L * kVocab;
   const float* sw = student + (size_t)b * L * kVocab;
+  const float inv_L = __fdiv_rn(1.f, (float)L);
   float acc = 0.f;
   for (int j = lane; j < L; j += 32) {
-    float tl[kVocab], sl[kVocab], t[kVocab], s[kVocab];
+    float tl[kVocab], sl[kVocab], t[kVocab], s[kVocab], g[kVocab];
     for (int c = 0; c < kVocab; ++c) {
       tl[c] = __ldg(tw + j * kVocab + c);
       sl[c] = __ldg(sw + j * kVocab + c);
@@ -453,13 +466,21 @@ distill_loss_kernel(const float* __restrict__ teacher, const float* __restrict__
         const float tc = fminf(fmaxf(t[c], kEps), 1.f), sc = fminf(fmaxf(s[c], kEps), 1.f);
         const float term = __fmul_rn(tc, logf(__fdiv_rn(tc, sc)));
         v = c == 0 ? term : __fadd_rn(v, term);
+        if (kGrad) g[c] = s[c] >= kEps && s[c] <= 1.f ? __fmul_rn(-__fdiv_rn(tc, sc), inv_L) : 0.f;
       }
     } else {
       for (int c = 0; c < kVocab; ++c) {
         const float d = __fsub_rn(s[c], t[c]);
         v = c == 0 ? __fmul_rn(d, d) : __fadd_rn(v, __fmul_rn(d, d));
+        if (kGrad) g[c] = __fmul_rn(__fdiv_rn(__fmul_rn(2.f, d), (float)kVocab), inv_L);
       }
       v = __fdiv_rn(v, (float)kVocab);
+    }
+    if (kGrad) {
+      float dot = __fmul_rn(g[0], s[0]);
+      for (int c = 1; c < kVocab; ++c) dot = __fadd_rn(dot, __fmul_rn(g[c], s[c]));
+      float* gw = grad_out + ((size_t)b * L + j) * kVocab;
+      for (int c = 0; c < kVocab; ++c) gw[c] = __fdiv_rn(__fmul_rn(__fsub_rn(g[c], dot), s[c]), temperature);
     }
     acc = j == lane ? v : __fadd_rn(acc, v);
   }
@@ -470,8 +491,21 @@ distill_loss_kernel(const float* __restrict__ teacher, const float* __restrict__
 cudaError_t launch_distill_loss(const float* teacher, const float* student, int B, int L, float temperature,
                                 int logit_loss, float* loss, cudaStream_t st) {
   if (B <= 0) return cudaSuccess;
-  distill_loss_kernel<<<(B + kDistillWarps - 1) / kDistillWarps, kDistillWarps * 32, 0, st>>>(
-      teacher, student, B, L, temperature, logit_loss, loss);
+  distill_loss_kernel<false><<<(B + kDistillWarps - 1) / kDistillWarps, kDistillWarps * 32, 0, st>>>(
+      teacher, student, B, L, temperature, logit_loss, loss, nullptr);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_distill_loss_grad(const float* teacher, const float* student, int B, int L, float temperature,
+                                     int logit_loss, float* loss, float* grad, cudaStream_t st) {
+  if (B <= 0) return cudaSuccess;
+  const int grid = (B + kDistillWarps - 1) / kDistillWarps;
+  if (grad)
+    distill_loss_kernel<true><<<grid, kDistillWarps * 32, 0, st>>>(teacher, student, B, L, temperature, logit_loss,
+                                                                   loss, grad);
+  else
+    distill_loss_kernel<false><<<grid, kDistillWarps * 32, 0, st>>>(teacher, student, B, L, temperature, logit_loss,
+                                                                    loss, nullptr);
   return cudaGetLastError();
 }
 

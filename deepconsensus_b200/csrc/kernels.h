@@ -66,6 +66,10 @@ cudaError_t launch_loss_grad(const float* probs, const uint8_t* labels, int B, i
 // divergence (DCB_LOGIT_LOSS_*).  Device pointers.
 cudaError_t launch_distill_loss(const float* teacher, const float* student, int B, int L, float temperature,
                                 int logit_loss, float* loss, cudaStream_t st);
+// The same loss (identical bits) and, when grad is not null, its gradient d loss / d student [B, L, 5] with the
+// teacher held constant.  Device pointers.
+cudaError_t launch_distill_loss_grad(const float* teacher, const float* student, int B, int L, float temperature,
+                                     int logit_loss, float* loss, float* grad, cudaStream_t st);
 
 // ---- strict-fp32 path (strict_kernels.cu): row-major float32 activations, windows packed back to back
 void launch_strict_embed(const float* rows, int R, int L, int E, int nwindows, const StrictEmbedRow* meta,

@@ -86,7 +86,7 @@ ABI_SYMBOLS = (
     "dcb_create", "dcb_load_weights", "dcb_forward", "dcb_submit", "dcb_wait", "dcb_stitch", "dcb_last_forward_ms",
     "dcb_packed_window_bytes", "dcb_pack_rows", "dcb_forward_packed", "dcb_submit_packed",
     "dcb_stitch_fastq", "dcb_skip_mask", "dcb_fill_skipped", "dcb_evaluate", "dcb_distill_loss",
-    "dcb_alignment_loss_grad", "dcb_prep_open", "dcb_prep_set_threads", "dcb_prep_next_zmw", "dcb_prep_get_windows", "dcb_prep_ccs_header", "dcb_prep_close",
+    "dcb_alignment_loss_grad", "dcb_distill_loss_grad", "dcb_prep_open", "dcb_prep_set_threads", "dcb_prep_next_zmw", "dcb_prep_get_windows", "dcb_prep_ccs_header", "dcb_prep_close",
     "dcb_prep_last_error", "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
     "dcb_last_forward_launches", "dcb_set_profile", "dcb_get_profile", "dcb_get_profile_kernels", "dcb_alloc_host",
     "dcb_free_host", "dcb_alloc_device", "dcb_free_device", "dcb_memcpy_h2d", "dcb_memcpy_d2h",
@@ -147,6 +147,7 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_evaluate.argtypes = [vp, vp, vp, vp, i32, i32, f64, f64, i32, u32, vp, vp, vp, vp,
                                ctypes.POINTER(ctypes.c_float)]
   lib.dcb_distill_loss.argtypes = [vp, vp, vp, i32, i32, f64, i32, u32, vp, ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_distill_loss_grad.argtypes = [vp, vp, vp, i32, i32, f64, i32, u32, vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_alignment_loss_grad.argtypes = [vp, vp, vp, i32, i32, f64, f64, i32, u32, vp, vp, vp,
                                           ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
@@ -656,6 +657,44 @@ class B200Model:
                                            loss.ctypes.data_as(ctypes.c_void_p), ctypes.byref(ms)))
     return dict(loss=loss, ms=float(ms.value))
 
+  def distill_loss_grad(self, teacher_logits, student_logits, temperature: float = 1.0,
+                        logit_loss: Any = "kl_divergence", want_grad: bool = True, on_device: bool = False,
+                        batch: Optional[int] = None, length: Optional[int] = None,
+                        out: Optional[Dict[str, int]] = None) -> Dict[str, Any]:
+    """dcb_distill_loss_grad: per-window DistillationLoss (bitwise equal to distill_loss's) and its gradient with
+    respect to the student's logits, the teacher held constant.  Logits float32 [B, L, 5] are host arrays, or device
+    addresses with on_device=True, `batch` and optionally `length` (default max_length).  Returns loss float32 [B],
+    grad float32 [B, L, 5] (None unless want_grad) and ms, the kernel's device time.  With `out`, a dict of device
+    addresses for "loss" and, if wanted, "grad", the results are written there instead and returned as None."""
+    lid = logit_loss_id(logit_loss)
+    if on_device:
+      if batch is None:
+        raise ValueError("distill_loss_grad(on_device=True) needs batch")
+      B, L = int(batch), int(length) if length is not None else self.max_length
+      t_ptr, s_ptr, flags = ctypes.c_void_p(int(teacher_logits)), ctypes.c_void_p(int(student_logits)), DCB_ROWS_ON_DEVICE
+    else:
+      teacher = np.ascontiguousarray(teacher_logits, dtype=np.float32)
+      student = np.ascontiguousarray(student_logits, dtype=np.float32)
+      if teacher.ndim != 3 or teacher.shape[2] != 5 or student.shape != teacher.shape:
+        raise ValueError("teacher and student logits must both be float32 [B, L, 5], got %s and %s" %
+                         (teacher.shape, student.shape))
+      B, L = teacher.shape[:2]
+      t_ptr, s_ptr, flags = teacher.ctypes.data_as(ctypes.c_void_p), student.ctypes.data_as(ctypes.c_void_p), 0
+    res: Dict[str, Any] = dict(loss=None, grad=None)
+    if out is not None:
+      flags |= DCB_OUT_ON_DEVICE
+      ptrs = [ctypes.c_void_p(int(out["loss"])), ctypes.c_void_p(int(out["grad"])) if want_grad else None]
+    else:
+      res["loss"] = np.zeros(B, np.float32)
+      if want_grad:
+        res["grad"] = np.zeros((B, L, 5), np.float32)
+      ptrs = [None if res[k] is None else res[k].ctypes.data_as(ctypes.c_void_p) for k in ("loss", "grad")]
+    ms = ctypes.c_float()
+    self._check(self._lib.dcb_distill_loss_grad(self._handle, t_ptr, s_ptr, B, L, float(temperature), lid, flags,
+                                                *ptrs, ctypes.byref(ms)))
+    res["ms"] = float(ms.value)
+    return res
+
   def alignment_loss_grad(self, probs, labels, del_cost: Optional[float] = None, loss_reg: Any = "params",
                           band_width: Any = "params", want_grad: bool = True, want_matches: bool = False,
                           on_device: bool = False, batch: Optional[int] = None, length: Optional[int] = None,
@@ -851,6 +890,14 @@ class B200Model:
                                       ctypes.c_void_p(bases_ptr), ctypes.c_void_p(quals_ptr),
                                       ctypes.c_void_p(probs_ptr) if probs_ptr else None,
                                       ctypes.c_void_p(logits_ptr) if logits_ptr else None))
+
+  def forward_packed_raw(self, packed_ptr: int, batch: int, flags: int, bases_ptr: int, quals_ptr: int,
+                         probs_ptr: int = 0, logits_ptr: int = 0) -> None:
+    """dcb_forward_packed on caller-managed pointers (host or device per `flags`)."""
+    self._check(self._lib.dcb_forward_packed(self._handle, ctypes.c_void_p(packed_ptr), batch, flags,
+                                             ctypes.c_void_p(bases_ptr), ctypes.c_void_p(quals_ptr),
+                                             ctypes.c_void_p(probs_ptr) if probs_ptr else None,
+                                             ctypes.c_void_p(logits_ptr) if logits_ptr else None))
 
   def synchronize(self) -> None:
     self._check(self._lib.dcb_synchronize(self._handle))

@@ -120,3 +120,54 @@ def check_weights(params: params_lib.Params, weights: Weights) -> None:
     got = tuple(np.shape(weights[name]))
     if got != tuple(shape):
       raise ValueError("variable %s has shape %s, expected %s" % (name, got, tuple(shape)))
+
+
+def _copy_checked(dst: Weights, src: Weights, dst_name: str, src_name: str) -> None:
+  if dst_name not in dst or src_name not in src:
+    raise ValueError("cannot copy %s to %s: the %s has no such variable" %
+                     (src_name, dst_name, "student" if dst_name not in dst else "teacher"))
+  got, want = np.shape(src[src_name]), np.shape(dst[dst_name])
+  if tuple(got) != tuple(want):
+    raise ValueError("cannot copy %s %s to %s %s: shapes differ" % (src_name, tuple(got), dst_name, tuple(want)))
+  dst[dst_name] = np.array(src[src_name], dtype=np.float32)
+
+
+def _layer_index(i, n: int, which: str) -> int:
+  if isinstance(i, bool) or not isinstance(i, (int, np.integer)) or not -n <= int(i) < n:
+    raise ValueError("%s encoder layer %r out of range for %d layers" % (which, i, n))
+  return int(i) % n                  # a Python list index, as the reference indexes encoder_stack.layers
+
+
+def student_from_teacher(teacher_weights: Weights, teacher_params: params_lib.Params,
+                         student_params: params_lib.Params, student_init: Weights) -> Weights:
+  """init_student_from_teacher (model_distillation.py:104-144) on reference-named variables: the student's initial
+  variables `student_init` with the teacher's copied in, as student_params (the distillation config) asks.
+
+    init_encoder_stack      for every pair of dict(zip(teacher_encoder_layers, student_encoder_layers)), the
+                            attention and FFN layers' own variables, layers/t/{0,1}/layer/* -> layers/s/{0,1}/layer/*
+                            (`.layer.get_weights()`: the wrappers' alpha and layer_norm/* are not copied)
+    init_nonencoder_layers  the embeddings, the input condenser and fc1 (every layer with variables whose name does not
+                            contain 'encoder_stack'; encoder_stack/output_normalization is not copied)
+
+  Raises ValueError where Keras' set_weights would (a variable missing on either side, or a shape mismatch) and for an
+  encoder layer index outside either stack."""
+  out = {k: np.array(v, dtype=np.float32) for k, v in student_init.items()}
+  if student_params.get("init_encoder_stack"):
+    nt, ns = int(teacher_params.num_hidden_layers), int(student_params.num_hidden_layers)
+    pairs = dict(zip(student_params.teacher_encoder_layers, student_params.student_encoder_layers))
+    for t_id, s_id in pairs.items():
+      t, s = _layer_index(t_id, nt, "teacher"), _layer_index(s_id, ns, "student")
+      for sub in (0, 1):
+        t_pre, s_pre = ("model/encoder_stack/layers/%d/%d/layer/" % (n, sub) for n in (t, s))
+        t_names = sorted(k[len(t_pre):] for k in teacher_weights if k.startswith(t_pre))
+        s_names = sorted(k[len(s_pre):] for k in out if k.startswith(s_pre))
+        if t_names != s_names:
+          raise ValueError("teacher layer %d/%d and student layer %d/%d hold different variables: %s vs %s" %
+                           (t, sub, s, sub, t_names, s_names))
+        for leaf in t_names:
+          _copy_checked(out, teacher_weights, s_pre + leaf, t_pre + leaf)
+  if student_params.get("init_nonencoder_layers"):
+    for name in teacher_weights:
+      if not name.startswith("model/encoder_stack/"):
+        _copy_checked(out, teacher_weights, name, name)
+  return out

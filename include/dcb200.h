@@ -282,6 +282,22 @@ int dcb_distill_loss(dcb_engine* e, const float* teacher_logits, const float* st
                      int32_t L, double temperature, int32_t logit_loss, uint32_t flags, float* loss_out,
                      float* ms_out);
 
+/* The distillation term with its gradient, for training a student (model_distillation.py:281-318, whose tape holds the
+ * teacher's logits constant):
+ *   loss_out [B]          the loss, bitwise equal to dcb_distill_loss's loss_out on the same arguments
+ *   grad_out [B, L, 5]    d loss[b] / d student_logits[b] (nullable), float32, with TensorFlow's gradient semantics:
+ *                         per position the logit loss's gradient with respect to s -- MSE 2 (s_c - t_c) / 5, KL
+ *                         -t'_c / s'_c (t', s' clipped to [1e-7, 1]; 0 where s_c lies outside [1e-7, 1], as
+ *                         clip_by_value passes at its bounds and blocks outside them) -- times 1 / L (the mean over
+ *                         the window), then the softmax backward (g_c - sum_c' g_c' s_c') s_c and the division by T
+ * Arguments and checks as dcb_distill_loss.  Inputs are host arrays, or device arrays with DCB_ROWS_ON_DEVICE; outputs
+ * are host arrays, or device arrays with DCB_OUT_ON_DEVICE.  ms_out (nullable) receives the kernel's device time.
+ * Returns once the work on the engine's stream has finished.  Deterministic: no atomics; repeated calls, and host vs
+ * device pointers, give identical bits. */
+int dcb_distill_loss_grad(dcb_engine* e, const float* teacher_logits, const float* student_logits, int32_t batch,
+                          int32_t L, double temperature, int32_t logit_loss, uint32_t flags, float* loss_out,
+                          float* grad_out, float* ms_out);
+
 /* ---- feature construction from BAM (host C++, htslib-free, needs no GPU) -----------------------------------------------
  * What `deepconsensus run` does in front of the model: stream the subreads-to-CCS BAM ZMW by ZMW (SubreadGrouper,
  * pre_lib.py:50-91), expand / clip / indent every subread (expand_clip_indent with trim_insertions, :1061-1239), fetch

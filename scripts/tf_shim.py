@@ -45,10 +45,17 @@ class TensorShape:
 
 
 # --------------------------------------------------------------------------- keras base classes
+def _snake_case(name):
+  return "".join("_" + c.lower() if c.isupper() and i else c.lower() for i, c in enumerate(name))
+
+
 class Layer:
+  # attributes that hold arrays but are not variables (count_variables in make_model_golden.py skips the same)
+  _NOT_VARIABLES = ("params", "attn_mask")
+
   def __init__(self, *args, name=None, dtype=None, **kwargs):
     self._built = False
-    self.name = name
+    self.name = name or _snake_case(type(self).__name__)   # Keras' default name, without the uniquifying suffix
 
   def build(self, input_shape):
     self._built = True
@@ -60,10 +67,68 @@ class Layer:
       self._built = True
     return self.call(*args, **kwargs)
 
+  def _variables(self):
+    """(owner, attribute) of every variable this layer and its sublayers hold, in attribute order (layer.weights)."""
+    out, seen = [], set()
+
+    def walk(obj):
+      if id(obj) in seen:
+        return
+      seen.add(id(obj))
+      if isinstance(obj, Layer):
+        for k, v in vars(obj).items():
+          if k in self._NOT_VARIABLES:
+            continue
+          if isinstance(v, np.ndarray):
+            out.append((obj, k))
+          elif isinstance(v, (Layer, list, tuple)):
+            walk(v)
+        return
+      for v in obj:   # a list of layers
+        if isinstance(v, (Layer, list, tuple)):
+          walk(v)
+
+    walk(self)
+    return out
+
+  @property
+  def trainable_weights(self):
+    return [getattr(o, k) for o, k in self._variables()]
+
+  def get_weights(self):
+    return [np.array(getattr(o, k)) for o, k in self._variables()]
+
+  def set_weights(self, weights):
+    """keras Layer.set_weights: ValueError on a count or shape mismatch."""
+    slots = self._variables()
+    if len(weights) != len(slots):
+      raise ValueError("layer %s expects %d weights, got %d" % (self.name, len(slots), len(weights)))
+    for (o, k), w in zip(slots, weights):
+      if np.shape(getattr(o, k)) != np.shape(w):
+        raise ValueError("layer %s weight %s has shape %s, got %s" % (self.name, k, np.shape(getattr(o, k)),
+                                                                      np.shape(w)))
+    for (o, k), w in zip(slots, weights):
+      setattr(o, k, np.array(w, dtype=F32))
+
 
 class Model(Layer):
   def summary(self):
     pass
+
+  def __call__(self, *args, **kwargs):
+    if len(args) < 2 and "training" not in kwargs:   # keras passes the learning phase: inference
+      kwargs["training"] = False
+    return super().__call__(*args, **kwargs)
+
+  @property
+  def layers(self):
+    """The directly tracked sublayers, in the order they were assigned (keras Model.layers)."""
+    return [v for v in vars(self).values() if isinstance(v, Layer)]
+
+  def get_layer(self, name=None, index=None):
+    if index is not None:
+      return self.layers[index]
+    return next(layer for layer in self.layers if layer.name == name)
 
 
 def _activation(a):
