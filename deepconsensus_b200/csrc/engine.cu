@@ -1335,22 +1335,44 @@ int dcb_debug_head_epilogue(dcb_engine* e, const float* logits, int64_t n, uint8
   return DCB_OK;
 }
 
+// The argument checks of dcb_evaluate and dcb_alignment_loss_grad (`fn` names the call in the message).
+static int check_alignment_args(dcb_engine* e, const char* fn, int32_t batch, int32_t L, double del_cost, int32_t band_width) {
+  if (band_width >= 0)
+    return fail(e, DCB_ERR_INVALID, "%s: the banded alignment loss (band_width=%d) is not supported; pass "
+                "DCB_BAND_WIDTH_NONE (params.band_width None, as the released models are trained)", fn, band_width);
+  if (batch < 0 || L <= 0 || L > 256)
+    return fail(e, DCB_ERR_INVALID, "%s: need batch >= 0 and 0 < L <= 256 (batch=%d, L=%d)", fn, batch, L);
+  if (!(del_cost == del_cost)) return fail(e, DCB_ERR_INVALID, "%s: del_cost is NaN", fn);
+  return DCB_OK;
+}
+
+// Every label must be a base id 0..4.  Device labels are read back to the host first.
+static int check_labels(dcb_engine* e, const char* fn, const uint8_t* labels, int32_t batch, int32_t L, bool on_device) {
+  const size_t ntok = (size_t)batch * L;
+  std::vector<uint8_t> copy;
+  if (on_device) {
+    copy.resize(ntok);
+    CU(e, cudaMemcpyAsync(copy.data(), labels, ntok, cudaMemcpyDeviceToHost, e->stream));
+    CU(e, cudaStreamSynchronize(e->stream));
+    labels = copy.data();
+  }
+  for (size_t i = 0; i < ntok; ++i)
+    if (labels[i] > 4) return fail(e, DCB_ERR_INVALID, "%s: label id %d outside 0..4 at window %zu", fn, labels[i], i / L);
+  return DCB_OK;
+}
+
 int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const uint8_t* ccs_ids, int32_t batch,
                  int32_t L, double del_cost, double loss_reg, int32_t band_width, uint32_t flags, float* loss_out,
                  uint8_t* exact_out, int32_t* pred_counts, int32_t* ccs_counts, float* ms_out) {
   if (!e) return DCB_ERR_INVALID;
-  if (band_width >= 0)
-    return fail(e, DCB_ERR_INVALID, "dcb_evaluate: the banded alignment loss (band_width=%d) is not supported; "
-                "pass DCB_BAND_WIDTH_NONE (params.band_width None, as the released models are trained)", band_width);
-  if (batch < 0 || L <= 0 || L > 256) return fail(e, DCB_ERR_INVALID, "dcb_evaluate: need batch >= 0 and 0 < L <= 256");
-  if (!(del_cost == del_cost)) return fail(e, DCB_ERR_INVALID, "dcb_evaluate: del_cost is NaN");
+  int rc = check_alignment_args(e, "dcb_evaluate", batch, L, del_cost, band_width);
+  if (rc) return rc;
   if (ms_out) *ms_out = 0.f;
   if (batch == 0) return DCB_OK;
   if (!probs || !labels || !ccs_ids || !loss_out || !exact_out || !pred_counts || !ccs_counts)
     return fail(e, DCB_ERR_INVALID, "dcb_evaluate: null pointer");
   const size_t ntok = (size_t)batch * L;
-  for (size_t i = 0; i < ntok; ++i)
-    if (labels[i] > 4) return fail(e, DCB_ERR_INVALID, "dcb_evaluate: label id %d outside 0..4 at window %zu", labels[i], i / L);
+  if ((rc = check_labels(e, "dcb_evaluate", labels, batch, L, false))) return rc;
   CU(e, cudaSetDevice(e->cfg.device));
   cudaStream_t st = e->stream;
   const float* d_probs;
@@ -1358,7 +1380,6 @@ int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const
   Output<float> loss;
   Output<int32_t> pred, ccs;
   Output<uint8_t> exact;
-  int rc;
   if ((rc = stage_in(e, e->ev.probs, probs, ntok * kVocab, flags & DCB_ROWS_ON_DEVICE, &d_probs)) ||
       (rc = stage_in(e, e->ev.labels, labels, ntok, false, &d_labels)) || (rc = stage_in(e, e->ev.ccs, ccs_ids, ntok, false, &d_ccs)) ||
       (rc = stage_out(e, e->ev.loss, loss_out, (size_t)batch, false, &loss)) ||
@@ -1391,46 +1412,17 @@ static int check_distill_args(dcb_engine* e, const char* fn, int32_t batch, int3
   return DCB_OK;
 }
 
-int dcb_distill_loss(dcb_engine* e, const float* teacher_logits, const float* student_logits, int32_t batch,
-                     int32_t L, double temperature, int32_t logit_loss, uint32_t flags, float* loss_out,
-                     float* ms_out) {
+// dcb_distill_loss and dcb_distill_loss_grad: the loss, and its gradient when grad_out is not null (`fn` names the call
+// in messages).
+static int distill_impl(dcb_engine* e, const char* fn, const float* teacher_logits, const float* student_logits,
+                        int32_t batch, int32_t L, double temperature, int32_t logit_loss, uint32_t flags, float* loss_out,
+                        float* grad_out, float* ms_out) {
   if (!e) return DCB_ERR_INVALID;
-  int rc = check_distill_args(e, "dcb_distill_loss", batch, L, temperature, logit_loss);
+  int rc = check_distill_args(e, fn, batch, L, temperature, logit_loss);
   if (rc) return rc;
   if (ms_out) *ms_out = 0.f;
   if (batch == 0) return DCB_OK;
-  if (!teacher_logits || !student_logits || !loss_out)
-    return fail(e, DCB_ERR_INVALID, "dcb_distill_loss: null pointer");
-  CU(e, cudaSetDevice(e->cfg.device));
-  cudaStream_t st = e->stream;
-  const size_t nlog = (size_t)batch * L * kVocab;
-  const bool in_dev = flags & DCB_ROWS_ON_DEVICE;
-  const float *d_teacher, *d_student;
-  Output<float> loss;
-  if ((rc = stage_in(e, e->ds.teacher, teacher_logits, nlog, in_dev, &d_teacher)) ||
-      (rc = stage_in(e, e->ds.student, student_logits, nlog, in_dev, &d_student)) ||
-      (rc = stage_out(e, e->ds.loss, loss_out, (size_t)batch, false, &loss)))
-    return rc;
-  CU(e, cudaEventRecord(e->ev_eval0, st));
-  CU(e, launch_distill_loss(d_teacher, d_student, batch, L, (float)temperature, logit_loss, loss.d, st));
-  CU(e, cudaEventRecord(e->ev_eval1, st));
-  if ((rc = copy_out(e, loss))) return rc;
-  CU(e, cudaStreamSynchronize(st));
-  CU(e, cudaGetLastError());
-  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
-  return DCB_OK;
-}
-
-int dcb_distill_loss_grad(dcb_engine* e, const float* teacher_logits, const float* student_logits, int32_t batch,
-                          int32_t L, double temperature, int32_t logit_loss, uint32_t flags, float* loss_out,
-                          float* grad_out, float* ms_out) {
-  if (!e) return DCB_ERR_INVALID;
-  int rc = check_distill_args(e, "dcb_distill_loss_grad", batch, L, temperature, logit_loss);
-  if (rc) return rc;
-  if (ms_out) *ms_out = 0.f;
-  if (batch == 0) return DCB_OK;
-  if (!teacher_logits || !student_logits || !loss_out)
-    return fail(e, DCB_ERR_INVALID, "dcb_distill_loss_grad: null pointer");
+  if (!teacher_logits || !student_logits || !loss_out) return fail(e, DCB_ERR_INVALID, "%s: null pointer", fn);
   CU(e, cudaSetDevice(e->cfg.device));
   cudaStream_t st = e->stream;
   const size_t nlog = (size_t)batch * L * kVocab;
@@ -1452,16 +1444,27 @@ int dcb_distill_loss_grad(dcb_engine* e, const float* teacher_logits, const floa
   return DCB_OK;
 }
 
+int dcb_distill_loss(dcb_engine* e, const float* teacher_logits, const float* student_logits, int32_t batch,
+                     int32_t L, double temperature, int32_t logit_loss, uint32_t flags, float* loss_out,
+                     float* ms_out) {
+  // loss_out is always a host array: DCB_OUT_ON_DEVICE does not apply here
+  return distill_impl(e, "dcb_distill_loss", teacher_logits, student_logits, batch, L, temperature, logit_loss,
+                      flags & ~DCB_OUT_ON_DEVICE, loss_out, nullptr, ms_out);
+}
+
+int dcb_distill_loss_grad(dcb_engine* e, const float* teacher_logits, const float* student_logits, int32_t batch,
+                          int32_t L, double temperature, int32_t logit_loss, uint32_t flags, float* loss_out,
+                          float* grad_out, float* ms_out) {
+  return distill_impl(e, "dcb_distill_loss_grad", teacher_logits, student_logits, batch, L, temperature, logit_loss,
+                      flags, loss_out, grad_out, ms_out);
+}
+
 int dcb_alignment_loss_grad(dcb_engine* e, const float* probs, const uint8_t* labels, int32_t batch, int32_t L,
                             double del_cost, double loss_reg, int32_t band_width, uint32_t flags, float* loss_out,
                             float* grad_out, float* matches_out, float* ms_out) {
   if (!e) return DCB_ERR_INVALID;
-  if (band_width >= 0)
-    return fail(e, DCB_ERR_INVALID, "dcb_alignment_loss_grad: the banded alignment loss (band_width=%d) is not "
-                "supported; pass DCB_BAND_WIDTH_NONE", band_width);
-  if (batch < 0 || L <= 0 || L > 256)
-    return fail(e, DCB_ERR_INVALID, "dcb_alignment_loss_grad: need batch >= 0 and 0 < L <= 256 (batch=%d, L=%d)", batch, L);
-  if (!(del_cost == del_cost)) return fail(e, DCB_ERR_INVALID, "dcb_alignment_loss_grad: del_cost is NaN");
+  int rc = check_alignment_args(e, "dcb_alignment_loss_grad", batch, L, del_cost, band_width);
+  if (rc) return rc;
   if (ms_out) *ms_out = 0.f;
   if (batch == 0) return DCB_OK;
   if (!probs || !labels || !loss_out) return fail(e, DCB_ERR_INVALID, "dcb_alignment_loss_grad: null pointer");
@@ -1469,23 +1472,12 @@ int dcb_alignment_loss_grad(dcb_engine* e, const float* probs, const uint8_t* la
   cudaStream_t st = e->stream;
   const bool in_dev = flags & DCB_ROWS_ON_DEVICE, out_dev = flags & DCB_OUT_ON_DEVICE;
   const size_t ntok = (size_t)batch * L;
-  const uint8_t* hl = labels;
-  std::vector<uint8_t> lab_copy;
-  if (in_dev) {   // the label check reads them on the host
-    lab_copy.resize(ntok);
-    CU(e, cudaMemcpyAsync(lab_copy.data(), labels, ntok, cudaMemcpyDeviceToHost, st));
-    CU(e, cudaStreamSynchronize(st));
-    hl = lab_copy.data();
-  }
-  for (size_t i = 0; i < ntok; ++i)
-    if (hl[i] > 4)
-      return fail(e, DCB_ERR_INVALID, "dcb_alignment_loss_grad: label id %d outside 0..4 at window %zu", hl[i], i / L);
+  if ((rc = check_labels(e, "dcb_alignment_loss_grad", labels, batch, L, in_dev))) return rc;
   int ctas = 0;
   CU(e, loss_grad_grid(batch, &ctas));
   const float* d_probs;
   const uint8_t* d_labels;
   Output<float> loss, grad, match;
-  int rc;
   if ((rc = ensure(e, e->lg.dp, loss_grad_table_bytes(L, ctas) / sizeof(float))) ||
       (rc = stage_in(e, e->lg.probs, probs, ntok * kVocab, in_dev, &d_probs)) ||
       (rc = stage_in(e, e->lg.labels, labels, ntok, in_dev, &d_labels)) ||

@@ -488,14 +488,6 @@ distill_loss_kernel(const float* __restrict__ teacher, const float* __restrict__
   if (lane == 0) loss_out[b] = __fdiv_rn(acc, (float)L);
 }
 
-cudaError_t launch_distill_loss(const float* teacher, const float* student, int B, int L, float temperature,
-                                int logit_loss, float* loss, cudaStream_t st) {
-  if (B <= 0) return cudaSuccess;
-  distill_loss_kernel<false><<<(B + kDistillWarps - 1) / kDistillWarps, kDistillWarps * 32, 0, st>>>(
-      teacher, student, B, L, temperature, logit_loss, loss, nullptr);
-  return cudaGetLastError();
-}
-
 cudaError_t launch_distill_loss_grad(const float* teacher, const float* student, int B, int L, float temperature,
                                      int logit_loss, float* loss, float* grad, cudaStream_t st) {
   if (B <= 0) return cudaSuccess;

@@ -63,11 +63,8 @@ cudaError_t launch_loss_grad(const float* probs, const uint8_t* labels, int B, i
                              int hard_min, float* tables, int ctas, float* loss, float* grad, float* matches,
                              cudaStream_t st);
 // DistillationLoss per window from teacher / student logits [B, L, 5]; logit_loss 0 = mean squared error, 1 = KL
-// divergence (DCB_LOGIT_LOSS_*).  Device pointers.
-cudaError_t launch_distill_loss(const float* teacher, const float* student, int B, int L, float temperature,
-                                int logit_loss, float* loss, cudaStream_t st);
-// The same loss (identical bits) and, when grad is not null, its gradient d loss / d student [B, L, 5] with the
-// teacher held constant.  Device pointers.
+// divergence (DCB_LOGIT_LOSS_*).  When grad is not null, also its gradient d loss / d student [B, L, 5] with the
+// teacher held constant; the loss bits are the same either way.  Device pointers.
 cudaError_t launch_distill_loss_grad(const float* teacher, const float* student, int B, int L, float temperature,
                                      int logit_loss, float* loss, float* grad, cudaStream_t st);
 

@@ -15,7 +15,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from typing import Any, Dict, Optional, Tuple
+from typing import Any, Callable, Dict, Iterable, Iterator, List, Optional, Tuple
 
 import numpy as np
 
@@ -139,7 +139,7 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_pack_rows.argtypes = [ctypes.POINTER(DcbConfig), vp, i32, vp]
   lib.dcb_forward_packed.argtypes = [vp, vp, i32, u32, vp, vp, vp, vp]
   lib.dcb_submit_packed.argtypes = [vp, vp, i32, u32, vp, vp, vp, vp, ctypes.POINTER(ctypes.c_int64)]
-  lib.dcb_stitch.argtypes = [vp, vp, vp, i32, i32, ctypes.POINTER(i32), i32, u32, vp, vp, vp]
+  lib.dcb_stitch.argtypes = [vp, vp, vp, i32, i32, vp, i32, u32, vp, vp, vp]
   f64 = ctypes.c_double
   lib.dcb_stitch_fastq.argtypes = [vp, vp, vp, i32, i32, vp, i32, vp, vp, vp, f64, i32, u32, vp, ctypes.c_int64, vp, vp, vp]
   lib.dcb_skip_mask.argtypes = [vp, vp, i32, i32, f64, vp, vp]
@@ -221,6 +221,48 @@ class _Prediction:
     return self._array
 
 
+def _ptr(x: Any) -> Optional[ctypes.c_void_p]:
+  """A void* argument: an ndarray's data, or an integer address (0 or None: NULL)."""
+  if isinstance(x, np.ndarray):
+    return x.ctypes.data_as(ctypes.c_void_p)
+  return ctypes.c_void_p(int(x)) if x else None
+
+
+def _arg(x: Any, dtype: Any, on_device: bool = False) -> Tuple[Optional[ctypes.c_void_p], Optional[np.ndarray]]:
+  """A host-or-device input: with on_device a device address, else x as a C-contiguous `dtype` array.  Returns the
+  pointer and the array it points into (None for an address), which must stay alive until the call returns."""
+  if on_device:
+    return _ptr(x), None
+  a = np.ascontiguousarray(x, dtype=dtype)
+  return _ptr(a), a
+
+
+def _outputs(out: Optional[Dict[str, int]], shapes: Dict[str, Optional[Tuple[int, ...]]]):
+  """float32 outputs of a call that can write device memory; shapes[k] is None for an output not wanted.  With `out`, a
+  dict of device addresses, the results go there (DCB_OUT_ON_DEVICE) and come back as None; otherwise host arrays are
+  allocated.  Returns (flag, pointers in the order of `shapes`, result dict)."""
+  res: Dict[str, Any] = dict.fromkeys(shapes)
+  if out is not None:
+    return DCB_OUT_ON_DEVICE, [None if shape is None else _ptr(out[k]) for k, shape in shapes.items()], res
+  for k, shape in shapes.items():
+    if shape is not None:
+      res[k] = np.zeros(shape, np.float32)
+  return 0, [_ptr(res[k]) for k in shapes], res
+
+
+def _rows3(params: params_lib.Params, rows: np.ndarray) -> np.ndarray:
+  """float32 rows [B, R, L(,1)] of `params`' geometry as a C-contiguous float32 [B, R, L] array."""
+  rows = np.asarray(rows)
+  if rows.ndim == 4:
+    if rows.shape[-1] != 1:
+      raise ValueError("rows must be [B, R, L, 1]")
+    rows = rows[..., 0]
+  R, L = params_lib.get_total_rows(params.max_passes, params.use_ccs_bq), int(params.max_length)
+  if rows.ndim != 3 or rows.shape[1] != R or rows.shape[2] != L:
+    raise ValueError("rows must be [B, %d, %d(, 1)], got %s" % (R, L, rows.shape))
+  return np.ascontiguousarray(rows, dtype=np.float32)
+
+
 class B200Model:
   """The encoder-only learned-values transformer on one H100, behind the C-ABI."""
 
@@ -282,17 +324,6 @@ class B200Model:
     self._check(self._lib.dcb_load_weights(self._handle, tensors, len(weights)))
 
   # -- the hot path ------------------------------------------------------------------------
-  def _rows3(self, rows: np.ndarray) -> np.ndarray:
-    rows = np.asarray(rows)
-    if rows.ndim == 4:
-      if rows.shape[-1] != 1:
-        raise ValueError("rows must be [B, R, L, 1]")
-      rows = rows[..., 0]
-    if rows.ndim != 3 or rows.shape[1] != self.total_rows or rows.shape[2] != self.max_length:
-      raise ValueError("rows must be [B, %d, %d(, 1)], got %s" %
-                       (self.total_rows, self.max_length, rows.shape))
-    return np.ascontiguousarray(rows, dtype=np.float32)
-
   @staticmethod
   def _precision_flag(strict: Optional[bool]) -> int:
     return 0 if strict is None else (DCB_STRICT_FP32 if strict else DCB_FAST_BF16)
@@ -304,8 +335,14 @@ class B200Model:
     Batches larger than `max_batch` are split, like `batch_examples` does with
     `options.batch_size` (quick_inference.py:304-338).
     """
-    rows = self._rows3(rows)
-    B, L = rows.shape[0], self.max_length
+    return self._forward_chunks(self._lib.dcb_forward, _rows3(self.params, rows), want_probs, want_logits,
+                                strict_input, strict)
+
+  def _forward_chunks(self, fn, x: np.ndarray, want_probs: bool, want_logits: bool, strict_input: bool,
+                      strict: Optional[bool]) -> Dict[str, np.ndarray]:
+    """forward() / forward_packed() on validated input x [B, ...]: dcb_forward or dcb_forward_packed (`fn`) per
+    max_batch chunk into host arrays."""
+    B, L = x.shape[0], self.max_length
     out = dict(bases=np.empty((B, L), np.uint8), quals=np.empty((B, L), np.uint8))
     if want_probs:
       out["probs"] = np.empty((B, L, 5), np.float32)
@@ -314,14 +351,18 @@ class B200Model:
     ms, launches = 0.0, 0
     for b0 in range(0, B, self.max_batch):
       b1 = min(B, b0 + self.max_batch)
-      ptr = lambda k: out[k][b0:b1].ctypes.data_as(ctypes.c_void_p) if k in out else None
-      rc = self._lib.dcb_forward(self._handle, rows[b0:b1].ctypes.data_as(ctypes.c_void_p), b1 - b0,
-                                 self._precision_flag(strict), ptr("bases"), ptr("quals"), ptr("probs"), ptr("logits"))
-      self._check(rc, tolerate=() if strict_input else (-5,))
+      part = [out[k][b0:b1] if k in out else None for k in ("bases", "quals", "probs", "logits")]
+      self._forward_chunk(fn, x[b0:b1], self._precision_flag(strict), *part, strict_input=strict_input)
       ms += self.last_forward_ms()
       launches += self.last_forward_launches()
     self.last_ms, self.last_launches = ms, launches
     return out
+
+  def _forward_chunk(self, fn, x: np.ndarray, flags: int, bases, quals, probs, logits, strict_input: bool) -> None:
+    """One dcb_forward / dcb_forward_packed call on at most max_batch windows; outputs are host arrays or device
+    addresses (per `flags`), None for one not wanted."""
+    rc = fn(self._handle, _ptr(x), x.shape[0], flags, _ptr(bases), _ptr(quals), _ptr(probs), _ptr(logits))
+    self._check(rc, tolerate=() if strict_input else (-5,))
 
   # -- packed input rows (include/dcb200.h "packed input rows")1) -------------------------
   @property
@@ -338,31 +379,13 @@ class B200Model:
     packed = np.ascontiguousarray(packed, dtype=np.uint8)
     if packed.ndim != 2 or packed.shape[1] != self.packed_window_bytes:
       raise ValueError("packed rows must be uint8 [B, %d]" % self.packed_window_bytes)
-    B, L = packed.shape[0], self.max_length
-    out = dict(bases=np.empty((B, L), np.uint8), quals=np.empty((B, L), np.uint8))
-    if want_probs:
-      out["probs"] = np.empty((B, L, 5), np.float32)
-    if want_logits:
-      out["logits"] = np.empty((B, L, 5), np.float32)
-    ms, launches = 0.0, 0
-    for b0 in range(0, B, self.max_batch):
-      b1 = min(B, b0 + self.max_batch)
-      ptr = lambda k: out[k][b0:b1].ctypes.data_as(ctypes.c_void_p) if k in out else None
-      rc = self._lib.dcb_forward_packed(self._handle, packed[b0:b1].ctypes.data_as(ctypes.c_void_p), b1 - b0,
-                                        self._precision_flag(strict), ptr("bases"), ptr("quals"), ptr("probs"),
-                                        ptr("logits"))
-      self._check(rc, tolerate=() if strict_input else (-5,))
-      ms += self.last_forward_ms()
-      launches += self.last_forward_launches()
-    self.last_ms, self.last_launches = ms, launches
-    return out
+    return self._forward_chunks(self._lib.dcb_forward_packed, packed, want_probs, want_logits, strict_input, strict)
 
   def submit_packed_raw(self, packed_ptr: int, batch: int, flags: int, bases_ptr: int, quals_ptr: int) -> int:
     """dcb_submit_packed on caller-managed pointers; returns the ticket for wait_raw()."""
     ticket = ctypes.c_int64(-1)
-    self._check(self._lib.dcb_submit_packed(self._handle, ctypes.c_void_p(packed_ptr), batch, flags,
-                                            ctypes.c_void_p(bases_ptr), ctypes.c_void_p(quals_ptr), None, None,
-                                            ctypes.byref(ticket)))
+    self._check(self._lib.dcb_submit_packed(self._handle, _ptr(packed_ptr), batch, flags, _ptr(bases_ptr),
+                                            _ptr(quals_ptr), None, None, ctypes.byref(ticket)))
     return int(ticket.value)
 
   # -- the hot path, pipelined over a stream of batches ----------------------------------------
@@ -370,33 +393,19 @@ class B200Model:
   # (two sets, allocated on first use) is owned here so that callers can stack their windows straight into it.
   def staging_rows(self, slot: int) -> np.ndarray:
     """Pinned float32 [max_batch, R, L] buffer of pipeline slot 0/1 (fill [:batch], then submit(slot=...))."""
-    st = self._staging(slot)
-    return st["rows"]
+    return self._staging(slot, "rows")
 
-  def _staging(self, slot: int) -> Dict[str, Any]:
-    if not hasattr(self, "_stage"):
-      self._stage = {}
-    if slot not in self._stage:
-      mb, R, L = self.max_batch, self.total_rows, self.max_length
-      def pinned(shape, dtype):
-        n = int(np.prod(shape)) * np.dtype(dtype).itemsize
-        addr, raw = alloc_pinned(max(n, 1))
-        return addr, raw[:n].view(dtype).reshape(shape)
-      st = {"addrs": []}
-      for key, shape, dt in (("rows", (mb, R, L), np.float32), ("bases", (mb, L), np.uint8),
-                             ("quals", (mb, L), np.uint8)):
-        addr, st[key] = pinned(shape, dt)
-        st["addrs"].append(addr)
-      self._stage[slot] = st
-    return self._stage[slot]
-
-  def _staging_opt(self, slot: int, key: str) -> np.ndarray:
-    st = self._staging(slot)
+  def _staging(self, slot: int, key: str) -> np.ndarray:
+    """Pinned buffer `key` (rows, bases, quals, probs or logits) of pipeline slot 0/1, allocated on first use."""
+    st = self.__dict__.setdefault("_stage", {}).setdefault(slot, {"addrs": []})
     if key not in st:
-      n = self.max_batch * self.max_length * 5 * 4
-      addr, raw = alloc_pinned(n)
-      st[key] = raw.view(np.float32).reshape(self.max_batch, self.max_length, 5)
+      mb, R, L = self.max_batch, self.total_rows, self.max_length
+      shape, dtype = {"rows": ((mb, R, L), np.float32), "bases": ((mb, L), np.uint8), "quals": ((mb, L), np.uint8),
+                      "probs": ((mb, L, 5), np.float32), "logits": ((mb, L, 5), np.float32)}[key]
+      n = int(np.prod(shape)) * np.dtype(dtype).itemsize
+      addr, raw = alloc_pinned(max(n, 1))
       st["addrs"].append(addr)
+      st[key] = raw[:n].view(dtype).reshape(shape)
     return st[key]
 
   def submit(self, rows: Optional[np.ndarray] = None, batch: Optional[int] = None, slot: Optional[int] = None,
@@ -412,23 +421,20 @@ class B200Model:
     if busy[slot]:   # its pinned staging may still be read by the copy engine: refuse before touching it
       raise DcbError(-4, "two submissions in flight: wait() for the oldest first")
     self._last_slot = slot
-    st = self._staging(slot)
+    staged = self._staging(slot, "rows")
     if rows is not None:
-      rows = self._rows3(rows)
+      rows = _rows3(self.params, rows)
       batch = rows.shape[0]
       if batch > self.max_batch:
         raise ValueError("submit(): batch %d > max_batch %d" % (batch, self.max_batch))
-      st["rows"][:batch] = rows
+      staged[:batch] = rows
     elif batch is None:
       raise ValueError("submit(): rows or batch required")
-    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    probs = self._staging_opt(slot, "probs") if want_probs else None
-    logits = self._staging_opt(slot, "logits") if want_logits else None
+    out = [self._staging(slot, k) if want else None
+           for k, want in (("bases", True), ("quals", True), ("probs", want_probs), ("logits", want_logits))]
     ticket = ctypes.c_int64(-1)
-    self._check(self._lib.dcb_submit(self._handle, vp(st["rows"]), batch, self._precision_flag(strict),
-                                     vp(st["bases"]), vp(st["quals"]),
-                                     vp(probs) if want_probs else None, vp(logits) if want_logits else None,
-                                     ctypes.byref(ticket)))
+    self._check(self._lib.dcb_submit(self._handle, _ptr(staged), batch, self._precision_flag(strict),
+                                     *(_ptr(a) for a in out), ctypes.byref(ticket)))
     busy[slot] = True
     return dict(ticket=int(ticket.value), slot=slot, batch=batch, probs=want_probs, logits=want_logits)
 
@@ -438,12 +444,8 @@ class B200Model:
     if rc != -4:   # anything but "not in flight" retires the slot
       self._slot_busy[handle["slot"]] = False
     self._check(rc, tolerate=() if strict_input else (-5,))
-    st, b = self._stage[handle["slot"]], handle["batch"]
-    out = dict(bases=st["bases"][:b].copy(), quals=st["quals"][:b].copy())
-    if handle["probs"]:
-      out["probs"] = st["probs"][:b].copy()
-    if handle["logits"]:
-      out["logits"] = st["logits"][:b].copy()
+    keys = ["bases", "quals"] + [k for k in ("probs", "logits") if handle[k]]
+    out = {k: self._staging(handle["slot"], k)[:handle["batch"]].copy() for k in keys}
     self.last_ms, self.last_launches = self.last_forward_ms(), self.last_forward_launches()
     return out
 
@@ -461,18 +463,9 @@ class B200Model:
   def forward_batches(self, batches, want_probs: bool = False, want_logits: bool = False,
                       strict_input: bool = True, strict: Optional[bool] = None):
     """Pipelined forward over an iterable of row batches; yields one output dict per batch, in order."""
-    pending = None
-    try:
-      for rows in batches:
-        h = self.submit(rows, want_probs=want_probs, want_logits=want_logits, strict=strict)
-        prev, pending = pending, h
-        if prev is not None:
-          yield self.wait(prev, strict_input)
-      if pending is not None:
-        h, pending = pending, None
-        yield self.wait(h, strict_input)
-    finally:
-      self.drain(pending)
+    submit = lambda rows: self.submit(rows, want_probs=want_probs, want_logits=want_logits, strict=strict)
+    for _, out in pipelined(batches, submit, lambda h: self.wait(h, strict_input), self.drain):
+      yield out
 
   # -- stitch: per-read window concatenation + gap compaction on the device -------------------------
   def stitch(self, bases, quals, zmw_start: np.ndarray, n_windows: Optional[int] = None,
@@ -483,24 +476,17 @@ class B200Model:
     zs = np.ascontiguousarray(zmw_start, dtype=np.int32)
     nz = int(zs.shape[0]) - 1
     L = int(length) if length is not None else self.max_length   # characters per window
-    if on_device:
-      if n_windows is None:
-        raise ValueError("stitch(on_device=True) needs n_windows")
-      b_ptr, q_ptr = ctypes.c_void_p(int(bases)), ctypes.c_void_p(int(quals))
-      flags = DCB_ROWS_ON_DEVICE
-    else:
-      bases = np.ascontiguousarray(bases, dtype=np.uint8)
-      quals = np.ascontiguousarray(quals, dtype=np.uint8)
+    if on_device and n_windows is None:
+      raise ValueError("stitch(on_device=True) needs n_windows")
+    b_ptr, bases = _arg(bases, np.uint8, on_device)
+    q_ptr, quals = _arg(quals, np.uint8, on_device)
+    if not on_device:
       n_windows = int(bases.shape[0])
-      b_ptr, q_ptr = bases.ctypes.data_as(ctypes.c_void_p), quals.ctypes.data_as(ctypes.c_void_p)
-      flags = 0
     seq = np.empty(n_windows * L, np.uint8)
     qual = np.empty(n_windows * L, np.uint8)
     lens = np.zeros(max(nz, 0), np.int32)
-    self._check(self._lib.dcb_stitch(self._handle, b_ptr, q_ptr, n_windows, L,
-                                     zs.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), nz, flags,
-                                     seq.ctypes.data_as(ctypes.c_void_p), qual.ctypes.data_as(ctypes.c_void_p),
-                                     lens.ctypes.data_as(ctypes.c_void_p)))
+    self._check(self._lib.dcb_stitch(self._handle, b_ptr, q_ptr, n_windows, L, _ptr(zs), nz,
+                                     DCB_ROWS_ON_DEVICE if on_device else 0, _ptr(seq), _ptr(qual), _ptr(lens)))
     return seq, qual, lens
 
   def stitch_fastq(self, bases, quals, zmw_start: np.ndarray, window_pos, names, min_quality: float, min_length: int,
@@ -511,15 +497,12 @@ class B200Model:
     zs = np.ascontiguousarray(zmw_start, dtype=np.int32)
     nz = int(zs.shape[0]) - 1
     L = int(length) if length is not None else self.max_length
-    if on_device:
-      if n_windows is None:
-        raise ValueError("stitch_fastq(on_device=True) needs n_windows")
-      b_ptr, q_ptr, flags = ctypes.c_void_p(int(bases)), ctypes.c_void_p(int(quals)), DCB_ROWS_ON_DEVICE
-    else:
-      bases = np.ascontiguousarray(bases, dtype=np.uint8)
-      quals = np.ascontiguousarray(quals, dtype=np.uint8)
+    if on_device and n_windows is None:
+      raise ValueError("stitch_fastq(on_device=True) needs n_windows")
+    b_ptr, bases = _arg(bases, np.uint8, on_device)
+    q_ptr, quals = _arg(quals, np.uint8, on_device)
+    if not on_device:
       n_windows = int(bases.shape[0])
-      b_ptr, q_ptr, flags = bases.ctypes.data_as(ctypes.c_void_p), quals.ctypes.data_as(ctypes.c_void_p), 0
     pos = np.ascontiguousarray(window_pos, dtype=np.int32)
     if pos.shape[0] != n_windows:
       raise ValueError("window_pos must have one entry per window")
@@ -535,10 +518,10 @@ class B200Model:
     rec_off = np.zeros(nz + 1, np.int64)
     outcome = np.zeros(max(nz, 0), np.int32)
     avg_q = np.zeros(max(nz, 0), np.float64)
-    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    self._check(self._lib.dcb_stitch_fastq(self._handle, b_ptr, q_ptr, n_windows, L, vp(zs), nz, vp(pos), vp(blob),
-                                           vp(name_off), float(min_quality), int(min_length), flags, vp(fastq), cap,
-                                           vp(rec_off), vp(outcome), vp(avg_q)))
+    self._check(self._lib.dcb_stitch_fastq(self._handle, b_ptr, q_ptr, n_windows, L, _ptr(zs), nz, _ptr(pos),
+                                           _ptr(blob), _ptr(name_off), float(min_quality), int(min_length),
+                                           DCB_ROWS_ON_DEVICE if on_device else 0, _ptr(fastq), cap, _ptr(rec_off),
+                                           _ptr(outcome), _ptr(avg_q)))
     return fastq[:int(rec_off[-1])].tobytes(), rec_off, outcome, avg_q
 
   def skip_mask(self, ccs_base_quality_scores: np.ndarray, skip_windows_above: float) -> Tuple[np.ndarray, np.ndarray]:
@@ -549,8 +532,7 @@ class B200Model:
       raise ValueError("ccs_base_quality_scores must be [n_windows, L]")
     n, L = bq.shape
     mask, avg = np.zeros(n, np.uint8), np.zeros(n, np.float64)
-    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    self._check(self._lib.dcb_skip_mask(self._handle, vp(bq), n, L, float(skip_windows_above), vp(mask), vp(avg)))
+    self._check(self._lib.dcb_skip_mask(self._handle, _ptr(bq), n, L, float(skip_windows_above), _ptr(mask), _ptr(avg)))
     return mask, avg
 
   def fill_skipped(self, ccs_ids: np.ndarray, ccs_base_quality_scores: np.ndarray, dst_window: np.ndarray,
@@ -566,27 +548,23 @@ class B200Model:
       raise ValueError("fill_skipped: ccs_ids / ccs_base_quality_scores [k, L] and dst_window [k] expected")
     cal = calibration
     en = int(bool(cal is not None and cal.enabled))
-    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    if on_device:
-      b_ptr, q_ptr, flags = ctypes.c_void_p(int(bases)), ctypes.c_void_p(int(quals)), DCB_OUT_ON_DEVICE
-    else:
+    if not on_device:   # written in place: no copy may stand in for the caller's arrays
       if not (bases.flags.c_contiguous and quals.flags.c_contiguous and bases.dtype == np.uint8 and quals.dtype == np.uint8):
         raise ValueError("fill_skipped: bases / quals must be C-contiguous uint8 arrays")
       if k and int(dst.max()) >= bases.shape[0]:
         raise ValueError("fill_skipped: destination window outside the output arrays")
-      b_ptr, q_ptr, flags = vp(bases), vp(quals), 0
-    self._check(self._lib.dcb_fill_skipped(self._handle, vp(ids), vp(bq), vp(dst), k, L, en,
+    self._check(self._lib.dcb_fill_skipped(self._handle, _ptr(ids), _ptr(bq), _ptr(dst), k, L, en,
                                            float(cal.threshold) if en else 0.0, float(cal.w) if en else 1.0,
-                                           float(cal.b) if en else 0.0, flags, b_ptr, q_ptr))
+                                           float(cal.b) if en else 0.0, DCB_OUT_ON_DEVICE if on_device else 0,
+                                           _ptr(bases), _ptr(quals)))
 
   def stitch_raw(self, bases_ptr: int, quals_ptr: int, n_windows: int, zmw_start: np.ndarray, flags: int,
                  seq_ptr: int, qual_ptr: int, len_ptr: int, length: Optional[int] = None) -> None:
     """dcb_stitch on caller-managed pointers (host or device per `flags`)."""
     zs = np.ascontiguousarray(zmw_start, dtype=np.int32)
-    self._check(self._lib.dcb_stitch(self._handle, ctypes.c_void_p(bases_ptr), ctypes.c_void_p(quals_ptr), n_windows,
-                                     int(length) if length is not None else self.max_length,
-                                     zs.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), int(zs.shape[0]) - 1, flags,
-                                     ctypes.c_void_p(seq_ptr), ctypes.c_void_p(qual_ptr), ctypes.c_void_p(len_ptr)))
+    self._check(self._lib.dcb_stitch(self._handle, _ptr(bases_ptr), _ptr(quals_ptr), n_windows,
+                                     int(length) if length is not None else self.max_length, _ptr(zs),
+                                     int(zs.shape[0]) - 1, flags, _ptr(seq_ptr), _ptr(qual_ptr), _ptr(len_ptr)))
 
   # -- evaluation of labelled windows (include/dcb200.h "evaluation of labelled windows") -------------------------
   def _eval_args(self, del_cost, loss_reg, band_width):
@@ -610,88 +588,59 @@ class B200Model:
     if labels.ndim != 2 or ccs.shape != labels.shape:
       raise ValueError("labels and ccs_ids must both be uint8 [B, L]")
     B, L = labels.shape
-    if on_device:
-      if batch is None or int(batch) != B:
-        raise ValueError("evaluate_windows(on_device=True) needs batch == labels.shape[0]")
-      p_ptr, flags = ctypes.c_void_p(int(probs)), DCB_ROWS_ON_DEVICE
-    else:
-      probs = np.ascontiguousarray(probs, dtype=np.float32)
-      if probs.shape != (B, L, 5):
-        raise ValueError("probs must be float32 [%d, %d, 5], got %s" % (B, L, probs.shape))
-      p_ptr, flags = probs.ctypes.data_as(ctypes.c_void_p), 0
+    if on_device and (batch is None or int(batch) != B):
+      raise ValueError("evaluate_windows(on_device=True) needs batch == labels.shape[0]")
+    p_ptr, probs = _arg(probs, np.float32, on_device)
+    if not on_device and probs.shape != (B, L, 5):
+      raise ValueError("probs must be float32 [%d, %d, 5], got %s" % (B, L, probs.shape))
     dc, reg, bw = self._eval_args(del_cost, loss_reg, band_width)
-    out = dict(loss=np.zeros(B, np.float32), exact=np.zeros(B, np.uint8), pred_counts=np.zeros((B, 5), np.int32),
-               ccs_counts=np.zeros((B, 5), np.int32))
+    out = _empty_eval(B)
     ms = ctypes.c_float()
-    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    self._check(self._lib.dcb_evaluate(self._handle, p_ptr, vp(labels), vp(ccs), B, L, dc, reg, bw, flags,
-                                       vp(out["loss"]), vp(out["exact"]), vp(out["pred_counts"]),
-                                       vp(out["ccs_counts"]), ctypes.byref(ms)))
+    self._check(self._lib.dcb_evaluate(self._handle, p_ptr, _ptr(labels), _ptr(ccs), B, L, dc, reg, bw,
+                                       DCB_ROWS_ON_DEVICE if on_device else 0, _ptr(out["loss"]), _ptr(out["exact"]),
+                                       _ptr(out["pred_counts"]), _ptr(out["ccs_counts"]), ctypes.byref(ms)))
     out["ms"] = float(ms.value)
     return out
 
   def distill_loss(self, teacher_logits, student_logits, temperature: float = 1.0, logit_loss: Any = "kl_divergence",
                    on_device: bool = False, batch: Optional[int] = None,
                    length: Optional[int] = None) -> Dict[str, Any]:
-    """dcb_distill_loss: per-window DistillationLoss between teacher and student logits float32 [B, L, 5] (host arrays,
-    or device addresses with on_device=True, `batch` and optionally `length`, default max_length).  logit_loss is a
-    Keras identifier (LOGIT_LOSS_IDS) or a DCB_LOGIT_LOSS_* id.  Returns loss float32 [B] and ms, the kernel's device
-    time."""
-    lid = logit_loss_id(logit_loss)
-    if on_device:
-      if batch is None:
-        raise ValueError("distill_loss(on_device=True) needs batch")
-      B, L = int(batch), int(length) if length is not None else self.max_length
-      t_ptr, s_ptr, flags = ctypes.c_void_p(int(teacher_logits)), ctypes.c_void_p(int(student_logits)), DCB_ROWS_ON_DEVICE
-    else:
-      teacher = np.ascontiguousarray(teacher_logits, dtype=np.float32)
-      student = np.ascontiguousarray(student_logits, dtype=np.float32)
-      if teacher.ndim != 3 or teacher.shape[2] != 5 or student.shape != teacher.shape:
-        raise ValueError("teacher and student logits must both be float32 [B, L, 5], got %s and %s" %
-                         (teacher.shape, student.shape))
-      B, L = teacher.shape[:2]
-      t_ptr, s_ptr, flags = teacher.ctypes.data_as(ctypes.c_void_p), student.ctypes.data_as(ctypes.c_void_p), 0
-    loss = np.zeros(B, np.float32)
-    ms = ctypes.c_float()
-    self._check(self._lib.dcb_distill_loss(self._handle, t_ptr, s_ptr, B, L, float(temperature), lid, flags,
-                                           loss.ctypes.data_as(ctypes.c_void_p), ctypes.byref(ms)))
-    return dict(loss=loss, ms=float(ms.value))
+    """Per-window DistillationLoss between teacher and student logits float32 [B, L, 5] (host arrays, or device
+    addresses with on_device=True, `batch` and optionally `length`, default max_length): distill_loss_grad() without
+    the gradient, so dcb_distill_loss_grad computes it.  logit_loss is a Keras identifier (LOGIT_LOSS_IDS) or a
+    DCB_LOGIT_LOSS_* id.  Returns loss float32 [B] and ms, the kernel's device time."""
+    if on_device and batch is None:
+      raise ValueError("distill_loss(on_device=True) needs batch")
+    r = self.distill_loss_grad(teacher_logits, student_logits, temperature, logit_loss, want_grad=False,
+                               on_device=on_device, batch=batch, length=length)
+    return dict(loss=r["loss"], ms=r["ms"])
 
   def distill_loss_grad(self, teacher_logits, student_logits, temperature: float = 1.0,
                         logit_loss: Any = "kl_divergence", want_grad: bool = True, on_device: bool = False,
                         batch: Optional[int] = None, length: Optional[int] = None,
                         out: Optional[Dict[str, int]] = None) -> Dict[str, Any]:
-    """dcb_distill_loss_grad: per-window DistillationLoss (bitwise equal to distill_loss's) and its gradient with
+    """dcb_distill_loss_grad: per-window DistillationLoss (bitwise equal to dcb_distill_loss's) and its gradient with
     respect to the student's logits, the teacher held constant.  Logits float32 [B, L, 5] are host arrays, or device
     addresses with on_device=True, `batch` and optionally `length` (default max_length).  Returns loss float32 [B],
     grad float32 [B, L, 5] (None unless want_grad) and ms, the kernel's device time.  With `out`, a dict of device
     addresses for "loss" and, if wanted, "grad", the results are written there instead and returned as None."""
     lid = logit_loss_id(logit_loss)
+    if on_device and batch is None:
+      raise ValueError("distill_loss_grad(on_device=True) needs batch")
+    t_ptr, teacher = _arg(teacher_logits, np.float32, on_device)
+    s_ptr, student = _arg(student_logits, np.float32, on_device)
     if on_device:
-      if batch is None:
-        raise ValueError("distill_loss_grad(on_device=True) needs batch")
       B, L = int(batch), int(length) if length is not None else self.max_length
-      t_ptr, s_ptr, flags = ctypes.c_void_p(int(teacher_logits)), ctypes.c_void_p(int(student_logits)), DCB_ROWS_ON_DEVICE
+    elif teacher.ndim != 3 or teacher.shape[2] != 5 or student.shape != teacher.shape:
+      raise ValueError("teacher and student logits must both be float32 [B, L, 5], got %s and %s" %
+                       (teacher.shape, student.shape))
     else:
-      teacher = np.ascontiguousarray(teacher_logits, dtype=np.float32)
-      student = np.ascontiguousarray(student_logits, dtype=np.float32)
-      if teacher.ndim != 3 or teacher.shape[2] != 5 or student.shape != teacher.shape:
-        raise ValueError("teacher and student logits must both be float32 [B, L, 5], got %s and %s" %
-                         (teacher.shape, student.shape))
       B, L = teacher.shape[:2]
-      t_ptr, s_ptr, flags = teacher.ctypes.data_as(ctypes.c_void_p), student.ctypes.data_as(ctypes.c_void_p), 0
-    res: Dict[str, Any] = dict(loss=None, grad=None)
-    if out is not None:
-      flags |= DCB_OUT_ON_DEVICE
-      ptrs = [ctypes.c_void_p(int(out["loss"])), ctypes.c_void_p(int(out["grad"])) if want_grad else None]
-    else:
-      res["loss"] = np.zeros(B, np.float32)
-      if want_grad:
-        res["grad"] = np.zeros((B, L, 5), np.float32)
-      ptrs = [None if res[k] is None else res[k].ctypes.data_as(ctypes.c_void_p) for k in ("loss", "grad")]
+    out_flag, ptrs, res = _outputs(out, dict(loss=(B,), grad=(B, L, 5) if want_grad else None))
     ms = ctypes.c_float()
-    self._check(self._lib.dcb_distill_loss_grad(self._handle, t_ptr, s_ptr, B, L, float(temperature), lid, flags,
-                                                *ptrs, ctypes.byref(ms)))
+    self._check(self._lib.dcb_distill_loss_grad(self._handle, t_ptr, s_ptr, B, L, float(temperature), lid,
+                                                (DCB_ROWS_ON_DEVICE if on_device else 0) | out_flag, *ptrs,
+                                                ctypes.byref(ms)))
     res["ms"] = float(ms.value)
     return res
 
@@ -706,36 +655,24 @@ class B200Model:
     (None unless want_grad), matches float32 [B, L, L] (None unless want_matches) and ms, the kernel's device time.
     With `out`, a dict of device addresses for "loss" and, as wanted, "grad" / "matches", the results are written
     there instead and returned as None."""
+    if on_device and batch is None:
+      raise ValueError("alignment_loss_grad(on_device=True) needs batch")
+    l_ptr, labels = _arg(labels, np.uint8, on_device)
     if on_device:
-      if batch is None:
-        raise ValueError("alignment_loss_grad(on_device=True) needs batch")
       B, L = int(batch), int(length) if length is not None else self.max_length
-      p_ptr, l_ptr, flags = ctypes.c_void_p(int(probs)), ctypes.c_void_p(int(labels)), DCB_ROWS_ON_DEVICE
+    elif labels.ndim != 2:
+      raise ValueError("labels must be uint8 [B, L], got %s" % (labels.shape,))
     else:
-      labels = np.ascontiguousarray(labels, dtype=np.uint8)
-      if labels.ndim != 2:
-        raise ValueError("labels must be uint8 [B, L], got %s" % (labels.shape,))
       B, L = labels.shape
-      probs = np.ascontiguousarray(probs, dtype=np.float32)
-      if probs.shape != (B, L, 5):
-        raise ValueError("probs must be float32 [%d, %d, 5], got %s" % (B, L, probs.shape))
-      p_ptr, l_ptr, flags = probs.ctypes.data_as(ctypes.c_void_p), labels.ctypes.data_as(ctypes.c_void_p), 0
+    p_ptr, probs = _arg(probs, np.float32, on_device)
+    if not on_device and probs.shape != (B, L, 5):
+      raise ValueError("probs must be float32 [%d, %d, 5], got %s" % (B, L, probs.shape))
     dc, reg, bw = self._eval_args(del_cost, loss_reg, band_width)
-    res: Dict[str, Any] = dict(loss=None, grad=None, matches=None)
-    if out is not None:
-      flags |= DCB_OUT_ON_DEVICE
-      ptrs = [ctypes.c_void_p(int(out["loss"])),
-              ctypes.c_void_p(int(out["grad"])) if want_grad else None,
-              ctypes.c_void_p(int(out["matches"])) if want_matches else None]
-    else:
-      res["loss"] = np.zeros(B, np.float32)
-      if want_grad:
-        res["grad"] = np.zeros((B, L, 5), np.float32)
-      if want_matches:
-        res["matches"] = np.zeros((B, L, L), np.float32)
-      ptrs = [None if res[k] is None else res[k].ctypes.data_as(ctypes.c_void_p) for k in ("loss", "grad", "matches")]
+    out_flag, ptrs, res = _outputs(out, dict(loss=(B,), grad=(B, L, 5) if want_grad else None,
+                                             matches=(B, L, L) if want_matches else None))
     ms = ctypes.c_float()
-    self._check(self._lib.dcb_alignment_loss_grad(self._handle, p_ptr, l_ptr, B, L, dc, reg, bw, flags, *ptrs,
+    self._check(self._lib.dcb_alignment_loss_grad(self._handle, p_ptr, l_ptr, B, L, dc, reg, bw,
+                                                  (DCB_ROWS_ON_DEVICE if on_device else 0) | out_flag, *ptrs,
                                                   ctypes.byref(ms)))
     res["ms"] = float(ms.value)
     return res
@@ -758,7 +695,7 @@ class B200Model:
       if x.shape[1] != self.packed_window_bytes:
         raise ValueError("packed rows must be uint8 [B, %d]" % self.packed_window_bytes)
     else:
-      x = self._rows3(x)
+      x = _rows3(self.params, x)
     B, L = x.shape[0], self.max_length
     labels = np.ascontiguousarray(labels, dtype=np.uint8)
     if labels.shape != (B, L):
@@ -773,10 +710,8 @@ class B200Model:
       fn = self._lib.dcb_forward_packed if packed else self._lib.dcb_forward
       for b0 in range(0, B, mb):
         b1 = min(B, b0 + mb)
-        rc = fn(self._handle, x[b0:b1].ctypes.data_as(ctypes.c_void_p), b1 - b0,
-                DCB_OUT_ON_DEVICE | self._precision_flag(strict), ctypes.c_void_p(d_bq),
-                ctypes.c_void_p(d_bq + mb * L), ctypes.c_void_p(d_probs), None)
-        self._check(rc, tolerate=() if strict_input else (-5,))
+        self._forward_chunk(fn, x[b0:b1], DCB_OUT_ON_DEVICE | self._precision_flag(strict), d_bq, d_bq + mb * L,
+                            d_probs, None, strict_input)
         fwd_ms += self.last_forward_ms()
         r = self.evaluate_windows(d_probs, labels[b0:b1], ccs[b0:b1], del_cost, loss_reg, band_width, on_device=True,
                                   batch=b1 - b0)
@@ -785,10 +720,7 @@ class B200Model:
     finally:
       self.free_device(d_probs)
       self.free_device(d_bq)
-    if not parts:
-      parts = [dict(loss=np.zeros(0, np.float32), exact=np.zeros(0, np.uint8), pred_counts=np.zeros((0, 5), np.int32),
-                    ccs_counts=np.zeros((0, 5), np.int32))]
-    out = {k: np.concatenate([p_[k] for p_ in parts]) for k in parts[0]}
+    out = _concat_eval(parts)
     out["forward_ms"], out["eval_ms"] = fwd_ms, eval_ms
     return out
 
@@ -825,8 +757,7 @@ class B200Model:
 
   def debug_residual(self, stage: int, tokens: int) -> np.ndarray:
     out = np.empty((tokens, 280), np.float32)
-    self._check(self._lib.dcb_debug_residual(self._handle, stage, out.ctypes.data_as(ctypes.c_void_p),
-                                             out.size))
+    self._check(self._lib.dcb_debug_residual(self._handle, stage, _ptr(out), out.size))
     return out
 
   def debug_operand(self, stage: int, which: str, tokens: int) -> np.ndarray:
@@ -835,8 +766,7 @@ class B200Model:
     width = {"embed": (params_lib.embedded_width(self.params) + 15) // 16 * 16, "xb": 288, "qkv": 864, "att": 288,
              "hid": int(self.params.filter_size)}[which]
     out = np.empty((tokens, width), np.uint16)
-    self._check(self._lib.dcb_debug_operand(self._handle, stage, DEBUG_OPERANDS[which],
-                                            out.ctypes.data_as(ctypes.c_void_p), out.size))
+    self._check(self._lib.dcb_debug_operand(self._handle, stage, DEBUG_OPERANDS[which], _ptr(out), out.size))
     return out
 
   def debug_head_epilogue(self, logits: np.ndarray) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
@@ -848,8 +778,7 @@ class B200Model:
       raise ValueError("debug_head_epilogue: logits must be [n, 5]")
     n = int(lg.shape[0])
     bases, quals, probs = np.empty(n, np.uint8), np.empty(n, np.uint8), np.empty((n, 5), np.float32)
-    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    self._check(self._lib.dcb_debug_head_epilogue(self._handle, vp(lg), n, vp(bases), vp(quals), vp(probs)))
+    self._check(self._lib.dcb_debug_head_epilogue(self._handle, _ptr(lg), n, _ptr(bases), _ptr(quals), _ptr(probs)))
     return bases, quals, probs
 
   # -- raw device / pinned buffers (bench, multi-GPU driver) ----------------------------------
@@ -859,25 +788,21 @@ class B200Model:
     return p.value
 
   def free_device(self, ptr: int) -> None:
-    self._check(self._lib.dcb_free_device(self._handle, ctypes.c_void_p(ptr)))
+    self._check(self._lib.dcb_free_device(self._handle, _ptr(ptr)))
 
   def memcpy_h2d(self, dst: int, src: np.ndarray) -> None:
     src = np.ascontiguousarray(src)
-    self._check(self._lib.dcb_memcpy_h2d(self._handle, ctypes.c_void_p(dst),
-                                         src.ctypes.data_as(ctypes.c_void_p), src.nbytes))
+    self._check(self._lib.dcb_memcpy_h2d(self._handle, _ptr(dst), _ptr(src), src.nbytes))
 
   def memcpy_d2h(self, dst: np.ndarray, src: int) -> None:
-    self._check(self._lib.dcb_memcpy_d2h(self._handle, dst.ctypes.data_as(ctypes.c_void_p),
-                                         ctypes.c_void_p(src), dst.nbytes))
+    self._check(self._lib.dcb_memcpy_d2h(self._handle, _ptr(dst), _ptr(src), dst.nbytes))
 
   def submit_raw(self, rows_ptr: int, batch: int, flags: int, bases_ptr: int, quals_ptr: int,
                  probs_ptr: int = 0, logits_ptr: int = 0) -> int:
     """dcb_submit on caller-managed pointers; returns the ticket for wait_raw()."""
     ticket = ctypes.c_int64(-1)
-    self._check(self._lib.dcb_submit(self._handle, ctypes.c_void_p(rows_ptr), batch, flags,
-                                     ctypes.c_void_p(bases_ptr), ctypes.c_void_p(quals_ptr),
-                                     ctypes.c_void_p(probs_ptr) if probs_ptr else None,
-                                     ctypes.c_void_p(logits_ptr) if logits_ptr else None, ctypes.byref(ticket)))
+    self._check(self._lib.dcb_submit(self._handle, _ptr(rows_ptr), batch, flags, _ptr(bases_ptr), _ptr(quals_ptr),
+                                     _ptr(probs_ptr), _ptr(logits_ptr), ctypes.byref(ticket)))
     return int(ticket.value)
 
   def wait_raw(self, ticket: int) -> None:
@@ -886,18 +811,14 @@ class B200Model:
   def forward_raw(self, rows_ptr: int, batch: int, flags: int, bases_ptr: int, quals_ptr: int,
                   probs_ptr: int = 0, logits_ptr: int = 0) -> None:
     """dcb_forward on caller-managed pointers (host or device per `flags`)."""
-    self._check(self._lib.dcb_forward(self._handle, ctypes.c_void_p(rows_ptr), batch, flags,
-                                      ctypes.c_void_p(bases_ptr), ctypes.c_void_p(quals_ptr),
-                                      ctypes.c_void_p(probs_ptr) if probs_ptr else None,
-                                      ctypes.c_void_p(logits_ptr) if logits_ptr else None))
+    self._check(self._lib.dcb_forward(self._handle, _ptr(rows_ptr), batch, flags, _ptr(bases_ptr), _ptr(quals_ptr),
+                                      _ptr(probs_ptr), _ptr(logits_ptr)))
 
   def forward_packed_raw(self, packed_ptr: int, batch: int, flags: int, bases_ptr: int, quals_ptr: int,
                          probs_ptr: int = 0, logits_ptr: int = 0) -> None:
     """dcb_forward_packed on caller-managed pointers (host or device per `flags`)."""
-    self._check(self._lib.dcb_forward_packed(self._handle, ctypes.c_void_p(packed_ptr), batch, flags,
-                                             ctypes.c_void_p(bases_ptr), ctypes.c_void_p(quals_ptr),
-                                             ctypes.c_void_p(probs_ptr) if probs_ptr else None,
-                                             ctypes.c_void_p(logits_ptr) if logits_ptr else None))
+    self._check(self._lib.dcb_forward_packed(self._handle, _ptr(packed_ptr), batch, flags, _ptr(bases_ptr),
+                                             _ptr(quals_ptr), _ptr(probs_ptr), _ptr(logits_ptr)))
 
   def synchronize(self) -> None:
     self._check(self._lib.dcb_synchronize(self._handle))
@@ -914,24 +835,53 @@ def pack_rows(params: params_lib.Params, rows: np.ndarray, out: Optional[np.ndar
   """float32 rows [B, R, L(,1)] -> packed uint8 [B, packed_window_bytes] (dcb_pack_rows; host code, needs no GPU).
   Raises DcbError(-5) when a base / strand / ccs / ccs_bq value lies outside its vocabulary (TensorFlow's gather would
   raise) or an SN row is not constant, unless `strict_input` is False (values are clamped either way)."""
-  rows = np.asarray(rows)
-  if rows.ndim == 4:
-    rows = rows[..., 0]
-  R = params_lib.get_total_rows(params.max_passes, params.use_ccs_bq)
-  if rows.ndim != 3 or rows.shape[1] != R or rows.shape[2] != int(params.max_length):
-    raise ValueError("rows must be [B, %d, %d(, 1)], got %s" % (R, int(params.max_length), rows.shape))
-  rows = np.ascontiguousarray(rows, dtype=np.float32)
+  rows = _rows3(params, rows)
   lib, cfg = load_library(), make_config(params, max_batch=1)
-  stride = int(lib.dcb_packed_window_bytes(ctypes.byref(cfg)))
+  stride = packed_window_bytes(params)
   B = rows.shape[0]
   if out is None:
     out = np.empty((B, stride), np.uint8)
   if out.shape != (B, stride) or out.dtype != np.uint8 or not out.flags.c_contiguous:
     raise ValueError("pack_rows(out=...): need C-contiguous uint8 [%d, %d]" % (B, stride))
-  rc = lib.dcb_pack_rows(ctypes.byref(cfg), rows.ctypes.data_as(ctypes.c_void_p), B, out.ctypes.data_as(ctypes.c_void_p))
+  rc = lib.dcb_pack_rows(ctypes.byref(cfg), _ptr(rows), B, _ptr(out))
   if rc and not (rc == -5 and not strict_input):
     raise DcbError(rc, lib.dcb_last_error(None).decode())
   return out
+
+
+def pipelined(items: Iterable[Any], submit: Callable[[Any], Any], wait: Callable[[Any], Any],
+              retire: Callable[[Any], None]) -> Iterator[Tuple[Any, Any]]:
+  """Two submissions in flight: yields (item, wait(submit(item))) in order, submitting item i + 1 before waiting for
+  item i, so that the device works on one while the host prepares the next.  If a submit or a wait raises, or the
+  consumer closes the generator, every submission not yet waited for is passed to `retire` (which must swallow
+  DcbError) before the exception propagates, so the engines' slots are free again."""
+  pending = []
+  try:
+    for item in items:
+      pending.append((item, submit(item)))
+      if len(pending) == 2:
+        done, handle = pending.pop(0)
+        yield done, wait(handle)
+    while pending:
+      done, handle = pending.pop(0)
+      yield done, wait(handle)
+  finally:
+    for _, handle in pending:
+      retire(handle)
+
+
+def _empty_eval(n: int) -> Dict[str, np.ndarray]:
+  """Zeroed per-window results of dcb_evaluate for n windows."""
+  return dict(loss=np.zeros(n, np.float32), exact=np.zeros(n, np.uint8), pred_counts=np.zeros((n, 5), np.int32),
+              ccs_counts=np.zeros((n, 5), np.int32))
+
+
+def _concat_eval(parts: List[Dict[str, np.ndarray]], extra: Tuple[str, ...] = ()) -> Dict[str, np.ndarray]:
+  """Per-chunk evaluate_windows() results, each with float32 [n] arrays `extra` added, concatenated over the chunks;
+  empty arrays of the same dtypes when there is no chunk."""
+  if not parts:
+    parts = [dict(_empty_eval(0), **{k: np.zeros(0, np.float32) for k in extra})]
+  return {k: np.concatenate([p[k] for p in parts]) for k in parts[0]}
 
 
 def unpack_rows(params: params_lib.Params, packed: np.ndarray) -> np.ndarray:
@@ -990,4 +940,4 @@ def alloc_pinned(nbytes: int) -> Tuple[int, np.ndarray]:
 
 
 def free_pinned(addr: int) -> None:
-  load_library().dcb_free_host(ctypes.c_void_p(addr))
+  load_library().dcb_free_host(_ptr(addr))

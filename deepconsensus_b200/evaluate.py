@@ -23,7 +23,7 @@ of model_utils.get_deepconsensus_metrics):
 Distilled students (the reference's model_distillation.py): `--teacher_model_dir CKPT` (with `--teacher_random_weights
 SEED` the counterpart of `--random_weights`) builds the teacher as a second engine on the same device and precision,
 from its own params.json; its inputs (max_passes, max_length, use_ccs_bq, the embedding widths and the *_MAX clips) must
-be the student's.  Both forwards leave their logits in device memory, dcb_distill_loss compares them there, and
+be the student's.  Both forwards leave their logits in device memory, dcb_distill_loss_grad compares them there, and
 `eval_metrics.json` gains a "distillation" entry per dataset with what the distillation loop's eval step reports
 (model_distillation.py:242-270,320-349): per example student_alpha * AlignmentLoss + distill_alpha * DistillationLoss,
 per batch their sum / batch_size (tf.nn.compute_average_loss), `loss` (eval/loss) the mean over batches, the same for
@@ -35,6 +35,7 @@ transformer_learn_values_distill config).  `inference.csv` and the other entries
 from __future__ import annotations
 
 import argparse
+import contextlib
 import json
 import os
 import time
@@ -132,123 +133,87 @@ def write_inference_csv(path: str, rows: Sequence[Tuple[str, float, float]]) -> 
 
 
 def evaluate_rows(model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndarray, chunk: int,
-                  strict: Optional[bool] = None) -> Dict[str, Any]:
-  """Per-window evaluation of float32 rows [N, R, L] through dcb_submit (device outputs, two batches in flight) and
-  dcb_evaluate on the device probabilities."""
+                  strict: Optional[bool] = None, teacher: Optional[engine_lib.B200Model] = None,
+                  temperature: float = 1.0, logit_loss: Any = "kl_divergence") -> Dict[str, Any]:
+  """Per-window evaluation of float32 rows [N, R, L]: per chunk of the rows the forward runs through dcb_submit from the
+  pipeline slot's pinned staging (device outputs, two chunks in flight) and dcb_evaluate reads its probabilities on the
+  device.  Returns evaluate_windows()'s arrays over all N windows and forward_ms / eval_ms, the summed device times.
+
+  With the `teacher` of a distilled student, the teacher's forward runs from the same pinned rows, and once both are
+  done dcb_distill_loss_grad compares the two engines' logits on the device.  This adds distill_loss float32 [N] and
+  the teacher's forward and the distillation kernel's device times (teacher_forward_ms, distill_ms)."""
   N, L = rows.shape[0], model.max_length
   ccs = model.ccs_ids(rows)
   flag = engine_lib.DCB_OUT_ON_DEVICE | model._precision_flag(strict)
-  d_probs = [model.alloc_device(chunk * L * 5 * 4) for _ in range(2)]
-  d_bq = [model.alloc_device(2 * chunk * L) for _ in range(2)]
+  engines = [model] if teacher is None else [model, teacher]
+  out_bytes = chunk * L * 5 * 4
+  owned = []                                            # (engine, device address) of every buffer allocated here
   parts: List[Dict[str, np.ndarray]] = []
-  times = dict(forward_ms=0.0, eval_ms=0.0)
+  if teacher is None:
+    times = dict(forward_ms=0.0, eval_ms=0.0)
+  else:
+    times = dict(forward_ms=0.0, teacher_forward_ms=0.0, eval_ms=0.0, distill_ms=0.0)
 
-  def finish(p):
-    ticket, slot, b0, b1 = p
-    model.wait_raw(ticket)
-    times["forward_ms"] += model.last_forward_ms()
-    r = model.evaluate_windows(d_probs[slot], labels[b0:b1], ccs[b0:b1], on_device=True, batch=b1 - b0)
-    times["eval_ms"] += r.pop("ms")
-    parts.append(r)
+  def alloc(m, nbytes):
+    owned.append((m, m.alloc_device(nbytes)))
+    return owned[-1][1]
 
-  pending = None
-  try:
-    for i, b0 in enumerate(range(0, N, chunk)):
-      b1, slot = min(N, b0 + chunk), i % 2
-      staging = model.staging_rows(slot)
-      staging[:b1 - b0] = rows[b0:b1]
-      ticket = model.submit_raw(staging.ctypes.data, b1 - b0, flag, d_bq[slot], d_bq[slot] + chunk * L,
-                                probs_ptr=d_probs[slot])
-      prev, pending = pending, (ticket, slot, b0, b1)
-      if prev is not None:
-        finish(prev)
-    if pending is not None:
-      prev, pending = pending, None
-      finish(prev)
-  finally:
-    if pending is not None:
+  def retire(handle):
+    for m, ticket in handle:
       try:
-        model.wait_raw(pending[0])
+        m.wait_raw(ticket)
       except engine_lib.DcbError:
         pass
-    for p in d_probs + d_bq:
-      model.free_device(p)
-  if not parts:
-    parts = [dict(loss=np.zeros(0, np.float32), exact=np.zeros(0, np.uint8), pred_counts=np.zeros((0, 5), np.int32),
-                  ccs_counts=np.zeros((0, 5), np.int32))]
-  out = {k: np.concatenate([p[k] for p in parts]) for k in parts[0]}
-  out.update(times)
-  return out
 
+  def submit(item):
+    """Both engines' forwards of one chunk; if the teacher's submit fails, the student's ticket is retired."""
+    slot, b0, b1 = item
+    staging = model.staging_rows(slot)
+    staging[:b1 - b0] = rows[b0:b1]
+    handle = []
+    try:
+      for m, buf in zip(engines, bufs[slot]):
+        handle.append((m, m.submit_raw(staging.ctypes.data, b1 - b0, flag, buf["bq"], buf["bq"] + chunk * L,
+                                       probs_ptr=buf.get("probs", 0), logits_ptr=buf.get("logits", 0))))
+    except BaseException:
+      retire(handle)
+      raise
+    return handle
 
-def evaluate_rows_distill(student: engine_lib.B200Model, teacher: engine_lib.B200Model, rows: np.ndarray,
-                          labels: np.ndarray, chunk: int, temperature: float, logit_loss: str) -> Dict[str, Any]:
-  """evaluate_rows() for a student and its teacher: per chunk both engines run their forward from the same pinned rows
-  through dcb_submit (device probabilities and logits, two batches in flight per engine); once both tickets are done,
-  dcb_evaluate reads the student's probabilities and dcb_distill_loss the two logits buffers, all on the device.  Adds
-  distill_loss float32 [N] and the teacher's forward and the distillation kernel's device times."""
-  N, L = rows.shape[0], student.max_length
-  ccs = student.ccs_ids(rows)
-  logit_bytes = chunk * L * 5 * 4
-  d_probs = [student.alloc_device(logit_bytes) for _ in range(2)]
-  d_logits_s = [student.alloc_device(logit_bytes) for _ in range(2)]
-  d_bq_s = [student.alloc_device(2 * chunk * L) for _ in range(2)]
-  d_logits_t = [teacher.alloc_device(logit_bytes) for _ in range(2)]
-  d_bq_t = [teacher.alloc_device(2 * chunk * L) for _ in range(2)]
-  parts: List[Dict[str, np.ndarray]] = []
-  times = dict(forward_ms=0.0, teacher_forward_ms=0.0, eval_ms=0.0, distill_ms=0.0)
+  def wait(handle):
+    """Waits for the chunk's ticket on every engine (the teacher's also when the student's wait fails)."""
+    for i, (m, ticket) in enumerate(handle):
+      try:
+        m.wait_raw(ticket)
+      except BaseException:
+        retire(handle[i + 1:])
+        raise
+    times["forward_ms"] += model.last_forward_ms()
+    if teacher is not None:
+      times["teacher_forward_ms"] += teacher.last_forward_ms()
 
-  in_flight = {id(student): [], id(teacher): []}      # tickets submitted and not yet waited for, per engine
-
-  def wait(m):
-    m.wait_raw(in_flight[id(m)].pop(0))
-
-  def finish(slot, b0, b1):
-    wait(student)
-    times["forward_ms"] += student.last_forward_ms()
-    wait(teacher)
-    times["teacher_forward_ms"] += teacher.last_forward_ms()
-    r = student.evaluate_windows(d_probs[slot], labels[b0:b1], ccs[b0:b1], on_device=True, batch=b1 - b0)
-    times["eval_ms"] += r.pop("ms")
-    d = student.distill_loss(d_logits_t[slot], d_logits_s[slot], temperature, logit_loss, on_device=True,
-                             batch=b1 - b0, length=L)
-    times["distill_ms"] += d["ms"]
-    r["distill_loss"] = d["loss"]
-    parts.append(r)
-
-  pending = None
   try:
-    for i, b0 in enumerate(range(0, N, chunk)):
-      b1, slot = min(N, b0 + chunk), i % 2
-      staging = student.staging_rows(slot)
-      staging[:b1 - b0] = rows[b0:b1]
-      out_flag = engine_lib.DCB_OUT_ON_DEVICE
-      in_flight[id(student)].append(student.submit_raw(staging.ctypes.data, b1 - b0, out_flag, d_bq_s[slot],
-                                                       d_bq_s[slot] + chunk * L, probs_ptr=d_probs[slot],
-                                                       logits_ptr=d_logits_s[slot]))
-      in_flight[id(teacher)].append(teacher.submit_raw(staging.ctypes.data, b1 - b0, out_flag, d_bq_t[slot],
-                                                       d_bq_t[slot] + chunk * L, logits_ptr=d_logits_t[slot]))
-      prev, pending = pending, (slot, b0, b1)
-      if prev is not None:
-        finish(*prev)
-    if pending is not None:
-      prev, pending = pending, None
-      finish(*prev)
+    # per slot and engine: bases and quals, the student's probabilities, and with a teacher both engines' logits
+    bufs = [[dict(bq=alloc(m, 2 * chunk * L)) for m in engines] for _ in range(2)]
+    for slot in bufs:
+      slot[0]["probs"] = alloc(model, out_bytes)
+      if teacher is not None:
+        slot[0]["logits"], slot[1]["logits"] = alloc(model, out_bytes), alloc(teacher, out_bytes)
+    chunks = [(i % 2, b0, min(N, b0 + chunk)) for i, b0 in enumerate(range(0, N, chunk))]
+    with contextlib.closing(engine_lib.pipelined(chunks, submit, wait, retire)) as done:   # retired before the frees
+      for (slot, b0, b1), _ in done:
+        r = model.evaluate_windows(bufs[slot][0]["probs"], labels[b0:b1], ccs[b0:b1], on_device=True, batch=b1 - b0)
+        times["eval_ms"] += r.pop("ms")
+        if teacher is not None:
+          d = model.distill_loss(bufs[slot][1]["logits"], bufs[slot][0]["logits"], temperature, logit_loss,
+                                 on_device=True, batch=b1 - b0, length=L)
+          times["distill_ms"] += d["ms"]
+          r["distill_loss"] = d["loss"]
+        parts.append(r)
   finally:
-    for m in (student, teacher):
-      while in_flight[id(m)]:
-        try:
-          wait(m)
-        except engine_lib.DcbError:
-          pass
-    for p in d_probs + d_logits_s + d_bq_s:
-      student.free_device(p)
-    for p in d_logits_t + d_bq_t:
-      teacher.free_device(p)
-  if not parts:
-    parts = [dict(loss=np.zeros(0, np.float32), exact=np.zeros(0, np.uint8), pred_counts=np.zeros((0, 5), np.int32),
-                  ccs_counts=np.zeros((0, 5), np.int32), distill_loss=np.zeros(0, np.float32))]
-  out = {k: np.concatenate([p[k] for p in parts]) for k in parts[0]}
+    for m, addr in owned:
+      m.free_device(addr)
+  out = engine_lib._concat_eval(parts, () if teacher is None else ("distill_loss",))
   out.update(times)
   return out
 
@@ -313,8 +278,8 @@ def run(checkpoint: str, eval_path: Sequence[str], out_dir: str, limit: int = -1
       if teacher is None:
         per = evaluate_rows(model, rows, labels, chunk)
       else:
-        per = evaluate_rows_distill(model, teacher, rows, labels, chunk, float(distill["temperature"]),
-                                    distill["logit_loss_identifier"])
+        per = evaluate_rows(model, rows, labels, chunk, teacher=teacher, temperature=float(distill["temperature"]),
+                            logit_loss=distill["logit_loss_identifier"])
       agg = aggregate(per["loss"], per["exact"], per["pred_counts"], per["ccs_counts"], bs)
       agg.update(precision=precision, forward_ms=per["forward_ms"], eval_ms=per["eval_ms"],
                  seconds_read=t1 - t0, seconds_model_and_eval=time.time() - t1)

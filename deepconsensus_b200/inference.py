@@ -87,8 +87,8 @@ def run_model_on_examples(feature_dicts: List[Dict[str, Any]], model: engine_lib
                           options: InferenceOptions) -> List[stitch_utils.DCModelOutput]:
   """Runs the model over windows and returns one DCModelOutput per window (quick_inference.py:341-415)."""
   predictions: List[stitch_utils.DCModelOutput] = []
-
-  def collect(data, out):
+  batches = batch_examples(feature_dicts, model_params, options)
+  for data, out in engine_lib.pipelined(batches, lambda d: model.submit(d["rows"]), model.wait, model.drain):
     bases, quals = out["bases"], out["quals"]
     for i in range(bases.shape[0]):
       predictions.append(stitch_utils.DCModelOutput(
@@ -96,27 +96,7 @@ def run_model_on_examples(feature_dicts: List[Dict[str, Any]], model: engine_lib
           np_num_passes=data["np_num_passes"][i], rq=data["rq"][i], rg=data["rg"][i],
           sequence=bases[i].tobytes().decode("ascii"),
           quality_string=quals[i].tobytes().decode("ascii")))
-
-  _pipelined(model, batch_examples(feature_dicts, model_params, options), collect)
   return predictions
-
-
-def _pipelined(model: engine_lib.B200Model, batches: Iterable[Dict[str, Any]], collect) -> None:
-  """Two batches in flight: while the device scores batch i, batch i+1 is stacked and copied (dcb_submit / dcb_wait).
-  If a wait raises (e.g. DCB_ERR_INPUT_RANGE), the younger submission is retired too, so the model stays usable."""
-  pending = None
-  try:
-    for data in batches:
-      handle = model.submit(data["rows"])
-      prev, pending = pending, (data, handle)
-      if prev is not None:
-        collect(prev[0], model.wait(prev[1]))
-    if pending is not None:
-      last, pending = pending, None
-      collect(last[0], model.wait(last[1]))
-  finally:
-    if pending is not None:
-      model.drain(pending[1])
 
 
 def process_skipped_window(feature_dict: Dict[str, Any], options: InferenceOptions) -> stitch_utils.DCModelOutput:
@@ -175,14 +155,12 @@ def run_model_and_stitch(feature_dicts: List[Dict[str, Any]], model: engine_lib.
   from deepconsensus_b200 import stitch_gpu
   L = int(model_params.max_length)
   names, positions, bases, quals = [], [], [], []
-
-  def collect(data, out):
+  batches = batch_examples(feature_dicts, model_params, options)
+  for data, out in engine_lib.pipelined(batches, lambda d: model.submit(d["rows"]), model.wait, model.drain):
     bases.append(out["bases"])
     quals.append(out["quals"])
     names.extend(_as_str(x) for x in data["name"])
     positions.extend(int(x) for x in data["window_pos"])
-
-  _pipelined(model, batch_examples(feature_dicts, model_params, options), collect)
   if skipped_outputs:
     sb = np.empty((len(skipped_outputs), L), np.uint8)
     sq = np.empty((len(skipped_outputs), L), np.uint8)
@@ -249,15 +227,13 @@ def inference_on_zmw_windows(feature_dicts_for_zmws: Iterable[Iterable[Dict[str,
   dest[order] = np.arange(n, dtype=np.int32)
   all_b, all_q = np.empty((n, L), np.uint8), np.empty((n, L), np.uint8)
   scored = np.nonzero(~skip)[0]
-  cursor = [0]
-
-  def collect(data, out):
+  cursor = 0
+  batches = batch_examples([windows[i] for i in scored], model_params, options)
+  for _, out in engine_lib.pipelined(batches, lambda d: model.submit(d["rows"]), model.wait, model.drain):
     k = out["bases"].shape[0]
-    rows = dest[scored[cursor[0]:cursor[0] + k]]
+    rows = dest[scored[cursor:cursor + k]]
     all_b[rows], all_q[rows] = out["bases"], out["quals"]
-    cursor[0] += k
-
-  _pipelined(model, batch_examples([windows[i] for i in scored], model_params, options), collect)
+    cursor += k
   skipped = np.nonzero(skip)[0]
   if len(skipped):
     ccs_row = params_lib.get_indices(options.max_passes, options.use_ccs_bq)[4][0]

@@ -248,3 +248,44 @@ def test_evaluate_driver_refuses_mismatched_teacher(tmp_path):
   with pytest.raises(ValueError, match="band_width"):
     evaluate.run(banded, [EVAL], str(tmp_path / "out"), random_weights=6, teacher_model_dir=CKPT,
                  teacher_random_weights=5)
+
+
+def test_evaluate_rows_with_teacher_recovers_from_a_bad_chunk():
+  """evaluate_rows with a teacher on rows whose second chunk holds an out-of-range base id raises DCB_ERR_INPUT_RANGE;
+  the tickets of that chunk and of the one submitted after it are retired on both engines, so both then run a clean
+  evaluate_rows that is bitwise equal to the same call on fresh engines."""
+  from deepconsensus_b200 import engine, evaluate
+  p = params_lib.synthetic_params(20, 100, num_hidden_layers=2)
+  ws, wt = weights_lib.init_weights(p, seed=31), weights_lib.init_weights(p, seed=32)
+  N, chunk = 40, 16
+  rows = np.ascontiguousarray(synthetic.make_rows(p, N, seed=33).reshape(N, p.total_rows, 100), np.float32)
+  labels = rows[:, 4 * 20, :].astype(np.uint8)
+  bad = rows.copy()
+  bad[chunk + 3, 0, 7] = 9.0                              # base ids are 0..4
+  kw = dict(temperature=2.0, logit_loss="kl_divergence")
+
+  def engines():
+    return engine.B200Model(p, ws, max_batch=chunk), engine.B200Model(p, wt, max_batch=chunk)
+
+  def arrays(r):
+    return {k: v for k, v in r.items() if not k.endswith("_ms")}
+
+  student, teacher = engines()
+  try:
+    with pytest.raises(engine.DcbError) as ei:
+      evaluate.evaluate_rows(student, bad, labels, chunk, teacher=teacher, **kw)
+    assert ei.value.code == -5
+    got = arrays(evaluate.evaluate_rows(student, rows, labels, chunk, teacher=teacher, **kw))
+  finally:
+    student.close()
+    teacher.close()
+  student, teacher = engines()
+  try:
+    want = arrays(evaluate.evaluate_rows(student, rows, labels, chunk, teacher=teacher, **kw))
+  finally:
+    student.close()
+    teacher.close()
+  assert sorted(got) == ["ccs_counts", "distill_loss", "exact", "loss", "pred_counts"]
+  assert got["distill_loss"].shape == (N,) and (got["distill_loss"] > 0).all()
+  for k in want:
+    assert got[k].dtype == want[k].dtype and got[k].tobytes() == want[k].tobytes(), k

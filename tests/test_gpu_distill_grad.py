@@ -90,13 +90,29 @@ def _bound_ratio(got, t, s, T, ident):
   return float((np.abs(got.astype(np.float64) - r["grad"]) / bound).max())
 
 
+def _abi_losses(model, t, s, T, lid):
+  """The loss of dcb_distill_loss, of dcb_distill_loss_grad with a gradient and of dcb_distill_loss_grad with a NULL
+  gradient, each called directly with host arrays."""
+  vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+  lib, h, (B, L) = model._lib, model._handle, t.shape[:2]
+  loss = [np.full(B, np.nan, np.float32) for _ in range(3)]
+  grad = np.empty_like(t)
+  assert lib.dcb_distill_loss(h, vp(t), vp(s), B, L, T, lid, 0, vp(loss[0]), None) == 0
+  assert lib.dcb_distill_loss_grad(h, vp(t), vp(s), B, L, T, lid, 0, vp(loss[1]), vp(grad), None) == 0
+  assert lib.dcb_distill_loss_grad(h, vp(t), vp(s), B, L, T, lid, 0, vp(loss[2]), None, None) == 0
+  return loss
+
+
 @pytest.mark.parametrize("L", [1, 31, 32, 33, 100, 120, 256])
 def test_loss_bits_equal_dcb_distill_loss_and_gradient_within_bound(model, L):
+  from deepconsensus_b200 import engine
   t, s = _random_logits(L)
   worst = 0.0
   for ident in LOSSES.values():
     for T in (0.5, 1.0, 2.5):
       r = model.distill_loss_grad(t, s, T, ident)
+      plain, with_grad, null_grad = _abi_losses(model, t, s, T, engine.logit_loss_id(ident))
+      assert plain.tobytes() == with_grad.tobytes() == null_grad.tobytes() == r["loss"].tobytes(), (ident, T)
       assert r["loss"].tobytes() == model.distill_loss(t, s, T, ident)["loss"].tobytes(), (ident, T)
       worst = max(worst, _bound_ratio(r["grad"], t, s, T, ident))
   print("L = %d: largest gradient error / bound %.3g" % (L, worst))
