@@ -111,7 +111,16 @@ embed_rows_kernel(const float* __restrict__ rows, const uint8_t* __restrict__ pa
 // k-steps through the stage ring; warpgroup w owns tile 2i + w and issues two m64 wgmmas (tile rows 0-63, 64-127) per B
 // k-step, so every weight byte that crosses from L2 feeds 256 tokens.  An odd tile count leaves the last pair with one
 // tile: the other warpgroup then waits and arrives on every barrier like its partner but issues no wgmma and stores
-// nothing.  Otherwise (the row epilogue GEMMs, one n-group covering all 288 columns, K up to 2048) warpgroup w owns tile
+// nothing.
+//
+// kAres epilogues are ordered: the warpgroups take turns, one n-group at a time (WG0 group g, WG1 group g, WG0 group
+// g + 1, ...), through two mbarriers (turn[w]: warpgroup w may run its next epilogue).  A warpgroup waits for its turn
+// only after it has released every stage of the group, so its partner can always drain the ring; it passes the turn on
+// once its stores are issued.  In steady state warpgroup 1 runs about one epilogue behind warpgroup 0, so while one
+// converts and stores its accumulators the other keeps the tensor cores busy, and the output stores drain under the
+// partner's MMAs.  The idle warpgroup of a one-tile pair takes and passes its turns like a working one.
+//
+// Otherwise (the row epilogue GEMMs, one n-group covering all 288 columns, K up to 2048) warpgroup w owns tile
 // rows [64 w, 64 w + 64) of one tile, and A and B k-steps stream together.
 //
 // Split-bf16 weights: the B image may hold K twice as [W_hi; W_lo] (b_ksteps = 2 * a_ksteps, W_lo = bf16(W - W_hi));
@@ -129,13 +138,27 @@ struct GemmCfg {
   static constexpr int kABytesPerK = 2 * kTileM * 16;             // 4096
   static constexpr int kBBytesPerK = 2 * kNI * 16;
   static constexpr int kStageBytes = kSK * ((kAres ? 0 : kABytesPerK) + kBBytesPerK);
-  static constexpr int kStages = 4;
+  // Ring depth.  kAres: the warpgroups take turns at their epilogues (gemm_kernel), so one runs up to an epilogue ahead
+  // of the other over the same B stages; 8 stages hold that offset on top of the prefetch depth.  The row GEMMs keep
+  // their epilogues in lockstep (taking turns made the condenser and the out-projection slower) and take 8 stages when
+  // an item streams at least kLongK of them (condenser, FFN down-projection: 10 % and 14 % faster on an H100 at 700 W);
+  // the out-projection (18 stages per item) keeps 4.
+  static constexpr int kStages = 8;
+  static constexpr int kShortStages = 4;
+  static constexpr int kLongK = 32;
+  __host__ __device__ static constexpr int stages(int kstages) {
+    return kAres || kstages >= kLongK ? kStages : kShortStages;
+  }
   static constexpr int kMH = kAres ? 2 : 1;                       // m64 row blocks per consumer warpgroup
   static constexpr int kATileBytes = (kDP / 16) * kABytesPerK;    // kAres: one resident A tile, K = 288
   static constexpr int kAresBytes = kAres ? 2 * kATileBytes : 0;  // kAres: the item's two tiles
   static constexpr int kThreads = 384;                            // 2 consumer warpgroups + 1 producer warpgroup
   static constexpr int kVecBytes = kAres ? 0 : 3 * kDP * 4;       // row epilogue: bias, LayerNorm gamma, beta (fp32)
-  static constexpr int kSmemBytes = kAresBytes + kStages * kStageBytes + 256 + kVecBytes;
+  // ring of nst stages, then 256 bytes of mbarriers, then the row epilogue's vectors
+  __host__ __device__ static constexpr int smem_bytes(int nst) { return kAresBytes + nst * kStageBytes + 256 + kVecBytes; }
+  static constexpr int kSmemBytes = smem_bytes(kStages);          // the most any launch asks for
+  static_assert(kSmemBytes <= 232448, "over the sm_90 opt-in shared memory per block");
+  static_assert((2 * kStages + 4) * 8 <= 256, "the mbarriers (full, empty, a_full, a_empty, turn[2]) fill 256 bytes");
 };
 
 template <int BN>
@@ -162,12 +185,16 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
   static_assert(EPI != EPI_ROW || (Cfg::kNI == kDP && !kAres), "row epilogue needs the full 288-wide row");
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* a_res = smem;
+  const int kstages = ksteps / Cfg::kSK;   // ksteps % kSK == 0 (launchers): every stage holds exactly kSK k-steps, so
+                                           // its wgmma run is straight-line code with no register moves in between
+  const int nst = Cfg::stages(kstages);   // ring depth; the launch asks for Cfg::smem_bytes(nst)
   uint8_t* stage_base = smem + Cfg::kAresBytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(stage_base + Cfg::kStages * Cfg::kStageBytes);
-  uint64_t* empty = full + Cfg::kStages;
-  uint64_t* a_full = empty + Cfg::kStages;
+  uint64_t* full = reinterpret_cast<uint64_t*>(stage_base + nst * Cfg::kStageBytes);
+  uint64_t* empty = full + nst;
+  uint64_t* a_full = empty + nst;
   uint64_t* a_empty = a_full + 1;
-  float* s_vec = reinterpret_cast<float*>(stage_base + Cfg::kStages * Cfg::kStageBytes + 256);   // [3][kDP]
+  uint64_t* turn = a_empty + 1;   // [2], kAres: ordered epilogues
+  float* s_vec = reinterpret_cast<float*>(stage_base + nst * Cfg::kStageBytes + 256);   // [3][kDP]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -178,12 +205,14 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
     }
   }
   if (threadIdx.x == 0) {
-    for (int i = 0; i < Cfg::kStages; ++i) {
+    for (int i = 0; i < nst; ++i) {
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], 256);   // every consumer thread (no lane-divergent code between the wgmma)
     }
     mbar_init(a_full, 1);
     mbar_init(a_empty, 256);
+    mbar_init(&turn[0], 128);   // the other warpgroup's threads, once per epilogue
+    mbar_init(&turn[1], 128);
     mbar_fence_init();
   }
   __syncthreads();
@@ -191,8 +220,6 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
   // kAres: a work item is a tile pair (its n-groups run back to back on the resident A); otherwise a (tile, n-group) pair
   const int nitems = kAres ? (ntiles + 1) / 2 : ntiles * ngroups;
   const int gper = kAres ? ngroups : 1;
-  const int kstages = ksteps / Cfg::kSK;   // ksteps % kSK == 0 (launchers): every stage holds exactly kSK k-steps, so
-                                           // its wgmma run is straight-line code with no register moves in between
   const size_t a_tile_bytes = (size_t)a_ksteps * Cfg::kABytesPerK;
   const size_t b_group_bytes = (size_t)ksteps * Cfg::kBBytesPerK;
 
@@ -228,7 +255,7 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
               st += Cfg::kSK * Cfg::kABytesPerK;
             }
             bulk_g2s(st, b_src + (size_t)s * Cfg::kSK * Cfg::kBBytesPerK, kh * Cfg::kBBytesPerK, &full[slot]);
-            if (++slot == Cfg::kStages) { slot = 0; phase ^= 1; }
+            if (++slot == nst) { slot = 0; phase ^= 1; }
           }
         }
       }
@@ -244,6 +271,10 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
   const int row0 = (kAres ? 0 : wg * 64) + (warp & 3) * 16 + g;
   float accm[Cfg::kMH][NCH][BN / 2];
   uint32_t slot = 0, phase = 0, it = 0;
+  // kAres: this warpgroup's n-th epilogue waits until the partner has passed the turn n - wg times (warpgroup 0 starts)
+  uint32_t epis = 0;
+  auto wait_turn = [&]() { mbar_wait(&turn[wg], (epis & 1) ^ (wg ^ 1)); };
+  auto pass_turn = [&]() { mbar_arrive(&turn[wg ^ 1]); ++epis; };
   for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++it) {
     const int tile = kAres ? 2 * item + wg : item / ngroups;
     if constexpr (kAres) {
@@ -251,10 +282,14 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
       if (tile >= ntiles) {
         // the pair has one tile: step through the same barrier phases as the partner warpgroup without MMAs or stores
         // (waiting on `full` keeps these arrivals from running ahead into the slot's next phase)
-        for (int s = 0; s < gper * kstages; ++s) {
-          mbar_wait(&full[slot], phase);
-          mbar_arrive(&empty[slot]);
-          if (++slot == Cfg::kStages) { slot = 0; phase ^= 1; }
+        for (int gi = 0; gi < gper; ++gi) {
+          for (int s = 0; s < kstages; ++s) {
+            mbar_wait(&full[slot], phase);
+            mbar_arrive(&empty[slot]);
+            if (++slot == nst) { slot = 0; phase ^= 1; }
+          }
+          wait_turn();
+          pass_turn();
         }
         mbar_arrive(a_empty);
         continue;
@@ -296,7 +331,7 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
         wgmma_wait<1>();
         if (s > 0) mbar_arrive(&empty[prev]);
         prev = slot;
-        if (++slot == Cfg::kStages) { slot = 0; phase ^= 1; }
+        if (++slot == nst) { slot = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
 #pragma unroll
@@ -307,6 +342,7 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
       if (kAres && gi + 1 == gper) mbar_arrive(a_empty);   // the last group's MMAs have read A
 
       // ----------------------------------------------------------- epilogue (fragment: row, 2 adjacent columns)
+      if constexpr (kAres) wait_turn();
       if constexpr (EPI == EPI_QKV || EPI == EPI_RELU) {
         __nv_bfloat16* obase = out_img + (size_t)tile * kTileM * out_chunks * 8;
 #pragma unroll
@@ -328,6 +364,7 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
                     pack_bf16x2(v0, v1);
               }
           }
+        if constexpr (kAres) pass_turn();   // the stores are issued; they drain under the partner's MMAs
       } else {
         float (&acc)[NCH][BN / 2] = accm[0];   // one m64 block per warpgroup
         // x is updated in place, so the compiler keeps each x_old load behind every store that precedes it in source
@@ -762,7 +799,8 @@ void launch_gemm_row(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int
                      const RowEpi& epi, cudaStream_t st) {
   using Cfg = GemmCfg<kNC, 2, false>;
   const int grid = ntiles < num_sms() ? ntiles : num_sms();
-  gemm_kernel<kNC, 2, EPI_ROW, false><<<grid, Cfg::kThreads, Cfg::kSmemBytes, st>>>(a_img, b_img, a_ksteps, b_ksteps, ntiles, 1,
+  const int smem = Cfg::smem_bytes(Cfg::stages(b_ksteps / Cfg::kSK));
+  gemm_kernel<kNC, 2, EPI_ROW, false><<<grid, Cfg::kThreads, smem, st>>>(a_img, b_img, a_ksteps, b_ksteps, ntiles, 1,
                                                                                     nullptr, 0, nullptr, epi);
 }
 
