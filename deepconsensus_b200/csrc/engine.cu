@@ -146,7 +146,8 @@ struct dcb_engine {
   DevBuf<float> d_x;
   DevBuf<__nv_bfloat16> d_xb;
   DevBuf<__nv_bfloat16> d_att;
-  DevBuf<__nv_bfloat16> d_hid;   // FFN hidden activation, bf16 operand image [tile][ff/8][128][8]
+  DevBuf<float> d_part;          // the FFN's partial sums between its two launches, residual image layout
+  DevBuf<__nv_bfloat16> d_hid;   // FFN hidden activation, bf16 operand image [tile][ff/8][128][8] (debug capture only)
   DevBuf<double> d_p10;          // 10^(-q/10), q = 0..255 (host libm pow, as NumPy)
   DevBuf<float> d_dbg;           // [stages][chunk_tiles * x_image]
   DevBuf<__nv_bfloat16> d_dbg_op;   // bf16 operand images per stage (dbg_operand_slot)
@@ -646,7 +647,7 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
     if (!rc) rc = alloc(e, e->d_x, T * x_image_elems());
     if (!rc) rc = alloc(e, e->d_xb, T * act_image_elems(kDP));
     if (!rc) rc = alloc(e, e->d_att, T * act_image_elems(kDP));
-    if (!rc) rc = alloc(e, e->d_hid, T * act_image_elems(cfg->filter_size));
+    if (!rc) rc = alloc(e, e->d_part, T * x_image_elems());
     return rc;
   }();
   if (rc) {
@@ -762,6 +763,8 @@ int dcb_set_debug(dcb_engine* e, int32_t enabled) {
     int w = 0;
     dbg_operand_slot(e, (int)stages - 1, DCB_DEBUG_HID, &cols, &w);   // the last stage holds HID only
     rc = alloc(e, e->d_dbg_op, (cols + w) * e->chunk_tiles * kTileM);
+    if (rc) return rc;
+    rc = alloc(e, e->d_hid, e->chunk_tiles * act_image_elems(e->cfg.filter_size));
     if (rc) return rc;
   }
   return DCB_OK;
@@ -929,15 +932,16 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
       launch_gemm_row(e->d_att, ld.wo, kDP / 16, 2 * (kDP / 16), T, ea, st);
       pend();
       snap();
-      // FFN: hidden = relu(xb W1 + b1), then hidden W2 + b2 + residual; xb = the next layer's input
+      // FFN: relu(xb W1 + b1) W2 + b2 + residual, half of the filter per launch; xb = the next layer's input
       RowEpi ef{};
       ef.x = e->d_x; ef.xb = last ? nullptr : e->d_xb.p; ef.bias = ld.b2; ef.pe = nullptr;
       ef.ln_g = (c.rezero || last) ? nullptr : e->w.layers[n_ + 1].ln_g[0].p;
       ef.ln_b = (c.rezero || last) ? nullptr : e->w.layers[n_ + 1].ln_b[0].p;
       ef.has_xold = 1; ef.L = Lw;
       pbegin(kProfFfn);
-      launch_ffn_up(e->d_xb, ld.w1, ld.b1, c.filter_size, T, e->d_hid, st);
-      launch_gemm_row(e->d_hid, ld.w2, c.filter_size / 16, c.filter_size / 16, T, ef, st);
+      __nv_bfloat16* hid = e->debug ? e->d_hid.p : nullptr;
+      launch_ffn(false, e->d_xb, ld.w1, ld.b1, ld.w2, c.filter_size, T, e->d_part, hid, ef, st);
+      launch_ffn(true, e->d_xb, ld.w1, ld.b1, ld.w2, c.filter_size, T, e->d_part, hid, ef, st);
       pend();
       if (e->profile) e->prof_ffn_tokens += (long long)bw * L;   // valid tokens (layout padding is not algorithmic work)
       snap();

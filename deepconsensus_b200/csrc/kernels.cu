@@ -5,8 +5,9 @@
 //                        data_providers.py:151-162, networks.py:42-63,457-507)
 //   gemm_kernel         persistent, warp-specialised wgmma GEMM: bulk-copy (TMA) producer warp
 //                       feeding two consumer warpgroups through an mbarrier ring.  Used for the
-//                       condenser (+pos-enc), fused QKV, attention out-proj and both FFN
-//                       projections (relu(x W1 + b1) W2 + b2, ffn_layer.py:83-86).
+//                       condenser (+pos-enc), fused QKV and attention out-proj.
+//   ffn_gemm_kernel     the FFN relu(x W1 + b1) W2 + b2 (ffn_layer.py:83-86) with the hidden
+//                       activation kept in registers, half of the filter per launch.
 //   band_attention_kernel  banded multi-head softmax attention (attention_layer.py:198-214)
 //   head_kernel         final LayerNorm -> fc1 -> softmax -> argmax -> Phred -> ASCII
 //                       (encoder_stack.py:197, networks.py:342,238, quick_inference.py:377-414)
@@ -106,7 +107,7 @@ embed_rows_kernel(const float* __restrict__ rows, const uint8_t* __restrict__ pa
 // 64-127, accumulators in registers); one thread of warpgroup 2 streams operands into shared memory with bulk copies
 // (TMA) that complete on mbarriers.  setmaxnreg moves the producer warpgroup's registers to the consumers.
 //
-// kAres (the K = 288 projections with several n-groups: fused QKV, FFN up-projection): a work item is a pair of
+// kAres (the K = 288 projection with several n-groups: fused QKV): a work item is a pair of
 // consecutive tiles (2i, 2i + 1).  Both A tiles are loaded once and stay resident while every n-group streams its B
 // k-steps through the stage ring; warpgroup w owns tile 2i + w and issues two m64 wgmmas (tile rows 0-63, 64-127) per B
 // k-step, so every weight byte that crosses from L2 feeds 256 tokens.  An odd tile count leaves the last pair with one
@@ -120,16 +121,15 @@ embed_rows_kernel(const float* __restrict__ rows, const uint8_t* __restrict__ pa
 // converts and stores its accumulators the other keeps the tensor cores busy, and the output stores drain under the
 // partner's MMAs.  The idle warpgroup of a one-tile pair takes and passes its turns like a working one.
 //
-// Otherwise (the row epilogue GEMMs, one n-group covering all 288 columns, K up to 2048) warpgroup w owns tile
-// rows [64 w, 64 w + 64) of one tile, and A and B k-steps stream together.
+// Otherwise (the row epilogue GEMMs, one n-group covering all 288 columns) warpgroup w owns tile rows
+// [64 w, 64 w + 64) of one tile, and A and B k-steps stream together.
 //
 // Split-bf16 weights: the B image may hold K twice as [W_hi; W_lo] (b_ksteps = 2 * a_ksteps, W_lo = bf16(W - W_hi));
 // the A k-steps are then read twice, so the accumulator sums A W_hi + A W_lo and the weights carry ~16 mantissa bits.
 //
 // EPI_QKV  : bf16 into an operand image (column offset group * NI)
-// EPI_RELU : bf16(relu(acc + bias)) into an operand image (the FFN hidden activation)
 // EPI_ROW  : row epilogue (residual / bias / pos-enc / LayerNorm), NI must be the full 288-wide row
-enum { EPI_QKV = 0, EPI_ROW = 1, EPI_RELU = 2 };
+enum { EPI_QKV = 0, EPI_ROW = 1 };
 
 template <int BN, int NCH, bool kAres>
 struct GemmCfg {
@@ -141,8 +141,8 @@ struct GemmCfg {
   // Ring depth.  kAres: the warpgroups take turns at their epilogues (gemm_kernel), so one runs up to an epilogue ahead
   // of the other over the same B stages; 8 stages hold that offset on top of the prefetch depth.  The row GEMMs keep
   // their epilogues in lockstep (taking turns made the condenser and the out-projection slower) and take 8 stages when
-  // an item streams at least kLongK of them (condenser, FFN down-projection: 10 % and 14 % faster on an H100 at 700 W);
-  // the out-projection (18 stages per item) keeps 4.
+  // an item streams at least kLongK of them (the condenser: 10 % faster on an H100 at 700 W); the out-projection (18
+  // stages per item) keeps 4.
   static constexpr int kStages = 8;
   static constexpr int kShortStages = 4;
   static constexpr int kLongK = 32;
@@ -175,12 +175,119 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v;
 }
 
+// The row epilogue's per-column vectors in shared memory: bias, LayerNorm gamma, beta (fp32 [3][kDP]).
+__device__ __forceinline__ void row_vectors_to_smem(float* s_vec, const RowEpi& epi) {
+  for (int i = threadIdx.x; i < kDP; i += blockDim.x) {
+    if (epi.bias) s_vec[i] = epi.bias[i];
+    if (epi.ln_g) { s_vec[kDP + i] = epi.ln_g[i]; s_vec[2 * kDP + i] = epi.ln_b[i]; }
+  }
+}
+
+// Row epilogue of one consumer warpgroup's 64 rows of a tile (accumulator fragment: row, 2 adjacent columns; the
+// thread's rows are row0 and row0 + 8): x_new = acc (+ x_old) (+ bias) (+ pos-enc) into the residual image, and the next
+// sub-layer's bf16 operand (identity or LayerNorm) into epi.xb unless it is null.  Ends the accumulators' live range.
+// kPe false: the caller never adds the positional encoding (epi.pe is ignored), which leaves the epilogue the
+// registers its address arithmetic would take.
+template <int BN, int NCH, bool kPe = true>
+__device__ __forceinline__ void row_epilogue(float (&acc)[NCH][BN / 2], int tile, int row0, int q, const float* s_vec,
+                                             const RowEpi& epi) {
+  // x is updated in place, so the compiler keeps each x_old load behind every store that precedes it in source
+  // order.  Each pass (row half h, accumulator chunk j) therefore issues all of its global loads before its first
+  // store: four batches of 18 loads per tile instead of a load -> store round trip per fragment.  The per-column
+  // vectors come from shared memory (s_vec).  Fragment (j, jj) holds columns c0 + 2q, c0 + 2q + 1 with
+  // c0 = j * BN + jj * 8; in the residual image (and pe_img) it sits c0 * kTileM floats past this thread's xr.
+  // (Prefetching the residual tile into L2 from the producer when it starts the item was measured ~3 % slower
+  // per step on an H100 SXM at 400 W than these batched loads alone.)
+  float* xt = epi.x + (size_t)tile * x_image_elems();
+  const int xoff = ((q >> 1) * kTileM + row0) * 4 + 2 * (q & 1);
+  const bool ln = epi.ln_g != nullptr;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + 8 * h;
+    const int l = (tile * kTileM + row) % epi.L;
+    float* xr = xt + xoff + 32 * h;
+    const float* per = epi.pe_img ? epi.pe_img + xoff + 32 * h : epi.pe + (size_t)l * kDP + 2 * q;
+    const int pe_stride = epi.pe_img ? kTileM : 1;   // floats per column step of c0
+    float s1 = 0.f;
+#pragma unroll
+    for (int j = 0; j < NCH; ++j) {
+      float2 ld[BN / 8];
+      if (epi.has_xold) {
+#pragma unroll
+        for (int jj = 0; jj < BN / 8; ++jj)
+          ld[jj] = *reinterpret_cast<const float2*>(xr + (j * BN + jj * 8) * kTileM);
+#pragma unroll
+        for (int jj = 0; jj < BN / 8; ++jj) {
+          acc[j][jj * 4 + 2 * h] += ld[jj].x;
+          acc[j][jj * 4 + 2 * h + 1] += ld[jj].y;
+        }
+      }
+      if (kPe && epi.pe) {
+#pragma unroll
+        for (int jj = 0; jj < BN / 8; ++jj)
+          ld[jj] = __ldg(reinterpret_cast<const float2*>(per + (size_t)(j * BN + jj * 8) * pe_stride));
+      }
+#pragma unroll
+      for (int jj = 0; jj < BN / 8; ++jj) {
+        const int col = j * BN + jj * 8 + 2 * q;
+        float2 v = make_float2(acc[j][jj * 4 + 2 * h], acc[j][jj * 4 + 2 * h + 1]);
+        if (epi.bias) {
+          const float2 b = *reinterpret_cast<const float2*>(s_vec + col);
+          v.x += b.x; v.y += b.y;
+        }
+        if (kPe && epi.pe) { v.x += ld[jj].x; v.y += ld[jj].y; }
+        v.x = col < kD ? v.x : 0.f;
+        v.y = col + 1 < kD ? v.y : 0.f;
+        *reinterpret_cast<float2*>(xr + (j * BN + jj * 8) * kTileM) = v;
+        acc[j][jj * 4 + 2 * h] = v.x;
+        acc[j][jj * 4 + 2 * h + 1] = v.y;
+        s1 += v.x + v.y;
+      }
+    }
+    if (!epi.xb) continue;
+    float mean = 0.f, rstd = 1.f;
+    if (ln) {   // LayerNorm, eps = 1e-6, biased variance (two passes over the registers)
+      mean = quad_sum(s1) * (1.f / kD);
+      float s2 = 0.f;
+#pragma unroll
+      for (int j = 0; j < NCH; ++j)
+#pragma unroll
+        for (int jj = 0; jj < BN / 8; ++jj) {
+          const int col = j * BN + jj * 8 + 2 * q;
+          const float d0 = col < kD ? acc[j][jj * 4 + 2 * h] - mean : 0.f;
+          const float d1 = col + 1 < kD ? acc[j][jj * 4 + 2 * h + 1] - mean : 0.f;
+          s2 += d0 * d0 + d1 * d1;
+        }
+      rstd = rsqrtf(quad_sum(s2) * (1.f / kD) + 1e-6f);
+    }
+    __nv_bfloat16* xb = epi.xb + (size_t)tile * act_image_elems(kDP) + row * 8 + 2 * q;
+#pragma unroll
+    for (int j = 0; j < NCH; ++j)
+#pragma unroll
+      for (int jj = 0; jj < BN / 8; ++jj) {
+        const int col = j * BN + jj * 8 + 2 * q;
+        float v0 = acc[j][jj * 4 + 2 * h], v1 = acc[j][jj * 4 + 2 * h + 1];
+        if (ln) {
+          v0 = col < kD ? (v0 - mean) * rstd * s_vec[kDP + col] + s_vec[2 * kDP + col] : 0.f;
+          v1 = col + 1 < kD ? (v1 - mean) * rstd * s_vec[kDP + col + 1] + s_vec[2 * kDP + col + 1] : 0.f;
+        }
+        *reinterpret_cast<uint32_t*>(xb + (j * BN + jj * 8) * kTileM) = pack_bf16x2(v0, v1);
+      }
+  }
+  // The next item's first wgmma does not read the accumulators (scale-d 0), but the register fences before it
+  // do.  Redefining them here ends each half's live range after its last use above, which leaves the second
+  // half the registers its batched loads need (without this ptxas spills).
+#pragma unroll
+  for (int j = 0; j < NCH; ++j)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[j][i] = 0.f;
+}
+
 template <int BN, int NCH, int EPI, bool kAres>
 __global__ void __launch_bounds__(384, 1)
 gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __restrict__ b_img, int a_ksteps, int ksteps,
             int ntiles,
-            int ngroups, __nv_bfloat16* __restrict__ out_img, int out_chunks, const float* __restrict__ out_bias,
-            RowEpi epi) {
+            int ngroups, __nv_bfloat16* __restrict__ out_img, int out_chunks, RowEpi epi) {
   using Cfg = GemmCfg<BN, NCH, kAres>;
   static_assert(EPI != EPI_ROW || (Cfg::kNI == kDP && !kAres), "row epilogue needs the full 288-wide row");
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -198,12 +305,7 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  if constexpr (EPI == EPI_ROW) {
-    for (int i = threadIdx.x; i < kDP; i += blockDim.x) {
-      if (epi.bias) s_vec[i] = epi.bias[i];
-      if (epi.ln_g) { s_vec[kDP + i] = epi.ln_g[i]; s_vec[2 * kDP + i] = epi.ln_b[i]; }
-    }
-  }
+  if constexpr (EPI == EPI_ROW) row_vectors_to_smem(s_vec, epi);
   if (threadIdx.x == 0) {
     for (int i = 0; i < nst; ++i) {
       mbar_init(&full[i], 1);
@@ -343,7 +445,7 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
 
       // ----------------------------------------------------------- epilogue (fragment: row, 2 adjacent columns)
       if constexpr (kAres) wait_turn();
-      if constexpr (EPI == EPI_QKV || EPI == EPI_RELU) {
+      if constexpr (EPI == EPI_QKV) {
         __nv_bfloat16* obase = out_img + (size_t)tile * kTileM * out_chunks * 8;
 #pragma unroll
         for (int mh = 0; mh < Cfg::kMH; ++mh)
@@ -355,109 +457,241 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
 #pragma unroll
               for (int jj = 0; jj < BN / 8; ++jj) {
                 const int col = grp * Cfg::kNI + j * BN + jj * 8 + 2 * q;
-                float v0 = accm[mh][j][jj * 4 + 2 * h], v1 = accm[mh][j][jj * 4 + 2 * h + 1];
-                if constexpr (EPI == EPI_RELU) {
-                  v0 = fmaxf(v0 + __ldg(out_bias + col), 0.f);
-                  v1 = fmaxf(v1 + __ldg(out_bias + col + 1), 0.f);
-                }
                 *reinterpret_cast<uint32_t*>(obase + ((size_t)(col >> 3) * kTileM + row) * 8 + (col & 7)) =
-                    pack_bf16x2(v0, v1);
+                    pack_bf16x2(accm[mh][j][jj * 4 + 2 * h], accm[mh][j][jj * 4 + 2 * h + 1]);
               }
           }
         if constexpr (kAres) pass_turn();   // the stores are issued; they drain under the partner's MMAs
       } else {
-        float (&acc)[NCH][BN / 2] = accm[0];   // one m64 block per warpgroup
-        // x is updated in place, so the compiler keeps each x_old load behind every store that precedes it in source
-        // order.  Each pass (row half h, accumulator chunk j) therefore issues all of its global loads before its first
-        // store: four batches of 18 loads per tile instead of a load -> store round trip per fragment.  The per-column
-        // vectors come from shared memory (s_vec).  Fragment (j, jj) holds columns c0 + 2q, c0 + 2q + 1 with
-        // c0 = j * BN + jj * 8; in the residual image (and pe_img) it sits c0 * kTileM floats past this thread's xr.
-        // (Prefetching the residual tile into L2 from the producer when it starts the item was measured ~3 % slower
-        // per step on an H100 SXM at 400 W than these batched loads alone.)
-        float* xt = epi.x + (size_t)tile * x_image_elems();
-        const int xoff = ((q >> 1) * kTileM + row0) * 4 + 2 * (q & 1);
-        const bool ln = epi.ln_g != nullptr;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = row0 + 8 * h;
-          const int l = (tile * kTileM + row) % epi.L;
-          float* xr = xt + xoff + 32 * h;
-          const float* per = epi.pe_img ? epi.pe_img + xoff + 32 * h : epi.pe + (size_t)l * kDP + 2 * q;
-          const int pe_stride = epi.pe_img ? kTileM : 1;   // floats per column step of c0
-          float s1 = 0.f;
-#pragma unroll
-          for (int j = 0; j < NCH; ++j) {
-            float2 ld[BN / 8];
-            if (epi.has_xold) {
-#pragma unroll
-              for (int jj = 0; jj < BN / 8; ++jj)
-                ld[jj] = *reinterpret_cast<const float2*>(xr + (j * BN + jj * 8) * kTileM);
-#pragma unroll
-              for (int jj = 0; jj < BN / 8; ++jj) {
-                acc[j][jj * 4 + 2 * h] += ld[jj].x;
-                acc[j][jj * 4 + 2 * h + 1] += ld[jj].y;
-              }
-            }
-            if (epi.pe) {
-#pragma unroll
-              for (int jj = 0; jj < BN / 8; ++jj)
-                ld[jj] = __ldg(reinterpret_cast<const float2*>(per + (size_t)(j * BN + jj * 8) * pe_stride));
-            }
-#pragma unroll
-            for (int jj = 0; jj < BN / 8; ++jj) {
-              const int col = j * BN + jj * 8 + 2 * q;
-              float2 v = make_float2(acc[j][jj * 4 + 2 * h], acc[j][jj * 4 + 2 * h + 1]);
-              if (epi.bias) {
-                const float2 b = *reinterpret_cast<const float2*>(s_vec + col);
-                v.x += b.x; v.y += b.y;
-              }
-              if (epi.pe) { v.x += ld[jj].x; v.y += ld[jj].y; }
-              v.x = col < kD ? v.x : 0.f;
-              v.y = col + 1 < kD ? v.y : 0.f;
-              *reinterpret_cast<float2*>(xr + (j * BN + jj * 8) * kTileM) = v;
-              acc[j][jj * 4 + 2 * h] = v.x;
-              acc[j][jj * 4 + 2 * h + 1] = v.y;
-              s1 += v.x + v.y;
-            }
-          }
-          if (!epi.xb) continue;
-          float mean = 0.f, rstd = 1.f;
-          if (ln) {   // LayerNorm, eps = 1e-6, biased variance (two passes over the registers)
-            mean = quad_sum(s1) * (1.f / kD);
-            float s2 = 0.f;
-#pragma unroll
-            for (int j = 0; j < NCH; ++j)
-#pragma unroll
-              for (int jj = 0; jj < BN / 8; ++jj) {
-                const int col = j * BN + jj * 8 + 2 * q;
-                const float d0 = col < kD ? acc[j][jj * 4 + 2 * h] - mean : 0.f;
-                const float d1 = col + 1 < kD ? acc[j][jj * 4 + 2 * h + 1] - mean : 0.f;
-                s2 += d0 * d0 + d1 * d1;
-              }
-            rstd = rsqrtf(quad_sum(s2) * (1.f / kD) + 1e-6f);
-          }
-          __nv_bfloat16* xb = epi.xb + (size_t)tile * act_image_elems(kDP) + row * 8 + 2 * q;
-#pragma unroll
-          for (int j = 0; j < NCH; ++j)
-#pragma unroll
-            for (int jj = 0; jj < BN / 8; ++jj) {
-              const int col = j * BN + jj * 8 + 2 * q;
-              float v0 = acc[j][jj * 4 + 2 * h], v1 = acc[j][jj * 4 + 2 * h + 1];
-              if (ln) {
-                v0 = col < kD ? (v0 - mean) * rstd * s_vec[kDP + col] + s_vec[2 * kDP + col] : 0.f;
-                v1 = col + 1 < kD ? (v1 - mean) * rstd * s_vec[kDP + col + 1] + s_vec[2 * kDP + col + 1] : 0.f;
-              }
-              *reinterpret_cast<uint32_t*>(xb + (j * BN + jj * 8) * kTileM) = pack_bf16x2(v0, v1);
-            }
-        }
-        // The next item's first wgmma does not read the accumulators (scale-d 0), but the register fences before it
-        // do.  Redefining them here ends each half's live range after its last use above, which leaves the second
-        // half the registers its batched loads need (without this ptxas spills).
-#pragma unroll
-        for (int j = 0; j < NCH; ++j)
-#pragma unroll
-          for (int i = 0; i < BN / 2; ++i) acc[j][i] = 0.f;
+        row_epilogue<BN, NCH>(accm[0], tile, row0, q, s_vec, epi);   // one m64 block per warpgroup
       }
+    }
+  }
+}
+
+// =====================================================================================
+// FFN with the hidden activation on the SM
+// =====================================================================================
+// out = relu(xb W1 + b1) W2 + b2 + x for one 128-token tile per work item, over the filter's 128-unit chunks
+// [c_begin, c_end).  The tile's xb (A) image is loaded once and stays resident; warpgroup w owns tile rows
+// [64 w, 64 w + 64).  Per chunk c each consumer warpgroup
+//   1. computes H = xb W1[:, c] with m64n128k16 wgmmas over the 18 k-steps (the W1 image holds chunk c as one
+//      contiguous [36][128][8] group),
+//   2. turns H into bf16(relu(H + b1)) in registers, packed straight into the A fragments of the next step (for
+//      hidden k-step kk: pack(d[8kk + 0..1]), pack(d[8kk + 2..3]), pack(d[8kk + 4..5]), pack(d[8kk + 6..7])),
+//   3. accumulates that times W2's rows of chunk c (k-steps [8c, 8c + 8) of the [ff/8][288][8] image) with register-A
+//      m64n144k16 wgmmas into the 288-wide fp32 accumulators.
+// The producer streams W1 group c and then W2's k-steps of c through one ring of 9216-byte stages (two W1 k-steps or
+// one W2 k-step each).
+//
+// The forward launches the kernel twice per layer, each over half of the chunks, because each of the forward's five
+// launches per layer ends on a captured stage.  The first launch (kFinish false) starts from zero and stores the fp32
+// accumulators to `part`, an image with the residual image's layout; the second (kFinish true) loads them back and
+// ends with the row epilogue.  Every output element sees the same k16 MMAs in the same order on one fp32 accumulator,
+// and the hidden values come from the same instruction shape, K order, bias, ReLU and rounding as a separate
+// up-projection would give, so the result does not depend on where the filter is split.  When `hid` is not null the
+// hidden activation is also stored there as a bf16 operand image [tile][ff/8][128][8] (debug capture).
+struct FfnCfg {
+  static constexpr int kUpK = kDP / 16;                   // up-projection k-steps per chunk
+  static constexpr int kDownK = kFFChunk / 16;            // down-projection k-steps per chunk
+  static constexpr int kABytesPerK = 2 * kTileM * 16;     // 4096
+  static constexpr int kW1Bytes = 2 * kFFChunk * 16;      // one W1 k-step: 4096
+  static constexpr int kW2Bytes = 2 * kDP * 16;           // one W2 k-step: 9216
+  static constexpr int kStageBytes = kW2Bytes;            // two W1 k-steps or one W2 k-step
+  static constexpr int kStages = 16;
+  static constexpr int kATileBytes = kUpK * kABytesPerK;  // the resident xb tile
+  static constexpr int kBarBytes = 512;
+  static constexpr int kVecBytes = 3 * kDP * 4;           // row epilogue: bias, LayerNorm gamma, beta (fp32)
+  static constexpr int kMaxChunks = (2048 / kFFChunk + 1) / 2;   // a launch's chunks at filter_size 2048
+  static constexpr int kB1Bytes = kMaxChunks * kFFChunk * 4;     // the launch's b1 slice (fp32)
+  // the xb tile, the ring, the mbarriers, the row vectors, b1
+  static constexpr int kSmemBytes = kATileBytes + kStages * kStageBytes + kBarBytes + kVecBytes + kB1Bytes;
+  static constexpr int kThreads = 384;
+  static_assert(kSmemBytes <= 232448, "over the sm_90 opt-in shared memory per block");
+  static_assert((2 * kStages + 2) * 8 <= kBarBytes, "the mbarriers (full, empty, a_full, a_empty) fit");
+  static_assert(2 * kW1Bytes <= kStageBytes && kUpK % 2 == 0, "a stage holds two W1 k-steps");
+};
+
+template <bool kFinish>
+__global__ void __launch_bounds__(384, 1)
+ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* __restrict__ w1_img,
+                const float* __restrict__ b1, const __nv_bfloat16* __restrict__ w2_img, int ff, int c_begin, int c_end,
+                int ntiles, float* __restrict__ part, __nv_bfloat16* __restrict__ hid, RowEpi epi) {
+  using Cfg = FfnCfg;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* a_res = smem;
+  uint8_t* stage_base = smem + Cfg::kATileBytes;
+  uint64_t* full = reinterpret_cast<uint64_t*>(stage_base + Cfg::kStages * Cfg::kStageBytes);
+  uint64_t* empty = full + Cfg::kStages;
+  uint64_t* a_full = empty + Cfg::kStages;
+  uint64_t* a_empty = a_full + 1;
+  float* s_vec = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + Cfg::kBarBytes);   // [3][kDP]
+  float* s_b1 = s_vec + 3 * kDP;                                                                  // chunks c_begin..
+  const int nch = c_end - c_begin;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if constexpr (kFinish) row_vectors_to_smem(s_vec, epi);
+  for (int i = threadIdx.x; i < nch * kFFChunk; i += blockDim.x) s_b1[i] = b1[c_begin * kFFChunk + i];
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < Cfg::kStages; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 256);   // every consumer thread
+    }
+    mbar_init(a_full, 1);
+    mbar_init(a_empty, 256);
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // ------------------------------------------------------------- producer
+    setmaxnreg_dec<24>();
+    if (warp == 8 && lane == 0 && nch > 0) {
+      uint32_t slot = 0, phase = 0, it = 0;
+      auto stage = [&](const uint8_t* src, uint32_t bytes) {
+        mbar_wait(&empty[slot], phase ^ 1);
+        mbar_arrive_expect_tx(&full[slot], bytes);
+        bulk_g2s(stage_base + slot * Cfg::kStageBytes, src, bytes, &full[slot]);
+        if (++slot == Cfg::kStages) { slot = 0; phase ^= 1; }
+      };
+      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+        mbar_wait(a_empty, (it & 1) ^ 1);
+        mbar_arrive_expect_tx(a_full, Cfg::kATileBytes);
+        bulk_g2s(a_res, reinterpret_cast<const uint8_t*>(xb_img) + (size_t)tile * Cfg::kATileBytes, Cfg::kATileBytes,
+                 a_full);
+        for (int c = c_begin; c < c_end; ++c) {
+          const uint8_t* w1 = reinterpret_cast<const uint8_t*>(w1_img) + (size_t)c * Cfg::kUpK * Cfg::kW1Bytes;
+          for (int s = 0; s < Cfg::kUpK / 2; ++s) stage(w1 + (size_t)s * 2 * Cfg::kW1Bytes, 2 * Cfg::kW1Bytes);
+          const uint8_t* w2 = reinterpret_cast<const uint8_t*>(w2_img) + (size_t)c * Cfg::kDownK * Cfg::kW2Bytes;
+          for (int kk = 0; kk < Cfg::kDownK; ++kk) stage(w2 + (size_t)kk * Cfg::kW2Bytes, Cfg::kW2Bytes);
+        }
+      }
+    }
+    return;
+  }
+
+  // --------------------------------------------------------------- consumers (2 warpgroups)
+  setmaxnreg_inc<240>();
+  const int wg = warp >> 2;
+  const int g = lane >> 2, q = lane & 3;
+  const int row0 = wg * 64 + (warp & 3) * 16 + g;   // this thread's accumulator rows: row0, row0 + 8
+  const uint32_t a_base = smem_u32(a_res) + wg * 64 * 16;
+  float acc[2][kNC / 2];          // out[:, 0..287]
+  float hacc[kFFChunk / 2];       // H of the current chunk
+  uint32_t slot = 0, phase = 0, it = 0;
+  auto next_slot = [&]() { if (++slot == Cfg::kStages) { slot = 0; phase ^= 1; } };
+  // the accumulators' fragments in the partial image (the residual image's layout, as in row_epilogue)
+  auto part_frag = [&](int tile, int h, int j, int jj) {
+    return part + (size_t)tile * x_image_elems() + ((q >> 1) * kTileM + row0) * 4 + 2 * (q & 1) + 32 * h +
+           (j * kNC + jj * 8) * kTileM;
+  };
+  auto load_part = [&](int tile) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int jj = 0; jj < kNC / 8; ++jj) {
+          const float2 v = *reinterpret_cast<const float2*>(part_frag(tile, h, j, jj));
+          acc[j][jj * 4 + 2 * h] = v.x;
+          acc[j][jj * 4 + 2 * h + 1] = v.y;
+        }
+  };
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+    if constexpr (kFinish) load_part(tile);   // the partial sums load while xb and the first weights arrive
+    if (nch > 0) mbar_wait(a_full, it & 1);
+    for (int c = c_begin; c < c_end; ++c) {
+      // ---- 1. H = xb W1[:, c]
+      uint32_t prev = 0;
+#pragma unroll
+      for (int s = 0; s < Cfg::kUpK / 2; ++s) {
+        mbar_wait(&full[slot], phase);
+        const uint32_t st = smem_u32(stage_base + slot * Cfg::kStageBytes);
+        // H starts at the chunk's first wgmma (scale-d 0, written only), so it is not live between chunks
+        if (s > 0) wgmma_fence_regs(hacc);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk) {
+          const uint64_t adesc = make_kc16_desc(a_base + (2 * s + kk) * Cfg::kABytesPerK, kTileM * 16, 128);
+          const uint64_t bdesc = make_kc16_desc(st + kk * Cfg::kW1Bytes, kFFChunk * 16, 128);
+          if (s == 0 && kk == 0) wgmma_m64n128k16_first(hacc, adesc, bdesc);
+          else wgmma_m64n128k16(hacc, adesc, bdesc, 1);
+        }
+        wgmma_commit();
+        wgmma_fence_regs(hacc);
+        wgmma_wait<1>();
+        if (s > 0) mbar_arrive(&empty[prev]);
+        prev = slot;
+        next_slot();
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(hacc);
+      mbar_arrive(&empty[prev]);
+      if (c + 1 == c_end) mbar_arrive(a_empty);   // the item's last MMAs on xb have completed
+
+      // ---- 2. bf16(relu(H + b1)) as A fragments: fragment (kk, i) holds hidden columns 16 kk + 8 (i >> 1) + 2q, +1
+      // of row row0 + 8 (i & 1), i.e. accumulator elements 8 kk + 2 i, + 1
+      uint32_t af[Cfg::kDownK][4];
+      const float* bc = s_b1 + (c - c_begin) * kFFChunk + 2 * q;
+#pragma unroll
+      for (int kk = 0; kk < Cfg::kDownK; ++kk)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float2 b = *reinterpret_cast<const float2*>(bc + 16 * kk + 8 * (i >> 1));
+          af[kk][i] = pack_bf16x2(fmaxf(hacc[8 * kk + 2 * i] + b.x, 0.f), fmaxf(hacc[8 * kk + 2 * i + 1] + b.y, 0.f));
+        }
+      if (hid) {
+        __nv_bfloat16* hb = hid + (size_t)tile * kTileM * ff + (size_t)row0 * 8 + 2 * q;
+#pragma unroll
+        for (int kk = 0; kk < Cfg::kDownK; ++kk)
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+            *reinterpret_cast<uint32_t*>(hb + ((size_t)(c * 16 + 2 * kk + (i >> 1)) * kTileM + 8 * (i & 1)) * 8) =
+                af[kk][i];
+      }
+
+      // ---- 3. acc += bf16(H) W2[c rows, :]
+#pragma unroll
+      for (int kk = 0; kk < Cfg::kDownK; ++kk) {
+        mbar_wait(&full[slot], phase);
+        const uint32_t st = smem_u32(stage_base + slot * Cfg::kStageBytes);
+        wgmma_fence_regs(acc[0]);
+        wgmma_fence_regs(acc[1]);
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+          wgmma_m64n144k16_rs(acc[j], af[kk], make_kc16_desc(st + j * kNC * 16, kDP * 16, 128),
+                              kFinish || c != c_begin || kk != 0);
+        wgmma_commit();
+        wgmma_fence_regs(acc[0]);
+        wgmma_fence_regs(acc[1]);
+        wgmma_wait<1>();
+        if (kk > 0) {
+          wgmma_fence_regs(af[kk - 1]);   // read by the group that just completed
+          mbar_arrive(&empty[prev]);
+        }
+        prev = slot;
+        next_slot();
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc[0]);
+      wgmma_fence_regs(acc[1]);
+      wgmma_fence_regs(af[Cfg::kDownK - 1]);
+      mbar_arrive(&empty[prev]);
+    }
+
+    if constexpr (kFinish) {
+      row_epilogue<kNC, 2, false>(acc, tile, row0, q, s_vec, epi);
+    } else {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+          for (int jj = 0; jj < kNC / 8; ++jj)
+            *reinterpret_cast<float2*>(part_frag(tile, h, j, jj)) =
+                make_float2(acc[j][jj * 4 + 2 * h], acc[j][jj * 4 + 2 * h + 1]);
     }
   }
 }
@@ -775,7 +1009,9 @@ cudaError_t kernels_init() {
   cudaError_t e;
   if ((e = gemm_init<kNC, 2, EPI_ROW, false>()) != cudaSuccess) return e;
   if ((e = gemm_init<kNC, 1, EPI_QKV, true>()) != cudaSuccess) return e;
-  if ((e = gemm_init<kFFChunk, 1, EPI_RELU, true>()) != cudaSuccess) return e;
+  for (auto fn : {ffn_gemm_kernel<false>, ffn_gemm_kernel<true>})
+    if ((e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, FfnCfg::kSmemBytes)) != cudaSuccess)
+      return e;
   e = cudaFuncSetAttribute(embed_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(band_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -801,7 +1037,7 @@ void launch_gemm_row(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int
   const int grid = ntiles < num_sms() ? ntiles : num_sms();
   const int smem = Cfg::smem_bytes(Cfg::stages(b_ksteps / Cfg::kSK));
   gemm_kernel<kNC, 2, EPI_ROW, false><<<grid, Cfg::kThreads, smem, st>>>(a_img, b_img, a_ksteps, b_ksteps, ntiles, 1,
-                                                                                    nullptr, 0, nullptr, epi);
+                                                                                    nullptr, 0, epi);
 }
 
 void launch_gemm_qkv(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int ntiles,
@@ -811,17 +1047,20 @@ void launch_gemm_qkv(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int
   const int grid = npairs < num_sms() ? npairs : num_sms();
   RowEpi none{};
   gemm_kernel<kNC, 1, EPI_QKV, true><<<grid, Cfg::kThreads, Cfg::kSmemBytes, st>>>(
-      a_img, b_img, kDP / 16, 2 * (kDP / 16), ntiles, kQKVN / kQKVGroup, qkv_img, kQKVN / 8, nullptr, none);
+      a_img, b_img, kDP / 16, 2 * (kDP / 16), ntiles, kQKVN / kQKVGroup, qkv_img, kQKVN / 8, none);
 }
 
-void launch_ffn_up(const __nv_bfloat16* a_img, const __nv_bfloat16* w1_img, const float* b1, int ff, int ntiles,
-                   __nv_bfloat16* hid_img, cudaStream_t st) {
-  using Cfg = GemmCfg<kFFChunk, 1, true>;
-  const int npairs = (ntiles + 1) / 2;
-  const int grid = npairs < num_sms() ? npairs : num_sms();
-  RowEpi none{};
-  gemm_kernel<kFFChunk, 1, EPI_RELU, true><<<grid, Cfg::kThreads, Cfg::kSmemBytes, st>>>(
-      a_img, w1_img, kDP / 16, kDP / 16, ntiles, ff / kFFChunk, hid_img, ff / 8, b1, none);
+void launch_ffn(bool finish, const __nv_bfloat16* xb_img, const __nv_bfloat16* w1_img, const float* b1,
+                const __nv_bfloat16* w2_img, int ff, int ntiles, float* part_img, __nv_bfloat16* hid_img,
+                const RowEpi& epi, cudaStream_t st) {
+  const int nch = ff / kFFChunk, half = (nch + 1) / 2;
+  const int grid = ntiles < num_sms() ? ntiles : num_sms();
+  if (finish)
+    ffn_gemm_kernel<true><<<grid, FfnCfg::kThreads, FfnCfg::kSmemBytes, st>>>(xb_img, w1_img, b1, w2_img, ff, half, nch,
+                                                                              ntiles, part_img, hid_img, epi);
+  else
+    ffn_gemm_kernel<false><<<grid, FfnCfg::kThreads, FfnCfg::kSmemBytes, st>>>(xb_img, w1_img, b1, w2_img, ff, 0, half,
+                                                                               ntiles, part_img, hid_img, epi);
 }
 
 // packed rows -> the float32 [B, R, L] rows they stand for (the strict-fp32 path reads float32 rows)

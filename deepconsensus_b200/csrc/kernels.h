@@ -13,7 +13,7 @@ size_t embed_smem_bytes(int R, int echunks, int table_elems);
 void launch_embed(const float* rows, const uint8_t* packed, const PackedLayout& pl, int R, int L, int Lw, int M, int ntiles, int echunks,
                   const EmbedCol* cols, const EmbedRow* rowmeta, const __nv_bfloat16* tables,
                   int table_elems, __nv_bfloat16* emb, int* status, cudaStream_t st);
-// D = A * B^T with the 288-wide row epilogue (condenser + pos-enc, attention out-proj, FFN down-projection).
+// D = A * B^T with the 288-wide row epilogue (condenser + pos-enc, attention out-proj).
 // b_ksteps == 2 * a_ksteps: b_img holds split-bf16 weights [W_hi; W_lo] along K (kernels.cu, gemm_kernel).
 void launch_gemm_row(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int a_ksteps, int b_ksteps, int ntiles,
                      const RowEpi& epi, cudaStream_t st);
@@ -21,10 +21,14 @@ void launch_gemm_row(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int
 // split-bf16 weights [72][kQKVGroup][8] (hi chunks, then lo chunks)
 void launch_gemm_qkv(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int ntiles,
                      __nv_bfloat16* qkv_img, cudaStream_t st);
-// FFN up-projection: hid = relu(A W1 + b1) as a bf16 operand image [tile][ff/8][128][8]; w1_img: ff / kFFChunk groups
-// of [36][kFFChunk][8]
-void launch_ffn_up(const __nv_bfloat16* a_img, const __nv_bfloat16* w1_img, const float* b1, int ff, int ntiles,
-                   __nv_bfloat16* hid_img, cudaStream_t st);
+// One half of the FFN relu(xb W1 + b1) W2 + b2 with the row epilogue `epi` (kernels.cu, ffn_gemm_kernel): the first
+// launch (finish false) takes the first ceil(n / 2) of the n = ff / kFFChunk hidden chunks and writes its partial sums
+// to part_img (fp32, the residual image's layout), the second (finish true) adds the other chunks to them and runs the
+// epilogue.  w1_img: ff / kFFChunk groups of [36][kFFChunk][8]; w2_img: [ff/8][288][8].  hid_img, when not null,
+// receives the bf16 hidden activation as an operand image [tile][ff/8][128][8].
+void launch_ffn(bool finish, const __nv_bfloat16* xb_img, const __nv_bfloat16* w1_img, const float* b1,
+                const __nv_bfloat16* w2_img, int ff, int ntiles, float* part_img, __nv_bfloat16* hid_img,
+                const RowEpi& epi, cudaStream_t st);
 void launch_unpack_rows(const uint8_t* packed, const PackedLayout& pl, int nwindows, float* rows, cudaStream_t st);
 void launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* att, int L, int Lw, int win, int nwindows,
                       cudaStream_t st);

@@ -6,9 +6,12 @@ Writes DIR/profile_gemms.json (and DIR/trace.json, the torch.profiler trace it w
   kernels  torch.profiler (CUDA activities) over K pipelined steps of the bench workload (P20, L120, 6 layers, batch
            1024, packed rows resident in HBM).  The row-epilogue GEMM is one kernel for three launches of a layer, so
            each launch is named by the kernel before it: the condenser follows the embedding, the out-projection the
-           attention, the FFN down-projection the FFN up-projection.
+           attention, the FFN down-projection the FFN up-projection.  Builds with the fused FFN launch it twice per
+           layer: ffn_first (the first half of the filter, partial sums out) and ffn_final (the rest, row epilogue).
   l2_read  for each GEMM, the bytes its CTAs read from L2 per launch (weights once per work item, activations,
            residual), computed from the shapes and the tiling, over its kernel time.
+  hbm      for each FFN launch, the activation bytes it reads and writes in HBM (the weights stay in L2), computed
+           from the image shapes, over its kernel time and against the H100 SXM data sheet's 3.35 TB/s.
   l2_ceiling  scripts/l2_stream.cu, compiled into a temporary directory: every SM streams the same L2-resident 1.18 MB
            weight image through the GEMM's 4-stage bulk-copy ring with consumers that only release the slots.
 The card's name, power limit and clocks are recorded beside the numbers.  DCB200_LIB selects another build of the
@@ -62,7 +65,24 @@ def l2_bytes(role, ntiles, ff, epad, tokens):
     return passes * (KDP * ff * 2) + ntiles * a_tile * ff + res
   if role == "condenser":
     return passes * (KDP * 2 * epad * 2) + ntiles * 2 * a_tile * epad
+  if role in ("ffn_first", "ffn_final"):    # one tile per work item; W1 and W2 rows of the launch's hidden chunks
+    nch = ff // 128
+    chunks = (nch + 1) // 2 if role == "ffn_first" else nch // 2
+    return ntiles * (chunks * 128 * KDP * 2 * 2 + a_tile * KDP) + (2 * res if role == "ffn_final" else 0)
   return None
+
+
+HBM_TBPS = 3.35    # H100 SXM data sheet
+
+
+def hbm_bytes(role, ntiles, ff):
+  """Activation bytes one FFN launch reads and writes in HBM: bf16 xb / hidden images, fp32 residual and partial-sum
+  images (the next layer's xb is counted for every layer)."""
+  xb = ntiles * TILE * KDP * 2
+  x = ntiles * TILE * KDP * 4
+  hid = ntiles * TILE * ff * 2
+  return {"ffn_up": xb + hid, "ffn_down": hid + x + x + xb,
+          "ffn_first": xb + x, "ffn_final": xb + x + x + x + xb}.get(role)
 
 
 def main():
@@ -128,6 +148,9 @@ def main():
   kernels = sorted((e for e in events if e.get("cat") == "kernel"), key=lambda e: e["ts"])
 
   def role_of(name, prev):
+    m = re.search(r"ffn_gemm_kernel<(true|false)>", name)
+    if m:
+      return "ffn_final" if m.group(1) == "true" else "ffn_first"
     m = re.search(r"gemm_kernel<(\d+), (\d+), (\d+), (true|false)>", name)
     if m:
       epi = int(m.group(3))
@@ -161,6 +184,11 @@ def main():
     if nb is not None:
       rec["l2_read_bytes_per_launch"] = nb
       rec["l2_read_tbps"] = nb / (float(np.median(us)) * 1e-6) / 1e12
+    hb = hbm_bytes(r, ntiles, p.filter_size)
+    if hb is not None:
+      rec["hbm_bytes_per_launch"] = hb
+      rec["hbm_tbps"] = hb / (float(np.median(us)) * 1e-6) / 1e12
+      rec["hbm_share_of_3_35_tbps"] = rec["hbm_tbps"] / HBM_TBPS
     out[r] = rec
   result.update(kernels=out, steps=args.steps, batch=B, ntiles=ntiles, tokens=args.tokens,
                 kernel_ms_per_step=total / 1e3 / args.steps, gpu_after=gpu_info())
