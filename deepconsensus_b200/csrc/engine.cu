@@ -94,8 +94,11 @@ struct Weights {
   } strict;
 };
 
-// Kernel classes of the forward's profile, in dcb_get_profile_kernels' order.
-enum ProfKind { kProfEmbed, kProfRowGemm, kProfQkv, kProfAttention, kProfFfn, kProfHead, kProfKinds };
+// Kernel classes of the forward's profile, in dcb_get_profile_kernels' order; kProfNone: counted, never timed.
+enum ProfKind { kProfEmbed, kProfRowGemm, kProfQkv, kProfAttention, kProfFfn, kProfHead, kProfKinds, kProfNone };
+
+// The events around one profiled region of launches.
+struct ProfRegion { cudaEvent_t start, end; ProfKind kind; };
 
 }  // namespace
 
@@ -122,8 +125,7 @@ struct dcb_engine {
     bool busy = false, used = false;
     int64_t ticket = -1;
     int launches = 0;
-    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events;  // around every launch when profiling
-    std::vector<ProfKind> prof_kind;                               // kernel class of each event pair
+    std::vector<ProfRegion> prof;   // when profiling: the first prof_used are this submission's regions
     size_t prof_used = 0;
   } slots[2];
   int64_t next_ticket = 0;
@@ -180,7 +182,7 @@ struct dcb_engine {
     std::vector<cudaEvent_t> events = {ev_eval0, ev_eval1};
     for (Slot& sl : slots) {
       events.insert(events.end(), {sl.rows_ready, sl.ev0, sl.ev1, sl.done});
-      for (auto& pr : sl.prof_events) events.insert(events.end(), {pr.first, pr.second});
+      for (const ProfRegion& r : sl.prof) events.insert(events.end(), {r.start, r.end});
       if (sl.h_status) cudaFreeHost(sl.h_status);
     }
     for (cudaEvent_t ev : events)
@@ -531,6 +533,212 @@ int upload_weights(dcb_engine* e, const Checkpoint& ck, Weights* w) {
   return DCB_OK;
 }
 
+// Every launch of one submission's forward goes through run(): it counts the launches and, when profiling is on and
+// `kind` is a kernel class, times them as one region of that class in the slot's events.
+struct LaunchRecorder {
+  dcb_engine* e;
+  dcb_engine::Slot& sl;
+  cudaStream_t st;
+  int count = 0;
+  template <typename F>
+  void run(ProfKind kind, int n_launches, F&& launch) {
+    count += n_launches;
+    const ProfRegion* r = e->profile && kind != kProfNone ? begin(kind) : nullptr;
+    launch();
+    if (r) cudaEventRecord(r->end, st);
+  }
+
+  // the slot's next region, its start recorded; null (untimed; the forward still succeeds) if its events fail
+  const ProfRegion* begin(ProfKind kind) {
+    if (sl.prof_used == sl.prof.size()) {
+      const bool clean = cudaPeekAtLastError() == cudaSuccess;
+      ProfRegion r{nullptr, nullptr, kind};
+      if (cudaEventCreate(&r.start) != cudaSuccess || cudaEventCreate(&r.end) != cudaSuccess) {
+        if (r.start) cudaEventDestroy(r.start);
+        if (clean) cudaGetLastError();   // only this failure is cleared, not an earlier launch's
+        return nullptr;
+      }
+      sl.prof.push_back(r);
+    }
+    ProfRegion& r = sl.prof[sl.prof_used++];
+    r.kind = kind;
+    cudaEventRecord(r.start, st);
+    return &r;
+  }
+};
+
+// The head of the chunk from window w0 on: final LayerNorm, fc1, quality settings and the submission's outputs (device
+// arrays; probs and logits nullable) from that window.  The chunk function sets the residual and the layout.
+HeadParams chunk_head(const dcb_engine* e, uint8_t* bases, uint8_t* quals, float* probs, float* logits, int w0) {
+  HeadParams hp{};
+  hp.ln_g = e->w.fln_g; hp.ln_b = e->w.fln_b; hp.wfc = e->w.wfc; hp.bfc = e->w.bfc;
+  hp.gw8 = e->w.head_gw8; hp.ab = e->w.head_ab;
+  const size_t t0 = (size_t)w0 * e->L;
+  hp.bases = bases + t0; hp.quals = quals + t0;
+  hp.probs = probs ? probs + t0 * kVocab : nullptr;
+  hp.logits = logits ? logits + t0 * kVocab : nullptr;
+  set_head_quality(hp, e->cfg);
+  return hp;
+}
+
+// One chunk of the strict-fp32 forward (strict_kernels.cu): rows [bw, R, L] -> outputs via hp.  Its launches are
+// counted, not profiled.
+void strict_forward_chunk(dcb_engine* e, LaunchRecorder& rec, const float* rows_chunk, int bw, HeadParams hp,
+                          int* d_status) {
+  const dcb_config& c = e->cfg;
+  dcb_engine::Strict& S = e->strict;
+  const Weights& W = e->w;
+  const int L = e->L, M = bw * L, ff = c.filter_size;
+  const cudaStream_t st = rec.st;
+  rec.run(kProfNone, 2, [&] {
+    launch_strict_embed(rows_chunk, e->R, L, e->E, bw, W.strict.embed, W.strict.tables, S.emb, d_status, st);
+    StrictEpi ep;
+    if (c.add_pos_encoding) { ep.pe = W.strict.pe; ep.pe_L = L; }
+    launch_strict_gemm(S.emb, W.strict.wc, S.x, M, kD, e->E, ep, st);                 // networks.py:509-516, :319-323
+  });
+  const float qscale = 1.0f / sqrtf((float)kDH);                                       // attention_layer.py:196-197
+  for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
+    const LayerDev& ld = W.layers[n_];
+    const float* yin = c.rezero ? S.x.p : S.y.p;   // each sub-layer's input: x, or LayerNorm(x) in y
+    rec.run(kProfNone, c.rezero ? 7 : 9, [&] {
+      if (!c.rezero) launch_strict_layernorm(S.x, S.y, M, ld.ln_g[0], ld.ln_b[0], st);
+      StrictEpi eq; eq.scale = qscale;
+      launch_strict_gemm(yin, ld.strict.wq, S.q, M, kD, kD, eq, st);
+      launch_strict_gemm(yin, ld.strict.wk, S.k, M, kD, kD, StrictEpi(), st);
+      launch_strict_gemm(yin, ld.strict.wv, S.v, M, kD, kD, StrictEpi(), st);
+      launch_strict_attention(S.q, S.k, S.v, S.att, bw, L, c.attn_win_size, st);
+      StrictEpi eo; eo.residual = S.x; eo.scale = c.rezero ? ld.strict.alpha[0] : 1.f;     // encoder_stack.py:88-92
+      launch_strict_gemm(S.att, ld.strict.wo, S.x, M, kD, kD, eo, st);
+      if (!c.rezero) launch_strict_layernorm(S.x, S.y, M, ld.ln_g[1], ld.ln_b[1], st);
+      StrictEpi e1; e1.bias = ld.b1; e1.relu = 1;                                      // ffn_layer.py:83-86
+      launch_strict_gemm(yin, ld.strict.w1, S.hid, M, ff, kD, e1, st);
+      StrictEpi e2; e2.bias = ld.strict.b2; e2.residual = S.x; e2.scale = c.rezero ? ld.strict.alpha[1] : 1.f;
+      launch_strict_gemm(S.hid, ld.strict.w2, S.x, M, kD, ff, e2, st);
+    });
+  }
+  hp.x = S.x; hp.M = M; hp.L = L; hp.Lw = L;
+  rec.run(kProfNone, 1, [&] { launch_strict_head(S.x, M, hp, st); });
+}
+
+// The row epilogue of the bf16 forward's residual GEMMs: x = [x_old +] product [+ bias] [+ positional encoding], and
+// xb = the input of sub-layer `sub` (0 attention, 1 FFN) of layer `layer`: LayerNorm(x) for pre-LN models, x for
+// ReZero, none after the last layer.
+RowEpi row_epi(const dcb_engine* e, bool has_xold, const float* bias, int layer, int sub, bool pos) {
+  const dcb_config& c = e->cfg;
+  RowEpi epi{};
+  epi.x = e->d_x;
+  epi.bias = bias;
+  if (pos && c.add_pos_encoding) { epi.pe = e->w.pe; epi.pe_img = e->w.pe_img; }
+  if (layer < c.num_hidden_layers) {
+    epi.xb = e->d_xb;
+    if (!c.rezero) { epi.ln_g = e->w.layers[layer].ln_g[sub]; epi.ln_b = e->w.layers[layer].ln_b[sub]; }
+  }
+  epi.has_xold = has_xold;
+  epi.L = e->Lw;
+  return epi;
+}
+
+// One bf16 operand image the debug capture keeps: the stage and DCB_DEBUG_* id it is read back by, the workspace image
+// it is copied from, and its width.
+struct DbgImage { int stage, which; const DevBuf<__nv_bfloat16>* src; int width; };
+
+// Every image the debug capture keeps, in the order d_dbg_op stores them (include/dcb200_debug.h documents the list).
+// Each is chunk_tiles tiles long; at each stage the capture copies the images the launches since the previous one wrote.
+std::vector<DbgImage> dbg_images(const dcb_engine* e) {
+  const int layers = e->cfg.num_hidden_layers, ff = e->cfg.filter_size;
+  std::vector<DbgImage> v = {{0, DCB_DEBUG_EMBED, &e->d_embqkv, e->Epad}, {0, DCB_DEBUG_XB, &e->d_xb, kDP}};
+  for (int n = 0; n < layers; ++n) {
+    v.insert(v.end(), {{1 + 2 * n, DCB_DEBUG_QKV, &e->d_embqkv, kQKVN}, {1 + 2 * n, DCB_DEBUG_ATT, &e->d_att, kDP},
+                       {1 + 2 * n, DCB_DEBUG_XB, &e->d_xb, kDP}, {2 + 2 * n, DCB_DEBUG_HID, &e->d_hid, ff}});
+    if (n + 1 < layers) v.push_back({2 + 2 * n, DCB_DEBUG_XB, &e->d_xb, kDP});
+  }
+  return v;
+}
+
+// Where d_dbg_op keeps image `which` of `stage`: its first column (per 128-token tile row) and its width.  False for a
+// pair that is not captured.
+bool dbg_operand_slot(const dcb_engine* e, int stage, int which, size_t* cols, int* width) {
+  *cols = 0;
+  for (const DbgImage& im : dbg_images(e)) {
+    if (im.stage == stage && im.which == which) { *width = im.width; return true; }
+    *cols += im.width;
+  }
+  return false;
+}
+
+// The last chunk's valid tokens of a captured image [tile][iw / K][128][K] (device) as token-major out [tokens][ow],
+// ow <= iw.
+template <int K, typename T>
+int read_capture(dcb_engine* e, const T* image, int iw, int ow, T* out, int64_t out_elems) {
+  const int Mlay = e->last_chunk_tokens;               // tokens in the layout
+  const int M = Mlay / e->Lw * e->L;                   // valid tokens
+  if (out_elems < (int64_t)M * ow) return fail(e, DCB_ERR_INVALID, "output too small: need %lld", (long long)M * ow);
+  CU(e, cudaSetDevice(e->cfg.device));
+  std::vector<T> img((size_t)(Mlay + kTileM - 1) / kTileM * kTileM * iw);
+  CU(e, cudaMemcpy(img.data(), image, img.size() * sizeof(T), cudaMemcpyDeviceToHost));
+  for (int t = 0; t < M; ++t) {
+    const int tl = t / e->L * e->Lw + t % e->L;        // position of valid token t in the layout
+    const int tile = tl / kTileM, r = tl % kTileM;
+    for (int col = 0; col < ow; ++col)
+      out[(size_t)t * ow + col] = img[(((size_t)tile * (iw / K) + col / K) * kTileM + r) * K + col % K];
+  }
+  return DCB_OK;
+}
+
+// One chunk of the bf16 forward (kernels.cu): windows from float32 rows [bw, R, L] or packed rows (the other null) ->
+// outputs via hp.  With debug capture on, each stage's residual and operand images are copied aside.
+void bf16_forward_chunk(dcb_engine* e, LaunchRecorder& rec, const float* rows_chunk, const uint8_t* packed_chunk,
+                        int bw, HeadParams hp, int* d_status) {
+  const dcb_config& c = e->cfg;
+  const Weights& W = e->w;
+  const int L = e->L, Lw = e->Lw, M = bw * Lw;   // M: tokens in the (possibly window-aligned) layout
+  const int T = (M + kTileM - 1) / kTileM;
+  const cudaStream_t st = rec.st;
+  int stage = 0;
+  auto snap = [&]() {
+    if (e->debug) {   // stream-ordered copies only
+      const size_t ximg = x_image_elems(), cw = (size_t)e->chunk_tiles * kTileM;
+      cudaMemcpyAsync(e->d_dbg + (size_t)stage * e->chunk_tiles * ximg, e->d_x, T * ximg * sizeof(float), cudaMemcpyDeviceToDevice, st);
+      size_t cols = 0;
+      for (const DbgImage& im : dbg_images(e)) {
+        if (im.stage == stage)
+          cudaMemcpyAsync(e->d_dbg_op + cols * cw, im.src->p, (size_t)T * kTileM * im.width * sizeof(__nv_bfloat16),
+                          cudaMemcpyDeviceToDevice, st);
+        cols += im.width;
+      }
+    }
+    ++stage;
+  };
+  rec.run(kProfEmbed, 1, [&] {
+    launch_embed(rows_chunk, packed_chunk, e->pl, e->R, L, Lw, M, T, e->echunks, W.cols, W.rowmeta, W.tables,
+                 e->table_elems, e->d_embqkv, d_status, st);
+  });
+  rec.run(kProfRowGemm, 1, [&] {   // condenser + positional encoding; xb = layer 0's attention input
+    launch_gemm_row(e->d_embqkv, W.wc, e->Epad / 16, 2 * (e->Epad / 16), T, row_epi(e, false, nullptr, 0, 0, true), st);
+  });
+  snap();
+  for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
+    const LayerDev& ld = W.layers[n_];
+    rec.run(kProfQkv, 1, [&] { launch_gemm_qkv(e->d_xb, ld.wqkv, T, e->d_embqkv, st); });
+    rec.run(kProfAttention, 1, [&] { launch_attention(e->d_embqkv, e->d_att, L, Lw, c.attn_win_size, bw, st); });
+    rec.run(kProfRowGemm, 1, [&] {   // attention out-projection + residual; xb = the FFN sub-layer's input
+      launch_gemm_row(e->d_att, ld.wo, kDP / 16, 2 * (kDP / 16), T, row_epi(e, true, nullptr, n_, 1, false), st);
+    });
+    snap();
+    rec.run(kProfFfn, 2, [&] {   // relu(xb W1 + b1) W2 + b2 + residual, half of the filter per launch; xb = next layer's
+      const RowEpi epi = row_epi(e, true, ld.b2, n_ + 1, 0, false);
+      __nv_bfloat16* hid = e->debug ? e->d_hid.p : nullptr;
+      launch_ffn(false, e->d_xb, ld.w1, ld.b1, ld.w2, c.filter_size, T, e->d_part, hid, epi, st);
+      launch_ffn(true, e->d_xb, ld.w1, ld.b1, ld.w2, c.filter_size, T, e->d_part, hid, epi, st);
+    });
+    if (e->profile) e->prof_ffn_tokens += (long long)bw * L;   // valid tokens (layout padding is not algorithmic work)
+    snap();
+  }
+  hp.x = e->d_x; hp.M = M; hp.L = L; hp.Lw = Lw;
+  rec.run(kProfHead, 1, [&] { launch_head(hp, T, st); });
+  e->last_chunk_tokens = M;
+}
+
 }  // namespace
 
 extern "C" {
@@ -572,12 +780,10 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
   e->L = cfg->max_length;
   e->Lw = e->L;
   bool align = true;
-  int ct = cfg->chunk_tiles;
 #ifdef DCB_DEV_SWITCHES
-  // Developer build only (libdcb200_dev.so, csrc/build.sh): environment switches that select the alternative token
-  // layout and chunking.  The product library ignores the environment.
+  // Developer build only (libdcb200_dev.so, csrc/build.sh): an environment switch that selects the alternative token
+  // layout.  The product library ignores the environment.
   if (const char* env = getenv("DCB_ALIGN")) align = atoi(env) != 0;
-  if (const char* env = getenv("DCB_CHUNK_TILES")) ct = atoi(env);
 #endif
   // window-aligned tiling: one window per 128-token tile when it fits (the positional table is then read in residual-
   // image order); otherwise windows are packed back to back
@@ -612,7 +818,7 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
   }
   e->Epad = (e->E + 15) / 16 * 16;
   e->echunks = e->Epad / 8;
-  if (ct <= 0) ct = 8 * e->num_sms;   // measured: larger chunks win (kernels are not DRAM-bound)
+  const int ct = cfg->chunk_tiles > 0 ? cfg->chunk_tiles : 8 * e->num_sms;   // measured: larger chunks win (kernels are not DRAM-bound)
   const int max_tiles = (int)(((int64_t)cfg->max_batch * e->Lw + kTileM - 1) / kTileM);
   e->chunk_windows = std::max(1, std::min(cfg->max_batch, ct * kTileM / e->Lw));
   e->chunk_tiles = std::min(max_tiles, (e->chunk_windows * e->Lw + kTileM - 1) / kTileM);
@@ -681,90 +887,17 @@ int dcb_load_weights(dcb_engine* e, const dcb_tensor* tensors, int32_t n) {
   return DCB_OK;
 }
 
-// One chunk of the strict-fp32 forward (strict_kernels.cu): rows [bw, R, L] -> outputs via hp.  Returns launches.
-static int strict_forward_chunk(dcb_engine* e, const float* rows_chunk, int bw, const HeadParams& hp, int* d_status,
-                                cudaStream_t st) {
-  const dcb_config& c = e->cfg;
-  dcb_engine::Strict& S = e->strict;
-  const Weights& W = e->w;
-  const int L = e->L, M = bw * L, ff = c.filter_size;
-  int launches = 0;
-  launch_strict_embed(rows_chunk, e->R, L, e->E, bw, W.strict.embed, W.strict.tables, S.emb, d_status, st); ++launches;
-  {
-    StrictEpi ep;
-    if (c.add_pos_encoding) { ep.pe = W.strict.pe; ep.pe_L = L; }
-    launch_strict_gemm(S.emb, W.strict.wc, S.x, M, kD, e->E, ep, st); ++launches;            // networks.py:509-516, :319-323
-  }
-  const float qscale = 1.0f / sqrtf((float)kDH);                                       // attention_layer.py:196-197
-  for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
-    const LayerDev& ld = W.layers[n_];
-    const float* yin = S.x;
-    if (!c.rezero) { launch_strict_layernorm(S.x, S.y, M, ld.ln_g[0], ld.ln_b[0], st); ++launches; yin = S.y; }
-    StrictEpi eq; eq.scale = qscale;
-    launch_strict_gemm(yin, ld.strict.wq, S.q, M, kD, kD, eq, st);
-    launch_strict_gemm(yin, ld.strict.wk, S.k, M, kD, kD, StrictEpi(), st);
-    launch_strict_gemm(yin, ld.strict.wv, S.v, M, kD, kD, StrictEpi(), st);
-    launch_strict_attention(S.q, S.k, S.v, S.att, bw, L, c.attn_win_size, st);
-    StrictEpi eo; eo.residual = S.x; eo.scale = c.rezero ? ld.strict.alpha[0] : 1.f;         // encoder_stack.py:88-92
-    launch_strict_gemm(S.att, ld.strict.wo, S.x, M, kD, kD, eo, st);
-    launches += 5;
-    yin = S.x;
-    if (!c.rezero) { launch_strict_layernorm(S.x, S.y, M, ld.ln_g[1], ld.ln_b[1], st); ++launches; yin = S.y; }
-    StrictEpi e1; e1.bias = ld.b1; e1.relu = 1;                                        // ffn_layer.py:83-86
-    launch_strict_gemm(yin, ld.strict.w1, S.hid, M, ff, kD, e1, st);
-    StrictEpi e2; e2.bias = ld.strict.b2; e2.residual = S.x; e2.scale = c.rezero ? ld.strict.alpha[1] : 1.f;
-    launch_strict_gemm(S.hid, ld.strict.w2, S.x, M, kD, ff, e2, st);
-    launches += 2;
-  }
-  HeadParams h = hp;
-  h.x = S.x; h.M = M; h.L = L; h.Lw = L;
-  launch_strict_head(S.x, M, h, st); ++launches;
-  return launches;
-}
-
-// Where the debug capture keeps bf16 operand image `which` (DCB_DEBUG_*) of stage `stage`: element offset into d_dbg_op
-// per tile row of 128 tokens and the image width.  Per stage the images are stored back to back, each chunk_tiles
-// tiles long.  Returns false for a pair that is not captured.
-//   stage 0     : EMBED (Epad), XB (layer 0's q/k/v operand)
-//   stage 1 + 2n: QKV (864), ATT (288), XB (the FFN's operand)
-//   stage 2 + 2n: HID (ff), XB (layer n + 1's q/k/v operand; not after the last layer)
-static bool dbg_operand_slot(const dcb_engine* e, int stage, int which, size_t* off_cols, int* width) {
-  const int layers = e->cfg.num_hidden_layers, ff = e->cfg.filter_size;
-  if (stage < 0 || stage > 2 * layers) return false;
-  size_t cols = 0;
-  for (int s = 0; s < stage; ++s) cols += s == 0 ? e->Epad + kDP : (s & 1) ? kQKVN + 2 * kDP : ff + kDP;
-  int w = -1;
-  if (stage == 0) {
-    if (which == DCB_DEBUG_EMBED) w = e->Epad;
-    else if (which == DCB_DEBUG_XB) { cols += e->Epad; w = kDP; }
-  } else if (stage & 1) {
-    if (which == DCB_DEBUG_QKV) w = kQKVN;
-    else if (which == DCB_DEBUG_ATT) { cols += kQKVN; w = kDP; }
-    else if (which == DCB_DEBUG_XB) { cols += kQKVN + kDP; w = kDP; }
-  } else {
-    if (which == DCB_DEBUG_HID) w = ff;
-    else if (which == DCB_DEBUG_XB && stage < 2 * layers) { cols += ff; w = kDP; }
-  }
-  if (w < 0) return false;
-  *off_cols = cols;
-  *width = w;
-  return true;
-}
-
 int dcb_set_debug(dcb_engine* e, int32_t enabled) {
   if (!e) return DCB_ERR_INVALID;
   e->debug = enabled != 0;
   if (e->debug && !e->d_dbg) {
     CU(e, cudaSetDevice(e->cfg.device));
     const size_t stages = 1 + 2 * (size_t)e->cfg.num_hidden_layers;
-    int rc = alloc(e, e->d_dbg, stages * e->chunk_tiles * x_image_elems());
-    if (rc) return rc;
     size_t cols = 0;
-    int w = 0;
-    dbg_operand_slot(e, (int)stages - 1, DCB_DEBUG_HID, &cols, &w);   // the last stage holds HID only
-    rc = alloc(e, e->d_dbg_op, (cols + w) * e->chunk_tiles * kTileM);
-    if (rc) return rc;
-    rc = alloc(e, e->d_hid, e->chunk_tiles * act_image_elems(e->cfg.filter_size));
+    for (const DbgImage& im : dbg_images(e)) cols += im.width;
+    int rc = alloc(e, e->d_dbg, stages * e->chunk_tiles * x_image_elems());
+    if (!rc) rc = alloc(e, e->d_dbg_op, cols * e->chunk_tiles * kTileM);
+    if (!rc) rc = alloc(e, e->d_hid, e->chunk_tiles * act_image_elems(e->cfg.filter_size));
     if (rc) return rc;
   }
   return DCB_OK;
@@ -782,7 +915,6 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
   if (sl.busy) return fail(e, DCB_ERR_STATE, "two submissions in flight: dcb_wait(ticket %lld) first",
                            (long long)std::min(e->slots[0].ticket, e->slots[1].ticket));
   if (batch < 0 || batch > e->cfg.max_batch) return fail(e, DCB_ERR_INVALID, "batch %d outside [0, max_batch=%d]", batch, e->cfg.max_batch);
-  sl.launches = 0;
   sl.ticket = e->next_ticket;
   if (batch == 0) { sl.busy = true; sl.used = false; *ticket_out = e->next_ticket++; return DCB_OK; }
   if ((!rows && !packed) || !bases_out || !quals_out) return fail(e, DCB_ERR_INVALID, "null rows / output buffer");
@@ -825,133 +957,25 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
     CU(e, cudaEventRecord(sl.rows_ready, e->copy_stream));
     CU(e, cudaStreamWaitEvent(st, sl.rows_ready, 0));
   }
+  LaunchRecorder rec{e, sl, st};
   const uint8_t* packed_base = packed ? (rows_dev ? packed : sl.d_packed) : nullptr;
   // the default path's embedding kernel reads packed rows directly; the strict path gets the float32 rows they stand for
-  if (packed_base && strict) launch_unpack_rows(packed_base, e->pl, batch, sl.d_rows, st);
+  if (packed_base && strict) rec.run(kProfNone, 1, [&] { launch_unpack_rows(packed_base, e->pl, batch, sl.d_rows, st); });
   const float* rows_base = packed ? sl.d_rows : (rows_dev ? rows : sl.d_rows);
   CU(e, cudaMemsetAsync(sl.d_status, 0, sizeof(int), st));
   CU(e, cudaEventRecord(sl.ev0, st));
-  int launches = (packed_base && strict) ? 1 : 0;
-  const size_t ximg = x_image_elems();
-  bool prof_err = false;
-  auto pbegin = [&](ProfKind kind) {
-    if (!e->profile) return;
-    if (sl.prof_used == sl.prof_events.size()) {
-      cudaEvent_t a, b;
-      if (cudaEventCreate(&a) != cudaSuccess || cudaEventCreate(&b) != cudaSuccess) { prof_err = true; return; }
-      sl.prof_events.emplace_back(a, b);
-    }
-    if (sl.prof_kind.size() <= sl.prof_used) sl.prof_kind.resize(sl.prof_used + 1);
-    sl.prof_kind[sl.prof_used] = kind;
-    cudaEventRecord(sl.prof_events[sl.prof_used].first, st);
-  };
-  auto pend = [&]() {
-    if (!e->profile || prof_err) return;
-    cudaEventRecord(sl.prof_events[sl.prof_used].second, st);
-    ++sl.prof_used;
-  };
-  auto make_head_at = [&](int w0) {
-    HeadParams hp{};
-    hp.x = e->d_x; hp.ln_g = e->w.fln_g; hp.ln_b = e->w.fln_b; hp.wfc = e->w.wfc; hp.bfc = e->w.bfc;
-    hp.gw8 = e->w.head_gw8; hp.ab = e->w.head_ab;
-    const size_t t0 = (size_t)w0 * L;
-    hp.bases = (out_dev ? bases_out : sl.d_bases) + t0;
-    hp.quals = (out_dev ? quals_out : sl.d_quals) + t0;
-    hp.probs = probs_out ? ((out_dev ? probs_out : sl.d_probs) + t0 * kVocab) : nullptr;
-    hp.logits = logits_out ? ((out_dev ? logits_out : sl.d_logits) + t0 * kVocab) : nullptr;
-    set_head_quality(hp, c);
-    return hp;
-  };
-  if (strict) {
-    for (int w0 = 0; w0 < batch; w0 += e->strict.chunk_windows) {
-      const int bw = std::min(e->strict.chunk_windows, batch - w0);
-      launches += strict_forward_chunk(e, rows_base + (size_t)w0 * R * L, bw, make_head_at(w0), sl.d_status, st);
-    }
-  }
-  for (int w0 = 0; !strict && w0 < batch; w0 += e->chunk_windows) {
-    const int bw = std::min(e->chunk_windows, batch - w0);
-    const int Lw = e->Lw;
-    const int M = bw * Lw;          // tokens in the (possibly window-aligned) layout
-    const int T = (M + kTileM - 1) / kTileM;
+  uint8_t* bases = out_dev ? bases_out : sl.d_bases.p;
+  uint8_t* quals = out_dev ? quals_out : sl.d_quals.p;
+  float* probs = probs_out ? (out_dev ? probs_out : sl.d_probs.p) : nullptr;
+  float* logits = logits_out ? (out_dev ? logits_out : sl.d_logits.p) : nullptr;
+  const int chunk_windows = strict ? e->strict.chunk_windows : e->chunk_windows;
+  for (int w0 = 0; w0 < batch; w0 += chunk_windows) {
+    const int bw = std::min(chunk_windows, batch - w0);
+    const HeadParams hp = chunk_head(e, bases, quals, probs, logits, w0);
     const float* rows_chunk = rows_base + (size_t)w0 * R * L;
-    int stage = 0;
-    auto snap = [&]() {
-      if (e->debug) {
-        cudaMemcpyAsync(e->d_dbg + (size_t)stage * e->chunk_tiles * ximg, e->d_x, (size_t)T * ximg * sizeof(float), cudaMemcpyDeviceToDevice, st);
-        // the bf16 operand images the launches since the previous snapshot wrote (stream-ordered copies only)
-        const __nv_bfloat16* src[5] = {e->d_embqkv, e->d_xb, e->d_embqkv, e->d_att, e->d_hid};   // DCB_DEBUG_* order
-        for (int which = 0; which < 5; ++which) {
-          size_t cols = 0;
-          int w = 0;
-          if (dbg_operand_slot(e, stage, which, &cols, &w))
-            cudaMemcpyAsync(e->d_dbg_op + cols * e->chunk_tiles * kTileM, src[which], (size_t)T * kTileM * w * sizeof(__nv_bfloat16),
-                            cudaMemcpyDeviceToDevice, st);
-        }
-      }
-      ++stage;
-    };
-    auto make_head = [&]() {
-      HeadParams hp = make_head_at(w0);
-      hp.M = M; hp.L = L; hp.Lw = Lw;
-      return hp;
-    };
-    {
-      RowEpi epi{};
-      epi.x = e->d_x; epi.xb = e->d_xb; epi.bias = nullptr;
-      epi.pe = c.add_pos_encoding ? e->w.pe.p : nullptr;
-      epi.pe_img = c.add_pos_encoding ? e->w.pe_img.p : nullptr;
-      epi.ln_g = c.rezero ? nullptr : e->w.layers[0].ln_g[0].p;
-      epi.ln_b = c.rezero ? nullptr : e->w.layers[0].ln_b[0].p;
-      epi.has_xold = 0; epi.L = Lw;
-      pbegin(kProfEmbed);
-      launch_embed(packed_base ? nullptr : rows_chunk, packed_base ? packed_base + (size_t)w0 * e->pl.stride : nullptr, e->pl,
-                   R, L, Lw, M, T, e->echunks, e->w.cols, e->w.rowmeta, e->w.tables, e->table_elems, e->d_embqkv, sl.d_status, st);
-      pend();
-      pbegin(kProfRowGemm);
-      launch_gemm_row(e->d_embqkv, e->w.wc, e->Epad / 16, 2 * (e->Epad / 16), T, epi, st);
-      pend();
-      launches += 2;
-      snap();
-    }
-    for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
-      const LayerDev& ld = e->w.layers[n_];
-      const bool last = n_ + 1 == c.num_hidden_layers;
-      pbegin(kProfQkv);
-      launch_gemm_qkv(e->d_xb, ld.wqkv, T, e->d_embqkv, st);
-      pend();
-      pbegin(kProfAttention);
-      launch_attention(e->d_embqkv, e->d_att, L, Lw, c.attn_win_size, bw, st);
-      pend();
-      // attention out-projection + residual; xb = the FFN sub-layer's input (pre-LayerNorm or identity)
-      RowEpi ea{};
-      ea.x = e->d_x; ea.xb = e->d_xb; ea.bias = nullptr; ea.pe = nullptr;
-      ea.ln_g = c.rezero ? nullptr : ld.ln_g[1].p;
-      ea.ln_b = c.rezero ? nullptr : ld.ln_b[1].p;
-      ea.has_xold = 1; ea.L = Lw;
-      pbegin(kProfRowGemm);
-      launch_gemm_row(e->d_att, ld.wo, kDP / 16, 2 * (kDP / 16), T, ea, st);
-      pend();
-      snap();
-      // FFN: relu(xb W1 + b1) W2 + b2 + residual, half of the filter per launch; xb = the next layer's input
-      RowEpi ef{};
-      ef.x = e->d_x; ef.xb = last ? nullptr : e->d_xb.p; ef.bias = ld.b2; ef.pe = nullptr;
-      ef.ln_g = (c.rezero || last) ? nullptr : e->w.layers[n_ + 1].ln_g[0].p;
-      ef.ln_b = (c.rezero || last) ? nullptr : e->w.layers[n_ + 1].ln_b[0].p;
-      ef.has_xold = 1; ef.L = Lw;
-      pbegin(kProfFfn);
-      __nv_bfloat16* hid = e->debug ? e->d_hid.p : nullptr;
-      launch_ffn(false, e->d_xb, ld.w1, ld.b1, ld.w2, c.filter_size, T, e->d_part, hid, ef, st);
-      launch_ffn(true, e->d_xb, ld.w1, ld.b1, ld.w2, c.filter_size, T, e->d_part, hid, ef, st);
-      pend();
-      if (e->profile) e->prof_ffn_tokens += (long long)bw * L;   // valid tokens (layout padding is not algorithmic work)
-      snap();
-      launches += 5;
-    }
-    pbegin(kProfHead);
-    launch_head(make_head(), T, st);
-    pend();
-    ++launches;
-    e->last_chunk_tokens = M;
+    if (strict) strict_forward_chunk(e, rec, rows_chunk, bw, hp, sl.d_status);
+    else if (packed_base) bf16_forward_chunk(e, rec, nullptr, packed_base + (size_t)w0 * e->pl.stride, bw, hp, sl.d_status);
+    else bf16_forward_chunk(e, rec, rows_chunk, nullptr, bw, hp, sl.d_status);
   }
   CU(e, cudaEventRecord(sl.ev1, st));
   // results and status go back on their own stream: the compute stream is free for the next submission's kernels
@@ -967,7 +991,7 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
   CU(e, cudaMemcpyAsync(sl.h_status, sl.d_status, sizeof(int), cudaMemcpyDeviceToHost, os));
   CU(e, cudaEventRecord(sl.done, os));
   CU(e, cudaGetLastError());
-  sl.launches = launches;
+  sl.launches = rec.count;
   sl.busy = true;
   sl.used = true;
   *ticket_out = e->next_ticket++;
@@ -1057,16 +1081,14 @@ int dcb_wait(dcb_engine* e, int64_t ticket) {
   CU(e, cudaEventElapsedTime(&e->last_ms, sl.ev0, sl.ev1));
   e->last_launches = sl.launches;
   const int status = *sl.h_status;
-  {
-    for (size_t i = 0; i < sl.prof_used; ++i) {
-      float ms = 0.f;
-      CU(e, cudaEventElapsedTime(&ms, sl.prof_events[i].first, sl.prof_events[i].second));
-      const ProfKind kind = sl.prof_kind[i];
-      e->prof_ms[kind] += ms;
-      ++e->prof_n[kind];
-    }
-    sl.prof_used = 0;
+  for (size_t i = 0; i < sl.prof_used; ++i) {
+    const ProfRegion& r = sl.prof[i];
+    float ms = 0.f;
+    CU(e, cudaEventElapsedTime(&ms, r.start, r.end));
+    e->prof_ms[r.kind] += ms;
+    ++e->prof_n[r.kind];
   }
+  sl.prof_used = 0;
   if (status & 1) return fail(e, DCB_ERR_INPUT_RANGE, "embedding id out of range in the input rows (clamped)");
   return DCB_OK;
 }
@@ -1119,20 +1141,7 @@ int dcb_debug_residual(dcb_engine* e, int32_t stage, float* out, int64_t out_ele
   if (!e->debug || !e->d_dbg) return fail(e, DCB_ERR_STATE, "debug capture not enabled");
   const int stages = 1 + 2 * e->cfg.num_hidden_layers;
   if (stage < 0 || stage >= stages) return fail(e, DCB_ERR_INVALID, "stage %d outside [0,%d)", stage, stages);
-  const int Mlay = e->last_chunk_tokens;               // tokens in the layout
-  const int M = Mlay / e->Lw * e->L;                   // valid tokens
-  if (out_elems < (int64_t)M * kD) return fail(e, DCB_ERR_INVALID, "output too small: need %lld", (long long)M * kD);
-  CU(e, cudaSetDevice(e->cfg.device));
-  const int T = (Mlay + kTileM - 1) / kTileM;
-  std::vector<float> img((size_t)T * x_image_elems());
-  CU(e, cudaMemcpy(img.data(), e->d_dbg + (size_t)stage * e->chunk_tiles * x_image_elems(), img.size() * sizeof(float), cudaMemcpyDeviceToHost));
-  for (int t = 0; t < M; ++t) {
-    const int tl = t / e->L * e->Lw + t % e->L;        // position of valid token t in the layout
-    const int tile = tl / kTileM, r = tl % kTileM;
-    for (int col = 0; col < kD; ++col)
-      out[(size_t)t * kD + col] = img[(((size_t)tile * kXChunks + col / 4) * kTileM + r) * 4 + col % 4];
-  }
-  return DCB_OK;
+  return read_capture<4>(e, e->d_dbg + (size_t)stage * e->chunk_tiles * x_image_elems(), kDP, kD, out, out_elems);
 }
 
 int dcb_debug_operand(dcb_engine* e, int32_t stage, int32_t which, uint16_t* out, int64_t out_elems) {
@@ -1142,21 +1151,8 @@ int dcb_debug_operand(dcb_engine* e, int32_t stage, int32_t which, uint16_t* out
   int w = 0;
   if (!dbg_operand_slot(e, stage, which, &cols, &w))
     return fail(e, DCB_ERR_INVALID, "operand %d is not captured at stage %d", which, stage);
-  const int Mlay = e->last_chunk_tokens;               // tokens in the layout
-  const int M = Mlay / e->Lw * e->L;                   // valid tokens
-  if (out_elems < (int64_t)M * w) return fail(e, DCB_ERR_INVALID, "output too small: need %lld", (long long)M * w);
-  CU(e, cudaSetDevice(e->cfg.device));
-  const int T = (Mlay + kTileM - 1) / kTileM;
-  std::vector<uint16_t> img((size_t)T * kTileM * w);
-  CU(e, cudaMemcpy(img.data(), e->d_dbg_op + cols * e->chunk_tiles * kTileM, img.size() * sizeof(uint16_t), cudaMemcpyDeviceToHost));
-  const int chunks = w / 8;
-  for (int t = 0; t < M; ++t) {
-    const int tl = t / e->L * e->Lw + t % e->L;        // position of valid token t in the layout
-    const int tile = tl / kTileM, r = tl % kTileM;
-    for (int col = 0; col < w; ++col)
-      out[(size_t)t * w + col] = img[(((size_t)tile * chunks + col / 8) * kTileM + r) * 8 + col % 8];
-  }
-  return DCB_OK;
+  const __nv_bfloat16* img = e->d_dbg_op + cols * e->chunk_tiles * kTileM;
+  return read_capture<8>(e, reinterpret_cast<const uint16_t*>(img), w, w, out, out_elems);
 }
 
 // read z is the windows [zmw_start[z], zmw_start[z + 1]) of n_windows

@@ -114,8 +114,8 @@ _dev_lib = None
 
 
 def load_dev_library() -> ctypes.CDLL:
-  """libdcb200_dev.so: the same sources built with -DDCB_DEV_SWITCHES, where DCB_* environment variables select the
-  alternative token layout and chunking (tests and scripts only; pass as B200Model(..., library=...))."""
+  """libdcb200_dev.so: the same sources built with -DDCB_DEV_SWITCHES, where DCB_ALIGN=0 selects the alternative
+  token layout (tests and scripts only; pass as B200Model(..., library=...))."""
   global _dev_lib
   if _dev_lib is None:
     _dev_lib = _load(os.path.join(os.path.dirname(_LIB_PATH), "libdcb200_dev.so"))
@@ -768,6 +768,17 @@ class B200Model:
     out = np.empty((tokens, width), np.uint16)
     self._check(self._lib.dcb_debug_operand(self._handle, stage, DEBUG_OPERANDS[which], _ptr(out), out.size))
     return out
+
+  def debug_capture(self, tokens: int) -> Dict[str, object]:
+    """Everything the debug capture kept of the last chunk's `tokens` valid tokens, by stage (include/dcb200_debug.h):
+    emb; x, the residual of every stage; xb, the q/k/v or FFN operand by stage; and per layer qkv, att and hid."""
+    nl = int(self.params.num_hidden_layers)
+    return dict(emb=self.debug_operand(0, "embed", tokens),
+                x=[self.debug_residual(s, tokens) for s in range(1 + 2 * nl)],
+                xb={s: self.debug_operand(s, "xb", tokens) for s in range(2 * nl)},
+                qkv=[self.debug_operand(1 + 2 * n, "qkv", tokens) for n in range(nl)],
+                att=[self.debug_operand(1 + 2 * n, "att", tokens) for n in range(nl)],
+                hid=[self.debug_operand(2 + 2 * n, "hid", tokens) for n in range(nl)])
 
   def debug_head_epilogue(self, logits: np.ndarray) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
     """dcb_debug_head_epilogue: the head's per-token epilogue (softmax .. ASCII, with this engine's calibration and

@@ -35,17 +35,11 @@ def layout(request, golden_dir):
 def _check_stages(engine_mod, name, p, w, rows):
   """One forward with debug capture; every stage against its reference fed the device's own input to it."""
   B = rows.shape[0]
-  M, nl = B * int(p.max_length), int(p.num_hidden_layers)
   model = engine_mod.B200Model(p, w, max_batch=B)
   model.set_debug(True)
   out = model.forward(rows, want_logits=True)
-  dev = dict(emb=model.debug_operand(0, "embed", M),
-             x=[model.debug_residual(s, M) for s in range(1 + 2 * nl)],
-             xb={s: model.debug_operand(s, "xb", M) for s in range(2 * nl)},
-             qkv=[model.debug_operand(1 + 2 * n, "qkv", M) for n in range(nl)],
-             att=[model.debug_operand(1 + 2 * n, "att", M) for n in range(nl)],
-             hid=[model.debug_operand(2 + 2 * n, "hid", M) for n in range(nl)],
-             logits=out["logits"].reshape(-1, 5))
+  dev = model.debug_capture(B * int(p.max_length))
+  dev["logits"] = out["logits"].reshape(-1, 5)
   model.close()
   worst = stages.check_forward(stages.prepare(p, w), rows, dev)
   print("%-26s worst err/bound: %s" % (name, "  ".join("%s %.3g" % kv for kv in worst.items())))

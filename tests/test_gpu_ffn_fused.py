@@ -33,8 +33,8 @@ def engine_mod():
   return engine
 
 
-def _forward(engine_mod, cfg, p, w, rows, debug=False, library=None):
-  model = engine_mod.B200Model(p, w, max_batch=cfg["windows"], library=library)
+def _forward(engine_mod, cfg, p, w, rows, debug=False, chunk_tiles=0):
+  model = engine_mod.B200Model(p, w, max_batch=cfg["windows"], chunk_tiles=chunk_tiles)
   if debug:
     model.set_debug(True)
   out = model.forward(rows, want_logits=True)
@@ -66,13 +66,12 @@ def test_debug_capture_changes_nothing(engine_mod, golden, name):
     assert np.array_equal(plain[k], dbg[k]), (name, k)
 
 
-def test_one_tile_chunks(engine_mod, golden, monkeypatch):
-  """DCB_CHUNK_TILES=1 (developer library): every window is a chunk of its own, so each FFN launch has one tile."""
+def test_one_tile_chunks(engine_mod, golden):
+  """chunk_tiles=1: every window is a chunk of its own, so each FFN launch has one tile."""
   mk, cfgs, g = golden
   cfg = cfgs["ff640"]
   p, w, rows = mk.make(cfg)
-  monkeypatch.setenv("DCB_CHUNK_TILES", "1")
-  out, launches = _forward(engine_mod, cfg, p, w, rows, library=engine_mod.load_dev_library())
+  out, launches = _forward(engine_mod, cfg, p, w, rows, chunk_tiles=1)
   assert launches == cfg["windows"] * (3 + 5 * p.num_hidden_layers)
   for k in ("bases", "quals", "logits"):
     assert np.array_equal(out[k], g["ff640/%s" % k]), k

@@ -542,40 +542,34 @@ def test_failed_weight_load_keeps_the_previous_weights(engine_mod, monkeypatch):
   model.close()
 
 
-def test_unfused_fallback_paths_agree_with_fused(engine_mod):
-  """DCB_ALIGN / DCB_CHUNK_TILES select alternative token layouts and chunkings of the same math.  They exist only in
-  the developer build (libdcb200_dev.so, -DDCB_DEV_SWITCHES) and are read when an engine is created; the product
-  library ignores the environment (checked first)."""
+def test_unfused_fallback_paths_agree_with_fused(engine_mod, monkeypatch):
+  """DCB_ALIGN=0 selects the alternative token layout and chunk_tiles=1 the smallest chunks, of the same math.  The
+  switch exists only in the developer build (libdcb200_dev.so, -DDCB_DEV_SWITCHES) and is read when an engine is
+  created; the product library ignores the environment."""
   p = params_lib.synthetic_params(20, 120, num_hidden_layers=2)
   w = weights_lib.init_weights(p, seed=21)
   rows = synthetic.make_rows(p, 5, seed=22)
   ref = omodel.forward(rows, p, w)["logits"]
-  dev = engine_mod.load_dev_library()
   one_chunk = 3 + 5 * p.num_hidden_layers                          # embed, condenser, 5 per layer, head
+
+  def run(**kw):
+    model = engine_mod.B200Model(p, w, max_batch=8, **kw)
+    logits = model.forward(rows, want_logits=True)["logits"]
+    launches = model.last_launches
+    model.close()
+    return logits, launches
+
   outs = {}
-  for name, env in (("default", {}),                                   # one window per 128-token tile, one chunk
-                    ("packed", {"DCB_ALIGN": "0"}),                     # windows packed back to back across tiles
-                    ("chunked", {"DCB_CHUNK_TILES": "1"})):             # one tile (one window) per chunk
-    old = {k: os.environ.get(k) for k in env}
-    os.environ.update(env)
-    try:
-      model = engine_mod.B200Model(p, w, max_batch=8, library=dev)
-      outs[name] = model.forward(rows, want_logits=True)["logits"]
-      launches = model.last_launches
-      model.close()
-      if name == "chunked":
-        assert launches == rows.shape[0] * one_chunk
-        prod = engine_mod.B200Model(p, w, max_batch=8)              # product library: the switch is ignored
-        prod.forward(rows)
-        assert prod.last_launches == one_chunk
-        prod.close()
-    finally:
-      for k, v in old.items():
-        if v is None:
-          os.environ.pop(k, None)
-        else:
-          os.environ[k] = v
-    assert np.abs(outs[name] - ref).max() <= LOGIT_TOL_FP32, name
+  outs["default"], launches = run()                                  # one window per 128-token tile, one chunk
+  assert launches == one_chunk
+  outs["chunked"], launches = run(chunk_tiles=1)                     # one tile (one window) per chunk
+  assert launches == rows.shape[0] * one_chunk
+  monkeypatch.setenv("DCB_ALIGN", "0")
+  outs["packed"], _ = run(library=engine_mod.load_dev_library())    # windows packed back to back across tiles
+  prod, launches = run()                                             # product library: the switch is ignored
+  assert np.array_equal(prod, outs["default"]) and launches == one_chunk
+  for name, out in outs.items():
+    assert np.abs(out - ref).max() <= LOGIT_TOL_FP32, name
   assert np.array_equal(outs["default"], outs["chunked"])
   assert np.abs(outs["default"] - outs["packed"]).max() < 0.05
 

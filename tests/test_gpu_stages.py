@@ -24,23 +24,12 @@ def engine_mod():
   return engine
 
 
-def _capture(model, p, B):
-  """Everything check_forward needs from the last forward's debug capture."""
-  M, nl = B * int(p.max_length), int(p.num_hidden_layers)
-  return dict(emb=model.debug_operand(0, "embed", M),
-              x=[model.debug_residual(s, M) for s in range(1 + 2 * nl)],
-              xb={s: model.debug_operand(s, "xb", M) for s in range(2 * nl)},
-              qkv=[model.debug_operand(1 + 2 * n, "qkv", M) for n in range(nl)],
-              att=[model.debug_operand(1 + 2 * n, "att", M) for n in range(nl)],
-              hid=[model.debug_operand(2 + 2 * n, "hid", M) for n in range(nl)])
-
-
 def _check_stages(engine_mod, name, p, w, rows, library=None):
   B = rows.shape[0]
   model = engine_mod.B200Model(p, w, max_batch=B, library=library)
   model.set_debug(True)
   out = model.forward(rows, want_logits=True)
-  dev = _capture(model, p, B)
+  dev = model.debug_capture(B * int(p.max_length))
   model.close()
   dev["logits"] = out["logits"].reshape(-1, 5)
   worst = stages.check_forward(stages.prepare(p, w), rows, dev)
