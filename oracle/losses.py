@@ -197,18 +197,25 @@ def per_example_accuracy(probs: np.ndarray, labels: np.ndarray) -> np.ndarray:
   return (y == x).all(-1).astype(np.uint8)
 
 
+def decode_ccs_ids(ccs: np.ndarray) -> np.ndarray:
+  """get_batch_identity_ccs_pred's one_hot(ccs, 5) followed by AlignmentMetric's argmax: ids outside 0..4 give an
+  all-zero row, whose argmax is 0, the gap."""
+  ccs = np.asarray(ccs).astype(np.int32)
+  return np.where((ccs >= 0) & (ccs <= 4), ccs, 0).astype(np.uint8)
+
+
 def ccs_ids_from_rows(rows: np.ndarray, max_passes: int) -> np.ndarray:
   """model_utils.get_ccs_from_example + one_hot/argmax decoding: row 4P of every window (data_providers.get_indices),
   ids outside 0..4 decode to 0 (an all-zero one-hot row)."""
-  ccs = np.asarray(rows)[:, 4 * max_passes, :].astype(np.int32)
-  return np.where((ccs >= 0) & (ccs <= 4), ccs, 0).astype(np.uint8)
+  return decode_ccs_ids(np.asarray(rows)[:, 4 * max_passes, :])
 
 
 def evaluate_windows(probs: np.ndarray, labels: np.ndarray, ccs_ids: np.ndarray, del_cost: float = 10.0,
                      loss_reg: Optional[float] = 0.1) -> Dict[str, np.ndarray]:
-  """Per-window values the engine's dcb_evaluate computes: loss, exact-match flag, counts for prediction and CCS."""
+  """Per-window values the engine's dcb_evaluate computes: loss, exact-match flag, counts for prediction and CCS.
+  `ccs_ids` are the stored CCS ids (uint8 [B, L]); ids above 4 decode as gaps (decode_ccs_ids)."""
   pred = alignment_metric(labels, np.asarray(probs).argmax(-1))
-  ccs = alignment_metric(labels, ccs_ids)
+  ccs = alignment_metric(labels, decode_ccs_ids(ccs_ids))
   return dict(loss=alignment_loss(probs, labels, del_cost, loss_reg), exact=per_example_accuracy(probs, labels),
               pred_counts=np.stack([pred[k] for k in COUNT_KEYS], -1).astype(np.int32),
               ccs_counts=np.stack([ccs[k] for k in COUNT_KEYS], -1).astype(np.int32))
