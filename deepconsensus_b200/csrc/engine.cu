@@ -148,7 +148,6 @@ struct dcb_engine {
   DevBuf<float> d_x;
   DevBuf<__nv_bfloat16> d_xb;
   DevBuf<__nv_bfloat16> d_att;
-  DevBuf<float> d_part;          // the FFN's partial sums between its two launches, residual image layout
   DevBuf<__nv_bfloat16> d_hid;   // FFN hidden activation, bf16 operand image [tile][ff/8][128][8] (debug capture only)
   DevBuf<double> d_p10;          // 10^(-q/10), q = 0..255 (host libm pow, as NumPy)
   DevBuf<float> d_dbg;           // [stages][chunk_tiles * x_image]
@@ -725,11 +724,10 @@ void bf16_forward_chunk(dcb_engine* e, LaunchRecorder& rec, const float* rows_ch
       launch_gemm_row(e->d_att, ld.wo, kDP / 16, 2 * (kDP / 16), T, row_epi(e, true, nullptr, n_, 1, false), st);
     });
     snap();
-    rec.run(kProfFfn, 2, [&] {   // relu(xb W1 + b1) W2 + b2 + residual, half of the filter per launch; xb = next layer's
+    rec.run(kProfFfn, 2, [&] {   // relu(xb W1 + b1) W2 + b2 + residual, half of the tiles per launch; xb = next layer's
       const RowEpi epi = row_epi(e, true, ld.b2, n_ + 1, 0, false);
       __nv_bfloat16* hid = e->debug ? e->d_hid.p : nullptr;
-      launch_ffn(false, e->d_xb, ld.w1, ld.b1, ld.w2, c.filter_size, T, e->d_part, hid, epi, st);
-      launch_ffn(true, e->d_xb, ld.w1, ld.b1, ld.w2, c.filter_size, T, e->d_part, hid, epi, st);
+      for (int half = 0; half < 2; ++half) launch_ffn(half, e->d_xb, ld.w1, ld.b1, ld.w2, c.filter_size, T, hid, epi, st);
     });
     if (e->profile) e->prof_ffn_tokens += (long long)bw * L;   // valid tokens (layout padding is not algorithmic work)
     snap();
@@ -853,7 +851,6 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
     if (!rc) rc = alloc(e, e->d_x, T * x_image_elems());
     if (!rc) rc = alloc(e, e->d_xb, T * act_image_elems(kDP));
     if (!rc) rc = alloc(e, e->d_att, T * act_image_elems(kDP));
-    if (!rc) rc = alloc(e, e->d_part, T * x_image_elems());
     return rc;
   }();
   if (rc) {

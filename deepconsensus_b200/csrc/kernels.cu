@@ -7,7 +7,7 @@
 //                       feeding two consumer warpgroups through an mbarrier ring.  Used for the
 //                       condenser (+pos-enc), fused QKV and attention out-proj.
 //   ffn_gemm_kernel     the FFN relu(x W1 + b1) W2 + b2 (ffn_layer.py:83-86) with the hidden
-//                       activation kept in registers, half of the filter per launch.
+//                       activation kept in registers, half of the tiles per launch.
 //   band_attention_kernel  banded multi-head softmax attention (attention_layer.py:198-214)
 //   head_kernel         final LayerNorm -> fc1 -> softmax -> argmax -> Phred -> ASCII
 //                       (encoder_stack.py:197, networks.py:342,238, quick_inference.py:377-414)
@@ -472,25 +472,27 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
 // =====================================================================================
 // FFN with the hidden activation on the SM
 // =====================================================================================
-// out = relu(xb W1 + b1) W2 + b2 + x for one 128-token tile per work item, over the filter's 128-unit chunks
-// [c_begin, c_end).  The tile's xb (A) image is loaded once and stays resident; warpgroup w owns tile rows
-// [64 w, 64 w + 64).  Per chunk c each consumer warpgroup
+// out = relu(xb W1 + b1) W2 + b2 + x for one 128-token tile per work item, over all of the filter's 128-unit chunks.
+// The tile's xb (A) image is loaded once and stays resident; warpgroup w owns tile rows [64 w, 64 w + 64).  Per chunk
+// c each consumer warpgroup
 //   1. computes H = xb W1[:, c] with m64n128k16 wgmmas over the 18 k-steps (the W1 image holds chunk c as one
 //      contiguous [36][128][8] group),
 //   2. turns H into bf16(relu(H + b1)) in registers, packed straight into the A fragments of the next step (for
 //      hidden k-step kk: pack(d[8kk + 0..1]), pack(d[8kk + 2..3]), pack(d[8kk + 4..5]), pack(d[8kk + 6..7])),
 //   3. accumulates that times W2's rows of chunk c (k-steps [8c, 8c + 8) of the [ff/8][288][8] image) with register-A
-//      m64n144k16 wgmmas into the 288-wide fp32 accumulators.
-// The producer streams W1 group c and then W2's k-steps of c through one ring of 9216-byte stages (two W1 k-steps or
-// one W2 k-step each).
+//      m64n144k16 wgmmas into the 288-wide fp32 accumulators,
+// and the tile ends with the row epilogue.  The producer streams W1 group c and then W2's k-steps of c through one
+// ring of 9216-byte stages (two W1 k-steps or one W2 k-step each).  A W1 stage leaves 1 KB free: the chunk's last W1
+// stage also brings the chunk's 128 b1 values there, and the consumers hand that stage back only after step 2 has
+// read them.  (Held in the first W1 stage, b1 would stall the producer before this chunk's last W2 stage, which
+// reuses that slot; the last W1 stage's slot is not needed again until the next chunk.)
 //
-// The forward launches the kernel twice per layer, each over half of the chunks, because each of the forward's five
-// launches per layer ends on a captured stage.  The first launch (kFinish false) starts from zero and stores the fp32
-// accumulators to `part`, an image with the residual image's layout; the second (kFinish true) loads them back and
-// ends with the row epilogue.  Every output element sees the same k16 MMAs in the same order on one fp32 accumulator,
-// and the hidden values come from the same instruction shape, K order, bias, ReLU and rounding as a separate
-// up-projection would give, so the result does not depend on where the filter is split.  When `hid` is not null the
-// hidden activation is also stored there as a bf16 operand image [tile][ff/8][128][8] (debug capture).
+// The forward launches the kernel twice per layer, over the first and the second half of the tiles, because each of
+// the forward's five launches per layer ends on a captured stage.  Each tile runs the whole filter once; its first
+// MMA starts from zero, so every output element sees the same k16 MMAs in the same order on one fp32 accumulator
+// wherever the tiles are split, and the hidden values come from the same instruction shape, K order, bias, ReLU and
+// rounding as a separate up-projection would give.  kHid: the hidden activation is also stored to `hid` as a bf16
+// operand image [tile][ff/8][128][8] (debug capture).
 struct FfnCfg {
   static constexpr int kUpK = kDP / 16;                   // up-projection k-steps per chunk
   static constexpr int kDownK = kFFChunk / 16;            // down-projection k-steps per chunk
@@ -498,25 +500,25 @@ struct FfnCfg {
   static constexpr int kW1Bytes = 2 * kFFChunk * 16;      // one W1 k-step: 4096
   static constexpr int kW2Bytes = 2 * kDP * 16;           // one W2 k-step: 9216
   static constexpr int kStageBytes = kW2Bytes;            // two W1 k-steps or one W2 k-step
+  static constexpr int kB1Off = 2 * kW1Bytes;             // a chunk's b1 in its last W1 stage
+  static constexpr int kB1Bytes = kFFChunk * 4;
   static constexpr int kStages = 16;
   static constexpr int kATileBytes = kUpK * kABytesPerK;  // the resident xb tile
   static constexpr int kBarBytes = 512;
   static constexpr int kVecBytes = 3 * kDP * 4;           // row epilogue: bias, LayerNorm gamma, beta (fp32)
-  static constexpr int kMaxChunks = (2048 / kFFChunk + 1) / 2;   // a launch's chunks at filter_size 2048
-  static constexpr int kB1Bytes = kMaxChunks * kFFChunk * 4;     // the launch's b1 slice (fp32)
-  // the xb tile, the ring, the mbarriers, the row vectors, b1
-  static constexpr int kSmemBytes = kATileBytes + kStages * kStageBytes + kBarBytes + kVecBytes + kB1Bytes;
+  // the xb tile, the ring, the mbarriers, the row vectors
+  static constexpr int kSmemBytes = kATileBytes + kStages * kStageBytes + kBarBytes + kVecBytes;
   static constexpr int kThreads = 384;
   static_assert(kSmemBytes <= 232448, "over the sm_90 opt-in shared memory per block");
   static_assert((2 * kStages + 2) * 8 <= kBarBytes, "the mbarriers (full, empty, a_full, a_empty) fit");
-  static_assert(2 * kW1Bytes <= kStageBytes && kUpK % 2 == 0, "a stage holds two W1 k-steps");
+  static_assert(kB1Off + kB1Bytes <= kStageBytes && kUpK % 2 == 0, "a stage holds two W1 k-steps and b1");
 };
 
-template <bool kFinish>
+template <bool kHid>
 __global__ void __launch_bounds__(384, 1)
 ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* __restrict__ w1_img,
-                const float* __restrict__ b1, const __nv_bfloat16* __restrict__ w2_img, int ff, int c_begin, int c_end,
-                int ntiles, float* __restrict__ part, __nv_bfloat16* __restrict__ hid, RowEpi epi) {
+                const float* __restrict__ b1, const __nv_bfloat16* __restrict__ w2_img, int ff, int tile_begin,
+                int tile_end, __nv_bfloat16* __restrict__ hid, RowEpi epi) {
   using Cfg = FfnCfg;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* a_res = smem;
@@ -526,13 +528,11 @@ ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* _
   uint64_t* a_full = empty + Cfg::kStages;
   uint64_t* a_empty = a_full + 1;
   float* s_vec = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + Cfg::kBarBytes);   // [3][kDP]
-  float* s_b1 = s_vec + 3 * kDP;                                                                  // chunks c_begin..
-  const int nch = c_end - c_begin;
+  const int nch = ff / kFFChunk;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  if constexpr (kFinish) row_vectors_to_smem(s_vec, epi);
-  for (int i = threadIdx.x; i < nch * kFFChunk; i += blockDim.x) s_b1[i] = b1[c_begin * kFFChunk + i];
+  row_vectors_to_smem(s_vec, epi);
   if (threadIdx.x == 0) {
     for (int i = 0; i < Cfg::kStages; ++i) {
       mbar_init(&full[i], 1);
@@ -547,24 +547,29 @@ ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* _
   if (warp >= 8) {
     // ------------------------------------------------------------- producer
     setmaxnreg_dec<24>();
-    if (warp == 8 && lane == 0 && nch > 0) {
+    if (warp == 8 && lane == 0) {
       uint32_t slot = 0, phase = 0, it = 0;
-      auto stage = [&](const uint8_t* src, uint32_t bytes) {
+      // one stage: `bytes` from src, and b1_bytes (0 or the chunk's b1) from b1_src behind them
+      auto stage = [&](const uint8_t* src, uint32_t bytes, const float* b1_src, uint32_t b1_bytes) {
         mbar_wait(&empty[slot], phase ^ 1);
-        mbar_arrive_expect_tx(&full[slot], bytes);
-        bulk_g2s(stage_base + slot * Cfg::kStageBytes, src, bytes, &full[slot]);
+        uint8_t* st = stage_base + slot * Cfg::kStageBytes;
+        mbar_arrive_expect_tx(&full[slot], bytes + b1_bytes);
+        bulk_g2s(st, src, bytes, &full[slot]);
+        if (b1_bytes) bulk_g2s(st + Cfg::kB1Off, b1_src, b1_bytes, &full[slot]);
         if (++slot == Cfg::kStages) { slot = 0; phase ^= 1; }
       };
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+      for (int tile = tile_begin + blockIdx.x; tile < tile_end; tile += gridDim.x, ++it) {
         mbar_wait(a_empty, (it & 1) ^ 1);
         mbar_arrive_expect_tx(a_full, Cfg::kATileBytes);
         bulk_g2s(a_res, reinterpret_cast<const uint8_t*>(xb_img) + (size_t)tile * Cfg::kATileBytes, Cfg::kATileBytes,
                  a_full);
-        for (int c = c_begin; c < c_end; ++c) {
+        for (int c = 0; c < nch; ++c) {
           const uint8_t* w1 = reinterpret_cast<const uint8_t*>(w1_img) + (size_t)c * Cfg::kUpK * Cfg::kW1Bytes;
-          for (int s = 0; s < Cfg::kUpK / 2; ++s) stage(w1 + (size_t)s * 2 * Cfg::kW1Bytes, 2 * Cfg::kW1Bytes);
+          for (int s = 0; s < Cfg::kUpK / 2; ++s)
+            stage(w1 + (size_t)s * 2 * Cfg::kW1Bytes, 2 * Cfg::kW1Bytes, b1 + c * kFFChunk,
+                  s + 1 == Cfg::kUpK / 2 ? Cfg::kB1Bytes : 0);
           const uint8_t* w2 = reinterpret_cast<const uint8_t*>(w2_img) + (size_t)c * Cfg::kDownK * Cfg::kW2Bytes;
-          for (int kk = 0; kk < Cfg::kDownK; ++kk) stage(w2 + (size_t)kk * Cfg::kW2Bytes, Cfg::kW2Bytes);
+          for (int kk = 0; kk < Cfg::kDownK; ++kk) stage(w2 + (size_t)kk * Cfg::kW2Bytes, Cfg::kW2Bytes, nullptr, 0);
         }
       }
     }
@@ -581,27 +586,9 @@ ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* _
   float hacc[kFFChunk / 2];       // H of the current chunk
   uint32_t slot = 0, phase = 0, it = 0;
   auto next_slot = [&]() { if (++slot == Cfg::kStages) { slot = 0; phase ^= 1; } };
-  // the accumulators' fragments in the partial image (the residual image's layout, as in row_epilogue)
-  auto part_frag = [&](int tile, int h, int j, int jj) {
-    return part + (size_t)tile * x_image_elems() + ((q >> 1) * kTileM + row0) * 4 + 2 * (q & 1) + 32 * h +
-           (j * kNC + jj * 8) * kTileM;
-  };
-  auto load_part = [&](int tile) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-#pragma unroll
-      for (int j = 0; j < 2; ++j)
-#pragma unroll
-        for (int jj = 0; jj < kNC / 8; ++jj) {
-          const float2 v = *reinterpret_cast<const float2*>(part_frag(tile, h, j, jj));
-          acc[j][jj * 4 + 2 * h] = v.x;
-          acc[j][jj * 4 + 2 * h + 1] = v.y;
-        }
-  };
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-    if constexpr (kFinish) load_part(tile);   // the partial sums load while xb and the first weights arrive
-    if (nch > 0) mbar_wait(a_full, it & 1);
-    for (int c = c_begin; c < c_end; ++c) {
+  for (int tile = tile_begin + blockIdx.x; tile < tile_end; tile += gridDim.x, ++it) {
+    mbar_wait(a_full, it & 1);
+    for (int c = 0; c < nch; ++c) {
       // ---- 1. H = xb W1[:, c]
       uint32_t prev = 0;
 #pragma unroll
@@ -627,13 +614,12 @@ ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* _
       }
       wgmma_wait<0>();
       wgmma_fence_regs(hacc);
-      mbar_arrive(&empty[prev]);
-      if (c + 1 == c_end) mbar_arrive(a_empty);   // the item's last MMAs on xb have completed
+      if (c + 1 == nch) mbar_arrive(a_empty);   // the item's last MMAs on xb have completed
 
       // ---- 2. bf16(relu(H + b1)) as A fragments: fragment (kk, i) holds hidden columns 16 kk + 8 (i >> 1) + 2q, +1
-      // of row row0 + 8 (i & 1), i.e. accumulator elements 8 kk + 2 i, + 1
+      // of row row0 + 8 (i & 1), i.e. accumulator elements 8 kk + 2 i, + 1.  b1 is in the last W1 stage (prev).
       uint32_t af[Cfg::kDownK][4];
-      const float* bc = s_b1 + (c - c_begin) * kFFChunk + 2 * q;
+      const float* bc = reinterpret_cast<const float*>(stage_base + prev * Cfg::kStageBytes + Cfg::kB1Off) + 2 * q;
 #pragma unroll
       for (int kk = 0; kk < Cfg::kDownK; ++kk)
 #pragma unroll
@@ -641,7 +627,8 @@ ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* _
           const float2 b = *reinterpret_cast<const float2*>(bc + 16 * kk + 8 * (i >> 1));
           af[kk][i] = pack_bf16x2(fmaxf(hacc[8 * kk + 2 * i] + b.x, 0.f), fmaxf(hacc[8 * kk + 2 * i + 1] + b.y, 0.f));
         }
-      if (hid) {
+      mbar_arrive(&empty[prev]);
+      if constexpr (kHid) {
         __nv_bfloat16* hb = hid + (size_t)tile * kTileM * ff + (size_t)row0 * 8 + 2 * q;
 #pragma unroll
         for (int kk = 0; kk < Cfg::kDownK; ++kk)
@@ -661,8 +648,7 @@ ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* _
         wgmma_fence();
 #pragma unroll
         for (int j = 0; j < 2; ++j)
-          wgmma_m64n144k16_rs(acc[j], af[kk], make_kc16_desc(st + j * kNC * 16, kDP * 16, 128),
-                              kFinish || c != c_begin || kk != 0);
+          wgmma_m64n144k16_rs(acc[j], af[kk], make_kc16_desc(st + j * kNC * 16, kDP * 16, 128), c != 0 || kk != 0);
         wgmma_commit();
         wgmma_fence_regs(acc[0]);
         wgmma_fence_regs(acc[1]);
@@ -681,18 +667,7 @@ ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* _
       mbar_arrive(&empty[prev]);
     }
 
-    if constexpr (kFinish) {
-      row_epilogue<kNC, 2, false>(acc, tile, row0, q, s_vec, epi);
-    } else {
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int j = 0; j < 2; ++j)
-#pragma unroll
-          for (int jj = 0; jj < kNC / 8; ++jj)
-            *reinterpret_cast<float2*>(part_frag(tile, h, j, jj)) =
-                make_float2(acc[j][jj * 4 + 2 * h], acc[j][jj * 4 + 2 * h + 1]);
-    }
+    row_epilogue<kNC, 2, false>(acc, tile, row0, q, s_vec, epi);
   }
 }
 
@@ -1050,17 +1025,21 @@ void launch_gemm_qkv(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int
       a_img, b_img, kDP / 16, 2 * (kDP / 16), ntiles, kQKVN / kQKVGroup, qkv_img, kQKVN / 8, none);
 }
 
-void launch_ffn(bool finish, const __nv_bfloat16* xb_img, const __nv_bfloat16* w1_img, const float* b1,
-                const __nv_bfloat16* w2_img, int ff, int ntiles, float* part_img, __nv_bfloat16* hid_img,
-                const RowEpi& epi, cudaStream_t st) {
-  const int nch = ff / kFFChunk, half = (nch + 1) / 2;
-  const int grid = ntiles < num_sms() ? ntiles : num_sms();
-  if (finish)
-    ffn_gemm_kernel<true><<<grid, FfnCfg::kThreads, FfnCfg::kSmemBytes, st>>>(xb_img, w1_img, b1, w2_img, ff, half, nch,
-                                                                              ntiles, part_img, hid_img, epi);
+void launch_ffn(int half, const __nv_bfloat16* xb_img, const __nv_bfloat16* w1_img, const float* b1,
+                const __nv_bfloat16* w2_img, int ff, int ntiles, __nv_bfloat16* hid_img, const RowEpi& epi,
+                cudaStream_t st) {
+  const int split = (ntiles + 1) / 2;
+  const int t0 = half ? split : 0, t1 = half ? ntiles : split;
+  // a half without tiles still launches (one CTA that finds no work), so the forward's launch count does not depend
+  // on the chunk size
+  const int n = t1 - t0;
+  const int grid = n < 1 ? 1 : n < num_sms() ? n : num_sms();
+  if (hid_img)
+    ffn_gemm_kernel<true><<<grid, FfnCfg::kThreads, FfnCfg::kSmemBytes, st>>>(xb_img, w1_img, b1, w2_img, ff, t0, t1,
+                                                                              hid_img, epi);
   else
-    ffn_gemm_kernel<false><<<grid, FfnCfg::kThreads, FfnCfg::kSmemBytes, st>>>(xb_img, w1_img, b1, w2_img, ff, 0, half,
-                                                                               ntiles, part_img, hid_img, epi);
+    ffn_gemm_kernel<false><<<grid, FfnCfg::kThreads, FfnCfg::kSmemBytes, st>>>(xb_img, w1_img, b1, w2_img, ff, t0, t1,
+                                                                               nullptr, epi);
 }
 
 // packed rows -> the float32 [B, R, L] rows they stand for (the strict-fp32 path reads float32 rows)

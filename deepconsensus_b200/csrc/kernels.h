@@ -21,14 +21,13 @@ void launch_gemm_row(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int
 // split-bf16 weights [72][kQKVGroup][8] (hi chunks, then lo chunks)
 void launch_gemm_qkv(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int ntiles,
                      __nv_bfloat16* qkv_img, cudaStream_t st);
-// One half of the FFN relu(xb W1 + b1) W2 + b2 with the row epilogue `epi` (kernels.cu, ffn_gemm_kernel): the first
-// launch (finish false) takes the first ceil(n / 2) of the n = ff / kFFChunk hidden chunks and writes its partial sums
-// to part_img (fp32, the residual image's layout), the second (finish true) adds the other chunks to them and runs the
-// epilogue.  w1_img: ff / kFFChunk groups of [36][kFFChunk][8]; w2_img: [ff/8][288][8].  hid_img, when not null,
-// receives the bf16 hidden activation as an operand image [tile][ff/8][128][8].
-void launch_ffn(bool finish, const __nv_bfloat16* xb_img, const __nv_bfloat16* w1_img, const float* b1,
-                const __nv_bfloat16* w2_img, int ff, int ntiles, float* part_img, __nv_bfloat16* hid_img,
-                const RowEpi& epi, cudaStream_t st);
+// One half of the FFN relu(xb W1 + b1) W2 + b2 with the row epilogue `epi` (kernels.cu, ffn_gemm_kernel): half 0
+// runs tiles [0, ceil(ntiles / 2)), half 1 the rest, each over the whole filter.  w1_img: ff / kFFChunk groups of
+// [36][kFFChunk][8]; w2_img: [ff/8][288][8].  hid_img, when not null, receives the bf16 hidden activation as an
+// operand image [tile][ff/8][128][8].
+void launch_ffn(int half, const __nv_bfloat16* xb_img, const __nv_bfloat16* w1_img, const float* b1,
+                const __nv_bfloat16* w2_img, int ff, int ntiles, __nv_bfloat16* hid_img, const RowEpi& epi,
+                cudaStream_t st);
 void launch_unpack_rows(const uint8_t* packed, const PackedLayout& pl, int nwindows, float* rows, cudaStream_t st);
 void launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* att, int L, int Lw, int win, int nwindows,
                       cudaStream_t st);

@@ -7,7 +7,8 @@ Writes DIR/profile_gemms.json (and DIR/trace.json, the torch.profiler trace it w
            1024, packed rows resident in HBM).  The row-epilogue GEMM is one kernel for three launches of a layer, so
            each launch is named by the kernel before it: the condenser follows the embedding, the out-projection the
            attention, the FFN down-projection the FFN up-projection.  Builds with the fused FFN launch it twice per
-           layer: ffn_first (the first half of the filter, partial sums out) and ffn_final (the rest, row epilogue).
+           layer, named by their order in the layer: ffn_first and ffn_second, each over half of the tiles and the
+           whole filter, with the row epilogue.
   l2_read  for each GEMM, the bytes its CTAs read from L2 per launch (weights once per work item, activations,
            residual), computed from the shapes and the tiling, over its kernel time.
   hbm      for each FFN launch, the activation bytes it reads and writes in HBM (the weights stay in L2), computed
@@ -65,24 +66,31 @@ def l2_bytes(role, ntiles, ff, epad, tokens):
     return passes * (KDP * ff * 2) + ntiles * a_tile * ff + res
   if role == "condenser":
     return passes * (KDP * 2 * epad * 2) + ntiles * 2 * a_tile * epad
-  if role in ("ffn_first", "ffn_final"):    # one tile per work item; W1 and W2 rows of the launch's hidden chunks
-    nch = ff // 128
-    chunks = (nch + 1) // 2 if role == "ffn_first" else nch // 2
-    return ntiles * (chunks * 128 * KDP * 2 * 2 + a_tile * KDP) + (2 * res if role == "ffn_final" else 0)
+  if role in ("ffn_first", "ffn_second"):    # one tile per work item: the whole of W1 and W2, xb, the residual
+    n = ffn_half_tiles(role, ntiles)
+    return n * (ff * KDP * 2 * 2 + a_tile * KDP + TILE * KDP * 4)
   return None
+
+
+def ffn_half_tiles(role, ntiles):
+  """Tiles of the FFN launch `role`: the first takes ceil(ntiles / 2), the second the rest."""
+  return (ntiles + 1) // 2 if role == "ffn_first" else ntiles // 2
 
 
 HBM_TBPS = 3.35    # H100 SXM data sheet
 
 
 def hbm_bytes(role, ntiles, ff):
-  """Activation bytes one FFN launch reads and writes in HBM: bf16 xb / hidden images, fp32 residual and partial-sum
-  images (the next layer's xb is counted for every layer)."""
+  """Activation bytes one FFN launch reads and writes in HBM: bf16 xb / hidden images and the fp32 residual image
+  (the next layer's xb is counted for every layer).  ffn_first / ffn_second: xb in, residual in and out, next xb out
+  for the launch's half of the tiles."""
+  if role in ("ffn_first", "ffn_second"):
+    ntiles = ffn_half_tiles(role, ntiles)
   xb = ntiles * TILE * KDP * 2
   x = ntiles * TILE * KDP * 4
   hid = ntiles * TILE * ff * 2
   return {"ffn_up": xb + hid, "ffn_down": hid + x + x + xb,
-          "ffn_first": xb + x, "ffn_final": xb + x + x + x + xb}.get(role)
+          "ffn_first": xb + x + x + xb, "ffn_second": xb + x + x + xb}.get(role)
 
 
 def main():
@@ -148,9 +156,8 @@ def main():
   kernels = sorted((e for e in events if e.get("cat") == "kernel"), key=lambda e: e["ts"])
 
   def role_of(name, prev):
-    m = re.search(r"ffn_gemm_kernel<(true|false)>", name)
-    if m:
-      return "ffn_final" if m.group(1) == "true" else "ffn_first"
+    if "ffn_gemm_kernel" in name:
+      return "ffn_second" if prev == "ffn_first" else "ffn_first"
     m = re.search(r"gemm_kernel<(\d+), (\d+), (\d+), (true|false)>", name)
     if m:
       epi = int(m.group(3))
