@@ -306,19 +306,92 @@ void trim_insertions(BamRecord* r, std::vector<double>* pw, std::vector<double>*
   r->cigar = cig;
 }
 
-int expand_clip_indent(BamRecord* rec, int ins_trim, Read* out) {
+// pw / ip tags of a subread as the reference reads them (pre_lib.py:1141-1146)
+void load_kinetics(const BamRecord& rec, std::vector<double>* pw, std::vector<double>* ip) {
   Tag t;
-  std::vector<double> pw, ip;
-  if (rec->find("pw", &t) && t.type == 'B') { pw.resize(t.count); for (size_t i = 0; i < t.count; ++i) pw[i] = BamRecord::element(t, i); }
-  if (rec->find("ip", &t) && t.type == 'B') { ip.resize(t.count); for (size_t i = 0; i < t.count; ++i) ip[i] = BamRecord::element(t, i); }
-  {
-    // sanity before anything is sized from the record: alignments to a CCS read span at most a few hundred kilobases
-    uint64_t cols = 0;
-    for (uint32_t c : rec->cigar) cols += c >> 4;
-    if (cols > (1u << 24) || rec->pos < 0 || rec->pos > (1 << 24))
-      return pfail(DCB_ERR_INVALID, "%s: implausible alignment (cigar / position)", rec->qname.c_str());
+  if (rec.find("pw", &t) && t.type == 'B') { pw->resize(t.count); for (size_t i = 0; i < t.count; ++i) (*pw)[i] = BamRecord::element(t, i); }
+  if (rec.find("ip", &t) && t.type == 'B') { ip->resize(t.count); for (size_t i = 0; i < t.count; ++i) (*ip)[i] = BamRecord::element(t, i); }
+}
+
+// uint8 arrays (pre_lib.py:1166-1167)
+inline uint8_t kinetic_u8(double v) { return (uint8_t)v; }
+
+inline bool op_has_column(int op) { return op == kCMatch || op == kCEq || op == kCDiff || op == kCIns || op == kCSoft || op == kCDel || op == kCRefSkip; }
+inline bool op_has_query(int op) { return op == kCMatch || op == kCEq || op == kCDiff || op == kCIns || op == kCSoft; }
+
+// sanity before anything is sized from the record: alignments to a CCS read span at most a few hundred kilobases
+int check_plausible(const BamRecord& rec) {
+  uint64_t cols = 0;
+  for (uint32_t c : rec.cigar) cols += c >> 4;
+  if (cols > (1u << 24) || rec.pos < 0 || rec.pos > (1 << 24))
+    return pfail(DCB_ERR_INVALID, "%s: implausible alignment (cigar / position)", rec.qname.c_str());
+  return DCB_OK;
+}
+
+// Alignment columns [qs, qe) that survive the soft clips, out of `aln`
+struct Clip { size_t aln = 0, qs = 0, qe = 0; };
+
+// Every check expand_clip_indent makes on a subread once trim_insertions has run, from the trimmed cigar and the
+// trimmed lengths of its sequence and kinetics alone, so that the host construction and the raw-record export refuse
+// the same records with the same messages.  Fills the clip and the four sn values.
+int check_trimmed(const BamRecord& rec, const std::vector<uint32_t>& cigar, size_t seq_len, size_t n_pw, size_t n_ip,
+                  Clip* clip, float* sn) {
+  size_t aln = 0, nq = 0, cig_cols = 0;
+  bool any_soft = false;
+  for (uint32_t c : cigar) {
+    const int op = c & 15;
+    const size_t len = c >> 4;
+    if (op_has_column(op)) aln += len;
+    if (op_has_query(op)) nq += len;
+    if (op != kCHard) cig_cols += len;
+    any_soft |= op == kCSoft && len;
   }
+  if (nq != seq_len) return pfail(DCB_ERR_INVALID, "%s: cigar covers %zu query bases, sequence has %zu", rec.qname.c_str(), nq, seq_len);
+  if (n_pw != nq || n_ip != nq) return pfail(DCB_ERR_INVALID, "%s: pw / ip tags do not match the sequence length", rec.qname.c_str());
+  Tag t;
+  if (!rec.find("sn", &t) || t.type != 'B' || t.count < 4) return pfail(DCB_ERR_INVALID, "%s: no sn tag", rec.qname.c_str());
+  for (int i = 0; i < 4; ++i) sn[i] = (float)BamRecord::element(t, i);
+  if (cig_cols != aln) return pfail(DCB_ERR_INVALID, "%s: unsupported cigar operation (pad)", rec.qname.c_str());
+  clip->aln = aln; clip->qs = 0; clip->qe = aln;
+  if (!any_soft) return DCB_OK;
+  // query_alignment_start / _end: query bases outside leading / trailing soft clips
+  size_t lead_soft = 0, trail_soft = 0;
+  size_t i = 0;
+  while (i < cigar.size() && (cigar[i] & 15) == kCHard) ++i;
+  if (i < cigar.size() && (cigar[i] & 15) == kCSoft) lead_soft = cigar[i] >> 4;
+  size_t j = cigar.size();
+  while (j > 0 && (cigar[j - 1] & 15) == kCHard) --j;
+  if (j > 0 && (cigar[j - 1] & 15) == kCSoft && j - 1 != i) trail_soft = cigar[j - 1] >> 4;
+  // the alignment column of a query index
+  auto column_of = [&](int64_t q, size_t* col) {
+    if (q < 0) return false;
+    size_t c0 = 0, q0 = 0;
+    for (uint32_t c : cigar) {
+      const int op = c & 15;
+      const size_t len = c >> 4;
+      if (op_has_query(op)) {
+        if ((size_t)q < q0 + len) { *col = c0 + ((size_t)q - q0); return true; }
+        q0 += len;
+      }
+      if (op_has_column(op)) c0 += len;
+    }
+    return false;
+  };
+  size_t last = 0;
+  const bool f1 = column_of((int64_t)lead_soft, &clip->qs);
+  const bool f2 = column_of((int64_t)seq_len - (int64_t)trail_soft - 1, &last);
+  clip->qe = last + 1;
+  if (!f1 || !f2 || clip->qe < clip->qs) return pfail(DCB_ERR_INVALID, "%s: cannot locate the aligned part", rec.qname.c_str());
+  return DCB_OK;
+}
+
+int expand_clip_indent(BamRecord* rec, int ins_trim, Read* out) {
+  std::vector<double> pw, ip;
+  load_kinetics(*rec, &pw, &ip);
+  if (int rc = check_plausible(*rec)) return rc;
   trim_insertions(rec, &pw, &ip, ins_trim);
+  Clip clip;
+  if (int rc = check_trimmed(*rec, rec->cigar, rec->seq.size(), pw.size(), ip.size(), &clip, out->sn)) return rc;
   std::vector<int32_t> read_idx, ccs_idx;
   aligned_pairs(rec->cigar, rec->pos, &read_idx, &ccs_idx);
   const size_t aln = read_idx.size();
@@ -326,47 +399,19 @@ int expand_clip_indent(BamRecord* rec, int ins_trim, Read* out) {
   std::vector<uint8_t> npw(aln, 0), nip(aln, 0);
   const bool rev = rec->flag & 16;
   if (rev) { std::reverse(pw.begin(), pw.end()); std::reverse(ip.begin(), ip.end()); }
-  size_t nq = 0;
-  for (size_t i = 0; i < aln; ++i) nq += read_idx[i] >= 0;
-  if (nq != rec->seq.size()) return pfail(DCB_ERR_INVALID, "%s: cigar covers %zu query bases, sequence has %zu", rec->qname.c_str(), nq, rec->seq.size());
-  if (pw.size() != nq || ip.size() != nq) return pfail(DCB_ERR_INVALID, "%s: pw / ip tags do not match the sequence length", rec->qname.c_str());
   {
     size_t k = 0;
     for (size_t i = 0; i < aln; ++i)
-      if (read_idx[i] >= 0) { seq[i] = rec->seq[k]; npw[i] = (uint8_t)pw[k]; nip[i] = (uint8_t)ip[k]; ++k; }   // uint8 arrays (pre_lib.py:1166-1167)
+      if (read_idx[i] >= 0) { seq[i] = rec->seq[k]; npw[i] = kinetic_u8(pw[k]); nip[i] = kinetic_u8(ip[k]); ++k; }
   }
-  if (!rec->find("sn", &t) || t.type != 'B' || t.count < 4) return pfail(DCB_ERR_INVALID, "%s: no sn tag", rec->qname.c_str());
-  for (int i = 0; i < 4; ++i) out->sn[i] = (float)BamRecord::element(t, i);
   std::vector<uint8_t> cig;
-  size_t lead_soft = 0, trail_soft = 0;
   for (size_t ci = 0; ci < rec->cigar.size(); ++ci) {
     const int op = rec->cigar[ci] & 15;
     const size_t len = rec->cigar[ci] >> 4;
     if (op != kCHard) cig.insert(cig.end(), len, (uint8_t)op);
   }
-  {
-    // query_alignment_start / _end: query bases outside leading / trailing soft clips
-    size_t i = 0;
-    while (i < rec->cigar.size() && (rec->cigar[i] & 15) == kCHard) ++i;
-    if (i < rec->cigar.size() && (rec->cigar[i] & 15) == kCSoft) lead_soft = rec->cigar[i] >> 4;
-    size_t j = rec->cigar.size();
-    while (j > 0 && (rec->cigar[j - 1] & 15) == kCHard) --j;
-    if (j > 0 && (rec->cigar[j - 1] & 15) == kCSoft && j - 1 != i) trail_soft = rec->cigar[j - 1] >> 4;
-  }
-  if (cig.size() != aln) return pfail(DCB_ERR_INVALID, "%s: unsupported cigar operation (pad)", rec->qname.c_str());
-  bool any_soft = false;
-  for (uint8_t c : cig) any_soft |= c == kCSoft;
-  size_t qs = 0, qe = aln;
-  if (any_soft) {
-    for (size_t i = 0; i < aln; ++i) if (cig[i] == kCSoft) seq[i] = kGap;
-    const int32_t qstart = (int32_t)lead_soft, qlast = (int32_t)rec->seq.size() - (int32_t)trail_soft - 1;
-    bool f1 = false, f2 = false;
-    for (size_t i = 0; i < aln; ++i) {
-      if (!f1 && read_idx[i] == qstart) { qs = i; f1 = true; }
-      if (!f2 && read_idx[i] == qlast) { qe = i + 1; f2 = true; }
-    }
-    if (!f1 || !f2 || qe < qs) return pfail(DCB_ERR_INVALID, "%s: cannot locate the aligned part", rec->qname.c_str());
-  }
+  for (size_t i = 0; i < aln; ++i) if (cig[i] == kCSoft) seq[i] = kGap;
+  const size_t qs = clip.qs, qe = clip.qe;
   const size_t indent = rec->pos > 0 ? (size_t)rec->pos : 0;
   const size_t n = indent + (qe - qs);
   out->name = rec->qname;
@@ -441,6 +486,15 @@ inline float encode_base(char c) {          // dc_constants.SEQ_VOCAB = ' ATCG'
   switch (c) { case 'A': return 1.f; case 'T': return 2.f; case 'C': return 3.f; case 'G': return 4.f; default: return 0.f; }
 }
 
+// One ZMW's records before any construction, in the flat arrays of dcb_prep_get_records (include/dcb200.h)
+struct RawRecords {
+  std::vector<int32_t> meta;      // [n_subreads][DCB_READ_META]
+  std::vector<float> sn;          // [n_subreads][4]
+  std::vector<uint32_t> cigar;
+  std::vector<uint8_t> bases, pw, ip, ccs_bases, ccs_bq;
+  int32_t ccs_bq_any = 0;
+};
+
 // Everything derived from one ZMW (what a DcExample holds after space_out_subreads + the window list)
 struct ZmwState {
   std::vector<Read> reads;        // subreads..., ccs (spaced)
@@ -449,6 +503,7 @@ struct ZmwState {
   int has_ec = 0, has_np = 0, has_rq = 0, has_rg = 0;
   int32_t np_passes = 0, n_subreads = 0, ccs_length = 0;
   std::vector<int32_t> win_start; // column of every emitted window
+  RawRecords raw;                 // raw-record mode (dcb_prep_export_records): the records instead of `reads`
   int rc = DCB_OK;                // error of the processing step (message in `error`)
   std::string error;
 };
@@ -459,26 +514,112 @@ struct ZmwJob {
   std::string name;
 };
 
-struct PrepCfg { int P = 0, L = 0, bq = 0, ins_trim = 0, R = 0; dcb::PackedLayout pl{}; };
+struct PrepCfg { int P = 0, L = 0, bq = 0, ins_trim = 0, R = 0; bool records = false; dcb::PackedLayout pl{}; };
+
+// What trim_insertions would leave of a record, without building it: the trimmed cigar and the lengths of the trimmed
+// sequence and kinetics.  Follows trim_insertions to the letter: every operation but a deletion advances the sequence
+// position, substrings and the kinetics mask are cut at the end of the sequence, and the mask is read from the far end
+// for reverse-strand reads.
+void trimmed_shape(const BamRecord& r, size_t n_pw, size_t n_ip, int ins_trim, std::vector<uint32_t>* cig, size_t* seq_len,
+                   size_t* n_pw_out, size_t* n_ip_out) {
+  if (ins_trim <= 0) { *cig = r.cigar; *seq_len = r.seq.size(); *n_pw_out = n_pw; *n_ip_out = n_ip; return; }
+  const size_t n = r.seq.size();
+  std::vector<std::pair<size_t, size_t>> cut;   // masked [begin, end) of the sequence, ascending and disjoint
+  size_t sp = 0, kept = 0;
+  cig->clear();
+  for (uint32_t c : r.cigar) {
+    const int op = c & 15;
+    const size_t len = c >> 4;
+    if (op == kCIns && (int)len > ins_trim) {
+      if (sp < n) cut.emplace_back(sp, std::min(sp + len, n));
+      sp += len;
+    } else {
+      cig->push_back(c);
+      if (op != kCDel) { kept += std::min(len, n - std::min(sp, n)); sp += len; }
+    }
+  }
+  *seq_len = kept;
+  const bool rev = r.flag & 16;
+  auto filtered = [&](size_t nv) {
+    if (nv == 0) return (size_t)0;
+    const size_t m = std::min(nv, n), lo = rev ? n - m : 0, hi = rev ? n : m;   // the mask positions the tag reaches
+    size_t left = m;
+    for (const auto& iv : cut) {
+      const size_t a = std::max(iv.first, lo), b = std::min(iv.second, hi);
+      if (b > a) left -= b - a;
+    }
+    return left;
+  };
+  *n_pw_out = filtered(n_pw);
+  *n_ip_out = filtered(n_ip);
+}
+
+// Raw-record mode of process_zmw's per-subread step: the checks of expand_clip_indent, then the record as it is, with
+// the clip the checks located.  Nothing is written for a record that fails.
+int export_subread(const BamRecord& rec, int ins_trim, RawRecords* out) {
+  std::vector<double> pw, ip;
+  load_kinetics(rec, &pw, &ip);
+  if (int rc = check_plausible(rec)) return rc;
+  std::vector<uint32_t> cig;
+  size_t seq_len, n_pw, n_ip;
+  trimmed_shape(rec, pw.size(), ip.size(), ins_trim, &cig, &seq_len, &n_pw, &n_ip);
+  Clip clip;
+  float sn[4];
+  if (int rc = check_trimmed(rec, cig, seq_len, n_pw, n_ip, &clip, sn)) return rc;
+  // the construction kernels read the cigar as the SAM specification defines it; trim_insertions treats hard clips and
+  // reference skips as if they held query bases, which only a record without them is unaffected by
+  int64_t n_ins = 0;
+  for (uint32_t c : cig) {
+    const int op = c & 15;
+    if (op == kCHard || op == kCRefSkip)
+      return pfail(DCB_ERR_INVALID, "%s: hard clips / reference skips are not supported by the raw-record export", rec.qname.c_str());
+    if (op == kCIns) n_ins += c >> 4;
+  }
+  const size_t n = rec.seq.size();
+  const int32_t m[DCB_READ_META] = {(int32_t)out->cigar.size(), (int32_t)rec.cigar.size(), (int32_t)out->bases.size(), (int32_t)n,
+                                    rec.pos, (rec.flag & 16) ? 1 : 0, (int32_t)clip.qs, (int32_t)clip.qe, (int32_t)n_ins, 0};
+  out->meta.insert(out->meta.end(), m, m + DCB_READ_META);
+  out->sn.insert(out->sn.end(), sn, sn + 4);
+  out->cigar.insert(out->cigar.end(), rec.cigar.begin(), rec.cigar.end());
+  for (size_t i = 0; i < n; ++i) {
+    out->bases.push_back((uint8_t)encode_base(rec.seq[i]));
+    out->pw.push_back(i < pw.size() ? kinetic_u8(pw[i]) : 0);
+    out->ip.push_back(i < ip.size() ? kinetic_u8(ip[i]) : 0);
+  }
+  return DCB_OK;
+}
 
 // CPU-heavy part, no I/O: expand_clip_indent per subread, construct_ccs_read, space_out_subreads, window list
 void process_zmw(const PrepCfg& cfg, ZmwJob* job, ZmwState* st) {
   st->name = job->name;
   st->n_subreads = (int32_t)job->group.size();
   st->reads.clear();
-  st->reads.resize(job->group.size() + 1);
-  for (size_t i = 0; i < job->group.size(); ++i) {
-    const int rc = expand_clip_indent(&job->group[i], cfg.ins_trim, &st->reads[i]);
-    if (rc) { st->rc = rc; st->error = g_prep_error; return; }
-  }
   const BamRecord& c = job->ccs;
-  construct_ccs_read(c, &st->reads.back());
+  if (cfg.records) {
+    for (const BamRecord& r : job->group) {
+      const int rc = export_subread(r, cfg.ins_trim, &st->raw);
+      if (rc) { st->rc = rc; st->error = g_prep_error; st->raw = RawRecords(); return; }
+    }
+    for (size_t i = 0; i < c.seq.size(); ++i) {
+      st->raw.ccs_bases.push_back((uint8_t)encode_base(c.seq[i]));
+      st->raw.ccs_bq.push_back(c.qual[i]);
+      st->raw.ccs_bq_any |= c.qual[i] != 0;
+    }
+  } else {
+    st->reads.resize(job->group.size() + 1);
+    for (size_t i = 0; i < job->group.size(); ++i) {
+      const int rc = expand_clip_indent(&job->group[i], cfg.ins_trim, &st->reads[i]);
+      if (rc) { st->rc = rc; st->error = g_prep_error; return; }
+    }
+    construct_ccs_read(c, &st->reads.back());
+  }
   Tag t;
   st->has_ec = c.find("ec", &t); if (st->has_ec) st->ec = (float)BamRecord::scalar(t);
   st->has_np = c.find("np", &t); if (st->has_np) st->np_passes = (int32_t)BamRecord::scalar(t);
   st->has_rq = c.find("rq", &t); if (st->has_rq) st->rq = (float)BamRecord::scalar(t);
   st->has_rg = c.find("RG", &t) && t.type == 'Z'; if (st->has_rg) st->rg = reinterpret_cast<const char*>(t.p);
   st->ccs_length = (int32_t)c.seq.size();
+  if (cfg.records) return;
   space_out(st->reads);
   // DcExample.iter_examples (pre_lib.py:625-697), fixed-width windows
   const Read& ccs = st->reads.back();
@@ -669,6 +810,7 @@ int dcb_prep_next_zmw(dcb_prep* p, dcb_zmw_info* info) {
     p->cv_res.wait(lk, [&] { return p->results.count(p->next_seq) || (p->total >= 0 && p->next_seq >= p->total); });
     auto it = p->results.find(p->next_seq);
     if (it == p->results.end()) {
+      p->cur.raw = RawRecords();   // nothing to export after the end or an error
       if (p->reader_rc) { g_prep_error = p->reader_error; return p->reader_rc; }
       return 0;
     }
@@ -680,7 +822,7 @@ int dcb_prep_next_zmw(dcb_prep* p, dcb_zmw_info* info) {
   } else {
     ZmwJob job;
     const int rc = read_job(p, &job);
-    if (rc <= 0) return rc;
+    if (rc <= 0) { p->cur.raw = RawRecords(); return rc; }
     p->cur = ZmwState();
     process_zmw(p->cfg, &job, &p->cur);
     ++p->next_seq;
@@ -696,7 +838,7 @@ int dcb_prep_next_zmw(dcb_prep* p, dcb_zmw_info* info) {
   info->has_rq = st.has_rq; info->rq = st.rq;
   info->rg = st.has_rg ? st.rg.c_str() : nullptr;
   info->ccs_length = st.ccs_length;
-  info->spaced_width = (int32_t)st.reads.back().bases.size();
+  info->spaced_width = st.reads.empty() ? 0 : (int32_t)st.reads.back().bases.size();
   return 1;
 }
 
@@ -707,7 +849,7 @@ int dcb_prep_get_windows(dcb_prep* p, float* rows, uint8_t* packed, int32_t* win
                          int16_t* ccs_bq, int32_t* num_passes) {
   if (!p) return pfail(DCB_ERR_INVALID, "dcb_prep_get_windows: null handle");
   const ZmwState& st = p->cur;
-  if (st.reads.empty()) return pfail(DCB_ERR_STATE, "dcb_prep_get_windows: no ZMW loaded");
+  if (st.reads.empty()) return pfail(DCB_ERR_STATE, "dcb_prep_get_windows: no ZMW loaded (or the stream is in raw-record mode)");
   const PrepCfg& cf = p->cfg;
   const int L = cf.L, P = cf.P, R = cf.R;
   const size_t nsub = st.reads.size() - 1;
@@ -765,6 +907,32 @@ int dcb_prep_get_windows(dcb_prep* p, float* rows, uint8_t* packed, int32_t* win
     if (ccs_bq)
       for (int i = 0; i < L; ++i) ccs_bq[w * (size_t)L + i] = (int16_t)((i < n && ccs.bq_any) ? ccs.bq[s + i] : -1);
   }
+  return DCB_OK;
+}
+
+// Raw-record mode: dcb_prep_next_zmw decodes, validates and keeps the records of each ZMW for dcb_prep_get_records and
+// builds no windows (n_windows and spaced_width are 0).  Call before the first dcb_prep_next_zmw.
+int dcb_prep_export_records(dcb_prep* p, int32_t enabled) {
+  if (!p) return pfail(DCB_ERR_INVALID, "dcb_prep_export_records: null handle");
+  if (p->started || p->next_seq) return pfail(DCB_ERR_STATE, "dcb_prep_export_records: the stream has already started");
+  p->cfg.records = enabled != 0;
+  return DCB_OK;
+}
+
+// The loaded ZMW's records.  sizes (always written): subreads, cigar operations, query bases, CCS length, whether any
+// CCS base quality is non-zero.  Every array may be NULL (a first call with only `sizes` tells how to size them).
+int dcb_prep_get_records(dcb_prep* p, int64_t* sizes, int32_t* read_meta, float* read_sn, uint32_t* cigar,
+                         uint8_t* bases, uint8_t* pw, uint8_t* ip, uint8_t* ccs_bases, uint8_t* ccs_bq) {
+  if (!p || !sizes) return pfail(DCB_ERR_INVALID, "dcb_prep_get_records: null argument");
+  if (!p->cfg.records || p->cur.raw.meta.empty()) return pfail(DCB_ERR_STATE, "dcb_prep_get_records: no ZMW loaded in raw-record mode");
+  const RawRecords& r = p->cur.raw;
+  sizes[0] = (int64_t)(r.meta.size() / DCB_READ_META); sizes[1] = (int64_t)r.cigar.size(); sizes[2] = (int64_t)r.bases.size();
+  sizes[3] = (int64_t)r.ccs_bases.size(); sizes[4] = r.ccs_bq_any;
+  auto put = [](void* dst, const void* src, size_t bytes) { if (dst && bytes) memcpy(dst, src, bytes); };
+  put(read_meta, r.meta.data(), r.meta.size() * 4); put(read_sn, r.sn.data(), r.sn.size() * 4);
+  put(cigar, r.cigar.data(), r.cigar.size() * 4);
+  put(bases, r.bases.data(), r.bases.size()); put(pw, r.pw.data(), r.pw.size()); put(ip, r.ip.data(), r.ip.size());
+  put(ccs_bases, r.ccs_bases.data(), r.ccs_bases.size()); put(ccs_bq, r.ccs_bq.data(), r.ccs_bq.size());
   return DCB_OK;
 }
 

@@ -171,6 +171,20 @@ struct dcb_engine {
   struct { DevBuf<float> teacher, student, loss, grad; } ds;   // dcb_distill_loss, dcb_distill_loss_grad
   struct { DevBuf<float> probs, loss, grad, matches, dp; DevBuf<uint8_t> labels; } lg;   // dcb_alignment_loss_grad
   struct { DevBuf<float> bias, logits, probs; DevBuf<uint8_t> bases, quals; } he;   // dcb_debug_head_epilogue
+  // dcb_features_layout / dcb_features_pack: the uploaded records and the spaced state stay resident between the two
+  struct {
+    DevBuf<PrepZmw> zmw;
+    DevBuf<int32_t> meta, noni, gap, zmw_windows, window_pos, num_passes, list;
+    DevBuf<float> sn;
+    DevBuf<uint32_t> cigar;
+    DevBuf<uint8_t> bases, pw, ip, ccs_bases, ccs_bq, spaced, overflow, ccs_ids, packed;
+    DevBuf<int4> op_scan, zmw_out;
+    DevBuf<int2> win_list, window;
+    DevBuf<int16_t> out_bq;
+    DevBuf<int> status;
+    PrepBatch batch{};
+    int n_windows = -1;   // windows of the resident layout; -1: none
+  } fp;
   cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;   // around the kernel of dcb_evaluate / _distill_loss / _loss_grad
 
   // Safe on a partly built engine.  The caller has made cfg.device current; the DevBuf members free themselves after
@@ -1488,6 +1502,152 @@ int dcb_alignment_loss_grad(dcb_engine* e, const float* probs, const uint8_t* la
                          e->lg.dp, ctas, loss.d, grad.d, match.d, st));
   CU(e, cudaEventRecord(e->ev_eval1, st));
   if ((rc = copy_out(e, loss)) || (rc = copy_out(e, grad)) || (rc = copy_out(e, match))) return rc;
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  return DCB_OK;
+}
+
+// Spaced state one dcb_features_layout call may hold (bytes); a larger batch of ZMWs is split by the caller.
+static constexpr int64_t kPrepScratchMax = 1ll << 31;
+
+int dcb_features_layout(dcb_engine* e, const dcb_records* rec, int32_t ins_trim, int32_t max_windows, int32_t* zmw_windows,
+                        int32_t* window_pos, uint8_t* overflow, int16_t* ccs_bq, int32_t* num_passes, uint8_t* ccs_ids,
+                        int32_t* n_windows_out, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  auto& fp = e->fp;
+  fp.n_windows = -1;
+  if (!rec || !n_windows_out || rec->n_zmw < 0 || max_windows < 0) return fail(e, DCB_ERR_INVALID, "dcb_features_layout: bad argument");
+  *n_windows_out = 0;
+  if (ms_out) *ms_out = 0.f;
+  const int nz = rec->n_zmw;
+  if (nz == 0) { fp.n_windows = 0; return DCB_OK; }
+  if (!rec->zmw_read_off || !rec->zmw_ccs_off || !rec->zmw_ccs_bq_any || !rec->read_meta || !rec->read_sn || !zmw_windows ||
+      (max_windows && (!window_pos || !overflow || !ccs_bq || !num_passes || !ccs_ids)))
+    return fail(e, DCB_ERR_INVALID, "dcb_features_layout: null pointer");
+  if (e->pl.stride > 48 * 1024) return fail(e, DCB_ERR_INVALID, "dcb_features_layout: packed rows above 48 KB per window are not supported");
+  // Size everything from the records' own numbers; the kernel checks what it derives from the cigars against these
+  // bounds, so inconsistent records end in an error, never in a write outside the scratch.
+  const int L = e->L, P = e->cfg.max_passes;
+  const int n_reads = rec->zmw_read_off[nz], n_ccs = rec->zmw_ccs_off[nz];
+  if (rec->zmw_read_off[0] != 0 || rec->zmw_ccs_off[0] != 0 || n_reads < 0 || n_ccs < 0 || rec->n_cigar < 0 || rec->n_query < 0)
+    return fail(e, DCB_ERR_INVALID, "dcb_features_layout: bad offsets");
+  std::vector<PrepZmw> zmw(nz);
+  int64_t gap_total = 0, plane_total = 0, win_total = 0;
+  for (int z = 0; z < nz; ++z) {
+    PrepZmw& zm = zmw[z];
+    zm.read0 = rec->zmw_read_off[z];
+    zm.n_reads = rec->zmw_read_off[z + 1] - zm.read0;
+    zm.ccs_off = rec->zmw_ccs_off[z];
+    zm.ccs_len = rec->zmw_ccs_off[z + 1] - zm.ccs_off;
+    if (zm.read0 < 0 || zm.n_reads < 1 || zm.ccs_off < 0 || zm.ccs_len < 0 || zm.ccs_len > (1 << 24))
+      return fail(e, DCB_ERR_INVALID, "dcb_features_layout: ZMW %d needs at least one subread and non-decreasing offsets", z);
+    zm.keep = std::min(P, zm.n_reads);
+    zm.bq_any = rec->zmw_ccs_bq_any[z] != 0;
+    int64_t mb = zm.ccs_len, ins = 0;
+    for (int r = zm.read0; r < zm.read0 + zm.n_reads; ++r) {
+      const int32_t* m = rec->read_meta + (size_t)r * DCB_READ_META;
+      if (m[0] < 0 || m[1] < 0 || (int64_t)m[0] + m[1] > rec->n_cigar || m[2] < 0 || m[3] < 0 || (int64_t)m[2] + m[3] > rec->n_query ||
+          m[4] < 0 || m[4] > (1 << 24) || m[6] < 0 || m[7] < m[6] || m[7] > (1 << 24) || m[8] < 0 || m[8] > (1 << 24))
+        return fail(e, DCB_ERR_INVALID, "dcb_features_layout: read %d of ZMW %d has offsets or lengths out of range", r - zm.read0, z);
+      mb = std::max<int64_t>(mb, (int64_t)m[4] + (m[7] - m[6]));
+      ins += m[8];
+    }
+    const int64_t wb = (mb + ins + 15) / 16 * 16 + 16;
+    const int64_t bytes = wb * (3 * zm.keep + 3);
+    if (plane_total + bytes > kPrepScratchMax)
+      return fail(e, DCB_ERR_INVALID, "dcb_features_layout: the spaced reads of this batch need more than %lld bytes of scratch "
+                  "(ZMW %d alone: %lld); pass fewer ZMWs per call", (long long)kPrepScratchMax, z, (long long)bytes);
+    zm.mb = (int32_t)mb; zm.wb = (int32_t)wb;
+    zm.gap_off = gap_total; gap_total += mb + 2;
+    zm.plane_off = plane_total; plane_total += bytes;
+    zm.win_off = (int32_t)win_total; zm.win_cap = (int32_t)std::min<int64_t>((wb + L - 1) / L, std::max(zm.ccs_len, 1));
+    win_total += zm.win_cap;
+  }
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  PrepBatch& b = fp.batch;
+  b = PrepBatch{};
+  b.n_zmw = nz; b.ins_trim = ins_trim; b.pl = e->pl;
+  int rc;
+  if ((rc = stage_in(e, fp.zmw, (const PrepZmw*)zmw.data(), (size_t)nz, false, &b.zmw)) ||
+      (rc = stage_in(e, fp.meta, rec->read_meta, (size_t)n_reads * DCB_READ_META, false, &b.read_meta)) ||
+      (rc = stage_in(e, fp.sn, rec->read_sn, (size_t)n_reads * 4, false, &b.read_sn)) ||
+      (rc = stage_in(e, fp.cigar, rec->cigar, (size_t)rec->n_cigar, false, &b.cigar)) ||
+      (rc = stage_in(e, fp.bases, rec->bases, (size_t)rec->n_query, false, &b.bases)) ||
+      (rc = stage_in(e, fp.pw, rec->pw, (size_t)rec->n_query, false, &b.pw)) ||
+      (rc = stage_in(e, fp.ip, rec->ip, (size_t)rec->n_query, false, &b.ip)) ||
+      (rc = stage_in(e, fp.ccs_bases, rec->ccs_bases, (size_t)n_ccs, false, &b.ccs_bases)) ||
+      (rc = stage_in(e, fp.ccs_bq, rec->ccs_bq, (size_t)n_ccs, false, &b.ccs_bq)) ||
+      (rc = ensure(e, fp.op_scan, (size_t)rec->n_cigar + 1)) || (rc = ensure(e, fp.noni, (size_t)n_reads)) ||
+      (rc = ensure(e, fp.gap, (size_t)gap_total)) || (rc = ensure(e, fp.spaced, (size_t)plane_total)) ||
+      (rc = ensure(e, fp.win_list, (size_t)win_total)) || (rc = ensure(e, fp.zmw_out, (size_t)nz)) ||
+      (rc = ensure(e, fp.status, 1)) || (rc = ensure(e, fp.zmw_windows, (size_t)nz)) ||
+      (rc = ensure(e, fp.window, (size_t)win_total)) || (rc = ensure(e, fp.window_pos, (size_t)win_total)) ||
+      (rc = ensure(e, fp.overflow, (size_t)win_total)) || (rc = ensure(e, fp.num_passes, (size_t)win_total)) ||
+      (rc = ensure(e, fp.ccs_ids, (size_t)win_total * L)) || (rc = ensure(e, fp.out_bq, (size_t)win_total * L)))
+    return rc;
+  b.op_scan = fp.op_scan; b.read_noni_qs = fp.noni; b.gap = fp.gap; b.spaced = fp.spaced; b.win_list = fp.win_list;
+  b.zmw_out = fp.zmw_out; b.status = fp.status;
+  CU(e, cudaMemsetAsync(fp.status.p, 0, sizeof(int), st));
+  CU(e, cudaMemsetAsync(fp.gap.p, 0, (size_t)gap_total * sizeof(int32_t), st));
+  for (const PrepZmw& zm : zmw) {   // gaps: base 0, kinetics 0, CCS id 0, CCS quality -1
+    CU(e, cudaMemsetAsync(fp.spaced.p + zm.plane_off, 0, (size_t)zm.wb * (3 * zm.keep + 1), st));
+    CU(e, cudaMemsetAsync(fp.spaced.p + zm.plane_off + (size_t)zm.wb * (3 * zm.keep + 1), 0xff, (size_t)zm.wb * 2, st));
+  }
+  const PrepWindows out{fp.zmw_windows, fp.window, fp.window_pos, fp.overflow, fp.num_passes, fp.ccs_ids, fp.out_bq};
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  launch_prep_layout(b, out, st);
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  int status = 0;
+  CU(e, cudaMemcpyAsync(&status, fp.status.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(e, cudaMemcpyAsync(zmw_windows, fp.zmw_windows.p, (size_t)nz * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  if (status) return fail(e, DCB_ERR_INVALID, "dcb_features_layout: a record's cigar disagrees with the columns, query bases or "
+                          "insertion count its read_meta states");
+  int64_t n = 0;
+  for (int z = 0; z < nz; ++z) n += zmw_windows[z];
+  *n_windows_out = (int32_t)n;
+  if (n > max_windows) return fail(e, DCB_ERR_INVALID, "dcb_features_layout: %lld windows, max_windows is %d", (long long)n, max_windows);
+  if (n) {
+    CU(e, cudaMemcpyAsync(window_pos, fp.window_pos.p, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CU(e, cudaMemcpyAsync(overflow, fp.overflow.p, (size_t)n, cudaMemcpyDeviceToHost, st));
+    CU(e, cudaMemcpyAsync(num_passes, fp.num_passes.p, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CU(e, cudaMemcpyAsync(ccs_ids, fp.ccs_ids.p, (size_t)n * L, cudaMemcpyDeviceToHost, st));
+    CU(e, cudaMemcpyAsync(ccs_bq, fp.out_bq.p, (size_t)n * L * sizeof(int16_t), cudaMemcpyDeviceToHost, st));
+    CU(e, cudaStreamSynchronize(st));
+  }
+  fp.n_windows = (int)n;
+  return DCB_OK;
+}
+
+int dcb_features_pack(dcb_engine* e, const int32_t* windows, int32_t n, uint32_t flags, uint8_t* packed_out, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  auto& fp = e->fp;
+  if (ms_out) *ms_out = 0.f;
+  if (n < 0) return fail(e, DCB_ERR_INVALID, "dcb_features_pack: negative size");
+  if (fp.n_windows < 0) return fail(e, DCB_ERR_STATE, "dcb_features_pack before a successful dcb_features_layout");
+  if (n == 0) return DCB_OK;
+  if (!windows || !packed_out) return fail(e, DCB_ERR_INVALID, "dcb_features_pack: null pointer");
+  const bool out_dev = flags & DCB_OUT_ON_DEVICE;
+  if (out_dev && (reinterpret_cast<uintptr_t>(packed_out) & 15)) return fail(e, DCB_ERR_INVALID, "dcb_features_pack: device output must be 16-byte aligned");
+  for (int i = 0; i < n; ++i)
+    if (windows[i] < 0 || windows[i] >= fp.n_windows)
+      return fail(e, DCB_ERR_INVALID, "dcb_features_pack: window %d outside the layout's %d windows", windows[i], fp.n_windows);
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  const int32_t* d_list;
+  Output<uint8_t> packed;
+  int rc;
+  if ((rc = stage_in(e, fp.list, windows, (size_t)n, false, &d_list)) ||
+      (rc = stage_out(e, fp.packed, packed_out, (size_t)n * e->pl.stride, out_dev, &packed)))
+    return rc;
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  launch_prep_pack(fp.batch, fp.window, d_list, n, fp.n_windows, packed.d, st);
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  if ((rc = copy_out(e, packed))) return rc;
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));

@@ -52,6 +52,50 @@ void launch_fill_skipped(const uint8_t* ccs_ids, const int16_t* ccs_bq, const in
 // head_finish on final logits [n][5] (device pointer) into p.bases / p.quals / p.probs (dcb_debug_head_epilogue)
 void launch_head_epilogue(const float* logits, int n, const HeadParams& p, cudaStream_t st);
 
+// ---- feature construction from raw records (prep_kernels.cu); the record arrays are those of dcb_records
+// (include/dcb200.h), all pointers device pointers
+constexpr int kReadMeta = 10;   // DCB_READ_META
+struct PrepZmw {
+  int32_t read0, n_reads;     // its subreads in read_meta / read_sn
+  int32_t keep;               // min(max_passes, n_reads): the subreads that feed rows (all of them take part in spacing)
+  int32_t ccs_off, ccs_len, bq_any;
+  int32_t mb;                 // bound on any read's non-insertion columns: `gap` holds mb + 2 entries
+  int32_t wb;                 // bound on the spaced width, a multiple of 16
+  int32_t win_off, win_cap;   // its slice of win_list
+  int64_t gap_off;            // element offset into gap
+  int64_t plane_off;          // byte offset into spaced: u8 [keep][3][wb] base / pw / ip, u8 [wb] CCS ids, i16 [wb] CCS bq
+};
+struct PrepBatch {
+  int n_zmw, ins_trim;
+  PackedLayout pl;
+  const PrepZmw* zmw;
+  const int32_t* read_meta;
+  const float* read_sn;
+  const uint32_t* cigar;
+  const uint8_t *bases, *pw, *ip, *ccs_bases, *ccs_bq;
+  // scratch, kept from the layout to the pack calls
+  int4* op_scan;              // per cigar operation: columns, non-insertion columns, query bases before it, insertion run in front
+  int32_t* read_noni_qs;      // per read: non-insertion columns cut away in front of the clip
+  int32_t* gap;               // zeroed before the layout: the gap widths G, then their exclusive scan E
+  uint8_t* spaced;            // planes zeroed, CCS bq filled with -1 before the layout
+  int2* win_list;             // per ZMW: (start column, window_pos) of the windows that hold a CCS position
+  int4* zmw_out;              // per ZMW: spaced width, ccs_width, windows, largest non-insertion count
+  int* status;                // bit 0: records exceed the bounds they were sized by; bit 1: window index out of range
+};
+struct PrepWindows {          // dense over the batch, ZMW by ZMW
+  int32_t* zmw_windows;       // [n_zmw]
+  int2* window;               // (ZMW, start column)
+  int32_t* window_pos;
+  uint8_t* overflow;
+  int32_t* num_passes;
+  uint8_t* ccs_ids;           // [n][L]
+  int16_t* ccs_bq;            // [n][L]
+};
+void launch_prep_layout(const PrepBatch& b, const PrepWindows& out, cudaStream_t st);
+// packed rows of windows list[0..n_list) (indices into the layout's n_windows windows), in that order
+void launch_prep_pack(const PrepBatch& b, const int2* window, const int32_t* list, int n_list, int n_windows, uint8_t* packed,
+                      cudaStream_t st);
+
 // ---- evaluation on labelled windows (eval_kernels.cu): alignment loss, exact-match flag, alignment counts [B][5] of
 // the prediction and of the CCS row.  hard_min != 0: loss_reg None.  All pointers are device pointers.
 cudaError_t launch_evaluate(const float* probs, const uint8_t* labels, const uint8_t* ccs_ids, int B, int L,

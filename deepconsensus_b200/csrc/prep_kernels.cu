@@ -1,0 +1,311 @@
+// Feature construction on the device: what csrc/bam_prep.cpp does between the BAM decoder and the packed rows --
+// trim_insertions, expand_clip_indent, space_out_subreads, the window cut of DcExample.iter_examples and the packed-row
+// layout of extract_features (pre_lib.py:1061-1276,625-744) -- from the raw records dcb_prep_get_records hands out.
+// One CTA per ZMW, no atomics: every output byte is the host path's (tests/test_gpu_prep.py).
+//
+//   prep_layout_kernel   per ZMW: cigar scan per read, the spacing, the spaced planes of the reads that feed rows, the
+//                        spaced CCS read and the list of windows that hold a CCS position
+//   prep_emit_kernel     the per-window arrays of dcb_prep_get_windows except the rows, dense over the batch
+//   prep_pack_kernel     packed rows of the windows the caller lists, in the caller's order
+//
+// Spacing in closed form.  space_out (bam_prep.cpp; pre_lib.py:1242-1276) steps all reads in lock-step: while any read
+// that is not done has an insertion next, the reads with an insertion next advance by it and every other unfinished read
+// receives a gap; otherwise every unfinished read advances by one non-insertion column.  Every unfinished read grows by
+// exactly one spaced column per step, so all of them are at the same spaced column, and a step of the second kind
+// consumes the k-th non-insertion column of every read that still has one: the k-th non-insertion columns of all reads
+// share one spaced column.  Between the (k-1)-th and the k-th such step the automaton makes as many insertion steps as
+// the longest insertion run any read has in front of its k-th non-insertion column (a read's trailing insertions count
+// as the run in front of the column it does not have); a read that is done has no columns left and so contributes
+// nothing, and within the gap a read's own insertions come first because it advances while it can.  With
+//   run_r(k)  insertion columns of read r directly in front of its k-th non-insertion column
+//   G(k) = max_r run_r(k),   E(k) = sum_{k' < k} G(k')
+// the i-th insertion of that run lands in spaced column k + E(k) + i and the k-th non-insertion column in
+// k + E(k + 1); the spaced width is M + E(M + 1) for M the largest non-insertion count of any read.  (A read without
+// columns collects G(0) gaps before it is marked done, which the read owning that run reaches too, so the width holds.)
+#include "kernels.h"
+
+namespace dcb {
+namespace {
+
+constexpr int kPrepThreads = 512;
+constexpr unsigned kSat = 1u << 30;   // column counts saturate here; anything near it fails the bounds checks
+
+enum { kOpM = 0, kOpI = 1, kOpD = 2, kOpN = 3, kOpS = 4, kOpEq = 7, kOpX = 8 };
+
+__device__ __forceinline__ unsigned sat_add(unsigned a, unsigned b) { return min(a + b, kSat); }
+
+// Running state of the scan over one read's cigar operations, trimmed insertions already gone: alignment columns,
+// non-insertion columns and raw query bases before an operation, and the insertion columns directly in front of it.
+struct OpScan {
+  unsigned cols, noni, q, run, reset;
+};
+
+__device__ __forceinline__ OpScan op_identity() { return OpScan{0, 0, 0, 0, 0}; }
+
+__device__ __forceinline__ OpScan op_combine(const OpScan& a, const OpScan& b) {
+  return OpScan{sat_add(a.cols, b.cols), sat_add(a.noni, b.noni), sat_add(a.q, b.q),
+                b.reset ? b.run : sat_add(a.run, b.run), a.reset | b.reset};
+}
+
+__device__ __forceinline__ bool op_query(int op) { return op == kOpM || op == kOpI || op == kOpS || op == kOpEq || op == kOpX; }
+__device__ __forceinline__ bool op_column(int op) { return op_query(op) || op == kOpD || op == kOpN; }
+
+// trim_insertions: an insertion longer than ins_trim (> 0) has no column, but its query bases still count
+__device__ __forceinline__ OpScan op_element(uint32_t c, int ins_trim) {
+  const int op = c & 15;
+  const unsigned len = c >> 4;
+  const bool trimmed = op == kOpI && ins_trim > 0 && len > (unsigned)ins_trim;
+  OpScan e = op_identity();
+  e.q = op_query(op) ? len : 0;
+  if (trimmed || !op_column(op) || len == 0) return e;
+  e.cols = len;
+  if (op == kOpI) e.run = len;
+  else { e.noni = len; e.reset = 1; }
+  return e;
+}
+
+// Inclusive scan of one value per thread over the CTA (sh: kPrepThreads entries); returns the exclusive prefix of this
+// thread and leaves the inclusive values in sh.
+template <typename T, typename F>
+__device__ T block_scan(T v, T identity, T* sh, F combine) {
+  const int tid = threadIdx.x;
+  sh[tid] = v;
+  __syncthreads();
+  for (int d = 1; d < kPrepThreads; d <<= 1) {
+    const T x = tid >= d ? combine(sh[tid - d], sh[tid]) : sh[tid];
+    __syncthreads();
+    sh[tid] = x;
+    __syncthreads();
+  }
+  return tid ? sh[tid - 1] : identity;
+}
+
+// The last operation whose column offset is <= c: the one that holds alignment column c
+__device__ __forceinline__ int op_of_column(const int4* scan, int n, unsigned c) {
+  int lo = 0, hi = n;   // scan[lo].x <= c < scan[hi].x
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if ((unsigned)scan[mid].x <= c) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+__global__ void __launch_bounds__(kPrepThreads) prep_layout_kernel(PrepBatch b) {
+  __shared__ OpScan sh_op[kPrepThreads];
+  __shared__ int sh_int[kPrepThreads];
+  __shared__ unsigned s_noni_qs, s_noni_qe, s_tail;
+  __shared__ int s_mmax, s_bad;
+  const int tid = threadIdx.x, z = blockIdx.x;
+  const PrepZmw zm = b.zmw[z];
+  int* gap = b.gap + zm.gap_off;   // G, then E in place: zm.mb + 2 entries, zeroed by the caller
+  if (tid == 0) { s_mmax = zm.ccs_len; s_bad = 0; }
+  __syncthreads();
+
+  // ---- per read: scan the cigar, note where the clip falls, raise G by the read's insertion runs
+  for (int r = zm.read0; r < zm.read0 + zm.n_reads; ++r) {
+    const int* m = b.read_meta + (size_t)r * kReadMeta;
+    const int cig0 = m[0], ncig = m[1], indent = m[4];
+    const unsigned qs = m[6], qe = m[7];
+    const uint32_t* cig = b.cigar + cig0;
+    int4* scan = b.op_scan + cig0;
+    const int per = (ncig + kPrepThreads - 1) / kPrepThreads;
+    const int lo = min(tid * per, ncig), hi = min(lo + per, ncig);
+    OpScan agg = op_identity();
+    for (int o = lo; o < hi; ++o) agg = op_combine(agg, op_element(cig[o], b.ins_trim));
+    OpScan pre = block_scan(agg, op_identity(), sh_op, op_combine);
+    const OpScan total = sh_op[kPrepThreads - 1];
+    if (tid == 0) {
+      s_noni_qs = qs >= total.cols ? total.noni : 0;
+      s_noni_qe = total.noni;
+      s_tail = 0;
+      if (qe > total.cols || total.cols >= kSat || total.q > (unsigned)m[3]) s_bad = 1;
+    }
+    __syncthreads();
+    for (int o = lo; o < hi; ++o) {
+      const OpScan e = op_element(cig[o], b.ins_trim);
+      scan[o] = make_int4((int)pre.cols, (int)pre.noni, (int)pre.q, (int)pre.run);
+      if (e.cols) {
+        const unsigned c0 = pre.cols, c1 = pre.cols + e.cols;
+        if (qs >= c0 && qs < c1) s_noni_qs = pre.noni + (e.noni ? qs - c0 : 0);
+        if (qe >= c0 && qe < c1) s_noni_qe = pre.noni + (e.noni ? qe - c0 : 0);
+        if (qe > qs && qe - 1 >= c0 && qe - 1 < c1 && !e.noni) s_tail = pre.run + (qe - c0);
+      }
+      pre = op_combine(pre, e);
+    }
+    __syncthreads();
+    const unsigned noni_qs = s_noni_qs;
+    const long long m_r = (long long)indent + ((long long)s_noni_qe - noni_qs);
+    if (m_r < 0 || m_r > zm.mb) { if (tid == 0) s_bad = 1; }
+    else {
+      // a non-insertion operation that starts inside the clip: the run in front of its first column
+      OpScan p2 = tid ? sh_op[tid - 1] : op_identity();
+      for (int o = lo; o < hi; ++o) {
+        const OpScan e = op_element(cig[o], b.ins_trim);
+        if (e.noni && p2.run && p2.cols >= qs && p2.cols < qe) {
+          const int j = indent + (int)(p2.noni - noni_qs);
+          gap[j] = max(gap[j], (int)p2.run);
+        }
+        p2 = op_combine(p2, e);
+      }
+      if (tid == 0) {
+        gap[m_r] = max(gap[m_r], (int)s_tail);   // no operation starts at the read's m_r-th non-insertion column
+        s_mmax = max(s_mmax, (int)m_r);
+        b.read_noni_qs[r] = (int)noni_qs;
+      }
+    }
+    __syncthreads();
+  }
+  if (s_bad) { if (tid == 0) { *b.status |= 1; b.zmw_out[z] = make_int4(0, 0, 0, 0); } return; }
+
+  // ---- E = exclusive scan of G over [0, mmax + 1]
+  const int mmax = s_mmax, ne = mmax + 2;
+  {
+    const int per = (ne + kPrepThreads - 1) / kPrepThreads;
+    const int lo = min(tid * per, ne), hi = min(lo + per, ne);
+    int sum = 0;
+    for (int k = lo; k < hi; ++k) sum += k <= mmax ? gap[k] : 0;
+    int pre = block_scan(sum, 0, sh_int, [](int a, int c) { return a + c; });
+    for (int k = lo; k < hi; ++k) { const int g = k <= mmax ? gap[k] : 0; gap[k] = pre; pre += g; }
+  }
+  __syncthreads();
+  const int* E = gap;
+  const int width = mmax + E[mmax + 1];
+  if (width > zm.wb) { if (tid == 0) { *b.status |= 1; b.zmw_out[z] = make_int4(0, 0, 0, 0); } return; }
+
+  // ---- scatter the reads that feed rows into their spaced planes (zeroed by the caller: gaps)
+  uint8_t* planes = b.spaced + zm.plane_off;
+  for (int k = 0; k < zm.keep; ++k) {
+    const int r = zm.read0 + k;
+    const int* m = b.read_meta + (size_t)r * kReadMeta;
+    const int cig0 = m[0], ncig = m[1], q0 = m[2], nq = m[3], indent = m[4], rev = m[5];
+    const unsigned qs = m[6], qe = m[7];
+    const uint32_t* cig = b.cigar + cig0;
+    const int4* scan = b.op_scan + cig0;
+    const int noni_qs = b.read_noni_qs[r];
+    uint8_t* pb = planes + (size_t)k * 3 * zm.wb;
+    for (unsigned c = qs + tid; c < qe; c += kPrepThreads) {
+      const int o = op_of_column(scan, ncig, c);
+      const int4 s = scan[o];
+      const int op = cig[o] & 15;
+      const int i = (int)(c - (unsigned)s.x);
+      int col;
+      if (op == kOpI) { const int j = indent + s.y - noni_qs; col = j + E[j] + s.w + i; }
+      else { const int j = indent + s.y + i - noni_qs; col = j + E[j + 1]; }
+      if (!op_query(op)) continue;   // a deletion is a gap with zero kinetics
+      const int q = s.z + i;
+      const int kq = rev ? nq - 1 - q : q;   // the kinetics run along the read, the bases along the CCS
+      pb[col] = op == kOpS ? 0 : b.bases[q0 + q];
+      pb[zm.wb + col] = b.pw[q0 + kq];
+      pb[2 * zm.wb + col] = b.ip[q0 + kq];
+    }
+  }
+  // ---- the CCS read: every column is a match
+  uint8_t* ccs_ids = planes + (size_t)zm.keep * 3 * zm.wb;
+  int16_t* ccs_bq = reinterpret_cast<int16_t*>(ccs_ids + zm.wb);   // -1 from the caller's fill
+  for (int j = tid; j < zm.ccs_len; j += kPrepThreads) {
+    const int col = j + E[j + 1];
+    ccs_ids[col] = b.ccs_bases[zm.ccs_off + j];
+    if (zm.bq_any) ccs_bq[col] = b.ccs_bq[zm.ccs_off + j];   // pre_lib.py:247-250: all-zero qualities stay unspaced
+  }
+
+  // ---- windows of L columns over the CCS read's extent; one without a CCS position is dropped
+  const int L = b.pl.L;
+  const int ccs_width = zm.ccs_len ? zm.ccs_len - 1 + E[zm.ccs_len] + 1 : 0;
+  const int nwin = (ccs_width + L - 1) / L;
+  const int per = (nwin + kPrepThreads - 1) / kPrepThreads;
+  const int lo = min(tid * per, nwin), hi = min(lo + per, nwin);
+  auto first_ccs = [&](int start) {   // the first CCS position at or after spaced column `start`
+    int a = 0, c = zm.ccs_len;
+    while (a < c) { const int mid = (a + c) >> 1; if (mid + E[mid + 1] < start) a = mid + 1; else c = mid; }
+    return a;
+  };
+  int kept = 0;
+  for (int w = lo; w < hi; ++w) { const int j = first_ccs(w * L); kept += j < zm.ccs_len && j + E[j + 1] < w * L + L; }
+  int at = block_scan(kept, 0, sh_int, [](int a, int c) { return a + c; });
+  const int n_win = sh_int[kPrepThreads - 1];
+  if (n_win > zm.win_cap) { if (tid == 0) { *b.status |= 1; b.zmw_out[z] = make_int4(0, 0, 0, 0); } return; }
+  for (int w = lo; w < hi; ++w) {
+    const int j = first_ccs(w * L);
+    if (j < zm.ccs_len && j + E[j + 1] < w * L + L) { b.win_list[zm.win_off + at] = make_int2(w * L, j); ++at; }
+  }
+  if (tid == 0) b.zmw_out[z] = make_int4(width, ccs_width, n_win, mmax);
+}
+
+// Window base of ZMW z in the batch's dense window order
+__device__ __forceinline__ int window_base(const int4* zmw_out, int z) {
+  int base = 0;
+  for (int k = 0; k < z; ++k) base += zmw_out[k].z;
+  return base;
+}
+
+__global__ void __launch_bounds__(256) prep_emit_kernel(PrepBatch b, PrepWindows out) {
+  const int z = blockIdx.x;
+  const PrepZmw zm = b.zmw[z];
+  const int4 zo = b.zmw_out[z];
+  const int base = window_base(b.zmw_out, z), L = b.pl.L, width = zo.x;
+  const uint8_t* ccs_ids = b.spaced + zm.plane_off + (size_t)zm.keep * 3 * zm.wb;
+  const int16_t* ccs_bq = reinterpret_cast<const int16_t*>(ccs_ids + zm.wb);
+  if (threadIdx.x == 0) out.zmw_windows[z] = zo.z;
+  for (int w = threadIdx.x; w < zo.z; w += blockDim.x) {
+    const int2 wl = b.win_list[zm.win_off + w];
+    out.window[base + w] = make_int2(z, wl.x);
+    out.window_pos[base + w] = wl.y;
+    out.overflow[base + w] = 0;
+    out.num_passes[base + w] = zm.keep;
+  }
+  for (int t = threadIdx.x; t < zo.z * L; t += blockDim.x) {
+    const int w = t / L, i = t - w * L;
+    const int c = b.win_list[zm.win_off + w].x + i;
+    out.ccs_ids[(size_t)(base + w) * L + i] = c < width ? ccs_ids[c] : 0;
+    out.ccs_bq[(size_t)(base + w) * L + i] = c < width ? ccs_bq[c] : (int16_t)-1;
+  }
+}
+
+// One CTA per listed window: the packed row is assembled in shared memory and leaves in 16-byte stores.
+__global__ void __launch_bounds__(256) prep_pack_kernel(PrepBatch b, const int2* window, const int32_t* list, int n_windows,
+                                                        uint8_t* packed, int* status) {
+  extern __shared__ uint4 sh_row[];
+  uint8_t* row = reinterpret_cast<uint8_t*>(sh_row);
+  const int idx = list[blockIdx.x];
+  if (idx < 0 || idx >= n_windows) { if (threadIdx.x == 0) *status |= 2; return; }
+  const int2 wz = window[idx];
+  const PrepZmw zm = b.zmw[wz.x];
+  const int P = b.pl.P, L = b.pl.L, start = wz.y;
+  const int n = min(L, b.zmw_out[wz.x].x - start);   // columns present; the rest is padding
+  for (int t = threadIdx.x; t < b.pl.stride / 16; t += blockDim.x) sh_row[t] = make_uint4(0, 0, 0, 0);
+  __syncthreads();
+  const uint8_t* planes = b.spaced + zm.plane_off;
+  for (int t = threadIdx.x; t < zm.keep * L; t += blockDim.x) {
+    const int k = t / L, i = t - k * L;
+    const uint8_t* pb = planes + (size_t)k * 3 * zm.wb + start + i;
+    const int strand = b.read_meta[(size_t)(zm.read0 + k) * kReadMeta + 5] ? 2 : 1;
+    row[k * L + i] = (uint8_t)((i < n ? pb[0] : 0) | (strand << 3));
+    if (i < n) { row[(P + k) * L + i] = pb[zm.wb]; row[(2 * P + k) * L + i] = pb[2 * zm.wb]; }
+  }
+  const uint8_t* ccs_ids = planes + (size_t)zm.keep * 3 * zm.wb;
+  const int16_t* ccs_bq = reinterpret_cast<const int16_t*>(ccs_ids + zm.wb);
+  for (int i = threadIdx.x; i < L; i += blockDim.x) {
+    if (i < n) row[3 * P * L + i] = ccs_ids[start + i];
+    if (b.pl.bq) row[(3 * P + 1) * L + i] = (uint8_t)((i < n ? ccs_bq[start + i] : -1) + 1);
+  }
+  if (threadIdx.x < 4) reinterpret_cast<float*>(row + b.pl.sn_off)[threadIdx.x] = b.read_sn[(size_t)zm.read0 * 4 + threadIdx.x];
+  __syncthreads();
+  uint4* dst = reinterpret_cast<uint4*>(packed + (size_t)blockIdx.x * b.pl.stride);
+  for (int t = threadIdx.x; t < b.pl.stride / 16; t += blockDim.x) dst[t] = sh_row[t];
+}
+
+}  // namespace
+
+void launch_prep_layout(const PrepBatch& b, const PrepWindows& out, cudaStream_t st) {
+  if (b.n_zmw == 0) return;
+  prep_layout_kernel<<<b.n_zmw, kPrepThreads, 0, st>>>(b);
+  prep_emit_kernel<<<b.n_zmw, 256, 0, st>>>(b, out);
+}
+
+void launch_prep_pack(const PrepBatch& b, const int2* window, const int32_t* list, int n_list, int n_windows, uint8_t* packed,
+                      cudaStream_t st) {
+  if (n_list == 0) return;
+  prep_pack_kernel<<<n_list, 256, b.pl.stride, st>>>(b, window, list, n_windows, packed, b.status);
+}
+
+}  // namespace dcb

@@ -81,13 +81,24 @@ class DcbTensor(ctypes.Structure):
               ("ndim", ctypes.c_int32), ("shape", ctypes.c_int64 * 4)]
 
 
+READ_META = 10   # DCB_READ_META: int32 fields per subread in the raw records
+
+
+class DcbRecords(ctypes.Structure):
+  """dcb_records: the raw records of a batch of ZMWs (include/dcb200.h "feature construction on the device")."""
+  _fields_ = [("n_zmw", ctypes.c_int32), ("n_cigar", ctypes.c_int32), ("n_query", ctypes.c_int32), ("reserved", ctypes.c_int32)] + [
+      (k, ctypes.c_void_p) for k in ("zmw_read_off", "zmw_ccs_off", "zmw_ccs_bq_any", "read_meta", "read_sn", "cigar", "bases",
+                                     "pw", "ip", "ccs_bases", "ccs_bq")]
+
+
 # Every symbol include/dcb200.h declares; tests check the built library exports all of them.
 ABI_SYMBOLS = (
     "dcb_create", "dcb_load_weights", "dcb_forward", "dcb_submit", "dcb_wait", "dcb_stitch", "dcb_last_forward_ms",
     "dcb_packed_window_bytes", "dcb_pack_rows", "dcb_forward_packed", "dcb_submit_packed",
     "dcb_stitch_fastq", "dcb_skip_mask", "dcb_fill_skipped", "dcb_evaluate", "dcb_distill_loss",
     "dcb_alignment_loss_grad", "dcb_distill_loss_grad", "dcb_prep_open", "dcb_prep_set_threads", "dcb_prep_next_zmw", "dcb_prep_get_windows", "dcb_prep_ccs_header", "dcb_prep_close",
-    "dcb_prep_last_error", "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
+    "dcb_prep_last_error", "dcb_prep_export_records", "dcb_prep_get_records", "dcb_features_layout", "dcb_features_pack",
+    "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
     "dcb_last_forward_launches", "dcb_set_profile", "dcb_get_profile", "dcb_get_profile_kernels", "dcb_alloc_host",
     "dcb_free_host", "dcb_alloc_device", "dcb_free_device", "dcb_memcpy_h2d", "dcb_memcpy_d2h",
     "dcb_synchronize", "dcb_last_error", "dcb_version", "dcb_destroy",
@@ -150,6 +161,9 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_distill_loss_grad.argtypes = [vp, vp, vp, i32, i32, f64, i32, u32, vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_alignment_loss_grad.argtypes = [vp, vp, vp, i32, i32, f64, f64, i32, u32, vp, vp, vp,
                                           ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_features_layout.argtypes = [vp, ctypes.POINTER(DcbRecords), i32, i32, vp, vp, vp, vp, vp, vp, ctypes.POINTER(i32),
+                                      ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_features_pack.argtypes = [vp, vp, i32, u32, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_launches.argtypes = [vp, ctypes.POINTER(i32)]
   lib.dcb_set_debug.argtypes = [vp, i32]
@@ -558,6 +572,49 @@ class B200Model:
                                            float(cal.b) if en else 0.0, DCB_OUT_ON_DEVICE if on_device else 0,
                                            _ptr(bases), _ptr(quals)))
 
+  # -- feature construction on the device (include/dcb200.h "feature construction on the device") -----------------
+  def features_layout(self, records: Dict[str, np.ndarray], ins_trim: int = 5) -> Dict[str, Any]:
+    """dcb_features_layout (phase A) on a batch of raw records (`concat_records` of
+    `preprocess.BamFeatureStream.next_zmw_records()` bundles): spaces the reads of every ZMW on the device and returns
+    what dcb_prep_get_windows returns apart from the rows, dense over the batch -- dict(zmw_windows [n_zmw], window_pos
+    [n], overflow [n], num_passes [n], ccs_bq int16 [n, L], ccs_ids uint8 [n, L], ms).  The spaced reads stay on the
+    device for features_pack."""
+    L = self.max_length
+    spec = dict(zmw_read_off=np.int32, zmw_ccs_off=np.int32, zmw_ccs_bq_any=np.int32, read_meta=np.int32, read_sn=np.float32,
+                cigar=np.uint32, bases=np.uint8, pw=np.uint8, ip=np.uint8, ccs_bases=np.uint8, ccs_bq=np.uint8)
+    held = {k: _arg(records[k], dt) for k, dt in spec.items()}
+    rec = DcbRecords(n_zmw=len(held["zmw_ccs_bq_any"][1]), n_cigar=held["cigar"][1].size, n_query=held["bases"][1].size)
+    for k, (ptr, _) in held.items():
+      setattr(rec, k, ptr)
+    # a capacity that always suffices: the spaced width is at most the longest read plus every insertion column
+    meta = held["read_meta"][1].reshape(-1, READ_META)
+    ro = held["zmw_read_off"][1]
+    cap = 0
+    for z in range(rec.n_zmw):
+      m = meta[ro[z]:ro[z + 1]]
+      longest = max(int(np.diff(held["zmw_ccs_off"][1])[z]), int((m[:, 4] + m[:, 7] - m[:, 6]).max(initial=0)))
+      cap += (longest + int(m[:, 8].sum()) + 32 + L - 1) // L
+    out = dict(zmw_windows=np.zeros(rec.n_zmw, np.int32), window_pos=np.zeros(cap, np.int32), overflow=np.zeros(cap, np.uint8),
+               ccs_bq=np.zeros((cap, L), np.int16), num_passes=np.zeros(cap, np.int32), ccs_ids=np.zeros((cap, L), np.uint8))
+    n, ms = ctypes.c_int32(0), ctypes.c_float(0)
+    self._check(self._lib.dcb_features_layout(self._handle, ctypes.byref(rec), int(ins_trim), cap, _ptr(out["zmw_windows"]),
+                                              _ptr(out["window_pos"]), _ptr(out["overflow"]), _ptr(out["ccs_bq"]),
+                                              _ptr(out["num_passes"]), _ptr(out["ccs_ids"]), ctypes.byref(n), ctypes.byref(ms)))
+    res: Dict[str, Any] = {k: (v if k == "zmw_windows" else v[:n.value]) for k, v in out.items()}
+    res["ms"] = float(ms.value)
+    return res
+
+  def features_pack(self, windows: np.ndarray, out: Optional[int] = None) -> Dict[str, Any]:
+    """dcb_features_pack (phase B): packed rows of the listed windows of the last features_layout, in the list's order.
+    Returns dict(packed uint8 [k, packed_window_bytes], ms); with `out`, a 16-byte-aligned device address, the rows are
+    written there (ready for forward_packed_raw with DCB_ROWS_ON_DEVICE) and `packed` is None."""
+    idx = np.ascontiguousarray(windows, dtype=np.int32).reshape(-1)
+    packed = None if out is not None else np.empty((len(idx), self.packed_window_bytes), np.uint8)
+    ms = ctypes.c_float(0)
+    self._check(self._lib.dcb_features_pack(self._handle, _ptr(idx), len(idx), DCB_OUT_ON_DEVICE if out is not None else 0,
+                                            _ptr(out) if out is not None else _ptr(packed), ctypes.byref(ms)))
+    return dict(packed=packed, ms=float(ms.value))
+
   def stitch_raw(self, bases_ptr: int, quals_ptr: int, n_windows: int, zmw_start: np.ndarray, flags: int,
                  seq_ptr: int, qual_ptr: int, len_ptr: int, length: Optional[int] = None) -> None:
     """dcb_stitch on caller-managed pointers (host or device per `flags`)."""
@@ -858,6 +915,27 @@ def pack_rows(params: params_lib.Params, rows: np.ndarray, out: Optional[np.ndar
   if rc and not (rc == -5 and not strict_input):
     raise DcbError(rc, lib.dcb_last_error(None).decode())
   return out
+
+
+def concat_records(zmws: List[Dict[str, Any]]) -> Dict[str, np.ndarray]:
+  """The raw-record bundles of `preprocess.BamFeatureStream.next_zmw_records()` as one dcb_records batch: arrays
+  concatenated, per-read offsets shifted, per-ZMW offsets added."""
+  cig0 = np.cumsum([0] + [len(z["cigar"]) for z in zmws])
+  q0 = np.cumsum([0] + [len(z["bases"]) for z in zmws])
+  meta = []
+  for k, z in enumerate(zmws):
+    m = np.array(z["read_meta"], np.int32).reshape(-1, READ_META)
+    m[:, 0] += cig0[k]
+    m[:, 2] += q0[k]
+    meta.append(m)
+  cat = lambda key, dt, tail=(): (np.concatenate([np.asarray(z[key], dt).reshape((-1,) + tail) for z in zmws])
+                                  if zmws else np.zeros((0,) + tail, dt))
+  return dict(zmw_read_off=np.cumsum([0] + [len(m) for m in meta]).astype(np.int32),
+              zmw_ccs_off=np.cumsum([0] + [len(z["ccs_bases"]) for z in zmws]).astype(np.int32),
+              zmw_ccs_bq_any=np.array([int(z["ccs_bq_any"]) for z in zmws], np.int32),
+              read_meta=np.concatenate(meta) if meta else np.zeros((0, READ_META), np.int32),
+              read_sn=cat("read_sn", np.float32, (4,)), cigar=cat("cigar", np.uint32), bases=cat("bases", np.uint8),
+              pw=cat("pw", np.uint8), ip=cat("ip", np.uint8), ccs_bases=cat("ccs_bases", np.uint8), ccs_bq=cat("ccs_bq", np.uint8))
 
 
 def pipelined(items: Iterable[Any], submit: Callable[[Any], Any], wait: Callable[[Any], Any],

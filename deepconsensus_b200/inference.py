@@ -253,22 +253,71 @@ def inference_on_packed_zmws(zmws: List[Dict[str, Any]], model: engine_lib.B200M
   Returns (fastq bytes, rec_off, passed, names): read z (sorted-name order) has the record
   fastq[rec_off[z]:rec_off[z + 1]] when passed[z].
   """
-  from deepconsensus_b200 import stitch_gpu
   L, P = int(model_params.max_length), int(model_params.max_passes)
   zmws = [z for z in zmws if len(z["window_pos"])]
   if not zmws:
     return b"", np.zeros(1, np.int64), np.zeros(0, bool), []
   packed = np.concatenate([z["packed"] for z in zmws])
-  pos = np.concatenate([z["window_pos"] for z in zmws]).astype(np.int64)
-  bq = np.concatenate([z["ccs_bq"] for z in zmws])
-  skip = np.concatenate([z["overflow"] for z in zmws]).astype(bool)
-  counts = np.array([len(z["window_pos"]) for z in zmws])
-  names_z = [z["name"] for z in zmws]
+
+  def score(idx):
+    out = model.forward_packed(packed[idx])
+    return out["bases"], out["quals"]
+
+  return _skip_score_stitch(
+      model, model_params, options, outcome_counter, [z["name"] for z in zmws], np.array([len(z["window_pos"]) for z in zmws]),
+      np.concatenate([z["window_pos"] for z in zmws]).astype(np.int64), np.concatenate([z["ccs_bq"] for z in zmws]),
+      np.concatenate([z["overflow"] for z in zmws]).astype(bool), score,
+      lambda skipped: packed[skipped][:, 3 * P * L:3 * P * L + L])    # the CCS plane of the packed rows
+
+
+def inference_on_record_zmws(zmws: List[Dict[str, Any]], model: engine_lib.B200Model, model_params: params_lib.Params,
+                             options: InferenceOptions, outcome_counter: stitch_utils.OutcomeCounter, ins_trim: int = 5,
+                             stats: Optional[Dict[str, Any]] = None) -> Tuple[bytes, np.ndarray, np.ndarray, List[str]]:
+  """`inference_on_packed_zmws` with the feature construction on the device: `zmws` are the raw-record bundles of
+  `preprocess.BamFeatureStream.next_zmw_records()`.  dcb_features_layout spaces the reads and returns what the skip
+  decision needs; rows are laid out (dcb_features_pack) only for the windows the model scores, in device memory that
+  dcb_forward_packed reads in place; skipped windows take their CCS ids and qualities from the layout.  Same return
+  value, and the same bytes, as `inference_on_packed_zmws` on the host-built windows of the same ZMWs.  `stats`, when
+  given, accumulates "windows" and "windows_skipped"."""
+  if not zmws:
+    return b"", np.zeros(1, np.int64), np.zeros(0, bool), []
+  lay = model.features_layout(engine_lib.concat_records(zmws), ins_trim)
+  counts = lay["zmw_windows"]
+  if stats is not None:
+    stats["windows"] = stats.get("windows", 0) + int(counts.sum())
+  has = np.nonzero(counts)[0]
+  if not len(has):
+    return b"", np.zeros(1, np.int64), np.zeros(0, bool), []
+  rows_dev = model.alloc_device(options.batch_size * model.packed_window_bytes)
+
+  def score(idx):
+    bases, quals = np.empty((len(idx), model.max_length), np.uint8), np.empty((len(idx), model.max_length), np.uint8)
+    model.features_pack(idx, out=rows_dev)
+    model.forward_packed_raw(rows_dev, len(idx), engine_lib.DCB_ROWS_ON_DEVICE, bases.ctypes.data, quals.ctypes.data)
+    return bases, quals
+
+  try:
+    return _skip_score_stitch(model, model_params, options, outcome_counter, [zmws[k]["name"] for k in has], counts[has],
+                              lay["window_pos"].astype(np.int64), lay["ccs_bq"], lay["overflow"].astype(bool), score,
+                              lambda skipped: lay["ccs_ids"][skipped], stats)
+  finally:
+    model.free_device(rows_dev)
+
+
+def _skip_score_stitch(model, model_params, options, outcome_counter, names_z, counts, pos, bq, skip, score, ccs_ids_of,
+                       stats=None):
+  """The part of `inference_on_n_zmws` behind the features, for windows given as arrays (ZMW k owns counts[k]
+  consecutive windows): skip decision, `score(window indices) -> (bases, quals)` for the rest in batches of
+  options.batch_size, skipped-window fill from `ccs_ids_of(window indices)`, sort and stitch."""
+  from deepconsensus_b200 import stitch_gpu
+  L = int(model_params.max_length)
   n = len(pos)
   if options.skip_windows_above:
-    skip |= skip_decisions(model, bq, options.skip_windows_above)
+    skip = skip | skip_decisions(model, bq, options.skip_windows_above)
+  if stats is not None:
+    stats["windows_skipped"] = stats.get("windows_skipped", 0) + int(skip.sum())
   # sort by (name, window_pos): ZMW order by name, windows inside a ZMW by position (quick_inference.py:721-728)
-  zorder = sorted(range(len(zmws)), key=lambda k: names_z[k])
+  zorder = sorted(range(len(names_z)), key=lambda k: names_z[k])
   starts = np.concatenate([[0], np.cumsum(counts)])
   order = np.concatenate([starts[k] + np.argsort(pos[starts[k]:starts[k + 1]], kind="stable") for k in zorder])
   dest = np.empty(n, np.int64)
@@ -277,12 +326,10 @@ def inference_on_packed_zmws(zmws: List[Dict[str, Any]], model: engine_lib.B200M
   scored = np.nonzero(~skip)[0]
   for b0 in range(0, len(scored), options.batch_size):          # batch_examples (quick_inference.py:304-338)
     idx = scored[b0:b0 + options.batch_size]
-    out = model.forward_packed(packed[idx])
-    all_b[dest[idx]], all_q[dest[idx]] = out["bases"], out["quals"]
+    all_b[dest[idx]], all_q[dest[idx]] = score(idx)
   skipped = np.nonzero(skip)[0]
   if len(skipped):
-    ccs_ids = packed[skipped][:, 3 * P * L:3 * P * L + L]        # the CCS plane of the packed rows
-    model.fill_skipped(ccs_ids, bq[skipped], dest[skipped].astype(np.int32), all_b, all_q,
+    model.fill_skipped(ccs_ids_of(skipped), bq[skipped], dest[skipped].astype(np.int32), all_b, all_q,
                        calibration=options.ccs_calibration_values)
   names_sorted = [names_z[k] for k in zorder for _ in range(counts[k])]
   fastq, rec_off, passed = stitch_gpu.stitch_batch_to_fastq_bytes(model, all_b, all_q, names_sorted, pos[order].tolist(), L,

@@ -43,6 +43,8 @@ def _lib():
     lib.dcb_prep_set_threads.argtypes = [vp, i32]
     lib.dcb_prep_next_zmw.argtypes = [vp, ctypes.POINTER(DcbZmwInfo)]
     lib.dcb_prep_get_windows.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    lib.dcb_prep_export_records.argtypes = [vp, i32]
+    lib.dcb_prep_get_records.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.dcb_prep_ccs_header.argtypes = [vp]
     lib.dcb_prep_ccs_header.restype = ctypes.c_char_p
     lib.dcb_prep_close.argtypes = [vp]
@@ -60,9 +62,11 @@ class BamFeatureStream:
   iter_examples, pre_lib.py:1279-1384,625-697)."""
 
   def __init__(self, subreads_to_ccs: str, ccs_bam: str, max_passes: int, max_length: int, use_ccs_bq: bool = False,
-               ins_trim: int = 5, threads: int = 0):
+               ins_trim: int = 5, threads: int = 0, records: bool = False):
     """threads > 0: ZMWs are processed by that many native worker threads (plus one BAM-decoding thread) while the
-    caller consumes them; the order of the ZMWs is the file's either way (`--cpus` of `deepconsensus run`)."""
+    caller consumes them; the order of the ZMWs is the file's either way (`--cpus` of `deepconsensus run`).
+    records: the stream only decodes and validates, and hands each ZMW out as raw records (`next_zmw_records`) for
+    feature construction on the device; `next_zmw` is not available then."""
     self._lib = _lib()
     self._h = ctypes.c_void_p()
     self.max_passes, self.max_length, self.use_ccs_bq = int(max_passes), int(max_length), bool(use_ccs_bq)
@@ -72,6 +76,9 @@ class BamFeatureStream:
     if rc:
       raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
     if threads > 0 and self._lib.dcb_prep_set_threads(self._h, int(threads)):
+      raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
+    self.records = bool(records)
+    if records and self._lib.dcb_prep_export_records(self._h, 1):
       raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
     self._stride = ((3 * self.max_passes + 1 + int(self.use_ccs_bq)) * self.max_length + 15) // 16 * 16 + 16   # PackedLayout
 
@@ -120,6 +127,35 @@ class BamFeatureStream:
                                         vp(out["packed"]) if want_packed else None, vp(out["window_pos"]),
                                         vp(out["overflow"]), vp(out["ccs_bq"]), vp(out["num_passes"]))
     if rc:
+      raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
+    return out
+
+  def next_zmw_records(self) -> Optional[Dict[str, Any]]:
+    """The next ZMW as raw records (dcb_prep_get_records, include/dcb200.h): dict(name, n_subreads, ec, np_num_passes,
+    rq, rg, read_meta int32 [n, 10], read_sn float32 [n, 4], cigar uint32, bases / pw / ip uint8 per query base,
+    ccs_bases / ccs_bq uint8, ccs_bq_any); None at EOF.  Needs `records=True`."""
+    info = DcbZmwInfo()
+    rc = self._lib.dcb_prep_next_zmw(self._h, ctypes.byref(info))
+    if rc < 0:
+      raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
+    if rc == 0:
+      return None
+    out: Dict[str, Any] = dict(name=info.name.decode("utf-8", "replace"), n_subreads=int(info.n_subreads),
+                               ec=float(info.ec) if info.has_ec else None,
+                               np_num_passes=int(info.np_num_passes) if info.has_np else None,
+                               rq=float(info.rq) if info.has_rq else None,
+                               rg=info.rg.decode("utf-8", "replace") if info.rg else None)
+    sizes = np.zeros(5, np.int64)
+    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    if self._lib.dcb_prep_get_records(self._h, vp(sizes), *([None] * 8)):
+      raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
+    n, n_cig, n_q, n_ccs = (int(x) for x in sizes[:4])
+    out.update(read_meta=np.zeros((n, engine_lib.READ_META), np.int32), read_sn=np.zeros((n, 4), np.float32),
+               cigar=np.zeros(n_cig, np.uint32), bases=np.zeros(n_q, np.uint8), pw=np.zeros(n_q, np.uint8),
+               ip=np.zeros(n_q, np.uint8), ccs_bases=np.zeros(n_ccs, np.uint8), ccs_bq=np.zeros(n_ccs, np.uint8),
+               ccs_bq_any=bool(sizes[4]))
+    if self._lib.dcb_prep_get_records(self._h, vp(sizes), *(vp(out[k]) for k in (
+        "read_meta", "read_sn", "cigar", "bases", "pw", "ip", "ccs_bases", "ccs_bq"))):
       raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
     return out
 

@@ -4,7 +4,8 @@ BAM + CCS BAM in, polished reads (FASTQ or unaligned BAM) out.
   python -m deepconsensus_b200.run --subreads_to_ccs S.bam --ccs_bam C.bam --checkpoint model_dir/checkpoint-50 \\
          --output out.fastq [--batch_zmws 100 --batch_size 1024 --min_quality 20 --skip_windows_above 45 ...]
 
-Stages (all but the driver loop in native code): feature construction from BAM (csrc/bam_prep.cpp), skip decision,
+Stages (all but the driver loop in native code): feature construction from BAM (csrc/bam_prep.cpp; with
+`--features gpu` only the decoding stays there and csrc/prep_kernels.cu builds the windows), skip decision,
 model, skipped-window fill, sort, stitch + filters + FASTQ bytes (CUDA, `inference.inference_on_zmw_windows`), output
 writer (FASTQ text or BGZF/BAM, csrc/bam_prep.cpp).  `--checkpoint` is a TF2 checkpoint (read without TensorFlow), a
 directory, or an .npz; params.json is read from next to it.  `--random_weights SEED` replaces the variables by seeded
@@ -30,9 +31,13 @@ from deepconsensus_b200 import weights as weights_lib
 def run(subreads_to_ccs: str, ccs_bam: str, checkpoint: str, output: str, batch_zmws: int = 100, batch_size: int = 1024,
         min_quality: int = 20, min_length: int = 0, skip_windows_above: int = 45, ins_trim: int = 5,
         max_base_quality: int = 93, dc_calibration: Optional[str] = None, ccs_calibration: str = "skip",
-        limit: int = 0, random_weights: Optional[int] = None, precision: str = "bf16", device: int = 0, cpus: int = 0
-        ) -> stitch_utils.OutcomeCounter:
-  """One inference run; returns the OutcomeCounter (quick_inference.run's return value)."""
+        limit: int = 0, random_weights: Optional[int] = None, precision: str = "bf16", device: int = 0, cpus: int = 0,
+        features: str = "host") -> stitch_utils.OutcomeCounter:
+  """One inference run; returns the OutcomeCounter (quick_inference.run's return value).  features: "host" builds
+  every window in csrc/bam_prep.cpp; "gpu" has the stream only decode and validate, and builds the windows on the
+  device, rows only for the windows the model scores (csrc/prep_kernels.cu).  Same output either way."""
+  if features not in ("host", "gpu"):
+    raise ValueError("features must be 'host' or 'gpu'")
   params = params_lib.read_params_from_json(checkpoint)
   if dc_calibration is None:
     dc_calibration = params.get("dc_calibration", "skip")                      # quick_inference.py:817-831
@@ -49,7 +54,7 @@ def run(subreads_to_ccs: str, ccs_bam: str, checkpoint: str, output: str, batch_
   model, params = inference.initialize_model(checkpoint, params, options, weights=weights, device=device, precision=precision)
   counter = stitch_utils.OutcomeCounter()
   stream = preprocess.BamFeatureStream(subreads_to_ccs, ccs_bam, options.max_passes, options.max_length,
-                                       options.use_ccs_bq, ins_trim, threads=cpus)
+                                       options.use_ccs_bq, ins_trim, threads=cpus, records=features == "gpu")
   as_bam = output.endswith(".bam")
   writer: Any = preprocess.BamWriter(output, stream.ccs_header) if as_bam else open(output, "wb")
   stats = dict(zmws=0, windows=0, seconds_features=0.0, seconds_model_and_stitch=0.0)
@@ -59,7 +64,7 @@ def run(subreads_to_ccs: str, ccs_bam: str, checkpoint: str, output: str, batch_
       t0 = time.time()
       batch = []                      # per-ZMW array bundles: packed rows + metadata, no per-window objects
       while len(batch) < batch_zmws:
-        z = stream.next_zmw(want_rows=False, want_packed=True)
+        z = stream.next_zmw_records() if features == "gpu" else stream.next_zmw(want_rows=False, want_packed=True)
         if z is None or (limit and stats["zmws"] + len(batch) >= limit):
           done = True
           break
@@ -68,10 +73,13 @@ def run(subreads_to_ccs: str, ccs_bam: str, checkpoint: str, output: str, batch_
       if not batch:
         break
       t0 = time.time()
-      fastq, rec_off, passed, names = inference.inference_on_packed_zmws(batch, model, params, options, counter)
+      if features == "gpu":
+        fastq, rec_off, passed, names = inference.inference_on_record_zmws(batch, model, params, options, counter, ins_trim, stats)
+      else:
+        fastq, rec_off, passed, names = inference.inference_on_packed_zmws(batch, model, params, options, counter)
+        stats["windows"] += sum(len(z["window_pos"]) for z in batch)
       stats["seconds_model_and_stitch"] += time.time() - t0
       stats["zmws"] += len(batch)
-      stats["windows"] += sum(len(z["window_pos"]) for z in batch)
       tags = {z["name"]: z for z in batch}
       if as_bam:
         for k, name in enumerate(names):
@@ -113,6 +121,9 @@ def main(argv: Optional[List[str]] = None) -> None:
   ap.add_argument("--random_weights", type=int, default=None)
   ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
   ap.add_argument("--cpus", type=int, default=0, help="native feature-construction threads (0: on the calling thread)")
+  ap.add_argument("--features", default="host", choices=["host", "gpu"],
+                  help="where windows are built from the decoded BAM records: host C++, or CUDA kernels that lay rows out "
+                       "only for the windows the model scores")
   a = ap.parse_args(argv)
   c = run(**vars(a))
   print(json.dumps(c.__dict__))

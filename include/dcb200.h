@@ -325,6 +325,32 @@ int dcb_prep_next_zmw(dcb_prep* p, dcb_zmw_info* info);   /* 1 = a ZMW is loaded
  * window_pos / num_passes int32 [n]; overflow u8 [n]; ccs_bq int16 [n, L] (-1 at gaps and padding). */
 int dcb_prep_get_windows(dcb_prep* p, float* rows, uint8_t* packed, int32_t* window_pos, uint8_t* overflow,
                          int16_t* ccs_bq, int32_t* num_passes);
+/* Raw-record mode, for feature construction on the device (dcb_features_layout below): enabled before the first
+ * dcb_prep_next_zmw, the stream decodes and validates each ZMW and keeps its records as they are -- no trimming, spacing
+ * or windows (dcb_zmw_info.n_windows and spaced_width are 0, dcb_prep_get_windows is DCB_ERR_STATE), so the worker
+ * threads only decode, validate and export.  Every check expand_clip_indent makes (pre_lib.py:1128-1239: implausible
+ * cigar / position, cigar vs sequence length, pw / ip length, missing sn tag, pad operations, an aligned part that
+ * cannot be located) is made here with the same message, on what trim_insertions (pre_lib.py:1061-1125) would leave of
+ * the record; the export also refuses hard clips and reference skips, which subread alignments to a CCS read do not
+ * contain.  dcb_prep_get_records writes nothing for a ZMW that failed.
+ * dcb_prep_get_records, for the loaded ZMW -- every array may be NULL, so a first call sizes the second:
+ *   sizes [DCB_RECORD_SIZES]    subreads, cigar operations, query bases, CCS length, 1 when any CCS quality is non-zero
+ *                               (spacing of the qualities only applies then, pre_lib.py:247-250)
+ *   read_meta [n][DCB_READ_META] per mapped subread, ALL of them (space_out_subreads runs over every subread before
+ *                               extract_features keeps the first max_passes, pre_lib.py:1242-1276,704-744): offset and
+ *                               count of its cigar operations, offset and count of its query bases, pos, reverse flag,
+ *                               first and one-past-last alignment column (after trimming) that survive the soft clips,
+ *                               insertion columns left after trimming, 0.  Offsets are relative to this ZMW's arrays.
+ *   read_sn [n][4]              the sn tag
+ *   cigar                       u32 per operation, op | len << 4, as stored in the BAM (untrimmed)
+ *   bases / pw / ip             per query base, in the BAM's order: base id over ' ATCG' (others 0), and the kinetics
+ *                               cast to uint8 as expand_clip_indent does (pre_lib.py:1166-1167)
+ *   ccs_bases / ccs_bq          the CCS read's base ids and base qualities */
+#define DCB_READ_META 10
+#define DCB_RECORD_SIZES 5
+int dcb_prep_export_records(dcb_prep* p, int32_t enabled);
+int dcb_prep_get_records(dcb_prep* p, int64_t* sizes, int32_t* read_meta, float* read_sn, uint32_t* cigar, uint8_t* bases,
+                         uint8_t* pw, uint8_t* ip, uint8_t* ccs_bases, uint8_t* ccs_bq);
 const char* dcb_prep_ccs_header(dcb_prep* p);             /* SAM header text of the CCS BAM */
 void dcb_prep_close(dcb_prep* p);
 const char* dcb_prep_last_error(void);
@@ -334,6 +360,44 @@ int dcb_bamw_open(const char* path, const char* header_text, dcb_bamw** out);
 int dcb_bamw_write(dcb_bamw* w, const char* name, const uint8_t* seq, const uint8_t* qual_phred33, int32_t len,
                    int32_t has_ec, float ec, int32_t np_num_passes, float rq, const char* rg);
 int dcb_bamw_close(dcb_bamw* w);
+
+/* ---- feature construction on the device ---------------------------------------------------------------------------------
+ * trim_insertions, expand_clip_indent, space_out_subreads, the window cut and the packed rows (pre_lib.py:1061-1276,
+ * 625-744) from the records of a batch of ZMWs, in two phases so that rows are only laid out for the windows the model
+ * will score.  dcb_records is dcb_prep_get_records' arrays of n_zmw ZMWs concatenated (host pointers): read_meta's
+ * offsets made relative to the concatenated cigar / base arrays, ZMW z owning reads [zmw_read_off[z],
+ * zmw_read_off[z + 1]) and CCS bases [zmw_ccs_off[z], zmw_ccs_off[z + 1]).  Records must come from
+ * dcb_prep_get_records or hold what it guarantees; the engine checks every offset and sizes its scratch from read_meta,
+ * and a cigar that disagrees with its read_meta ends in DCB_ERR_INVALID.
+ *
+ * dcb_features_layout (phase A) spaces the batch and returns, dense over the batch and ZMW by ZMW, exactly what
+ * dcb_prep_get_windows returns apart from the rows: zmw_windows [n_zmw] (windows per ZMW; windows without a CCS
+ * position are dropped, pre_lib.py:625-697), window_pos / num_passes int32 [n], overflow u8 [n], ccs_bq int16 [n, L]
+ * (-1 at gaps and padding), ccs_ids u8 [n, L] (the CCS row, pre_lib.py:739) -- what the skip decision
+ * (dcb_skip_mask) and dcb_fill_skipped need.  *n_windows_out receives n; max_windows is the capacity of the per-window
+ * arrays, and sum over ZMWs of ceil((max(ccs_len, max_r(pos + col_end - col_begin)) + sum_r insertion columns + 32) / L)
+ * always suffices.  The spaced reads stay in engine scratch until the next call; a batch whose spaced reads would
+ * exceed 2 GiB is DCB_ERR_INVALID (pass fewer ZMWs), and the engine stays usable after any error.
+ *
+ * dcb_features_pack (phase B) writes the packed rows (above) of windows[0..n) -- indices into phase A's n windows, any
+ * order, repeats allowed -- to packed_out [n, dcb_packed_window_bytes]: a host array, or with DCB_OUT_ON_DEVICE a
+ * 16-byte-aligned device array that dcb_forward_packed(..., DCB_ROWS_ON_DEVICE) reads in place.  Byte for byte the
+ * `packed` of dcb_prep_get_windows.  ms_out (nullable): device time of the kernels.  Deterministic, no atomics. */
+typedef struct dcb_records {
+  int32_t n_zmw, n_cigar, n_query, reserved;
+  const int32_t* zmw_read_off;     /* [n_zmw + 1] */
+  const int32_t* zmw_ccs_off;      /* [n_zmw + 1] */
+  const int32_t* zmw_ccs_bq_any;   /* [n_zmw] */
+  const int32_t* read_meta;        /* [n_reads, DCB_READ_META] */
+  const float* read_sn;            /* [n_reads, 4] */
+  const uint32_t* cigar;           /* [n_cigar] */
+  const uint8_t *bases, *pw, *ip;  /* [n_query] */
+  const uint8_t *ccs_bases, *ccs_bq;
+} dcb_records;
+int dcb_features_layout(dcb_engine* e, const dcb_records* rec, int32_t ins_trim, int32_t max_windows, int32_t* zmw_windows,
+                        int32_t* window_pos, uint8_t* overflow, int16_t* ccs_bq, int32_t* num_passes, uint8_t* ccs_ids,
+                        int32_t* n_windows_out, float* ms_out);
+int dcb_features_pack(dcb_engine* e, const int32_t* windows, int32_t n, uint32_t flags, uint8_t* packed_out, float* ms_out);
 
 /* Device time of the last dcb_forward (milliseconds, CUDA events on the engine's stream). */
 int dcb_last_forward_ms(dcb_engine* e, float* ms);
