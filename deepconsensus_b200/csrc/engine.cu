@@ -732,8 +732,18 @@ void bf16_forward_chunk(dcb_engine* e, LaunchRecorder& rec, const float* rows_ch
   snap();
   for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
     const LayerDev& ld = W.layers[n_];
-    rec.run(kProfQkv, 1, [&] { launch_gemm_qkv(e->d_xb, ld.wqkv, T, e->d_embqkv, st); });
-    rec.run(kProfAttention, 1, [&] { launch_attention(e->d_embqkv, e->d_att, L, Lw, c.attn_win_size, bw, st); });
+    if (Lw == kTileM) {
+      // one window per tile: q/k/v stay on the SM, two launches over half of the tiles each (the debug capture's
+      // q/k/v image is stored only when it is kept)
+      rec.run(kProfAttention, 2, [&] {
+        __nv_bfloat16* qkv = e->debug ? e->d_embqkv.p : nullptr;
+        for (int half = 0; half < 2; ++half)
+          launch_qkv_attention(half, e->d_xb, ld.wqkv, L, c.attn_win_size, T, qkv, e->d_att, st);
+      });
+    } else {
+      rec.run(kProfQkv, 1, [&] { launch_gemm_qkv(e->d_xb, ld.wqkv, T, e->d_embqkv, st); });
+      rec.run(kProfAttention, 1, [&] { launch_attention(e->d_embqkv, e->d_att, L, Lw, c.attn_win_size, bw, st); });
+    }
     rec.run(kProfRowGemm, 1, [&] {   // attention out-projection + residual; xb = the FFN sub-layer's input
       launch_gemm_row(e->d_att, ld.wo, kDP / 16, 2 * (kDP / 16), T, row_epi(e, true, nullptr, n_, 1, false), st);
     });

@@ -9,6 +9,8 @@
 //   ffn_gemm_kernel     the FFN relu(x W1 + b1) W2 + b2 (ffn_layer.py:83-86) with the hidden
 //                       activation kept in registers, half of the tiles per launch.
 //   band_attention_kernel  banded multi-head softmax attention (attention_layer.py:198-214)
+//   qkv_attention_kernel   the q/k/v projection and the banded attention of one window-aligned tile, with q/k/v
+//                       kept on the SM, half of the tiles per launch
 //   head_kernel         final LayerNorm -> fc1 -> softmax -> argmax -> Phred -> ASCII
 //                       (encoder_stack.py:197, networks.py:342,238, quick_inference.py:377-414)
 #include "kernels.h"
@@ -712,6 +714,131 @@ __device__ __forceinline__ int att_rot(int chunk, int rowmod) {
   return t >= kAttChunks ? t - kAttChunks : t;
 }
 
+// The banded online-softmax attention of one 16-row query block [i0, i0 + 16) of a window against its K and V rows in
+// shared memory (the rotated layout above, zero beyond L up to a multiple of 16), called by a whole warp.  qa holds the
+// block's Q as mma.sync A fragments, one per 16-column k-step (zero for rows >= L).  The bf16 output of the rows < L
+// goes to columns [head * kDHP, head * kDHP + kDHP) of the attention image, whose window starts at token tok0.  A
+// block's arithmetic does not depend on which warp runs it, so both attention kernels give the same bits.
+__device__ __forceinline__ void attend_block(const uint32_t (&qa)[kDHP / 16][4], const __nv_bfloat16* sK,
+                                             const __nv_bfloat16* sV, int i0, int L, int band,
+                                             __nv_bfloat16* __restrict__ att, int tok0, int head) {
+  const int lane = threadIdx.x & 31;
+  const int g = lane >> 2, t = lane & 3;
+  constexpr float kLog2e = 1.4426950408889634f;
+  constexpr int kChunkElems = kTileM * 8;
+  const int r0 = i0 + g, r1 = i0 + g + 8;
+  float o[kDHP / 8][4];
+#pragma unroll
+  for (int nt = 0; nt < kDHP / 8; ++nt) { o[nt][0] = o[nt][1] = o[nt][2] = o[nt][3] = 0.f; }
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+
+  int jlo = i0 - band; if (jlo < 0) jlo = 0; jlo &= ~15;
+  int jhi = i0 + 15 + band + 1; if (jhi > L) jhi = L;
+  for (int j0 = jlo; j0 < jhi; j0 += 16) {
+    // S tile 16 x 16 = two n-tiles of 8 keys; two partial accumulators per n-tile shorten the
+    // dependent HMMA chains (4 independent chains instead of 2)
+    float s[2][4], s2[2][4];
+#pragma unroll
+    for (int nt = 0; nt < 2; ++nt) {
+      s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
+      s2[nt][0] = s2[nt][1] = s2[nt][2] = s2[nt][3] = 0.f;
+    }
+    const int krow0 = j0 + g, krow1 = j0 + 8 + g;
+    const __nv_bfloat16* kr0 = sK + (size_t)krow0 * kAttStride + 2 * t;
+    const __nv_bfloat16* kr1 = sK + (size_t)krow1 * kAttStride + 2 * t;
+    const int km0 = krow0 % kAttChunks, km1 = krow1 % kAttChunks;
+#pragma unroll
+    for (int ks = 0; ks < kDHP / 16; ++ks) {
+      const uint32_t a0 = *reinterpret_cast<const uint32_t*>(kr0 + att_rot(2 * ks, km0) * 8);
+      const uint32_t a1 = *reinterpret_cast<const uint32_t*>(kr0 + att_rot(2 * ks + 1, km0) * 8);
+      const uint32_t c0 = *reinterpret_cast<const uint32_t*>(kr1 + att_rot(2 * ks, km1) * 8);
+      const uint32_t c1 = *reinterpret_cast<const uint32_t*>(kr1 + att_rot(2 * ks + 1, km1) * 8);
+      if (ks & 1) {
+        mma_bf16_16816(s2[0], qa[ks], a0, a1);
+        mma_bf16_16816(s2[1], qa[ks], c0, c1);
+      } else {
+        mma_bf16_16816(s[0], qa[ks], a0, a1);
+        mma_bf16_16816(s[1], qa[ks], c0, c1);
+      }
+    }
+#pragma unroll
+    for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) s[nt][e] += s2[nt][e];
+    // mask: |i - j| <= band and j < L  (tf.where(mask, logits, -1e9): exp underflows to 0)
+    float tmax0 = -INFINITY, tmax1 = -INFINITY;
+#pragma unroll
+    for (int nt = 0; nt < 2; ++nt) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int i = (e < 2) ? r0 : r1;
+        const int j = j0 + nt * 8 + 2 * t + (e & 1);
+        const int dlt = i - j;
+        const bool ok = (j < L) && (dlt <= band) && (dlt >= -band);
+        s[nt][e] = ok ? s[nt][e] : -INFINITY;
+      }
+      tmax0 = fmaxf(tmax0, fmaxf(s[nt][0], s[nt][1]));
+      tmax1 = fmaxf(tmax1, fmaxf(s[nt][2], s[nt][3]));
+    }
+    tmax0 = fmaxf(tmax0, __shfl_xor_sync(0xffffffffu, tmax0, 1));
+    tmax0 = fmaxf(tmax0, __shfl_xor_sync(0xffffffffu, tmax0, 2));
+    tmax1 = fmaxf(tmax1, __shfl_xor_sync(0xffffffffu, tmax1, 1));
+    tmax1 = fmaxf(tmax1, __shfl_xor_sync(0xffffffffu, tmax1, 2));
+    const float mn0 = fmaxf(m0, tmax0), mn1 = fmaxf(m1, tmax1);
+    // rows with no valid key yet keep m = -inf; use 0 as the subtraction base there
+    const float base0 = mn0 == -INFINITY ? 0.f : mn0, base1 = mn1 == -INFINITY ? 0.f : mn1;
+    const float sc0 = exp2f((m0 - base0) * kLog2e), sc1 = exp2f((m1 - base1) * kLog2e);
+    m0 = mn0; m1 = mn1;
+    float ps0 = 0.f, ps1 = 0.f;
+    uint32_t pa[4];
+    {
+      float p[2][4];
+#pragma unroll
+      for (int nt = 0; nt < 2; ++nt) {
+        p[nt][0] = exp2f((s[nt][0] - base0) * kLog2e);
+        p[nt][1] = exp2f((s[nt][1] - base0) * kLog2e);
+        p[nt][2] = exp2f((s[nt][2] - base1) * kLog2e);
+        p[nt][3] = exp2f((s[nt][3] - base1) * kLog2e);
+        ps0 += p[nt][0] + p[nt][1];
+        ps1 += p[nt][2] + p[nt][3];
+      }
+      // C fragments of the two n-tiles form the A fragment of one 16-key k-step
+      pa[0] = pack_bf16x2(p[0][0], p[0][1]);
+      pa[1] = pack_bf16x2(p[0][2], p[0][3]);
+      pa[2] = pack_bf16x2(p[1][0], p[1][1]);
+      pa[3] = pack_bf16x2(p[1][2], p[1][3]);
+    }
+    l0 = l0 * sc0 + ps0;
+    l1 = l1 * sc1 + ps1;
+    // O = O * scale + P V
+    const int vrow = j0 + (lane & 15);
+    const int vm = vrow % kAttChunks;
+    const uint32_t vbase = smem_u32(sV + (size_t)vrow * kAttStride);
+#pragma unroll
+    for (int nt = 0; nt < kDHP / 8; ++nt) {
+      o[nt][0] *= sc0; o[nt][1] *= sc0; o[nt][2] *= sc1; o[nt][3] *= sc1;
+      uint32_t b0, b1;
+      ldmatrix_x2_trans(b0, b1, vbase + att_rot(nt, vm) * 16);
+      mma_bf16_16816(o[nt], pa, b0, b1);
+    }
+  }
+  // normalise (row sums live in the quad) and store bf16 to the attention operand image
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float inv0 = 1.f / l0, inv1 = 1.f / l1;
+  __nv_bfloat16* o0 = att + img_off(tok0 + (r0 < L ? r0 : 0), head * kDHP + 2 * t, kDP / 8);
+  __nv_bfloat16* o1 = att + img_off(tok0 + (r1 < L ? r1 : 0), head * kDHP + 2 * t, kDP / 8);
+#pragma unroll
+  for (int nt = 0; nt < kDHP / 8; ++nt) {
+    if (r0 < L)
+      *reinterpret_cast<uint32_t*>(o0 + nt * kChunkElems) = pack_bf16x2(o[nt][0] * inv0, o[nt][1] * inv0);
+    if (r1 < L)
+      *reinterpret_cast<uint32_t*>(o1 + nt * kChunkElems) = pack_bf16x2(o[nt][2] * inv1, o[nt][3] * inv1);
+  }
+}
+
 __global__ void __launch_bounds__(128, 3)
 band_attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ att,
                       int L, int Lw, int win, int nwindows) {
@@ -757,7 +884,6 @@ band_attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __re
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
   const int band = win > 0 ? win : L;  // attn_win_size None/0 => full attention
-  constexpr float kLog2e = 1.4426950408889634f;
 
   // Q fragments for 9 k-steps: rows i0+g, i0+g+8 (zero beyond L), straight from global.
   // In the operand image a row's k-chunks are kTileM*8 elements apart, so every fragment address is
@@ -785,118 +911,203 @@ band_attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __re
   __syncthreads();
 
   for (int qb = warp; qb * 16 < L; qb += 4) {
-    const int i0 = qb * 16;
-    const int r0 = i0 + g, r1 = i0 + g + 8;
     if (qb != warp) load_q(qb);
-    float o[kDHP / 8][4];
-#pragma unroll
-    for (int nt = 0; nt < kDHP / 8; ++nt) { o[nt][0] = o[nt][1] = o[nt][2] = o[nt][3] = 0.f; }
-    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+    attend_block(qa, sK, sV, qb * 16, L, band, att, tok0, head);
+  }
+}
 
-    int jlo = i0 - band; if (jlo < 0) jlo = 0; jlo &= ~15;
-    int jhi = i0 + 15 + band + 1; if (jhi > L) jhi = L;
-    for (int j0 = jlo; j0 < jhi; j0 += 16) {
-      // S tile 16 x 16 = two n-tiles of 8 keys; two partial accumulators per n-tile shorten the
-      // dependent HMMA chains (4 independent chains instead of 2)
-      float s[2][4], s2[2][4];
-#pragma unroll
-      for (int nt = 0; nt < 2; ++nt) {
-        s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
-        s2[nt][0] = s2[nt][1] = s2[nt][2] = s2[nt][3] = 0.f;
-      }
-      const int krow0 = j0 + g, krow1 = j0 + 8 + g;
-      const __nv_bfloat16* kr0 = sK + (size_t)krow0 * kAttStride + 2 * t;
-      const __nv_bfloat16* kr1 = sK + (size_t)krow1 * kAttStride + 2 * t;
-      const int km0 = krow0 % kAttChunks, km1 = krow1 % kAttChunks;
-#pragma unroll
-      for (int ks = 0; ks < kDHP / 16; ++ks) {
-        const uint32_t a0 = *reinterpret_cast<const uint32_t*>(kr0 + att_rot(2 * ks, km0) * 8);
-        const uint32_t a1 = *reinterpret_cast<const uint32_t*>(kr0 + att_rot(2 * ks + 1, km0) * 8);
-        const uint32_t c0 = *reinterpret_cast<const uint32_t*>(kr1 + att_rot(2 * ks, km1) * 8);
-        const uint32_t c1 = *reinterpret_cast<const uint32_t*>(kr1 + att_rot(2 * ks + 1, km1) * 8);
-        if (ks & 1) {
-          mma_bf16_16816(s2[0], qa[ks], a0, a1);
-          mma_bf16_16816(s2[1], qa[ks], c0, c1);
-        } else {
-          mma_bf16_16816(s[0], qa[ks], a0, a1);
-          mma_bf16_16816(s[1], qa[ks], c0, c1);
+// =====================================================================================
+// q/k/v projection and attention of one window-aligned tile on the SM
+// =====================================================================================
+// In the window-aligned layout (Lw == kTileM, L <= 128) a tile is one window, and the band never leaves it, so the
+// attention of a tile needs only that tile's q/k/v.  One work item is one tile in [tile_begin, tile_end).  Its xb (A)
+// image is loaded once and stays resident; warpgroup w owns tile rows [64 w, 64 w + 64).  Per head h each consumer
+// warpgroup
+//   1. runs the k_h and then the v_h n-group of the q/k/v weights (split-bf16, 36 k-steps: W_hi then W_lo, A k-step
+//      (s * 2 + kk) % 18, as gemm_kernel's EPI_QKV) and stores each, rounded to bf16, into sK / sV in the attention's
+//      rotated layout, zero for rows >= L,
+//   2. runs the q_h n-group and keeps it in registers as mma.sync A fragments (the m64n144 accumulator of warp w & 3
+//      covers its 16 rows in the m16n8k16 C layout: k-step ks is pack(d[8ks..+1]), pack(d[8ks+2..+3]),
+//      pack(d[8ks+4..+5]), pack(d[8ks+6..+7]), the mapping the FFN uses for its hidden activation),
+//   3. meets its partner on named barrier 1 (the band crosses row 64, so both halves of K and V must be in place),
+//   4. runs attend_block for the warp's own 16-row query block.
+// Before a warpgroup next writes sK / sV it meets its partner again, so no warp still reads the previous head's K and
+// V; the wgmmas of the next group are already under way by then.  The producer streams the groups in the order k_h0,
+// v_h0, q_h0, k_h1, v_h1, q_h1 (groups 2, 4, 0, 3, 5, 1 of the [q_h0|q_h1|k_h0|k_h1|v_h0|v_h1] weight image) through
+// a ring of 9216-byte stages (two k-steps of one group), and the next tile's xb loads once q_h1's MMAs have read it,
+// under head 1's attention.
+//
+// Every q/k/v value is the accumulator gemm_kernel<144, 1, EPI_QKV, true> computes (same wgmma shape, same K order)
+// rounded the same way, and attend_block is band_attention_kernel's, so the attention image is the same bit for bit.
+// kQkv: the q/k/v accumulators are also stored to the q/k/v operand image as the EPI_QKV epilogue does (debug capture).
+struct QkvAttCfg {
+  static constexpr int kAK = kDP / 16;                    // A k-steps: 18
+  static constexpr int kSK = 2;                           // k-steps per stage
+  static constexpr int kGroupStages = 2 * kAK / kSK;      // split-bf16 weights: 36 k-steps per group, 18 stages
+  static constexpr int kABytesPerK = 2 * kTileM * 16;     // 4096
+  static constexpr int kBBytesPerK = 2 * kQKVGroup * 16;  // 4608
+  static constexpr int kStageBytes = kSK * kBBytesPerK;   // 9216
+  static constexpr int kGroupBytes = 2 * kAK * kBBytesPerK;
+  static constexpr int kStages = 8;
+  static constexpr int kATileBytes = kAK * kABytesPerK;   // the resident xb tile: 72 KB
+  static constexpr int kKVBytes = kTileM * kAttStride * 2;  // K or V of one head: 36 KB
+  static constexpr int kBarBytes = 256;
+  // the xb tile, sK, sV, the ring, the mbarriers
+  static constexpr int kSmemBytes = kATileBytes + 2 * kKVBytes + kStages * kStageBytes + kBarBytes;
+  static constexpr int kThreads = 384;
+  static_assert(kSmemBytes <= 232448, "over the sm_90 opt-in shared memory per block");
+  static_assert((2 * kStages + 2) * 8 <= kBarBytes, "the mbarriers (full, empty, a_full, a_empty) fit");
+  static_assert(kQKVGroup == kDHP && kQKVN == 6 * kQKVGroup, "one n-group is one head's q, k or v");
+};
+
+// the n-group of the q/k/v weight image that item step i (0..5) of a tile runs: k_h0, v_h0, q_h0, k_h1, v_h1, q_h1
+__device__ __forceinline__ int qkv_att_group(int i) {
+  const int h = i / 3, part = i % 3;
+  return part == 0 ? 2 + h : part == 1 ? 4 + h : h;
+}
+
+__device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+template <bool kQkv>
+__global__ void __launch_bounds__(384, 1)
+qkv_attention_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* __restrict__ b_img, int L,
+                     int win, int tile_begin, int tile_end, __nv_bfloat16* __restrict__ qkv_img,
+                     __nv_bfloat16* __restrict__ att) {
+  using Cfg = QkvAttCfg;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* a_res = smem;
+  __nv_bfloat16* sK = reinterpret_cast<__nv_bfloat16*>(smem + Cfg::kATileBytes);
+  __nv_bfloat16* sV = reinterpret_cast<__nv_bfloat16*>(smem + Cfg::kATileBytes + Cfg::kKVBytes);
+  uint8_t* stage_base = smem + Cfg::kATileBytes + 2 * Cfg::kKVBytes;
+  uint64_t* full = reinterpret_cast<uint64_t*>(stage_base + Cfg::kStages * Cfg::kStageBytes);
+  uint64_t* empty = full + Cfg::kStages;
+  uint64_t* a_full = empty + Cfg::kStages;
+  uint64_t* a_empty = a_full + 1;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < Cfg::kStages; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 256);   // every consumer thread
+    }
+    mbar_init(a_full, 1);
+    mbar_init(a_empty, 256);
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // ------------------------------------------------------------- producer
+    setmaxnreg_dec<24>();
+    if (warp == 8 && lane == 0) {
+      uint32_t slot = 0, phase = 0, it = 0;
+      for (int tile = tile_begin + blockIdx.x; tile < tile_end; tile += gridDim.x, ++it) {
+        mbar_wait(a_empty, (it & 1) ^ 1);
+        mbar_arrive_expect_tx(a_full, Cfg::kATileBytes);
+        bulk_g2s(a_res, reinterpret_cast<const uint8_t*>(xb_img) + (size_t)tile * Cfg::kATileBytes, Cfg::kATileBytes,
+                 a_full);
+        for (int i = 0; i < 6; ++i) {
+          const uint8_t* b_src = reinterpret_cast<const uint8_t*>(b_img) + (size_t)qkv_att_group(i) * Cfg::kGroupBytes;
+          for (int s = 0; s < Cfg::kGroupStages; ++s) {
+            mbar_wait(&empty[slot], phase ^ 1);
+            mbar_arrive_expect_tx(&full[slot], Cfg::kStageBytes);
+            bulk_g2s(stage_base + slot * Cfg::kStageBytes, b_src + (size_t)s * Cfg::kStageBytes, Cfg::kStageBytes,
+                     &full[slot]);
+            if (++slot == Cfg::kStages) { slot = 0; phase ^= 1; }
+          }
         }
-      }
-#pragma unroll
-      for (int nt = 0; nt < 2; ++nt)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) s[nt][e] += s2[nt][e];
-      // mask: |i - j| <= band and j < L  (tf.where(mask, logits, -1e9): exp underflows to 0)
-      float tmax0 = -INFINITY, tmax1 = -INFINITY;
-#pragma unroll
-      for (int nt = 0; nt < 2; ++nt) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int i = (e < 2) ? r0 : r1;
-          const int j = j0 + nt * 8 + 2 * t + (e & 1);
-          const int dlt = i - j;
-          const bool ok = (j < L) && (dlt <= band) && (dlt >= -band);
-          s[nt][e] = ok ? s[nt][e] : -INFINITY;
-        }
-        tmax0 = fmaxf(tmax0, fmaxf(s[nt][0], s[nt][1]));
-        tmax1 = fmaxf(tmax1, fmaxf(s[nt][2], s[nt][3]));
-      }
-      tmax0 = fmaxf(tmax0, __shfl_xor_sync(0xffffffffu, tmax0, 1));
-      tmax0 = fmaxf(tmax0, __shfl_xor_sync(0xffffffffu, tmax0, 2));
-      tmax1 = fmaxf(tmax1, __shfl_xor_sync(0xffffffffu, tmax1, 1));
-      tmax1 = fmaxf(tmax1, __shfl_xor_sync(0xffffffffu, tmax1, 2));
-      const float mn0 = fmaxf(m0, tmax0), mn1 = fmaxf(m1, tmax1);
-      // rows with no valid key yet keep m = -inf; use 0 as the subtraction base there
-      const float base0 = mn0 == -INFINITY ? 0.f : mn0, base1 = mn1 == -INFINITY ? 0.f : mn1;
-      const float sc0 = exp2f((m0 - base0) * kLog2e), sc1 = exp2f((m1 - base1) * kLog2e);
-      m0 = mn0; m1 = mn1;
-      float ps0 = 0.f, ps1 = 0.f;
-      uint32_t pa[4];
-      {
-        float p[2][4];
-#pragma unroll
-        for (int nt = 0; nt < 2; ++nt) {
-          p[nt][0] = exp2f((s[nt][0] - base0) * kLog2e);
-          p[nt][1] = exp2f((s[nt][1] - base0) * kLog2e);
-          p[nt][2] = exp2f((s[nt][2] - base1) * kLog2e);
-          p[nt][3] = exp2f((s[nt][3] - base1) * kLog2e);
-          ps0 += p[nt][0] + p[nt][1];
-          ps1 += p[nt][2] + p[nt][3];
-        }
-        // C fragments of the two n-tiles form the A fragment of one 16-key k-step
-        pa[0] = pack_bf16x2(p[0][0], p[0][1]);
-        pa[1] = pack_bf16x2(p[0][2], p[0][3]);
-        pa[2] = pack_bf16x2(p[1][0], p[1][1]);
-        pa[3] = pack_bf16x2(p[1][2], p[1][3]);
-      }
-      l0 = l0 * sc0 + ps0;
-      l1 = l1 * sc1 + ps1;
-      // O = O * scale + P V
-      const int vrow = j0 + (lane & 15);
-      const int vm = vrow % kAttChunks;
-      const uint32_t vbase = smem_u32(sV + (size_t)vrow * kAttStride);
-#pragma unroll
-      for (int nt = 0; nt < kDHP / 8; ++nt) {
-        o[nt][0] *= sc0; o[nt][1] *= sc0; o[nt][2] *= sc1; o[nt][3] *= sc1;
-        uint32_t b0, b1;
-        ldmatrix_x2_trans(b0, b1, vbase + att_rot(nt, vm) * 16);
-        mma_bf16_16816(o[nt], pa, b0, b1);
       }
     }
-    // normalise (row sums live in the quad) and store bf16 to the attention operand image
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-    const float inv0 = 1.f / l0, inv1 = 1.f / l1;
-    __nv_bfloat16* o0 = att + img_off(tok0 + (r0 < L ? r0 : 0), head * kDHP + 2 * t, kDP / 8);
-    __nv_bfloat16* o1 = att + img_off(tok0 + (r1 < L ? r1 : 0), head * kDHP + 2 * t, kDP / 8);
+    return;
+  }
+
+  // --------------------------------------------------------------- consumers (2 warpgroups)
+  setmaxnreg_inc<240>();
+  const int wg = warp >> 2;
+  const int g = lane >> 2, q = lane & 3;
+  const int row0 = wg * 64 + (warp & 3) * 16 + g;   // this thread's accumulator rows: row0, row0 + 8
+  const uint32_t a_base = smem_u32(a_res) + wg * 64 * 16;
+  const int band = win > 0 ? win : L;   // attn_win_size None/0 => full attention
+  float acc[kQKVGroup / 2];
+  uint32_t slot = 0, phase = 0, it = 0;
+  for (int tile = tile_begin + blockIdx.x; tile < tile_end; tile += gridDim.x, ++it) {
+    mbar_wait(a_full, it & 1);
+#pragma unroll 1
+    for (int h = 0; h < kHeads; ++h) {
+      uint32_t qa[kDHP / 16][4];
 #pragma unroll
-    for (int nt = 0; nt < kDHP / 8; ++nt) {
-      if (r0 < L)
-        *reinterpret_cast<uint32_t*>(o0 + nt * kChunkElems) = pack_bf16x2(o[nt][0] * inv0, o[nt][1] * inv0);
-      if (r1 < L)
-        *reinterpret_cast<uint32_t*>(o1 + nt * kChunkElems) = pack_bf16x2(o[nt][2] * inv1, o[nt][3] * inv1);
+      for (int part = 0; part < 3; ++part) {
+        // ---- acc = xb W[:, group]
+        uint32_t prev = 0;
+#pragma unroll 1
+        for (int s = 0; s < Cfg::kGroupStages; ++s) {
+          mbar_wait(&full[slot], phase);
+          const uint32_t st = smem_u32(stage_base + slot * Cfg::kStageBytes);
+          wgmma_fence_regs(acc);
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < Cfg::kSK; ++kk) {
+            const uint64_t adesc =
+                make_kc16_desc(a_base + ((s * Cfg::kSK + kk) % Cfg::kAK) * Cfg::kABytesPerK, kTileM * 16, 128);
+            const uint64_t bdesc = make_kc16_desc(st + kk * Cfg::kBBytesPerK, kQKVGroup * 16, 128);
+            wgmma_m64n144k16(acc, adesc, bdesc, (s | kk) != 0);
+          }
+          wgmma_commit();
+          wgmma_fence_regs(acc);
+          // the previous stage's MMAs are complete once at most this stage's group is in flight: hand it back
+          wgmma_wait<1>();
+          if (s > 0) mbar_arrive(&empty[prev]);
+          prev = slot;
+          if (++slot == Cfg::kStages) { slot = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        mbar_arrive(&empty[prev]);
+        if (h + 1 == kHeads && part == 2) mbar_arrive(a_empty);   // the item's last MMAs on xb have completed
+
+        const int grp = part == 0 ? 2 + h : part == 1 ? 4 + h : h;   // qkv_att_group(3 h + part)
+        if constexpr (kQkv) {   // the EPI_QKV epilogue's stores
+          __nv_bfloat16* obase = qkv_img + (size_t)tile * kTileM * (kQKVN / 8) * 8;
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+            for (int jj = 0; jj < kQKVGroup / 8; ++jj) {
+              const int col = grp * kQKVGroup + jj * 8 + 2 * q;
+              *reinterpret_cast<uint32_t*>(obase + ((size_t)(col >> 3) * kTileM + row0 + 8 * hr) * 8 + (col & 7)) =
+                  pack_bf16x2(acc[jj * 4 + 2 * hr], acc[jj * 4 + 2 * hr + 1]);
+            }
+        }
+        if (part < 2) {
+          // ---- K or V into shared memory; before K, every warp is done with the previous head's K and V
+          if (part == 0) consumer_bar_sync();
+          __nv_bfloat16* dst = part == 0 ? sK : sV;
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            const int r = row0 + 8 * hr;
+            const int rm = r % kAttChunks;
+            __nv_bfloat16* drow = dst + (size_t)r * kAttStride + 2 * q;
+#pragma unroll
+            for (int jj = 0; jj < kDHP / 8; ++jj)
+              *reinterpret_cast<uint32_t*>(drow + att_rot(jj, rm) * 8) =
+                  r < L ? pack_bf16x2(acc[jj * 4 + 2 * hr], acc[jj * 4 + 2 * hr + 1]) : 0u;
+          }
+        } else {
+          // ---- Q as A fragments (zero for rows >= L)
+          const bool v0 = row0 < L, v1 = row0 + 8 < L;
+#pragma unroll
+          for (int ks = 0; ks < kDHP / 16; ++ks) {
+            qa[ks][0] = v0 ? pack_bf16x2(acc[8 * ks + 0], acc[8 * ks + 1]) : 0u;
+            qa[ks][1] = v1 ? pack_bf16x2(acc[8 * ks + 2], acc[8 * ks + 3]) : 0u;
+            qa[ks][2] = v0 ? pack_bf16x2(acc[8 * ks + 4], acc[8 * ks + 5]) : 0u;
+            qa[ks][3] = v1 ? pack_bf16x2(acc[8 * ks + 6], acc[8 * ks + 7]) : 0u;
+          }
+        }
+      }
+      // ---- attention of this warp's query block once both halves of K and V are in place
+      consumer_bar_sync();
+      const int i0 = warp * 16;
+      if (i0 < L) attend_block(qa, sK, sV, i0, L, band, att, tile * kTileM, h);
     }
   }
 }
@@ -987,6 +1198,10 @@ cudaError_t kernels_init() {
   for (auto fn : {ffn_gemm_kernel<false>, ffn_gemm_kernel<true>})
     if ((e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, FfnCfg::kSmemBytes)) != cudaSuccess)
       return e;
+  for (auto fn : {qkv_attention_kernel<false>, qkv_attention_kernel<true>})
+    if ((e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, QkvAttCfg::kSmemBytes)) !=
+        cudaSuccess)
+      return e;
   e = cudaFuncSetAttribute(embed_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(band_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1064,6 +1279,21 @@ void launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* att, int L, int L
   const int Lp = (L + 15) & ~15;
   const size_t smem = (size_t)2 * Lp * kAttStride * 2;
   band_attention_kernel<<<nwindows * 2, 128, smem, st>>>(qkv, att, L, Lw, win, nwindows);
+}
+
+void launch_qkv_attention(int half, const __nv_bfloat16* xb_img, const __nv_bfloat16* wqkv, int L, int win,
+                          int ntiles, __nv_bfloat16* qkv_img, __nv_bfloat16* att, cudaStream_t st) {
+  const int split = (ntiles + 1) / 2;
+  const int t0 = half ? split : 0, t1 = half ? ntiles : split;
+  // a half without tiles still launches (one CTA that finds no work), as launch_ffn's
+  const int n = t1 - t0;
+  const int grid = n < 1 ? 1 : n < num_sms() ? n : num_sms();
+  if (qkv_img)
+    qkv_attention_kernel<true><<<grid, QkvAttCfg::kThreads, QkvAttCfg::kSmemBytes, st>>>(xb_img, wqkv, L, win, t0, t1,
+                                                                                        qkv_img, att);
+  else
+    qkv_attention_kernel<false><<<grid, QkvAttCfg::kThreads, QkvAttCfg::kSmemBytes, st>>>(xb_img, wqkv, L, win, t0,
+                                                                                         t1, nullptr, att);
 }
 
 

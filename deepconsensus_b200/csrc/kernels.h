@@ -31,6 +31,12 @@ void launch_ffn(int half, const __nv_bfloat16* xb_img, const __nv_bfloat16* w1_i
 void launch_unpack_rows(const uint8_t* packed, const PackedLayout& pl, int nwindows, float* rows, cudaStream_t st);
 void launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* att, int L, int Lw, int win, int nwindows,
                       cudaStream_t st);
+// The window-aligned layout only (Lw == kTileM, L <= 128): one half of the q/k/v projection and banded attention with
+// q/k/v kept on the SM (kernels.cu, qkv_attention_kernel): half 0 runs tiles [0, ceil(ntiles / 2)), half 1 the rest.
+// xb_img: A [tile][36][128][8]; wqkv: launch_gemm_qkv's weight image; att: [tile][36][128][8], rows < L written.
+// qkv_img, when not null, also receives the q/k/v image launch_gemm_qkv writes (debug capture).
+void launch_qkv_attention(int half, const __nv_bfloat16* xb_img, const __nv_bfloat16* wqkv, int L, int win,
+                          int ntiles, __nv_bfloat16* qkv_img, __nv_bfloat16* att, cudaStream_t st);
 void launch_head(const HeadParams& p, int ntiles, cudaStream_t st);
 // per-read window concatenation + gap compaction; read z = windows [zmw_start[z], zmw_start[z+1]) (device pointers)
 void launch_stitch(const uint8_t* bases, const uint8_t* quals, int L, const int32_t* zmw_start, int n_zmw,

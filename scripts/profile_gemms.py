@@ -8,11 +8,14 @@ Writes DIR/profile_gemms.json (and DIR/trace.json, the torch.profiler trace it w
            each launch is named by the kernel before it: the condenser follows the embedding, the out-projection the
            attention, the FFN down-projection the FFN up-projection.  Builds with the fused FFN launch it twice per
            layer, named by their order in the layer: ffn_first and ffn_second, each over half of the tiles and the
-           whole filter, with the row epilogue.
+           whole filter, with the row epilogue.  Builds that keep q/k/v on the SM (window-aligned layout) run the
+           q/k/v projection and the attention as one kernel, also launched twice per layer: qkv_att_first and
+           qkv_att_second; the out-projection then follows qkv_att_second.
   l2_read  for each GEMM, the bytes its CTAs read from L2 per launch (weights once per work item, activations,
            residual), computed from the shapes and the tiling, over its kernel time.
-  hbm      for each FFN launch, the activation bytes it reads and writes in HBM (the weights stay in L2), computed
-           from the image shapes, over its kernel time and against the H100 SXM data sheet's 3.35 TB/s.
+  hbm      for each FFN launch and each fused q/k/v + attention launch, the activation bytes it reads and writes in
+           HBM (the weights stay in L2), computed from the image shapes, over its kernel time and against the H100
+           SXM data sheet's 3.35 TB/s.
   l2_ceiling  scripts/l2_stream.cu, compiled into a temporary directory: every SM streams the same L2-resident 1.18 MB
            weight image through the GEMM's 4-stage bulk-copy ring with consumers that only release the slots.
 The card's name, power limit and clocks are recorded beside the numbers.  DCB200_LIB selects another build of the
@@ -69,12 +72,15 @@ def l2_bytes(role, ntiles, ff, epad, tokens):
   if role in ("ffn_first", "ffn_second"):    # one tile per work item: the whole of W1 and W2, xb, the residual
     n = ffn_half_tiles(role, ntiles)
     return n * (ff * KDP * 2 * 2 + a_tile * KDP + TILE * KDP * 4)
+  if role in ("qkv_att_first", "qkv_att_second"):   # one tile per work item: the split-bf16 q/k/v weights, xb
+    return ffn_half_tiles(role, ntiles) * (864 * 2 * KDP * 2 + a_tile * KDP)
   return None
 
 
 def ffn_half_tiles(role, ntiles):
-  """Tiles of the FFN launch `role`: the first takes ceil(ntiles / 2), the second the rest."""
-  return (ntiles + 1) // 2 if role == "ffn_first" else ntiles // 2
+  """Tiles of the two-launch kernel `role` (FFN or q/k/v + attention): the first takes ceil(ntiles / 2), the second
+  the rest."""
+  return (ntiles + 1) // 2 if role in ("ffn_first", "qkv_att_first") else ntiles // 2
 
 
 HBM_TBPS = 3.35    # H100 SXM data sheet
@@ -83,14 +89,15 @@ HBM_TBPS = 3.35    # H100 SXM data sheet
 def hbm_bytes(role, ntiles, ff):
   """Activation bytes one FFN launch reads and writes in HBM: bf16 xb / hidden images and the fp32 residual image
   (the next layer's xb is counted for every layer).  ffn_first / ffn_second: xb in, residual in and out, next xb out
-  for the launch's half of the tiles."""
-  if role in ("ffn_first", "ffn_second"):
+  for the launch's half of the tiles.  qkv_att_first / qkv_att_second: xb in, the attention image out."""
+  if role in ("ffn_first", "ffn_second", "qkv_att_first", "qkv_att_second"):
     ntiles = ffn_half_tiles(role, ntiles)
   xb = ntiles * TILE * KDP * 2
   x = ntiles * TILE * KDP * 4
   hid = ntiles * TILE * ff * 2
   return {"ffn_up": xb + hid, "ffn_down": hid + x + x + xb,
-          "ffn_first": xb + x + x + xb, "ffn_second": xb + x + x + xb}.get(role)
+          "ffn_first": xb + x + x + xb, "ffn_second": xb + x + x + xb,
+          "qkv_att_first": xb + xb, "qkv_att_second": xb + xb}.get(role)
 
 
 def main():
@@ -158,6 +165,8 @@ def main():
   def role_of(name, prev):
     if "ffn_gemm_kernel" in name:
       return "ffn_second" if prev == "ffn_first" else "ffn_first"
+    if "qkv_attention_kernel" in name:
+      return "qkv_att_second" if prev == "qkv_att_first" else "qkv_att_first"
     m = re.search(r"gemm_kernel<(\d+), (\d+), (\d+), (true|false)>", name)
     if m:
       epi = int(m.group(3))
@@ -165,7 +174,8 @@ def main():
         return "qkv"
       if epi == 2:
         return "ffn_up"
-      return {"embed": "condenser", "attention": "out_proj", "ffn_up": "ffn_down"}.get(prev, "row_other")
+      return {"embed": "condenser", "attention": "out_proj", "qkv_att_second": "out_proj",
+              "ffn_up": "ffn_down"}.get(prev, "row_other")
     for key in ("embed", "attention", "head", "unpack", "stitch"):
       if key in name:
         return key
