@@ -492,6 +492,7 @@ struct RawRecords {
   std::vector<float> sn;          // [n_subreads][4]
   std::vector<uint32_t> cigar;
   std::vector<uint8_t> bases, pw, ip, ccs_bases, ccs_bq;
+  std::vector<int32_t> wl;        // the `wl` tag, with smart windows
   int32_t ccs_bq_any = 0;
 };
 
@@ -503,6 +504,7 @@ struct ZmwState {
   int has_ec = 0, has_np = 0, has_rq = 0, has_rg = 0;
   int32_t np_passes = 0, n_subreads = 0, ccs_length = 0;
   std::vector<int32_t> win_start; // column of every emitted window
+  std::vector<int32_t> win_width; // its spaced width (overflow when > max_length)
   RawRecords raw;                 // raw-record mode (dcb_prep_export_records): the records instead of `reads`
   int rc = DCB_OK;                // error of the processing step (message in `error`)
   std::string error;
@@ -514,7 +516,7 @@ struct ZmwJob {
   std::string name;
 };
 
-struct PrepCfg { int P = 0, L = 0, bq = 0, ins_trim = 0, R = 0; bool records = false; dcb::PackedLayout pl{}; };
+struct PrepCfg { int P = 0, L = 0, bq = 0, ins_trim = 0, R = 0; bool records = false, smart = false; dcb::PackedLayout pl{}; };
 
 // What trim_insertions would leave of a record, without building it: the trimmed cigar and the lengths of the trimmed
 // sequence and kinetics.  Follows trim_insertions to the letter: every operation but a deletion advances the sequence
@@ -589,6 +591,44 @@ int export_subread(const BamRecord& rec, int ins_trim, RawRecords* out) {
   return DCB_OK;
 }
 
+// The `wl` tag of a CCS record (`--use_ccs_smart_windows`, pre_lib.py:1329-1331): CCS bases per window.  The reference
+// fails on a missing tag, on a negative entry and on widths that do not add up to the CCS length; so does this.
+int window_lengths(const BamRecord& c, const std::string& name, std::vector<int64_t>* wl) {
+  Tag t;
+  if (!c.find("wl", &t)) return pfail(DCB_ERR_INVALID, "%s: no wl tag (needed by --use_ccs_smart_windows)", name.c_str());
+  if (t.type != 'B' || !strchr("cCsSiI", t.sub) || !t.sub)
+    return pfail(DCB_ERR_INVALID, "%s: the wl tag is not an integer array", name.c_str());
+  int64_t sum = 0;
+  wl->resize(t.count);
+  for (size_t j = 0; j < t.count; ++j) {
+    (*wl)[j] = (int64_t)BamRecord::element(t, j);
+    if ((*wl)[j] < 0) return pfail(DCB_ERR_INVALID, "%s: negative window length in the wl tag", name.c_str());
+    sum += (*wl)[j];
+  }
+  if (sum != (int64_t)c.seq.size())
+    return pfail(DCB_ERR_INVALID, "%s: the wl tag covers %lld CCS bases, the CCS read has %zu", name.c_str(), (long long)sum,
+                 c.seq.size());
+  return DCB_OK;
+}
+
+// DcExample.calculate_windows with window_widths (pre_lib.py:625-650) in closed form: window j holds the CCS bases
+// [S, S + wl[j]) with S = wl[0] + ... + wl[j-1], plus the gap columns before the last of them, i.e. the spaced columns
+// [col(S - 1) + 1, col(S + wl[j] - 1) + 1) where col(k) is the column of CCS base k (0 for S = 0).  An entry of 0 gives
+// an empty window, which iter_examples drops (n_examples_no_ccs_idx).  Requires sum(wl) == CCS length.
+void smart_windows(const Read& ccs, const std::vector<int64_t>& wl, std::vector<int32_t>* start, std::vector<int32_t>* width) {
+  std::vector<int32_t> col;
+  for (size_t i = 0; i < ccs.ccs_idx.size(); ++i)
+    if (ccs.ccs_idx[i] >= 0) col.push_back((int32_t)i);
+  int64_t s = 0;
+  for (int64_t w : wl) {
+    if (w == 0) continue;
+    const int32_t a = s ? col[s - 1] + 1 : 0, b = col[s + w - 1] + 1;
+    start->push_back(a);
+    width->push_back(b - a);
+    s += w;
+  }
+}
+
 // CPU-heavy part, no I/O: expand_clip_indent per subread, construct_ccs_read, space_out_subreads, window list
 void process_zmw(const PrepCfg& cfg, ZmwJob* job, ZmwState* st) {
   st->name = job->name;
@@ -619,15 +659,32 @@ void process_zmw(const PrepCfg& cfg, ZmwJob* job, ZmwState* st) {
   st->has_rq = c.find("rq", &t); if (st->has_rq) st->rq = (float)BamRecord::scalar(t);
   st->has_rg = c.find("RG", &t) && t.type == 'Z'; if (st->has_rg) st->rg = reinterpret_cast<const char*>(t.p);
   st->ccs_length = (int32_t)c.seq.size();
+  std::vector<int64_t> wl;
+  if (cfg.smart) {
+    const int rc = window_lengths(c, job->name, &wl);
+    if (rc) { st->rc = rc; st->error = g_prep_error; st->raw = RawRecords(); return; }
+    if (cfg.records) st->raw.wl.assign(wl.begin(), wl.end());   // each entry <= the CCS length: fits
+  }
   if (cfg.records) return;
   space_out(st->reads);
-  // DcExample.iter_examples (pre_lib.py:625-697), fixed-width windows
   const Read& ccs = st->reads.back();
   const int width = (int)ccs.bases.size();
+  st->win_start.clear();
+  st->win_width.clear();
+  if (cfg.smart) {
+    smart_windows(ccs, wl, &st->win_start, &st->win_width);
+    for (int32_t w : st->win_width)
+      if (w > cfg.L && !ccs.bq_any) {
+        st->rc = pfail(DCB_ERR_INVALID, "%s: overflow window in a CCS read without base qualities (not supported)", job->name.c_str());
+        st->error = g_prep_error;
+        return;
+      }
+    return;
+  }
+  // DcExample.iter_examples (pre_lib.py:625-697), fixed-width windows
   int ccs_width = width;
   while (ccs_width > 0 && (ccs.bases[ccs_width - 1] == ' ' || ccs.bases[ccs_width - 1] == '\t' || ccs.bases[ccs_width - 1] == '\n')) --ccs_width;
   const int nwin = (ccs_width + cfg.L - 1) / cfg.L;
-  st->win_start.clear();
   int start = 0;
   for (int w = 0; w < nwin; ++w) {
     if (start > ccs_width) break;
@@ -637,6 +694,7 @@ void process_zmw(const PrepCfg& cfg, ZmwJob* job, ZmwState* st) {
     for (int i = s0; i < std::min(s0 + cfg.L, width); ++i) any |= ccs.ccs_idx[i] >= 0;
     if (!any) continue;                                         // n_examples_no_ccs_idx
     st->win_start.push_back(s0);
+    st->win_width.push_back(std::min(cfg.L, width - s0));
   }
 }
 
@@ -855,10 +913,11 @@ int dcb_prep_get_windows(dcb_prep* p, float* rows, uint8_t* packed, int32_t* win
   const size_t nsub = st.reads.size() - 1;
   const int keep = (int)std::min<size_t>(P, nsub);
   const Read& ccs = st.reads.back();
-  const int width = (int)ccs.bases.size();
   for (size_t w = 0; w < st.win_start.size(); ++w) {
     const int s = st.win_start[w];
-    const int n = std::min(L, width - s);                      // columns present; the rest is padding
+    // columns present; the rest is padding.  An overflow window (width > L) is never scored: its rows hold its first L
+    // columns, and dcb_prep_get_overflow_ccs hands out the full-width CCS that replaces it.
+    const int n = std::min(L, st.win_width[w]);
     if (rows) {
       float* d = rows + w * (size_t)R * L;
       memset(d, 0, sizeof(float) * (size_t)R * L);
@@ -896,16 +955,63 @@ int dcb_prep_get_windows(dcb_prep* p, float* rows, uint8_t* packed, int32_t* win
     if (window_pos) {
       int32_t mn = 0;
       bool found = false;
-      for (int i = 0; i < n; ++i) {
+      for (int i = 0; i < st.win_width[w]; ++i) {
         const int32_t v = ccs.ccs_idx[s + i];
         if (v >= 0 && (!found || v < mn)) { mn = v; found = true; }
       }
       window_pos[w] = mn;                                       // ccs_bounds.start
     }
-    if (overflow) overflow[w] = 0;
+    if (overflow) overflow[w] = st.win_width[w] > L;
     if (num_passes) num_passes[w] = keep;
     if (ccs_bq)
       for (int i = 0; i < L; ++i) ccs_bq[w * (size_t)L + i] = (int16_t)((i < n && ccs.bq_any) ? ccs.bq[s + i] : -1);
+  }
+  return DCB_OK;
+}
+
+// Windows cut at the CCS record's `wl` widths instead of every max_length columns.  Call before the first
+// dcb_prep_next_zmw.  In raw-record mode the tag is checked and handed out (dcb_prep_get_window_lengths).
+int dcb_prep_use_ccs_smart_windows(dcb_prep* p, int32_t enabled) {
+  if (!p) return pfail(DCB_ERR_INVALID, "dcb_prep_use_ccs_smart_windows: null handle");
+  if (p->started || p->next_seq) return pfail(DCB_ERR_STATE, "dcb_prep_use_ccs_smart_windows: the stream has already started");
+  p->cfg.smart = enabled != 0;
+  return DCB_OK;
+}
+
+// Raw-record mode with smart windows: the loaded ZMW's `wl` tag.
+int dcb_prep_get_window_lengths(dcb_prep* p, int32_t* n, int32_t* wl) {
+  if (!p || !n) return pfail(DCB_ERR_INVALID, "dcb_prep_get_window_lengths: null argument");
+  if (!p->cfg.records || !p->cfg.smart || p->cur.raw.meta.empty())
+    return pfail(DCB_ERR_STATE, "dcb_prep_get_window_lengths: no ZMW loaded in raw-record mode with smart windows");
+  *n = (int32_t)p->cur.raw.wl.size();
+  if (wl) std::copy(p->cur.raw.wl.begin(), p->cur.raw.wl.end(), wl);
+  return DCB_OK;
+}
+
+// Spaced width of every window of the current ZMW, int32 [n_windows].
+int dcb_prep_get_window_widths(dcb_prep* p, int32_t* width) {
+  if (!p || !width) return pfail(DCB_ERR_INVALID, "dcb_prep_get_window_widths: null argument");
+  if (p->cur.reads.empty()) return pfail(DCB_ERR_STATE, "dcb_prep_get_window_widths: no ZMW loaded (or the stream is in raw-record mode)");
+  std::copy(p->cur.win_width.begin(), p->cur.win_width.end(), width);
+  return DCB_OK;
+}
+
+// The CCS of every overflow window of the current ZMW over its full width, windows back to back in window order:
+// ccs_ids u8 (0..4, ' ATCG') and ccs_bq int16 (-1 at gap columns), sum of the overflow windows' widths each.  These
+// are the feature values to_features_dict gives such a window (it is neither padded nor truncated).  Either may be NULL.
+int dcb_prep_get_overflow_ccs(dcb_prep* p, uint8_t* ccs_ids, int16_t* ccs_bq) {
+  if (!p) return pfail(DCB_ERR_INVALID, "dcb_prep_get_overflow_ccs: null handle");
+  const ZmwState& st = p->cur;
+  if (st.reads.empty()) return pfail(DCB_ERR_STATE, "dcb_prep_get_overflow_ccs: no ZMW loaded (or the stream is in raw-record mode)");
+  const Read& ccs = st.reads.back();
+  size_t o = 0;
+  for (size_t w = 0; w < st.win_start.size(); ++w) {
+    if (st.win_width[w] <= p->cfg.L) continue;
+    for (int i = 0; i < st.win_width[w]; ++i, ++o) {
+      const int c = st.win_start[w] + i;
+      if (ccs_ids) ccs_ids[o] = (uint8_t)encode_base(ccs.bases[c]);
+      if (ccs_bq) ccs_bq[o] = (int16_t)ccs.bq[c];   // overflow windows only exist where bq_any (process_zmw)
+    }
   }
   return DCB_OK;
 }

@@ -159,14 +159,16 @@ struct dcb_engine {
   } strict;
   // Host-or-device staging of the entry points besides the forward, one buffer per array, grown on demand (ensure,
   // stage_in, stage_out).  Every such call ends with a stream synchronisation, so the next one may reuse them.
-  struct {   // dcb_stitch, dcb_stitch_fastq
+  struct {   // dcb_stitch, dcb_stitch_fastq (and their _ragged forms)
     DevBuf<uint8_t> bases, quals, seq, qual, names, fastq;
     DevBuf<int32_t> start, len, pos, name_off, outcome;
-    DevBuf<int64_t> rec_off;
+    DevBuf<int64_t> rec_off, win_off;
     DevBuf<double> avg_q;
   } st;
   struct { DevBuf<int16_t> bq; DevBuf<uint8_t> mask; DevBuf<double> avg; } sk;   // dcb_skip_mask
-  struct { DevBuf<uint8_t> ids, bases, quals; DevBuf<int16_t> bq; DevBuf<int32_t> dst; DevBuf<int> status; } fs;   // dcb_fill_skipped
+  struct {   // dcb_fill_skipped(_ragged)
+    DevBuf<uint8_t> ids, bases, quals; DevBuf<int16_t> bq; DevBuf<int32_t> dst; DevBuf<int64_t> src_off, dst_off; DevBuf<int> status;
+  } fs;
   struct { DevBuf<float> probs, loss; DevBuf<uint8_t> labels, ccs, exact; DevBuf<int32_t> pred, ccs_counts; } ev;   // dcb_evaluate
   struct { DevBuf<float> teacher, student, loss, grad; } ds;   // dcb_distill_loss, dcb_distill_loss_grad
   struct { DevBuf<float> probs, loss, grad, matches, dp; DevBuf<uint8_t> labels; } lg;   // dcb_alignment_loss_grad
@@ -174,13 +176,16 @@ struct dcb_engine {
   // dcb_features_layout / dcb_features_pack: the uploaded records and the spaced state stay resident between the two
   struct {
     DevBuf<PrepZmw> zmw;
-    DevBuf<int32_t> meta, noni, gap, zmw_windows, window_pos, num_passes, list;
+    DevBuf<int32_t> meta, noni, gap, zmw_windows, window_pos, window_width, num_passes, list, wl;
+    DevBuf<int64_t> ccs_off;
     DevBuf<float> sn;
     DevBuf<uint32_t> cigar;
     DevBuf<uint8_t> bases, pw, ip, ccs_bases, ccs_bq, spaced, overflow, ccs_ids, packed;
     DevBuf<int4> op_scan, zmw_out;
-    DevBuf<int2> win_list, window;
-    DevBuf<int16_t> out_bq;
+    DevBuf<int4> win_list, window;
+    DevBuf<int16_t> out_bq, ccs_bq_full;
+    DevBuf<uint8_t> ccs_ids_full;
+    std::vector<int32_t> width;   // spaced width of every window of the resident layout
     DevBuf<int> status;
     PrepBatch batch{};
     int n_windows = -1;   // windows of the resident layout; -1: none
@@ -1184,41 +1189,68 @@ static int check_zmw_start(dcb_engine* e, const int32_t* zmw_start, int n_zmw, i
   return DCB_OK;
 }
 
-int dcb_stitch(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, int32_t n_windows, int32_t L,
-               const int32_t* zmw_start, int32_t n_zmw, uint32_t flags,
-               uint8_t* seq_out, uint8_t* qual_out, int32_t* len_out) {
-  if (!e) return DCB_ERR_INVALID;
-  if (n_windows < 0 || L <= 0 || n_zmw < 0) return fail(e, DCB_ERR_INVALID, "dcb_stitch: negative size");
+// window offsets [n + 1] of a ragged call: 0 first, non-decreasing
+static int check_offsets(dcb_engine* e, const char* fn, const int64_t* off, int n) {
+  if (!off) return fail(e, DCB_ERR_INVALID, "%s: null window offsets", fn);
+  if (off[0] != 0) return fail(e, DCB_ERR_INVALID, "%s: window offsets must start at 0", fn);
+  for (int w = 0; w < n; ++w)
+    if (off[w + 1] < off[w]) return fail(e, DCB_ERR_INVALID, "%s: window offsets must be non-decreasing", fn);
+  return DCB_OK;
+}
+
+// win_off (host, nullable): window w starts at win_off[w]; NULL: every window is L wide
+static int stitch_impl(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, const int64_t* win_off, int32_t n_windows,
+                       int32_t L, const int32_t* zmw_start, int32_t n_zmw, uint32_t flags, uint8_t* seq_out, uint8_t* qual_out,
+                       int32_t* len_out) {
   if (n_zmw == 0 || n_windows == 0) return DCB_OK;
   if (!bases || !quals || !zmw_start || !seq_out || !qual_out || !len_out) return fail(e, DCB_ERR_INVALID, "dcb_stitch: null pointer");
   int rc = check_zmw_start(e, zmw_start, n_zmw, n_windows);
   if (rc) return rc;
   CU(e, cudaSetDevice(e->cfg.device));
-  const size_t nbytes = (size_t)n_windows * L;
+  const size_t nbytes = (size_t)window_offset(win_off, n_windows, L);
   const bool in_dev = flags & DCB_ROWS_ON_DEVICE, out_dev = flags & DCB_OUT_ON_DEVICE;
   const uint8_t *db, *dq;
   const int32_t* d_start;
+  const int64_t* d_off = nullptr;
   Output<uint8_t> seq, qual;
   Output<int32_t> len;
   if ((rc = stage_in(e, e->st.bases, bases, nbytes, in_dev, &db)) || (rc = stage_in(e, e->st.quals, quals, nbytes, in_dev, &dq)) ||
       (rc = stage_in(e, e->st.start, zmw_start, (size_t)n_zmw + 1, false, &d_start)) ||
+      (win_off && (rc = stage_in(e, e->st.win_off, win_off, (size_t)n_windows + 1, false, &d_off))) ||
       (rc = stage_out(e, e->st.seq, seq_out, nbytes, out_dev, &seq)) ||
       (rc = stage_out(e, e->st.qual, qual_out, nbytes, out_dev, &qual)) ||
       (rc = stage_out(e, e->st.len, len_out, (size_t)n_zmw, out_dev, &len)))
     return rc;
-  launch_stitch(db, dq, L, d_start, n_zmw, seq.d, qual.d, len.d, e->stream);
+  launch_stitch(db, dq, L, d_off, d_start, n_zmw, seq.d, qual.d, len.d, e->stream);
   if ((rc = copy_out(e, seq)) || (rc = copy_out(e, qual)) || (rc = copy_out(e, len))) return rc;
   CU(e, cudaStreamSynchronize(e->stream));
   CU(e, cudaGetLastError());
   return DCB_OK;
 }
 
-int dcb_stitch_fastq(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, int32_t n_windows, int32_t L,
-                     const int32_t* zmw_start, int32_t n_zmw, const int32_t* window_pos, const uint8_t* names,
-                     const int32_t* name_off, double min_quality, int32_t min_length, uint32_t flags, uint8_t* fastq_out,
-                     int64_t fastq_cap, int64_t* rec_off, int32_t* outcome, double* avg_q) {
+int dcb_stitch(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, int32_t n_windows, int32_t L,
+               const int32_t* zmw_start, int32_t n_zmw, uint32_t flags,
+               uint8_t* seq_out, uint8_t* qual_out, int32_t* len_out) {
   if (!e) return DCB_ERR_INVALID;
-  if (n_windows < 0 || L <= 0 || n_zmw < 0 || fastq_cap < 0) return fail(e, DCB_ERR_INVALID, "dcb_stitch_fastq: negative size");
+  if (n_windows < 0 || L <= 0 || n_zmw < 0) return fail(e, DCB_ERR_INVALID, "dcb_stitch: negative size");
+  return stitch_impl(e, bases, quals, nullptr, n_windows, L, zmw_start, n_zmw, flags, seq_out, qual_out, len_out);
+}
+
+int dcb_stitch_ragged(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, const int64_t* win_off, int32_t n_windows,
+                      const int32_t* zmw_start, int32_t n_zmw, uint32_t flags, uint8_t* seq_out, uint8_t* qual_out,
+                      int32_t* len_out) {
+  if (!e) return DCB_ERR_INVALID;
+  if (n_windows < 0 || n_zmw < 0) return fail(e, DCB_ERR_INVALID, "dcb_stitch_ragged: negative size");
+  int rc = check_offsets(e, "dcb_stitch_ragged", win_off, n_windows);
+  if (rc) return rc;
+  return stitch_impl(e, bases, quals, win_off, n_windows, 1, zmw_start, n_zmw, flags, seq_out, qual_out, len_out);
+}
+
+static int stitch_fastq_impl(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, const int64_t* win_off,
+                             int32_t n_windows, int32_t L, const int32_t* zmw_start, int32_t n_zmw, const int32_t* window_pos,
+                             const uint8_t* names, const int32_t* name_off, double min_quality, int32_t min_length,
+                             uint32_t flags, uint8_t* fastq_out, int64_t fastq_cap, int64_t* rec_off, int32_t* outcome,
+                             double* avg_q) {
   if (!rec_off) return fail(e, DCB_ERR_INVALID, "dcb_stitch_fastq: null pointer");
   if (n_zmw == 0) { rec_off[0] = 0; return DCB_OK; }
   if (!bases || !quals || !zmw_start || !window_pos || !names || !name_off || !fastq_out || !outcome || !avg_q)
@@ -1230,15 +1262,17 @@ int dcb_stitch_fastq(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, 
   if (rc) return rc;
   CU(e, cudaSetDevice(e->cfg.device));
   cudaStream_t st = e->stream;
-  const size_t nbytes = (size_t)n_windows * L, nz = n_zmw;
+  const size_t nbytes = (size_t)window_offset(win_off, n_windows, L), nz = n_zmw;
   const bool in_dev = flags & DCB_ROWS_ON_DEVICE;
   const uint8_t *db, *dq, *d_names;
   const int32_t *d_start, *d_pos, *d_name_off;
+  const int64_t* d_off = nullptr;
   Output<int64_t> rec;
   Output<int32_t> out;
   Output<double> avg;
   if ((rc = stage_in(e, e->st.bases, bases, nbytes, in_dev, &db)) || (rc = stage_in(e, e->st.quals, quals, nbytes, in_dev, &dq)) ||
       (rc = stage_in(e, e->st.start, zmw_start, nz + 1, false, &d_start)) ||
+      (win_off && (rc = stage_in(e, e->st.win_off, win_off, (size_t)n_windows + 1, false, &d_off))) ||
       (rc = stage_in(e, e->st.pos, window_pos, (size_t)n_windows, false, &d_pos)) ||
       (rc = stage_in(e, e->st.names, names, (size_t)name_off[n_zmw], false, &d_names)) ||
       (rc = stage_in(e, e->st.name_off, name_off, nz + 1, false, &d_name_off)) ||
@@ -1247,9 +1281,9 @@ int dcb_stitch_fastq(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, 
       (rc = stage_out(e, e->st.outcome, outcome, nz, false, &out)) || (rc = stage_out(e, e->st.avg_q, avg_q, nz, false, &avg)))
     return rc;
   // concatenation + gap compaction (with no windows, every read is empty), then the filters and the records
-  launch_stitch(db, dq, L, d_start, n_zmw, e->st.seq, e->st.qual, e->st.len, st);
-  launch_read_outcome(e->st.qual, e->st.len, d_start, d_pos, L, n_zmw, e->d_p10, min_quality, min_length, out.d, avg.d, st);
-  launch_fastq(e->st.seq, e->st.qual, e->st.len, d_start, L, n_zmw, out.d, d_names, d_name_off, rec.d, e->st.fastq,
+  launch_stitch(db, dq, L, d_off, d_start, n_zmw, e->st.seq, e->st.qual, e->st.len, st);
+  launch_read_outcome(e->st.qual, e->st.len, d_off, d_start, d_pos, L, n_zmw, e->d_p10, min_quality, min_length, out.d, avg.d, st);
+  launch_fastq(e->st.seq, e->st.qual, e->st.len, d_off, d_start, L, n_zmw, out.d, d_names, d_name_off, rec.d, e->st.fastq,
                fastq_cap, st);
   if ((rc = copy_out(e, rec)) || (rc = copy_out(e, out)) || (rc = copy_out(e, avg))) return rc;
   CU(e, cudaStreamSynchronize(st));
@@ -1257,6 +1291,29 @@ int dcb_stitch_fastq(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, 
   if (rec_off[n_zmw] > 0) CU(e, cudaMemcpy(fastq_out, e->st.fastq, (size_t)rec_off[n_zmw], cudaMemcpyDeviceToHost));
   CU(e, cudaGetLastError());
   return DCB_OK;
+}
+
+int dcb_stitch_fastq(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, int32_t n_windows, int32_t L,
+                     const int32_t* zmw_start, int32_t n_zmw, const int32_t* window_pos, const uint8_t* names,
+                     const int32_t* name_off, double min_quality, int32_t min_length, uint32_t flags, uint8_t* fastq_out,
+                     int64_t fastq_cap, int64_t* rec_off, int32_t* outcome, double* avg_q) {
+  if (!e) return DCB_ERR_INVALID;
+  if (n_windows < 0 || L <= 0 || n_zmw < 0 || fastq_cap < 0) return fail(e, DCB_ERR_INVALID, "dcb_stitch_fastq: negative size");
+  return stitch_fastq_impl(e, bases, quals, nullptr, n_windows, L, zmw_start, n_zmw, window_pos, names, name_off, min_quality,
+                           min_length, flags, fastq_out, fastq_cap, rec_off, outcome, avg_q);
+}
+
+int dcb_stitch_fastq_ragged(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, const int64_t* win_off,
+                            int32_t n_windows, int32_t L, const int32_t* zmw_start, int32_t n_zmw, const int32_t* window_pos,
+                            const uint8_t* names, const int32_t* name_off, double min_quality, int32_t min_length,
+                            uint32_t flags, uint8_t* fastq_out, int64_t fastq_cap, int64_t* rec_off, int32_t* outcome,
+                            double* avg_q) {
+  if (!e) return DCB_ERR_INVALID;
+  if (n_windows < 0 || L <= 0 || n_zmw < 0 || fastq_cap < 0) return fail(e, DCB_ERR_INVALID, "dcb_stitch_fastq_ragged: negative size");
+  int rc = check_offsets(e, "dcb_stitch_fastq_ragged", win_off, n_windows);
+  if (rc) return rc;
+  return stitch_fastq_impl(e, bases, quals, win_off, n_windows, L, zmw_start, n_zmw, window_pos, names, name_off, min_quality,
+                           min_length, flags, fastq_out, fastq_cap, rec_off, outcome, avg_q);
 }
 
 int dcb_skip_mask(dcb_engine* e, const int16_t* ccs_bq, int32_t n_windows, int32_t L, double skip_windows_above,
@@ -1281,48 +1338,83 @@ int dcb_skip_mask(dcb_engine* e, const int16_t* ccs_bq, int32_t n_windows, int32
   return DCB_OK;
 }
 
-int dcb_fill_skipped(dcb_engine* e, const uint8_t* ccs_ids, const int16_t* ccs_bq, const int32_t* dst_window, int32_t k,
-                     int32_t L, int32_t calibration_enabled, double calibration_threshold, double calibration_w,
-                     double calibration_b, uint32_t flags, uint8_t* bases, uint8_t* quals) {
-  if (!e) return DCB_ERR_INVALID;
-  if (k < 0 || L <= 0) return fail(e, DCB_ERR_INVALID, "dcb_fill_skipped: negative size");
+// src_off (host, nullable): skipped window j is src_off[j] .. src_off[j + 1] of ccs_ids / ccs_bq, else j * L ..;
+// dst_off (host, nullable, [n_dst + 1]): output window d starts at dst_off[d], else d * L
+static int fill_skipped_impl(dcb_engine* e, const uint8_t* ccs_ids, const int16_t* ccs_bq, const int64_t* src_off,
+                             const int32_t* dst_window, int32_t k, const int64_t* dst_off, int32_t n_dst, int32_t L,
+                             int32_t calibration_enabled, double calibration_threshold, double calibration_w,
+                             double calibration_b, uint32_t flags, uint8_t* bases, uint8_t* quals) {
   if (k == 0) return DCB_OK;
   if (!ccs_ids || !ccs_bq || !dst_window || !bases || !quals) return fail(e, DCB_ERR_INVALID, "dcb_fill_skipped: null pointer");
-  for (int j = 0; j < k; ++j)
+  for (int j = 0; j < k; ++j) {
     if (dst_window[j] < 0) return fail(e, DCB_ERR_INVALID, "dcb_fill_skipped: negative destination window");
+    if (dst_off && dst_window[j] >= n_dst) return fail(e, DCB_ERR_INVALID, "dcb_fill_skipped: destination window outside [0, n_dst)");
+    if (dst_off && dst_off[dst_window[j] + 1] - dst_off[dst_window[j]] != src_off[j + 1] - src_off[j])
+      return fail(e, DCB_ERR_INVALID, "dcb_fill_skipped: skipped window %d and its destination differ in width", j);
+  }
   CU(e, cudaSetDevice(e->cfg.device));
   cudaStream_t st = e->stream;
-  const size_t n = (size_t)k * L;
+  const size_t n = (size_t)window_offset(src_off, k, L);
   const bool out_dev = flags & DCB_OUT_ON_DEVICE;
-  // host outputs: the kernel writes a dense [k, L] temporary, scattered into the caller's rows on the host below
+  // host outputs: the kernel writes the windows back to back as they come in (destination j, offsets src_off), and
+  // they are scattered into the caller's rows on the host below
   std::vector<int32_t> dst(dst_window, dst_window + k);
   std::vector<uint8_t> hb(out_dev ? 0 : n), hq(out_dev ? 0 : n);
   if (!out_dev) for (int j = 0; j < k; ++j) dst[j] = j;
+  const int64_t* kernel_dst_off = out_dev ? dst_off : src_off;
   const uint8_t* d_ids;
   const int16_t* d_bq;
   const int32_t* d_dst;
+  const int64_t *d_src_off = nullptr, *d_dst_off = nullptr;
   Output<uint8_t> ob, oq;
   Output<int> ostatus;
   int status = 0;
   int rc;
   if ((rc = stage_in(e, e->fs.ids, ccs_ids, n, false, &d_ids)) || (rc = stage_in(e, e->fs.bq, ccs_bq, n, false, &d_bq)) ||
       (rc = stage_in(e, e->fs.dst, dst.data(), (size_t)k, false, &d_dst)) ||
+      (src_off && (rc = stage_in(e, e->fs.src_off, src_off, (size_t)k + 1, false, &d_src_off))) ||
+      (kernel_dst_off && (rc = stage_in(e, e->fs.dst_off, kernel_dst_off, out_dev ? (size_t)n_dst + 1 : (size_t)k + 1, false,
+                                        &d_dst_off))) ||
       (rc = stage_out(e, e->fs.status, &status, 1, false, &ostatus)) ||
       (rc = stage_out(e, e->fs.bases, out_dev ? bases : hb.data(), n, out_dev, &ob)) ||
       (rc = stage_out(e, e->fs.quals, out_dev ? quals : hq.data(), n, out_dev, &oq)))
     return rc;
   CU(e, cudaMemsetAsync(ostatus.d, 0, sizeof(int), st));
-  launch_fill_skipped(d_ids, d_bq, d_dst, k, L, calibration_enabled, calibration_threshold, calibration_w, calibration_b,
-                      e->cfg.max_base_quality, ob.d, oq.d, ostatus.d, st);
+  launch_fill_skipped(d_ids, d_bq, d_src_off, d_dst, d_dst_off, k, L, (int64_t)n, calibration_enabled, calibration_threshold, calibration_w,
+                      calibration_b, e->cfg.max_base_quality, ob.d, oq.d, ostatus.d, st);
   if ((rc = copy_out(e, ostatus)) || (rc = copy_out(e, ob)) || (rc = copy_out(e, oq))) return rc;
   CU(e, cudaStreamSynchronize(st));
   for (int j = 0; j < k && !out_dev; ++j) {
-    memcpy(bases + (size_t)dst_window[j] * L, hb.data() + (size_t)j * L, L);
-    memcpy(quals + (size_t)dst_window[j] * L, hq.data() + (size_t)j * L, L);
+    const size_t s0 = (size_t)window_offset(src_off, j, L), w = (size_t)window_offset(src_off, j + 1, L) - s0;
+    const size_t o = (size_t)window_offset(dst_off, dst_window[j], L);
+    memcpy(bases + o, hb.data() + s0, w);
+    memcpy(quals + o, hq.data() + s0, w);
   }
   CU(e, cudaGetLastError());
   if (status & 1) return fail(e, DCB_ERR_INPUT_RANGE, "dcb_fill_skipped: CCS base id outside 0..4 (clamped)");
   return DCB_OK;
+}
+
+int dcb_fill_skipped(dcb_engine* e, const uint8_t* ccs_ids, const int16_t* ccs_bq, const int32_t* dst_window, int32_t k,
+                     int32_t L, int32_t calibration_enabled, double calibration_threshold, double calibration_w,
+                     double calibration_b, uint32_t flags, uint8_t* bases, uint8_t* quals) {
+  if (!e) return DCB_ERR_INVALID;
+  if (k < 0 || L <= 0) return fail(e, DCB_ERR_INVALID, "dcb_fill_skipped: negative size");
+  return fill_skipped_impl(e, ccs_ids, ccs_bq, nullptr, dst_window, k, nullptr, 0, L, calibration_enabled,
+                           calibration_threshold, calibration_w, calibration_b, flags, bases, quals);
+}
+
+int dcb_fill_skipped_ragged(dcb_engine* e, const uint8_t* ccs_ids, const int16_t* ccs_bq, const int64_t* src_off,
+                            const int32_t* dst_window, int32_t k, const int64_t* dst_off, int32_t n_dst,
+                            int32_t calibration_enabled, double calibration_threshold, double calibration_w,
+                            double calibration_b, uint32_t flags, uint8_t* bases, uint8_t* quals) {
+  if (!e) return DCB_ERR_INVALID;
+  if (k < 0 || n_dst < 0) return fail(e, DCB_ERR_INVALID, "dcb_fill_skipped_ragged: negative size");
+  int rc;
+  if ((rc = check_offsets(e, "dcb_fill_skipped_ragged", src_off, k)) || (rc = check_offsets(e, "dcb_fill_skipped_ragged", dst_off, n_dst)))
+    return rc;
+  return fill_skipped_impl(e, ccs_ids, ccs_bq, src_off, dst_window, k, dst_off, n_dst, 1, calibration_enabled,
+                           calibration_threshold, calibration_w, calibration_b, flags, bases, quals);
 }
 
 int dcb_debug_head_epilogue(dcb_engine* e, const float* logits, int64_t n, uint8_t* bases, uint8_t* quals, float* probs) {
@@ -1521,10 +1613,11 @@ int dcb_alignment_loss_grad(dcb_engine* e, const float* probs, const uint8_t* la
 // Spaced state one dcb_features_layout call may hold (bytes); a larger batch of ZMWs is split by the caller.
 static constexpr int64_t kPrepScratchMax = 1ll << 31;
 
-int dcb_features_layout(dcb_engine* e, const dcb_records* rec, int32_t ins_trim, int32_t max_windows, int32_t* zmw_windows,
-                        int32_t* window_pos, uint8_t* overflow, int16_t* ccs_bq, int32_t* num_passes, uint8_t* ccs_ids,
-                        int32_t* n_windows_out, float* ms_out) {
-  if (!e) return DCB_ERR_INVALID;
+// wl_off / wl (host, nullable): CCS smart windows, ZMW z cut at wl[wl_off[z] .. wl_off[z + 1])
+static int features_layout_impl(dcb_engine* e, const dcb_records* rec, const int32_t* wl_off, const int32_t* wl, int32_t ins_trim,
+                                int32_t max_windows, int32_t* zmw_windows, int32_t* window_pos, uint8_t* overflow,
+                                int32_t* window_width, int16_t* ccs_bq, int32_t* num_passes, uint8_t* ccs_ids,
+                                int32_t* n_windows_out, float* ms_out) {
   auto& fp = e->fp;
   fp.n_windows = -1;
   if (!rec || !n_windows_out || rec->n_zmw < 0 || max_windows < 0) return fail(e, DCB_ERR_INVALID, "dcb_features_layout: bad argument");
@@ -1542,6 +1635,7 @@ int dcb_features_layout(dcb_engine* e, const dcb_records* rec, int32_t ins_trim,
   const int n_reads = rec->zmw_read_off[nz], n_ccs = rec->zmw_ccs_off[nz];
   if (rec->zmw_read_off[0] != 0 || rec->zmw_ccs_off[0] != 0 || n_reads < 0 || n_ccs < 0 || rec->n_cigar < 0 || rec->n_query < 0)
     return fail(e, DCB_ERR_INVALID, "dcb_features_layout: bad offsets");
+  if (wl_off && (wl_off[0] != 0 || !wl)) return fail(e, DCB_ERR_INVALID, "dcb_features_layout_smart: bad window length offsets");
   std::vector<PrepZmw> zmw(nz);
   int64_t gap_total = 0, plane_total = 0, win_total = 0;
   for (int z = 0; z < nz; ++z) {
@@ -1572,6 +1666,20 @@ int dcb_features_layout(dcb_engine* e, const dcb_records* rec, int32_t ins_trim,
     zm.gap_off = gap_total; gap_total += mb + 2;
     zm.plane_off = plane_total; plane_total += bytes;
     zm.win_off = (int32_t)win_total; zm.win_cap = (int32_t)std::min<int64_t>((wb + L - 1) / L, std::max(zm.ccs_len, 1));
+    if (wl_off) {   // the reference fails on these (pre_lib.py:625-650): an AssertionError or an IndexError
+      zm.wl_off = wl_off[z]; zm.wl_n = wl_off[z + 1] - wl_off[z];
+      if (zm.wl_n < 0) return fail(e, DCB_ERR_INVALID, "dcb_features_layout_smart: window length offsets of ZMW %d decrease", z);
+      int64_t sum = 0, nonzero = 0;
+      for (int j = 0; j < zm.wl_n; ++j) {
+        if (wl[zm.wl_off + j] < 0) return fail(e, DCB_ERR_INVALID, "dcb_features_layout_smart: negative window length in ZMW %d", z);
+        sum += wl[zm.wl_off + j];
+        nonzero += wl[zm.wl_off + j] > 0;
+      }
+      if (sum != zm.ccs_len)
+        return fail(e, DCB_ERR_INVALID, "dcb_features_layout_smart: the window lengths of ZMW %d cover %lld CCS bases, its CCS read has %d",
+                    z, (long long)sum, zm.ccs_len);
+      zm.win_cap = (int32_t)nonzero;
+    }
     win_total += zm.win_cap;
   }
   CU(e, cudaSetDevice(e->cfg.device));
@@ -1589,6 +1697,8 @@ int dcb_features_layout(dcb_engine* e, const dcb_records* rec, int32_t ins_trim,
       (rc = stage_in(e, fp.ip, rec->ip, (size_t)rec->n_query, false, &b.ip)) ||
       (rc = stage_in(e, fp.ccs_bases, rec->ccs_bases, (size_t)n_ccs, false, &b.ccs_bases)) ||
       (rc = stage_in(e, fp.ccs_bq, rec->ccs_bq, (size_t)n_ccs, false, &b.ccs_bq)) ||
+      (wl_off && (rc = stage_in(e, fp.wl, wl, (size_t)wl_off[nz], false, &b.wl))) ||
+      (rc = ensure(e, fp.window_width, (size_t)win_total)) ||
       (rc = ensure(e, fp.op_scan, (size_t)rec->n_cigar + 1)) || (rc = ensure(e, fp.noni, (size_t)n_reads)) ||
       (rc = ensure(e, fp.gap, (size_t)gap_total)) || (rc = ensure(e, fp.spaced, (size_t)plane_total)) ||
       (rc = ensure(e, fp.win_list, (size_t)win_total)) || (rc = ensure(e, fp.zmw_out, (size_t)nz)) ||
@@ -1605,7 +1715,7 @@ int dcb_features_layout(dcb_engine* e, const dcb_records* rec, int32_t ins_trim,
     CU(e, cudaMemsetAsync(fp.spaced.p + zm.plane_off, 0, (size_t)zm.wb * (3 * zm.keep + 1), st));
     CU(e, cudaMemsetAsync(fp.spaced.p + zm.plane_off + (size_t)zm.wb * (3 * zm.keep + 1), 0xff, (size_t)zm.wb * 2, st));
   }
-  const PrepWindows out{fp.zmw_windows, fp.window, fp.window_pos, fp.overflow, fp.num_passes, fp.ccs_ids, fp.out_bq};
+  const PrepWindows out{fp.zmw_windows, fp.window, fp.window_pos, fp.overflow, fp.window_width, fp.num_passes, fp.ccs_ids, fp.out_bq};
   CU(e, cudaEventRecord(e->ev_eval0, st));
   launch_prep_layout(b, out, st);
   CU(e, cudaEventRecord(e->ev_eval1, st));
@@ -1615,6 +1725,8 @@ int dcb_features_layout(dcb_engine* e, const dcb_records* rec, int32_t ins_trim,
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  if (status & 4) return fail(e, DCB_ERR_INVALID, "dcb_features_layout_smart: overflow window in a CCS read without base "
+                               "qualities (not supported)");
   if (status) return fail(e, DCB_ERR_INVALID, "dcb_features_layout: a record's cigar disagrees with the columns, query bases or "
                           "insertion count its read_meta states");
   int64_t n = 0;
@@ -1627,10 +1739,33 @@ int dcb_features_layout(dcb_engine* e, const dcb_records* rec, int32_t ins_trim,
     CU(e, cudaMemcpyAsync(num_passes, fp.num_passes.p, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CU(e, cudaMemcpyAsync(ccs_ids, fp.ccs_ids.p, (size_t)n * L, cudaMemcpyDeviceToHost, st));
     CU(e, cudaMemcpyAsync(ccs_bq, fp.out_bq.p, (size_t)n * L * sizeof(int16_t), cudaMemcpyDeviceToHost, st));
+    fp.width.resize(n);
+    CU(e, cudaMemcpyAsync(fp.width.data(), fp.window_width.p, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CU(e, cudaStreamSynchronize(st));
+    if (window_width) memcpy(window_width, fp.width.data(), (size_t)n * sizeof(int32_t));
   }
   fp.n_windows = (int)n;
   return DCB_OK;
+}
+
+int dcb_features_layout(dcb_engine* e, const dcb_records* rec, int32_t ins_trim, int32_t max_windows, int32_t* zmw_windows,
+                        int32_t* window_pos, uint8_t* overflow, int16_t* ccs_bq, int32_t* num_passes, uint8_t* ccs_ids,
+                        int32_t* n_windows_out, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  return features_layout_impl(e, rec, nullptr, nullptr, ins_trim, max_windows, zmw_windows, window_pos, overflow, nullptr, ccs_bq,
+                              num_passes, ccs_ids, n_windows_out, ms_out);
+}
+
+int dcb_features_layout_smart(dcb_engine* e, const dcb_records* rec, const int32_t* wl_off, const int32_t* wl, int32_t ins_trim,
+                              int32_t max_windows, int32_t* zmw_windows, int32_t* window_pos, uint8_t* overflow,
+                              int32_t* window_width, int16_t* ccs_bq, int32_t* num_passes, uint8_t* ccs_ids,
+                              int32_t* n_windows_out, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  e->fp.n_windows = -1;
+  if (!wl_off) return fail(e, DCB_ERR_INVALID, "dcb_features_layout_smart: null window lengths");
+  if (max_windows && !window_width) return fail(e, DCB_ERR_INVALID, "dcb_features_layout_smart: null pointer");
+  return features_layout_impl(e, rec, wl_off, wl, ins_trim, max_windows, zmw_windows, window_pos, overflow, window_width, ccs_bq,
+                              num_passes, ccs_ids, n_windows_out, ms_out);
 }
 
 int dcb_features_pack(dcb_engine* e, const int32_t* windows, int32_t n, uint32_t flags, uint8_t* packed_out, float* ms_out) {
@@ -1658,6 +1793,43 @@ int dcb_features_pack(dcb_engine* e, const int32_t* windows, int32_t n, uint32_t
   launch_prep_pack(fp.batch, fp.window, d_list, n, fp.n_windows, packed.d, st);
   CU(e, cudaEventRecord(e->ev_eval1, st));
   if ((rc = copy_out(e, packed))) return rc;
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  return DCB_OK;
+}
+
+int dcb_features_ccs(dcb_engine* e, const int32_t* windows, int32_t n, const int64_t* off, uint8_t* ccs_ids, int16_t* ccs_bq,
+                     float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  auto& fp = e->fp;
+  if (ms_out) *ms_out = 0.f;
+  if (n < 0) return fail(e, DCB_ERR_INVALID, "dcb_features_ccs: negative size");
+  if (fp.n_windows < 0) return fail(e, DCB_ERR_STATE, "dcb_features_ccs before a successful dcb_features_layout");
+  if (n == 0) return DCB_OK;
+  if (!windows || !off || !ccs_ids || !ccs_bq) return fail(e, DCB_ERR_INVALID, "dcb_features_ccs: null pointer");
+  if (off[0] != 0) return fail(e, DCB_ERR_INVALID, "dcb_features_ccs: off[0] must be 0");
+  for (int i = 0; i < n; ++i) {
+    if (windows[i] < 0 || windows[i] >= fp.n_windows)
+      return fail(e, DCB_ERR_INVALID, "dcb_features_ccs: window %d outside the layout's %d windows", windows[i], fp.n_windows);
+    if (off[i + 1] - off[i] != fp.width[windows[i]])
+      return fail(e, DCB_ERR_INVALID, "dcb_features_ccs: entry %d: window %d is %d columns wide", i, windows[i], fp.width[windows[i]]);
+  }
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  const size_t total = (size_t)off[n];
+  const int32_t* d_list;
+  const int64_t* d_off;
+  Output<uint8_t> ids;
+  Output<int16_t> bq;
+  int rc;
+  if ((rc = stage_in(e, fp.list, windows, (size_t)n, false, &d_list)) || (rc = stage_in(e, fp.ccs_off, off, (size_t)n + 1, false, &d_off)) ||
+      (rc = stage_out(e, fp.ccs_ids_full, ccs_ids, total, false, &ids)) || (rc = stage_out(e, fp.ccs_bq_full, ccs_bq, total, false, &bq)))
+    return rc;
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  launch_features_ccs(fp.batch, fp.window, d_list, n, d_off, ids.d, bq.d, st);
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  if ((rc = copy_out(e, ids)) || (rc = copy_out(e, bq))) return rc;
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));

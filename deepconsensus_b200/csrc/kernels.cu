@@ -1301,19 +1301,20 @@ void launch_qkv_attention(int half, const __nv_bfloat16* xb_img, const __nv_bflo
 // =====================================================================================
 // stitch: per-read concatenation of windows + gap compaction (stitch_utils.py:51-98)
 // =====================================================================================
-// One CTA per read (ZMW).  Its windows are contiguous in the batch, so the read's input is one span of
-// (w1 - w0) * L bytes in `bases` / `quals`; the gap character ' ' and the quality character under it are dropped
-// (order preserving: ballot-free block prefix sum over 1024-character tiles) and the compacted read is written at the
-// same offset of seq_out / qual_out.  Integer / byte work only: bit-exact against the reference's string loops.
+// One CTA per read (ZMW).  Its windows are contiguous in the batch, so the read's input is one span of `bases` /
+// `quals`: window w starts at win_off[w] (windows of any width, win_off [n_windows + 1]) or, with win_off NULL, at
+// w * L.  The gap character ' ' and the quality character under it are dropped (order preserving: ballot-free block
+// prefix sum over 1024-character tiles) and the compacted read is written at the same offset of seq_out / qual_out.
+// Integer / byte work only: bit-exact against the reference's string loops.
 __global__ void __launch_bounds__(256)
 stitch_kernel(const uint8_t* __restrict__ bases, const uint8_t* __restrict__ quals, int L,
-              const int32_t* __restrict__ zmw_start, uint8_t* __restrict__ seq_out, uint8_t* __restrict__ qual_out,
-              int32_t* __restrict__ len_out) {
+              const int64_t* __restrict__ win_off, const int32_t* __restrict__ zmw_start, uint8_t* __restrict__ seq_out,
+              uint8_t* __restrict__ qual_out, int32_t* __restrict__ len_out) {
   __shared__ int s_warp[8];
   __shared__ int s_total;
   const int z = blockIdx.x;
-  const size_t off = (size_t)zmw_start[z] * L;
-  const int n = (zmw_start[z + 1] - zmw_start[z]) * L;
+  const size_t off = (size_t)window_offset(win_off, zmw_start[z], L);
+  const int n = (int)(window_offset(win_off, zmw_start[z + 1], L) - (int64_t)off);
   const uint8_t* in_b = bases + off;
   const uint8_t* in_q = quals + off;
   uint8_t* out_b = seq_out + off;
@@ -1360,9 +1361,9 @@ stitch_kernel(const uint8_t* __restrict__ bases, const uint8_t* __restrict__ qua
   if (threadIdx.x == 0) len_out[z] = running;
 }
 
-void launch_stitch(const uint8_t* bases, const uint8_t* quals, int L, const int32_t* zmw_start, int n_zmw,
-                   uint8_t* seq_out, uint8_t* qual_out, int32_t* len_out, cudaStream_t st) {
-  if (n_zmw > 0) stitch_kernel<<<n_zmw, 256, 0, st>>>(bases, quals, L, zmw_start, seq_out, qual_out, len_out);
+void launch_stitch(const uint8_t* bases, const uint8_t* quals, int L, const int64_t* win_off, const int32_t* zmw_start,
+                   int n_zmw, uint8_t* seq_out, uint8_t* qual_out, int32_t* len_out, cudaStream_t st) {
+  if (n_zmw > 0) stitch_kernel<<<n_zmw, 256, 0, st>>>(bases, quals, L, win_off, zmw_start, seq_out, qual_out, len_out);
 }
 
 void launch_head(const HeadParams& p, int ntiles, cudaStream_t st) {

@@ -38,23 +38,32 @@ void launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* att, int L, int L
 void launch_qkv_attention(int half, const __nv_bfloat16* xb_img, const __nv_bfloat16* wqkv, int L, int win,
                           int ntiles, __nv_bfloat16* qkv_img, __nv_bfloat16* att, cudaStream_t st);
 void launch_head(const HeadParams& p, int ntiles, cudaStream_t st);
+// Windows of the post-model stage are contiguous in their byte arrays: window w starts at win_off[w] (int64
+// [n_windows + 1], windows of any width) or, with win_off NULL, at w * L.
+__host__ __device__ inline int64_t window_offset(const int64_t* win_off, int w, int L) {
+  return win_off ? win_off[w] : (int64_t)w * L;
+}
 // per-read window concatenation + gap compaction; read z = windows [zmw_start[z], zmw_start[z+1]) (device pointers)
-void launch_stitch(const uint8_t* bases, const uint8_t* quals, int L, const int32_t* zmw_start, int n_zmw,
-                   uint8_t* seq_out, uint8_t* qual_out, int32_t* len_out, cudaStream_t st);
+void launch_stitch(const uint8_t* bases, const uint8_t* quals, int L, const int64_t* win_off, const int32_t* zmw_start,
+                   int n_zmw, uint8_t* seq_out, uint8_t* qual_out, int32_t* len_out, cudaStream_t st);
 
 
 // ---- post-model stage on the device (post_kernels.cu); outcome codes: DCB_READ_* of include/dcb200.h
-void launch_read_outcome(const uint8_t* qual, const int32_t* len, const int32_t* zmw_start, const int32_t* window_pos,
-                         int L, int n_zmw, const double* p10, double min_quality, int min_length, int32_t* outcome,
-                         double* avg_q, cudaStream_t st);
-void launch_fastq(const uint8_t* seq, const uint8_t* qual, const int32_t* len, const int32_t* zmw_start, int L, int n_zmw,
-                  const int32_t* outcome, const uint8_t* names, const int32_t* name_off, int64_t* rec_off, uint8_t* fastq,
-                  int64_t cap, cudaStream_t st);
+// The missing-window check counts windows: window i of a read is missing when it starts beyond i * L, whatever the
+// widths of the windows before it (stitch_utils.py:60-78).
+void launch_read_outcome(const uint8_t* qual, const int32_t* len, const int64_t* win_off, const int32_t* zmw_start,
+                         const int32_t* window_pos, int L, int n_zmw, const double* p10, double min_quality, int min_length,
+                         int32_t* outcome, double* avg_q, cudaStream_t st);
+void launch_fastq(const uint8_t* seq, const uint8_t* qual, const int32_t* len, const int64_t* win_off, const int32_t* zmw_start,
+                  int L, int n_zmw, const int32_t* outcome, const uint8_t* names, const int32_t* name_off, int64_t* rec_off,
+                  uint8_t* fastq, int64_t cap, cudaStream_t st);
 void launch_skip_mask(const int16_t* ccs_bq, int n_windows, int L, const double* p10, double thr, uint8_t* mask,
                       double* avg_out, cudaStream_t st);
-void launch_fill_skipped(const uint8_t* ccs_ids, const int16_t* ccs_bq, const int32_t* dst, int k, int L, int calib_enabled,
-                         double thr, double cw, double cb, int max_q, uint8_t* bases, uint8_t* quals, int* status,
-                         cudaStream_t st);
+// window j of the k skipped windows: src_off[j] .. src_off[j + 1] of ccs_ids / ccs_bq (j * L .. (j + 1) * L with src_off
+// NULL; total = the characters of all k), written at window_offset(dst_off, dst[j], L) of bases / quals
+void launch_fill_skipped(const uint8_t* ccs_ids, const int16_t* ccs_bq, const int64_t* src_off, const int32_t* dst,
+                         const int64_t* dst_off, int k, int L, int64_t total, int calib_enabled, double thr, double cw,
+                         double cb, int max_q, uint8_t* bases, uint8_t* quals, int* status, cudaStream_t st);
 // head_finish on final logits [n][5] (device pointer) into p.bases / p.quals / p.probs (dcb_debug_head_epilogue)
 void launch_head_epilogue(const float* logits, int n, const HeadParams& p, cudaStream_t st);
 
@@ -68,6 +77,7 @@ struct PrepZmw {
   int32_t mb;                 // bound on any read's non-insertion columns: `gap` holds mb + 2 entries
   int32_t wb;                 // bound on the spaced width, a multiple of 16
   int32_t win_off, win_cap;   // its slice of win_list
+  int32_t wl_off, wl_n;       // CCS smart windows: its window lengths wl[wl_off .. wl_off + wl_n)
   int64_t gap_off;            // element offset into gap
   int64_t plane_off;          // byte offset into spaced: u8 [keep][3][wb] base / pw / ip, u8 [wb] CCS ids, i16 [wb] CCS bq
 };
@@ -79,28 +89,34 @@ struct PrepBatch {
   const float* read_sn;
   const uint32_t* cigar;
   const uint8_t *bases, *pw, *ip, *ccs_bases, *ccs_bq;
+  const int32_t* wl;          // CCS smart windows (the `wl` tags, sum = CCS length per ZMW); NULL: fixed-width windows
   // scratch, kept from the layout to the pack calls
   int4* op_scan;              // per cigar operation: columns, non-insertion columns, query bases before it, insertion run in front
   int32_t* read_noni_qs;      // per read: non-insertion columns cut away in front of the clip
   int32_t* gap;               // zeroed before the layout: the gap widths G, then their exclusive scan E
   uint8_t* spaced;            // planes zeroed, CCS bq filled with -1 before the layout
-  int2* win_list;             // per ZMW: (start column, window_pos) of the windows that hold a CCS position
+  int4* win_list;             // per ZMW: (start column, window_pos, spaced width) of the windows that hold a CCS position
   int4* zmw_out;              // per ZMW: spaced width, ccs_width, windows, largest non-insertion count
-  int* status;                // bit 0: records exceed the bounds they were sized by; bit 1: window index out of range
+  int* status;                // bit 0: records exceed the bounds they were sized by; bit 1: window index out of range;
+                              // bit 2: an overflow window in a CCS read without base qualities
 };
 struct PrepWindows {          // dense over the batch, ZMW by ZMW
   int32_t* zmw_windows;       // [n_zmw]
-  int2* window;               // (ZMW, start column)
+  int4* window;               // (ZMW, start column, spaced width)
   int32_t* window_pos;
   uint8_t* overflow;
+  int32_t* window_width;
   int32_t* num_passes;
   uint8_t* ccs_ids;           // [n][L]
   int16_t* ccs_bq;            // [n][L]
 };
 void launch_prep_layout(const PrepBatch& b, const PrepWindows& out, cudaStream_t st);
 // packed rows of windows list[0..n_list) (indices into the layout's n_windows windows), in that order
-void launch_prep_pack(const PrepBatch& b, const int2* window, const int32_t* list, int n_list, int n_windows, uint8_t* packed,
+void launch_prep_pack(const PrepBatch& b, const int4* window, const int32_t* list, int n_list, int n_windows, uint8_t* packed,
                       cudaStream_t st);
+// the CCS ids / qualities of windows list[0..n_list) at full width, window j at off[j] of ccs_ids / ccs_bq
+void launch_features_ccs(const PrepBatch& b, const int4* window, const int32_t* list, int n_list, const int64_t* off,
+                         uint8_t* ccs_ids, int16_t* ccs_bq, cudaStream_t st);
 
 // ---- evaluation on labelled windows (eval_kernels.cu): alignment loss, exact-match flag, alignment counts [B][5] of
 // the prediction and of the CCS row.  hard_min != 0: loss_reg None.  All pointers are device pointers.

@@ -1,6 +1,8 @@
 // Post-model stage of the path on the device : what `stitch_utils.stitch_to_fastq` and the
 // skip branch of `inference_on_n_zmws` do per read / per window after the model, as integer / byte kernels.
 //
+// Windows may have any width (int64 window offsets, kernels.h window_offset); without offsets every window is L wide.
+//
 //   read_outcome_kernel   per read: missing-window check of get_full_sequence (stitch_utils.py:60-78), only-gaps check,
 //                         avg-Phred quality filter (utils.py:88-106, stitch_utils.py:101-109) and length filter
 //                         (stitch_utils.py:131-189) on the compacted read dcb_stitch's kernel wrote -> outcome code
@@ -27,8 +29,8 @@
 namespace dcb {
 
 __global__ void __launch_bounds__(256)
-read_outcome_kernel(const uint8_t* __restrict__ qual, const int32_t* __restrict__ len, const int32_t* __restrict__ zmw_start,
-                    const int32_t* __restrict__ window_pos, int L, const double* __restrict__ p10, double min_quality,
+read_outcome_kernel(const uint8_t* __restrict__ qual, const int32_t* __restrict__ len, const int64_t* __restrict__ win_off,
+                    const int32_t* __restrict__ zmw_start, const int32_t* __restrict__ window_pos, int L, const double* __restrict__ p10, double min_quality,
                     int min_length, int32_t* __restrict__ outcome, double* __restrict__ avg_q_out) {
   __shared__ int s_hist[256];
   __shared__ int s_missing;
@@ -41,7 +43,7 @@ read_outcome_kernel(const uint8_t* __restrict__ qual, const int32_t* __restrict_
   for (int i = threadIdx.x; i < w1 - w0; i += blockDim.x)
     if (window_pos[w0 + i] > i * L) s_missing = 1;
   const int n = len[z];
-  const uint8_t* q = qual + (size_t)w0 * L;
+  const uint8_t* q = qual + window_offset(win_off, w0, L);
   for (int i = threadIdx.x; i < n; i += blockDim.x) atomicAdd(&s_hist[q[i]], 1);   // integer atomics: exact
   __syncthreads();
   if (threadIdx.x != 0) return;
@@ -98,7 +100,7 @@ fastq_layout_kernel(const int32_t* __restrict__ len, const int32_t* __restrict__
 
 __global__ void __launch_bounds__(256)
 fastq_write_kernel(const uint8_t* __restrict__ seq, const uint8_t* __restrict__ qual, const int32_t* __restrict__ len,
-                   const int32_t* __restrict__ zmw_start, int L, const int32_t* __restrict__ outcome,
+                   const int64_t* __restrict__ win_off, const int32_t* __restrict__ zmw_start, int L, const int32_t* __restrict__ outcome,
                    const uint8_t* __restrict__ names, const int32_t* __restrict__ name_off,
                    const int64_t* __restrict__ rec_off, uint8_t* __restrict__ fastq, int64_t cap) {
   const int z = blockIdx.x;
@@ -106,8 +108,8 @@ fastq_write_kernel(const uint8_t* __restrict__ seq, const uint8_t* __restrict__ 
   const int n = len[z], nl = name_off[z + 1] - name_off[z];
   const int64_t o = rec_off[z];
   if (o + nl + 2ll * n + 6 > cap) return;                  // caller sized the buffer too small: rec_off[n_zmw] tells
-  const uint8_t* s = seq + (size_t)zmw_start[z] * L;
-  const uint8_t* q = qual + (size_t)zmw_start[z] * L;
+  const uint8_t* s = seq + window_offset(win_off, zmw_start[z], L);
+  const uint8_t* q = qual + window_offset(win_off, zmw_start[z], L);
   const uint8_t* nm = names + name_off[z];
   uint8_t* out = fastq + o;
   if (threadIdx.x == 0) {
@@ -143,21 +145,46 @@ skip_mask_kernel(const int16_t* __restrict__ ccs_bq, int n_windows, int L, const
   if (avg_out) avg_out[w] = avg;
 }
 
-// process_skipped_window for k windows: window j goes to row dst[j] of the [*, L] output arrays
+// process_skipped_window for k windows, one thread per character: window j (src_off[j] .. src_off[j + 1] of the inputs,
+// found by binary search, or j * L .. (j + 1) * L) is written at window_offset(dst_off, dst[j], L) of the output arrays
 __global__ void __launch_bounds__(256)
-fill_skipped_kernel(const uint8_t* __restrict__ ccs_ids, const int16_t* __restrict__ ccs_bq, const int32_t* __restrict__ dst,
-                    int k, int L, int calib_enabled, double thr, double cw, double cb, int max_q,
-                    uint8_t* __restrict__ bases, uint8_t* __restrict__ quals, int* __restrict__ status) {
-  const char vocab[5] = {' ', 'A', 'T', 'C', 'G'};
-  const long long total = (long long)k * L;
+fill_skipped_kernel(const uint8_t* __restrict__ ccs_ids, const int16_t* __restrict__ ccs_bq, const int64_t* __restrict__ src_off,
+                    const int32_t* __restrict__ dst, const int64_t* __restrict__ dst_off, int k, int L, int calib_enabled,
+                    double thr, double cw, double cb, int max_q, uint8_t* __restrict__ bases, uint8_t* __restrict__ quals,
+                    int* __restrict__ status) {
+  constexpr unsigned long long kIdChars = 0x4743544120ull;   // ' ', 'A', 'T', 'C', 'G' from the low byte up: no stack array
+  const long long total = window_offset(src_off, k, L);
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int j = (int)(i / L), l = (int)(i - (long long)j * L);
+    int j;
+    if (src_off) {                                       // the last window starting at or before i
+      int lo = 0, hi = k;
+      while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (src_off[mid] <= i) lo = mid; else hi = mid; }
+      j = lo;
+    } else {
+      j = (int)(i / L);
+    }
+    const long long l = i - window_offset(src_off, j, L);
     int id = ccs_ids[i];
     if (id > 4) { atomicOr(status, 1); id = 4; }
     const int qi = ccs_quality(ccs_bq[i], calib_enabled, thr, cw, cb, max_q);   // quality.cuh
-    const size_t o = (size_t)dst[j] * L + l;
-    bases[o] = (uint8_t)vocab[id];
+    const long long o = window_offset(dst_off, dst[j], L) + l;
+    bases[o] = (uint8_t)(kIdChars >> (8 * id));
     quals[o] = (uint8_t)(qi + 33);                      // quality_scores_to_string (utils.py:60-62)
+  }
+}
+
+// Feature construction on the device, after dcb_features_layout (prep_kernels.cu): one CTA per listed window copies its
+// CCS ids and qualities at full width out of the spaced CCS planes (overflow windows, which are never packed)
+__global__ void __launch_bounds__(256) features_ccs_kernel(PrepBatch b, const int4* window, const int32_t* list, const int64_t* off,
+                                                           uint8_t* ccs_ids_out, int16_t* ccs_bq_out) {
+  const int4 wz = window[list[blockIdx.x]];
+  const PrepZmw zm = b.zmw[wz.x];
+  const uint8_t* ccs_ids = b.spaced + zm.plane_off + (size_t)zm.keep * 3 * zm.wb;
+  const int16_t* ccs_bq = reinterpret_cast<const int16_t*>(ccs_ids + zm.wb);
+  const int64_t o = off[blockIdx.x];
+  for (int i = threadIdx.x; i < wz.z; i += blockDim.x) {
+    ccs_ids_out[o + i] = ccs_ids[wz.y + i];
+    ccs_bq_out[o + i] = ccs_bq[wz.y + i];
   }
 }
 
@@ -176,18 +203,20 @@ void launch_head_epilogue(const float* logits, int n, const HeadParams& p, cudaS
   if (n > 0) head_epilogue_kernel<<<(n + 255) / 256, 256, 0, st>>>(logits, n, p);
 }
 
-void launch_read_outcome(const uint8_t* qual, const int32_t* len, const int32_t* zmw_start, const int32_t* window_pos,
-                         int L, int n_zmw, const double* p10, double min_quality, int min_length, int32_t* outcome,
-                         double* avg_q, cudaStream_t st) {
-  if (n_zmw > 0) read_outcome_kernel<<<n_zmw, 256, 0, st>>>(qual, len, zmw_start, window_pos, L, p10, min_quality, min_length, outcome, avg_q);
+void launch_read_outcome(const uint8_t* qual, const int32_t* len, const int64_t* win_off, const int32_t* zmw_start,
+                         const int32_t* window_pos, int L, int n_zmw, const double* p10, double min_quality, int min_length,
+                         int32_t* outcome, double* avg_q, cudaStream_t st) {
+  if (n_zmw > 0)
+    read_outcome_kernel<<<n_zmw, 256, 0, st>>>(qual, len, win_off, zmw_start, window_pos, L, p10, min_quality, min_length,
+                                               outcome, avg_q);
 }
 
-void launch_fastq(const uint8_t* seq, const uint8_t* qual, const int32_t* len, const int32_t* zmw_start, int L, int n_zmw,
-                  const int32_t* outcome, const uint8_t* names, const int32_t* name_off, int64_t* rec_off, uint8_t* fastq,
-                  int64_t cap, cudaStream_t st) {
+void launch_fastq(const uint8_t* seq, const uint8_t* qual, const int32_t* len, const int64_t* win_off, const int32_t* zmw_start,
+                  int L, int n_zmw, const int32_t* outcome, const uint8_t* names, const int32_t* name_off, int64_t* rec_off,
+                  uint8_t* fastq, int64_t cap, cudaStream_t st) {
   if (n_zmw <= 0) return;
   fastq_layout_kernel<<<1, 1024, 0, st>>>(len, outcome, name_off, n_zmw, rec_off);
-  fastq_write_kernel<<<n_zmw, 256, 0, st>>>(seq, qual, len, zmw_start, L, outcome, names, name_off, rec_off, fastq, cap);
+  fastq_write_kernel<<<n_zmw, 256, 0, st>>>(seq, qual, len, win_off, zmw_start, L, outcome, names, name_off, rec_off, fastq, cap);
 }
 
 void launch_skip_mask(const int16_t* ccs_bq, int n_windows, int L, const double* p10, double thr, uint8_t* mask,
@@ -195,13 +224,18 @@ void launch_skip_mask(const int16_t* ccs_bq, int n_windows, int L, const double*
   if (n_windows > 0) skip_mask_kernel<<<(n_windows + 7) / 8, 256, 0, st>>>(ccs_bq, n_windows, L, p10, thr, mask, avg_out);
 }
 
-void launch_fill_skipped(const uint8_t* ccs_ids, const int16_t* ccs_bq, const int32_t* dst, int k, int L, int calib_enabled,
-                         double thr, double cw, double cb, int max_q, uint8_t* bases, uint8_t* quals, int* status,
-                         cudaStream_t st) {
-  if (k <= 0) return;
-  const long long total = (long long)k * L;
+void launch_fill_skipped(const uint8_t* ccs_ids, const int16_t* ccs_bq, const int64_t* src_off, const int32_t* dst,
+                         const int64_t* dst_off, int k, int L, int64_t total, int calib_enabled, double thr, double cw,
+                         double cb, int max_q, uint8_t* bases, uint8_t* quals, int* status, cudaStream_t st) {
+  if (k <= 0 || total <= 0) return;
   const int grid = (int)((total + 255) / 256 < 1184 ? (total + 255) / 256 : 1184);
-  fill_skipped_kernel<<<grid, 256, 0, st>>>(ccs_ids, ccs_bq, dst, k, L, calib_enabled, thr, cw, cb, max_q, bases, quals, status);
+  fill_skipped_kernel<<<grid, 256, 0, st>>>(ccs_ids, ccs_bq, src_off, dst, dst_off, k, L, calib_enabled, thr, cw, cb, max_q,
+                                            bases, quals, status);
+}
+
+void launch_features_ccs(const PrepBatch& b, const int4* window, const int32_t* list, int n_list, const int64_t* off,
+                         uint8_t* ccs_ids, int16_t* ccs_bq, cudaStream_t st) {
+  if (n_list > 0) features_ccs_kernel<<<n_list, 256, 0, st>>>(b, window, list, off, ccs_ids, ccs_bq);
 }
 
 }  // namespace dcb

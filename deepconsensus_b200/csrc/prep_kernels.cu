@@ -208,25 +208,51 @@ __global__ void __launch_bounds__(kPrepThreads) prep_layout_kernel(PrepBatch b) 
     if (zm.bq_any) ccs_bq[col] = b.ccs_bq[zm.ccs_off + j];   // pre_lib.py:247-250: all-zero qualities stay unspaced
   }
 
-  // ---- windows of L columns over the CCS read's extent; one without a CCS position is dropped
   const int L = b.pl.L;
   const int ccs_width = zm.ccs_len ? zm.ccs_len - 1 + E[zm.ccs_len] + 1 : 0;
-  const int nwin = (ccs_width + L - 1) / L;
-  const int per = (nwin + kPrepThreads - 1) / kPrepThreads;
-  const int lo = min(tid * per, nwin), hi = min(lo + per, nwin);
-  auto first_ccs = [&](int start) {   // the first CCS position at or after spaced column `start`
-    int a = 0, c = zm.ccs_len;
-    while (a < c) { const int mid = (a + c) >> 1; if (mid + E[mid + 1] < start) a = mid + 1; else c = mid; }
-    return a;
-  };
-  int kept = 0;
-  for (int w = lo; w < hi; ++w) { const int j = first_ccs(w * L); kept += j < zm.ccs_len && j + E[j + 1] < w * L + L; }
-  int at = block_scan(kept, 0, sh_int, [](int a, int c) { return a + c; });
-  const int n_win = sh_int[kPrepThreads - 1];
-  if (n_win > zm.win_cap) { if (tid == 0) { *b.status |= 1; b.zmw_out[z] = make_int4(0, 0, 0, 0); } return; }
-  for (int w = lo; w < hi; ++w) {
-    const int j = first_ccs(w * L);
-    if (j < zm.ccs_len && j + E[j + 1] < w * L + L) { b.win_list[zm.win_off + at] = make_int2(w * L, j); ++at; }
+  int n_win;
+  if (b.wl) {
+    // ---- CCS smart windows (pre_lib.py:625-650): window j holds the CCS bases [S, S + wl[j]), S the exclusive scan
+    // of wl, i.e. the columns [col(S - 1) + 1, col(S + wl[j] - 1) + 1) with col(k) = k + E[k + 1]; wl[j] = 0 gives none
+    const int32_t* wl = b.wl + zm.wl_off;
+    const int per = (zm.wl_n + kPrepThreads - 1) / kPrepThreads;
+    const int lo = min(tid * per, zm.wl_n), hi = min(lo + per, zm.wl_n);
+    int sum = 0, kept = 0;
+    for (int j = lo; j < hi; ++j) { sum += wl[j]; kept += wl[j] > 0; }
+    int s = block_scan(sum, 0, sh_int, [](int a, int c) { return a + c; });
+    __syncthreads();
+    int at = block_scan(kept, 0, sh_int, [](int a, int c) { return a + c; });
+    n_win = sh_int[kPrepThreads - 1];
+    if (n_win > zm.win_cap) { if (tid == 0) { *b.status |= 1; b.zmw_out[z] = make_int4(0, 0, 0, 0); } return; }
+    bool bad = false;
+    for (int j = lo; j < hi; ++j) {
+      if (wl[j] <= 0) continue;
+      const int a = s ? s - 1 + E[s] + 1 : 0, e_ = s + wl[j] - 1 + E[s + wl[j]] + 1;
+      b.win_list[zm.win_off + at] = make_int4(a, s, e_ - a, 0);
+      bad |= e_ - a > L && !zm.bq_any;
+      ++at;
+      s += wl[j];
+    }
+    if (bad) *b.status |= 4;
+  } else {
+    // ---- windows of L columns over the CCS read's extent; one without a CCS position is dropped
+    const int nwin = (ccs_width + L - 1) / L;
+    const int per = (nwin + kPrepThreads - 1) / kPrepThreads;
+    const int lo = min(tid * per, nwin), hi = min(lo + per, nwin);
+    auto first_ccs = [&](int start) {   // the first CCS position at or after spaced column `start`
+      int a = 0, c = zm.ccs_len;
+      while (a < c) { const int mid = (a + c) >> 1; if (mid + E[mid + 1] < start) a = mid + 1; else c = mid; }
+      return a;
+    };
+    int kept = 0;
+    for (int w = lo; w < hi; ++w) { const int j = first_ccs(w * L); kept += j < zm.ccs_len && j + E[j + 1] < w * L + L; }
+    int at = block_scan(kept, 0, sh_int, [](int a, int c) { return a + c; });
+    n_win = sh_int[kPrepThreads - 1];
+    if (n_win > zm.win_cap) { if (tid == 0) { *b.status |= 1; b.zmw_out[z] = make_int4(0, 0, 0, 0); } return; }
+    for (int w = lo; w < hi; ++w) {
+      const int j = first_ccs(w * L);
+      if (j < zm.ccs_len && j + E[j + 1] < w * L + L) { b.win_list[zm.win_off + at] = make_int4(w * L, j, min(L, width - w * L), 0); ++at; }
+    }
   }
   if (tid == 0) b.zmw_out[z] = make_int4(width, ccs_width, n_win, mmax);
 }
@@ -242,36 +268,38 @@ __global__ void __launch_bounds__(256) prep_emit_kernel(PrepBatch b, PrepWindows
   const int z = blockIdx.x;
   const PrepZmw zm = b.zmw[z];
   const int4 zo = b.zmw_out[z];
-  const int base = window_base(b.zmw_out, z), L = b.pl.L, width = zo.x;
+  const int base = window_base(b.zmw_out, z), L = b.pl.L;
   const uint8_t* ccs_ids = b.spaced + zm.plane_off + (size_t)zm.keep * 3 * zm.wb;
   const int16_t* ccs_bq = reinterpret_cast<const int16_t*>(ccs_ids + zm.wb);
   if (threadIdx.x == 0) out.zmw_windows[z] = zo.z;
   for (int w = threadIdx.x; w < zo.z; w += blockDim.x) {
-    const int2 wl = b.win_list[zm.win_off + w];
-    out.window[base + w] = make_int2(z, wl.x);
+    const int4 wl = b.win_list[zm.win_off + w];
+    out.window[base + w] = make_int4(z, wl.x, wl.z, 0);
     out.window_pos[base + w] = wl.y;
-    out.overflow[base + w] = 0;
+    out.overflow[base + w] = wl.z > L;
+    out.window_width[base + w] = wl.z;
     out.num_passes[base + w] = zm.keep;
   }
-  for (int t = threadIdx.x; t < zo.z * L; t += blockDim.x) {
+  for (int t = threadIdx.x; t < zo.z * L; t += blockDim.x) {   // padding starts at the window's own width
     const int w = t / L, i = t - w * L;
-    const int c = b.win_list[zm.win_off + w].x + i;
-    out.ccs_ids[(size_t)(base + w) * L + i] = c < width ? ccs_ids[c] : 0;
-    out.ccs_bq[(size_t)(base + w) * L + i] = c < width ? ccs_bq[c] : (int16_t)-1;
+    const int4 wl = b.win_list[zm.win_off + w];
+    const int c = wl.x + i;
+    out.ccs_ids[(size_t)(base + w) * L + i] = i < wl.z ? ccs_ids[c] : 0;
+    out.ccs_bq[(size_t)(base + w) * L + i] = i < wl.z ? ccs_bq[c] : (int16_t)-1;
   }
 }
 
 // One CTA per listed window: the packed row is assembled in shared memory and leaves in 16-byte stores.
-__global__ void __launch_bounds__(256) prep_pack_kernel(PrepBatch b, const int2* window, const int32_t* list, int n_windows,
+__global__ void __launch_bounds__(256) prep_pack_kernel(PrepBatch b, const int4* window, const int32_t* list, int n_windows,
                                                         uint8_t* packed, int* status) {
   extern __shared__ uint4 sh_row[];
   uint8_t* row = reinterpret_cast<uint8_t*>(sh_row);
   const int idx = list[blockIdx.x];
   if (idx < 0 || idx >= n_windows) { if (threadIdx.x == 0) *status |= 2; return; }
-  const int2 wz = window[idx];
+  const int4 wz = window[idx];
   const PrepZmw zm = b.zmw[wz.x];
   const int P = b.pl.P, L = b.pl.L, start = wz.y;
-  const int n = min(L, b.zmw_out[wz.x].x - start);   // columns present; the rest is padding
+  const int n = min(L, wz.z);   // columns present (an overflow window's first L); the rest is padding
   for (int t = threadIdx.x; t < b.pl.stride / 16; t += blockDim.x) sh_row[t] = make_uint4(0, 0, 0, 0);
   __syncthreads();
   const uint8_t* planes = b.spaced + zm.plane_off;
@@ -302,7 +330,7 @@ void launch_prep_layout(const PrepBatch& b, const PrepWindows& out, cudaStream_t
   prep_emit_kernel<<<b.n_zmw, 256, 0, st>>>(b, out);
 }
 
-void launch_prep_pack(const PrepBatch& b, const int2* window, const int32_t* list, int n_list, int n_windows, uint8_t* packed,
+void launch_prep_pack(const PrepBatch& b, const int4* window, const int32_t* list, int n_list, int n_windows, uint8_t* packed,
                       cudaStream_t st) {
   if (n_list == 0) return;
   prep_pack_kernel<<<n_list, 256, b.pl.stride, st>>>(b, window, list, n_windows, packed, b.status);

@@ -95,9 +95,12 @@ class DcbRecords(ctypes.Structure):
 ABI_SYMBOLS = (
     "dcb_create", "dcb_load_weights", "dcb_forward", "dcb_submit", "dcb_wait", "dcb_stitch", "dcb_last_forward_ms",
     "dcb_packed_window_bytes", "dcb_pack_rows", "dcb_forward_packed", "dcb_submit_packed",
-    "dcb_stitch_fastq", "dcb_skip_mask", "dcb_fill_skipped", "dcb_evaluate", "dcb_distill_loss",
+    "dcb_stitch_fastq", "dcb_skip_mask", "dcb_fill_skipped", "dcb_stitch_ragged", "dcb_stitch_fastq_ragged",
+    "dcb_fill_skipped_ragged", "dcb_evaluate", "dcb_distill_loss",
     "dcb_alignment_loss_grad", "dcb_distill_loss_grad", "dcb_prep_open", "dcb_prep_set_threads", "dcb_prep_next_zmw", "dcb_prep_get_windows", "dcb_prep_ccs_header", "dcb_prep_close",
-    "dcb_prep_last_error", "dcb_prep_export_records", "dcb_prep_get_records", "dcb_features_layout", "dcb_features_pack",
+    "dcb_prep_last_error", "dcb_prep_export_records", "dcb_prep_get_records", "dcb_prep_use_ccs_smart_windows",
+    "dcb_prep_get_window_widths", "dcb_prep_get_overflow_ccs", "dcb_features_layout", "dcb_features_pack",
+    "dcb_features_layout_smart", "dcb_features_ccs", "dcb_prep_get_window_lengths",
     "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
     "dcb_last_forward_launches", "dcb_set_profile", "dcb_get_profile", "dcb_get_profile_kernels", "dcb_alloc_host",
     "dcb_free_host", "dcb_alloc_device", "dcb_free_device", "dcb_memcpy_h2d", "dcb_memcpy_d2h",
@@ -155,6 +158,10 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_stitch_fastq.argtypes = [vp, vp, vp, i32, i32, vp, i32, vp, vp, vp, f64, i32, u32, vp, ctypes.c_int64, vp, vp, vp]
   lib.dcb_skip_mask.argtypes = [vp, vp, i32, i32, f64, vp, vp]
   lib.dcb_fill_skipped.argtypes = [vp, vp, vp, vp, i32, i32, i32, f64, f64, f64, u32, vp, vp]
+  lib.dcb_stitch_ragged.argtypes = [vp, vp, vp, vp, i32, vp, i32, u32, vp, vp, vp]
+  lib.dcb_stitch_fastq_ragged.argtypes = [vp, vp, vp, vp, i32, i32, vp, i32, vp, vp, vp, f64, i32, u32, vp, ctypes.c_int64, vp,
+                                          vp, vp]
+  lib.dcb_fill_skipped_ragged.argtypes = [vp, vp, vp, vp, vp, i32, vp, i32, i32, f64, f64, f64, u32, vp, vp]
   lib.dcb_evaluate.argtypes = [vp, vp, vp, vp, i32, i32, f64, f64, i32, u32, vp, vp, vp, vp,
                                ctypes.POINTER(ctypes.c_float)]
   lib.dcb_distill_loss.argtypes = [vp, vp, vp, i32, i32, f64, i32, u32, vp, ctypes.POINTER(ctypes.c_float)]
@@ -164,6 +171,9 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_features_layout.argtypes = [vp, ctypes.POINTER(DcbRecords), i32, i32, vp, vp, vp, vp, vp, vp, ctypes.POINTER(i32),
                                       ctypes.POINTER(ctypes.c_float)]
   lib.dcb_features_pack.argtypes = [vp, vp, i32, u32, vp, ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_features_layout_smart.argtypes = [vp, ctypes.POINTER(DcbRecords), vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp,
+                                            ctypes.POINTER(i32), ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_features_ccs.argtypes = [vp, vp, i32, vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_launches.argtypes = [vp, ctypes.POINTER(i32)]
   lib.dcb_set_debug.argtypes = [vp, i32]
@@ -483,39 +493,54 @@ class B200Model:
 
   # -- stitch: per-read window concatenation + gap compaction on the device -------------------------
   def stitch(self, bases, quals, zmw_start: np.ndarray, n_windows: Optional[int] = None,
-             on_device: bool = False, length: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+             on_device: bool = False, length: Optional[int] = None, win_off: Optional[np.ndarray] = None
+             ) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
     """dcb_stitch: bases/quals are uint8 [n_windows, L] arrays (or device addresses when `on_device`); read z is the
     windows [zmw_start[z], zmw_start[z+1]).  Returns (seq, qual, lengths): read z's compacted characters are
-    seq[zmw_start[z] * L : zmw_start[z] * L + lengths[z]] (same for qual)."""
+    seq[zmw_start[z] * L : zmw_start[z] * L + lengths[z]] (same for qual).  With `win_off` (int64 [n_windows + 1]),
+    dcb_stitch_ragged: window w is bytes win_off[w] .. win_off[w + 1] of the flat bases / quals, and read z starts at
+    win_off[zmw_start[z]]."""
     zs = np.ascontiguousarray(zmw_start, dtype=np.int32)
     nz = int(zs.shape[0]) - 1
     L = int(length) if length is not None else self.max_length   # characters per window
-    if on_device and n_windows is None:
+    if on_device and n_windows is None and win_off is None:
       raise ValueError("stitch(on_device=True) needs n_windows")
     b_ptr, bases = _arg(bases, np.uint8, on_device)
     q_ptr, quals = _arg(quals, np.uint8, on_device)
+    flags = DCB_ROWS_ON_DEVICE if on_device else 0
+    lens = np.zeros(max(nz, 0), np.int32)
+    if win_off is not None:
+      off = np.ascontiguousarray(win_off, dtype=np.int64)
+      seq, qual = np.empty(int(off[-1]), np.uint8), np.empty(int(off[-1]), np.uint8)
+      self._check(self._lib.dcb_stitch_ragged(self._handle, b_ptr, q_ptr, _ptr(off), len(off) - 1, _ptr(zs), nz, flags,
+                                              _ptr(seq), _ptr(qual), _ptr(lens)))
+      return seq, qual, lens
     if not on_device:
       n_windows = int(bases.shape[0])
     seq = np.empty(n_windows * L, np.uint8)
     qual = np.empty(n_windows * L, np.uint8)
-    lens = np.zeros(max(nz, 0), np.int32)
-    self._check(self._lib.dcb_stitch(self._handle, b_ptr, q_ptr, n_windows, L, _ptr(zs), nz,
-                                     DCB_ROWS_ON_DEVICE if on_device else 0, _ptr(seq), _ptr(qual), _ptr(lens)))
+    self._check(self._lib.dcb_stitch(self._handle, b_ptr, q_ptr, n_windows, L, _ptr(zs), nz, flags, _ptr(seq), _ptr(qual),
+                                     _ptr(lens)))
     return seq, qual, lens
 
   def stitch_fastq(self, bases, quals, zmw_start: np.ndarray, window_pos, names, min_quality: float, min_length: int,
-                   n_windows: Optional[int] = None, on_device: bool = False, length: Optional[int] = None):
+                   n_windows: Optional[int] = None, on_device: bool = False, length: Optional[int] = None,
+                   win_off: Optional[np.ndarray] = None):
     """dcb_stitch_fastq: stitch_utils.stitch_to_fastq for a batch of reads on the device.  Returns (fastq bytes,
     rec_off int64 [n_zmw + 1], outcome int32 [n_zmw], avg_q float64 [n_zmw]); read z's record is
-    fastq[rec_off[z]:rec_off[z + 1]] (empty unless outcome[z] & 0x7f == DCB_READ_OK)."""
+    fastq[rec_off[z]:rec_off[z + 1]] (empty unless outcome[z] & 0x7f == DCB_READ_OK).  With `win_off` (int64
+    [n_windows + 1]), dcb_stitch_fastq_ragged on windows of any width (see `stitch`)."""
     zs = np.ascontiguousarray(zmw_start, dtype=np.int32)
     nz = int(zs.shape[0]) - 1
     L = int(length) if length is not None else self.max_length
-    if on_device and n_windows is None:
+    if on_device and n_windows is None and win_off is None:
       raise ValueError("stitch_fastq(on_device=True) needs n_windows")
     b_ptr, bases = _arg(bases, np.uint8, on_device)
     q_ptr, quals = _arg(quals, np.uint8, on_device)
-    if not on_device:
+    off = None if win_off is None else np.ascontiguousarray(win_off, dtype=np.int64)
+    if off is not None:
+      n_windows = len(off) - 1
+    elif not on_device:
       n_windows = int(bases.shape[0])
     pos = np.ascontiguousarray(window_pos, dtype=np.int32)
     if pos.shape[0] != n_windows:
@@ -527,15 +552,17 @@ class B200Model:
     if nz:
       name_off[1:] = np.cumsum([len(x) for x in enc])
     blob = np.frombuffer(b"".join(enc) or b"\0", np.uint8)
-    cap = int(name_off[-1]) + 2 * n_windows * L + 6 * nz + 16
+    cap = int(name_off[-1]) + 2 * (n_windows * L if off is None else int(off[-1])) + 6 * nz + 16
     fastq = np.empty(cap, np.uint8)
     rec_off = np.zeros(nz + 1, np.int64)
     outcome = np.zeros(max(nz, 0), np.int32)
     avg_q = np.zeros(max(nz, 0), np.float64)
-    self._check(self._lib.dcb_stitch_fastq(self._handle, b_ptr, q_ptr, n_windows, L, _ptr(zs), nz, _ptr(pos),
-                                           _ptr(blob), _ptr(name_off), float(min_quality), int(min_length),
-                                           DCB_ROWS_ON_DEVICE if on_device else 0, _ptr(fastq), cap, _ptr(rec_off),
-                                           _ptr(outcome), _ptr(avg_q)))
+    tail = (_ptr(zs), nz, _ptr(pos), _ptr(blob), _ptr(name_off), float(min_quality), int(min_length),
+            DCB_ROWS_ON_DEVICE if on_device else 0, _ptr(fastq), cap, _ptr(rec_off), _ptr(outcome), _ptr(avg_q))
+    if off is None:
+      self._check(self._lib.dcb_stitch_fastq(self._handle, b_ptr, q_ptr, n_windows, L, *tail))
+    else:
+      self._check(self._lib.dcb_stitch_fastq_ragged(self._handle, b_ptr, q_ptr, _ptr(off), n_windows, L, *tail))
     return fastq[:int(rec_off[-1])].tobytes(), rec_off, outcome, avg_q
 
   def skip_mask(self, ccs_base_quality_scores: np.ndarray, skip_windows_above: float) -> Tuple[np.ndarray, np.ndarray]:
@@ -572,13 +599,38 @@ class B200Model:
                                            float(cal.b) if en else 0.0, DCB_OUT_ON_DEVICE if on_device else 0,
                                            _ptr(bases), _ptr(quals)))
 
+  def fill_skipped_ragged(self, ccs_ids: np.ndarray, ccs_base_quality_scores: np.ndarray, src_off: np.ndarray,
+                          dst_window: np.ndarray, dst_off: np.ndarray, bases: np.ndarray, quals: np.ndarray,
+                          calibration: Optional[calibration_lib.QualityCalibrationValues] = None) -> None:
+    """dcb_fill_skipped_ragged: `fill_skipped` on windows of any width.  Skipped window j is ccs_ids /
+    ccs_base_quality_scores[src_off[j]:src_off[j + 1]] (flat uint8 / int16) and is written to window dst_window[j] of
+    the flat `bases` / `quals`, whose windows are dst_off (int64 [n_dst + 1]); the two widths must agree."""
+    ids = np.ascontiguousarray(ccs_ids, dtype=np.uint8).reshape(-1)
+    bq = np.ascontiguousarray(ccs_base_quality_scores, dtype=np.int16).reshape(-1)
+    so, do = np.ascontiguousarray(src_off, dtype=np.int64), np.ascontiguousarray(dst_off, dtype=np.int64)
+    dst = np.ascontiguousarray(dst_window, dtype=np.int32)
+    k = len(so) - 1
+    if ids.shape != bq.shape or len(ids) != int(so[-1]) or dst.shape != (k,):
+      raise ValueError("fill_skipped_ragged: ccs_ids / ccs_base_quality_scores [src_off[-1]] and dst_window [k] expected")
+    if not (bases.flags.c_contiguous and quals.flags.c_contiguous and bases.dtype == np.uint8 and quals.dtype == np.uint8):
+      raise ValueError("fill_skipped_ragged: bases / quals must be C-contiguous uint8 arrays")
+    if bases.size < int(do[-1]) or quals.size < int(do[-1]):
+      raise ValueError("fill_skipped_ragged: bases / quals smaller than dst_off[-1]")
+    cal = calibration
+    en = int(bool(cal is not None and cal.enabled))
+    self._check(self._lib.dcb_fill_skipped_ragged(self._handle, _ptr(ids), _ptr(bq), _ptr(so), _ptr(dst), k, _ptr(do),
+                                                  len(do) - 1, en, float(cal.threshold) if en else 0.0,
+                                                  float(cal.w) if en else 1.0, float(cal.b) if en else 0.0, 0,
+                                                  _ptr(bases), _ptr(quals)))
+
   # -- feature construction on the device (include/dcb200.h "feature construction on the device") -----------------
   def features_layout(self, records: Dict[str, np.ndarray], ins_trim: int = 5) -> Dict[str, Any]:
     """dcb_features_layout (phase A) on a batch of raw records (`concat_records` of
     `preprocess.BamFeatureStream.next_zmw_records()` bundles): spaces the reads of every ZMW on the device and returns
     what dcb_prep_get_windows returns apart from the rows, dense over the batch -- dict(zmw_windows [n_zmw], window_pos
     [n], overflow [n], num_passes [n], ccs_bq int16 [n, L], ccs_ids uint8 [n, L], ms).  The spaced reads stay on the
-    device for features_pack."""
+    device for features_pack.  When the records carry `wl` / `wl_off` (CCS smart windows), dcb_features_layout_smart
+    cuts the windows at those lengths and the result also has window_width [n]."""
     L = self.max_length
     spec = dict(zmw_read_off=np.int32, zmw_ccs_off=np.int32, zmw_ccs_bq_any=np.int32, read_meta=np.int32, read_sn=np.float32,
                 cigar=np.uint32, bases=np.uint8, pw=np.uint8, ip=np.uint8, ccs_bases=np.uint8, ccs_bq=np.uint8)
@@ -589,17 +641,28 @@ class B200Model:
     # a capacity that always suffices: the spaced width is at most the longest read plus every insertion column
     meta = held["read_meta"][1].reshape(-1, READ_META)
     ro = held["zmw_read_off"][1]
+    smart = "wl" in records
     cap = 0
     for z in range(rec.n_zmw):
       m = meta[ro[z]:ro[z + 1]]
       longest = max(int(np.diff(held["zmw_ccs_off"][1])[z]), int((m[:, 4] + m[:, 7] - m[:, 6]).max(initial=0)))
       cap += (longest + int(m[:, 8].sum()) + 32 + L - 1) // L
+    if smart:                                          # at most one window per length
+      wl_off, wl = (np.ascontiguousarray(records[k], np.int32) for k in ("wl_off", "wl"))
+      cap = len(wl)
     out = dict(zmw_windows=np.zeros(rec.n_zmw, np.int32), window_pos=np.zeros(cap, np.int32), overflow=np.zeros(cap, np.uint8),
                ccs_bq=np.zeros((cap, L), np.int16), num_passes=np.zeros(cap, np.int32), ccs_ids=np.zeros((cap, L), np.uint8))
     n, ms = ctypes.c_int32(0), ctypes.c_float(0)
-    self._check(self._lib.dcb_features_layout(self._handle, ctypes.byref(rec), int(ins_trim), cap, _ptr(out["zmw_windows"]),
-                                              _ptr(out["window_pos"]), _ptr(out["overflow"]), _ptr(out["ccs_bq"]),
-                                              _ptr(out["num_passes"]), _ptr(out["ccs_ids"]), ctypes.byref(n), ctypes.byref(ms)))
+    if smart:
+      out["window_width"] = np.zeros(cap, np.int32)
+      self._check(self._lib.dcb_features_layout_smart(
+          self._handle, ctypes.byref(rec), _ptr(wl_off), _ptr(wl), int(ins_trim), cap, _ptr(out["zmw_windows"]),
+          _ptr(out["window_pos"]), _ptr(out["overflow"]), _ptr(out["window_width"]), _ptr(out["ccs_bq"]),
+          _ptr(out["num_passes"]), _ptr(out["ccs_ids"]), ctypes.byref(n), ctypes.byref(ms)))
+    else:
+      self._check(self._lib.dcb_features_layout(self._handle, ctypes.byref(rec), int(ins_trim), cap, _ptr(out["zmw_windows"]),
+                                                _ptr(out["window_pos"]), _ptr(out["overflow"]), _ptr(out["ccs_bq"]),
+                                                _ptr(out["num_passes"]), _ptr(out["ccs_ids"]), ctypes.byref(n), ctypes.byref(ms)))
     res: Dict[str, Any] = {k: (v if k == "zmw_windows" else v[:n.value]) for k, v in out.items()}
     res["ms"] = float(ms.value)
     return res
@@ -614,6 +677,18 @@ class B200Model:
     self._check(self._lib.dcb_features_pack(self._handle, _ptr(idx), len(idx), DCB_OUT_ON_DEVICE if out is not None else 0,
                                             _ptr(out) if out is not None else _ptr(packed), ctypes.byref(ms)))
     return dict(packed=packed, ms=float(ms.value))
+
+  def features_ccs(self, windows: np.ndarray, widths: np.ndarray) -> Dict[str, Any]:
+    """dcb_features_ccs: the CCS ids and qualities of the listed windows of the last features_layout at full width
+    (`widths`: their window_width).  Returns dict(ccs_ids uint8, ccs_bq int16, off int64 [n + 1], ms); window i is
+    [off[i], off[i + 1])."""
+    idx = np.ascontiguousarray(windows, dtype=np.int32).reshape(-1)
+    off = np.zeros(len(idx) + 1, np.int64)
+    np.cumsum(np.asarray(widths, np.int64).reshape(-1), out=off[1:])
+    ids, bq = np.zeros(int(off[-1]), np.uint8), np.zeros(int(off[-1]), np.int16)
+    ms = ctypes.c_float(0)
+    self._check(self._lib.dcb_features_ccs(self._handle, _ptr(idx), len(idx), _ptr(off), _ptr(ids), _ptr(bq), ctypes.byref(ms)))
+    return dict(ccs_ids=ids, ccs_bq=bq, off=off, ms=float(ms.value))
 
   def stitch_raw(self, bases_ptr: int, quals_ptr: int, n_windows: int, zmw_start: np.ndarray, flags: int,
                  seq_ptr: int, qual_ptr: int, len_ptr: int, length: Optional[int] = None) -> None:
@@ -919,7 +994,7 @@ def pack_rows(params: params_lib.Params, rows: np.ndarray, out: Optional[np.ndar
 
 def concat_records(zmws: List[Dict[str, Any]]) -> Dict[str, np.ndarray]:
   """The raw-record bundles of `preprocess.BamFeatureStream.next_zmw_records()` as one dcb_records batch: arrays
-  concatenated, per-read offsets shifted, per-ZMW offsets added."""
+  concatenated, per-read offsets shifted, per-ZMW offsets added (and, with smart windows, the `wl` tags with wl_off)."""
   cig0 = np.cumsum([0] + [len(z["cigar"]) for z in zmws])
   q0 = np.cumsum([0] + [len(z["bases"]) for z in zmws])
   meta = []
@@ -930,7 +1005,9 @@ def concat_records(zmws: List[Dict[str, Any]]) -> Dict[str, np.ndarray]:
     meta.append(m)
   cat = lambda key, dt, tail=(): (np.concatenate([np.asarray(z[key], dt).reshape((-1,) + tail) for z in zmws])
                                   if zmws else np.zeros((0,) + tail, dt))
-  return dict(zmw_read_off=np.cumsum([0] + [len(m) for m in meta]).astype(np.int32),
+  smart = dict(wl_off=np.cumsum([0] + [len(z["wl"]) for z in zmws]).astype(np.int32), wl=cat("wl", np.int32)) \
+      if zmws and "wl" in zmws[0] else {}
+  return dict(**smart, zmw_read_off=np.cumsum([0] + [len(m) for m in meta]).astype(np.int32),
               zmw_ccs_off=np.cumsum([0] + [len(z["ccs_bases"]) for z in zmws]).astype(np.int32),
               zmw_ccs_bq_any=np.array([int(z["ccs_bq_any"]) for z in zmws], np.int32),
               read_meta=np.concatenate(meta) if meta else np.zeros((0, READ_META), np.int32),

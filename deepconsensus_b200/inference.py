@@ -161,29 +161,31 @@ def run_model_and_stitch(feature_dicts: List[Dict[str, Any]], model: engine_lib.
     quals.append(out["quals"])
     names.extend(_as_str(x) for x in data["name"])
     positions.extend(int(x) for x in data["window_pos"])
-  if skipped_outputs:
-    sb = np.empty((len(skipped_outputs), L), np.uint8)
-    sq = np.empty((len(skipped_outputs), L), np.uint8)
-    for i, o in enumerate(skipped_outputs):
-      seq, qual = o.sequence.encode("latin-1"), o.quality_string.encode("latin-1")
-      if len(seq) != L or len(qual) != L:
-        raise ValueError("skipped window %s@%s is not %d characters long" % (o.molecule_name, o.window_pos, L))
-      sb[i] = np.frombuffer(seq, np.uint8)
-      sq[i] = np.frombuffer(qual, np.uint8)
-      names.append(_as_str(o.molecule_name))
-      positions.append(int(o.window_pos))
-    bases.append(sb)
-    quals.append(sq)
+  # skipped windows: L characters, or any width for an overflow window (CCS smart windows keep it whole)
+  skipped = [(np.frombuffer(o.sequence.encode("latin-1"), np.uint8), np.frombuffer(o.quality_string.encode("latin-1"), np.uint8))
+             for o in (skipped_outputs or [])]
+  for o, (sb, sq) in zip(skipped_outputs or [], skipped):
+    if len(sb) != len(sq):
+      raise ValueError("skipped window %s@%s: sequence and quality string differ in length" % (o.molecule_name, o.window_pos))
+    names.append(_as_str(o.molecule_name))
+    positions.append(int(o.window_pos))
   if not names:
     return []
-  all_b, all_q = np.concatenate(bases), np.concatenate(quals)
   order = sorted(range(len(names)), key=lambda i: (names[i], positions[i]))     # quick_inference.py:721-728
-  if order != list(range(len(names))):
-    all_b, all_q = all_b[order], all_q[order]
-    names = [names[i] for i in order]
-    positions = [positions[i] for i in order]
-  return stitch_gpu.stitch_batch_to_fastq(model, all_b, all_q, names, positions, L, options.min_quality,
-                                          options.min_length, outcome_counter)
+  names = [names[i] for i in order]
+  positions = [positions[i] for i in order]
+  if all(len(sb) == L for sb, _ in skipped):
+    all_b = np.concatenate(bases + [np.stack([sb for sb, _ in skipped])] if skipped else bases)
+    all_q = np.concatenate(quals + [np.stack([sq for _, sq in skipped])] if skipped else quals)
+    return stitch_gpu.stitch_batch_to_fastq(model, all_b[order], all_q[order], names, positions, L, options.min_quality,
+                                            options.min_length, outcome_counter)
+  rows_b = [r for b in bases for r in b] + [sb for sb, _ in skipped]
+  rows_q = [r for q in quals for r in q] + [sq for _, sq in skipped]
+  win_off = np.zeros(len(order) + 1, np.int64)
+  np.cumsum([len(rows_b[i]) for i in order], out=win_off[1:])
+  return stitch_gpu.stitch_batch_to_fastq(model, np.concatenate([rows_b[i] for i in order]),
+                                          np.concatenate([rows_q[i] for i in order]), names, positions, L,
+                                          options.min_quality, options.min_length, outcome_counter, win_off=win_off)
 
 
 def skip_decisions(model: engine_lib.B200Model, ccs_bq: np.ndarray, skip_windows_above: float) -> np.ndarray:
@@ -208,39 +210,46 @@ def inference_on_zmw_windows(feature_dicts_for_zmws: Iterable[Iterable[Dict[str,
     stitch          sort by (name, window_pos), stitch_to_fastq per read          dcb_stitch_fastq
 
   Returns one FASTQ record (or None) per read in sorted-name order -- identical to the reference flow built from
-  `split_skipped_windows`, `run_model_on_examples`, `sorted(...)` and `stitch_utils.stitch_to_fastq`.
+  `split_skipped_windows`, `run_model_on_examples`, `sorted(...)` and `stitch_utils.stitch_to_fastq`.  Overflow windows
+  may have any width, as `to_features_dict` makes them with CCS smart windows (pre_lib.py:683-697): they adopt their
+  CCS at full width.
   """
-  from deepconsensus_b200 import stitch_gpu
   L = int(model_params.max_length)
   windows = [w for one_zmw in feature_dicts_for_zmws for w in one_zmw]
-  n = len(windows)
-  if n == 0:
+  if not windows:
     return []
-  names = [_as_str(w["name"]) for w in windows]
-  positions = [int(w["window_pos"]) for w in windows]
-  bq = np.stack([np.asarray(w["ccs_base_quality_scores"]) for w in windows]).astype(np.int16)
+  # windows grouped by read name, in order of appearance: the stable sort by (name, window_pos) of
+  # quick_inference.py:721-728 is then the sort by name of the reads and by position inside each
+  by_name: Dict[str, List[int]] = {}
+  for i, w in enumerate(windows):
+    by_name.setdefault(_as_str(w["name"]), []).append(i)
+  windows = [windows[i] for ids in by_name.values() for i in ids]
+  rows_of = lambda i: np.asarray(windows[i]["subreads"])
+  ccs_row = params_lib.get_indices(options.max_passes, options.use_ccs_bq)[4][0]
+  bq_full = [np.asarray(w["ccs_base_quality_scores"]) for w in windows]
+  bq = np.stack([q[:L] for q in bq_full]).astype(np.int16)
   skip = np.array([bool(w.get("overflow", False)) for w in windows])
-  if options.skip_windows_above:
-    skip |= skip_decisions(model, bq, options.skip_windows_above)
-  order = sorted(range(n), key=lambda i: (names[i], positions[i]))          # quick_inference.py:721-728
-  dest = np.empty(n, np.int32)
-  dest[order] = np.arange(n, dtype=np.int32)
-  all_b, all_q = np.empty((n, L), np.uint8), np.empty((n, L), np.uint8)
-  scored = np.nonzero(~skip)[0]
-  cursor = 0
-  batches = batch_examples([windows[i] for i in scored], model_params, options)
-  for _, out in engine_lib.pipelined(batches, lambda d: model.submit(d["rows"]), model.wait, model.drain):
-    k = out["bases"].shape[0]
-    rows = dest[scored[cursor:cursor + k]]
-    all_b[rows], all_q[rows] = out["bases"], out["quals"]
-    cursor += k
-  skipped = np.nonzero(skip)[0]
-  if len(skipped):
-    ccs_row = params_lib.get_indices(options.max_passes, options.use_ccs_bq)[4][0]
-    ccs_ids = np.stack([np.asarray(windows[i]["subreads"])[ccs_row, :, 0] for i in skipped]).astype(np.uint8)
-    model.fill_skipped(ccs_ids, bq[skipped], dest[skipped], all_b, all_q, calibration=options.ccs_calibration_values)
-  return stitch_gpu.stitch_batch_to_fastq(model, all_b, all_q, [names[i] for i in order], [positions[i] for i in order],
-                                          L, options.min_quality, options.min_length, outcome_counter)
+  wide = {i: (rows_of(i)[ccs_row, :, 0].astype(np.uint8), bq_full[i].astype(np.int16))
+          for i in range(len(windows)) if rows_of(i).shape[1] != L}
+  for i in wide:
+    if not skip[i]:
+      raise ValueError("window %s@%s is %d columns wide but not an overflow window" %
+                       (_as_str(windows[i]["name"]), windows[i]["window_pos"], rows_of(i).shape[1]))
+
+  def score(scored):       # run_model_on_examples' batches, two submissions in flight
+    cursor = 0
+    batches = batch_examples([windows[i] for i in scored], model_params, options)
+    for _, out in engine_lib.pipelined(batches, lambda d: model.submit(d["rows"]), model.wait, model.drain):
+      k = out["bases"].shape[0]
+      yield scored[cursor:cursor + k], out["bases"], out["quals"]
+      cursor += k
+  score.batches = True
+
+  fastq, rec_off, passed, _ = _skip_score_stitch(
+      model, model_params, options, outcome_counter, list(by_name), np.array([len(v) for v in by_name.values()]),
+      np.array([int(w["window_pos"]) for w in windows], np.int64), bq, skip, score,
+      lambda skipped: np.stack([rows_of(i)[ccs_row, :L, 0] for i in skipped]).astype(np.uint8), wide=wide or None)
+  return [fastq[int(rec_off[z]):int(rec_off[z + 1])].decode("latin-1") if passed[z] else None for z in range(len(passed))]
 
 
 def inference_on_packed_zmws(zmws: List[Dict[str, Any]], model: engine_lib.B200Model, model_params: params_lib.Params,
@@ -263,11 +272,21 @@ def inference_on_packed_zmws(zmws: List[Dict[str, Any]], model: engine_lib.B200M
     out = model.forward_packed(packed[idx])
     return out["bases"], out["quals"]
 
+  wide = None
+  if "overflow_ccs_ids" in zmws[0]:                    # BamFeatureStream(use_ccs_smart_windows=True)
+    wide, base = {}, 0
+    for z in zmws:
+      o = 0
+      for i in np.nonzero(z["overflow"])[0]:
+        w = int(z["window_width"][i])
+        wide[base + int(i)] = (z["overflow_ccs_ids"][o:o + w], z["overflow_ccs_bq"][o:o + w])
+        o += w
+      base += len(z["window_pos"])
   return _skip_score_stitch(
       model, model_params, options, outcome_counter, [z["name"] for z in zmws], np.array([len(z["window_pos"]) for z in zmws]),
       np.concatenate([z["window_pos"] for z in zmws]).astype(np.int64), np.concatenate([z["ccs_bq"] for z in zmws]),
       np.concatenate([z["overflow"] for z in zmws]).astype(bool), score,
-      lambda skipped: packed[skipped][:, 3 * P * L:3 * P * L + L])    # the CCS plane of the packed rows
+      lambda skipped: packed[skipped][:, 3 * P * L:3 * P * L + L], wide=wide)    # the CCS plane of the packed rows
 
 
 def inference_on_record_zmws(zmws: List[Dict[str, Any]], model: engine_lib.B200Model, model_params: params_lib.Params,
@@ -296,19 +315,31 @@ def inference_on_record_zmws(zmws: List[Dict[str, Any]], model: engine_lib.B200M
     model.forward_packed_raw(rows_dev, len(idx), engine_lib.DCB_ROWS_ON_DEVICE, bases.ctypes.data, quals.ctypes.data)
     return bases, quals
 
+  wide = None
+  if "window_width" in lay:                            # CCS smart windows: overflow windows adopt their full-width CCS
+    over = np.nonzero(lay["overflow"])[0]
+    full = model.features_ccs(over, lay["window_width"][over])
+    wide = {int(i): (full["ccs_ids"][full["off"][j]:full["off"][j + 1]], full["ccs_bq"][full["off"][j]:full["off"][j + 1]])
+            for j, i in enumerate(over)}
   try:
     return _skip_score_stitch(model, model_params, options, outcome_counter, [zmws[k]["name"] for k in has], counts[has],
                               lay["window_pos"].astype(np.int64), lay["ccs_bq"], lay["overflow"].astype(bool), score,
-                              lambda skipped: lay["ccs_ids"][skipped], stats)
+                              lambda skipped: lay["ccs_ids"][skipped], stats, wide=wide)
   finally:
     model.free_device(rows_dev)
 
 
 def _skip_score_stitch(model, model_params, options, outcome_counter, names_z, counts, pos, bq, skip, score, ccs_ids_of,
-                       stats=None):
+                       stats=None, wide=None):
   """The part of `inference_on_n_zmws` behind the features, for windows given as arrays (ZMW k owns counts[k]
   consecutive windows): skip decision, `score(window indices) -> (bases, quals)` for the rest in batches of
-  options.batch_size, skipped-window fill from `ccs_ids_of(window indices)`, sort and stitch."""
+  options.batch_size, skipped-window fill from `ccs_ids_of(window indices)`, sort and stitch.  `score` may instead be
+  a generator function `score(all scored indices)` yielding (indices, bases, quals) batch by batch (marked by the
+  attribute `batches`), so that the caller keeps its own submission pipeline.
+
+  wide: CCS smart windows -- {window index: (ccs ids, ccs base qualities)} at full width for every overflow window.
+  Those windows are always skipped and keep their width through the fill and the stitch; every other window is L
+  wide (quick_inference.py:661-664, process_skipped_window)."""
   from deepconsensus_b200 import stitch_gpu
   L = int(model_params.max_length)
   n = len(pos)
@@ -322,18 +353,46 @@ def _skip_score_stitch(model, model_params, options, outcome_counter, names_z, c
   order = np.concatenate([starts[k] + np.argsort(pos[starts[k]:starts[k + 1]], kind="stable") for k in zorder])
   dest = np.empty(n, np.int64)
   dest[order] = np.arange(n)
-  all_b, all_q = np.empty((n, L), np.uint8), np.empty((n, L), np.uint8)
-  scored = np.nonzero(~skip)[0]
-  for b0 in range(0, len(scored), options.batch_size):          # batch_examples (quick_inference.py:304-338)
-    idx = scored[b0:b0 + options.batch_size]
-    all_b[dest[idx]], all_q[dest[idx]] = score(idx)
-  skipped = np.nonzero(skip)[0]
-  if len(skipped):
-    model.fill_skipped(ccs_ids_of(skipped), bq[skipped], dest[skipped].astype(np.int32), all_b, all_q,
-                       calibration=options.ccs_calibration_values)
+  scored, skipped = np.nonzero(~skip)[0], np.nonzero(skip)[0]
   names_sorted = [names_z[k] for k in zorder for _ in range(counts[k])]
+
+  def scored_batches():
+    if getattr(score, "batches", False):
+      yield from score(scored)
+      return
+    for b0 in range(0, len(scored), options.batch_size):        # batch_examples (quick_inference.py:304-338)
+      idx = scored[b0:b0 + options.batch_size]
+      yield (idx,) + tuple(score(idx))
+
+  if wide is None:
+    all_b, all_q = np.empty((n, L), np.uint8), np.empty((n, L), np.uint8)
+    for idx, b, q in scored_batches():
+      all_b[dest[idx]], all_q[dest[idx]] = b, q
+    if len(skipped):
+      model.fill_skipped(ccs_ids_of(skipped), bq[skipped], dest[skipped].astype(np.int32), all_b, all_q,
+                         calibration=options.ccs_calibration_values)
+    win_off = None
+  else:
+    width = np.full(n, L, np.int64)
+    for i, (ids, _) in wide.items():
+      width[i] = len(ids)
+    win_off = np.zeros(n + 1, np.int64)
+    np.cumsum(width[order], out=win_off[1:])
+    all_b, all_q = np.empty(int(win_off[-1]), np.uint8), np.empty(int(win_off[-1]), np.uint8)
+    cols = np.arange(L)
+    for idx, b, q in scored_batches():
+      at = win_off[dest[idx]][:, None] + cols
+      all_b[at], all_q[at] = b, q
+    if len(skipped):
+      narrow = ccs_ids_of(skipped)
+      parts = [wide[i] if i in wide else (narrow[j], bq[i]) for j, i in enumerate(skipped)]
+      src_off = np.zeros(len(skipped) + 1, np.int64)
+      np.cumsum([len(p[0]) for p in parts], out=src_off[1:])
+      model.fill_skipped_ragged(np.concatenate([p[0] for p in parts]), np.concatenate([p[1] for p in parts]), src_off,
+                                dest[skipped], win_off, all_b, all_q, calibration=options.ccs_calibration_values)
   fastq, rec_off, passed = stitch_gpu.stitch_batch_to_fastq_bytes(model, all_b, all_q, names_sorted, pos[order].tolist(), L,
-                                                                  options.min_quality, options.min_length, outcome_counter)
+                                                                  options.min_quality, options.min_length, outcome_counter,
+                                                                  win_off=win_off)
   return fastq, rec_off, passed, [names_z[k] for k in zorder]
 
 

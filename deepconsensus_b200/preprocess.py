@@ -44,6 +44,10 @@ def _lib():
     lib.dcb_prep_next_zmw.argtypes = [vp, ctypes.POINTER(DcbZmwInfo)]
     lib.dcb_prep_get_windows.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.dcb_prep_export_records.argtypes = [vp, i32]
+    lib.dcb_prep_use_ccs_smart_windows.argtypes = [vp, i32]
+    lib.dcb_prep_get_window_widths.argtypes = [vp, vp]
+    lib.dcb_prep_get_overflow_ccs.argtypes = [vp, vp, vp]
+    lib.dcb_prep_get_window_lengths.argtypes = [vp, vp, vp]
     lib.dcb_prep_get_records.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.dcb_prep_ccs_header.argtypes = [vp]
     lib.dcb_prep_ccs_header.restype = ctypes.c_char_p
@@ -62,11 +66,14 @@ class BamFeatureStream:
   iter_examples, pre_lib.py:1279-1384,625-697)."""
 
   def __init__(self, subreads_to_ccs: str, ccs_bam: str, max_passes: int, max_length: int, use_ccs_bq: bool = False,
-               ins_trim: int = 5, threads: int = 0, records: bool = False):
+               ins_trim: int = 5, threads: int = 0, records: bool = False, use_ccs_smart_windows: bool = False):
     """threads > 0: ZMWs are processed by that many native worker threads (plus one BAM-decoding thread) while the
     caller consumes them; the order of the ZMWs is the file's either way (`--cpus` of `deepconsensus run`).
     records: the stream only decodes and validates, and hands each ZMW out as raw records (`next_zmw_records`) for
-    feature construction on the device; `next_zmw` is not available then."""
+    feature construction on the device; `next_zmw` is not available then.
+    use_ccs_smart_windows: windows are cut at the widths of each CCS record's `wl` tag (pre_lib.py:625-650); windows
+    wider than max_length are overflow windows, whose full-width CCS `next_zmw` returns as `overflow_ccs_ids` /
+    `overflow_ccs_bq`; with `records`, `next_zmw_records` hands out each ZMW's `wl` tag."""
     self._lib = _lib()
     self._h = ctypes.c_void_p()
     self.max_passes, self.max_length, self.use_ccs_bq = int(max_passes), int(max_length), bool(use_ccs_bq)
@@ -76,6 +83,9 @@ class BamFeatureStream:
     if rc:
       raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
     if threads > 0 and self._lib.dcb_prep_set_threads(self._h, int(threads)):
+      raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
+    self.use_ccs_smart_windows = bool(use_ccs_smart_windows)
+    if self.use_ccs_smart_windows and self._lib.dcb_prep_use_ccs_smart_windows(self._h, 1):
       raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
     self.records = bool(records)
     if records and self._lib.dcb_prep_export_records(self._h, 1):
@@ -103,7 +113,9 @@ class BamFeatureStream:
 
   def next_zmw(self, want_rows: bool = True, want_packed: bool = False) -> Optional[Dict[str, Any]]:
     """The next ZMW's windows as arrays: dict(name, n_subreads, ec, np_num_passes, rq, rg, window_pos [n], overflow
-    [n], num_passes [n], ccs_bq int16 [n, L], rows float32 [n, R, L] and / or packed uint8 [n, stride]); None at EOF."""
+    [n], window_width [n] (spaced columns before the padding), num_passes [n], ccs_bq int16 [n, L], rows float32
+    [n, R, L] and / or packed uint8 [n, stride]); None at EOF.  With smart windows, also overflow_ccs_ids uint8 and
+    overflow_ccs_bq int16: the full-width CCS of the overflow windows, back to back in window order."""
     info = DcbZmwInfo()
     rc = self._lib.dcb_prep_next_zmw(self._h, ctypes.byref(info))
     if rc < 0:
@@ -117,7 +129,8 @@ class BamFeatureStream:
                                rq=float(info.rq) if info.has_rq else None,
                                rg=info.rg.decode("utf-8", "replace") if info.rg else None,
                                window_pos=np.zeros(n, np.int32), overflow=np.zeros(n, np.uint8),
-                               num_passes=np.zeros(n, np.int32), ccs_bq=np.zeros((n, L), np.int16))
+                               window_width=np.zeros(n, np.int32), num_passes=np.zeros(n, np.int32),
+                               ccs_bq=np.zeros((n, L), np.int16))
     if want_rows:
       out["rows"] = np.empty((n, R, L), np.float32)
     if want_packed:
@@ -126,6 +139,12 @@ class BamFeatureStream:
     rc = self._lib.dcb_prep_get_windows(self._h, vp(out["rows"]) if want_rows else None,
                                         vp(out["packed"]) if want_packed else None, vp(out["window_pos"]),
                                         vp(out["overflow"]), vp(out["ccs_bq"]), vp(out["num_passes"]))
+    if not rc:
+      rc = self._lib.dcb_prep_get_window_widths(self._h, vp(out["window_width"]))
+    if not rc and self.use_ccs_smart_windows:
+      m = int(out["window_width"][out["overflow"] != 0].sum())
+      out["overflow_ccs_ids"], out["overflow_ccs_bq"] = np.zeros(m, np.uint8), np.zeros(m, np.int16)
+      rc = self._lib.dcb_prep_get_overflow_ccs(self._h, vp(out["overflow_ccs_ids"]), vp(out["overflow_ccs_bq"]))
     if rc:
       raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
     return out
@@ -133,7 +152,7 @@ class BamFeatureStream:
   def next_zmw_records(self) -> Optional[Dict[str, Any]]:
     """The next ZMW as raw records (dcb_prep_get_records, include/dcb200.h): dict(name, n_subreads, ec, np_num_passes,
     rq, rg, read_meta int32 [n, 10], read_sn float32 [n, 4], cigar uint32, bases / pw / ip uint8 per query base,
-    ccs_bases / ccs_bq uint8, ccs_bq_any); None at EOF.  Needs `records=True`."""
+    ccs_bases / ccs_bq uint8, ccs_bq_any, and wl int32 with smart windows); None at EOF.  Needs `records=True`."""
     info = DcbZmwInfo()
     rc = self._lib.dcb_prep_next_zmw(self._h, ctypes.byref(info))
     if rc < 0:
@@ -157,6 +176,12 @@ class BamFeatureStream:
     if self._lib.dcb_prep_get_records(self._h, vp(sizes), *(vp(out[k]) for k in (
         "read_meta", "read_sn", "cigar", "bases", "pw", "ip", "ccs_bases", "ccs_bq"))):
       raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
+    if self.use_ccs_smart_windows:
+      n_wl = np.zeros(1, np.int32)
+      if self._lib.dcb_prep_get_window_lengths(self._h, vp(n_wl), None):
+        raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
+      out["wl"] = np.zeros(int(n_wl[0]), np.int32)
+      self._lib.dcb_prep_get_window_lengths(self._h, vp(n_wl), vp(out["wl"]))
     return out
 
   def __iter__(self):

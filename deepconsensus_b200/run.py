@@ -32,10 +32,12 @@ def run(subreads_to_ccs: str, ccs_bam: str, checkpoint: str, output: str, batch_
         min_quality: int = 20, min_length: int = 0, skip_windows_above: int = 45, ins_trim: int = 5,
         max_base_quality: int = 93, dc_calibration: Optional[str] = None, ccs_calibration: str = "skip",
         limit: int = 0, random_weights: Optional[int] = None, precision: str = "bf16", device: int = 0, cpus: int = 0,
-        features: str = "host") -> stitch_utils.OutcomeCounter:
+        features: str = "host", use_ccs_smart_windows: bool = False) -> stitch_utils.OutcomeCounter:
   """One inference run; returns the OutcomeCounter (quick_inference.run's return value).  features: "host" builds
   every window in csrc/bam_prep.cpp; "gpu" has the stream only decode and validate, and builds the windows on the
-  device, rows only for the windows the model scores (csrc/prep_kernels.cu).  Same output either way."""
+  device, rows only for the windows the model scores (csrc/prep_kernels.cu).  Same output either way.
+  use_ccs_smart_windows: cut each ZMW's windows at the widths of its CCS record's `wl` tag (pre_lib.py:625-650,
+  1329-1331); windows wider than max_length bypass the model and adopt the CCS call at full width."""
   if features not in ("host", "gpu"):
     raise ValueError("features must be 'host' or 'gpu'")
   params = params_lib.read_params_from_json(checkpoint)
@@ -54,7 +56,8 @@ def run(subreads_to_ccs: str, ccs_bam: str, checkpoint: str, output: str, batch_
   model, params = inference.initialize_model(checkpoint, params, options, weights=weights, device=device, precision=precision)
   counter = stitch_utils.OutcomeCounter()
   stream = preprocess.BamFeatureStream(subreads_to_ccs, ccs_bam, options.max_passes, options.max_length,
-                                       options.use_ccs_bq, ins_trim, threads=cpus, records=features == "gpu")
+                                       options.use_ccs_bq, ins_trim, threads=cpus, records=features == "gpu",
+                                       use_ccs_smart_windows=use_ccs_smart_windows)
   as_bam = output.endswith(".bam")
   writer: Any = preprocess.BamWriter(output, stream.ccs_header) if as_bam else open(output, "wb")
   stats = dict(zmws=0, windows=0, seconds_features=0.0, seconds_model_and_stitch=0.0)
@@ -124,6 +127,9 @@ def main(argv: Optional[List[str]] = None) -> None:
   ap.add_argument("--features", default="host", choices=["host", "gpu"],
                   help="where windows are built from the decoded BAM records: host C++, or CUDA kernels that lay rows out "
                        "only for the windows the model scores")
+  ap.add_argument("--use_ccs_smart_windows", action="store_true",
+                  help="cut windows at the widths of each CCS record's wl tag instead of every max_length columns "
+                       "(pre_lib.py:625-650); wider windows bypass the model")
   a = ap.parse_args(argv)
   c = run(**vars(a))
   print(json.dumps(c.__dict__))

@@ -35,14 +35,17 @@ def group_reads(molecule_names: Sequence[str]) -> np.ndarray:
 def stitch_batch_to_fastq_bytes(model, bases, quals, molecule_names: Sequence[str], window_pos: Sequence[int],
                                 max_length: int, min_quality: int, min_length: int,
                                 outcome_counter: stitch_utils.OutcomeCounter,
-                                n_windows: Optional[int] = None, on_device: bool = False
-                                ) -> Tuple[bytes, np.ndarray, np.ndarray]:
-  """(fastq bytes, rec_off, passed): read z's record is fastq[rec_off[z]:rec_off[z + 1]] when passed[z]."""
+                                n_windows: Optional[int] = None, on_device: bool = False,
+                                win_off: Optional[np.ndarray] = None) -> Tuple[bytes, np.ndarray, np.ndarray]:
+  """(fastq bytes, rec_off, passed): read z's record is fastq[rec_off[z]:rec_off[z + 1]] when passed[z].  win_off
+  (int64 [n_windows + 1]): the windows have different widths and lie back to back in the flat bases / quals, window w at
+  win_off[w] (CCS smart windows: overflow windows keep their full width)."""
   zs = group_reads(molecule_names)
   nz = len(zs) - 1
   names = [molecule_names[int(zs[z])] for z in range(nz)]
   fastq, rec_off, outcome, _ = model.stitch_fastq(bases, quals, zs, window_pos, names, min_quality, min_length,
-                                                  n_windows=n_windows, on_device=on_device, length=max_length)
+                                                  n_windows=n_windows, on_device=on_device, length=max_length,
+                                                  win_off=win_off)
   passed = np.zeros(nz, bool)
   for z in range(nz):
     code = int(outcome[z])
@@ -53,7 +56,7 @@ def stitch_batch_to_fastq_bytes(model, bases, quals, molecule_names: Sequence[st
       if rec is not None:
         qual = rec.split(b"\n")[3]
       else:                                   # too short: the record was not written; recompute from the windows
-        qual = _read_quality_bytes(model, bases, quals, zs, z, max_length, n_windows, on_device)
+        qual = _read_quality_bytes(model, bases, quals, zs, z, max_length, n_windows, on_device, win_off)
       ok = round(utils.avg_phred(np.frombuffer(qual, np.uint8).astype(np.int64) - 33), 5) >= min_quality
       if not ok:
         code = engine_lib.DCB_READ_LOW_QUALITY
@@ -71,22 +74,25 @@ def stitch_batch_to_fastq_bytes(model, bases, quals, molecule_names: Sequence[st
   return fastq, rec_off, passed
 
 
-def _read_quality_bytes(model, bases, quals, zs, z, max_length, n_windows, on_device) -> bytes:
-  seq, qual, lens = model.stitch(bases, quals, zs, n_windows=n_windows, on_device=on_device, length=max_length)
-  o = int(zs[z]) * max_length
+def _read_quality_bytes(model, bases, quals, zs, z, max_length, n_windows, on_device, win_off=None) -> bytes:
+  seq, qual, lens = model.stitch(bases, quals, zs, n_windows=n_windows, on_device=on_device, length=max_length,
+                                 win_off=win_off)
+  o = int(zs[z]) * max_length if win_off is None else int(win_off[int(zs[z])])
   return qual[o:o + int(lens[z])].tobytes()
 
 
 def stitch_batch_to_fastq(model, bases, quals, molecule_names: Sequence[str], window_pos: Sequence[int],
                           max_length: int, min_quality: int, min_length: int,
                           outcome_counter: stitch_utils.OutcomeCounter,
-                          n_windows: Optional[int] = None, on_device: bool = False) -> List[Optional[str]]:
+                          n_windows: Optional[int] = None, on_device: bool = False,
+                          win_off: Optional[np.ndarray] = None) -> List[Optional[str]]:
   """One FASTQ record (or None) per read, for windows grouped by read and sorted by window position.
 
   `bases` / `quals`: uint8 [n_windows, max_length] arrays as `B200Model.forward` returns them, or device addresses
-  of the same (`on_device=True`, e.g. the DCB_OUT_ON_DEVICE outputs of `forward_raw`).
+  of the same (`on_device=True`, e.g. the DCB_OUT_ON_DEVICE outputs of `forward_raw`); flat arrays with `win_off`.
   """
   fastq, rec_off, passed = stitch_batch_to_fastq_bytes(model, bases, quals, molecule_names, window_pos, max_length,
-                                                       min_quality, min_length, outcome_counter, n_windows, on_device)
+                                                       min_quality, min_length, outcome_counter, n_windows, on_device,
+                                                       win_off)
   return [fastq[int(rec_off[z]):int(rec_off[z + 1])].decode("latin-1") if passed[z] else None
           for z in range(len(passed))]

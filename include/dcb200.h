@@ -209,6 +209,30 @@ int dcb_fill_skipped(dcb_engine* e, const uint8_t* ccs_ids, const int16_t* ccs_b
                      int32_t L, int32_t calibration_enabled, double calibration_threshold, double calibration_w,
                      double calibration_b, uint32_t flags, uint8_t* bases, uint8_t* quals);
 
+/* ---- windows of different widths (CCS smart windows: overflow windows keep their full width) ------------------------
+ * The same three calls on windows laid out back to back at any width: window w is bytes win_off[w] .. win_off[w + 1]
+ * of bases / quals (win_off: host int64 [n_windows + 1], win_off[0] = 0, non-decreasing).  dcb_stitch,
+ * dcb_stitch_fastq and dcb_fill_skipped are these calls with win_off[w] = w * L; they run the same kernels.
+ *   dcb_stitch_ragged        read z is written at win_off[zmw_start[z]] of seq_out / qual_out (win_off[n_windows] bytes)
+ *   dcb_stitch_fastq_ragged  the missing-window check still counts windows: window i of a read is missing when its
+ *                            window_pos exceeds i * L, whatever the widths before it (stitch_utils.py:60-78); fastq_cap:
+ *                            names + 2 * win_off[n_windows] + 6 * n_zmw bytes always suffice
+ *   dcb_fill_skipped_ragged  skipped window j is src_off[j] .. src_off[j + 1] of ccs_ids / ccs_bq (src_off [k + 1]) and
+ *                            goes to window dst_window[j] of the output arrays, whose windows are dst_off [n_dst + 1];
+ *                            the two widths must agree */
+int dcb_stitch_ragged(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, const int64_t* win_off, int32_t n_windows,
+                      const int32_t* zmw_start, int32_t n_zmw, uint32_t flags, uint8_t* seq_out, uint8_t* qual_out,
+                      int32_t* len_out);
+int dcb_stitch_fastq_ragged(dcb_engine* e, const uint8_t* bases, const uint8_t* quals, const int64_t* win_off,
+                            int32_t n_windows, int32_t L, const int32_t* zmw_start, int32_t n_zmw, const int32_t* window_pos,
+                            const uint8_t* names, const int32_t* name_off, double min_quality, int32_t min_length,
+                            uint32_t flags, uint8_t* fastq_out, int64_t fastq_cap, int64_t* rec_off, int32_t* outcome,
+                            double* avg_q);
+int dcb_fill_skipped_ragged(dcb_engine* e, const uint8_t* ccs_ids, const int16_t* ccs_bq, const int64_t* src_off,
+                            const int32_t* dst_window, int32_t k, const int64_t* dst_off, int32_t n_dst,
+                            int32_t calibration_enabled, double calibration_threshold, double calibration_w,
+                            double calibration_b, uint32_t flags, uint8_t* bases, uint8_t* quals);
+
 /* ---- evaluation of labelled windows ---------------------------------------------------------------------------------
  * What model_inference.py (models/model_inference.py:79-120 -> model_utils.run_inference_and_write_results,
  * model_utils.py:379-421) has `model.evaluate` compute per window, and the identity of the training loop's metrics
@@ -325,6 +349,25 @@ int dcb_prep_next_zmw(dcb_prep* p, dcb_zmw_info* info);   /* 1 = a ZMW is loaded
  * window_pos / num_passes int32 [n]; overflow u8 [n]; ccs_bq int16 [n, L] (-1 at gaps and padding). */
 int dcb_prep_get_windows(dcb_prep* p, float* rows, uint8_t* packed, int32_t* window_pos, uint8_t* overflow,
                          int16_t* ccs_bq, int32_t* num_passes);
+/* CCS smart windows (`deepconsensus run --use_ccs_smart_windows`, pre_lib.py:625-650,1329-1331): enabled before the first
+ * dcb_prep_next_zmw, each ZMW's windows are cut at the widths of its CCS record's `wl` tag (B array, any integer
+ * subtype) instead of every max_length columns.  Window j takes wl[j] CCS bases plus the gap columns before the last of
+ * them; an entry of 0 gives no window.  A window at most max_length wide is padded like the last fixed-width window; a
+ * wider one is an overflow window (overflow = 1): it is never scored, its rows / packed rows / ccs_bq hold only its
+ * first max_length columns, and dcb_prep_get_overflow_ccs hands out its CCS at full width.  dcb_prep_next_zmw fails
+ * with DCB_ERR_INVALID naming the ZMW on a missing or non-integer wl tag, a negative entry, or sum(wl) != CCS length
+ * (where the reference raises), and on an overflow window in a CCS read without any non-zero base quality (the
+ * reference slices the unspaced quality array by spaced columns there, and its output goes out of step).  In raw-record
+ * mode the tag is checked the same way and handed out by dcb_prep_get_window_lengths (for dcb_features_layout_smart).
+ * dcb_prep_get_window_widths: spaced width of every window, int32 [n_windows] (with fixed-width windows, the columns
+ * before the padding).
+ * dcb_prep_get_overflow_ccs: the CCS ids (u8, 0..4 = ' ATCG') and base qualities (int16, -1 at gap columns) of every
+ * overflow window at full width, windows back to back in window order; either output may be NULL. */
+int dcb_prep_use_ccs_smart_windows(dcb_prep* p, int32_t enabled);
+int dcb_prep_get_window_widths(dcb_prep* p, int32_t* width);
+int dcb_prep_get_overflow_ccs(dcb_prep* p, uint8_t* ccs_ids, int16_t* ccs_bq);
+/* Raw-record mode with smart windows: the loaded ZMW's `wl` tag; *n always receives its length, wl (nullable) int32 [n]. */
+int dcb_prep_get_window_lengths(dcb_prep* p, int32_t* n, int32_t* wl);
 /* Raw-record mode, for feature construction on the device (dcb_features_layout below): enabled before the first
  * dcb_prep_next_zmw, the stream decodes and validates each ZMW and keeps its records as they are -- no trimming, spacing
  * or windows (dcb_zmw_info.n_windows and spaced_width are 0, dcb_prep_get_windows is DCB_ERR_STATE), so the worker
@@ -398,6 +441,23 @@ int dcb_features_layout(dcb_engine* e, const dcb_records* rec, int32_t ins_trim,
                         int32_t* window_pos, uint8_t* overflow, int16_t* ccs_bq, int32_t* num_passes, uint8_t* ccs_ids,
                         int32_t* n_windows_out, float* ms_out);
 int dcb_features_pack(dcb_engine* e, const int32_t* windows, int32_t n, uint32_t flags, uint8_t* packed_out, float* ms_out);
+/* CCS smart windows on the device (`run --use_ccs_smart_windows --features gpu`): dcb_features_layout with each ZMW's
+ * windows cut at its `wl` tag (wl: host int32, ZMW z's lengths at wl[wl_off[z] .. wl_off[z + 1]), wl_off [n_zmw + 1]
+ * starting at 0) as dcb_prep_use_ccs_smart_windows cuts them on the host: window j holds CCS bases [S, S + wl[j]), S the
+ * sum of the lengths before it, with the gap columns in front of the last of them; a length of 0 gives no window.
+ * window_width int32 [n] receives every window's spaced width, overflow = width > L.  ccs_bq / ccs_ids and the packed
+ * rows of dcb_features_pack hold a window's first min(width, L) columns and padding after them.  Negative lengths,
+ * lengths that do not sum to the CCS length, or an overflow window in a CCS read without base qualities return
+ * DCB_ERR_INVALID and leave no layout; the engine stays usable.
+ * dcb_features_ccs: the CCS ids (0..4) and base qualities (-1 at gap columns) of the layout's windows[0..n) at full
+ * width, window i at off[i] .. off[i + 1] of ccs_ids / ccs_bq (host arrays; off [n + 1] starts at 0 and must follow the
+ * windows' widths) -- what an overflow window adopts.  ms_out (nullable): device time of the kernel. */
+int dcb_features_layout_smart(dcb_engine* e, const dcb_records* rec, const int32_t* wl_off, const int32_t* wl, int32_t ins_trim,
+                              int32_t max_windows, int32_t* zmw_windows, int32_t* window_pos, uint8_t* overflow,
+                              int32_t* window_width, int16_t* ccs_bq, int32_t* num_passes, uint8_t* ccs_ids,
+                              int32_t* n_windows_out, float* ms_out);
+int dcb_features_ccs(dcb_engine* e, const int32_t* windows, int32_t n, const int64_t* off, uint8_t* ccs_ids, int16_t* ccs_bq,
+                     float* ms_out);
 
 /* Device time of the last dcb_forward (milliseconds, CUDA events on the engine's stream). */
 int dcb_last_forward_ms(dcb_engine* e, float* ms);

@@ -9,6 +9,9 @@ the card and its power limit, then
   decode + validate + export alone (raw-record mode) at the same thread counts,
   device time of dcb_features_layout / dcb_features_pack per 1 024 windows (CUDA events, median of 20),
   `run` end to end with features="host" and "gpu" alternated, and the share of windows the skip decision removes.
+  --smart-windows: only the device cost of CCS smart windows (tests/golden/human_1m/ccs_smart.bam, repeated x4):
+  dcb_features_layout_smart plus dcb_features_ccs of the overflow windows per 1 024 windows, against
+  dcb_features_layout's fixed cut of the same ZMWs.
 Needs a GPU: there is no fallback."""
 import argparse, gzip, json, os, shutil, struct, subprocess, sys, tempfile, time, zlib
 
@@ -75,11 +78,45 @@ def device_times(model, records, reps=20):
               upload_bytes_per_window=round(sum(v.nbytes for v in records.values()) / n))
 
 
+def smart_window_times(reps=20):
+  """Median device ms per 1 024 windows: fixed-width layout vs smart layout + full-width CCS of the overflow windows."""
+  P, L = 20, 100
+  bam = os.path.join(GOLDEN, "human_1m")
+  recs = {}
+  for smart in (False, True):
+    s = preprocess.BamFeatureStream(os.path.join(bam, "subreads_to_ccs.bam"), os.path.join(bam, "ccs_smart.bam"), P, L, False, 5,
+                                    records=True, use_ccs_smart_windows=smart)
+    zs = []
+    while (z := s.next_zmw_records()) is not None:
+      zs.append(z)
+    s.close()
+    recs[smart] = engine.concat_records(zs * 4)
+  p = params_lib.synthetic_params(P, L)
+  model = engine.B200Model(p, weights_lib.init_weights(p, seed=3), max_batch=64)
+  res = {}
+  for smart, key in ((False, "fixed"), (True, "smart")):
+    lay_ms, ccs_ms = [], []
+    for _ in range(reps + 2):                                      # two warm-up rounds
+      lay = model.features_layout(recs[smart], 5)
+      lay_ms.append(lay["ms"])
+      if smart:
+        over = np.nonzero(lay["overflow"])[0]
+        ccs_ms.append(model.features_ccs(over, lay["window_width"][over])["ms"])
+    n = len(lay["window_pos"])
+    per = lambda ms: round(float(np.median(ms[2:])) * 1024 / n, 4)
+    res[key] = dict(windows=n, layout_ms_per_1024_windows=per(lay_ms))
+    if smart:
+      res[key].update(overflow_windows=int(len(over)), overflow_ccs_ms_per_1024_windows=per(ccs_ms))
+  model.close()
+  return res
+
+
 def main():
   ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
   ap.add_argument("--copies", type=int, default=60)
   ap.add_argument("--rounds", type=int, default=3)
   ap.add_argument("--out", default=None)
+  ap.add_argument("--smart-windows", action="store_true")
   a = ap.parse_args()
   import torch
   if not torch.cuda.is_available():
@@ -88,6 +125,13 @@ def main():
                                  capture_output=True, text=True).stdout.strip().splitlines()[0],
              host_cpus=os.cpu_count(), copies=a.copies)
   print(json.dumps(res), flush=True)
+  if a.smart_windows:
+    res["smart_windows"] = smart_window_times()
+    print(json.dumps(res, indent=1))
+    if a.out:
+      os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+      json.dump(res, open(a.out, "w"), indent=1)
+    return
   tmp = tempfile.mkdtemp()
   try:
     bams = tuple(os.path.join(tmp, n) for n in ("subreads_to_ccs.bam", "ccs.bam"))
