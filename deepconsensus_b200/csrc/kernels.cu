@@ -699,6 +699,13 @@ __device__ __forceinline__ void ldmatrix_x2_trans(uint32_t& r0, uint32_t& r1, ui
                : "r"(addr));
 }
 
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+
 // element (token, col) of a bf16 operand image with `chunks` 8-wide chunks per row
 __device__ __forceinline__ size_t img_off(int tok, int col, int chunks) {
   const int tile = tok / kTileM, r = tok % kTileM;
@@ -924,8 +931,12 @@ band_attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __re
 // image is loaded once and stays resident; warpgroup w owns tile rows [64 w, 64 w + 64).  Per head h each consumer
 // warpgroup
 //   1. runs the k_h and then the v_h n-group of the q/k/v weights (split-bf16, 36 k-steps: W_hi then W_lo, A k-step
-//      (s * 2 + kk) % 18, as gemm_kernel's EPI_QKV) and stores each, rounded to bf16, into sK / sV in the attention's
-//      rotated layout, zero for rows >= L,
+//      (s * kSK + kk) % 18, as gemm_kernel's EPI_QKV) and stores each, rounded to bf16, into sK / sV in the attention's
+//      rotated layout, zero for rows >= L.  A comes from registers: at the start of each group every warp loads its
+//      16 rows of the 18 A k-steps from the resident xb tile with ldmatrix, in the m16n8k16 A layout the register-A
+//      wgmma takes, and the group's 36 wgmmas read B alone from shared memory.  Shared-memory A operands were read
+//      once per wgmma, twice per group (W_hi and W_lo); register A halves the group's A reads from shared memory, and
+//      the wgmma arithmetic does not depend on where A comes from,
 //   2. runs the q_h n-group and keeps it in registers as mma.sync A fragments (the m64n144 accumulator of warp w & 3
 //      covers its 16 rows in the m16n8k16 C layout: k-step ks is pack(d[8ks..+1]), pack(d[8ks+2..+3]),
 //      pack(d[8ks+4..+5]), pack(d[8ks+6..+7]), the mapping the FFN uses for its hidden activation),
@@ -934,21 +945,25 @@ band_attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __re
 // Before a warpgroup next writes sK / sV it meets its partner again, so no warp still reads the previous head's K and
 // V; the wgmmas of the next group are already under way by then.  The producer streams the groups in the order k_h0,
 // v_h0, q_h0, k_h1, v_h1, q_h1 (groups 2, 4, 0, 3, 5, 1 of the [q_h0|q_h1|k_h0|k_h1|v_h0|v_h1] weight image) through
-// a ring of 9216-byte stages (two k-steps of one group), and the next tile's xb loads once q_h1's MMAs have read it,
-// under head 1's attention.
+// a ring of four 18432-byte stages (four k-steps of one group), and the next tile's xb loads once q_h1's MMAs have read
+// it, under head 1's attention.
 //
 // Every q/k/v value is the accumulator gemm_kernel<144, 1, EPI_QKV, true> computes (same wgmma shape, same K order)
 // rounded the same way, and attend_block is band_attention_kernel's, so the attention image is the same bit for bit.
 // kQkv: the q/k/v accumulators are also stored to the q/k/v operand image as the EPI_QKV epilogue does (debug capture).
 struct QkvAttCfg {
   static constexpr int kAK = kDP / 16;                    // A k-steps: 18
-  static constexpr int kSK = 2;                           // k-steps per stage
-  static constexpr int kGroupStages = 2 * kAK / kSK;      // split-bf16 weights: 36 k-steps per group, 18 stages
+  // Ring shape: the same 72 KB as eight stages of two k-steps, but each stage's wgmma run, commit, wait and release
+  // covers four k-steps, so a warpgroup synchronises half as often per weight byte.  On an H100 SXM at 700 W that
+  // made the kernel (A still from shared memory) about 3 % faster at the bench workload; six k-steps in three stages
+  // and a second stage group in flight per warpgroup (wait_group 2) were not faster.
+  static constexpr int kSK = 4;                           // k-steps per stage
+  static constexpr int kGroupStages = 2 * kAK / kSK;      // split-bf16 weights: 36 k-steps per group, 9 stages
   static constexpr int kABytesPerK = 2 * kTileM * 16;     // 4096
   static constexpr int kBBytesPerK = 2 * kQKVGroup * 16;  // 4608
-  static constexpr int kStageBytes = kSK * kBBytesPerK;   // 9216
+  static constexpr int kStageBytes = kSK * kBBytesPerK;   // 18432
   static constexpr int kGroupBytes = 2 * kAK * kBBytesPerK;
-  static constexpr int kStages = 8;
+  static constexpr int kStages = 4;
   static constexpr int kATileBytes = kAK * kABytesPerK;   // the resident xb tile: 72 KB
   static constexpr int kKVBytes = kTileM * kAttStride * 2;  // K or V of one head: 36 KB
   static constexpr int kBarBytes = 256;
@@ -957,6 +972,7 @@ struct QkvAttCfg {
   static constexpr int kThreads = 384;
   static_assert(kSmemBytes <= 232448, "over the sm_90 opt-in shared memory per block");
   static_assert((2 * kStages + 2) * 8 <= kBarBytes, "the mbarriers (full, empty, a_full, a_empty) fit");
+  static_assert((2 * kAK) % kSK == 0, "every stage holds kSK k-steps of one group");
   static_assert(kQKVGroup == kDHP && kQKVN == 6 * kQKVGroup, "one n-group is one head's q, k or v");
 };
 
@@ -1027,7 +1043,10 @@ qkv_attention_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat
   const int wg = warp >> 2;
   const int g = lane >> 2, q = lane & 3;
   const int row0 = wg * 64 + (warp & 3) * 16 + g;   // this thread's accumulator rows: row0, row0 + 8
-  const uint32_t a_base = smem_u32(a_res) + wg * 64 * 16;
+  // ldmatrix.x4 row address of this lane for A k-step 0: matrices (rows 0-7, chunk 0), (rows 8-15, chunk 0),
+  // (rows 0-7, chunk 1), (rows 8-15, chunk 1) of the warp's 16 rows, i.e. the m16n8k16 A fragment a0..a3
+  const uint32_t a_frag = smem_u32(a_res) +
+                          ((lane >> 4) * kTileM + wg * 64 + (warp & 3) * 16 + ((lane >> 3) & 1) * 8 + (lane & 7)) * 16;
   const int band = win > 0 ? win : L;   // attn_win_size None/0 => full attention
   float acc[kQKVGroup / 2];
   uint32_t slot = 0, phase = 0, it = 0;
@@ -1038,9 +1057,13 @@ qkv_attention_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat
       uint32_t qa[kDHP / 16][4];
 #pragma unroll
       for (int part = 0; part < 3; ++part) {
-        // ---- acc = xb W[:, group]
+        // ---- acc = xb W[:, group], A from registers: this warp's 16 rows of the 18 A k-steps (each used by the
+        // W_hi and the W_lo half of the group)
+        uint32_t af[Cfg::kAK][4];
+#pragma unroll
+        for (int k = 0; k < Cfg::kAK; ++k) ldmatrix_x4(af[k], a_frag + k * Cfg::kABytesPerK);
         uint32_t prev = 0;
-#pragma unroll 1
+#pragma unroll
         for (int s = 0; s < Cfg::kGroupStages; ++s) {
           mbar_wait(&full[slot], phase);
           const uint32_t st = smem_u32(stage_base + slot * Cfg::kStageBytes);
@@ -1048,10 +1071,8 @@ qkv_attention_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat
           wgmma_fence();
 #pragma unroll
           for (int kk = 0; kk < Cfg::kSK; ++kk) {
-            const uint64_t adesc =
-                make_kc16_desc(a_base + ((s * Cfg::kSK + kk) % Cfg::kAK) * Cfg::kABytesPerK, kTileM * 16, 128);
             const uint64_t bdesc = make_kc16_desc(st + kk * Cfg::kBBytesPerK, kQKVGroup * 16, 128);
-            wgmma_m64n144k16(acc, adesc, bdesc, (s | kk) != 0);
+            wgmma_m64n144k16_rs(acc, af[(s * Cfg::kSK + kk) % Cfg::kAK], bdesc, (s | kk) != 0);
           }
           wgmma_commit();
           wgmma_fence_regs(acc);
@@ -1063,8 +1084,10 @@ qkv_attention_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat
         }
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
+#pragma unroll
+        for (int k = 0; k < Cfg::kAK; ++k) wgmma_fence_regs(af[k]);   // read by MMAs up to the one just completed
         mbar_arrive(&empty[prev]);
-        if (h + 1 == kHeads && part == 2) mbar_arrive(a_empty);   // the item's last MMAs on xb have completed
+        if (h + 1 == kHeads && part == 2) mbar_arrive(a_empty);   // the item's last reads of xb are done
 
         const int grp = part == 0 ? 2 + h : part == 1 ? 4 + h : h;   // qkv_att_group(3 h + part)
         if constexpr (kQkv) {   // the EPI_QKV epilogue's stores
