@@ -2,7 +2,8 @@
 # Builds the C-ABI library of include/dcb200.h for sm_90a (H100), in-tree:
 #   libdcb200.so      the product (ignores the environment)
 #   libdcb200_dev.so  the same sources with -DDCB_DEV_SWITCHES: the environment switch DCB_ALIGN=0 selects the
-#                     alternative token layout (tests/test_gpu_parity.py::test_unfused_fallback_paths_agree_with_fused)
+#                     alternative token layout (tests/test_gpu_parity.py::test_unfused_fallback_paths_agree_with_fused),
+#                     DCB_TILE_FLOW=0 serializes the forward's launches (tests/test_gpu_tile_flow.py)
 # Experiment builds: DCB_OUT=libdcb200_exp.so DCB_EXTRA_FLAGS=-D... (loaded via DCB200_LIB); DCB_SKIP_DEV=1 skips the
 # developer library.
 set -euo pipefail

@@ -114,6 +114,17 @@ struct RowEpi {
   int L;                 // tokens per window in the flattened layout (Lw): position = token % L
 };
 
+// ------------------------------------------------------------------ tile flow
+// How one launch of the window-aligned forward meets the launches around it tile by tile (kernels.cu, tile_wait and
+// tile_done): before it reads tile t it waits until flags[t] == wait, and once tile t's outputs are visible it stores
+// `done` there.  flags null: the launch is serialized behind the one before it and neither waits nor stores.
+struct TileFlow {
+  int* flags;            // [tiles of a chunk]
+  int wait, done;
+  int* status;           // the submission's status word: kStatusTileWait is set when a wait times out
+};
+constexpr int kStatusTileWait = 2;
+
 struct HeadParams {
   const float* x;        // fp32 residual image
   const float* ln_g;     // final LayerNorm gamma/beta [288]

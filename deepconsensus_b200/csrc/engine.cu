@@ -149,6 +149,9 @@ struct dcb_engine {
   DevBuf<__nv_bfloat16> d_xb;
   DevBuf<__nv_bfloat16> d_att;
   DevBuf<__nv_bfloat16> d_hid;   // FFN hidden activation, bf16 operand image [tile][ff/8][128][8] (debug capture only)
+  DevBuf<int> d_flow;            // [chunk_tiles] the window-aligned forward's tile flags (TileFlow)
+  uint32_t flow_stamp = 0;       // the last stamp a chunk gave them
+  bool tile_flow = false;        // window-aligned layout: the forward's launches overlap through d_flow
   DevBuf<double> d_p10;          // 10^(-q/10), q = 0..255 (host libm pow, as NumPy)
   DevBuf<float> d_dbg;           // [stages][chunk_tiles * x_image]
   DevBuf<__nv_bfloat16> d_dbg_op;   // bf16 operand images per stage (dbg_operand_slot)
@@ -712,6 +715,30 @@ void bf16_forward_chunk(dcb_engine* e, LaunchRecorder& rec, const float* rows_ch
   const int L = e->L, Lw = e->Lw, M = bw * Lw;   // M: tokens in the (possibly window-aligned) layout
   const int T = (M + kTileM - 1) / kTileM;
   const cudaStream_t st = rec.st;
+  // Window-aligned layout: every launch reads only what the launches before it wrote at the same tile, so each one
+  // after the embedding may start a tile once the launch before it has stamped that tile (TileFlow; kernels.cu's
+  // launch() explains why the overlapping launches cannot deadlock).  A chunk's stamps follow the previous chunk's, so
+  // no launch mistakes a flag an earlier chunk left for its own; when the stamps would wrap, the flags start over
+  // from zero.  The embedding is a plain launch: the chunk before has completed when it starts.
+  const bool flow = e->tile_flow;
+  const uint32_t nstamps = 3 + 3 * (uint32_t)c.num_hidden_layers;
+  if (flow && e->flow_stamp > UINT32_MAX - nstamps) {
+    cudaMemsetAsync(e->d_flow, 0, e->chunk_tiles * sizeof(int), st);
+    e->flow_stamp = 0;
+  }
+  // the flow of the chunk's next launch (both halves of a two-launch kernel share one): it waits for the stamp of the
+  // launch before and leaves the next one
+  auto next_flow = [&](bool advance = true) {
+    TileFlow f{};
+    if (flow) {
+      f.flags = e->d_flow;
+      f.status = d_status;
+      f.wait = (int)e->flow_stamp;
+      f.done = (int)(e->flow_stamp + 1);
+      if (advance) ++e->flow_stamp;
+    }
+    return f;
+  };
   int stage = 0;
   auto snap = [&]() {
     if (e->debug) {   // stream-ordered copies only
@@ -729,10 +756,11 @@ void bf16_forward_chunk(dcb_engine* e, LaunchRecorder& rec, const float* rows_ch
   };
   rec.run(kProfEmbed, 1, [&] {
     launch_embed(rows_chunk, packed_chunk, e->pl, e->R, L, Lw, M, T, e->echunks, W.cols, W.rowmeta, W.tables,
-                 e->table_elems, e->d_embqkv, d_status, st);
+                 e->table_elems, e->d_embqkv, d_status, next_flow(), st);
   });
   rec.run(kProfRowGemm, 1, [&] {   // condenser + positional encoding; xb = layer 0's attention input
-    launch_gemm_row(e->d_embqkv, W.wc, e->Epad / 16, 2 * (e->Epad / 16), T, row_epi(e, false, nullptr, 0, 0, true), st);
+    launch_gemm_row(e->d_embqkv, W.wc, e->Epad / 16, 2 * (e->Epad / 16), T, row_epi(e, false, nullptr, 0, 0, true),
+                    next_flow(), st);
   });
   snap();
   for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
@@ -743,26 +771,28 @@ void bf16_forward_chunk(dcb_engine* e, LaunchRecorder& rec, const float* rows_ch
       rec.run(kProfAttention, 2, [&] {
         __nv_bfloat16* qkv = e->debug ? e->d_embqkv.p : nullptr;
         for (int half = 0; half < 2; ++half)
-          launch_qkv_attention(half, e->d_xb, ld.wqkv, L, c.attn_win_size, T, qkv, e->d_att, st);
+          launch_qkv_attention(half, e->d_xb, ld.wqkv, L, c.attn_win_size, T, qkv, e->d_att, next_flow(half == 1), st);
       });
     } else {
       rec.run(kProfQkv, 1, [&] { launch_gemm_qkv(e->d_xb, ld.wqkv, T, e->d_embqkv, st); });
       rec.run(kProfAttention, 1, [&] { launch_attention(e->d_embqkv, e->d_att, L, Lw, c.attn_win_size, bw, st); });
     }
     rec.run(kProfRowGemm, 1, [&] {   // attention out-projection + residual; xb = the FFN sub-layer's input
-      launch_gemm_row(e->d_att, ld.wo, kDP / 16, 2 * (kDP / 16), T, row_epi(e, true, nullptr, n_, 1, false), st);
+      launch_gemm_row(e->d_att, ld.wo, kDP / 16, 2 * (kDP / 16), T, row_epi(e, true, nullptr, n_, 1, false), next_flow(),
+                      st);
     });
     snap();
     rec.run(kProfFfn, 2, [&] {   // relu(xb W1 + b1) W2 + b2 + residual, half of the tiles per launch; xb = next layer's
       const RowEpi epi = row_epi(e, true, ld.b2, n_ + 1, 0, false);
       __nv_bfloat16* hid = e->debug ? e->d_hid.p : nullptr;
-      for (int half = 0; half < 2; ++half) launch_ffn(half, e->d_xb, ld.w1, ld.b1, ld.w2, c.filter_size, T, hid, epi, st);
+      for (int half = 0; half < 2; ++half)
+        launch_ffn(half, e->d_xb, ld.w1, ld.b1, ld.w2, c.filter_size, T, hid, epi, next_flow(half == 1), st);
     });
     if (e->profile) e->prof_ffn_tokens += (long long)bw * L;   // valid tokens (layout padding is not algorithmic work)
     snap();
   }
   hp.x = e->d_x; hp.M = M; hp.L = L; hp.Lw = Lw;
-  rec.run(kProfHead, 1, [&] { launch_head(hp, T, st); });
+  rec.run(kProfHead, 1, [&] { launch_head(hp, T, next_flow(), st); });
   e->last_chunk_tokens = M;
 }
 
@@ -806,15 +836,18 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
   e->num_sms = prop.multiProcessorCount;
   e->L = cfg->max_length;
   e->Lw = e->L;
-  bool align = true;
+  bool align = true, tile_flow = true;
 #ifdef DCB_DEV_SWITCHES
-  // Developer build only (libdcb200_dev.so, csrc/build.sh): an environment switch that selects the alternative token
-  // layout.  The product library ignores the environment.
+  // Developer build only (libdcb200_dev.so, csrc/build.sh): environment switches that select the alternative token
+  // layout (DCB_ALIGN=0) and serialize every launch of the window-aligned forward (DCB_TILE_FLOW=0).  The product
+  // library ignores the environment.
   if (const char* env = getenv("DCB_ALIGN")) align = atoi(env) != 0;
+  if (const char* env = getenv("DCB_TILE_FLOW")) tile_flow = atoi(env) != 0;
 #endif
   // window-aligned tiling: one window per 128-token tile when it fits (the positional table is then read in residual-
   // image order); otherwise windows are packed back to back
   if (align && e->L <= kTileM) e->Lw = kTileM;
+  e->tile_flow = tile_flow && e->Lw == kTileM;
   e->R = 4 * cfg->max_passes + (cfg->use_ccs_bq ? 6 : 5);  // data_providers.py:61-78
   e->pl = make_packed_layout(cfg->max_passes, cfg->max_length, cfg->use_ccs_bq ? 1 : 0);
   {
@@ -880,6 +913,7 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
     if (!rc) rc = alloc(e, e->d_x, T * x_image_elems());
     if (!rc) rc = alloc(e, e->d_xb, T * act_image_elems(kDP));
     if (!rc) rc = alloc(e, e->d_att, T * act_image_elems(kDP));
+    if (!rc && e->tile_flow) rc = alloc(e, e->d_flow, T);
     return rc;
   }();
   if (rc) {
@@ -1115,6 +1149,9 @@ int dcb_wait(dcb_engine* e, int64_t ticket) {
     ++e->prof_n[r.kind];
   }
   sl.prof_used = 0;
+  if (status & kStatusTileWait)
+    return fail(e, DCB_ERR_CUDA, "a launch of the forward waited over a second for a tile of the launch before it; "
+                                 "the outputs are not valid");
   if (status & 1) return fail(e, DCB_ERR_INPUT_RANGE, "embedding id out of range in the input rows (clamped)");
   return DCB_OK;
 }

@@ -25,6 +25,50 @@
 
 namespace dcb {
 
+// =====================================================================================
+// tile flow between the forward's launches
+// =====================================================================================
+// In the window-aligned layout every launch of the forward reads only the tiles the launches before it wrote at the
+// same index, so a launch may start tile t as soon as the one before it has finished tile t (TileFlow).  Those launches
+// are programmatic dependents of the launch before them (launch below): each one lets the next launch start early
+// (pdl_launch_dependents) and, before its threads exit, waits until the launch before it has completed (pdl_wait), so
+// a launch never completes before its predecessor and whatever follows the forward in the stream still sees it whole.
+// Both instructions do nothing in a plain launch.
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// One thread: wait until tile `tile` carries the stamp of the launch before this one (a gpu-scope acquire, so the
+// tile's data is visible to this thread and to the threads it later releases through a barrier).  A wait is bounded:
+// after a second it sets kStatusTileWait in the submission's status and goes on, so the host reports an error
+// instead of the GPU hanging.  Readers with bulk copies (async proxy) follow it with fence.proxy.async.
+__device__ __forceinline__ void tile_wait(const TileFlow& f, int tile) {
+  if (!f.flags) return;
+  if (ld_acquire_gpu(f.flags + tile) == f.wait) return;
+  uint64_t t0, t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+  while (ld_acquire_gpu(f.flags + tile) != f.wait) {
+    __nanosleep(100);
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    if (t - t0 > 1000000000ull) { atomicOr(f.status, kStatusTileWait); return; }
+  }
+}
+
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+
+// One thread, after every thread that wrote tile `tile` has met it at a barrier: publish the tile (gpu-scope release,
+// cumulative over the writes the barrier ordered before it).
+__device__ __forceinline__ void tile_done(const TileFlow& f, int tile) {
+  if (f.flags) asm volatile("st.release.gpu.global.b32 [%0], %1;" ::"l"(f.flags + tile), "r"(f.done) : "memory");
+}
+
+// The two consumer warpgroups (threads 0-255) of the warp-specialised kernels meet on named barrier 1.
+__device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // =====================================================================================
 // embed
@@ -37,8 +81,9 @@ embed_rows_kernel(const float* __restrict__ rows, const uint8_t* __restrict__ pa
                   int Lw, int M, int echunks,
                   const EmbedCol* __restrict__ cols, const EmbedRow* __restrict__ rowmeta,
                   const __nv_bfloat16* __restrict__ tables, int table_elems,
-                  __nv_bfloat16* __restrict__ emb, int* __restrict__ status) {
+                  __nv_bfloat16* __restrict__ emb, int* __restrict__ status, TileFlow flow) {
   extern __shared__ __align__(1024) uint8_t smem[];
+  pdl_launch_dependents();
   __nv_bfloat16* s_tab = reinterpret_cast<__nv_bfloat16*>(smem);
   const int tab_bytes = (table_elems * 2 + 15) & ~15;
   EmbedCol* s_cols = reinterpret_cast<EmbedCol*>(smem + tab_bytes);
@@ -99,6 +144,8 @@ embed_rows_kernel(const float* __restrict__ rows, const uint8_t* __restrict__ pa
     uint4* dst = reinterpret_cast<uint4*>(emb + ((size_t)tile * echunks + kc) * kTileM * 8) + r;
     *dst = val;
   }
+  __syncthreads();
+  if (threadIdx.x == 0) tile_done(flow, tile);
 }
 
 // =====================================================================================
@@ -289,7 +336,7 @@ template <int BN, int NCH, int EPI, bool kAres>
 __global__ void __launch_bounds__(384, 1)
 gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __restrict__ b_img, int a_ksteps, int ksteps,
             int ntiles,
-            int ngroups, __nv_bfloat16* __restrict__ out_img, int out_chunks, RowEpi epi) {
+            int ngroups, __nv_bfloat16* __restrict__ out_img, int out_chunks, RowEpi epi, TileFlow flow) {
   using Cfg = GemmCfg<BN, NCH, kAres>;
   static_assert(EPI != EPI_ROW || (Cfg::kNI == kDP && !kAres), "row epilogue needs the full 288-wide row");
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -320,6 +367,7 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
     mbar_fence_init();
   }
   __syncthreads();
+  pdl_launch_dependents();
 
   // kAres: a work item is a tile pair (its n-groups run back to back on the resident A); otherwise a (tile, n-group) pair
   const int nitems = kAres ? (ntiles + 1) / 2 : ntiles * ngroups;
@@ -335,6 +383,11 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
       for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++it) {
         const int tile = kAres ? 2 * item : item / ngroups;
         const uint8_t* a_src = reinterpret_cast<const uint8_t*>(a_img) + tile * a_tile_bytes;
+        // (flags are set for the row GEMM only, whose items are tiles) the tile is in place before its A copies; the
+        // row epilogue's residual loads follow this acquire through the stage barriers (arrive.expect_tx here, then
+        // the consumers' wait on `full`)
+        tile_wait(flow, tile);
+        fence_proxy_async();
         if constexpr (kAres) {   // the pair's A images are contiguous: one copy of one or two tiles
           const uint32_t a_bytes = (uint32_t)((tile + 1 < ntiles ? 2 : 1) * a_tile_bytes);
           mbar_wait(a_empty, (it & 1) ^ 1);
@@ -468,7 +521,12 @@ gemm_kernel(const __nv_bfloat16* __restrict__ a_img, const __nv_bfloat16* __rest
         row_epilogue<BN, NCH>(accm[0], tile, row0, q, s_vec, epi);   // one m64 block per warpgroup
       }
     }
+    if (flow.flags) {   // the tile's stores are done
+      consumer_bar_sync();
+      if (threadIdx.x == 0) tile_done(flow, item);
+    }
   }
+  pdl_wait();
 }
 
 // =====================================================================================
@@ -520,7 +578,7 @@ template <bool kHid>
 __global__ void __launch_bounds__(384, 1)
 ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* __restrict__ w1_img,
                 const float* __restrict__ b1, const __nv_bfloat16* __restrict__ w2_img, int ff, int tile_begin,
-                int tile_end, __nv_bfloat16* __restrict__ hid, RowEpi epi) {
+                int tile_end, __nv_bfloat16* __restrict__ hid, RowEpi epi, TileFlow flow) {
   using Cfg = FfnCfg;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* a_res = smem;
@@ -545,6 +603,7 @@ ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* _
     mbar_fence_init();
   }
   __syncthreads();
+  pdl_launch_dependents();
 
   if (warp >= 8) {
     // ------------------------------------------------------------- producer
@@ -561,6 +620,10 @@ ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* _
         if (++slot == Cfg::kStages) { slot = 0; phase ^= 1; }
       };
       for (int tile = tile_begin + blockIdx.x; tile < tile_end; tile += gridDim.x, ++it) {
+        // the tile is in place before its xb copy; the row epilogue's residual loads follow this acquire through
+        // a_full (arrive.expect_tx here, the consumers' wait there)
+        tile_wait(flow, tile);
+        fence_proxy_async();
         mbar_wait(a_empty, (it & 1) ^ 1);
         mbar_arrive_expect_tx(a_full, Cfg::kATileBytes);
         bulk_g2s(a_res, reinterpret_cast<const uint8_t*>(xb_img) + (size_t)tile * Cfg::kATileBytes, Cfg::kATileBytes,
@@ -670,7 +733,12 @@ ffn_gemm_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* _
     }
 
     row_epilogue<kNC, 2, false>(acc, tile, row0, q, s_vec, epi);
+    if (flow.flags) {
+      consumer_bar_sync();
+      if (threadIdx.x == 0) tile_done(flow, tile);
+    }
   }
+  pdl_wait();
 }
 
 // =====================================================================================
@@ -982,13 +1050,11 @@ __device__ __forceinline__ int qkv_att_group(int i) {
   return part == 0 ? 2 + h : part == 1 ? 4 + h : h;
 }
 
-__device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-
 template <bool kQkv>
 __global__ void __launch_bounds__(384, 1)
 qkv_attention_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat16* __restrict__ b_img, int L,
                      int win, int tile_begin, int tile_end, __nv_bfloat16* __restrict__ qkv_img,
-                     __nv_bfloat16* __restrict__ att) {
+                     __nv_bfloat16* __restrict__ att, TileFlow flow) {
   using Cfg = QkvAttCfg;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* a_res = smem;
@@ -1012,6 +1078,7 @@ qkv_attention_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat
     mbar_fence_init();
   }
   __syncthreads();
+  pdl_launch_dependents();
 
   if (warp >= 8) {
     // ------------------------------------------------------------- producer
@@ -1019,6 +1086,8 @@ qkv_attention_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat
     if (warp == 8 && lane == 0) {
       uint32_t slot = 0, phase = 0, it = 0;
       for (int tile = tile_begin + blockIdx.x; tile < tile_end; tile += gridDim.x, ++it) {
+        tile_wait(flow, tile);   // the tile's xb is in place before its copy
+        fence_proxy_async();
         mbar_wait(a_empty, (it & 1) ^ 1);
         mbar_arrive_expect_tx(a_full, Cfg::kATileBytes);
         bulk_g2s(a_res, reinterpret_cast<const uint8_t*>(xb_img) + (size_t)tile * Cfg::kATileBytes, Cfg::kATileBytes,
@@ -1132,25 +1201,24 @@ qkv_attention_kernel(const __nv_bfloat16* __restrict__ xb_img, const __nv_bfloat
       const int i0 = warp * 16;
       if (i0 < L) attend_block(qa, sK, sV, i0, L, band, att, tile * kTileM, h);
     }
+    if (flow.flags) {
+      consumer_bar_sync();
+      if (threadIdx.x == 0) tile_done(flow, tile);
+    }
   }
+  pdl_wait();
 }
 
 // =====================================================================================
 // head: final LayerNorm -> fc1 -> softmax -> argmax / Phred / ASCII
 // =====================================================================================
-__global__ void __launch_bounds__(128)
-head_kernel(HeadParams p) {
+// Token tile * kTileM + r of head_kernel; sGW, sA, sBj: its shared-memory copies of p.gw8 and p.ab.
+__device__ __forceinline__ void head_row(const HeadParams& p, const float* sGW, const float* sA, const float* sBj,
+                                         int tile, int r) {
   // logits_j = sum_c ((x_c - mean) * rstd * g_c + b_c) * W_cj + bfc_j
   //          = rstd * (sum_c y_c * (g_c W_cj) - mean_y * A_j) + B_j + bfc_j,   y = x - shift, A_j = sum_c g_c W_cj,
   //            B_j = sum_c b_c W_cj
   // so ONE pass over the row accumulates sum y, sum y^2 and the five sums y * gW_j (the residual image is read once).
-  __shared__ __align__(16) float sGW[kD * 8];
-  __shared__ float sA[kVocab], sBj[kVocab];
-  for (int i = threadIdx.x; i < kD * 2; i += blockDim.x)
-    reinterpret_cast<float4*>(sGW)[i] = __ldg(reinterpret_cast<const float4*>(p.gw8) + i);
-  if (threadIdx.x < kVocab) { sA[threadIdx.x] = p.ab[threadIdx.x]; sBj[threadIdx.x] = p.ab[8 + threadIdx.x]; }
-  __syncthreads();
-  const int tile = blockIdx.x, r = threadIdx.x;
   const int tok = tile * kTileM + r;
   if (tok >= p.M) return;
   const int wdw = tok / p.Lw, pos = tok - wdw * p.Lw;
@@ -1193,6 +1261,19 @@ head_kernel(HeadParams p) {
   head_finish(p, lg, oidx);
 }
 
+__global__ void __launch_bounds__(128)
+head_kernel(HeadParams p, TileFlow flow) {
+  __shared__ __align__(16) float sGW[kD * 8];
+  __shared__ float sA[kVocab], sBj[kVocab];
+  for (int i = threadIdx.x; i < kD * 2; i += blockDim.x)
+    reinterpret_cast<float4*>(sGW)[i] = __ldg(reinterpret_cast<const float4*>(p.gw8) + i);
+  if (threadIdx.x < kVocab) { sA[threadIdx.x] = p.ab[threadIdx.x]; sBj[threadIdx.x] = p.ab[8 + threadIdx.x]; }
+  if (threadIdx.x == 0) tile_wait(flow, blockIdx.x);   // every thread's residual loads follow it through the barrier
+  __syncthreads();
+  head_row(p, sGW, sA, sBj, blockIdx.x, threadIdx.x);
+  pdl_wait();
+}
+
 // =====================================================================================
 // launchers
 // =====================================================================================
@@ -1232,6 +1313,27 @@ cudaError_t kernels_init() {
   return e;
 }
 
+// kernel<<<grid, threads, smem, st>>>(args...), as a programmatic dependent of the launch before it in the stream when
+// `flow` carries flags (the tile flow above).  Such a launch may start before the one it depends on has finished; it
+// cannot deadlock on it: a dependent launch starts only once every CTA of the launch before it has issued
+// launch_dependents, i.e. is resident or finished, and so every tile a CTA waits for belongs to a CTA that is running
+// or done (the chain's launches wait only on the launch just before them).
+template <typename... P, typename... A>
+static void launch(const TileFlow& flow, void (*kernel)(P...), int grid, int threads, size_t smem, cudaStream_t st,
+                   A... args) {
+  cudaLaunchAttribute attr{};
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(threads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cfg.attrs = flow.flags ? &attr : nullptr;
+  cfg.numAttrs = flow.flags ? 1 : 0;
+  cudaLaunchKernelEx(&cfg, kernel, args...);   // an error is left for the submission's cudaGetLastError
+}
+
 size_t embed_smem_bytes(int R, int echunks, int table_elems) {
   return (size_t)((table_elems * 2 + 15) & ~15) + ((echunks * 8 * sizeof(EmbedCol) + 15) & ~(size_t)15) +
          (size_t)R * kTileM * 2;
@@ -1239,18 +1341,18 @@ size_t embed_smem_bytes(int R, int echunks, int table_elems) {
 
 void launch_embed(const float* rows, const uint8_t* packed, const PackedLayout& pl, int R, int L, int Lw, int M, int ntiles, int echunks,
                   const EmbedCol* cols, const EmbedRow* rowmeta, const __nv_bfloat16* tables,
-                  int table_elems, __nv_bfloat16* emb, int* status, cudaStream_t st) {
+                  int table_elems, __nv_bfloat16* emb, int* status, const TileFlow& flow, cudaStream_t st) {
   embed_rows_kernel<<<ntiles, 256, embed_smem_bytes(R, echunks, table_elems), st>>>(
-      rows, packed, pl, R, L, Lw, M, echunks, cols, rowmeta, tables, table_elems, emb, status);
+      rows, packed, pl, R, L, Lw, M, echunks, cols, rowmeta, tables, table_elems, emb, status, flow);
 }
 
 void launch_gemm_row(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int a_ksteps, int b_ksteps, int ntiles,
-                     const RowEpi& epi, cudaStream_t st) {
+                     const RowEpi& epi, const TileFlow& flow, cudaStream_t st) {
   using Cfg = GemmCfg<kNC, 2, false>;
   const int grid = ntiles < num_sms() ? ntiles : num_sms();
   const int smem = Cfg::smem_bytes(Cfg::stages(b_ksteps / Cfg::kSK));
-  gemm_kernel<kNC, 2, EPI_ROW, false><<<grid, Cfg::kThreads, smem, st>>>(a_img, b_img, a_ksteps, b_ksteps, ntiles, 1,
-                                                                                    nullptr, 0, epi);
+  launch(flow, gemm_kernel<kNC, 2, EPI_ROW, false>, grid, Cfg::kThreads, smem, st, a_img, b_img, a_ksteps, b_ksteps,
+         ntiles, 1, (__nv_bfloat16*)nullptr, 0, epi, flow);
 }
 
 void launch_gemm_qkv(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int ntiles,
@@ -1260,24 +1362,20 @@ void launch_gemm_qkv(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int
   const int grid = npairs < num_sms() ? npairs : num_sms();
   RowEpi none{};
   gemm_kernel<kNC, 1, EPI_QKV, true><<<grid, Cfg::kThreads, Cfg::kSmemBytes, st>>>(
-      a_img, b_img, kDP / 16, 2 * (kDP / 16), ntiles, kQKVN / kQKVGroup, qkv_img, kQKVN / 8, none);
+      a_img, b_img, kDP / 16, 2 * (kDP / 16), ntiles, kQKVN / kQKVGroup, qkv_img, kQKVN / 8, none, TileFlow{});
 }
 
 void launch_ffn(int half, const __nv_bfloat16* xb_img, const __nv_bfloat16* w1_img, const float* b1,
                 const __nv_bfloat16* w2_img, int ff, int ntiles, __nv_bfloat16* hid_img, const RowEpi& epi,
-                cudaStream_t st) {
+                const TileFlow& flow, cudaStream_t st) {
   const int split = (ntiles + 1) / 2;
   const int t0 = half ? split : 0, t1 = half ? ntiles : split;
   // a half without tiles still launches (one CTA that finds no work), so the forward's launch count does not depend
   // on the chunk size
   const int n = t1 - t0;
   const int grid = n < 1 ? 1 : n < num_sms() ? n : num_sms();
-  if (hid_img)
-    ffn_gemm_kernel<true><<<grid, FfnCfg::kThreads, FfnCfg::kSmemBytes, st>>>(xb_img, w1_img, b1, w2_img, ff, t0, t1,
-                                                                              hid_img, epi);
-  else
-    ffn_gemm_kernel<false><<<grid, FfnCfg::kThreads, FfnCfg::kSmemBytes, st>>>(xb_img, w1_img, b1, w2_img, ff, t0, t1,
-                                                                               nullptr, epi);
+  launch(flow, hid_img ? ffn_gemm_kernel<true> : ffn_gemm_kernel<false>, grid, FfnCfg::kThreads, FfnCfg::kSmemBytes,
+         st, xb_img, w1_img, b1, w2_img, ff, t0, t1, hid_img, epi, flow);
 }
 
 // packed rows -> the float32 [B, R, L] rows they stand for (the strict-fp32 path reads float32 rows)
@@ -1305,18 +1403,15 @@ void launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* att, int L, int L
 }
 
 void launch_qkv_attention(int half, const __nv_bfloat16* xb_img, const __nv_bfloat16* wqkv, int L, int win,
-                          int ntiles, __nv_bfloat16* qkv_img, __nv_bfloat16* att, cudaStream_t st) {
+                          int ntiles, __nv_bfloat16* qkv_img, __nv_bfloat16* att, const TileFlow& flow,
+                          cudaStream_t st) {
   const int split = (ntiles + 1) / 2;
   const int t0 = half ? split : 0, t1 = half ? ntiles : split;
   // a half without tiles still launches (one CTA that finds no work), as launch_ffn's
   const int n = t1 - t0;
   const int grid = n < 1 ? 1 : n < num_sms() ? n : num_sms();
-  if (qkv_img)
-    qkv_attention_kernel<true><<<grid, QkvAttCfg::kThreads, QkvAttCfg::kSmemBytes, st>>>(xb_img, wqkv, L, win, t0, t1,
-                                                                                        qkv_img, att);
-  else
-    qkv_attention_kernel<false><<<grid, QkvAttCfg::kThreads, QkvAttCfg::kSmemBytes, st>>>(xb_img, wqkv, L, win, t0,
-                                                                                         t1, nullptr, att);
+  launch(flow, qkv_img ? qkv_attention_kernel<true> : qkv_attention_kernel<false>, grid, QkvAttCfg::kThreads,
+         QkvAttCfg::kSmemBytes, st, xb_img, wqkv, L, win, t0, t1, qkv_img, att, flow);
 }
 
 
@@ -1389,8 +1484,8 @@ void launch_stitch(const uint8_t* bases, const uint8_t* quals, int L, const int6
   if (n_zmw > 0) stitch_kernel<<<n_zmw, 256, 0, st>>>(bases, quals, L, win_off, zmw_start, seq_out, qual_out, len_out);
 }
 
-void launch_head(const HeadParams& p, int ntiles, cudaStream_t st) {
-  head_kernel<<<ntiles, 128, 0, st>>>(p);
+void launch_head(const HeadParams& p, int ntiles, const TileFlow& flow, cudaStream_t st) {
+  launch(flow, head_kernel, ntiles, 128, 0, st, p, flow);
 }
 
 }  // namespace dcb

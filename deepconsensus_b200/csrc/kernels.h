@@ -9,14 +9,16 @@ namespace dcb {
 cudaError_t kernels_init();
 
 size_t embed_smem_bytes(int R, int echunks, int table_elems);
+// `flow` (common.h, TileFlow): the launch's place in the window-aligned forward's tile flow; null flags elsewhere (a
+// plain, serialized launch).
 // `packed` != null: the rows are read from packed input rows (include/dcb200.h) instead of `rows`.
 void launch_embed(const float* rows, const uint8_t* packed, const PackedLayout& pl, int R, int L, int Lw, int M, int ntiles, int echunks,
                   const EmbedCol* cols, const EmbedRow* rowmeta, const __nv_bfloat16* tables,
-                  int table_elems, __nv_bfloat16* emb, int* status, cudaStream_t st);
+                  int table_elems, __nv_bfloat16* emb, int* status, const TileFlow& flow, cudaStream_t st);
 // D = A * B^T with the 288-wide row epilogue (condenser + pos-enc, attention out-proj).
 // b_ksteps == 2 * a_ksteps: b_img holds split-bf16 weights [W_hi; W_lo] along K (kernels.cu, gemm_kernel).
 void launch_gemm_row(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int a_ksteps, int b_ksteps, int ntiles,
-                     const RowEpi& epi, cudaStream_t st);
+                     const RowEpi& epi, const TileFlow& flow, cudaStream_t st);
 // fused q/k/v projection: A [tile][36][128][8] -> qkv image [tile][108][128][8]; b_img: kQKVN / kQKVGroup groups of
 // split-bf16 weights [72][kQKVGroup][8] (hi chunks, then lo chunks)
 void launch_gemm_qkv(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int ntiles,
@@ -27,7 +29,7 @@ void launch_gemm_qkv(const __nv_bfloat16* a_img, const __nv_bfloat16* b_img, int
 // operand image [tile][ff/8][128][8].
 void launch_ffn(int half, const __nv_bfloat16* xb_img, const __nv_bfloat16* w1_img, const float* b1,
                 const __nv_bfloat16* w2_img, int ff, int ntiles, __nv_bfloat16* hid_img, const RowEpi& epi,
-                cudaStream_t st);
+                const TileFlow& flow, cudaStream_t st);
 void launch_unpack_rows(const uint8_t* packed, const PackedLayout& pl, int nwindows, float* rows, cudaStream_t st);
 void launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* att, int L, int Lw, int win, int nwindows,
                       cudaStream_t st);
@@ -36,8 +38,9 @@ void launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* att, int L, int L
 // xb_img: A [tile][36][128][8]; wqkv: launch_gemm_qkv's weight image; att: [tile][36][128][8], rows < L written.
 // qkv_img, when not null, also receives the q/k/v image launch_gemm_qkv writes (debug capture).
 void launch_qkv_attention(int half, const __nv_bfloat16* xb_img, const __nv_bfloat16* wqkv, int L, int win,
-                          int ntiles, __nv_bfloat16* qkv_img, __nv_bfloat16* att, cudaStream_t st);
-void launch_head(const HeadParams& p, int ntiles, cudaStream_t st);
+                          int ntiles, __nv_bfloat16* qkv_img, __nv_bfloat16* att, const TileFlow& flow,
+                          cudaStream_t st);
+void launch_head(const HeadParams& p, int ntiles, const TileFlow& flow, cudaStream_t st);
 // Windows of the post-model stage are contiguous in their byte arrays: window w starts at win_off[w] (int64
 // [n_windows + 1], windows of any width) or, with win_off NULL, at w * L.
 __host__ __device__ inline int64_t window_offset(const int64_t* win_off, int w, int L) {

@@ -16,6 +16,9 @@ Writes DIR/profile_gemms.json (and DIR/trace.json, the torch.profiler trace it w
   hbm      for each FFN launch and each fused q/k/v + attention launch, the activation bytes it reads and writes in
            HBM (the weights stay in L2), computed from the image shapes, over its kernel time and against the H100
            SXM data sheet's 3.35 TB/s.
+  timeline how the launches of one step sit on the GPU's clock: the span from its first kernel start to its last
+           kernel end, the sum of kernel durations and the gap from each kernel to the next (negative where launches
+           overlap), medians over the profiled steps.
   l2_ceiling  scripts/l2_stream.cu, compiled into a temporary directory: every SM streams the same L2-resident 1.18 MB
            weight image through the GEMM's 4-stage bulk-copy ring with consumers that only release the slots.
 The card's name, power limit and clocks are recorded beside the numbers.  DCB200_LIB selects another build of the
@@ -98,6 +101,36 @@ def hbm_bytes(role, ntiles, ff):
   return {"ffn_up": xb + hid, "ffn_down": hid + x + x + xb,
           "ffn_first": xb + x + x + xb, "ffn_second": xb + x + x + xb,
           "qkv_att_first": xb + xb, "qkv_att_second": xb + xb}.get(role)
+
+
+def timeline(kernels, roles):
+  """How the launches of one step sit on the GPU's clock.  A step runs from one embedding kernel to the kernel before
+  the next.  span_us: first kernel start to last kernel end; kernel_us: the sum of kernel durations; gaps_us: from each
+  kernel's end to the next one's start, named by the two roles (negative where the next launch overlaps the one
+  before it).  Each is the median over the profiled steps; between_steps_us is the gap from a step's last kernel to
+  the next step's first."""
+  steps, cur = [], []
+  for e, r in zip(kernels, roles):
+    if r == "embed" and cur:
+      steps.append(cur)
+      cur = []
+    cur.append((r, float(e["ts"]), float(e["dur"])))
+  if cur:
+    steps.append(cur)
+  full = [s for s in steps if len(s) == len(steps[0])]
+  gaps, spans, sums = {}, [], []
+  for s in full:
+    spans.append(max(t + d for _, t, d in s) - s[0][1])
+    sums.append(sum(d for _, _, d in s))
+    for i in range(1, len(s)):
+      name = "%02d %s->%s" % (i, s[i - 1][0], s[i][0])
+      gaps.setdefault(name, []).append(s[i][1] - (s[i - 1][1] + s[i - 1][2]))
+  between = [b[0][1] - max(t + d for _, t, d in a) for a, b in zip(steps, steps[1:])]
+  med = lambda v: float(np.median(v)) if v else None  # noqa: E731
+  g = {k: med(v) for k, v in gaps.items()}
+  return dict(steps=len(full), launches_per_step=len(steps[0]) if steps else 0, span_us=med(spans),
+              kernel_us=med(sums), idle_us=med([a - b for a, b in zip(spans, sums)]),
+              gap_sum_us=float(sum(g.values())), between_steps_us=med(between), gaps_us=g)
 
 
 def main():
@@ -183,9 +216,11 @@ def main():
 
   per = {}
   prev = None
+  roles = []
   for e in kernels:
     r = role_of(e["name"], prev)
     prev = r
+    roles.append(r)
     d = per.setdefault(r, dict(launches=0, us=[], name=e["name"].split("(")[0]))
     d["launches"] += 1
     d["us"].append(float(e["dur"]))
@@ -208,7 +243,7 @@ def main():
       rec["hbm_share_of_3_35_tbps"] = rec["hbm_tbps"] / HBM_TBPS
     out[r] = rec
   result.update(kernels=out, steps=args.steps, batch=B, ntiles=ntiles, tokens=args.tokens,
-                kernel_ms_per_step=total / 1e3 / args.steps, gpu_after=gpu_info())
+                kernel_ms_per_step=total / 1e3 / args.steps, timeline=timeline(kernels, roles), gpu_after=gpu_info())
   with open(os.path.join(args.out, "profile_gemms.json"), "w") as f:
     json.dump(result, f, indent=1)
   print(json.dumps(result))
