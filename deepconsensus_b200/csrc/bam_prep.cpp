@@ -106,6 +106,15 @@ struct Bgzf {
     }
     return 1;
   }
+  // Positions the reader at a BGZF virtual offset: the compressed block starts at voff >> 16, the record at byte
+  // voff & 0xffff of its inflated contents.
+  bool seek(uint64_t voff) {
+    fail = false;
+    if (fseeko(f, (off_t)(voff >> 16), SEEK_SET) != 0 || !next_block()) { fail = true; return false; }
+    pos = voff & 0xffff;
+    if (pos > block.size()) { fail = true; return false; }
+    return true;
+  }
 };
 
 struct Tag { char type = 0, sub = 0; const uint8_t* p = nullptr; size_t count = 0; };
@@ -506,6 +515,13 @@ struct ZmwState {
   std::vector<int32_t> win_start; // column of every emitted window
   std::vector<int32_t> win_width; // its spaced width (overflow when > max_length)
   RawRecords raw;                 // raw-record mode (dcb_prep_export_records): the records instead of `reads`
+  int label_status = -1;          // with a truth alignment open: DCB_LABEL_* of the fetch, the record in `label`
+  BamRecord label;
+  int label_rc = -1;              // label_of of `label` once dcb_prep_get_label asked for it (-1: not yet)
+  std::string label_error;
+  std::vector<uint32_t> label_cigar;
+  std::vector<uint8_t> label_bases;
+  int32_t label_info[DCB_LABEL_INFO] = {};
   int rc = DCB_OK;                // error of the processing step (message in `error`)
   std::string error;
 };
@@ -514,7 +530,103 @@ struct ZmwJob {
   std::vector<BamRecord> group;
   BamRecord ccs;
   std::string name;
+  int label_status = -1;
+  BamRecord label;
 };
+
+// The part of a BAM index (.bai, SAM/BAM spec v1.6 section 5.2) a whole-reference fetch needs: per reference, the
+// smallest virtual offset any of its bins' chunks starts at (UINT64_MAX: the reference has no records).
+int read_bai(const std::string& path, size_t n_ref, std::vector<uint64_t>* first) {
+  FILE* f = fopen(path.c_str(), "rb");
+  if (!f) return pfail(DCB_ERR_INVALID, "cannot open the index %s (the truth alignment must be indexed)", path.c_str());
+  std::vector<uint8_t> d;
+  uint8_t buf[1 << 16];
+  size_t n;
+  while ((n = fread(buf, 1, sizeof buf, f)) > 0) d.insert(d.end(), buf, buf + n);
+  fclose(f);
+  size_t o = 0;
+  bool bad = false;
+  auto get = [&](void* dst, size_t bytes) { if (o + bytes > d.size()) { bad = true; return; } memcpy(dst, &d[o], bytes); o += bytes; };
+  char magic[4] = {0, 0, 0, 0};
+  int32_t nr = 0;
+  get(magic, 4);
+  get(&nr, 4);
+  if (bad || memcmp(magic, "BAI\1", 4) || nr < 0 || (size_t)nr != n_ref)
+    return pfail(DCB_ERR_INVALID, "%s: not a BAM index for this BAM", path.c_str());
+  first->assign(n_ref, UINT64_MAX);
+  for (int32_t r = 0; r < nr && !bad; ++r) {
+    int32_t n_bin = 0;
+    get(&n_bin, 4);
+    for (int32_t b = 0; b < n_bin && !bad; ++b) {
+      uint32_t bin = 0;
+      int32_t n_chunk = 0;
+      get(&bin, 4);
+      get(&n_chunk, 4);
+      if (n_chunk < 0) bad = true;
+      for (int32_t c = 0; c < n_chunk && !bad; ++c) {
+        uint64_t beg = 0, end = 0;
+        get(&beg, 8);
+        get(&end, 8);
+        if (bin != 37450) (*first)[r] = std::min((*first)[r], beg);   // 37450: the pseudo-bin of per-reference counts
+      }
+    }
+    int32_t n_intv = 0;
+    get(&n_intv, 4);
+    if (n_intv < 0 || o + 8ull * n_intv > d.size()) bad = true; else o += 8ull * n_intv;
+  }
+  if (bad) return pfail(DCB_ERR_INVALID, "%s: truncated BAM index", path.c_str());
+  return DCB_OK;
+}
+
+// The label record in the shape dcb_prep_get_label hands out: what expand_clip_indent keeps of it with truth_range set
+// (pre_lib.py:1128-1239; no ins_trim).  Hard clips give no column; with any soft clip, the columns outside
+// [query_alignment_start, query_alignment_end) go -- the soft clips and the deletions between them and the first / last
+// aligned base.  info: DCB_LABEL_INFO entries.
+int label_of(const BamRecord& rec, std::vector<uint32_t>* cigar, std::vector<uint8_t>* bases, int32_t* info) {
+  const char* nm = rec.qname.c_str();
+  if (rec.flag & 4) return pfail(DCB_ERR_INVALID, "%s: the truth alignment is unmapped", nm);
+  if (int rc = check_plausible(rec)) return rc;
+  std::vector<uint32_t> ops;
+  for (uint32_t c : rec.cigar) {
+    const int op = c & 15;
+    if (op == kCHard || (c >> 4) == 0) continue;
+    if (op != kCMatch && op != kCIns && op != kCDel && op != kCSoft && op != kCEq && op != kCDiff)
+      return pfail(DCB_ERR_INVALID, "%s: truth alignment with a reference skip, pad or unknown cigar operation (not supported)", nm);
+    ops.push_back(c);
+  }
+  size_t nq = 0;
+  for (uint32_t c : ops) nq += op_has_query(c & 15) ? c >> 4 : 0;
+  if (nq != rec.seq.size()) return pfail(DCB_ERR_INVALID, "%s: cigar covers %zu query bases, sequence has %zu", nm, nq, rec.seq.size());
+  int32_t lead = 0, trail = 0;
+  size_t a = 0, b = ops.size();
+  if (a < b && (ops[a] & 15) == kCSoft) lead = (int32_t)(ops[a++] >> 4);
+  if (a < b && (ops[b - 1] & 15) == kCSoft) trail = (int32_t)(ops[--b] >> 4);
+  for (size_t i = a; i < b; ++i)
+    if ((ops[i] & 15) == kCSoft) return pfail(DCB_ERR_INVALID, "%s: soft clip inside the truth alignment", nm);
+  int32_t dropped = 0;
+  if (lead || trail) {
+    size_t i = a, j = b;
+    while (i < j && (ops[i] & 15) == kCDel) dropped += (int32_t)(ops[i++] >> 4);
+    while (j > i && (ops[j - 1] & 15) == kCDel) --j;
+    if (i == j) return pfail(DCB_ERR_INVALID, "%s: cannot locate the aligned part", nm);
+    a = i; b = j;
+  }
+  cigar->assign(ops.begin() + a, ops.begin() + b);
+  bases->clear();
+  size_t q = lead;
+  for (uint32_t c : *cigar) {
+    if (!op_has_query(c & 15)) continue;
+    for (size_t k = 0; k < (c >> 4); ++k) {
+      const char ch = rec.seq[q++];
+      const uint8_t id = (uint8_t)encode_base(ch);
+      if (!id) return pfail(DCB_ERR_INVALID, "%s: truth base '%c' outside ACGT (not supported)", nm, ch);
+      bases->push_back(id);
+    }
+  }
+  info[0] = DCB_LABEL_FOUND; info[1] = (int32_t)cigar->size(); info[2] = (int32_t)bases->size(); info[3] = rec.pos;
+  info[4] = rec.pos + dropped; info[5] = lead; info[6] = trail; info[7] = rec.flag;
+  return DCB_OK;
+}
 
 struct PrepCfg { int P = 0, L = 0, bq = 0, ins_trim = 0, R = 0; bool records = false, smart = false; dcb::PackedLayout pl{}; };
 
@@ -634,6 +746,8 @@ void process_zmw(const PrepCfg& cfg, ZmwJob* job, ZmwState* st) {
   st->name = job->name;
   st->n_subreads = (int32_t)job->group.size();
   st->reads.clear();
+  st->label_status = job->label_status;
+  st->label = std::move(job->label);
   const BamRecord& c = job->ccs;
   if (cfg.records) {
     for (const BamRecord& r : job->group) {
@@ -703,6 +817,11 @@ void process_zmw(const PrepCfg& cfg, ZmwJob* job, ZmwState* st) {
 struct dcb_prep {
   BamReader sub, ccs;
   PrepCfg cfg;
+  // dcb_prep_open_truth: the truth alignment, its references by name and each one's first virtual offset (read_bai)
+  BamReader truth;
+  bool have_truth = false;
+  std::map<std::string, int32_t> truth_tid;
+  std::vector<uint64_t> truth_first;
   bool have_pending = false, sub_eof = false;
   BamRecord pending;
   int64_t pending_zm = 0;
@@ -723,6 +842,24 @@ struct dcb_prep {
 };
 
 namespace {
+
+// next(truth_to_ccs.fetch(name)) (pre_lib.py:1001-1014): the first record of the reference named after the CCS read, found
+// by seeking to the smallest chunk start of its bins and reading on to the first record with its tid; none when the
+// reference is not in the header or has no records.  A supplementary first record is reported as such.
+int fetch_label(dcb_prep* p, ZmwJob* job) {
+  job->label_status = DCB_LABEL_NOT_FOUND;
+  auto it = p->truth_tid.find(job->name);
+  if (it == p->truth_tid.end() || p->truth_first[it->second] == UINT64_MAX) return 1;
+  if (!p->truth.z.seek(p->truth_first[it->second])) return pfail(DCB_ERR_INVALID, "truth alignment: bad index offset for %s", job->name.c_str());
+  for (;;) {
+    const int rc = p->truth.next(&job->label);
+    if (rc < 0) return rc;
+    if (rc == 0 || job->label.refid < 0 || job->label.refid > it->second) return 1;
+    if (job->label.refid == it->second) break;
+  }
+  job->label_status = (job->label.flag & 0x800) ? DCB_LABEL_SUPPLEMENTARY : DCB_LABEL_FOUND;
+  return 1;
+}
 
 // Sequential I/O: the next group of mapped subreads with one zm (SubreadGrouper, pre_lib.py:50-91) and its CCS record
 // (pre_lib.py:1322-1330).  1 = job filled, 0 = end of file, < 0 = error.
@@ -763,7 +900,7 @@ int read_job(dcb_prep* p, ZmwJob* job) {
     if (rc == 0) return pfail(DCB_ERR_INVALID, "ccs bam does not contain %s", job->name.c_str());
     if (job->ccs.qname == job->name) break;
   }
-  return 1;
+  return p->have_truth ? fetch_label(p, job) : 1;
 }
 
 void reader_main(dcb_prep* p) {
@@ -1039,6 +1176,37 @@ int dcb_prep_get_records(dcb_prep* p, int64_t* sizes, int32_t* read_meta, float*
   put(cigar, r.cigar.data(), r.cigar.size() * 4);
   put(bases, r.bases.data(), r.bases.size()); put(pw, r.pw.data(), r.pw.size()); put(ip, r.ip.data(), r.ip.size());
   put(ccs_bases, r.ccs_bases.data(), r.ccs_bases.size()); put(ccs_bq, r.ccs_bq.data(), r.ccs_bq.size());
+  return DCB_OK;
+}
+
+// Training mode: open the truth alignment to the CCS reads and its index (path + ".bai").  Call before the first
+// dcb_prep_next_zmw; every ZMW then fetches its label record on the decoding side.
+int dcb_prep_open_truth(dcb_prep* p, const char* truth_to_ccs_bam) {
+  if (!p || !truth_to_ccs_bam) return pfail(DCB_ERR_INVALID, "dcb_prep_open_truth: null argument");
+  if (p->started || p->next_seq || p->have_truth) return pfail(DCB_ERR_STATE, "dcb_prep_open_truth: the stream has already started");
+  if (int rc = p->truth.open(truth_to_ccs_bam)) return rc;
+  if (int rc = read_bai(std::string(truth_to_ccs_bam) + ".bai", p->truth.refs.size(), &p->truth_first)) return rc;
+  for (size_t i = 0; i < p->truth.refs.size(); ++i) p->truth_tid.emplace(p->truth.refs[i], (int32_t)i);
+  p->have_truth = true;
+  return DCB_OK;
+}
+
+// The loaded ZMW's label (include/dcb200.h).  info [DCB_LABEL_INFO] is always written; cigar / bases may be NULL.
+int dcb_prep_get_label(dcb_prep* p, int32_t* info, uint32_t* cigar, uint8_t* bases) {
+  if (!p || !info) return pfail(DCB_ERR_INVALID, "dcb_prep_get_label: null argument");
+  memset(info, 0, sizeof(int32_t) * DCB_LABEL_INFO);
+  if (!p->have_truth || p->cur.label_status < 0) return pfail(DCB_ERR_STATE, "dcb_prep_get_label: no ZMW loaded with a truth alignment open");
+  ZmwState& st = p->cur;
+  info[0] = st.label_status;
+  if (st.label_status != DCB_LABEL_FOUND) return DCB_OK;
+  if (st.label_rc < 0) {   // converted once per ZMW, on the first call
+    st.label_rc = label_of(st.label, &st.label_cigar, &st.label_bases, st.label_info);
+    if (st.label_rc) st.label_error = g_prep_error;
+  }
+  if (st.label_rc) { g_prep_error = st.label_error; return st.label_rc; }
+  std::copy(st.label_info, st.label_info + DCB_LABEL_INFO, info);
+  if (cigar) std::copy(st.label_cigar.begin(), st.label_cigar.end(), cigar);
+  if (bases) std::copy(st.label_bases.begin(), st.label_bases.end(), bases);
   return DCB_OK;
 }
 

@@ -188,6 +188,10 @@ struct dcb_engine {
     DevBuf<int4> win_list, window;
     DevBuf<int16_t> out_bq, ccs_bq_full;
     DevBuf<uint8_t> ccs_ids_full;
+    DevBuf<int32_t> label_meta;       // dcb_features_labels
+    DevBuf<uint32_t> label_cigar;
+    DevBuf<uint8_t> label_bases, labels, label_status;
+    DevBuf<int4> label_scan;
     std::vector<int32_t> width;   // spaced width of every window of the resident layout
     DevBuf<int> status;
     PrepBatch batch{};
@@ -1867,6 +1871,79 @@ int dcb_features_ccs(dcb_engine* e, const int32_t* windows, int32_t n, const int
   launch_features_ccs(fp.batch, fp.window, d_list, n, d_off, ids.d, bq.d, st);
   CU(e, cudaEventRecord(e->ev_eval1, st));
   if ((rc = copy_out(e, ids)) || (rc = copy_out(e, bq))) return rc;
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  return DCB_OK;
+}
+
+int dcb_features_labels(dcb_engine* e, const dcb_labels* lab, const int32_t* windows, int32_t n, uint8_t* labels_out,
+                        uint8_t* status_out, int32_t* ccs_width_out, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  auto& fp = e->fp;
+  if (ms_out) *ms_out = 0.f;
+  if (n < 0 || !lab) return fail(e, DCB_ERR_INVALID, "dcb_features_labels: bad argument");
+  if (fp.n_windows < 0) return fail(e, DCB_ERR_STATE, "dcb_features_labels before a successful dcb_features_layout");
+  const int nz = fp.batch.n_zmw;
+  if (lab->n_zmw != nz) return fail(e, DCB_ERR_INVALID, "dcb_features_labels: %d labels for a layout of %d ZMWs", lab->n_zmw, nz);
+  if (ccs_width_out && nz) {
+    std::vector<int4> zo(nz);
+    CU(e, cudaMemcpyAsync(zo.data(), fp.zmw_out.p, (size_t)nz * sizeof(int4), cudaMemcpyDeviceToHost, e->stream));
+    CU(e, cudaStreamSynchronize(e->stream));
+    for (int z = 0; z < nz; ++z) ccs_width_out[z] = zo[z].y;
+  }
+  if (n == 0) return DCB_OK;
+  if (!windows || !labels_out || !status_out || !lab->label_meta || (lab->n_cigar && !lab->cigar) || (lab->n_bases && !lab->bases) ||
+      lab->n_cigar < 0 || lab->n_bases < 0)
+    return fail(e, DCB_ERR_INVALID, "dcb_features_labels: null pointer or negative size");
+  for (int i = 0; i < n; ++i)
+    if (windows[i] < 0 || windows[i] >= fp.n_windows)
+      return fail(e, DCB_ERR_INVALID, "dcb_features_labels: window %d outside the layout's %d windows", windows[i], fp.n_windows);
+  // every offset and every operation is checked here, so the kernels index only inside the arrays they are given; the
+  // cigar ranges must follow one another (ZMW z's scan scratch is [offset + z, offset + z + count]), disjoint ranges
+  // keeping the CTAs' scratch apart
+  int64_t cig_end = 0;
+  for (int z = 0; z < nz; ++z) {
+    const int32_t* m = lab->label_meta + (size_t)z * DCB_LABEL_META;
+    if (m[0] < cig_end || m[1] < 0 || (int64_t)m[0] + m[1] > lab->n_cigar || m[2] < 0 || m[3] < 0 ||
+        (int64_t)m[2] + m[3] > lab->n_bases || m[4] < 0 || m[4] > (1 << 24) || m[5] < 0 || m[5] > (1 << 24))
+      return fail(e, DCB_ERR_INVALID, "dcb_features_labels: label of ZMW %d has offsets or lengths out of range, or a cigar "
+                  "range that overlaps or precedes the previous label's", z);
+    cig_end = (int64_t)m[0] + m[1];
+    int64_t noni = m[4], ins = 0, nq = 0;
+    for (int o = m[0]; o < m[0] + m[1]; ++o) {
+      const uint32_t c = lab->cigar[o], op = c & 15, len = c >> 4;
+      if (op != 0 && op != 1 && op != 2 && op != 7 && op != 8)
+        return fail(e, DCB_ERR_INVALID, "dcb_features_labels: label of ZMW %d has cigar operation %u (only M, I, D, =, X)", z, op);
+      (op == 1 ? ins : noni) += len;
+      if (op != 2) nq += len;
+    }
+    if (nq != m[3] || noni > (1 << 24) || ins > (1 << 24))
+      return fail(e, DCB_ERR_INVALID, "dcb_features_labels: the cigar of ZMW %d's label covers %lld bases, it has %d", z, (long long)nq, m[3]);
+    for (int q = m[2]; q < m[2] + m[3]; ++q)
+      if (lab->bases[q] < 1 || lab->bases[q] > 4)
+        return fail(e, DCB_ERR_INVALID, "dcb_features_labels: label of ZMW %d has base id %d (only 1..4)", z, lab->bases[q]);
+  }
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  const int L = e->L;
+  const int32_t* d_list;
+  LabelBatch lb{};
+  Output<uint8_t> rows, status;
+  int rc;
+  if ((rc = stage_in(e, fp.list, windows, (size_t)n, false, &d_list)) ||
+      (rc = stage_in(e, fp.label_meta, lab->label_meta, (size_t)nz * DCB_LABEL_META, false, &lb.meta)) ||
+      (rc = stage_in(e, fp.label_cigar, lab->cigar, (size_t)lab->n_cigar, false, &lb.cigar)) ||
+      (rc = stage_in(e, fp.label_bases, lab->bases, (size_t)lab->n_bases, false, &lb.bases)) ||
+      (rc = ensure(e, fp.label_scan, (size_t)lab->n_cigar + nz)) ||
+      (rc = stage_out(e, fp.labels, labels_out, (size_t)n * L, false, &rows)) ||
+      (rc = stage_out(e, fp.label_status, status_out, (size_t)n, false, &status)))
+    return rc;
+  lb.scan = fp.label_scan;
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  launch_labels(fp.batch, lb, fp.window, d_list, n, rows.d, status.d, st);
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  if ((rc = copy_out(e, rows)) || (rc = copy_out(e, status))) return rc;
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));

@@ -117,6 +117,18 @@ void launch_prep_layout(const PrepBatch& b, const PrepWindows& out, cudaStream_t
 // packed rows of windows list[0..n_list) (indices into the layout's n_windows windows), in that order
 void launch_prep_pack(const PrepBatch& b, const int4* window, const int32_t* list, int n_list, int n_windows, uint8_t* packed,
                       cudaStream_t st);
+// training labels of windows list[0..n_list) of the resident layout (dcb_features_labels): meta [n_zmw][kLabelMeta] =
+// cigar offset, cigar count, base offset, base count, pos (the indent), ccs0 (CCS index of the first cigar column);
+// the cigar holds M / I / D / = / X only, bases are ids 1..4.  scan: n_cigar + n_zmw entries of scratch.
+constexpr int kLabelMeta = 6;   // DCB_LABEL_META
+struct LabelBatch {
+  const int32_t* meta;
+  const uint32_t* cigar;
+  const uint8_t* bases;
+  int4* scan;
+};
+void launch_labels(const PrepBatch& b, const LabelBatch& lb, const int4* window, const int32_t* list, int n_list,
+                   uint8_t* labels_out, uint8_t* status_out, cudaStream_t st);
 // the CCS ids / qualities of windows list[0..n_list) at full width, window j at off[j] of ccs_ids / ccs_bq
 void launch_features_ccs(const PrepBatch& b, const int4* window, const int32_t* list, int n_list, const int64_t* off,
                          uint8_t* ccs_ids, int16_t* ccs_bq, cudaStream_t st);

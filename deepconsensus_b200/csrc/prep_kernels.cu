@@ -22,6 +22,19 @@
 // the i-th insertion of that run lands in spaced column k + E(k) + i and the k-th non-insertion column in
 // k + E(k + 1); the spaced width is M + E(M + 1) for M the largest non-insertion count of any read.  (A read without
 // columns collects G(0) gaps before it is marked done, which the read owning that run reaches too, so the width holds.)
+// The layout leaves E in the `gap` scratch (E(k) for k <= M + 1; E(k) = E(M + 1) beyond), for the label kernels.
+//
+// The label (training mode, pre_lib.py:200-216) walks the same lock-step but never reports an insertion: at every step it
+// first places all its pending insertion bases in consecutive columns of its own, then takes a gap on an insertion step
+// of the other reads and its next non-insertion column on any other step.  So G and E stay those of the other reads, the
+// label's k-th non-insertion column is still consumed on the k-th non-insertion step, and its column is shifted right by
+// the label insertions in front of it.  With I(k) the label's insertion columns before its k-th non-insertion column,
+//   label column of its k-th non-insertion column  k + E(k + 1) + I(k)
+//   label column of an insertion base in front of its k-th non-insertion column, n label insertions before it
+//                                                  k + E(k) + n
+// so between label columns k - 1 and k lie the label's own insertion bases, then G(k) gap columns.  A window's label is
+// `ccs_slice` of the label (pre_lib.py:308-334): every label column from the first to the last whose CCS index lies in
+// the window's inclusive CCS bounds, and the label's k-th non-insertion column holds CCS index k - pos + ccs0.
 #include "kernels.h"
 
 namespace dcb {
@@ -322,7 +335,126 @@ __global__ void __launch_bounds__(256) prep_pack_kernel(PrepBatch b, const int4*
   for (int t = threadIdx.x; t < b.pl.stride / 16; t += blockDim.x) dst[t] = sh_row[t];
 }
 
+// ---- labels (training mode).  Per ZMW: the label's cigar scanned into (non-insertion columns before the operation,
+// the indent included; insertion columns before it; bases of non-insertion columns before it; query bases before it),
+// with the totals in entry ncig.
+struct LabelScan {
+  int noni, ins, based, q;
+};
+
+__device__ __forceinline__ LabelScan label_combine(const LabelScan& a, const LabelScan& b) {
+  return LabelScan{a.noni + b.noni, a.ins + b.ins, a.based + b.based, a.q + b.q};
+}
+
+__device__ __forceinline__ LabelScan label_element(uint32_t c) {
+  const int op = c & 15, len = (int)(c >> 4);
+  const bool based = op == kOpM || op == kOpEq || op == kOpX;
+  return LabelScan{op == kOpI ? 0 : len, op == kOpI ? len : 0, based ? len : 0, (based || op == kOpI) ? len : 0};
+}
+
 }  // namespace
+
+// The label kernels have external linkage: the anonymous namespace above holds the inference construction kernels.
+__global__ void __launch_bounds__(kPrepThreads) label_scan_kernel(LabelBatch lb) {
+  __shared__ LabelScan sh[kPrepThreads];
+  const int z = blockIdx.x, tid = threadIdx.x;
+  const int* m = lb.meta + (size_t)z * kLabelMeta;
+  const int cig0 = m[0], ncig = m[1];
+  const uint32_t* cig = lb.cigar + cig0;
+  int4* scan = lb.scan + cig0 + z;
+  const int per = (ncig + kPrepThreads - 1) / kPrepThreads;
+  const int lo = min(tid * per, ncig), hi = min(lo + per, ncig);
+  LabelScan agg{0, 0, 0, 0};
+  for (int o = lo; o < hi; ++o) agg = label_combine(agg, label_element(cig[o]));
+  LabelScan pre = block_scan(agg, LabelScan{m[4], 0, 0, 0}, sh, label_combine);
+  if (tid) pre = label_combine(LabelScan{m[4], 0, 0, 0}, pre);
+  for (int o = lo; o < hi; ++o) {
+    scan[o] = make_int4(pre.noni, pre.ins, pre.based, pre.q);
+    pre = label_combine(pre, label_element(cig[o]));
+  }
+  if (tid == kPrepThreads - 1) scan[ncig] = make_int4(pre.noni, pre.ins, pre.based, pre.q);
+}
+
+// One CTA per listed window: the window's label row, built in shared memory.
+__global__ void __launch_bounds__(128) label_window_kernel(PrepBatch b, LabelBatch lb, const int4* window, const int32_t* list,
+                                                           uint8_t* labels_out, uint8_t* status_out) {
+  extern __shared__ uint8_t row[];
+  __shared__ int s_k1, s_k2, s_c1, s_mode, s_i1, s_b1;
+  const int L = b.pl.L, tid = threadIdx.x;
+  const int4 wz = window[list[blockIdx.x]];
+  const PrepZmw zm = b.zmw[wz.x];
+  const int mmax = b.zmw_out[wz.x].w;
+  const int* E = b.gap + zm.gap_off;
+  auto Ep = [&](int k) { return E[min(k, mmax + 1)]; };
+  const int* m = lb.meta + (size_t)wz.x * kLabelMeta;
+  const int ncig = m[1], pos = m[4], ccs0 = m[5];
+  const uint32_t* cig = lb.cigar + m[0];
+  const uint8_t* bases = lb.bases + m[2];
+  const int4* scan = lb.scan + m[0] + wz.x;
+  auto op_of = [&](int k) {   // the operation holding the label's k-th non-insertion column: first o with scan[o + 1].x > k
+    int a = 0, c = ncig - 1;
+    while (a < c) { const int mid = (a + c) >> 1; if (scan[mid + 1].x > k) c = mid; else a = mid + 1; }
+    return a;
+  };
+  auto is_based = [&](int o) { const int op = cig[o] & 15; return op == kOpM || op == kOpEq || op == kOpX; };
+  for (int i = tid; i < L; i += blockDim.x) row[i] = 0;
+  if (tid == 0) {
+    // the window's inclusive CCS bounds: its first and last CCS position (CCS position j sits in column j + E(j + 1))
+    auto first_at = [&](int col) {
+      int a = 0, c = zm.ccs_len;
+      while (a < c) { const int mid = (a + c) >> 1; if (mid + E[mid + 1] < col) a = mid + 1; else c = mid; }
+      return a;
+    };
+    const int s = first_at(wz.y), e = first_at(wz.y + wz.z) - 1;
+    const int m_lab = scan[ncig].x;
+    const int k1 = max(pos, s - ccs0 + pos), k2 = min(m_lab - 1, e - ccs0 + pos);
+    int mode = 0, c1 = 0, i1 = 0, b1 = 0;
+    if (k1 <= k2) {
+      const int o1 = op_of(k1), o2 = op_of(k2);
+      i1 = scan[o1].y;
+      c1 = k1 + Ep(k1 + 1) + i1;
+      const int c2 = k2 + Ep(k2 + 1) + scan[o2].y;
+      b1 = scan[o1].z + (is_based(o1) ? k1 - scan[o1].x : 0);
+      const int b2 = scan[o2].z + (is_based(o2) ? k2 + 1 - scan[o2].x : 0);
+      const int nongap = b2 - b1 + scan[o2].y - i1;
+      if (k1 == k2 && c1 == 0) mode = 3;                // ccs_slice's `locs.any()` is False for locs == [0]: no label
+      else if (c2 - c1 + 1 <= L) mode = 0;
+      else mode = nongap <= L ? 1 : 2;                  // remove_gaps; still too long: the window is dropped
+    } else {
+      mode = 3;
+    }
+    s_k1 = k1; s_k2 = k2; s_c1 = c1; s_mode = mode; s_i1 = i1; s_b1 = b1;
+  }
+  __syncthreads();
+  const int mode = s_mode;
+  if (mode <= 1) {
+    const int k1 = s_k1, k2 = s_k2, c1 = s_c1, i1 = s_i1, b1 = s_b1;
+    for (int k = k1 + tid; k <= k2; k += blockDim.x) {         // non-insertion columns: a base or a gap
+      const int o = op_of(k);
+      if (!is_based(o)) continue;
+      const int4 sc = scan[o];
+      const int at = mode == 0 ? k + Ep(k + 1) + sc.y - c1 : sc.z + (k - sc.x) - b1 + sc.y - i1;
+      row[at] = bases[sc.w + (k - sc.x)];
+    }
+    const int o1 = op_of(k1), o2 = op_of(k2);
+    for (int o = o1 + 1 + tid; o < o2; o += blockDim.x) {       // insertion bases between them
+      if ((cig[o] & 15) != kOpI) continue;
+      const int4 sc = scan[o];
+      const int len = (int)(cig[o] >> 4);
+      for (int i = 0; i < len; ++i)
+        row[mode == 0 ? sc.x + Ep(sc.x) + sc.y + i - c1 : sc.z - b1 + sc.y + i - i1] = bases[sc.w + i];
+    }
+  }
+  __syncthreads();
+  for (int i = tid; i < L; i += blockDim.x) labels_out[(size_t)blockIdx.x * L + i] = row[i];
+  if (tid == 0) status_out[blockIdx.x] = mode == 3 ? 0 : (uint8_t)mode;
+}
+
+void launch_labels(const PrepBatch& b, const LabelBatch& lb, const int4* window, const int32_t* list, int n_list,
+                   uint8_t* labels_out, uint8_t* status_out, cudaStream_t st) {
+  if (b.n_zmw > 0) label_scan_kernel<<<b.n_zmw, kPrepThreads, 0, st>>>(lb);
+  if (n_list > 0) label_window_kernel<<<n_list, 128, b.pl.L, st>>>(b, lb, window, list, labels_out, status_out);
+}
 
 void launch_prep_layout(const PrepBatch& b, const PrepWindows& out, cudaStream_t st) {
   if (b.n_zmw == 0) return;

@@ -84,6 +84,15 @@ class DcbTensor(ctypes.Structure):
 READ_META = 10   # DCB_READ_META: int32 fields per subread in the raw records
 
 
+LABEL_META = 6  # DCB_LABEL_META: int32 fields per label in dcb_labels
+
+
+class DcbLabels(ctypes.Structure):
+  """dcb_labels: one training label per ZMW of a dcb_features_layout batch (include/dcb200.h)."""
+  _fields_ = [("n_zmw", ctypes.c_int32), ("n_cigar", ctypes.c_int32), ("n_bases", ctypes.c_int32), ("reserved", ctypes.c_int32),
+              ("label_meta", ctypes.c_void_p), ("cigar", ctypes.c_void_p), ("bases", ctypes.c_void_p)]
+
+
 class DcbRecords(ctypes.Structure):
   """dcb_records: the raw records of a batch of ZMWs (include/dcb200.h "feature construction on the device")."""
   _fields_ = [("n_zmw", ctypes.c_int32), ("n_cigar", ctypes.c_int32), ("n_query", ctypes.c_int32), ("reserved", ctypes.c_int32)] + [
@@ -100,7 +109,8 @@ ABI_SYMBOLS = (
     "dcb_alignment_loss_grad", "dcb_distill_loss_grad", "dcb_prep_open", "dcb_prep_set_threads", "dcb_prep_next_zmw", "dcb_prep_get_windows", "dcb_prep_ccs_header", "dcb_prep_close",
     "dcb_prep_last_error", "dcb_prep_export_records", "dcb_prep_get_records", "dcb_prep_use_ccs_smart_windows",
     "dcb_prep_get_window_widths", "dcb_prep_get_overflow_ccs", "dcb_features_layout", "dcb_features_pack",
-    "dcb_features_layout_smart", "dcb_features_ccs", "dcb_prep_get_window_lengths",
+    "dcb_features_layout_smart", "dcb_features_ccs", "dcb_prep_get_window_lengths", "dcb_prep_open_truth",
+    "dcb_prep_get_label", "dcb_features_labels",
     "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
     "dcb_last_forward_launches", "dcb_set_profile", "dcb_get_profile", "dcb_get_profile_kernels", "dcb_alloc_host",
     "dcb_free_host", "dcb_alloc_device", "dcb_free_device", "dcb_memcpy_h2d", "dcb_memcpy_d2h",
@@ -174,6 +184,7 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_features_layout_smart.argtypes = [vp, ctypes.POINTER(DcbRecords), vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp,
                                             ctypes.POINTER(i32), ctypes.POINTER(ctypes.c_float)]
   lib.dcb_features_ccs.argtypes = [vp, vp, i32, vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_features_labels.argtypes = [vp, ctypes.POINTER(DcbLabels), vp, i32, vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_launches.argtypes = [vp, ctypes.POINTER(i32)]
   lib.dcb_set_debug.argtypes = [vp, i32]
@@ -690,6 +701,23 @@ class B200Model:
     self._check(self._lib.dcb_features_ccs(self._handle, _ptr(idx), len(idx), _ptr(off), _ptr(ids), _ptr(bq), ctypes.byref(ms)))
     return dict(ccs_ids=ids, ccs_bq=bq, off=off, ms=float(ms.value))
 
+  def features_labels(self, labels: Dict[str, np.ndarray], windows: np.ndarray) -> Dict[str, Any]:
+    """dcb_features_labels: the training label rows of the listed windows of the last features_layout.  `labels` is
+    `concat_labels` of one label per ZMW of that batch.  Returns dict(labels uint8 [k, L] over ' ATCG', status uint8 [k]
+    (0 kept, 1 gaps removed, 2 overflow), ccs_width int32 [n_zmw] (DcExample.ccs_width per ZMW of the batch), ms)."""
+    idx = np.ascontiguousarray(windows, dtype=np.int32).reshape(-1)
+    meta, cig, bases = (np.ascontiguousarray(labels[k], dt) for k, dt in (("label_meta", np.int32), ("cigar", np.uint32),
+                                                                         ("bases", np.uint8)))
+    lab = DcbLabels(n_zmw=meta.reshape(-1, LABEL_META).shape[0], n_cigar=cig.size, n_bases=bases.size,
+                    label_meta=_ptr(meta), cigar=_ptr(cig), bases=_ptr(bases))
+    out = dict(labels=np.zeros((len(idx), self.max_length), np.uint8), status=np.zeros(len(idx), np.uint8),
+               ccs_width=np.zeros(lab.n_zmw, np.int32))
+    ms = ctypes.c_float(0)
+    self._check(self._lib.dcb_features_labels(self._handle, ctypes.byref(lab), _ptr(idx), len(idx), _ptr(out["labels"]),
+                                              _ptr(out["status"]), _ptr(out["ccs_width"]), ctypes.byref(ms)))
+    out["ms"] = float(ms.value)
+    return out
+
   def stitch_raw(self, bases_ptr: int, quals_ptr: int, n_windows: int, zmw_start: np.ndarray, flags: int,
                  seq_ptr: int, qual_ptr: int, len_ptr: int, length: Optional[int] = None) -> None:
     """dcb_stitch on caller-managed pointers (host or device per `flags`)."""
@@ -1013,6 +1041,19 @@ def concat_records(zmws: List[Dict[str, Any]]) -> Dict[str, np.ndarray]:
               read_meta=np.concatenate(meta) if meta else np.zeros((0, READ_META), np.int32),
               read_sn=cat("read_sn", np.float32, (4,)), cigar=cat("cigar", np.uint32), bases=cat("bases", np.uint8),
               pw=cat("pw", np.uint8), ip=cat("ip", np.uint8), ccs_bases=cat("ccs_bases", np.uint8), ccs_bq=cat("ccs_bq", np.uint8))
+
+
+def concat_labels(labels: List[Dict[str, Any]]) -> Dict[str, np.ndarray]:
+  """Labels of `preprocess.BamFeatureStream.label()` (one per ZMW, in the order of the records batch) as dcb_labels
+  arrays: cigar and bases concatenated, label_meta [n, LABEL_META] with offsets into them."""
+  meta = np.zeros((len(labels), LABEL_META), np.int32)
+  c0 = b0 = 0
+  for i, lab in enumerate(labels):
+    meta[i] = (c0, len(lab["cigar"]), b0, len(lab["bases"]), lab["pos"], lab["ccs0"])
+    c0 += len(lab["cigar"])
+    b0 += len(lab["bases"])
+  cat = lambda k, dt: np.concatenate([np.asarray(lab[k], dt) for lab in labels]) if labels else np.zeros(0, dt)
+  return dict(label_meta=meta, cigar=cat("cigar", np.uint32), bases=cat("bases", np.uint8))
 
 
 def pipelined(items: Iterable[Any], submit: Callable[[Any], Any], wait: Callable[[Any], Any],

@@ -10,8 +10,10 @@ extract_features.  This module hands the results out in the reference's own shap
   stream_zmw_packed(...)    the same windows as packed rows (include/dcb200.h "packed input rows") + per-window metadata,
                             with no float32 rows and no per-window Python objects in between
   BamWriter                 the unaligned-BAM output of `deepconsensus run --output *.bam` (quick_inference.py:742-760)
+  make_examples / main      `deepconsensus preprocess`: tf.Example files, labelled from a truth alignment in training
+                            mode (`python -m deepconsensus_b200.preprocess`), with the windows and labels built on the GPU
 
-Needs no GPU.
+Everything but make_examples needs no GPU.
 """
 from __future__ import annotations
 
@@ -49,6 +51,8 @@ def _lib():
     lib.dcb_prep_get_overflow_ccs.argtypes = [vp, vp, vp]
     lib.dcb_prep_get_window_lengths.argtypes = [vp, vp, vp]
     lib.dcb_prep_get_records.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.dcb_prep_open_truth.argtypes = [vp, ctypes.c_char_p]
+    lib.dcb_prep_get_label.argtypes = [vp, vp, vp, vp]
     lib.dcb_prep_ccs_header.argtypes = [vp]
     lib.dcb_prep_ccs_header.restype = ctypes.c_char_p
     lib.dcb_prep_close.argtypes = [vp]
@@ -66,14 +70,17 @@ class BamFeatureStream:
   iter_examples, pre_lib.py:1279-1384,625-697)."""
 
   def __init__(self, subreads_to_ccs: str, ccs_bam: str, max_passes: int, max_length: int, use_ccs_bq: bool = False,
-               ins_trim: int = 5, threads: int = 0, records: bool = False, use_ccs_smart_windows: bool = False):
+               ins_trim: int = 5, threads: int = 0, records: bool = False, use_ccs_smart_windows: bool = False,
+               truth_to_ccs: Optional[str] = None):
     """threads > 0: ZMWs are processed by that many native worker threads (plus one BAM-decoding thread) while the
     caller consumes them; the order of the ZMWs is the file's either way (`--cpus` of `deepconsensus run`).
     records: the stream only decodes and validates, and hands each ZMW out as raw records (`next_zmw_records`) for
     feature construction on the device; `next_zmw` is not available then.
     use_ccs_smart_windows: windows are cut at the widths of each CCS record's `wl` tag (pre_lib.py:625-650); windows
     wider than max_length are overflow windows, whose full-width CCS `next_zmw` returns as `overflow_ccs_ids` /
-    `overflow_ccs_bq`; with `records`, `next_zmw_records` hands out each ZMW's `wl` tag."""
+    `overflow_ccs_bq`; with `records`, `next_zmw_records` hands out each ZMW's `wl` tag.
+    truth_to_ccs: the truth alignment to the CCS reads (indexed, path + ".bai"); each ZMW fetches its label record as it
+    is decoded, and `label()` hands it out."""
     self._lib = _lib()
     self._h = ctypes.c_void_p()
     self.max_passes, self.max_length, self.use_ccs_bq = int(max_passes), int(max_length), bool(use_ccs_bq)
@@ -86,6 +93,8 @@ class BamFeatureStream:
       raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
     self.use_ccs_smart_windows = bool(use_ccs_smart_windows)
     if self.use_ccs_smart_windows and self._lib.dcb_prep_use_ccs_smart_windows(self._h, 1):
+      raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
+    if truth_to_ccs and self._lib.dcb_prep_open_truth(self._h, truth_to_ccs.encode()):
       raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
     self.records = bool(records)
     if records and self._lib.dcb_prep_export_records(self._h, 1):
@@ -184,6 +193,23 @@ class BamFeatureStream:
       self._lib.dcb_prep_get_window_lengths(self._h, vp(n_wl), vp(out["wl"]))
     return out
 
+  def label(self) -> Dict[str, Any]:
+    """The loaded ZMW's label (dcb_prep_get_label): dict(status 'found' / 'not_found' / 'supplementary'), and when found
+    cigar uint32 (M / I / D / = / X), bases uint8 ids 1..4, pos (indent), ccs0 (CCS index of the first cigar column),
+    soft_clip (leading, trailing), flag.  Raises PrepError for a label record the reference cannot use."""
+    info = np.zeros(8, np.int32)
+    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    if self._lib.dcb_prep_get_label(self._h, vp(info), None, None):
+      raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
+    status = ("found", "not_found", "supplementary")[int(info[0])]
+    if status != "found":
+      return dict(status=status)
+    cigar, bases = np.zeros(int(info[1]), np.uint32), np.zeros(int(info[2]), np.uint8)
+    if self._lib.dcb_prep_get_label(self._h, vp(info), vp(cigar), vp(bases)):
+      raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
+    return dict(status=status, cigar=cigar, bases=bases, pos=int(info[3]), ccs0=int(info[4]),
+                soft_clip=(int(info[5]), int(info[6])), flag=int(info[7]))
+
   def __iter__(self):
     while True:
       z = self.next_zmw()
@@ -235,3 +261,225 @@ class BamWriter:
       self._h = ctypes.c_void_p()
       if rc:
         raise PrepError(self._lib.dcb_prep_last_error().decode("utf-8", "replace"))
+
+
+# ----------------------------------------------------------------------------------------------- `preprocess` CLI
+# Chromosomes of each split (the genome is chosen by the split file's path, as the reference's read_truth_split does).
+_HUMAN_TRAIN = [str(i) for i in range(1, 19)] + ["chr%d" % i for i in range(1, 19)] + ["X", "Y", "chrX", "chrY"]
+_SPLIT_CHROMS = {
+    "human": dict(train=_HUMAN_TRAIN, eval=["21", "22", "chr21", "chr22"], test=["19", "20", "chr19", "chr20"]),
+    "maize": dict(train=[str(i) for i in range(1, 9)] + ["chr%d" % i for i in range(1, 9)], eval=["9", "chr9"],
+                  test=["10", "chr10"]),
+}
+
+
+def read_truth_bed(path: str) -> Dict[str, Dict[str, Any]]:
+  """CCS read name -> dict(contig, begin, end) from the first four tab-separated columns of each line."""
+  out = {}
+  with open(path) as f:
+    for line in f:
+      contig, begin, end, name = line.strip().split("\t")[:4]
+      out[name] = dict(contig=contig, begin=int(begin), end=int(end))
+  return out
+
+
+def read_truth_split(path: str) -> Dict[str, str]:
+  """Contig -> 'train' / 'eval' / 'test' from a `contig chromosome` file; contigs on other chromosomes get no split."""
+  low = path.lower()
+  if any(x in low for x in ("chm13", "hg00", "human")):
+    chroms = _SPLIT_CHROMS["human"]
+  elif "maize" in low:
+    chroms = _SPLIT_CHROMS["maize"]
+  else:
+    raise ValueError("%s does not correspond to any known genome: its name must contain human, chm13, hg00 or maize" % path)
+  split_of = {c: s for s in ("train", "eval", "test") for c in chroms[s]}
+  out = {}
+  with open(path) as f:
+    for line in f:
+      contig, chrom = line.split()
+      if chrom in split_of:
+        out[contig] = split_of[chrom]
+  return out
+
+
+def _empty_label() -> Dict[str, Any]:
+  return dict(cigar=np.zeros(0, np.uint32), bases=np.zeros(0, np.uint8), pos=0, ccs0=0)
+
+
+def _zmw_bp_counts(z: Dict[str, Any], ins_trim: int, counter) -> None:
+  """trim_insertions' counters (pre_lib.py:1093-1108) from a ZMW's untrimmed subread cigars."""
+  if ins_trim <= 0:
+    return
+  ops, lens = z["cigar"] & 15, (z["cigar"] >> 4).astype(np.int64)
+  trimmed = (ops == 1) & (lens > ins_trim)
+  counter["zmw_total_bp"] += int(lens.sum())
+  if trimmed.any():
+    counter["zmw_trimmed_insertions"] += int(trimmed.sum())
+    counter["zmw_trimmed_insertions_bp"] += int(lens[trimmed].sum())
+
+
+def make_examples(subreads_to_ccs: str, ccs_bam: str, output: str, truth_to_ccs: Optional[str] = None,
+                  truth_bed: Optional[str] = None, truth_split: Optional[str] = None, max_passes: int = 20,
+                  max_length: int = 100, use_ccs_bq: bool = False, ins_trim: int = 5, limit: int = 0, cpus: int = 0,
+                  batch_zmws: int = 64, model=None) -> Dict[str, Any]:
+  """`deepconsensus preprocess` (preprocess.py:243-361): tf.Examples of every ZMW, with labels when the three truth
+  inputs are given, built on the GPU (dcb_features_layout / _pack / _labels).  Writes `output` per split and the summary
+  JSON; returns the summary."""
+  import collections
+  import json
+  import os
+
+  from deepconsensus_b200 import tfrecord, weights as weights_lib
+  training = bool(truth_to_ccs and truth_bed and truth_split)
+  if not output.endswith(".tfrecord.gz"):
+    raise ValueError("--output must end with .tfrecord.gz")
+  if training:
+    contig_split = read_truth_split(truth_split)
+    bed = read_truth_bed(truth_bed)
+    splits = sorted(set(contig_split.values()))
+    if splits and "@split" not in output:
+      raise ValueError("You must add @split to --output when training.")
+  elif truth_to_ccs or truth_bed or truth_split:
+    raise ValueError("You must specify truth_to_ccs, truth_bed, and truth_split to generate a training dataset.")
+  else:
+    splits = ["inference"]
+  P, L = int(max_passes), int(max_length)
+  params = params_lib.synthetic_params(P, L, use_ccs_bq, num_hidden_layers=1)
+  if model is None:
+    # The feature and label kernels live in the engine, which is built for a model geometry: a one-layer model of this
+    # window shape with seeded weights gives them their scratch; its forward is never run.
+    model = engine_lib.B200Model(params, weights_lib.init_weights(params, seed=0), max_batch=64)
+  writers = {}
+  for s in splits:
+    path = output.replace("@split", s)
+    if os.path.dirname(path):
+      os.makedirs(os.path.dirname(path), exist_ok=True)
+    writers[s] = tfrecord.TFRecordWriter(path)
+  counter: collections.Counter = collections.Counter()
+  stream = BamFeatureStream(subreads_to_ccs, ccs_bam, P, L, use_ccs_bq, ins_trim, threads=max(int(cpus), 0), records=True,
+                            truth_to_ccs=truth_to_ccs if training else None)
+
+  def flush(batch):
+    if not batch:
+      return
+    zmws, labels, split_of = zip(*batch)
+    lay = model.features_layout(engine_lib.concat_records(list(zmws)), ins_trim)
+    n = len(lay["window_pos"])
+    idx = np.arange(n, dtype=np.int32)
+    lab = model.features_labels(engine_lib.concat_labels(list(labels)), idx if training else idx[:0])
+    rows = engine_lib.unpack_rows(params, model.features_pack(idx)["packed"]) if n else None
+    w = 0
+    for z, (zmw, s) in enumerate(zip(zmws, split_of)):
+      n_win = int(lay["zmw_windows"][z])
+      total = -(-int(lab["ccs_width"][z]) // L)
+      counter["example_width_bucket_%d" % L] += total
+      if total > n_win:
+        counter["n_examples_no_ccs_idx"] += total - n_win
+      written = 0
+      for i in range(w, w + n_win):
+        st = int(lab["status"][i]) if training else 0
+        if st == 2:
+          counter["n_examples_label_overflow"] += 1
+          continue
+        if st == 1:
+          counter["n_examples_adjusted_label"] += 1
+        counter["n_examples_skip_large_windows_keep"] += 1
+        writers[s].write(tfrecord.dc_example(rows[i], int(lay["num_passes"][i]), zmw["name"], int(lay["window_pos"][i]),
+                                             lay["ccs_bq"][i], lab["labels"][i] if training else None))
+        written += 1
+      counter["n_examples_%s" % s] += written
+      counter["n_examples"] += written
+      w += n_win
+    batch.clear()
+
+  batch = []
+  try:
+    while (z := stream.next_zmw_records()) is not None:
+      counter["n_zmw_processed"] += 1
+      _zmw_bp_counts(z, ins_trim, counter)
+      label = _empty_label()
+      if training:
+        rng = bed.get(z["name"])
+        if rng is None:
+          counter["n_zmw_missing_truth_range"] += 1
+          continue
+        label = stream.label()
+        if label["status"] == "not_found":
+          counter["n_zmw_no_label_alignment"] += 1
+          continue
+        if label["status"] == "supplementary":
+          counter["n_zmw_truth_label_supp_alignment"] += 1
+          continue
+        split = contig_split.get(rng["contig"])
+        if not split:
+          counter["n_zmw_missing_contig_split"] += 1
+          continue
+        # put_spacing's assertion (pre_lib.py:237), reached only by ZMWs that have a split: the label's aligned bases
+        # cover the bed range minus the soft clips
+        if len(label["bases"]) != rng["end"] - rng["begin"] - sum(label["soft_clip"]):
+          raise PrepError("%s: the truth alignment has %d aligned bases, its bed range %d" % (
+              z["name"], len(label["bases"]), rng["end"] - rng["begin"] - sum(label["soft_clip"])))
+      else:
+        split = "inference"
+      counter["n_zmw_%s" % split] += 1
+      counter["n_zmw_pass"] += 1
+      batch.append((z, label, split))
+      if len(batch) >= batch_zmws:
+        flush(batch)
+      if limit and counter["n_zmw_pass"] >= limit:
+        break
+    flush(batch)
+  finally:
+    stream.close()
+    for wr in writers.values():
+      wr.close()
+  summary = dict(counter.items())
+  summary.update(max_passes=str(P), max_length=str(L), tensor_height=str(params_lib.get_total_rows(P, use_ccs_bq)),
+                 tensor_width=str(L))
+  for k, v in (("subreads_to_ccs", subreads_to_ccs), ("ccs_bam", ccs_bam), ("truth_to_ccs", truth_to_ccs),
+               ("truth_bed", truth_bed), ("truth_split", truth_split), ("max_passes", P), ("max_length", L),
+               ("ins_trim", ins_trim)):
+    summary[k] = str(v)
+  summary["version"] = "1.2.0"
+  path = output.replace(".tfrecord.gz", ".%s.json" % ("training" if training else "inference")).replace("@split", "summary")
+  if os.path.dirname(path):
+    os.makedirs(os.path.dirname(path), exist_ok=True)
+  with open(path, "w") as f:
+    f.write(json.dumps(summary, indent=True))
+  return summary
+
+
+def main(argv: Optional[List[str]] = None) -> int:
+  import argparse
+  ap = argparse.ArgumentParser(prog="python -m deepconsensus_b200.preprocess",
+                               description="tf.Examples from subreads aligned to CCS reads, labelled when a truth alignment "
+                                           "is given (`deepconsensus preprocess`), built on the GPU.")
+  ap.add_argument("--subreads_to_ccs", required=True)
+  ap.add_argument("--ccs_bam", required=True)
+  ap.add_argument("--output", required=True, help="must end in .tfrecord.gz; with the truth flags it must hold @split")
+  ap.add_argument("--truth_to_ccs")
+  ap.add_argument("--truth_bed")
+  ap.add_argument("--truth_split")
+  ap.add_argument("--max_passes", type=int, default=20)
+  ap.add_argument("--max_length", type=int, default=100)
+  ap.add_argument("--use_ccs_bq", action="store_true")
+  ap.add_argument("--use_ccs_smart_windows", action="store_true")
+  ap.add_argument("--ins_trim", type=int, default=5)
+  ap.add_argument("--limit", type=int, default=0)
+  ap.add_argument("--cpus", type=int, default=0, help="host threads that decode and validate the BAMs (0: none)")
+  a = ap.parse_args(argv)
+  if a.use_ccs_smart_windows:
+    if a.truth_to_ccs or a.truth_bed or a.truth_split:
+      ap.error("--use_ccs_smart_windows is not supported with the truth flags (training mode)")
+    # inference examples of overflow windows hold rows wider than max_length, which the packed rows cannot carry
+    ap.error("--use_ccs_smart_windows is not supported by preprocess; `run --use_ccs_smart_windows` builds smart windows")
+  if a.cpus == 1:
+    ap.error("Must set cpus to 0 or >=2 for parallel processing.")
+  summary = make_examples(a.subreads_to_ccs, a.ccs_bam, a.output, a.truth_to_ccs, a.truth_bed, a.truth_split, a.max_passes,
+                          a.max_length, a.use_ccs_bq, a.ins_trim, a.limit, a.cpus)
+  print("wrote %d examples of %d ZMWs" % (summary.get("n_examples", 0), summary.get("n_zmw_pass", 0)))
+  return 0
+
+
+if __name__ == "__main__":
+  raise SystemExit(main())

@@ -147,3 +147,70 @@ def read_examples(paths: Union[str, Sequence[str]], limit: int = -1) -> Dict[str
               names=np.array(names, dtype=object), window_pos=np.array(pos, np.int32),
               num_passes=np.array(npass, np.int32),
               ccs_base_quality_scores=np.stack(bq) if bq else np.zeros((0, L), np.int16))
+
+
+# ----------------------------------------------------------------------------------------------- writer
+def _varint(v: int) -> bytes:
+  v &= (1 << 64) - 1
+  out = bytearray()
+  while True:
+    b = v & 0x7F
+    v >>= 7
+    if v:
+      out.append(b | 0x80)
+    else:
+      out.append(b)
+      return bytes(out)
+
+
+def _field(num: int, payload: bytes) -> bytes:
+  return _varint(num << 3 | 2) + _varint(len(payload)) + payload
+
+
+def serialize_example(features: Dict[str, Union[List[bytes], List[int]]]) -> bytes:
+  """tf.Example with bytes_list (values of type bytes) and int64_list (ints) features, keys in the dict's order."""
+  entries = b""
+  for key, vals in features.items():
+    if vals and isinstance(vals[0], (bytes, bytearray)):
+      lst = _field(1, b"".join(_field(1, bytes(v)) for v in vals))                 # Feature.bytes_list = 1
+    else:
+      lst = _field(3, _field(1, b"".join(_varint(int(v)) for v in vals)))          # Feature.int64_list = 3, packed
+    entries += _field(1, _field(1, key.encode()) + _field(2, lst))                # Features.feature map entry
+  return _field(1, entries)                                                        # Example.features = 1
+
+
+def frame_record(payload: bytes) -> bytes:
+  """TFRecord framing: u64 length, masked crc32c of it, payload, masked crc32c of the payload."""
+  length = struct.pack("<Q", len(payload))
+  return (length + struct.pack("<I", tf_checkpoint.mask_crc(tf_checkpoint.crc32c(length))) + payload +
+          struct.pack("<I", tf_checkpoint.mask_crc(tf_checkpoint.crc32c(payload))))
+
+
+def dc_example(rows: np.ndarray, num_passes: int, name: str, window_pos: int, ccs_bq: np.ndarray,
+               label: "np.ndarray | None" = None) -> bytes:
+  """DcExample.tf_example (pre_lib.py:764-787) serialised: rows float32 [R, L] stored as [R, L, 1], the CCS base
+  qualities, and with a label (ids over ' ATCG', [L]) label/encoded float32 and label/shape."""
+  rows = np.ascontiguousarray(rows, "<f4")
+  f: Dict[str, Union[List[bytes], List[int]]] = {
+      "subreads/encoded": [rows.tobytes()], "subreads/shape": [rows.shape[0], rows.shape[1], 1],
+      "subreads/num_passes": [int(num_passes)], "name": [name.encode()], "window_pos": [int(window_pos)],
+      "ccs_base_quality_scores": [int(v) for v in np.asarray(ccs_bq).reshape(-1)]}
+  if label is not None:
+    lab = np.ascontiguousarray(label, "<f4")
+    f["label/encoded"] = [lab.tobytes()]
+    f["label/shape"] = [lab.shape[0]]
+  return serialize_example(f)
+
+
+class TFRecordWriter:
+  """GZIP'd TFRecord file (what tf.io.TFRecordWriter with compression_type='GZIP' writes; the compressed stream need not
+  be byte-identical)."""
+
+  def __init__(self, path: str):
+    self._f = gzip.open(path, "wb")
+
+  def write(self, payload: bytes) -> None:
+    self._f.write(frame_record(payload))
+
+  def close(self) -> None:
+    self._f.close()

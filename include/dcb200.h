@@ -394,6 +394,23 @@ int dcb_prep_get_window_lengths(dcb_prep* p, int32_t* n, int32_t* wl);
 int dcb_prep_export_records(dcb_prep* p, int32_t enabled);
 int dcb_prep_get_records(dcb_prep* p, int64_t* sizes, int32_t* read_meta, float* read_sn, uint32_t* cigar, uint8_t* bases,
                          uint8_t* pw, uint8_t* ip, uint8_t* ccs_bases, uint8_t* ccs_bq);
+/* Training mode (`preprocess` with a truth alignment): dcb_prep_open_truth opens the truth alignment to the CCS reads
+ * and its index (path + ".bai"), before the first dcb_prep_next_zmw.  Every ZMW then fetches, on the stream's decoding
+ * side, what next(truth_to_ccs.fetch(ccs_name)) gives (pre_lib.py:1001-1014): the first record of the reference named
+ * after the CCS read.  dcb_prep_get_label hands it out for the loaded ZMW; info [DCB_LABEL_INFO] is always written:
+ *   status (DCB_LABEL_*), cigar operations, bases, pos (the indent), ccs0 (CCS index of the first cigar column),
+ *   leading and trailing soft clip lengths, flag
+ * and with DCB_LABEL_FOUND cigar u32 [n] / bases u8 [n] (nullable) receive what expand_clip_indent keeps of the record
+ * (pre_lib.py:1128-1239, no ins_trim): hard clips dropped, and with any soft clip the soft clips and the deletions
+ * between them and the aligned bases removed, so the cigar holds M / I / D / = / X only; bases are ids 1..4 over
+ * ' ATCG'.  An unmapped record, reference skips, pads, inner soft clips, a cigar that disagrees with the sequence or a
+ * base outside ACGT is DCB_ERR_INVALID naming the ZMW (the reference leaves such label entries uninitialised). */
+#define DCB_LABEL_FOUND 0
+#define DCB_LABEL_NOT_FOUND 1
+#define DCB_LABEL_SUPPLEMENTARY 2
+#define DCB_LABEL_INFO 8
+int dcb_prep_open_truth(dcb_prep* p, const char* truth_to_ccs_bam);
+int dcb_prep_get_label(dcb_prep* p, int32_t* info, uint32_t* cigar, uint8_t* bases);
 const char* dcb_prep_ccs_header(dcb_prep* p);             /* SAM header text of the CCS BAM */
 void dcb_prep_close(dcb_prep* p);
 const char* dcb_prep_last_error(void);
@@ -458,6 +475,26 @@ int dcb_features_layout_smart(dcb_engine* e, const dcb_records* rec, const int32
                               int32_t* n_windows_out, float* ms_out);
 int dcb_features_ccs(dcb_engine* e, const int32_t* windows, int32_t n, const int64_t* off, uint8_t* ccs_ids, int16_t* ccs_bq,
                      float* ms_out);
+/* Training labels on the device, after dcb_features_layout on the same batch: labels holds one label per ZMW of that
+ * batch (host arrays; label_meta [n_zmw, DCB_LABEL_META] = cigar offset, cigar count, base offset, base count, pos,
+ * ccs0 of dcb_prep_get_label, offsets relative to the concatenated cigar / bases, the cigar ranges in ZMW order and
+ * disjoint; a label with no operations is all gaps).  labels_out u8 [n, L] receives the label row of windows[0..n) over ' ATCG' as bases_encoded gives it
+ * (pre_lib.py:652-697): the label columns whose CCS index lies in the window's inclusive CCS bounds and everything
+ * between them, padded with gaps to L; longer than L, its gaps removed (status 1, n_examples_adjusted_label); still
+ * longer, a row of gaps (status 2, n_examples_label_overflow: the window is dropped).  status_out u8 [n]: 0 kept,
+ * 1 adjusted, 2 overflow.  ccs_width_out (nullable) int32 [n_zmw]: DcExample.ccs_width of every ZMW of the layout
+ * (its spaced CCS read without trailing gaps), which iter_examples' window count follows.  Labels the engine cannot index, operations other than M / I / D / = / X, a cigar that
+ * disagrees with its base count or base ids outside 1..4 are DCB_ERR_INVALID; the engine and the layout stay usable.
+ * ms_out (nullable): device time of the kernels.  Deterministic, no atomics. */
+#define DCB_LABEL_META 6
+typedef struct dcb_labels {
+  int32_t n_zmw, n_cigar, n_bases, reserved;
+  const int32_t* label_meta;       /* [n_zmw, DCB_LABEL_META] */
+  const uint32_t* cigar;           /* [n_cigar] */
+  const uint8_t* bases;            /* [n_bases] */
+} dcb_labels;
+int dcb_features_labels(dcb_engine* e, const dcb_labels* labels, const int32_t* windows, int32_t n, uint8_t* labels_out,
+                        uint8_t* status_out, int32_t* ccs_width_out, float* ms_out);
 
 /* Device time of the last dcb_forward (milliseconds, CUDA events on the engine's stream). */
 int dcb_last_forward_ms(dcb_engine* e, float* ms);
