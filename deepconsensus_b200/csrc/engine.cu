@@ -172,7 +172,7 @@ struct dcb_engine {
   struct {   // dcb_fill_skipped(_ragged)
     DevBuf<uint8_t> ids, bases, quals; DevBuf<int16_t> bq; DevBuf<int32_t> dst; DevBuf<int64_t> src_off, dst_off; DevBuf<int> status;
   } fs;
-  struct { DevBuf<float> probs, loss; DevBuf<uint8_t> labels, ccs, exact; DevBuf<int32_t> pred, ccs_counts; } ev;   // dcb_evaluate
+  struct { DevBuf<float> probs, loss; DevBuf<uint8_t> labels, ccs, exact; DevBuf<int32_t> pred, ccs_counts; DevBuf<int> bad; } ev;   // dcb_evaluate
   struct { DevBuf<float> teacher, student, loss, grad; } ds;   // dcb_distill_loss, dcb_distill_loss_grad
   struct { DevBuf<float> probs, loss, grad, matches, dp; DevBuf<uint8_t> labels; } lg;   // dcb_alignment_loss_grad
   struct { DevBuf<float> bias, logits, probs; DevBuf<uint8_t> bases, quals; } he;   // dcb_debug_head_epilogue
@@ -192,6 +192,9 @@ struct dcb_engine {
     DevBuf<uint32_t> label_cigar;
     DevBuf<uint8_t> label_bases, labels, label_status;
     DevBuf<int4> label_scan;
+    DevBuf<int32_t> eval_dst;         // dcb_features_eval
+    DevBuf<uint8_t> keep;
+    DevBuf<int> eval_count;
     std::vector<int32_t> width;   // spaced width of every window of the resident layout
     DevBuf<int> status;
     PrepBatch batch{};
@@ -1526,7 +1529,8 @@ int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const
   if (!probs || !labels || !ccs_ids || !loss_out || !exact_out || !pred_counts || !ccs_counts)
     return fail(e, DCB_ERR_INVALID, "dcb_evaluate: null pointer");
   const size_t ntok = (size_t)batch * L;
-  if ((rc = check_labels(e, "dcb_evaluate", labels, batch, L, false))) return rc;
+  const bool lab_dev = flags & DCB_LABELS_ON_DEVICE;
+  if (!lab_dev && (rc = check_labels(e, "dcb_evaluate", labels, batch, L, false))) return rc;
   CU(e, cudaSetDevice(e->cfg.device));
   cudaStream_t st = e->stream;
   const float* d_probs;
@@ -1535,20 +1539,31 @@ int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const
   Output<int32_t> pred, ccs;
   Output<uint8_t> exact;
   if ((rc = stage_in(e, e->ev.probs, probs, ntok * kVocab, flags & DCB_ROWS_ON_DEVICE, &d_probs)) ||
-      (rc = stage_in(e, e->ev.labels, labels, ntok, false, &d_labels)) || (rc = stage_in(e, e->ev.ccs, ccs_ids, ntok, false, &d_ccs)) ||
+      (rc = stage_in(e, e->ev.labels, labels, ntok, lab_dev, &d_labels)) || (rc = stage_in(e, e->ev.ccs, ccs_ids, ntok, lab_dev, &d_ccs)) ||
+      (lab_dev && ((rc = ensure(e, e->ev.labels, ntok)) || (rc = ensure(e, e->ev.bad, 1)))) ||
       (rc = stage_out(e, e->ev.loss, loss_out, (size_t)batch, false, &loss)) ||
       (rc = stage_out(e, e->ev.pred, pred_counts, (size_t)batch * 5, false, &pred)) ||
       (rc = stage_out(e, e->ev.ccs_counts, ccs_counts, (size_t)batch * 5, false, &ccs)) ||
       (rc = stage_out(e, e->ev.exact, exact_out, (size_t)batch, false, &exact)))
     return rc;
+  int bad = 0;
+  if (lab_dev) {
+    // device labels are checked on the device: the kernels read a copy in which an id above 4 is 0, and the flag it
+    // raises comes back with the results
+    CU(e, cudaMemsetAsync(e->ev.bad.p, 0, sizeof(int), st));
+    launch_copy_label_ids(labels, e->ev.labels.p, ntok, e->ev.bad.p, st);
+    d_labels = e->ev.labels.p;
+  }
   const bool hard = !(loss_reg > 0.0);
   CU(e, cudaEventRecord(e->ev_eval0, st));
   CU(e, launch_evaluate(d_probs, d_labels, d_ccs, batch, L, (float)del_cost, hard ? 1.f : (float)loss_reg, hard ? 1 : 0,
                         loss.d, exact.d, pred.d, ccs.d, st));
   CU(e, cudaEventRecord(e->ev_eval1, st));
   if ((rc = copy_out(e, loss)) || (rc = copy_out(e, pred)) || (rc = copy_out(e, ccs)) || (rc = copy_out(e, exact))) return rc;
+  if (lab_dev) CU(e, cudaMemcpyAsync(&bad, e->ev.bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
+  if (bad) return fail(e, DCB_ERR_INVALID, "dcb_evaluate: a device label id lies outside 0..4");
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
   return DCB_OK;
 }
@@ -1877,6 +1892,50 @@ int dcb_features_ccs(dcb_engine* e, const int32_t* windows, int32_t n, const int
   return DCB_OK;
 }
 
+// The label batch of dcb_features_labels / dcb_features_eval: every offset and every operation is checked here, so the
+// kernels index only inside the arrays they are given; the cigar ranges must follow one another (ZMW z's scan scratch
+// is [offset + z, offset + z + count]), disjoint ranges keeping the CTAs' scratch apart.  `fn` names the call.
+static int check_label_batch(dcb_engine* e, const char* fn, const dcb_labels* lab, int nz) {
+  if (!lab->label_meta || (lab->n_cigar && !lab->cigar) || (lab->n_bases && !lab->bases) || lab->n_cigar < 0 || lab->n_bases < 0)
+    return fail(e, DCB_ERR_INVALID, "%s: null pointer or negative size", fn);
+  int64_t cig_end = 0;
+  for (int z = 0; z < nz; ++z) {
+    const int32_t* m = lab->label_meta + (size_t)z * DCB_LABEL_META;
+    if (m[0] < cig_end || m[1] < 0 || (int64_t)m[0] + m[1] > lab->n_cigar || m[2] < 0 || m[3] < 0 ||
+        (int64_t)m[2] + m[3] > lab->n_bases || m[4] < 0 || m[4] > (1 << 24) || m[5] < 0 || m[5] > (1 << 24))
+      return fail(e, DCB_ERR_INVALID, "%s: label of ZMW %d has offsets or lengths out of range, or a cigar "
+                  "range that overlaps or precedes the previous label's", fn, z);
+    cig_end = (int64_t)m[0] + m[1];
+    int64_t noni = m[4], ins = 0, nq = 0;
+    for (int o = m[0]; o < m[0] + m[1]; ++o) {
+      const uint32_t c = lab->cigar[o], op = c & 15, len = c >> 4;
+      if (op != 0 && op != 1 && op != 2 && op != 7 && op != 8)
+        return fail(e, DCB_ERR_INVALID, "%s: label of ZMW %d has cigar operation %u (only M, I, D, =, X)", fn, z, op);
+      (op == 1 ? ins : noni) += len;
+      if (op != 2) nq += len;
+    }
+    if (nq != m[3] || noni > (1 << 24) || ins > (1 << 24))
+      return fail(e, DCB_ERR_INVALID, "%s: the cigar of ZMW %d's label covers %lld bases, it has %d", fn, z, (long long)nq, m[3]);
+    for (int q = m[2]; q < m[2] + m[3]; ++q)
+      if (lab->bases[q] < 1 || lab->bases[q] > 4)
+        return fail(e, DCB_ERR_INVALID, "%s: label of ZMW %d has base id %d (only 1..4)", fn, z, lab->bases[q]);
+  }
+  return DCB_OK;
+}
+
+// Uploads a checked label batch and points lb at it (scan scratch included).
+static int stage_labels(dcb_engine* e, const dcb_labels* lab, int nz, LabelBatch* lb) {
+  auto& fp = e->fp;
+  int rc;
+  if ((rc = stage_in(e, fp.label_meta, lab->label_meta, (size_t)nz * DCB_LABEL_META, false, &lb->meta)) ||
+      (rc = stage_in(e, fp.label_cigar, lab->cigar, (size_t)lab->n_cigar, false, &lb->cigar)) ||
+      (rc = stage_in(e, fp.label_bases, lab->bases, (size_t)lab->n_bases, false, &lb->bases)) ||
+      (rc = ensure(e, fp.label_scan, (size_t)lab->n_cigar + nz)))
+    return rc;
+  lb->scan = fp.label_scan;
+  return DCB_OK;
+}
+
 int dcb_features_labels(dcb_engine* e, const dcb_labels* lab, const int32_t* windows, int32_t n, uint8_t* labels_out,
                         uint8_t* status_out, int32_t* ccs_width_out, float* ms_out) {
   if (!e) return DCB_ERR_INVALID;
@@ -1899,31 +1958,6 @@ int dcb_features_labels(dcb_engine* e, const dcb_labels* lab, const int32_t* win
   for (int i = 0; i < n; ++i)
     if (windows[i] < 0 || windows[i] >= fp.n_windows)
       return fail(e, DCB_ERR_INVALID, "dcb_features_labels: window %d outside the layout's %d windows", windows[i], fp.n_windows);
-  // every offset and every operation is checked here, so the kernels index only inside the arrays they are given; the
-  // cigar ranges must follow one another (ZMW z's scan scratch is [offset + z, offset + z + count]), disjoint ranges
-  // keeping the CTAs' scratch apart
-  int64_t cig_end = 0;
-  for (int z = 0; z < nz; ++z) {
-    const int32_t* m = lab->label_meta + (size_t)z * DCB_LABEL_META;
-    if (m[0] < cig_end || m[1] < 0 || (int64_t)m[0] + m[1] > lab->n_cigar || m[2] < 0 || m[3] < 0 ||
-        (int64_t)m[2] + m[3] > lab->n_bases || m[4] < 0 || m[4] > (1 << 24) || m[5] < 0 || m[5] > (1 << 24))
-      return fail(e, DCB_ERR_INVALID, "dcb_features_labels: label of ZMW %d has offsets or lengths out of range, or a cigar "
-                  "range that overlaps or precedes the previous label's", z);
-    cig_end = (int64_t)m[0] + m[1];
-    int64_t noni = m[4], ins = 0, nq = 0;
-    for (int o = m[0]; o < m[0] + m[1]; ++o) {
-      const uint32_t c = lab->cigar[o], op = c & 15, len = c >> 4;
-      if (op != 0 && op != 1 && op != 2 && op != 7 && op != 8)
-        return fail(e, DCB_ERR_INVALID, "dcb_features_labels: label of ZMW %d has cigar operation %u (only M, I, D, =, X)", z, op);
-      (op == 1 ? ins : noni) += len;
-      if (op != 2) nq += len;
-    }
-    if (nq != m[3] || noni > (1 << 24) || ins > (1 << 24))
-      return fail(e, DCB_ERR_INVALID, "dcb_features_labels: the cigar of ZMW %d's label covers %lld bases, it has %d", z, (long long)nq, m[3]);
-    for (int q = m[2]; q < m[2] + m[3]; ++q)
-      if (lab->bases[q] < 1 || lab->bases[q] > 4)
-        return fail(e, DCB_ERR_INVALID, "dcb_features_labels: label of ZMW %d has base id %d (only 1..4)", z, lab->bases[q]);
-  }
   CU(e, cudaSetDevice(e->cfg.device));
   cudaStream_t st = e->stream;
   const int L = e->L;
@@ -1931,21 +1965,69 @@ int dcb_features_labels(dcb_engine* e, const dcb_labels* lab, const int32_t* win
   LabelBatch lb{};
   Output<uint8_t> rows, status;
   int rc;
+  if ((rc = check_label_batch(e, "dcb_features_labels", lab, nz)) || (rc = stage_labels(e, lab, nz, &lb))) return rc;
   if ((rc = stage_in(e, fp.list, windows, (size_t)n, false, &d_list)) ||
-      (rc = stage_in(e, fp.label_meta, lab->label_meta, (size_t)nz * DCB_LABEL_META, false, &lb.meta)) ||
-      (rc = stage_in(e, fp.label_cigar, lab->cigar, (size_t)lab->n_cigar, false, &lb.cigar)) ||
-      (rc = stage_in(e, fp.label_bases, lab->bases, (size_t)lab->n_bases, false, &lb.bases)) ||
-      (rc = ensure(e, fp.label_scan, (size_t)lab->n_cigar + nz)) ||
       (rc = stage_out(e, fp.labels, labels_out, (size_t)n * L, false, &rows)) ||
       (rc = stage_out(e, fp.label_status, status_out, (size_t)n, false, &status)))
     return rc;
-  lb.scan = fp.label_scan;
   CU(e, cudaEventRecord(e->ev_eval0, st));
   launch_labels(fp.batch, lb, fp.window, d_list, n, rows.d, status.d, st);
   CU(e, cudaEventRecord(e->ev_eval1, st));
   if ((rc = copy_out(e, rows)) || (rc = copy_out(e, status))) return rc;
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  return DCB_OK;
+}
+
+int dcb_features_eval(dcb_engine* e, const dcb_labels* lab, const uint8_t* keep_zmw, int32_t n_keep, int32_t capacity,
+                      uint8_t* packed_out, uint8_t* labels_out, uint8_t* ccs_out, uint8_t* status_out, int32_t* ccs_width_out,
+                      int32_t* windows_out, int32_t* k_out, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  auto& fp = e->fp;
+  if (ms_out) *ms_out = 0.f;
+  if (!lab || !k_out || capacity < 0) return fail(e, DCB_ERR_INVALID, "dcb_features_eval: bad argument");
+  *k_out = 0;
+  if (fp.n_windows < 0) return fail(e, DCB_ERR_STATE, "dcb_features_eval before a successful dcb_features_layout");
+  const int nz = fp.batch.n_zmw, n = fp.n_windows;
+  if (lab->n_zmw != nz) return fail(e, DCB_ERR_INVALID, "dcb_features_eval: %d labels for a layout of %d ZMWs", lab->n_zmw, nz);
+  if (n_keep != nz || (nz && !keep_zmw))
+    return fail(e, DCB_ERR_INVALID, "dcb_features_eval: a keep mask of %d entries for a layout of %d ZMWs", n_keep, nz);
+  if (capacity && (!packed_out || !labels_out || !ccs_out)) return fail(e, DCB_ERR_INVALID, "dcb_features_eval: null pointer");
+  if (reinterpret_cast<uintptr_t>(packed_out) & 15) return fail(e, DCB_ERR_INVALID, "dcb_features_eval: packed_out must be 16-byte aligned");
+  int rc;
+  if ((rc = check_label_batch(e, "dcb_features_eval", lab, nz))) return rc;
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  if (ccs_width_out && nz) {
+    std::vector<int4> zo(nz);
+    CU(e, cudaMemcpyAsync(zo.data(), fp.zmw_out.p, (size_t)nz * sizeof(int4), cudaMemcpyDeviceToHost, st));
+    CU(e, cudaStreamSynchronize(st));
+    for (int z = 0; z < nz; ++z) ccs_width_out[z] = zo[z].y;
+  }
+  if (n == 0) return DCB_OK;
+  const int L = e->L;
+  LabelBatch lb{};
+  const uint8_t* d_keep;
+  if ((rc = stage_labels(e, lab, nz, &lb)) || (rc = stage_in(e, fp.keep, keep_zmw, (size_t)nz, false, &d_keep)) ||
+      (rc = ensure(e, fp.labels, (size_t)n * L)) || (rc = ensure(e, fp.label_status, (size_t)n)) ||
+      (rc = ensure(e, fp.eval_dst, (size_t)n)) || (rc = ensure(e, fp.list, (size_t)n)) || (rc = ensure(e, fp.eval_count, 1)))
+    return rc;
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  launch_features_eval(fp.batch, lb, fp.window, n, fp.ccs_ids, d_keep, capacity, fp.labels, fp.label_status, fp.eval_dst, fp.list,
+                       fp.eval_count, packed_out, labels_out, ccs_out, st);
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  int k = 0;
+  CU(e, cudaMemcpyAsync(&k, fp.eval_count.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  if (status_out) CU(e, cudaMemcpyAsync(status_out, fp.label_status.p, (size_t)n, cudaMemcpyDeviceToHost, st));
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  *k_out = k;
+  if (k > capacity) return fail(e, DCB_ERR_INVALID, "dcb_features_eval: %d windows are kept, the capacity is %d", k, capacity);
+  if (windows_out && k) {
+    CU(e, cudaMemcpyAsync(windows_out, fp.list.p, (size_t)k * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CU(e, cudaStreamSynchronize(st));
+  }
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
   return DCB_OK;
 }

@@ -501,6 +501,23 @@ cudaError_t launch_distill_loss_grad(const float* teacher, const float* student,
   return cudaGetLastError();
 }
 
+__global__ void __launch_bounds__(256)
+copy_label_ids_kernel(const uint8_t* __restrict__ labels, uint8_t* __restrict__ out, size_t n, int* __restrict__ bad) {
+  int any = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const uint8_t v = labels[i];
+    any |= v > 4;
+    out[i] = v > 4 ? 0 : v;
+  }
+  if (any) *bad = 1;   // a plain store: every writer stores the same value
+}
+
+void launch_copy_label_ids(const uint8_t* labels, uint8_t* out, size_t n, int* bad, cudaStream_t st) {
+  if (n == 0) return;
+  const size_t blocks = std::min<size_t>((n + 255) / 256, 1024);
+  copy_label_ids_kernel<<<(unsigned)blocks, 256, 0, st>>>(labels, out, n, bad);
+}
+
 size_t eval_identity_smem_bytes(int L) {
   return (size_t)9 * (L + 1) * sizeof(float) + 4 * (size_t)L + (size_t)(L + 1) * (L + 1);
 }

@@ -129,6 +129,13 @@ struct LabelBatch {
 };
 void launch_labels(const PrepBatch& b, const LabelBatch& lb, const int4* window, const int32_t* list, int n_list,
                    uint8_t* labels_out, uint8_t* status_out, cudaStream_t st);
+// evaluation inputs of the resident layout (dcb_features_eval): the label rows and statuses of all n_windows windows
+// (label_rows [n][L], status [n]), then the windows with status != 2 whose ZMW has keep_zmw set, compacted in window
+// order (dst [n]: place or -1; list [n]: window of each place; *count), and for places below cap their packed row,
+// label row and CCS row (ccs_rows: the layout's [n][L]) in packed / labels_out / ccs_out
+void launch_features_eval(const PrepBatch& b, const LabelBatch& lb, const int4* window, int n_windows, const uint8_t* ccs_rows,
+                          const uint8_t* keep_zmw, int cap, uint8_t* label_rows, uint8_t* status, int32_t* dst, int32_t* list,
+                          int* count, uint8_t* packed, uint8_t* labels_out, uint8_t* ccs_out, cudaStream_t st);
 // the CCS ids / qualities of windows list[0..n_list) at full width, window j at off[j] of ccs_ids / ccs_bq
 void launch_features_ccs(const PrepBatch& b, const int4* window, const int32_t* list, int n_list, const int64_t* off,
                          uint8_t* ccs_ids, int16_t* ccs_bq, cudaStream_t st);
@@ -138,6 +145,9 @@ void launch_features_ccs(const PrepBatch& b, const int4* window, const int32_t* 
 cudaError_t launch_evaluate(const float* probs, const uint8_t* labels, const uint8_t* ccs_ids, int B, int L,
                             float del_cost, float loss_reg, int hard_min, float* loss, uint8_t* exact,
                             int32_t* pred_counts, int32_t* ccs_counts, cudaStream_t st);
+// labels u8 [n] (device) copied to out with every id above 4 replaced by 0; *bad (zeroed by the caller) is set to 1 when
+// there was one, so that the evaluation kernels index only inside their tables and the call can refuse the labels
+void launch_copy_label_ids(const uint8_t* labels, uint8_t* out, size_t n, int* bad, cudaStream_t st);
 // AlignmentLoss per window with its gradient: loss [B], d loss / d probs [B, L, 5] and the soft alignment matches
 // [B, L, L] (both nullable).  `tables` is loss_grad_table_bytes(L, ctas) of device scratch, ctas from loss_grad_grid(B)
 // (persistent grid on the current device).  Device pointers.

@@ -7,6 +7,7 @@
 //                        spaced CCS read and the list of windows that hold a CCS position
 //   prep_emit_kernel     the per-window arrays of dcb_prep_get_windows except the rows, dense over the batch
 //   prep_pack_kernel     packed rows of the windows the caller lists, in the caller's order
+//   eval_*_kernel        the kept windows of a labelled batch compacted, with their packed, label and CCS rows
 //
 // Spacing in closed form.  space_out (bam_prep.cpp; pre_lib.py:1242-1276) steps all reads in lock-step: while any read
 // that is not done has an insertion next, the reads with an insertion next advance by it and every other unfinished read
@@ -302,14 +303,10 @@ __global__ void __launch_bounds__(256) prep_emit_kernel(PrepBatch b, PrepWindows
   }
 }
 
-// One CTA per listed window: the packed row is assembled in shared memory and leaves in 16-byte stores.
-__global__ void __launch_bounds__(256) prep_pack_kernel(PrepBatch b, const int4* window, const int32_t* list, int n_windows,
-                                                        uint8_t* packed, int* status) {
-  extern __shared__ uint4 sh_row[];
-  uint8_t* row = reinterpret_cast<uint8_t*>(sh_row);
-  const int idx = list[blockIdx.x];
-  if (idx < 0 || idx >= n_windows) { if (threadIdx.x == 0) *status |= 2; return; }
-  const int4 wz = window[idx];
+// The packed row of window wz (ZMW, start column, spaced width), assembled in shared memory `row` (pl.stride bytes) by the
+// whole CTA and written to dst in 16-byte stores.
+__device__ void assemble_packed_row(const PrepBatch& b, int4 wz, uint8_t* row, uint8_t* dst) {
+  uint4* sh_row = reinterpret_cast<uint4*>(row);
   const PrepZmw zm = b.zmw[wz.x];
   const int P = b.pl.P, L = b.pl.L, start = wz.y;
   const int n = min(L, wz.z);   // columns present (an overflow window's first L); the rest is padding
@@ -331,8 +328,17 @@ __global__ void __launch_bounds__(256) prep_pack_kernel(PrepBatch b, const int4*
   }
   if (threadIdx.x < 4) reinterpret_cast<float*>(row + b.pl.sn_off)[threadIdx.x] = b.read_sn[(size_t)zm.read0 * 4 + threadIdx.x];
   __syncthreads();
-  uint4* dst = reinterpret_cast<uint4*>(packed + (size_t)blockIdx.x * b.pl.stride);
-  for (int t = threadIdx.x; t < b.pl.stride / 16; t += blockDim.x) dst[t] = sh_row[t];
+  uint4* d = reinterpret_cast<uint4*>(dst);
+  for (int t = threadIdx.x; t < b.pl.stride / 16; t += blockDim.x) d[t] = sh_row[t];
+}
+
+// One CTA per listed window.
+__global__ void __launch_bounds__(256) prep_pack_kernel(PrepBatch b, const int4* window, const int32_t* list, int n_windows,
+                                                        uint8_t* packed, int* status) {
+  extern __shared__ uint4 sh_row[];
+  const int idx = list[blockIdx.x];
+  if (idx < 0 || idx >= n_windows) { if (threadIdx.x == 0) *status |= 2; return; }
+  assemble_packed_row(b, window[idx], reinterpret_cast<uint8_t*>(sh_row), packed + (size_t)blockIdx.x * b.pl.stride);
 }
 
 // ---- labels (training mode).  Per ZMW: the label's cigar scanned into (non-insertion columns before the operation,
@@ -375,13 +381,13 @@ __global__ void __launch_bounds__(kPrepThreads) label_scan_kernel(LabelBatch lb)
   if (tid == kPrepThreads - 1) scan[ncig] = make_int4(pre.noni, pre.ins, pre.based, pre.q);
 }
 
-// One CTA per listed window: the window's label row, built in shared memory.
+// One CTA per listed window (list null: window blockIdx.x): the window's label row, built in shared memory.
 __global__ void __launch_bounds__(128) label_window_kernel(PrepBatch b, LabelBatch lb, const int4* window, const int32_t* list,
                                                            uint8_t* labels_out, uint8_t* status_out) {
   extern __shared__ uint8_t row[];
   __shared__ int s_k1, s_k2, s_c1, s_mode, s_i1, s_b1;
   const int L = b.pl.L, tid = threadIdx.x;
-  const int4 wz = window[list[blockIdx.x]];
+  const int4 wz = window[list ? list[blockIdx.x] : blockIdx.x];
   const PrepZmw zm = b.zmw[wz.x];
   const int mmax = b.zmw_out[wz.x].w;
   const int* E = b.gap + zm.gap_off;
@@ -454,6 +460,51 @@ void launch_labels(const PrepBatch& b, const LabelBatch& lb, const int4* window,
                    uint8_t* labels_out, uint8_t* status_out, cudaStream_t st) {
   if (b.n_zmw > 0) label_scan_kernel<<<b.n_zmw, kPrepThreads, 0, st>>>(lb);
   if (n_list > 0) label_window_kernel<<<n_list, 128, b.pl.L, st>>>(b, lb, window, list, labels_out, status_out);
+}
+
+// ---- evaluation inputs (dcb_features_eval).  The kept windows -- label status != 2, ZMW kept by the caller -- are
+// compacted in window order by one CTA's block scan (no atomics, so the order is fixed): dst[w] is window w's place
+// among them or -1, list[j] the window in place j, *count their number.
+__global__ void __launch_bounds__(kPrepThreads) eval_compact_kernel(const int4* window, const uint8_t* status,
+                                                                    const uint8_t* keep_zmw, int n, int32_t* dst,
+                                                                    int32_t* list, int* count) {
+  __shared__ int sh[kPrepThreads];
+  const int tid = threadIdx.x;
+  const int per = (n + kPrepThreads - 1) / kPrepThreads;
+  const int lo = min(tid * per, n), hi = min(lo + per, n);
+  auto kept = [&](int w) { return status[w] != 2 && keep_zmw[window[w].x] != 0; };
+  int c = 0;
+  for (int w = lo; w < hi; ++w) c += kept(w);
+  int at = block_scan(c, 0, sh, [](int a, int x) { return a + x; });
+  for (int w = lo; w < hi; ++w) {
+    if (kept(w)) { dst[w] = at; list[at] = w; ++at; }
+    else dst[w] = -1;
+  }
+  if (tid == 0) *count = sh[kPrepThreads - 1];
+}
+
+// One CTA per window of the layout: a kept window's packed row, label row and CCS row go to its place among the kept
+// windows; places at or beyond `cap` are not written (the call reports the count and fails).
+__global__ void __launch_bounds__(256) eval_emit_kernel(PrepBatch b, const int4* window, const int32_t* dst, int cap,
+                                                        const uint8_t* label_rows, const uint8_t* ccs_rows, uint8_t* packed,
+                                                        uint8_t* labels_out, uint8_t* ccs_out) {
+  extern __shared__ uint4 sh_row[];
+  const int w = blockIdx.x, j = dst[w], L = b.pl.L;
+  if (j < 0 || j >= cap) return;
+  assemble_packed_row(b, window[w], reinterpret_cast<uint8_t*>(sh_row), packed + (size_t)j * b.pl.stride);
+  for (int i = threadIdx.x; i < L; i += blockDim.x) {
+    labels_out[(size_t)j * L + i] = label_rows[(size_t)w * L + i];
+    ccs_out[(size_t)j * L + i] = ccs_rows[(size_t)w * L + i];
+  }
+}
+
+void launch_features_eval(const PrepBatch& b, const LabelBatch& lb, const int4* window, int n_windows, const uint8_t* ccs_rows,
+                          const uint8_t* keep_zmw, int cap, uint8_t* label_rows, uint8_t* status, int32_t* dst, int32_t* list,
+                          int* count, uint8_t* packed, uint8_t* labels_out, uint8_t* ccs_out, cudaStream_t st) {
+  launch_labels(b, lb, window, nullptr, n_windows, label_rows, status, st);
+  eval_compact_kernel<<<1, kPrepThreads, 0, st>>>(window, status, keep_zmw, n_windows, dst, list, count);
+  if (n_windows > 0)
+    eval_emit_kernel<<<n_windows, 256, b.pl.stride, st>>>(b, window, dst, cap, label_rows, ccs_rows, packed, labels_out, ccs_out);
 }
 
 void launch_prep_layout(const PrepBatch& b, const PrepWindows& out, cudaStream_t st) {

@@ -32,6 +32,7 @@ DCB_ROWS_ON_DEVICE = 1
 DCB_OUT_ON_DEVICE = 2
 DCB_STRICT_FP32 = 4
 DCB_FAST_BF16 = 8
+DCB_LABELS_ON_DEVICE = 16
 DCB_PRECISION_BF16 = 0
 DCB_PRECISION_FP32 = 1
 # per-read outcome codes of dcb_stitch_fastq (the OutcomeCounter field the reference would bump)
@@ -110,7 +111,7 @@ ABI_SYMBOLS = (
     "dcb_prep_last_error", "dcb_prep_export_records", "dcb_prep_get_records", "dcb_prep_use_ccs_smart_windows",
     "dcb_prep_get_window_widths", "dcb_prep_get_overflow_ccs", "dcb_features_layout", "dcb_features_pack",
     "dcb_features_layout_smart", "dcb_features_ccs", "dcb_prep_get_window_lengths", "dcb_prep_open_truth",
-    "dcb_prep_get_label", "dcb_features_labels",
+    "dcb_prep_get_label", "dcb_features_labels", "dcb_features_eval",
     "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
     "dcb_last_forward_launches", "dcb_set_profile", "dcb_get_profile", "dcb_get_profile_kernels", "dcb_alloc_host",
     "dcb_free_host", "dcb_alloc_device", "dcb_free_device", "dcb_memcpy_h2d", "dcb_memcpy_d2h",
@@ -185,6 +186,8 @@ def _load(path: str) -> ctypes.CDLL:
                                             ctypes.POINTER(i32), ctypes.POINTER(ctypes.c_float)]
   lib.dcb_features_ccs.argtypes = [vp, vp, i32, vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_features_labels.argtypes = [vp, ctypes.POINTER(DcbLabels), vp, i32, vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_features_eval.argtypes = [vp, ctypes.POINTER(DcbLabels), vp, i32, i32, vp, vp, vp, vp, vp, vp, ctypes.POINTER(i32),
+                                    ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_launches.argtypes = [vp, ctypes.POINTER(i32)]
   lib.dcb_set_debug.argtypes = [vp, i32]
@@ -315,6 +318,7 @@ class B200Model:
     self.device = int(device)
     self.max_length = int(params.max_length)
     self.total_rows = params_lib.get_total_rows(params.max_passes, params.use_ccs_bq)
+    self._layout_windows = 0   # windows of the last successful features_layout
     cfg = make_config(params, max_batch, device, max_base_quality, calibration, chunk_tiles, precision)
     rc = self._lib.dcb_create(ctypes.byref(cfg), ctypes.byref(self._handle))
     if rc:
@@ -416,11 +420,12 @@ class B200Model:
       raise ValueError("packed rows must be uint8 [B, %d]" % self.packed_window_bytes)
     return self._forward_chunks(self._lib.dcb_forward_packed, packed, want_probs, want_logits, strict_input, strict)
 
-  def submit_packed_raw(self, packed_ptr: int, batch: int, flags: int, bases_ptr: int, quals_ptr: int) -> int:
+  def submit_packed_raw(self, packed_ptr: int, batch: int, flags: int, bases_ptr: int, quals_ptr: int,
+                        probs_ptr: int = 0, logits_ptr: int = 0) -> int:
     """dcb_submit_packed on caller-managed pointers; returns the ticket for wait_raw()."""
     ticket = ctypes.c_int64(-1)
     self._check(self._lib.dcb_submit_packed(self._handle, _ptr(packed_ptr), batch, flags, _ptr(bases_ptr),
-                                            _ptr(quals_ptr), None, None, ctypes.byref(ticket)))
+                                            _ptr(quals_ptr), _ptr(probs_ptr), _ptr(logits_ptr), ctypes.byref(ticket)))
     return int(ticket.value)
 
   # -- the hot path, pipelined over a stream of batches ----------------------------------------
@@ -676,6 +681,7 @@ class B200Model:
                                                 _ptr(out["num_passes"]), _ptr(out["ccs_ids"]), ctypes.byref(n), ctypes.byref(ms)))
     res: Dict[str, Any] = {k: (v if k == "zmw_windows" else v[:n.value]) for k, v in out.items()}
     res["ms"] = float(ms.value)
+    self._layout_windows = int(n.value)
     return res
 
   def features_pack(self, windows: np.ndarray, out: Optional[int] = None) -> Dict[str, Any]:
@@ -718,6 +724,31 @@ class B200Model:
     out["ms"] = float(ms.value)
     return out
 
+  def features_eval(self, labels: Dict[str, np.ndarray], keep_zmw: np.ndarray, capacity: int, packed_ptr: int,
+                    labels_ptr: int, ccs_ptr: int) -> Dict[str, Any]:
+    """dcb_features_eval: the evaluation inputs of the last features_layout's windows.  `labels` is `concat_labels` of
+    one label per ZMW of that batch, keep_zmw one flag per ZMW.  The kept windows (label status != 2, ZMW kept) go, in
+    window order, to the device arrays at packed_ptr (uint8 [capacity, packed_window_bytes], 16-byte aligned),
+    labels_ptr and ccs_ptr (uint8 [capacity, L] each).  Returns dict(k, status uint8 [n] of every window of the layout,
+    ccs_width int32 [n_zmw], windows int32 [k] (layout index of every kept window), ms).  DcbError(-1) when k exceeds
+    capacity."""
+    meta, cig, bases = (np.ascontiguousarray(labels[k], dt) for k, dt in (("label_meta", np.int32), ("cigar", np.uint32),
+                                                                         ("bases", np.uint8)))
+    lab = DcbLabels(n_zmw=meta.reshape(-1, LABEL_META).shape[0], n_cigar=cig.size, n_bases=bases.size,
+                    label_meta=_ptr(meta), cigar=_ptr(cig), bases=_ptr(bases))
+    keep = np.ascontiguousarray(keep_zmw, np.uint8).reshape(-1)
+    n = self._layout_windows
+    out = dict(status=np.zeros(n, np.uint8), ccs_width=np.zeros(lab.n_zmw, np.int32),
+               windows=np.zeros(max(int(capacity), 0), np.int32))
+    k, ms = ctypes.c_int32(0), ctypes.c_float(0)
+    self._check(self._lib.dcb_features_eval(self._handle, ctypes.byref(lab), _ptr(keep), len(keep), int(capacity),
+                                            _ptr(packed_ptr), _ptr(labels_ptr), _ptr(ccs_ptr), _ptr(out["status"]),
+                                            _ptr(out["ccs_width"]), _ptr(out["windows"]), ctypes.byref(k), ctypes.byref(ms)))
+    out["k"] = int(k.value)
+    out["windows"] = out["windows"][:out["k"]]
+    out["ms"] = float(ms.value)
+    return out
+
   def stitch_raw(self, bases_ptr: int, quals_ptr: int, n_windows: int, zmw_start: np.ndarray, flags: int,
                  seq_ptr: int, qual_ptr: int, len_ptr: int, length: Optional[int] = None) -> None:
     """dcb_stitch on caller-managed pointers (host or device per `flags`)."""
@@ -737,17 +768,23 @@ class B200Model:
 
   def evaluate_windows(self, probs, labels: np.ndarray, ccs_ids: np.ndarray, del_cost: Optional[float] = None,
                        loss_reg: Any = "params", band_width: Any = "params", on_device: bool = False,
-                       batch: Optional[int] = None) -> Dict[str, Any]:
+                       batch: Optional[int] = None, labels_on_device: bool = False) -> Dict[str, Any]:
     """dcb_evaluate: per-window AlignmentLoss, PerExampleAccuracy flag and AlignmentMetric counts of the prediction and
     of the CCS row.  probs float32 [B, L, 5] (host array, or a device address with on_device=True and `batch`);
-    labels / ccs_ids uint8 [B, L].  del_cost / loss_reg / band_width default to params.json's (loss_reg=None: hard
-    min; band_width set: DcbError -1).  Returns loss float32 [B], exact uint8 [B], pred_counts / ccs_counts int32
-    [B, 5] (columns EVAL_COUNT_KEYS) and ms, the device time of the evaluation kernels."""
-    labels = np.ascontiguousarray(labels, dtype=np.uint8)
-    ccs = np.ascontiguousarray(ccs_ids, dtype=np.uint8)
-    if labels.ndim != 2 or ccs.shape != labels.shape:
-      raise ValueError("labels and ccs_ids must both be uint8 [B, L]")
-    B, L = labels.shape
+    labels / ccs_ids uint8 [B, L] (host arrays, or with labels_on_device=True and `batch` device addresses of
+    [batch, max_length], e.g. features_eval's).  del_cost / loss_reg / band_width default to params.json's
+    (loss_reg=None: hard min; band_width set: DcbError -1).  Returns loss float32 [B], exact uint8 [B], pred_counts /
+    ccs_counts int32 [B, 5] (columns EVAL_COUNT_KEYS) and ms, the device time of the evaluation kernels."""
+    if labels_on_device:
+      if batch is None:
+        raise ValueError("evaluate_windows(labels_on_device=True) needs batch")
+      B, L = int(batch), self.max_length
+    else:
+      labels = np.ascontiguousarray(labels, dtype=np.uint8)
+      ccs_ids = np.ascontiguousarray(ccs_ids, dtype=np.uint8)
+      if labels.ndim != 2 or ccs_ids.shape != labels.shape:
+        raise ValueError("labels and ccs_ids must both be uint8 [B, L]")
+      B, L = labels.shape
     if on_device and (batch is None or int(batch) != B):
       raise ValueError("evaluate_windows(on_device=True) needs batch == labels.shape[0]")
     p_ptr, probs = _arg(probs, np.float32, on_device)
@@ -756,8 +793,9 @@ class B200Model:
     dc, reg, bw = self._eval_args(del_cost, loss_reg, band_width)
     out = _empty_eval(B)
     ms = ctypes.c_float()
-    self._check(self._lib.dcb_evaluate(self._handle, p_ptr, _ptr(labels), _ptr(ccs), B, L, dc, reg, bw,
-                                       DCB_ROWS_ON_DEVICE if on_device else 0, _ptr(out["loss"]), _ptr(out["exact"]),
+    flags = (DCB_ROWS_ON_DEVICE if on_device else 0) | (DCB_LABELS_ON_DEVICE if labels_on_device else 0)
+    self._check(self._lib.dcb_evaluate(self._handle, p_ptr, _ptr(labels), _ptr(ccs_ids), B, L, dc, reg, bw,
+                                       flags, _ptr(out["loss"]), _ptr(out["exact"]),
                                        _ptr(out["pred_counts"]), _ptr(out["ccs_counts"]), ctypes.byref(ms)))
     out["ms"] = float(ms.value)
     return out

@@ -3,6 +3,17 @@ training-mode tf.Examples in, `inference.csv` and `eval_metrics.json` out.
 
   python -m deepconsensus_b200.evaluate --checkpoint model_dir/checkpoint-50 --eval_path 'data/eval/*.tfrecord.gz' \\
          --out_dir OUT [--batch_size N --limit N --precision bf16|fp32 --random_weights SEED]
+  python -m deepconsensus_b200.evaluate --checkpoint model_dir/checkpoint-50 --subreads_to_ccs S.bam --ccs_bam C.bam \\
+         --truth_to_ccs T.bam --truth_bed B.bed --truth_split SPLIT.tsv --split eval [--split test] --out_dir OUT \\
+         [--ins_trim 5 --cpus N and the options above]
+
+The second form evaluates straight from BAMs: the labelled windows `preprocess` would write to the split's file are
+built on the GPU (dcb_features_layout, then dcb_features_eval, which keeps the split's windows and leaves their packed,
+label and CCS rows in device memory), scored there and measured there, with no tf.Example in between.  Window geometry
+(max_passes, max_length, use_ccs_bq) comes from the checkpoint's params.json; `--ins_trim` and `--cpus` mean what they
+mean in `preprocess`.  The dataset name of each split is the split itself, and its `eval_metrics.json` entry gains
+"examples": preprocess's counters of the ZMWs read.  The results equal `preprocess` followed by `--eval_path` on the
+split's file, window for window.
 
 The forward writes its probabilities to device memory (submit path, two batches in flight) and dcb_evaluate reads them
 there: AlignmentLoss, PerExampleAccuracy and the AlignmentMetric counts of the prediction and of the CCS row are
@@ -35,17 +46,19 @@ transformer_learn_values_distill config).  `inference.csv` and the other entries
 from __future__ import annotations
 
 import argparse
+import collections
 import contextlib
 import json
 import os
 import time
-from typing import Any, Dict, List, Optional, Sequence, Tuple
+from typing import Any, Dict, Iterable, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 
 from deepconsensus_b200 import engine as engine_lib
 from deepconsensus_b200 import inference
 from deepconsensus_b200 import params as params_lib
+from deepconsensus_b200 import preprocess
 from deepconsensus_b200 import tfrecord
 from deepconsensus_b200 import weights as weights_lib
 
@@ -132,18 +145,44 @@ def write_inference_csv(path: str, rows: Sequence[Tuple[str, float, float]]) -> 
     f.write("\n")
 
 
-def evaluate_rows(model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndarray, chunk: int,
-                  strict: Optional[bool] = None, teacher: Optional[engine_lib.B200Model] = None,
-                  temperature: float = 1.0, logit_loss: Any = "kl_divergence") -> Dict[str, Any]:
-  """Per-window evaluation of float32 rows [N, R, L]: per chunk of the rows the forward runs through dcb_submit from the
-  pipeline slot's pinned staging (device outputs, two chunks in flight) and dcb_evaluate reads its probabilities on the
-  device.  Returns evaluate_windows()'s arrays over all N windows and forward_ms / eval_ms, the summed device times.
+class HostRowsChunk:
+  """One chunk of host float32 rows (the tf.Example path): staged into the pipeline slot's pinned rows and submitted
+  with dcb_submit; dcb_evaluate gets its label and CCS rows as host arrays."""
+  packed, rows_flag, labels_on_device = False, 0, False
 
-  With the `teacher` of a distilled student, the teacher's forward runs from the same pinned rows, and once both are
-  done dcb_distill_loss_grad compares the two engines' logits on the device.  This adds distill_loss float32 [N] and
-  the teacher's forward and the distillation kernel's device times (teacher_forward_ms, distill_ms)."""
-  N, L = rows.shape[0], model.max_length
+  def __init__(self, model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndarray, ccs: np.ndarray):
+    self.model, self.rows, self.labels, self.ccs_ids = model, rows, labels, ccs
+    self.n = int(rows.shape[0])
+
+  def stage(self, slot: int) -> int:
+    staging = self.model.staging_rows(slot)
+    staging[:self.n] = self.rows
+    return staging.ctypes.data
+
+
+def host_row_chunks(model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndarray,
+                    chunk: int) -> Iterator[HostRowsChunk]:
+  """The chunk source of float32 rows [N, R, L] and uint8 labels [N, L] in host memory."""
   ccs = model.ccs_ids(rows)
+  for b0 in range(0, rows.shape[0], chunk):
+    b1 = min(rows.shape[0], b0 + chunk)
+    yield HostRowsChunk(model, rows[b0:b1], labels[b0:b1], ccs[b0:b1])
+
+
+def evaluate_chunks(model: engine_lib.B200Model, chunks: Iterable[Any], chunk: int, strict: Optional[bool] = None,
+                    teacher: Optional[engine_lib.B200Model] = None, temperature: float = 1.0,
+                    logit_loss: Any = "kl_divergence") -> Dict[str, Any]:
+  """Per-window evaluation of a chunk source: per chunk of at most `chunk` windows the forward runs through the submit
+  path (device outputs, two chunks in flight) and dcb_evaluate reads its probabilities on the device.  A chunk has `n`
+  windows and `stage(slot)`, which returns the address of its rows: pinned host float32 rows (packed False), or
+  device packed rows (packed True, rows_flag DCB_ROWS_ON_DEVICE); its `labels` / `ccs_ids` are host arrays, or device
+  addresses with labels_on_device.  Returns evaluate_windows()'s arrays over all windows and forward_ms / eval_ms, the
+  summed device times.
+
+  With the `teacher` of a distilled student, the teacher's forward runs from the same rows, and once both are done
+  dcb_distill_loss_grad compares the two engines' logits on the device.  This adds distill_loss float32 [N] and the
+  teacher's forward and the distillation kernel's device times (teacher_forward_ms, distill_ms)."""
+  L = model.max_length
   flag = engine_lib.DCB_OUT_ON_DEVICE | model._precision_flag(strict)
   engines = [model] if teacher is None else [model, teacher]
   out_bytes = chunk * L * 5 * 4
@@ -167,14 +206,14 @@ def evaluate_rows(model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndar
 
   def submit(item):
     """Both engines' forwards of one chunk; if the teacher's submit fails, the student's ticket is retired."""
-    slot, b0, b1 = item
-    staging = model.staging_rows(slot)
-    staging[:b1 - b0] = rows[b0:b1]
+    slot, c = item
+    ptr = c.stage(slot)
     handle = []
     try:
       for m, buf in zip(engines, bufs[slot]):
-        handle.append((m, m.submit_raw(staging.ctypes.data, b1 - b0, flag, buf["bq"], buf["bq"] + chunk * L,
-                                       probs_ptr=buf.get("probs", 0), logits_ptr=buf.get("logits", 0))))
+        fn = m.submit_packed_raw if c.packed else m.submit_raw
+        handle.append((m, fn(ptr, c.n, flag | c.rows_flag, buf["bq"], buf["bq"] + chunk * L,
+                             probs_ptr=buf.get("probs", 0), logits_ptr=buf.get("logits", 0))))
     except BaseException:
       retire(handle)
       raise
@@ -199,14 +238,15 @@ def evaluate_rows(model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndar
       slot[0]["probs"] = alloc(model, out_bytes)
       if teacher is not None:
         slot[0]["logits"], slot[1]["logits"] = alloc(model, out_bytes), alloc(teacher, out_bytes)
-    chunks = [(i % 2, b0, min(N, b0 + chunk)) for i, b0 in enumerate(range(0, N, chunk))]
-    with contextlib.closing(engine_lib.pipelined(chunks, submit, wait, retire)) as done:   # retired before the frees
-      for (slot, b0, b1), _ in done:
-        r = model.evaluate_windows(bufs[slot][0]["probs"], labels[b0:b1], ccs[b0:b1], on_device=True, batch=b1 - b0)
+    items = ((i % 2, c) for i, c in enumerate(chunks))
+    with contextlib.closing(engine_lib.pipelined(items, submit, wait, retire)) as done:   # retired before the frees
+      for (slot, c), _ in done:
+        r = model.evaluate_windows(bufs[slot][0]["probs"], c.labels, c.ccs_ids, on_device=True, batch=c.n,
+                                   labels_on_device=c.labels_on_device)
         times["eval_ms"] += r.pop("ms")
         if teacher is not None:
           d = model.distill_loss(bufs[slot][1]["logits"], bufs[slot][0]["logits"], temperature, logit_loss,
-                                 on_device=True, batch=b1 - b0, length=L)
+                                 on_device=True, batch=c.n, length=L)
           times["distill_ms"] += d["ms"]
           r["distill_loss"] = d["loss"]
         parts.append(r)
@@ -216,6 +256,122 @@ def evaluate_rows(model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndar
   out = engine_lib._concat_eval(parts, () if teacher is None else ("distill_loss",))
   out.update(times)
   return out
+
+
+def evaluate_rows(model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndarray, chunk: int,
+                  strict: Optional[bool] = None, teacher: Optional[engine_lib.B200Model] = None,
+                  temperature: float = 1.0, logit_loss: Any = "kl_divergence") -> Dict[str, Any]:
+  """evaluate_chunks() of float32 rows [N, R, L] and uint8 labels [N, L] in host memory: per chunk the rows go
+  through the pipeline slot's pinned staging and dcb_submit."""
+  return evaluate_chunks(model, host_row_chunks(model, rows, labels, chunk), chunk, strict, teacher, temperature,
+                         logit_loss)
+
+
+class DevicePackedChunk:
+  """One chunk of the BAM path: packed rows, label rows and CCS rows that dcb_features_eval left in device memory."""
+  packed, rows_flag, labels_on_device = True, engine_lib.DCB_ROWS_ON_DEVICE, True
+
+  def __init__(self, packed: int, labels: int, ccs: int, n: int):
+    self.packed_ptr, self.labels, self.ccs_ids, self.n = packed, labels, ccs, int(n)
+
+  def stage(self, slot: int) -> int:
+    return self.packed_ptr
+
+
+class BamWindows:
+  """The chunk source of the BAM path: the labelled windows of one split, built on the GPU from the subreads and CCS
+  BAMs and the truth alignment, in the order `preprocess` writes that split's file.
+
+  ZMWs are decoded (preprocess.BamFeatureStream with `cpus` worker threads), selected by preprocess.select_zmw and laid
+  out `batch_zmws` at a time (dcb_features_layout); dcb_features_eval then builds every window's label, keeps the
+  windows of the split's ZMWs whose label fits, and writes their packed, label and CCS rows to one of two device
+  buffer sets.  Chunks of at most `chunk` windows are slices of that set, so nothing goes through the host.  The sets
+  alternate between ZMW batches that keep a window: when a batch is laid out, every chunk of the batch before the
+  previous one has been waited for, on both engines.  `counter` receives preprocess's counters of every ZMW read;
+  `limit_windows` > 0 stops after that many windows."""
+
+  def __init__(self, model: engine_lib.B200Model, subreads_to_ccs: str, ccs_bam: str, truth_to_ccs: str,
+               bed: Dict[str, Dict[str, Any]], contig_split: Dict[str, str], split: str, chunk: int,
+               ins_trim: int = 5, cpus: int = 0, batch_zmws: int = 64, limit_windows: int = 0):
+    self.model, self.split, self.chunk, self.ins_trim = model, split, int(chunk), int(ins_trim)
+    self.bed, self.contig_split = bed, contig_split
+    self.batch_zmws, self.limit_windows = max(int(batch_zmws), 1), int(limit_windows)
+    self.paths = (subreads_to_ccs, ccs_bam, truth_to_ccs)
+    self.cpus = max(int(cpus), 0)
+    self.counter: collections.Counter = collections.Counter()
+    self.features_ms = 0.0
+    self.n_windows = 0
+    self._sets: List[Optional[Dict[str, int]]] = [None, None]
+
+  def _buffers(self, which: int, n: int) -> Dict[str, int]:
+    """Device buffer set `which` with room for n windows (grown, never shrunk)."""
+    cur = self._sets[which]
+    if cur is not None and cur["cap"] >= n:
+      return cur
+    self._free(which)
+    m, L, cap = self.model, self.model.max_length, max(n, self.chunk)
+    self._sets[which] = dict(cap=cap, packed=m.alloc_device(cap * m.packed_window_bytes), labels=m.alloc_device(cap * L),
+                             ccs=m.alloc_device(cap * L))
+    return self._sets[which]
+
+  def _free(self, which: int) -> None:
+    cur, self._sets[which] = self._sets[which], None
+    if cur is not None:
+      for k in ("packed", "labels", "ccs"):
+        self.model.free_device(cur[k])
+
+  def close(self) -> None:
+    for which in (0, 1):
+      self._free(which)
+
+  def _batch_chunks(self, batch: List[Tuple[Dict[str, Any], Dict[str, Any], str]], which: int):
+    """Lays out one ZMW batch into buffer set `which`; returns its chunks."""
+    m, L = self.model, self.model.max_length
+    zmws, labels, splits = zip(*batch)
+    lay = m.features_layout(engine_lib.concat_records(list(zmws)), self.ins_trim)
+    n = len(lay["window_pos"])
+    buf = self._buffers(which, n)
+    keep = np.array([s == self.split for s in splits], np.uint8)
+    r = m.features_eval(engine_lib.concat_labels(list(labels)), keep, buf["cap"], buf["packed"], buf["labels"],
+                        buf["ccs"])
+    self.features_ms += lay["ms"] + r["ms"]
+    w = 0
+    for z, s in enumerate(splits):
+      n_win = int(lay["zmw_windows"][z])
+      preprocess.count_zmw_windows(self.counter, L, n_win, int(r["ccs_width"][z]), r["status"][w:w + n_win], s)
+      w += n_win
+    k = r["k"]
+    if self.limit_windows:
+      k = min(k, self.limit_windows - self.n_windows)
+    self.n_windows += k
+    stride = m.packed_window_bytes
+    return [DevicePackedChunk(buf["packed"] + j0 * stride, buf["labels"] + j0 * L, buf["ccs"] + j0 * L,
+                              min(k, j0 + self.chunk) - j0) for j0 in range(0, k, self.chunk)]
+
+  def __iter__(self) -> Iterator[DevicePackedChunk]:
+    stream = preprocess.BamFeatureStream(self.paths[0], self.paths[1], self.model.params.max_passes,
+                                         self.model.max_length, bool(self.model.params.use_ccs_bq), self.ins_trim,
+                                         threads=self.cpus, records=True, truth_to_ccs=self.paths[2])
+    which, batch = 0, []
+    try:
+      while not (self.limit_windows and self.n_windows >= self.limit_windows):
+        z = stream.next_zmw_records()
+        if z is not None:
+          picked = preprocess.select_zmw(stream, z, self.ins_trim, self.counter, self.bed, self.contig_split)
+          if picked is not None:
+            batch.append((z,) + picked)
+          if len(batch) < self.batch_zmws:
+            continue
+        if batch:
+          chunks = self._batch_chunks(batch, which)
+          batch = []
+          if chunks:
+            which ^= 1
+          yield from chunks
+        if z is None:
+          break
+    finally:
+      stream.close()
 
 
 def _load_teacher(teacher_model_dir: str, options: inference.InferenceOptions, random_weights: Optional[int],
@@ -231,10 +387,52 @@ def _load_teacher(teacher_model_dir: str, options: inference.InferenceOptions, r
   return model
 
 
-def run(checkpoint: str, eval_path: Sequence[str], out_dir: str, limit: int = -1, batch_size: Optional[int] = None,
-        precision: str = "bf16", random_weights: Optional[int] = None, device: int = 0,
-        chunk: int = 1024, teacher_model_dir: Optional[str] = None,
-        teacher_random_weights: Optional[int] = None) -> Dict[str, Any]:
+def check_bam_source(eval_path: Optional[Sequence[str]], subreads_to_ccs: Optional[str], ccs_bam: Optional[str],
+                     truth_to_ccs: Optional[str], truth_bed: Optional[str], truth_split: Optional[str],
+                     split: Optional[Sequence[str]], use_ccs_smart_windows: bool = False) -> Optional[Dict[str, Any]]:
+  """Checks the input form before any decoding starts: tf.Example files (`eval_path`, returns None) or the BAM source
+  (returns dict(bed, contig_split)), never both.  The BAM source needs all five inputs and at least one --split, every
+  one a split truth_split gives some contig; smart windows are refused, as in training-mode preprocess."""
+  bam = dict(subreads_to_ccs=subreads_to_ccs, ccs_bam=ccs_bam, truth_to_ccs=truth_to_ccs, truth_bed=truth_bed,
+             truth_split=truth_split)
+  given = [k for k, v in bam.items() if v]
+  if eval_path and (given or split):
+    raise ValueError("--eval_path and the BAM inputs (%s) are exclusive: evaluate either tf.Examples or BAMs" %
+                     ", ".join("--" + k for k in given + (["split"] if split else [])))
+  if eval_path:
+    if use_ccs_smart_windows:
+      raise ValueError("--use_ccs_smart_windows applies to the BAM inputs only")
+    return None
+  if not given and not split:
+    raise ValueError("give either --eval_path or the BAM inputs (--subreads_to_ccs --ccs_bam --truth_to_ccs "
+                     "--truth_bed --truth_split --split)")
+  missing = [k for k in bam if not bam[k]]
+  if missing:
+    raise ValueError("the BAM inputs also need %s" % ", ".join("--" + k for k in missing))
+  if use_ccs_smart_windows:
+    raise ValueError("--use_ccs_smart_windows is not supported with the truth inputs (labelled windows are cut every "
+                     "max_length columns, as training-mode preprocess cuts them)")
+  if not split:
+    raise ValueError("the BAM inputs need at least one --split")
+  contig_split = preprocess.read_truth_split(truth_split)
+  produced = sorted(set(contig_split.values()))
+  for sp in split:
+    if sp not in produced:
+      raise ValueError("--split %s: %s assigns its contigs only to %s" % (sp, truth_split, ", ".join(produced) or "no split"))
+  return dict(bed=preprocess.read_truth_bed(truth_bed), contig_split=contig_split)
+
+
+def run(checkpoint: str, eval_path: Optional[Sequence[str]] = None, out_dir: str = ".", limit: int = -1,
+        batch_size: Optional[int] = None, precision: str = "bf16", random_weights: Optional[int] = None,
+        device: int = 0, chunk: int = 1024, teacher_model_dir: Optional[str] = None,
+        teacher_random_weights: Optional[int] = None, subreads_to_ccs: Optional[str] = None,
+        ccs_bam: Optional[str] = None, truth_to_ccs: Optional[str] = None, truth_bed: Optional[str] = None,
+        truth_split: Optional[str] = None, split: Optional[Sequence[str]] = None, ins_trim: int = 5, cpus: int = 0,
+        batch_zmws: int = 64, use_ccs_smart_windows: bool = False) -> Dict[str, Any]:
+  truth = check_bam_source(eval_path, subreads_to_ccs, ccs_bam, truth_to_ccs, truth_bed, truth_split, split,
+                           use_ccs_smart_windows)
+  if truth is not None and cpus == 1:
+    raise ValueError("Must set cpus to 0 or >=2 for parallel processing.")
   params = params_lib.read_params_from_json(checkpoint)
   if params.get("band_width") is not None:
     raise ValueError("params.band_width=%s: the banded alignment loss is not supported" % params.band_width)
@@ -266,23 +464,33 @@ def run(checkpoint: str, eval_path: Sequence[str], out_dir: str, limit: int = -1
       raise
   os.makedirs(out_dir, exist_ok=True)
   csv_rows, metrics = [], {}
+  kw = {} if teacher is None else dict(teacher=teacher, temperature=float(distill["temperature"]),
+                                       logit_loss=distill["logit_loss_identifier"])
   try:
-    for path in eval_path:
+    for path in (eval_path if truth is None else split):
       t0 = time.time()
-      d = tfrecord.read_examples(path, limit=-1 if limit < 0 else limit * bs)
-      rows, labels = d["rows"], d["labels"]
-      if rows.shape[0] and rows.shape[1:] != (model.total_rows, model.max_length):
-        raise ValueError("%s: windows of shape %s, the checkpoint's params expect [%d, %d]" %
-                         (path, rows.shape[1:], model.total_rows, model.max_length))
-      t1 = time.time()
-      if teacher is None:
-        per = evaluate_rows(model, rows, labels, chunk)
+      if truth is None:
+        d = tfrecord.read_examples(path, limit=-1 if limit < 0 else limit * bs)
+        rows, labels = d["rows"], d["labels"]
+        if rows.shape[0] and rows.shape[1:] != (model.total_rows, model.max_length):
+          raise ValueError("%s: windows of shape %s, the checkpoint's params expect [%d, %d]" %
+                           (path, rows.shape[1:], model.total_rows, model.max_length))
+        t1 = time.time()
+        per = evaluate_rows(model, rows, labels, chunk, **kw)
+        timing = dict(seconds_read=t1 - t0, seconds_model_and_eval=time.time() - t1)
       else:
-        per = evaluate_rows(model, rows, labels, chunk, teacher=teacher, temperature=float(distill["temperature"]),
-                            logit_loss=distill["logit_loss_identifier"])
+        source = BamWindows(model, subreads_to_ccs, ccs_bam, truth_to_ccs, truth["bed"], truth["contig_split"], path,
+                            chunk, ins_trim=ins_trim, cpus=cpus, batch_zmws=batch_zmws,
+                            limit_windows=0 if limit < 0 else limit * bs)
+        try:
+          per = evaluate_chunks(model, source, chunk, **kw)
+        finally:
+          source.close()
+        timing = dict(features_ms=source.features_ms, seconds=time.time() - t0)
       agg = aggregate(per["loss"], per["exact"], per["pred_counts"], per["ccs_counts"], bs)
-      agg.update(precision=precision, forward_ms=per["forward_ms"], eval_ms=per["eval_ms"],
-                 seconds_read=t1 - t0, seconds_model_and_eval=time.time() - t1)
+      agg.update(precision=precision, forward_ms=per["forward_ms"], eval_ms=per["eval_ms"], **timing)
+      if truth is not None:
+        agg["examples"] = dict(source.counter.items())
       if teacher is not None:
         dist = aggregate_distillation(per["loss"], per["distill_loss"], per["exact"], per["pred_counts"],
                                       per["ccs_counts"], bs, float(distill["student_alpha"]),
@@ -306,7 +514,19 @@ def run(checkpoint: str, eval_path: Sequence[str], out_dir: str, limit: int = -1
 def main(argv: Optional[List[str]] = None) -> None:
   ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
   ap.add_argument("--checkpoint", required=True)
-  ap.add_argument("--eval_path", required=True, nargs="+", help="glob(s) of labelled *.tfrecord.gz; one csv line each")
+  ap.add_argument("--eval_path", nargs="+", help="glob(s) of labelled *.tfrecord.gz; one csv line each")
+  bam = ap.add_argument_group("BAM inputs", "labelled windows built on the GPU, as training-mode preprocess builds them "
+                              "(exclusive with --eval_path)")
+  bam.add_argument("--subreads_to_ccs")
+  bam.add_argument("--ccs_bam")
+  bam.add_argument("--truth_to_ccs", help="truth alignment to the CCS reads, indexed (path + .bai)")
+  bam.add_argument("--truth_bed")
+  bam.add_argument("--truth_split")
+  bam.add_argument("--split", action="append", help="split to evaluate (train / eval / test); repeat for one csv line "
+                                                    "each")
+  bam.add_argument("--ins_trim", type=int, default=5)
+  bam.add_argument("--cpus", type=int, default=0, help="host threads that decode and validate the BAMs (0: none)")
+  bam.add_argument("--use_ccs_smart_windows", action="store_true", help="not supported: refused")
   ap.add_argument("--out_dir", required=True)
   ap.add_argument("--limit", type=int, default=-1, help="batches per dataset (-1: all)")
   ap.add_argument("--batch_size", type=int, default=None, help="windows per metric batch (default: params.batch_size)")
@@ -317,6 +537,13 @@ def main(argv: Optional[List[str]] = None) -> None:
                   help="checkpoint of the teacher of a distilled student: adds the distillation losses")
   ap.add_argument("--teacher_random_weights", type=int, default=None)
   a = ap.parse_args(argv)
+  try:
+    check_bam_source(a.eval_path, a.subreads_to_ccs, a.ccs_bam, a.truth_to_ccs, a.truth_bed, a.truth_split, a.split,
+                     a.use_ccs_smart_windows)
+  except ValueError as e:
+    ap.error(str(e))
+  if a.eval_path is None and a.cpus == 1:
+    ap.error("Must set cpus to 0 or >=2 for parallel processing.")
   m = run(**vars(a))
   print(json.dumps({p: {k: v for k, v in r.items() if not k.startswith("batch_identity")} for p, r in m.items()}))
 

@@ -318,6 +318,67 @@ def _zmw_bp_counts(z: Dict[str, Any], ins_trim: int, counter) -> None:
     counter["zmw_trimmed_insertions_bp"] += int(lens[trimmed].sum())
 
 
+def select_zmw(stream: BamFeatureStream, z: Dict[str, Any], ins_trim: int, counter,
+               bed: Optional[Dict[str, Dict[str, Any]]] = None,
+               contig_split: Optional[Dict[str, str]] = None) -> Optional[Tuple[Dict[str, Any], str]]:
+  """The ZMW-level decisions of `deepconsensus preprocess` (preprocess.py:274-331, pre_lib.py:1001-1014,237) for ZMW z,
+  just read from `stream` by next_zmw_records: counts it in `counter` and returns (label, split), or None when the ZMW
+  is skipped.  In training mode (`bed` and `contig_split` given) a ZMW without a bed range, without a label alignment,
+  with a supplementary label alignment or on a contig without a split is skipped, and one whose label's aligned bases
+  do not cover its bed range minus the soft clips raises PrepError (the reference's assertion); without them every ZMW
+  passes with an empty label and the split 'inference'."""
+  counter["n_zmw_processed"] += 1
+  _zmw_bp_counts(z, ins_trim, counter)
+  if bed is None:
+    label, split = _empty_label(), "inference"
+  else:
+    rng = bed.get(z["name"])
+    if rng is None:
+      counter["n_zmw_missing_truth_range"] += 1
+      return None
+    label = stream.label()
+    if label["status"] == "not_found":
+      counter["n_zmw_no_label_alignment"] += 1
+      return None
+    if label["status"] == "supplementary":
+      counter["n_zmw_truth_label_supp_alignment"] += 1
+      return None
+    split = contig_split.get(rng["contig"])
+    if not split:
+      counter["n_zmw_missing_contig_split"] += 1
+      return None
+    # put_spacing's assertion (pre_lib.py:237), reached only by ZMWs that have a split: the label's aligned bases
+    # cover the bed range minus the soft clips
+    if len(label["bases"]) != rng["end"] - rng["begin"] - sum(label["soft_clip"]):
+      raise PrepError("%s: the truth alignment has %d aligned bases, its bed range %d" % (
+          z["name"], len(label["bases"]), rng["end"] - rng["begin"] - sum(label["soft_clip"])))
+  counter["n_zmw_%s" % split] += 1
+  counter["n_zmw_pass"] += 1
+  return label, split
+
+
+def count_zmw_windows(counter, L: int, n_win: int, ccs_width: int, status: np.ndarray, split: str) -> np.ndarray:
+  """The window counters of one ZMW of `split` (iter_examples, pre_lib.py:652-697): its n_win windows with a CCS
+  position out of ceil(ccs_width / L), and their label statuses (0 kept, 1 gaps removed, 2 overflow; all 0 without
+  labels).  Returns the mask of the windows that become examples (status != 2)."""
+  total = -(-int(ccs_width) // L)
+  counter["example_width_bucket_%d" % L] += total
+  if total > n_win:
+    counter["n_examples_no_ccs_idx"] += total - n_win
+  status = np.asarray(status)
+  n_over, n_adj = int((status == 2).sum()), int((status == 1).sum())
+  written = n_win - n_over
+  if n_over:
+    counter["n_examples_label_overflow"] += n_over
+  if n_adj:
+    counter["n_examples_adjusted_label"] += n_adj
+  if written:
+    counter["n_examples_skip_large_windows_keep"] += written
+  counter["n_examples_%s" % split] += written
+  counter["n_examples"] += written
+  return status != 2
+
+
 def make_examples(subreads_to_ccs: str, ccs_bam: str, output: str, truth_to_ccs: Optional[str] = None,
                   truth_bed: Optional[str] = None, truth_split: Optional[str] = None, max_passes: int = 20,
                   max_length: int = 100, use_ccs_bq: bool = False, ins_trim: int = 5, limit: int = 0, cpus: int = 0,
@@ -371,58 +432,21 @@ def make_examples(subreads_to_ccs: str, ccs_bam: str, output: str, truth_to_ccs:
     w = 0
     for z, (zmw, s) in enumerate(zip(zmws, split_of)):
       n_win = int(lay["zmw_windows"][z])
-      total = -(-int(lab["ccs_width"][z]) // L)
-      counter["example_width_bucket_%d" % L] += total
-      if total > n_win:
-        counter["n_examples_no_ccs_idx"] += total - n_win
-      written = 0
-      for i in range(w, w + n_win):
-        st = int(lab["status"][i]) if training else 0
-        if st == 2:
-          counter["n_examples_label_overflow"] += 1
-          continue
-        if st == 1:
-          counter["n_examples_adjusted_label"] += 1
-        counter["n_examples_skip_large_windows_keep"] += 1
+      st = lab["status"][w:w + n_win] if training else np.zeros(n_win, np.uint8)
+      for i in np.nonzero(count_zmw_windows(counter, L, n_win, int(lab["ccs_width"][z]), st, s))[0] + w:
         writers[s].write(tfrecord.dc_example(rows[i], int(lay["num_passes"][i]), zmw["name"], int(lay["window_pos"][i]),
                                              lay["ccs_bq"][i], lab["labels"][i] if training else None))
-        written += 1
-      counter["n_examples_%s" % s] += written
-      counter["n_examples"] += written
       w += n_win
     batch.clear()
 
   batch = []
   try:
     while (z := stream.next_zmw_records()) is not None:
-      counter["n_zmw_processed"] += 1
-      _zmw_bp_counts(z, ins_trim, counter)
-      label = _empty_label()
-      if training:
-        rng = bed.get(z["name"])
-        if rng is None:
-          counter["n_zmw_missing_truth_range"] += 1
-          continue
-        label = stream.label()
-        if label["status"] == "not_found":
-          counter["n_zmw_no_label_alignment"] += 1
-          continue
-        if label["status"] == "supplementary":
-          counter["n_zmw_truth_label_supp_alignment"] += 1
-          continue
-        split = contig_split.get(rng["contig"])
-        if not split:
-          counter["n_zmw_missing_contig_split"] += 1
-          continue
-        # put_spacing's assertion (pre_lib.py:237), reached only by ZMWs that have a split: the label's aligned bases
-        # cover the bed range minus the soft clips
-        if len(label["bases"]) != rng["end"] - rng["begin"] - sum(label["soft_clip"]):
-          raise PrepError("%s: the truth alignment has %d aligned bases, its bed range %d" % (
-              z["name"], len(label["bases"]), rng["end"] - rng["begin"] - sum(label["soft_clip"])))
-      else:
-        split = "inference"
-      counter["n_zmw_%s" % split] += 1
-      counter["n_zmw_pass"] += 1
+      picked = select_zmw(stream, z, ins_trim, counter, bed, contig_split) if training else \
+          select_zmw(stream, z, ins_trim, counter)
+      if picked is None:
+        continue
+      label, split = picked
       batch.append((z, label, split))
       if len(batch) >= batch_zmws:
         flush(batch)

@@ -94,6 +94,7 @@ typedef struct dcb_tensor {
 #define DCB_OUT_ON_DEVICE 2u    /* output pointers are device pointers */
 #define DCB_STRICT_FP32 4u      /* this call runs in float32 (DCB_PRECISION_FP32) whatever dcb_config.precision says */
 #define DCB_FAST_BF16 8u        /* this call runs the bf16 tensor-core path whatever dcb_config.precision says */
+#define DCB_LABELS_ON_DEVICE 16u /* dcb_evaluate: `labels` and `ccs_ids` are device arrays (e.g. dcb_features_eval's) */
 
 /* Create an engine on cfg->device.  Replaces model construction in initialize_model
  * (quick_inference.py:515-526). */
@@ -254,7 +255,8 @@ int dcb_fill_skipped_ragged(dcb_engine* e, const uint8_t* ccs_ids, const int16_t
  * probs float32 [B, L, 5]: a host array, or with DCB_ROWS_ON_DEVICE a device array (e.g. the DCB_OUT_ON_DEVICE probs_out
  * of dcb_forward / dcb_forward_packed, so that the probabilities never leave the GPU).  labels / ccs_ids: host u8 [B, L],
  * ids 0..4 over ' ATCG' (labels outside 0..4 are DCB_ERR_INVALID; a CCS id outside 0..4 counts as a gap, as its
- * all-zero one-hot row decodes).  band_width >= 0 (the banded AlignmentLoss, params.band_width set) is DCB_ERR_INVALID;
+ * all-zero one-hot row decodes); with DCB_LABELS_ON_DEVICE both are device arrays, read in place, and the label check
+ * runs on the device (the kernels then see no label id above 4, and the call still returns DCB_ERR_INVALID).  band_width >= 0 (the banded AlignmentLoss, params.band_width set) is DCB_ERR_INVALID;
  * pass DCB_BAND_WIDTH_NONE.  Outputs are host arrays; ms_out (nullable) receives the device time of the evaluation
  * kernels.  Deterministic: repeated calls give identical bits. */
 #define DCB_BAND_WIDTH_NONE (-1)
@@ -495,6 +497,24 @@ typedef struct dcb_labels {
 } dcb_labels;
 int dcb_features_labels(dcb_engine* e, const dcb_labels* labels, const int32_t* windows, int32_t n, uint8_t* labels_out,
                         uint8_t* status_out, int32_t* ccs_width_out, float* ms_out);
+
+/* Evaluation inputs on the device, after dcb_features_layout on the same batch: the label rows and statuses of every
+ * window of the layout (dcb_features_labels' rows, from the same `labels`), then the kept windows -- label status != 2
+ * and keep_zmw[z] != 0 for their ZMW (host u8 [n_keep], n_keep the layout's ZMW count) -- compacted in ZMW and window
+ * order by a block scan (no atomics), and for each of them, in that order, written to caller-given device arrays:
+ *   packed_out [k, dcb_packed_window_bytes]  16-byte aligned, the packed rows dcb_forward_packed(..., DCB_ROWS_ON_DEVICE)
+ *                                            reads in place -- byte for byte dcb_features_pack's
+ *   labels_out u8 [k, L], ccs_out u8 [k, L]  label rows and CCS rows (the layout's ccs_ids), which dcb_evaluate reads in
+ *                                            place with DCB_LABELS_ON_DEVICE
+ * capacity is the room of these arrays in windows.  Host outputs: *k_out, k (written even when it exceeds capacity);
+ * status_out u8 [n] (nullable) the status of every window of the layout (0 kept, 1 adjusted, 2 overflow);
+ * ccs_width_out int32 [n_zmw] (nullable) as dcb_features_labels; windows_out int32 [capacity] (nullable) the layout
+ * index of every kept window.  DCB_ERR_INVALID for k > capacity (nothing beyond capacity is written), a keep mask of
+ * another length, and every label dcb_features_labels refuses; the engine and the layout stay usable.  ms_out
+ * (nullable): device time of the kernels.  Deterministic. */
+int dcb_features_eval(dcb_engine* e, const dcb_labels* labels, const uint8_t* keep_zmw, int32_t n_keep, int32_t capacity,
+                      uint8_t* packed_out, uint8_t* labels_out, uint8_t* ccs_out, uint8_t* status_out, int32_t* ccs_width_out,
+                      int32_t* windows_out, int32_t* k_out, float* ms_out);
 
 /* Device time of the last dcb_forward (milliseconds, CUDA events on the engine's stream). */
 int dcb_last_forward_ms(dcb_engine* e, float* ms);
