@@ -63,6 +63,11 @@ struct EmbedTable {
   int vocab, width, off;
 };
 
+// One layer's GEMM weights on a float32-activation path, in the form that path's GEMM reads.
+struct StrictMats {
+  DevBuf<float> wq, wk, wv, wo, w1, w2;
+};
+
 struct LayerDev {
   DevBuf<__nv_bfloat16> wqkv;   // 6 groups x split-bf16 [72][144][8]: q_h0, q_h1, k_h0, k_h1, v_h0, v_h1
   DevBuf<__nv_bfloat16> wo;     // split-bf16 [72][288][8]
@@ -71,10 +76,11 @@ struct LayerDev {
   DevBuf<float> b1;             // [ff] (both paths)
   DevBuf<float> b2;             // [288] (gain folded)
   DevBuf<float> ln_g[2], ln_b[2];   // [288] pre-norm gamma/beta of the attention / FFN sub-layer (both paths)
-  struct {   // strict-fp32 path (strict_kernels.cu): float32 in the reference's own shapes
-    DevBuf<float> wq, wk, wv, wo, w1, w2, b2;
+  struct : StrictMats {   // strict-fp32 path (strict_kernels.cu): float32 in the reference's own shapes
+    DevBuf<float> b2;
     float alpha[2] = {1.f, 1.f};
   } strict;
+  StrictMats tf32x3;      // tf32x3 path (tf32x3_kernels.cu): the same matrices as tf32x3_image (that precision only)
 };
 
 // The device copy of one checkpoint.  dcb_load_weights builds a complete new set before it frees the previous one.
@@ -92,6 +98,7 @@ struct Weights {
     DevBuf<StrictEmbedRow> embed;
     DevBuf<float> tables, wc, pe;   // pe: [L][280]
   } strict;
+  DevBuf<float> tf32x3_wc;          // the condenser as tf32x3_image (DCB_PRECISION_TF32X3 engines only)
 };
 
 // Kernel classes of the forward's profile, in dcb_get_profile_kernels' order; kProfNone: counted, never timed.
@@ -405,7 +412,7 @@ int read_checkpoint(dcb_engine* e, const dcb_tensor* tensors, int n, Checkpoint*
   return rc;
 }
 
-// Both paths' device weights from a validated checkpoint.
+// Every path's device weights from a validated checkpoint (the tf32x3 images only for engines of that precision).
 int upload_weights(dcb_engine* e, const Checkpoint& ck, Weights* w) {
   const dcb_config& c = e->cfg;
   int rc = DCB_OK;   // the first failure: later uploads are skipped
@@ -442,6 +449,7 @@ int upload_weights(dcb_engine* e, const Checkpoint& ck, Weights* w) {
     auto img = pack_b_split(e->Epad, kDP, [&](int k, int nn) { return (k < E && nn < kD) ? ck.wc[(size_t)k * kD + nn] : 0.f; });
     up(w->wc, img);
     copy(w->strict.wc, ck.wc, (size_t)E * kD);
+    if (c.precision == DCB_PRECISION_TF32X3) up(w->tf32x3_wc, tf32x3_image(ck.wc, E, kD));
   }
   // ---- positional encoding table [Lw][288] (tf-models RelativePositionEmbedding; networks.py:301-323)
   {
@@ -533,6 +541,15 @@ int upload_weights(dcb_engine* e, const Checkpoint& ck, Weights* w) {
     copy(ld.strict.w1, l.w1, (size_t)kD * ff);
     copy(ld.strict.w2, l.w2, (size_t)ff * kD);
     copy(ld.strict.b2, l.b2, kD);
+    if (c.precision == DCB_PRECISION_TF32X3) {
+      StrictMats& m = ld.tf32x3;
+      up(m.wq, tf32x3_image(l.wq, kD, kD));
+      up(m.wk, tf32x3_image(l.wk, kD, kD));
+      up(m.wv, tf32x3_image(l.wv, kD, kD));
+      up(m.wo, tf32x3_image(l.wo, kD, kD));
+      up(m.w1, tf32x3_image(l.w1, kD, ff));
+      up(m.w2, tf32x3_image(l.w2, ff, kD));
+    }
   }
   // ---- head
   up(w->fln_g, pad288(ck.fln_g));
@@ -609,10 +626,18 @@ HeadParams chunk_head(const dcb_engine* e, uint8_t* bases, uint8_t* quals, float
   return hp;
 }
 
-// One chunk of the strict-fp32 forward (strict_kernels.cu): rows [bw, R, L] -> outputs via hp.  Its launches are
-// counted, not profiled.
+// The one thing the strict-fp32 and tf32x3 forwards do differently: the GEMM, and the form of the weights it reads.
+struct StrictGemm {
+  void (*launch)(const float* A, const float* B, float* C, int M, int N, int K, const StrictEpi& ep, cudaStream_t st);
+  bool tf32x3;   // B is a tf32x3_image (LayerDev::tf32x3, Weights::tf32x3_wc), not a float32 [K][N] matrix
+};
+const StrictGemm kStrictGemm{launch_strict_gemm, false};
+const StrictGemm kTf32x3Gemm{launch_tf32x3_gemm, true};
+
+// One chunk of the strict-fp32 or tf32x3 forward (strict_kernels.cu, with the GEMM of `gemm`): rows [bw, R, L] ->
+// outputs via hp.  Its launches are counted, not profiled.
 void strict_forward_chunk(dcb_engine* e, LaunchRecorder& rec, const float* rows_chunk, int bw, HeadParams hp,
-                          int* d_status) {
+                          int* d_status, const StrictGemm& gemm) {
   const dcb_config& c = e->cfg;
   dcb_engine::Strict& S = e->strict;
   const Weights& W = e->w;
@@ -622,26 +647,27 @@ void strict_forward_chunk(dcb_engine* e, LaunchRecorder& rec, const float* rows_
     launch_strict_embed(rows_chunk, e->R, L, e->E, bw, W.strict.embed, W.strict.tables, S.emb, d_status, st);
     StrictEpi ep;
     if (c.add_pos_encoding) { ep.pe = W.strict.pe; ep.pe_L = L; }
-    launch_strict_gemm(S.emb, W.strict.wc, S.x, M, kD, e->E, ep, st);                 // networks.py:509-516, :319-323
+    gemm.launch(S.emb, gemm.tf32x3 ? W.tf32x3_wc.p : W.strict.wc.p, S.x, M, kD, e->E, ep, st);   // networks.py:509-516, :319-323
   });
   const float qscale = 1.0f / sqrtf((float)kDH);                                       // attention_layer.py:196-197
   for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
     const LayerDev& ld = W.layers[n_];
+    const StrictMats& wm = gemm.tf32x3 ? ld.tf32x3 : static_cast<const StrictMats&>(ld.strict);
     const float* yin = c.rezero ? S.x.p : S.y.p;   // each sub-layer's input: x, or LayerNorm(x) in y
     rec.run(kProfNone, c.rezero ? 7 : 9, [&] {
       if (!c.rezero) launch_strict_layernorm(S.x, S.y, M, ld.ln_g[0], ld.ln_b[0], st);
       StrictEpi eq; eq.scale = qscale;
-      launch_strict_gemm(yin, ld.strict.wq, S.q, M, kD, kD, eq, st);
-      launch_strict_gemm(yin, ld.strict.wk, S.k, M, kD, kD, StrictEpi(), st);
-      launch_strict_gemm(yin, ld.strict.wv, S.v, M, kD, kD, StrictEpi(), st);
+      gemm.launch(yin, wm.wq, S.q, M, kD, kD, eq, st);
+      gemm.launch(yin, wm.wk, S.k, M, kD, kD, StrictEpi(), st);
+      gemm.launch(yin, wm.wv, S.v, M, kD, kD, StrictEpi(), st);
       launch_strict_attention(S.q, S.k, S.v, S.att, bw, L, c.attn_win_size, st);
       StrictEpi eo; eo.residual = S.x; eo.scale = c.rezero ? ld.strict.alpha[0] : 1.f;     // encoder_stack.py:88-92
-      launch_strict_gemm(S.att, ld.strict.wo, S.x, M, kD, kD, eo, st);
+      gemm.launch(S.att, wm.wo, S.x, M, kD, kD, eo, st);
       if (!c.rezero) launch_strict_layernorm(S.x, S.y, M, ld.ln_g[1], ld.ln_b[1], st);
       StrictEpi e1; e1.bias = ld.b1; e1.relu = 1;                                      // ffn_layer.py:83-86
-      launch_strict_gemm(yin, ld.strict.w1, S.hid, M, ff, kD, e1, st);
+      gemm.launch(yin, wm.w1, S.hid, M, ff, kD, e1, st);
       StrictEpi e2; e2.bias = ld.strict.b2; e2.residual = S.x; e2.scale = c.rezero ? ld.strict.alpha[1] : 1.f;
-      launch_strict_gemm(S.hid, ld.strict.w2, S.x, M, kD, ff, e2, st);
+      gemm.launch(S.hid, wm.w2, S.x, M, kD, ff, e2, st);
     });
   }
   hp.x = S.x; hp.M = M; hp.L = L; hp.Lw = L;
@@ -826,8 +852,8 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
   if (cfg->max_passes <= 0 || cfg->max_length <= 0 || cfg->max_length > 256 || cfg->num_hidden_layers <= 0 ||
       cfg->max_batch <= 0)
     return fail(nullptr, DCB_ERR_INVALID, "bad max_passes/max_length(<=256)/num_hidden_layers/max_batch");
-  if (cfg->precision != DCB_PRECISION_BF16 && cfg->precision != DCB_PRECISION_FP32)
-    return fail(nullptr, DCB_ERR_INVALID, "precision must be DCB_PRECISION_BF16 or DCB_PRECISION_FP32");
+  if (cfg->precision != DCB_PRECISION_BF16 && cfg->precision != DCB_PRECISION_FP32 && cfg->precision != DCB_PRECISION_TF32X3)
+    return fail(nullptr, DCB_ERR_INVALID, "precision must be DCB_PRECISION_BF16, DCB_PRECISION_FP32 or DCB_PRECISION_TF32X3");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail(nullptr, DCB_ERR_CUDA, "no CUDA device available (the dcb200 engine has no CPU fallback)");
@@ -906,6 +932,7 @@ int dcb_create(const dcb_config* cfg, dcb_engine** out) {
     CU(e, cudaEventCreate(&e->ev_eval0));
     CU(e, cudaEventCreate(&e->ev_eval1));
     CU(e, kernels_init());
+    CU(e, tf32x3_init());
     std::vector<double> p10(256);
     for (int q = 0; q < 256; ++q) p10[q] = pow(10.0, (double)q / -10.0);    // utils.py:103: 10 ** (q / -10.0)
     int rc = upload(e, e->d_p10, p10);
@@ -997,9 +1024,11 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
   const bool out_dev = flags & DCB_OUT_ON_DEVICE;
   if ((flags & DCB_STRICT_FP32) && (flags & DCB_FAST_BF16)) return fail(e, DCB_ERR_INVALID, "DCB_STRICT_FP32 and DCB_FAST_BF16 are exclusive");
   const bool strict = (flags & DCB_STRICT_FP32) || (c.precision == DCB_PRECISION_FP32 && !(flags & DCB_FAST_BF16));
+  const bool tf32x3 = c.precision == DCB_PRECISION_TF32X3 && !(flags & (DCB_STRICT_FP32 | DCB_FAST_BF16));
+  const bool f32 = strict || tf32x3;   // the strict path's forward: float32 rows and activations
   if (rows_dev && ((reinterpret_cast<uintptr_t>(rows) | reinterpret_cast<uintptr_t>(packed)) & 15))
     return fail(e, DCB_ERR_INVALID, "device-resident rows must be 16-byte aligned");
-  if (strict && !e->strict.chunk_windows) {
+  if (f32 && !e->strict.chunk_windows) {
     // workspace of the strict path, on first use: ~16 k tokens per chunk
     dcb_engine::Strict& S = e->strict;
     const int cw = std::max(1, std::min(c.max_batch, 16384 / L));
@@ -1027,7 +1056,7 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
   LaunchRecorder rec{e, sl, st};
   const uint8_t* packed_base = packed ? (rows_dev ? packed : sl.d_packed) : nullptr;
   // the default path's embedding kernel reads packed rows directly; the strict path gets the float32 rows they stand for
-  if (packed_base && strict) rec.run(kProfNone, 1, [&] { launch_unpack_rows(packed_base, e->pl, batch, sl.d_rows, st); });
+  if (packed_base && f32) rec.run(kProfNone, 1, [&] { launch_unpack_rows(packed_base, e->pl, batch, sl.d_rows, st); });
   const float* rows_base = packed ? sl.d_rows : (rows_dev ? rows : sl.d_rows);
   CU(e, cudaMemsetAsync(sl.d_status, 0, sizeof(int), st));
   CU(e, cudaEventRecord(sl.ev0, st));
@@ -1035,12 +1064,12 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
   uint8_t* quals = out_dev ? quals_out : sl.d_quals.p;
   float* probs = probs_out ? (out_dev ? probs_out : sl.d_probs.p) : nullptr;
   float* logits = logits_out ? (out_dev ? logits_out : sl.d_logits.p) : nullptr;
-  const int chunk_windows = strict ? e->strict.chunk_windows : e->chunk_windows;
+  const int chunk_windows = f32 ? e->strict.chunk_windows : e->chunk_windows;
   for (int w0 = 0; w0 < batch; w0 += chunk_windows) {
     const int bw = std::min(chunk_windows, batch - w0);
     const HeadParams hp = chunk_head(e, bases, quals, probs, logits, w0);
     const float* rows_chunk = rows_base + (size_t)w0 * R * L;
-    if (strict) strict_forward_chunk(e, rec, rows_chunk, bw, hp, sl.d_status);
+    if (f32) strict_forward_chunk(e, rec, rows_chunk, bw, hp, sl.d_status, strict ? kStrictGemm : kTf32x3Gemm);
     else if (packed_base) bf16_forward_chunk(e, rec, nullptr, packed_base + (size_t)w0 * e->pl.stride, bw, hp, sl.d_status);
     else bf16_forward_chunk(e, rec, rows_chunk, nullptr, bw, hp, sl.d_status);
   }

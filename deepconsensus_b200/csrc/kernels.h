@@ -2,6 +2,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <vector>
+
 #include "common.h"
 
 namespace dcb {
@@ -171,5 +173,13 @@ void launch_strict_layernorm(const float* x, float* y, int M, const float* g, co
 void launch_strict_attention(const float* q, const float* k, const float* v, float* o, int nwindows, int L, int win,
                              cudaStream_t st);
 void launch_strict_head(const float* x, int M, const HeadParams& hp, cudaStream_t st);
+
+// ---- tf32x3 path (tf32x3_kernels.cu): the strict path's GEMM on the tensor cores, same arguments and epilogue, with
+// W [K][N] (row-major float32) given as its tf32x3_image
+cudaError_t tf32x3_init();
+size_t tf32x3_image_elems(int K, int N);
+std::vector<float> tf32x3_image(const float* W, int K, int N);
+void launch_tf32x3_gemm(const float* A, const float* Wimg, float* C, int M, int N, int K, const StrictEpi& ep,
+                        cudaStream_t st);
 
 }  // namespace dcb

@@ -35,6 +35,9 @@ DCB_FAST_BF16 = 8
 DCB_LABELS_ON_DEVICE = 16
 DCB_PRECISION_BF16 = 0
 DCB_PRECISION_FP32 = 1
+DCB_PRECISION_TF32X3 = 2
+# precision name -> dcb_config.precision
+PRECISIONS = {"bf16": DCB_PRECISION_BF16, "fp32": DCB_PRECISION_FP32, "tf32x3": DCB_PRECISION_TF32X3}
 # per-read outcome codes of dcb_stitch_fastq (the OutcomeCounter field the reference would bump)
 DCB_READ_OK, DCB_READ_EMPTY, DCB_READ_ONLY_GAPS, DCB_READ_LOW_QUALITY, DCB_READ_TOO_SHORT = 0, 1, 2, 3, 4
 DCB_READ_BORDERLINE = 0x80
@@ -218,8 +221,9 @@ def make_config(params: params_lib.Params, max_batch: int, device: int = 0,
                 calibration: Optional[calibration_lib.QualityCalibrationValues] = None,
                 chunk_tiles: int = 0, precision: str = "bf16") -> DcbConfig:
   """params (params.json surface) + InferenceOptions fields -> dcb_config."""
-  if precision not in ("bf16", "fp32"):
-    raise ValueError("precision must be 'bf16' (tensor cores) or 'fp32' (strict, the reference's arithmetic)")
+  if precision not in PRECISIONS:
+    raise ValueError("precision must be 'bf16' (tensor cores), 'fp32' (strict, the reference's arithmetic) or "
+                     "'tf32x3' (the strict forward with its GEMMs on the tensor cores), got %r" % (precision,))
   c = DcbConfig()
   c.struct_size = ctypes.sizeof(DcbConfig)
   c.device = device
@@ -242,7 +246,7 @@ def make_config(params: params_lib.Params, max_batch: int, device: int = 0,
     c.calibration_w, c.calibration_b = float(calibration.w), float(calibration.b)
   c.max_batch = int(max_batch)
   c.chunk_tiles = int(chunk_tiles)
-  c.precision = DCB_PRECISION_FP32 if precision == "fp32" else DCB_PRECISION_BF16
+  c.precision = PRECISIONS[precision]
   for need in ("use_bases", "use_pw", "use_ip", "use_strand", "use_ccs", "use_sn"):
     if not params.get(need, True):
       raise DcbError(-1, "params.%s=False is not supported by the dcb200 engine" % need)
@@ -309,8 +313,10 @@ class B200Model:
                calibration: Optional[calibration_lib.QualityCalibrationValues] = None,
                chunk_tiles: int = 0, precision: str = "bf16", library: Optional[ctypes.CDLL] = None):
     """precision: "bf16" = tensor-core path (default); "fp32" = strict path, the reference's float32 arithmetic
-    (identical bases wherever the float32 top-2 logit margin exceeds 1e-3; ~25x slower).  Either can be overridden
-    per call with forward(..., strict=True/False)."""
+    (identical bases wherever the float32 top-2 logit margin exceeds 1e-3; ~25x slower); "tf32x3" = the strict
+    path's forward with its GEMMs on the tensor cores, each float32 operand split into two tf32 parts (the same
+    accuracy gates as "fp32").  Any of them can be overridden per call with forward(..., strict=True/False), which
+    selects the "fp32" / "bf16" path."""
     self._lib = library if library is not None else load_library()
     self._handle = ctypes.c_void_p()
     self.params = params

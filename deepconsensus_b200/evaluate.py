@@ -2,7 +2,7 @@
 training-mode tf.Examples in, `inference.csv` and `eval_metrics.json` out.
 
   python -m deepconsensus_b200.evaluate --checkpoint model_dir/checkpoint-50 --eval_path 'data/eval/*.tfrecord.gz' \\
-         --out_dir OUT [--batch_size N --limit N --precision bf16|fp32 --random_weights SEED]
+         --out_dir OUT [--batch_size N --limit N --precision bf16|fp32|tf32x3 --random_weights SEED]
   python -m deepconsensus_b200.evaluate --checkpoint model_dir/checkpoint-50 --subreads_to_ccs S.bam --ccs_bam C.bam \\
          --truth_to_ccs T.bam --truth_bed B.bed --truth_split SPLIT.tsv --split eval [--split test] --out_dir OUT \\
          [--ins_trim 5 --cpus N and the options above]
@@ -530,7 +530,7 @@ def main(argv: Optional[List[str]] = None) -> None:
   ap.add_argument("--out_dir", required=True)
   ap.add_argument("--limit", type=int, default=-1, help="batches per dataset (-1: all)")
   ap.add_argument("--batch_size", type=int, default=None, help="windows per metric batch (default: params.batch_size)")
-  ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
+  ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32", "tf32x3"])
   ap.add_argument("--random_weights", type=int, default=None)
   ap.add_argument("--device", type=int, default=0)
   ap.add_argument("--teacher_model_dir", default=None,

@@ -122,7 +122,7 @@ def main(argv: Optional[List[str]] = None) -> None:
   ap.add_argument("--ccs_calibration", default="skip")
   ap.add_argument("--limit", type=int, default=0)
   ap.add_argument("--random_weights", type=int, default=None)
-  ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
+  ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32", "tf32x3"])
   ap.add_argument("--cpus", type=int, default=0, help="native feature-construction threads (0: on the calling thread)")
   ap.add_argument("--features", default="host", choices=["host", "gpu"],
                   help="where windows are built from the decoded BAM records: host C++, or CUDA kernels that lay rows out "

@@ -65,8 +65,8 @@ typedef struct dcb_config {
   /* engine sizing */
   int32_t max_batch;          /* largest B a single dcb_forward call will see */
   int32_t chunk_tiles;        /* 128-token tiles processed per pass through the layer stack; 0 = auto */
-  int32_t precision;          /* DCB_PRECISION_BF16 (default) or DCB_PRECISION_FP32: which arithmetic dcb_forward uses
-                                 when the call does not say (see DCB_STRICT_FP32) */
+  int32_t precision;          /* DCB_PRECISION_BF16 (default), DCB_PRECISION_FP32 or DCB_PRECISION_TF32X3: which
+                                 arithmetic dcb_forward uses when the call does not say (see DCB_STRICT_FP32) */
   int32_t reserved[5];
 } dcb_config;
 
@@ -76,9 +76,15 @@ typedef struct dcb_config {
  *                       random-weight models), so the argmax can flip at near-ties.
  *   DCB_PRECISION_FP32  the reference's own arithmetic (float32 operands and accumulation, networks.py:506-507):
  *                       differs from the reference by summation order only (~1e-5 on logits); identical bases wherever
- *                       the float32 top-2 logit margin exceeds 1e-3.  CUDA-core kernels, ~25x slower. */
+ *                       the float32 top-2 logit margin exceeds 1e-3.  CUDA-core kernels, ~25x slower.
+ *   DCB_PRECISION_TF32X3 the DCB_PRECISION_FP32 forward with its GEMMs on the tensor cores: every float32 operand is
+ *                       split into two tf32 parts and three products are accumulated in float32 (3xTF32), which loses
+ *                       ~2^-22 relative per operand.  The same accuracy gates as DCB_PRECISION_FP32; its split weight
+ *                       images are built only for engines created with this precision.  DCB_STRICT_FP32 and
+ *                       DCB_FAST_BF16 still select those paths per call. */
 #define DCB_PRECISION_BF16 0
 #define DCB_PRECISION_FP32 1
+#define DCB_PRECISION_TF32X3 2
 
 /* A named host tensor in the reference checkpoint's layout, e.g.
  * "model/encoder_stack/layers/0/0/layer/query_dense_layer/kernel" float32 [280,2,140]. */
