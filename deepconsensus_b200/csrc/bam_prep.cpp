@@ -16,6 +16,7 @@
 // Pinned against the reference's own fixture: the windows built here from testdata/human_1m/{subreads_to_ccs,ccs}.bam
 // equal, value for value, the 1 593 examples of testdata/human_1m/tf_examples/inference/inference.tfrecord.gz that the
 // reference's preprocess wrote from the same BAMs (tests/test_bam_prep.py).
+#include <ctype.h>
 #include <math.h>
 #include <stdarg.h>
 #include <stdint.h>
@@ -207,15 +208,31 @@ struct BamReader {
     }
     return DCB_OK;
   }
+  // Appends the next record's bytes (those after its block_size) to *b, after the size checks every record gets:
   // 1 = record, 0 = EOF, < 0 = error
-  int next(BamRecord* r) {
+  int next_raw(std::vector<uint8_t>* b) {
     int32_t bs;
     const int rc = z.read(&bs, 4);
     if (rc == 0) return 0;
     if (rc < 0 || bs < 32) return pfail(DCB_ERR_INVALID, "truncated BAM record");
     if (bs > (64 << 20)) return pfail(DCB_ERR_INVALID, "implausible BAM record size %d", bs);
-    std::vector<uint8_t> b(bs);
-    if (z.read(b.data(), bs) != 1) return pfail(DCB_ERR_INVALID, "truncated BAM record");
+    const size_t at = b->size();
+    b->resize(at + bs);
+    if (z.read(b->data() + at, bs) != 1) return pfail(DCB_ERR_INVALID, "truncated BAM record");
+    int32_t l_seq;
+    uint16_t n_cig;
+    memcpy(&n_cig, b->data() + at + 12, 2);
+    memcpy(&l_seq, b->data() + at + 16, 4);
+    if (l_seq < 0 || 32ull + (*b)[at + 8] + 4ull * n_cig + (l_seq + 1) / 2 + l_seq > (size_t)bs)
+      return pfail(DCB_ERR_INVALID, "corrupt BAM record");
+    return 1;
+  }
+  // 1 = record, 0 = EOF, < 0 = error
+  int next(BamRecord* r) {
+    std::vector<uint8_t> b;
+    const int rc = next_raw(&b);
+    if (rc <= 0) return rc;
+    const int32_t bs = (int32_t)b.size();
     int32_t l_seq;
     uint16_t n_cig;
     memcpy(&r->refid, &b[0], 4);
@@ -224,9 +241,7 @@ struct BamReader {
     memcpy(&n_cig, &b[12], 2);
     memcpy(&r->flag, &b[14], 2);
     memcpy(&l_seq, &b[16], 4);
-    if (l_seq < 0) return pfail(DCB_ERR_INVALID, "corrupt BAM record");
     size_t o = 32;
-    if (o + l_name + 4ull * n_cig + (l_seq + 1) / 2 + l_seq > (size_t)bs) return pfail(DCB_ERR_INVALID, "corrupt BAM record");
     r->qname.assign(reinterpret_cast<const char*>(&b[o]), l_name ? l_name - 1 : 0);
     o += l_name;
     r->cigar.resize(n_cig);
@@ -238,7 +253,7 @@ struct BamReader {
     o += (l_seq + 1) / 2;
     r->qual.assign(b.begin() + o, b.begin() + o + l_seq);
     o += l_seq;
-    r->aux.assign(b.begin() + o, b.end());
+    r->aux.assign(b.begin() + o, b.begin() + bs);
     return 1;
   }
 };
@@ -534,9 +549,11 @@ struct ZmwJob {
   BamRecord label;
 };
 
-// The part of a BAM index (.bai, SAM/BAM spec v1.6 section 5.2) a whole-reference fetch needs: per reference, the
-// smallest virtual offset any of its bins' chunks starts at (UINT64_MAX: the reference has no records).
-int read_bai(const std::string& path, size_t n_ref, std::vector<uint64_t>* first) {
+// The part of a BAM index (.bai, SAM/BAM spec v1.6 section 5.2) a fetch needs: per reference, the smallest virtual
+// offset any of its bins' chunks starts at (UINT64_MAX: the reference has no records) and, when `linear` is given, the
+// linear index: per 16 kb window, the smallest virtual offset of a record that overlaps it (0: none recorded).
+int read_bai(const std::string& path, size_t n_ref, std::vector<uint64_t>* first,
+             std::vector<std::vector<uint64_t>>* linear = nullptr) {
   FILE* f = fopen(path.c_str(), "rb");
   if (!f) return pfail(DCB_ERR_INVALID, "cannot open the index %s (the truth alignment must be indexed)", path.c_str());
   std::vector<uint8_t> d;
@@ -554,6 +571,7 @@ int read_bai(const std::string& path, size_t n_ref, std::vector<uint64_t>* first
   if (bad || memcmp(magic, "BAI\1", 4) || nr < 0 || (size_t)nr != n_ref)
     return pfail(DCB_ERR_INVALID, "%s: not a BAM index for this BAM", path.c_str());
   first->assign(n_ref, UINT64_MAX);
+  if (linear) linear->clear();
   for (int32_t r = 0; r < nr && !bad; ++r) {
     int32_t n_bin = 0;
     get(&n_bin, 4);
@@ -572,7 +590,10 @@ int read_bai(const std::string& path, size_t n_ref, std::vector<uint64_t>* first
     }
     int32_t n_intv = 0;
     get(&n_intv, 4);
-    if (n_intv < 0 || o + 8ull * n_intv > d.size()) bad = true; else o += 8ull * n_intv;
+    if (n_intv < 0 || o + 8ull * n_intv > d.size()) { bad = true; break; }
+    if (linear) linear->emplace_back((size_t)n_intv);
+    if (linear && n_intv) memcpy(linear->back().data(), &d[o], 8ull * n_intv);
+    o += 8ull * n_intv;
   }
   if (bad) return pfail(DCB_ERR_INVALID, "%s: truncated BAM index", path.c_str());
   return DCB_OK;
@@ -1324,6 +1345,334 @@ int dcb_bamw_close(dcb_bamw* w) {
   const bool bad = w->failed || fclose(w->f) != 0;
   delete w;
   return bad ? pfail(DCB_ERR_INVALID, "closing the BAM failed") : DCB_OK;
+}
+
+}  // extern "C"
+
+// ----------------------------------------------------------------------------------------------- calibration reader
+// The host side of `calculate_baseq_calibration` (include/dcb200.h "base-quality calibration"): the reads an indexed,
+// coordinate-sorted BAM holds over a reference span, filtered as get_quality_calibration_stats filters them, exported
+// in batches as flat arrays for dcb_calib_count; and the reference's bases from a FASTA file through its .fai.
+struct FaiEntry { std::string name; int64_t len = 0, off = 0, line_bases = 0, line_width = 0; };
+
+struct dcb_calib {
+  BamReader bam;
+  std::vector<uint64_t> first;
+  std::vector<std::vector<uint64_t>> linear;
+  std::map<std::string, int32_t> tid;
+  std::string bam_contigs, fasta_contigs;
+  FILE* fa = nullptr;
+  std::vector<FaiEntry> fai;
+  int n_threads = 1;
+  // the current query (dcb_calib_query)
+  int32_t q_tid = -1;
+  int64_t q_lo = 0, q_hi = 0, q_min_pos = 0;
+  int q_min_mapq = 0;
+  bool q_done = true;
+  // the current batch: the kept records' bytes, then their export
+  std::vector<uint8_t> arena;
+  std::vector<size_t> rec_at;
+  std::vector<int32_t> meta;
+  std::vector<uint32_t> cigar;
+  std::vector<uint8_t> seq, qual;
+  std::vector<std::string> names;
+  ~dcb_calib() { if (fa) fclose(fa); }
+};
+
+namespace {
+
+// BAM flags get_quality_calibration_stats skips: duplicate, qcfail, secondary, unmapped, supplementary
+constexpr uint16_t kCalibSkipFlags = 0x400 | 0x200 | 0x100 | 0x4 | 0x800;
+
+// Reference length of a raw record's cigar (M, D, N, =, X)
+int64_t raw_ref_len(const uint8_t* b) {
+  uint16_t n_cig;
+  memcpy(&n_cig, b + 12, 2);
+  const uint8_t* c = b + 32 + b[8];
+  int64_t n = 0;
+  for (int k = 0; k < n_cig; ++k) {
+    uint32_t v;
+    memcpy(&v, c + 4 * k, 4);
+    const int op = v & 15;
+    if (op == kCMatch || op == kCDel || op == kCRefSkip || op == kCEq || op == kCDiff) n += v >> 4;
+  }
+  return n;
+}
+
+// samtools faidx's index, built in memory: per sequence its length, the offset of its first base, and the bases and
+// bytes per line (every line but the last of a sequence has the same length).
+int build_fai(FILE* f, const char* path, std::vector<FaiEntry>* out) {
+  out->clear();
+  std::vector<char> buf(1 << 16);
+  std::string line;
+  int64_t off = 0;
+  bool in_seq = false, short_line = false;
+  auto finish_line = [&](int64_t line_start, int64_t bytes) -> int {
+    // `line` holds the line without its newline, `bytes` counts it with the newline
+    if (!line.empty() && line[0] == '>') {
+      FaiEntry e;
+      size_t k = 1;
+      while (k < line.size() && !isspace((unsigned char)line[k])) ++k;
+      e.name = line.substr(1, k - 1);
+      e.off = line_start + bytes;
+      out->push_back(e);
+      in_seq = true;
+      short_line = false;
+      return DCB_OK;
+    }
+    if (!in_seq) return line.empty() ? DCB_OK : pfail(DCB_ERR_INVALID, "%s: not a FASTA file", path);
+    FaiEntry& e = out->back();
+    int64_t nb = (int64_t)line.size();
+    if (nb && line.back() == '\r') --nb;
+    if (nb == 0) { short_line = true; return DCB_OK; }
+    if (short_line) return pfail(DCB_ERR_INVALID, "%s: sequence %s has lines of different lengths", path, e.name.c_str());
+    if (e.line_bases == 0) { e.line_bases = nb; e.line_width = bytes; }
+    else if (nb > e.line_bases || bytes - nb != e.line_width - e.line_bases)
+      return pfail(DCB_ERR_INVALID, "%s: sequence %s has lines of different lengths", path, e.name.c_str());
+    if (nb < e.line_bases) short_line = true;
+    e.len += nb;
+    return DCB_OK;
+  };
+  int64_t line_start = 0;
+  size_t n;
+  fseeko(f, 0, SEEK_SET);
+  while ((n = fread(buf.data(), 1, buf.size(), f)) > 0) {
+    for (size_t i = 0; i < n; ++i) {
+      if (buf[i] == '\n') {
+        const int rc = finish_line(line_start, off + (int64_t)i + 1 - line_start);
+        if (rc) return rc;
+        line.clear();
+        line_start = off + (int64_t)i + 1;
+      } else {
+        line.push_back(buf[i]);
+      }
+    }
+    off += (int64_t)n;
+  }
+  if (!line.empty()) {
+    const int rc = finish_line(line_start, off - line_start);
+    if (rc) return rc;
+  }
+  return DCB_OK;
+}
+
+int read_fai(const std::string& path, std::vector<FaiEntry>* out) {
+  FILE* f = fopen(path.c_str(), "r");
+  if (!f) return 1;   // none: the caller builds the index
+  char line[4096];
+  int rc = DCB_OK;
+  while (fgets(line, sizeof line, f)) {
+    char name[4096];
+    long long len, off, lb, lw;
+    if (line[0] == '\n') continue;
+    if (sscanf(line, "%4095s %lld %lld %lld %lld", name, &len, &off, &lb, &lw) != 5 || len < 0 || off < 0 || lb <= 0 || lw < lb) {
+      rc = pfail(DCB_ERR_INVALID, "%s: malformed FASTA index line", path.c_str());
+      break;
+    }
+    FaiEntry e;
+    e.name = name; e.len = len; e.off = off; e.line_bases = lb; e.line_width = lw;
+    out->push_back(e);
+  }
+  fclose(f);
+  return rc;
+}
+
+// Bases [start, stop) of sequence e, clipped to the sequence, as the file holds them (case kept).
+int fasta_fetch(dcb_calib* p, const FaiEntry& e, int64_t start, int64_t stop, std::string* out) {
+  out->clear();
+  start = std::max<int64_t>(start, 0);
+  stop = std::min(stop, e.len);
+  if (stop <= start) return DCB_OK;
+  auto at = [&](int64_t k) { return e.off + k / e.line_bases * e.line_width + k % e.line_bases; };
+  const int64_t b0 = at(start), b1 = at(stop - 1) + 1;
+  std::string raw((size_t)(b1 - b0), '\0');
+  if (fseeko(p->fa, (off_t)b0, SEEK_SET) != 0 || fread(&raw[0], 1, raw.size(), p->fa) != raw.size())
+    return pfail(DCB_ERR_INVALID, "FASTA: cannot read %s:%lld-%lld", e.name.c_str(), (long long)start, (long long)stop);
+  out->reserve((size_t)(stop - start));
+  for (char c : raw) if (c != '\n' && c != '\r') out->push_back(c);
+  if ((int64_t)out->size() != stop - start) return pfail(DCB_ERR_INVALID, "FASTA: %s does not match its index", e.name.c_str());
+  return DCB_OK;
+}
+
+// The virtual offset a fetch of [lo, ...) on reference t starts reading at: the linear index's entry for lo's 16 kb
+// window (or the last window's, past the end), never before the reference's first chunk.  A window with no entry
+// takes the nearest earlier one, which can only start the read earlier.
+uint64_t fetch_offset(const dcb_calib* p, int32_t t, int64_t lo) {
+  const uint64_t first = p->first[t];
+  const std::vector<uint64_t>& lin = p->linear[t];
+  if (lin.empty()) return first;
+  int64_t w = std::min<int64_t>(std::max<int64_t>(lo, 0) >> 14, (int64_t)lin.size() - 1);
+  while (w > 0 && lin[w] == 0) --w;
+  return std::max(first, lin[w]);
+}
+
+// Decode / validate the kept records [a, b) of the batch into the offsets the serial pass gave them.  Returns the index
+// of the first record that fails, or -1; its message goes to *err.
+int64_t export_records(dcb_calib* p, size_t a, size_t b, std::string* err) {
+  for (size_t k = a; k < b; ++k) {
+    const uint8_t* r = p->arena.data() + p->rec_at[k];
+    int32_t* m = &p->meta[k * DCB_CALIB_META];
+    const int l_name = r[8];
+    p->names[k].assign(reinterpret_cast<const char*>(r + 32), l_name ? l_name - 1 : 0);
+    const int32_t n_cig = m[3], l_seq = m[5];
+    const uint8_t* c = r + 32 + l_name;
+    memcpy(&p->cigar[m[2]], c, 4ull * n_cig);
+    int64_t qlen = 0;
+    for (int j = 0; j < n_cig; ++j) if (op_has_query(p->cigar[m[2] + j] & 15)) qlen += p->cigar[m[2] + j] >> 4;
+    const uint8_t* s = c + 4ull * n_cig;
+    const uint8_t* q = s + (l_seq + 1) / 2;
+    char buf[512];
+    if (l_seq == 0) snprintf(buf, sizeof buf, "read %s has no SEQ", p->names[k].c_str());
+    else if (q[0] == 0xff) snprintf(buf, sizeof buf, "read %s has no QUAL", p->names[k].c_str());
+    else if (qlen != l_seq)
+      snprintf(buf, sizeof buf, "read %s: its cigar covers %lld query bases, its SEQ holds %d", p->names[k].c_str(),
+               (long long)qlen, l_seq);
+    else buf[0] = 0;
+    if (buf[0]) { *err = buf; return (int64_t)k; }
+    uint8_t* so = &p->seq[m[4]];
+    for (int32_t i = 0; i < l_seq; ++i) so[i] = (s[i >> 1] >> (i & 1 ? 0 : 4)) & 15;
+    memcpy(&p->qual[m[4]], q, (size_t)l_seq);
+  }
+  return -1;
+}
+
+}  // namespace
+
+extern "C" {
+
+int dcb_calib_open(const char* bam, const char* fasta, int32_t n_threads, dcb_calib** out) {
+  if (!bam || !fasta || !out) return pfail(DCB_ERR_INVALID, "dcb_calib_open: null argument");
+  if (n_threads < 1) return pfail(DCB_ERR_INVALID, "dcb_calib_open: %d threads; need at least 1", n_threads);
+  dcb_calib* p = new dcb_calib();
+  p->n_threads = std::min(n_threads, 256);
+  int rc = p->bam.open(bam);
+  if (!rc) rc = read_bai(std::string(bam) + ".bai", p->bam.refs.size(), &p->first, &p->linear);
+  if (!rc && !(p->fa = fopen(fasta, "rb"))) rc = pfail(DCB_ERR_INVALID, "cannot open %s", fasta);
+  if (!rc) {
+    uint8_t magic[2] = {0, 0};
+    if (fread(magic, 1, 2, p->fa) == 2 && magic[0] == 0x1f && magic[1] == 0x8b)
+      rc = pfail(DCB_ERR_INVALID, "%s is compressed; a bgzipped FASTA is not supported, decompress it", fasta);
+  }
+  if (!rc) {
+    const int fr = read_fai(std::string(fasta) + ".fai", &p->fai);
+    if (fr == 1) rc = build_fai(p->fa, fasta, &p->fai);
+    else rc = fr;
+  }
+  if (rc) { delete p; return rc; }
+  for (size_t t = 0; t < p->bam.refs.size(); ++t) {
+    p->tid[p->bam.refs[t]] = (int32_t)t;
+    p->bam_contigs += p->bam.refs[t] + "\t" + std::to_string(p->bam.ref_len[t]) + "\n";
+  }
+  for (const FaiEntry& e : p->fai) p->fasta_contigs += e.name + "\t" + std::to_string(e.len) + "\n";
+  *out = p;
+  return DCB_OK;
+}
+
+void dcb_calib_close(dcb_calib* p) { delete p; }
+
+const char* dcb_calib_contigs(dcb_calib* p, int32_t fasta) {
+  if (!p) return "";
+  return fasta ? p->fasta_contigs.c_str() : p->bam_contigs.c_str();
+}
+
+int dcb_calib_fetch_reference(dcb_calib* p, const char* contig, int64_t start, int64_t stop, uint8_t* out, int64_t* n) {
+  if (!p || !contig || !n || stop < start) return pfail(DCB_ERR_INVALID, "dcb_calib_fetch_reference: bad argument");
+  *n = 0;
+  for (const FaiEntry& e : p->fai) {
+    if (e.name != contig) continue;
+    std::string s;
+    const int rc = fasta_fetch(p, e, start, stop, &s);
+    if (rc) return rc;
+    if (out && !s.empty()) memcpy(out, s.data(), s.size());
+    *n = (int64_t)s.size();
+    return DCB_OK;
+  }
+  return pfail(DCB_ERR_INVALID, "contig %s is not in the FASTA file", contig);
+}
+
+int dcb_calib_query(dcb_calib* p, const char* contig, int64_t start, int64_t stop, int64_t min_pos, int32_t min_mapq) {
+  if (!p || !contig || stop < start) return pfail(DCB_ERR_INVALID, "dcb_calib_query: bad argument");
+  auto it = p->tid.find(contig);
+  if (it == p->tid.end()) return pfail(DCB_ERR_INVALID, "contig %s is not in the BAM header", contig);
+  p->q_tid = it->second;
+  p->q_lo = start; p->q_hi = stop; p->q_min_pos = min_pos; p->q_min_mapq = min_mapq;
+  p->q_done = stop == start || p->first[p->q_tid] == UINT64_MAX;
+  if (!p->q_done && !p->bam.z.seek(fetch_offset(p, p->q_tid, start)))
+    return pfail(DCB_ERR_INVALID, "BAM: bad index offset for %s", contig);
+  return DCB_OK;
+}
+
+int dcb_calib_next_batch(dcb_calib* p, int64_t max_bases, int64_t* sizes) {
+  if (!p || !sizes || max_bases < 1) return pfail(DCB_ERR_INVALID, "dcb_calib_next_batch: bad argument");
+  sizes[0] = sizes[1] = sizes[2] = 0;
+  p->arena.clear(); p->rec_at.clear(); p->meta.clear();
+  max_bases = std::min<int64_t>(max_bases, 1 << 30);
+  int64_t n_cig = 0, n_bases = 0;
+  // Serial pass: inflate, select, and give every kept record its place in the flat arrays.
+  while (!p->q_done && n_bases < max_bases) {
+    const size_t at = p->arena.size();
+    const int rc = p->bam.next_raw(&p->arena);
+    if (rc < 0) return rc;
+    if (rc == 0) { p->q_done = true; break; }
+    const uint8_t* r = p->arena.data() + at;
+    int32_t refid, pos, l_seq;
+    uint16_t flag, nc;
+    memcpy(&refid, r, 4); memcpy(&pos, r + 4, 4); memcpy(&nc, r + 12, 2); memcpy(&flag, r + 14, 2); memcpy(&l_seq, r + 16, 4);
+    const int mapq = r[9];
+    if (refid != p->q_tid || pos >= p->q_hi) {
+      p->arena.resize(at);
+      if (refid < 0 || refid > p->q_tid || (refid == p->q_tid && pos >= p->q_hi)) p->q_done = true;
+      continue;
+    }
+    // AlignmentFile.fetch(contig, lo, hi) returns a record when htslib's overlap test holds: pos < hi and
+    // endpos > lo, where endpos (bam_endpos) is pos plus the cigar's reference length, or pos + 1 when that is 0 or
+    // the record is unmapped.
+    const int64_t rlen = (flag & 4) ? 0 : raw_ref_len(r);
+    const int64_t endpos = pos + (rlen ? rlen : 1);
+    if (endpos <= p->q_lo || pos < p->q_min_pos || (flag & kCalibSkipFlags) || mapq < p->q_min_mapq) {
+      p->arena.resize(at);
+      continue;
+    }
+    if (endpos > INT32_MAX) return pfail(DCB_ERR_INVALID, "a record at %d reaches past 2^31", pos);
+    p->rec_at.push_back(at);
+    const int32_t m[DCB_CALIB_META] = {pos, (int32_t)endpos, (int32_t)n_cig, nc, (int32_t)n_bases, l_seq};
+    p->meta.insert(p->meta.end(), m, m + DCB_CALIB_META);
+    n_cig += nc;
+    n_bases += l_seq;
+  }
+  const size_t n = p->rec_at.size();
+  p->cigar.resize((size_t)n_cig); p->seq.resize((size_t)n_bases); p->qual.resize((size_t)n_bases);
+  p->names.assign(n, std::string());
+  // Parallel pass: decode and validate on n_threads threads, contiguous slices of the batch; the first failing record
+  // in batch order is reported, whichever thread found it.
+  const int nt = (int)std::min<size_t>((size_t)p->n_threads, std::max<size_t>(n, 1));
+  std::vector<int64_t> bad(nt, -1);
+  std::vector<std::string> errs(nt);
+  auto work = [&](int t) { bad[t] = export_records(p, n * t / nt, n * (t + 1) / nt, &errs[t]); };
+  if (nt == 1) {
+    work(0);
+  } else {
+    std::vector<std::thread> th;
+    for (int t = 0; t < nt; ++t) th.emplace_back(work, t);
+    for (auto& x : th) x.join();
+  }
+  for (int t = 0; t < nt; ++t) if (bad[t] >= 0) return pfail(DCB_ERR_INVALID, "%s", errs[t].c_str());
+  sizes[0] = (int64_t)n; sizes[1] = n_cig; sizes[2] = n_bases;
+  return n ? 1 : 0;
+}
+
+int dcb_calib_get_batch(dcb_calib* p, int32_t* read_meta, uint32_t* cigar, uint8_t* seq, uint8_t* qual) {
+  if (!p) return pfail(DCB_ERR_INVALID, "dcb_calib_get_batch: null handle");
+  if (read_meta && !p->meta.empty()) memcpy(read_meta, p->meta.data(), p->meta.size() * sizeof(int32_t));
+  if (cigar && !p->cigar.empty()) memcpy(cigar, p->cigar.data(), p->cigar.size() * sizeof(uint32_t));
+  if (seq && !p->seq.empty()) memcpy(seq, p->seq.data(), p->seq.size());
+  if (qual && !p->qual.empty()) memcpy(qual, p->qual.data(), p->qual.size());
+  return DCB_OK;
+}
+
+const char* dcb_calib_read_name(dcb_calib* p, int64_t i) {
+  if (!p || i < 0 || i >= (int64_t)p->names.size()) return "";
+  return p->names[(size_t)i].c_str();
 }
 
 }  // extern "C"

@@ -207,6 +207,14 @@ struct dcb_engine {
     PrepBatch batch{};
     int n_windows = -1;   // windows of the resident layout; -1: none
   } fp;
+  struct {   // dcb_calib_count: one batch of reads, the regions, and the contig's bases (kept between calls)
+    DevBuf<int32_t> meta;
+    DevBuf<uint32_t> cigar;
+    DevBuf<uint8_t> seq, qual, ref;
+    DevBuf<int64_t> regions;
+    DevBuf<long long> partial, partial_fail, out;
+    int64_t ref_start = 0, ref_count = -1;   // ref_count -1: no bases uploaded yet
+  } cb;
   cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;   // around the kernel of dcb_evaluate / _distill_loss / _loss_grad
 
   // Safe on a partly built engine.  The caller has made cfg.device current; the DevBuf members free themselves after
@@ -2057,6 +2065,87 @@ int dcb_features_eval(dcb_engine* e, const dcb_labels* lab, const uint8_t* keep_
     CU(e, cudaMemcpyAsync(windows_out, fp.list.p, (size_t)k * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CU(e, cudaStreamSynchronize(st));
   }
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  return DCB_OK;
+}
+
+// The batch as dcb_calib_count's kernels may trust it: offsets inside the arrays, every cigar's query length equal to
+// its read's base count, and endpos equal to bam_endpos (pos plus the reference length, or pos + 1).
+static int check_calib_batch(dcb_engine* e, const dcb_calib_input* in) {
+  if (in->n_reads < 0 || in->n_regions < 0 || in->n_cigar < 0 || in->n_bases < 0 || in->interval_length <= 0 ||
+      in->ref_count < 0 || in->contig_length < 0 || in->n_bases > INT32_MAX || in->n_cigar > INT32_MAX)
+    return fail(e, DCB_ERR_INVALID, "dcb_calib_count: bad sizes");
+  if ((in->n_reads && (!in->read_meta || (in->n_cigar && !in->cigar) || (in->n_bases && (!in->seq || !in->qual)))) ||
+      (in->n_regions && !in->regions))
+    return fail(e, DCB_ERR_INVALID, "dcb_calib_count: null array");
+  for (int32_t k = 0; k < in->n_regions; ++k)
+    if (in->regions[2 * k] < 0 || in->regions[2 * k] > in->regions[2 * k + 1] || in->regions[2 * k + 1] > INT32_MAX)
+      return fail(e, DCB_ERR_INVALID, "dcb_calib_count: region %d is not 0 <= start <= stop < 2^31", k);
+  for (int32_t r = 0; r < in->n_reads; ++r) {
+    const int32_t* m = in->read_meta + (size_t)r * DCB_CALIB_META;
+    if (m[0] < 0 || m[2] < 0 || m[3] < 0 || m[4] < 0 || m[5] < 0 || (int64_t)m[2] + m[3] > in->n_cigar ||
+        (int64_t)m[4] + m[5] > in->n_bases)
+      return fail(e, DCB_ERR_INVALID, "dcb_calib_count: read %d: offsets outside the batch", r);
+    int64_t q = 0, rl = 0;
+    for (int32_t k = 0; k < m[3]; ++k) {
+      const uint32_t v = in->cigar[m[2] + k];
+      const int op = v & 15;
+      if (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) q += v >> 4;
+      if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) rl += v >> 4;
+    }
+    if (q != m[5]) return fail(e, DCB_ERR_INVALID, "dcb_calib_count: read %d: its cigar covers %lld bases, it has %d", r, (long long)q, m[5]);
+    if ((int64_t)m[5] * 2 * in->n_regions >= (1ll << 32))   // the kernel's per-read 32-bit histogram
+      return fail(e, DCB_ERR_INVALID, "dcb_calib_count: read %d: %d bases over %d regions could overflow a count", r, m[5], in->n_regions);
+    if ((int64_t)m[1] != m[0] + (rl ? rl : 1)) return fail(e, DCB_ERR_INVALID, "dcb_calib_count: read %d: endpos is not bam_endpos", r);
+  }
+  return DCB_OK;
+}
+
+int dcb_calib_count(dcb_engine* e, const dcb_calib_input* in, int64_t* counts, int64_t* failure, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  if (ms_out) *ms_out = 0.f;
+  if (!in || !counts || !failure) return fail(e, DCB_ERR_INVALID, "dcb_calib_count: null argument");
+  memset(counts, 0, 2 * kCalibBins * sizeof(int64_t));
+  failure[0] = -1; failure[1] = failure[2] = 0;
+  int rc;
+  if ((rc = check_calib_batch(e, in))) return rc;
+  auto& cb = e->cb;
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  if (in->ref_bases) {
+    if ((rc = ensure(e, cb.ref, (size_t)std::max<int64_t>(in->ref_count, 1)))) return rc;
+    cb.ref_count = -1;
+    if (in->ref_count) CU(e, cudaMemcpyAsync(cb.ref.p, in->ref_bases, (size_t)in->ref_count, cudaMemcpyHostToDevice, st));
+    cb.ref_start = in->ref_start;
+    cb.ref_count = in->ref_count;
+  } else if (cb.ref_count < 0 || cb.ref_start != in->ref_start || cb.ref_count != in->ref_count) {
+    return fail(e, DCB_ERR_STATE, "dcb_calib_count: no reference bases for [%lld, +%lld) were given", (long long)in->ref_start,
+                (long long)in->ref_count);
+  }
+  const int grid = std::min(in->n_reads, 1024);
+  const int32_t* d_meta;
+  const uint32_t* d_cigar;
+  const uint8_t *d_seq, *d_qual;
+  const int64_t* d_regions;
+  if ((rc = stage_in(e, cb.meta, in->read_meta, (size_t)in->n_reads * DCB_CALIB_META, false, &d_meta)) ||
+      (rc = stage_in(e, cb.cigar, in->cigar, (size_t)in->n_cigar, false, &d_cigar)) ||
+      (rc = stage_in(e, cb.seq, in->seq, (size_t)in->n_bases, false, &d_seq)) ||
+      (rc = stage_in(e, cb.qual, in->qual, (size_t)in->n_bases, false, &d_qual)) ||
+      (rc = stage_in(e, cb.regions, in->regions, (size_t)in->n_regions * 2, false, &d_regions)) ||
+      (rc = ensure(e, cb.partial, (size_t)std::max(grid, 1) * 2 * kCalibBins)) ||
+      (rc = ensure(e, cb.partial_fail, (size_t)std::max(grid, 1) * 2)) || (rc = ensure(e, cb.out, 2 * kCalibBins + 3)))
+    return rc;
+  CalibBatch c{d_meta, d_cigar, d_seq, d_qual, in->n_reads, in->n_regions, d_regions, in->interval_length, cb.ref.p,
+               in->ref_start, in->ref_count, in->contig_length, in->calibration_enabled ? 1 : 0, in->threshold, in->w, in->b};
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  launch_calib_count(c, grid, cb.partial.p, cb.partial_fail.p, cb.out.p, st);
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  long long out[2 * kCalibBins + 3];
+  CU(e, cudaMemcpyAsync(out, cb.out.p, sizeof out, cudaMemcpyDeviceToHost, st));
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  for (int k = 0; k < 2 * kCalibBins; ++k) counts[k] = out[k];
+  for (int k = 0; k < 3; ++k) failure[k] = out[2 * kCalibBins + k];
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
   return DCB_OK;
 }

@@ -138,6 +138,28 @@ void launch_labels(const PrepBatch& b, const LabelBatch& lb, const int4* window,
 void launch_features_eval(const PrepBatch& b, const LabelBatch& lb, const int4* window, int n_windows, const uint8_t* ccs_rows,
                           const uint8_t* keep_zmw, int cap, uint8_t* label_rows, uint8_t* status, int32_t* dst, int32_t* list,
                           int* count, uint8_t* packed, uint8_t* labels_out, uint8_t* ccs_out, cudaStream_t st);
+// ---- base-quality calibration counts (calib_kernels.cu, dcb_calib_count).  All pointers are device pointers; the
+// batch is validated on the host (offsets in bounds, each cigar's query length equal to its base count, endpos equal
+// to bam_endpos).  out: int64 [2 * kCalibBins + 3] = counts [bin][match, mismatch], then the lowest failing read
+// (-1: none), its reference position and its kind.  partial / partial_fail: grid * 2 * kCalibBins and grid * 2 entries.
+constexpr int kCalibMeta = 6;   // DCB_CALIB_META
+constexpr int kCalibBins = 100;
+constexpr int kCalibPastContig = 1, kCalibBadQuality = 2, kCalibBadInput = 3;   // DCB_CALIB_*
+struct CalibBatch {
+  const int32_t* read_meta;
+  const uint32_t* cigar;
+  const uint8_t* seq;
+  const uint8_t* qual;
+  int n_reads, n_regions;
+  const int64_t* regions;
+  int64_t interval_length;
+  const uint8_t* ref;
+  int64_t ref_start, ref_count, contig_length;
+  int calibration_enabled;
+  double threshold, w, b;
+};
+void launch_calib_count(const CalibBatch& c, int grid, long long* partial, long long* partial_fail, long long* out,
+                        cudaStream_t st);
 // the CCS ids / qualities of windows list[0..n_list) at full width, window j at off[j] of ccs_ids / ccs_bq
 void launch_features_ccs(const PrepBatch& b, const int4* window, const int32_t* list, int n_list, const int64_t* off,
                          uint8_t* ccs_ids, int16_t* ccs_bq, cudaStream_t st);

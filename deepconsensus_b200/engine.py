@@ -42,6 +42,9 @@ PRECISIONS = {"bf16": DCB_PRECISION_BF16, "fp32": DCB_PRECISION_FP32, "tf32x3": 
 DCB_READ_OK, DCB_READ_EMPTY, DCB_READ_ONLY_GAPS, DCB_READ_LOW_QUALITY, DCB_READ_TOO_SHORT = 0, 1, 2, 3, 4
 DCB_READ_BORDERLINE = 0x80
 DCB_BAND_WIDTH_NONE = -1
+# dcb_calib_count: per-read meta columns, quality bins, and the kinds of failure it reports
+CALIB_META, CALIB_BINS = 6, 100
+DCB_CALIB_PAST_CONTIG, DCB_CALIB_BAD_QUALITY, DCB_CALIB_BAD_INPUT = 1, 2, 3
 DCB_LOGIT_LOSS_MSE, DCB_LOGIT_LOSS_KL = 0, 1
 # Keras loss identifiers (tf.keras.losses.get) of the two logit losses DistillationLoss is used with
 LOGIT_LOSS_IDS = {"mean_squared_error": DCB_LOGIT_LOSS_MSE, "mse": DCB_LOGIT_LOSS_MSE, "MSE": DCB_LOGIT_LOSS_MSE,
@@ -104,6 +107,17 @@ class DcbRecords(ctypes.Structure):
                                      "pw", "ip", "ccs_bases", "ccs_bq")]
 
 
+class DcbCalibInput(ctypes.Structure):
+  """dcb_calib_input: one batch of aligned reads and the regions of one contig (include/dcb200.h "base-quality
+  calibration")."""
+  _fields_ = [("n_reads", ctypes.c_int32), ("n_regions", ctypes.c_int32), ("n_cigar", ctypes.c_int64),
+              ("n_bases", ctypes.c_int64), ("read_meta", ctypes.c_void_p), ("cigar", ctypes.c_void_p),
+              ("seq", ctypes.c_void_p), ("qual", ctypes.c_void_p), ("regions", ctypes.c_void_p),
+              ("interval_length", ctypes.c_int64), ("ref_bases", ctypes.c_void_p), ("ref_start", ctypes.c_int64),
+              ("ref_count", ctypes.c_int64), ("contig_length", ctypes.c_int64), ("calibration_enabled", ctypes.c_int32),
+              ("reserved", ctypes.c_int32), ("threshold", ctypes.c_double), ("w", ctypes.c_double), ("b", ctypes.c_double)]
+
+
 # Every symbol include/dcb200.h declares; tests check the built library exports all of them.
 ABI_SYMBOLS = (
     "dcb_create", "dcb_load_weights", "dcb_forward", "dcb_submit", "dcb_wait", "dcb_stitch", "dcb_last_forward_ms",
@@ -115,6 +129,8 @@ ABI_SYMBOLS = (
     "dcb_prep_get_window_widths", "dcb_prep_get_overflow_ccs", "dcb_features_layout", "dcb_features_pack",
     "dcb_features_layout_smart", "dcb_features_ccs", "dcb_prep_get_window_lengths", "dcb_prep_open_truth",
     "dcb_prep_get_label", "dcb_features_labels", "dcb_features_eval",
+    "dcb_calib_open", "dcb_calib_contigs", "dcb_calib_fetch_reference", "dcb_calib_query", "dcb_calib_next_batch",
+    "dcb_calib_get_batch", "dcb_calib_read_name", "dcb_calib_close", "dcb_calib_count",
     "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
     "dcb_last_forward_launches", "dcb_set_profile", "dcb_get_profile", "dcb_get_profile_kernels", "dcb_alloc_host",
     "dcb_free_host", "dcb_alloc_device", "dcb_free_device", "dcb_memcpy_h2d", "dcb_memcpy_d2h",
@@ -191,6 +207,7 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_features_labels.argtypes = [vp, ctypes.POINTER(DcbLabels), vp, i32, vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_features_eval.argtypes = [vp, ctypes.POINTER(DcbLabels), vp, i32, i32, vp, vp, vp, vp, vp, vp, ctypes.POINTER(i32),
                                     ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_calib_count.argtypes = [vp, ctypes.POINTER(DcbCalibInput), vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_launches.argtypes = [vp, ctypes.POINTER(i32)]
   lib.dcb_set_debug.argtypes = [vp, i32]
@@ -754,6 +771,32 @@ class B200Model:
     out["windows"] = out["windows"][:out["k"]]
     out["ms"] = float(ms.value)
     return out
+
+  def calib_count(self, batch: Dict[str, np.ndarray], regions: np.ndarray, interval_length: int,
+                  ref_bases: Optional[np.ndarray], ref_start: int, ref_count: int, contig_length: int,
+                  calibration: Optional[calibration_lib.QualityCalibrationValues] = None) -> Dict[str, Any]:
+    """dcb_calib_count: the (match, mismatch) events per quality bin of one batch of reads (dict of read_meta int32
+    [n, CALIB_META], cigar uint32, seq uint8 4-bit codes, qual uint8) over every interval of `regions` (int64 [k, 2],
+    start and stop on one contig).  ref_bases: the contig's bases [ref_start, ref_start + ref_count), or None to keep
+    the previous call's.  Returns dict(counts int64 [100, 2], failure (read index, position, DCB_CALIB_*) with read
+    index -1 when no counted event fails, ms)."""
+    meta = np.ascontiguousarray(batch["read_meta"], np.int32).reshape(-1, CALIB_META)
+    cig, seq, qual = (np.ascontiguousarray(batch[k], dt) for k, dt in (("cigar", np.uint32), ("seq", np.uint8),
+                                                                       ("qual", np.uint8)))
+    reg = np.ascontiguousarray(regions, np.int64).reshape(-1, 2)
+    # an empty array still has to reach the call as a non-NULL pointer: NULL keeps the previous call's bases
+    ref = None if ref_bases is None else np.ascontiguousarray(ref_bases, np.uint8) if len(ref_bases) else np.zeros(1, np.uint8)
+    cal = calibration
+    en = bool(cal is not None and cal.enabled)
+    arg = DcbCalibInput(n_reads=len(meta), n_regions=len(reg), n_cigar=cig.size, n_bases=seq.size, read_meta=_ptr(meta),
+                        cigar=_ptr(cig), seq=_ptr(seq), qual=_ptr(qual), regions=_ptr(reg),
+                        interval_length=int(interval_length), ref_bases=None if ref is None else _ptr(ref),
+                        ref_start=int(ref_start), ref_count=int(ref_count), contig_length=int(contig_length),
+                        calibration_enabled=int(en), threshold=float(cal.threshold) if en else 0.0,
+                        w=float(cal.w) if en else 1.0, b=float(cal.b) if en else 0.0)
+    counts, failure, ms = np.zeros((CALIB_BINS, 2), np.int64), np.zeros(3, np.int64), ctypes.c_float(0)
+    self._check(self._lib.dcb_calib_count(self._handle, ctypes.byref(arg), _ptr(counts), _ptr(failure), ctypes.byref(ms)))
+    return dict(counts=counts, failure=tuple(int(x) for x in failure), ms=float(ms.value))
 
   def stitch_raw(self, bases_ptr: int, quals_ptr: int, n_windows: int, zmw_start: np.ndarray, flags: int,
                  seq_ptr: int, qual_ptr: int, len_ptr: int, length: Optional[int] = None) -> None:

@@ -522,6 +522,62 @@ int dcb_features_eval(dcb_engine* e, const dcb_labels* labels, const uint8_t* ke
                       uint8_t* packed_out, uint8_t* labels_out, uint8_t* ccs_out, uint8_t* status_out, int32_t* ccs_width_out,
                       int32_t* windows_out, int32_t* k_out, float* ms_out);
 
+/* ---- base-quality calibration (calculate_baseq_calibration.py) ----------------------------------------------------------
+ * Per predicted quality, how many bases of reads aligned to a truth assembly match it and how many do not.
+ *
+ * The reader (host C++, needs no GPU).  dcb_calib_open opens a coordinate-sorted BAM with its index (path + ".bai"; a
+ * missing index is DCB_ERR_INVALID) and a plain FASTA file, through its .fai when there is one, else an index built in
+ * memory (a compressed FASTA is refused).  n_threads >= 1 threads decode and validate each batch.
+ * dcb_calib_contigs: "name\tlength\n" per contig of the BAM header (fasta = 0) or of the FASTA file (fasta = 1).
+ * dcb_calib_fetch_reference: the FASTA bases [start, stop) of a contig as the file holds them, clipped at its end;
+ * *n receives their count, out (nullable) needs stop - start bytes.
+ * dcb_calib_query starts a fetch of [start, stop) on a contig: what AlignmentFile.fetch returns (htslib's overlap
+ * test, pos < stop and bam_endpos > start), minus records with pos < min_pos, duplicate, qcfail, secondary, unmapped or
+ * supplementary records, and records with mapping quality < min_mapq.  dcb_calib_next_batch reads on until the batch
+ * holds at least max_bases bases (or the fetch ends): returns 1 with sizes [3] = reads, cigar operations, bases, or 0
+ * when nothing is left; a record without SEQ or QUAL, or whose cigar disagrees with its SEQ, is DCB_ERR_INVALID naming
+ * it.  dcb_calib_get_batch copies the batch out (every array nullable): read_meta int32 [reads, DCB_CALIB_META] = pos,
+ * endpos, cigar offset, cigar count, base offset, base count; cigar [operations] as the BAM stores it; seq [bases] the
+ * 4-bit codes of "=ACMGRSVTWYHKDBN"; qual [bases] Phred values.  dcb_calib_read_name: the name of read i of the batch.
+ * Errors: dcb_prep_last_error.
+ *
+ * The count (engine, sm_90a): dcb_calib_count walks every read of a batch on the device and returns in counts int64
+ * [100][2] how many (match, mismatch) events each quality bin received over every interval of the regions on the
+ * contig -- each region [start, stop] cut into intervals [s, min(stop, s + interval_length)], both ends inclusive, each
+ * counting the reads it fetches.  failure int64 [3] receives (read index, reference position, DCB_CALIB_*) of the
+ * lowest read of the batch that has a counted event the reference would fail on, or (-1, 0, 0): a base past the
+ * contig's end, a quality whose bin lies outside [-100, 100), or (DCB_CALIB_BAD_INPUT) bases the call was not given.
+ * ref_bases (host) are the contig's bases [ref_start, ref_start + ref_count); NULL keeps the previous call's, which
+ * must then have the same ref_start and ref_count.  ms_out (nullable): device time of the kernels.  The counts are sums
+ * of integers, so they do not depend on the order of the work; there are no global atomics. */
+#define DCB_CALIB_META 6
+#define DCB_CALIB_PAST_CONTIG 1
+#define DCB_CALIB_BAD_QUALITY 2
+#define DCB_CALIB_BAD_INPUT 3
+typedef struct dcb_calib dcb_calib;
+int dcb_calib_open(const char* bam, const char* fasta, int32_t n_threads, dcb_calib** out);
+const char* dcb_calib_contigs(dcb_calib* p, int32_t fasta);
+int dcb_calib_fetch_reference(dcb_calib* p, const char* contig, int64_t start, int64_t stop, uint8_t* out, int64_t* n);
+int dcb_calib_query(dcb_calib* p, const char* contig, int64_t start, int64_t stop, int64_t min_pos, int32_t min_mapq);
+int dcb_calib_next_batch(dcb_calib* p, int64_t max_bases, int64_t* sizes);
+int dcb_calib_get_batch(dcb_calib* p, int32_t* read_meta, uint32_t* cigar, uint8_t* seq, uint8_t* qual);
+const char* dcb_calib_read_name(dcb_calib* p, int64_t i);
+void dcb_calib_close(dcb_calib* p);
+typedef struct dcb_calib_input {
+  int32_t n_reads, n_regions;
+  int64_t n_cigar, n_bases;
+  const int32_t* read_meta;        /* [n_reads, DCB_CALIB_META] */
+  const uint32_t* cigar;           /* [n_cigar] */
+  const uint8_t *seq, *qual;       /* [n_bases] */
+  const int64_t* regions;          /* [n_regions, 2]: start, stop */
+  int64_t interval_length;         /* > 0 */
+  const uint8_t* ref_bases;        /* [ref_count] or NULL */
+  int64_t ref_start, ref_count, contig_length;
+  int32_t calibration_enabled, reserved;
+  double threshold, w, b;          /* calibrate_quality_scores' threshold, w, b */
+} dcb_calib_input;
+int dcb_calib_count(dcb_engine* e, const dcb_calib_input* in, int64_t* counts, int64_t* failure, float* ms_out);
+
 /* Device time of the last dcb_forward (milliseconds, CUDA events on the engine's stream). */
 int dcb_last_forward_ms(dcb_engine* e, float* ms);
 /* Number of engine kernels launched by the last dcb_forward. */
