@@ -22,10 +22,21 @@
 // s_k = S + kL and e_k = min(T, s_k + L), both ends inclusive.  For S <= r < T, r lies in interval (r - S) / L, and
 // also in the one before it when r is exactly an interval start (k > 0); r == T lies in the last interval only.  An
 // interval counts the event when it fetched the read: htslib's overlap test pos < e_k and endpos > s_k.
+//
+// Read identity (dcb_read_identity) walks the same cigars the same way:
+//   read_identity_kernel  one CTA per read.  The block scan places each operation, and its thread adds an I, D or S
+//                         operation's length to the read's insertions, deletions or soft clips (an N operation marks
+//                         the read); threads over the query bases compare each M / = / X base with the upper-cased
+//                         reference base (equal A, C, G or T: a match, anything else a mismatch).  Meanwhile a shared
+//                         histogram of the qualities gives avg_phred by read_outcome_kernel's arithmetic
+//                         (quality.cuh).  A fixed-order block reduction writes the read's five int64 counts; the read's
+//                         status says whether they count (see include/dcb200.h).  No global atomics.
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 
 #include "kernels.h"
+#include "quality.cuh"
 
 namespace dcb {
 
@@ -202,12 +213,103 @@ __global__ void __launch_bounds__(kCalibThreads) calib_reduce_kernel(const long 
   }
 }
 
+__global__ void __launch_bounds__(kCalibThreads) read_identity_kernel(IdentityBatch c, long long* counts, double* avg_q_out,
+                                                                      int32_t* status) {
+  static_assert(kCalibThreads == 256, "one histogram bin per thread");
+  __shared__ int hist[256];
+  __shared__ unsigned long long warp_sums[kCalibWarps];
+  __shared__ int s_qbeg[kCalibThreads], s_qend[kCalibThreads], s_rbeg[kCalibThreads];
+  __shared__ uint8_t s_op[kCalibThreads];
+  __shared__ long long s_red[kIdentityCounts][kCalibWarps];
+  const int tid = threadIdx.x, rd = blockIdx.x;
+  const int32_t* m = c.read_meta + (size_t)rd * kCalibMeta;
+  const uint32_t* cig = c.cigar + m[2];
+  const int n_ops = m[3], n_bases = m[5];
+  const uint8_t* seq = c.seq + m[4];
+  const uint8_t* qual = c.qual + m[4];
+  hist[tid] = 0;
+  __syncthreads();
+  for (int i = tid; i < n_bases; i += kCalibThreads) atomicAdd(&hist[qual[i]], 1);   // integer: exact
+  long long v[kIdentityCounts] = {0, 0, 0, 0, 0};   // matches, mismatches, insertions, deletions, soft clips
+  int skip = 0, bad = 0;
+  int64_t q0 = 0, r0 = m[0];
+  for (int base = 0; base < n_ops; base += kCalibThreads) {
+    const int k = base + tid;
+    const uint32_t x = k < n_ops ? cig[k] : 0u;
+    const int op = k < n_ops ? (int)(x & 15) : 15;
+    const unsigned long long len = x >> 4;
+    if (op == 1) v[2] += (long long)len;
+    else if (op == 2) v[3] += (long long)len;
+    else if (op == 4) v[4] += (long long)len;
+    skip |= op == 3;
+    const unsigned long long e = (calib_ref(op) ? len << 32 : 0ull) | (calib_query(op) ? len : 0ull);
+    unsigned long long total;
+    const unsigned long long incl = calib_scan(e, warp_sums, &total);
+    const unsigned long long excl = incl - e;
+    s_qbeg[tid] = (int)(uint32_t)excl;
+    s_qend[tid] = (int)(uint32_t)incl;
+    s_rbeg[tid] = (int)(excl >> 32);
+    s_op[tid] = (uint8_t)op;
+    __syncthreads();
+    const int chunk_q = (int)(uint32_t)total;
+    const int last = min(kCalibThreads, n_ops - base) - 1;
+    for (int j = tid; j < chunk_q; j += kCalibThreads) {
+      int lo = 0, hi = last;   // the first operation whose inclusive query end exceeds j
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (s_qend[mid] > j) hi = mid; else lo = mid + 1;
+      }
+      if (!calib_aligned(s_op[lo])) continue;
+      const int64_t r = r0 + s_rbeg[lo] + (j - s_qbeg[lo]);
+      if (r >= c.contig_length) continue;   // the read runs past the contig and does not count
+      const int64_t at = r - c.ref_start;
+      if (at < 0 || at >= c.ref_count) { bad = 1; continue; }
+      int rb = c.ref[at];
+      if (rb >= 'a' && rb <= 'z') rb -= 32;
+      const int code = rb == 'A' ? 1 : rb == 'C' ? 2 : rb == 'G' ? 4 : rb == 'T' ? 8 : 0;   // 4-bit SEQ codes
+      if (code != 0 && seq[q0 + j] == code) ++v[0]; else ++v[1];
+    }
+    q0 += chunk_q;
+    r0 += (int64_t)(total >> 32);
+    __syncthreads();
+  }
+  skip = __syncthreads_or(skip);
+  bad = __syncthreads_or(bad);
+  const int lane = tid & 31, w = tid >> 5;
+#pragma unroll
+  for (int k = 0; k < kIdentityCounts; ++k) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) v[k] += __shfl_down_sync(0xffffffffu, v[k], d);
+    if (lane == 0) s_red[k][w] = v[k];
+  }
+  __syncthreads();
+  // r0 is now pos plus the reference length: the read has a reference base at or past the contig's end when it exceeds it
+  const int st = skip ? kIdentitySkipOp : r0 > c.contig_length ? kIdentityPastContig : bad ? kIdentityBadInput : kIdentityOk;
+  if (tid < kIdentityCounts) {
+    long long s = 0;
+    for (int k = 0; k < kCalibWarps; ++k) s += s_red[tid][k];
+    counts[(size_t)rd * kIdentityCounts + tid] = st == kIdentityOk ? s : 0;
+  }
+  if (tid == 0) {
+    const double avg_q = avg_phred_hist(hist, 256, c.p10);
+    // round(avg_q, 5) >= q changes only at q - 5e-6 for an integer threshold q: flag the read near the closest one
+    bool border;
+    phred_passes(avg_q, rint(avg_q + 5e-6), &border);
+    avg_q_out[rd] = avg_q;
+    status[rd] = st == kIdentityOk && border ? kIdentityBorderline : st;
+  }
+}
+
 }  // namespace
 
 void launch_calib_count(const CalibBatch& c, int grid, long long* partial, long long* partial_fail, long long* out,
                         cudaStream_t st) {
   if (grid > 0) calib_count_kernel<<<grid, kCalibThreads, 0, st>>>(c, partial, partial_fail);
   calib_reduce_kernel<<<1, kCalibThreads, 0, st>>>(partial, partial_fail, grid, out);
+}
+
+void launch_read_identity(const IdentityBatch& c, long long* counts, double* avg_q, int32_t* status, cudaStream_t st) {
+  if (c.n_reads > 0) read_identity_kernel<<<c.n_reads, kCalibThreads, 0, st>>>(c, counts, avg_q, status);
 }
 
 }  // namespace dcb

@@ -215,6 +215,13 @@ struct dcb_engine {
     DevBuf<long long> partial, partial_fail, out;
     int64_t ref_start = 0, ref_count = -1;   // ref_count -1: no bases uploaded yet
   } cb;
+  struct {   // dcb_read_identity
+    DevBuf<int32_t> meta, status;
+    DevBuf<uint32_t> cigar;
+    DevBuf<uint8_t> seq, qual, ref;
+    DevBuf<long long> counts;
+    DevBuf<double> avg_q;
+  } ri;
   cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;   // around the kernel of dcb_evaluate / _distill_loss / _loss_grad
 
   // Safe on a partly built engine.  The caller has made cfg.device current; the DevBuf members free themselves after
@@ -2069,8 +2076,29 @@ int dcb_features_eval(dcb_engine* e, const dcb_labels* lab, const uint8_t* keep_
   return DCB_OK;
 }
 
-// The batch as dcb_calib_count's kernels may trust it: offsets inside the arrays, every cigar's query length equal to
-// its read's base count, and endpos equal to bam_endpos (pos plus the reference length, or pos + 1).
+// Read r of a batch from dcb_calib_get_batch as the kernels that walk it may trust it: offsets inside the arrays, its
+// cigar's query length equal to its base count, and endpos equal to bam_endpos (pos plus the reference length, or
+// pos + 1).
+static int check_aligned_read(dcb_engine* e, const char* who, int32_t r, const int32_t* read_meta, const uint32_t* cigar,
+                              int64_t n_cigar, int64_t n_bases) {
+  const int32_t* m = read_meta + (size_t)r * DCB_CALIB_META;
+  if (m[0] < 0 || m[2] < 0 || m[3] < 0 || m[4] < 0 || m[5] < 0 || (int64_t)m[2] + m[3] > n_cigar ||
+      (int64_t)m[4] + m[5] > n_bases)
+    return fail(e, DCB_ERR_INVALID, "%s: read %d: offsets outside the batch", who, r);
+  int64_t q = 0, rl = 0;
+  for (int32_t k = 0; k < m[3]; ++k) {
+    const uint32_t v = cigar[m[2] + k];
+    const int op = v & 15;
+    if (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) q += v >> 4;
+    if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) rl += v >> 4;
+  }
+  if (q != m[5]) return fail(e, DCB_ERR_INVALID, "%s: read %d: its cigar covers %lld bases, it has %d", who, r, (long long)q, m[5]);
+  if ((int64_t)m[1] != m[0] + (rl ? rl : 1)) return fail(e, DCB_ERR_INVALID, "%s: read %d: endpos is not bam_endpos", who, r);
+  return DCB_OK;
+}
+
+// The batch as dcb_calib_count's kernels may trust it: every read as check_aligned_read has it, and few enough bases
+// per read for the kernel's 32-bit histogram.
 static int check_calib_batch(dcb_engine* e, const dcb_calib_input* in) {
   if (in->n_reads < 0 || in->n_regions < 0 || in->n_cigar < 0 || in->n_bases < 0 || in->interval_length <= 0 ||
       in->ref_count < 0 || in->contig_length < 0 || in->n_bases > INT32_MAX || in->n_cigar > INT32_MAX)
@@ -2082,21 +2110,11 @@ static int check_calib_batch(dcb_engine* e, const dcb_calib_input* in) {
     if (in->regions[2 * k] < 0 || in->regions[2 * k] > in->regions[2 * k + 1] || in->regions[2 * k + 1] > INT32_MAX)
       return fail(e, DCB_ERR_INVALID, "dcb_calib_count: region %d is not 0 <= start <= stop < 2^31", k);
   for (int32_t r = 0; r < in->n_reads; ++r) {
-    const int32_t* m = in->read_meta + (size_t)r * DCB_CALIB_META;
-    if (m[0] < 0 || m[2] < 0 || m[3] < 0 || m[4] < 0 || m[5] < 0 || (int64_t)m[2] + m[3] > in->n_cigar ||
-        (int64_t)m[4] + m[5] > in->n_bases)
-      return fail(e, DCB_ERR_INVALID, "dcb_calib_count: read %d: offsets outside the batch", r);
-    int64_t q = 0, rl = 0;
-    for (int32_t k = 0; k < m[3]; ++k) {
-      const uint32_t v = in->cigar[m[2] + k];
-      const int op = v & 15;
-      if (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) q += v >> 4;
-      if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) rl += v >> 4;
-    }
-    if (q != m[5]) return fail(e, DCB_ERR_INVALID, "dcb_calib_count: read %d: its cigar covers %lld bases, it has %d", r, (long long)q, m[5]);
-    if ((int64_t)m[5] * 2 * in->n_regions >= (1ll << 32))   // the kernel's per-read 32-bit histogram
-      return fail(e, DCB_ERR_INVALID, "dcb_calib_count: read %d: %d bases over %d regions could overflow a count", r, m[5], in->n_regions);
-    if ((int64_t)m[1] != m[0] + (rl ? rl : 1)) return fail(e, DCB_ERR_INVALID, "dcb_calib_count: read %d: endpos is not bam_endpos", r);
+    int rc = check_aligned_read(e, "dcb_calib_count", r, in->read_meta, in->cigar, in->n_cigar, in->n_bases);
+    if (rc) return rc;
+    const int32_t nb = in->read_meta[(size_t)r * DCB_CALIB_META + 5];
+    if ((int64_t)nb * 2 * in->n_regions >= (1ll << 32))   // the kernel's per-read 32-bit histogram
+      return fail(e, DCB_ERR_INVALID, "dcb_calib_count: read %d: %d bases over %d regions could overflow a count", r, nb, in->n_regions);
   }
   return DCB_OK;
 }
@@ -2146,6 +2164,55 @@ int dcb_calib_count(dcb_engine* e, const dcb_calib_input* in, int64_t* counts, i
   CU(e, cudaGetLastError());
   for (int k = 0; k < 2 * kCalibBins; ++k) counts[k] = out[k];
   for (int k = 0; k < 3; ++k) failure[k] = out[2 * kCalibBins + k];
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  return DCB_OK;
+}
+
+static_assert(kIdentityCounts == DCB_IDENTITY_COUNTS && kIdentityOk == DCB_IDENTITY_OK &&
+              kIdentityPastContig == DCB_IDENTITY_PAST_CONTIG && kIdentitySkipOp == DCB_IDENTITY_SKIP_OP &&
+              kIdentityBorderline == DCB_IDENTITY_BORDERLINE && kIdentityBadInput == DCB_IDENTITY_BAD_INPUT,
+              "the kernel writes the ABI's status codes");
+
+int dcb_read_identity(dcb_engine* e, const dcb_identity_input* in, int64_t* counts, double* avg_q, int32_t* status,
+                      float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  if (ms_out) *ms_out = 0.f;
+  if (!in || !counts || !avg_q || !status) return fail(e, DCB_ERR_INVALID, "dcb_read_identity: null argument");
+  if (in->n_reads < 0 || in->n_cigar < 0 || in->n_bases < 0 || in->ref_count < 0 || in->contig_length < 0 ||
+      in->n_bases > INT32_MAX || in->n_cigar > INT32_MAX)
+    return fail(e, DCB_ERR_INVALID, "dcb_read_identity: bad sizes");
+  if ((in->n_reads && (!in->read_meta || (in->n_cigar && !in->cigar) || (in->n_bases && (!in->seq || !in->qual)))) ||
+      (in->ref_count && !in->ref_bases))
+    return fail(e, DCB_ERR_INVALID, "dcb_read_identity: null array");
+  int rc;
+  for (int32_t r = 0; r < in->n_reads; ++r)
+    if ((rc = check_aligned_read(e, "dcb_read_identity", r, in->read_meta, in->cigar, in->n_cigar, in->n_bases))) return rc;
+  auto& ri = e->ri;
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  const int32_t* d_meta;
+  const uint32_t* d_cigar;
+  const uint8_t *d_seq, *d_qual, *d_ref;
+  Output<long long> o_counts;
+  Output<double> o_avg;
+  Output<int32_t> o_status;
+  const size_t n = (size_t)in->n_reads;
+  if ((rc = stage_in(e, ri.meta, in->read_meta, n * DCB_CALIB_META, false, &d_meta)) ||
+      (rc = stage_in(e, ri.cigar, in->cigar, (size_t)in->n_cigar, false, &d_cigar)) ||
+      (rc = stage_in(e, ri.seq, in->seq, (size_t)in->n_bases, false, &d_seq)) ||
+      (rc = stage_in(e, ri.qual, in->qual, (size_t)in->n_bases, false, &d_qual)) ||
+      (rc = stage_in(e, ri.ref, in->ref_bases, (size_t)in->ref_count, false, &d_ref)) ||
+      (rc = stage_out(e, ri.counts, reinterpret_cast<long long*>(counts), n * kIdentityCounts, false, &o_counts)) ||
+      (rc = stage_out(e, ri.avg_q, avg_q, n, false, &o_avg)) || (rc = stage_out(e, ri.status, status, n, false, &o_status)))
+    return rc;
+  IdentityBatch c{d_meta, d_cigar, d_seq, d_qual, in->n_reads, d_ref, in->ref_start, in->ref_count, in->contig_length,
+                  e->d_p10.p};
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  launch_read_identity(c, o_counts.d, o_avg.d, o_status.d, st);
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  if ((rc = copy_out(e, o_counts)) || (rc = copy_out(e, o_avg)) || (rc = copy_out(e, o_status))) return rc;
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
   return DCB_OK;
 }

@@ -160,6 +160,23 @@ struct CalibBatch {
 };
 void launch_calib_count(const CalibBatch& c, int grid, long long* partial, long long* partial_fail, long long* out,
                         cudaStream_t st);
+// ---- read identity (calib_kernels.cu, dcb_read_identity), one CTA per read of a batch validated as for the
+// calibration counts.  counts: int64 [n_reads][kIdentityCounts] = matches, mismatches, insertions, deletions,
+// soft-clipped bases; avg_q [n_reads]; status [n_reads] = kIdentity*.
+constexpr int kIdentityCounts = 5;
+constexpr int kIdentityOk = 0, kIdentityPastContig = 1, kIdentitySkipOp = 2, kIdentityBorderline = 3,
+              kIdentityBadInput = 4;   // DCB_IDENTITY_*
+struct IdentityBatch {
+  const int32_t* read_meta;   // [n_reads][kCalibMeta]
+  const uint32_t* cigar;
+  const uint8_t* seq;
+  const uint8_t* qual;
+  int n_reads;
+  const uint8_t* ref;         // the contig's bases [ref_start, ref_start + ref_count)
+  int64_t ref_start, ref_count, contig_length;
+  const double* p10;          // 10^(-q/10), q = 0..255
+};
+void launch_read_identity(const IdentityBatch& c, long long* counts, double* avg_q, int32_t* status, cudaStream_t st);
 // the CCS ids / qualities of windows list[0..n_list) at full width, window j at off[j] of ccs_ids / ccs_bq
 void launch_features_ccs(const PrepBatch& b, const int4* window, const int32_t* list, int n_list, const int64_t* off,
                          uint8_t* ccs_ids, int16_t* ccs_bq, cudaStream_t st);

@@ -53,16 +53,11 @@ read_outcome_kernel(const uint8_t* __restrict__ qual, const int32_t* __restrict_
   else if (n == 0) code = DCB_READ_ONLY_GAPS;
   else {
     // quality_string_to_array subtracts 33; entries < 0 are dropped by avg_phred (none can be: chars >= '!')
-    int nonzero = 0, cnt = 0;
-    double s = 0.0;
-    for (int c = 33; c < 256; ++c)
-      if (s_hist[c]) { cnt += s_hist[c]; if (c > 33) nonzero = 1; s += (double)s_hist[c] * p10[c - 33]; }
-    if (nonzero && cnt > 0) avg_q = -10.0 * log10(s / (double)cnt);
-    const double thr = min_quality - 5e-6;                 // round(avg_q, 5) >= min_quality
+    avg_q = avg_phred_hist(s_hist + 33, 256 - 33, p10);
     // within 1e-7 of the threshold the host re-evaluates with the reference's NumPy expression: the read is treated
     // as passing the quality filter here (its record is written) and flagged
-    const bool border = fabs(avg_q - thr) < 1e-7;
-    const bool pass_q = border || avg_q >= thr;
+    bool border;
+    const bool pass_q = phred_passes(avg_q, min_quality, &border) || border;
     code = !pass_q ? DCB_READ_LOW_QUALITY : (n < min_length ? DCB_READ_TOO_SHORT : DCB_READ_OK);
     if (border) code |= DCB_READ_BORDERLINE;
   }

@@ -38,4 +38,23 @@ __device__ __forceinline__ int ccs_quality(int q, int calib_enabled, double thr,
   return (int)fmin(qd, (double)max_q);                     // np.minimum, then truncation
 }
 
+// avg_phred (utils.py:88-106) of a read from its quality histogram: hist[q] bases of Phred q, q = 0..n_q-1, and
+// p10[q] = 10^(-q/10) from the host's libm pow.  0 when no quality is above 0.  The exact integer counts times the
+// table give a float64 mean that can differ from NumPy's pairwise sum in the last bits (see phred_passes).
+__device__ __forceinline__ double avg_phred_hist(const int* hist, int n_q, const double* p10) {
+  int nonzero = 0, cnt = 0;
+  double s = 0.0;
+  for (int q = 0; q < n_q; ++q)
+    if (hist[q]) { cnt += hist[q]; if (q > 0) nonzero = 1; s += (double)hist[q] * p10[q]; }
+  return nonzero && cnt > 0 ? -10.0 * log10(s / (double)cnt) : 0.0;
+}
+
+// round(avg_q, 5) >= min_quality (stitch_utils.py:101-109) for a device avg_q.  *border is set when avg_q lies within
+// 1e-7 of the threshold: there the last bits decide, and the host re-evaluates the read with NumPy.
+__device__ __forceinline__ bool phred_passes(double avg_q, double min_quality, bool* border) {
+  const double thr = min_quality - 5e-6;
+  *border = fabs(avg_q - thr) < 1e-7;
+  return avg_q >= thr;
+}
+
 }  // namespace dcb

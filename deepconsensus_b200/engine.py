@@ -45,6 +45,10 @@ DCB_BAND_WIDTH_NONE = -1
 # dcb_calib_count: per-read meta columns, quality bins, and the kinds of failure it reports
 CALIB_META, CALIB_BINS = 6, 100
 DCB_CALIB_PAST_CONTIG, DCB_CALIB_BAD_QUALITY, DCB_CALIB_BAD_INPUT = 1, 2, 3
+# dcb_read_identity: per-read counts (matches, mismatches, insertions, deletions, soft clips) and status codes
+IDENTITY_COUNTS = 5
+(DCB_IDENTITY_OK, DCB_IDENTITY_PAST_CONTIG, DCB_IDENTITY_SKIP_OP, DCB_IDENTITY_BORDERLINE,
+ DCB_IDENTITY_BAD_INPUT) = range(5)
 DCB_LOGIT_LOSS_MSE, DCB_LOGIT_LOSS_KL = 0, 1
 # Keras loss identifiers (tf.keras.losses.get) of the two logit losses DistillationLoss is used with
 LOGIT_LOSS_IDS = {"mean_squared_error": DCB_LOGIT_LOSS_MSE, "mse": DCB_LOGIT_LOSS_MSE, "MSE": DCB_LOGIT_LOSS_MSE,
@@ -118,6 +122,15 @@ class DcbCalibInput(ctypes.Structure):
               ("reserved", ctypes.c_int32), ("threshold", ctypes.c_double), ("w", ctypes.c_double), ("b", ctypes.c_double)]
 
 
+class DcbIdentityInput(ctypes.Structure):
+  """dcb_identity_input: one batch of aligned reads and the reference bases they cover (include/dcb200.h "read
+  identity")."""
+  _fields_ = [("n_reads", ctypes.c_int32), ("reserved", ctypes.c_int32), ("n_cigar", ctypes.c_int64),
+              ("n_bases", ctypes.c_int64), ("read_meta", ctypes.c_void_p), ("cigar", ctypes.c_void_p),
+              ("seq", ctypes.c_void_p), ("qual", ctypes.c_void_p), ("ref_bases", ctypes.c_void_p),
+              ("ref_start", ctypes.c_int64), ("ref_count", ctypes.c_int64), ("contig_length", ctypes.c_int64)]
+
+
 # Every symbol include/dcb200.h declares; tests check the built library exports all of them.
 ABI_SYMBOLS = (
     "dcb_create", "dcb_load_weights", "dcb_forward", "dcb_submit", "dcb_wait", "dcb_stitch", "dcb_last_forward_ms",
@@ -130,7 +143,7 @@ ABI_SYMBOLS = (
     "dcb_features_layout_smart", "dcb_features_ccs", "dcb_prep_get_window_lengths", "dcb_prep_open_truth",
     "dcb_prep_get_label", "dcb_features_labels", "dcb_features_eval",
     "dcb_calib_open", "dcb_calib_contigs", "dcb_calib_fetch_reference", "dcb_calib_query", "dcb_calib_next_batch",
-    "dcb_calib_get_batch", "dcb_calib_read_name", "dcb_calib_close", "dcb_calib_count",
+    "dcb_calib_get_batch", "dcb_calib_read_name", "dcb_calib_close", "dcb_calib_count", "dcb_read_identity",
     "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
     "dcb_last_forward_launches", "dcb_set_profile", "dcb_get_profile", "dcb_get_profile_kernels", "dcb_alloc_host",
     "dcb_free_host", "dcb_alloc_device", "dcb_free_device", "dcb_memcpy_h2d", "dcb_memcpy_d2h",
@@ -208,6 +221,7 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_features_eval.argtypes = [vp, ctypes.POINTER(DcbLabels), vp, i32, i32, vp, vp, vp, vp, vp, vp, ctypes.POINTER(i32),
                                     ctypes.POINTER(ctypes.c_float)]
   lib.dcb_calib_count.argtypes = [vp, ctypes.POINTER(DcbCalibInput), vp, vp, ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_read_identity.argtypes = [vp, ctypes.POINTER(DcbIdentityInput), vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_launches.argtypes = [vp, ctypes.POINTER(i32)]
   lib.dcb_set_debug.argtypes = [vp, i32]
@@ -797,6 +811,26 @@ class B200Model:
     counts, failure, ms = np.zeros((CALIB_BINS, 2), np.int64), np.zeros(3, np.int64), ctypes.c_float(0)
     self._check(self._lib.dcb_calib_count(self._handle, ctypes.byref(arg), _ptr(counts), _ptr(failure), ctypes.byref(ms)))
     return dict(counts=counts, failure=tuple(int(x) for x in failure), ms=float(ms.value))
+
+  def read_identity(self, batch: Dict[str, np.ndarray], ref: np.ndarray, ref_start: int,
+                    contig_length: int) -> Dict[str, Any]:
+    """dcb_read_identity: per read of one batch (dict of read_meta int32 [n, CALIB_META], cigar uint32, seq uint8 4-bit
+    codes, qual uint8) against `ref`, the contig's bases [ref_start, ref_start + len(ref)) as uint8 characters.
+    Returns dict(counts int64 [n, IDENTITY_COUNTS] (matches, mismatches, insertions, deletions, soft clips), avg_q
+    float64 [n], status int32 [n] (DCB_IDENTITY_*), ms)."""
+    meta = np.ascontiguousarray(batch["read_meta"], np.int32).reshape(-1, CALIB_META)
+    cig, seq, qual = (np.ascontiguousarray(batch[k], dt) for k, dt in (("cigar", np.uint32), ("seq", np.uint8),
+                                                                       ("qual", np.uint8)))
+    ref = np.ascontiguousarray(ref, np.uint8)
+    n = len(meta)
+    arg = DcbIdentityInput(n_reads=n, n_cigar=cig.size, n_bases=seq.size, read_meta=_ptr(meta), cigar=_ptr(cig),
+                           seq=_ptr(seq), qual=_ptr(qual), ref_bases=_ptr(ref), ref_start=int(ref_start),
+                           ref_count=ref.size, contig_length=int(contig_length))
+    counts, avg_q, status = np.zeros((n, IDENTITY_COUNTS), np.int64), np.zeros(n, np.float64), np.zeros(n, np.int32)
+    ms = ctypes.c_float(0)
+    self._check(self._lib.dcb_read_identity(self._handle, ctypes.byref(arg), _ptr(counts), _ptr(avg_q), _ptr(status),
+                                            ctypes.byref(ms)))
+    return dict(counts=counts, avg_q=avg_q, status=status, ms=float(ms.value))
 
   def stitch_raw(self, bases_ptr: int, quals_ptr: int, n_windows: int, zmw_start: np.ndarray, flags: int,
                  seq_ptr: int, qual_ptr: int, len_ptr: int, length: Optional[int] = None) -> None:

@@ -578,6 +578,39 @@ typedef struct dcb_calib_input {
 } dcb_calib_input;
 int dcb_calib_count(dcb_engine* e, const dcb_calib_input* in, int64_t* counts, int64_t* failure, float* ms_out);
 
+/* ---- read identity (read_yield.py) --------------------------------------------------------------------------------------
+ * dcb_read_identity walks every read of a batch from dcb_calib_get_batch against the truth assembly on the device and
+ * returns per read, in counts int64 [n_reads][5]: matches, mismatches, insertions, deletions and soft-clipped bases.
+ * An M, = or X base is a match when it equals the upper-cased reference base and both are A, C, G or T, else a
+ * mismatch; I, D and S count their lengths; H and P count nothing.  avg_q [n_reads] receives avg_phred of the read's
+ * qualities (float64, an exact histogram times the engine's 10^(-q/10) table from the host's libm pow), and status
+ * [n_reads] one DCB_IDENTITY_* code:
+ *   OK          the counts are valid;
+ *   PAST_CONTIG the read has a reference base at or past contig_length: it is not counted (counts 0);
+ *   SKIP_OP     the cigar has an N operation, which has no meaning for identity (counts 0);
+ *   BORDERLINE  as OK, but avg_q lies within 1e-7 of q - 5e-6 for an integer q, where round(avg_q, 5) >= q turns: the
+ *               caller re-decides the quality filter with NumPy's own sum;
+ *   BAD_INPUT   ref_bases do not cover one of the read's bases inside the contig (counts 0).
+ * ref_bases (host) are the contig's bases [ref_start, ref_start + ref_count).  ms_out (nullable): device time of the
+ * kernel.  The results do not depend on how the reads are split into batches; there are no global atomics. */
+#define DCB_IDENTITY_COUNTS 5
+#define DCB_IDENTITY_OK 0
+#define DCB_IDENTITY_PAST_CONTIG 1
+#define DCB_IDENTITY_SKIP_OP 2
+#define DCB_IDENTITY_BORDERLINE 3
+#define DCB_IDENTITY_BAD_INPUT 4
+typedef struct dcb_identity_input {
+  int32_t n_reads, reserved;
+  int64_t n_cigar, n_bases;
+  const int32_t* read_meta;        /* [n_reads, DCB_CALIB_META] */
+  const uint32_t* cigar;           /* [n_cigar] */
+  const uint8_t *seq, *qual;       /* [n_bases] */
+  const uint8_t* ref_bases;        /* [ref_count] */
+  int64_t ref_start, ref_count, contig_length;
+} dcb_identity_input;
+int dcb_read_identity(dcb_engine* e, const dcb_identity_input* in, int64_t* counts, double* avg_q, int32_t* status,
+                      float* ms_out);
+
 /* Device time of the last dcb_forward (milliseconds, CUDA events on the engine's stream). */
 int dcb_last_forward_ms(dcb_engine* e, float* ms);
 /* Number of engine kernels launched by the last dcb_forward. */
