@@ -28,6 +28,7 @@
 #include <condition_variable>
 #include <deque>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -1674,5 +1675,217 @@ const char* dcb_calib_read_name(dcb_calib* p, int64_t i) {
   if (!p || i < 0 || i >= (int64_t)p->names.size()) return "";
   return p->names[(size_t)i].c_str();
 }
+
+}  // extern "C"
+
+// ----------------------------------------------------------------------------------------------- sequence reader
+// The host side of `kmer_qv` (include/dcb200.h "k-mer QV"): the reads of one FASTA, FASTQ or BAM file, in file order,
+// exported in batches of concatenated bases, Phred qualities and offsets.  The format comes from the content: a BGZF
+// stream that inflates to "BAM\1" is a BAM, anything else is read through zlib's gz* reader (plain or gzip text), where
+// '>' starts a FASTA file and '@' a FASTQ file.
+struct dcb_seq_reader {
+  std::string path;
+  bool bam_mode = false, fastq = false, done = false;
+  BamReader bam;
+  gzFile gz = nullptr;
+  std::vector<char> buf;
+  size_t at = 0, got = 0;
+  bool eof = false;
+  std::string pending;              // FASTA: the header line that starts the next record
+  int64_t line_no = 0;
+  // the current batch
+  std::vector<uint8_t> seq, qual, has_qual;
+  std::vector<int64_t> off;
+  std::vector<std::string> names;
+  ~dcb_seq_reader() { if (gz) gzclose(gz); }
+
+  // One line without its newline (and '\r'): 1 = line, 0 = end of the file, < 0 = error.  A gzip stream that is
+  // corrupt (a bad CRC or bad data) or ends before its end is an error, never a shorter file.
+  int getline(std::string* line) {
+    line->clear();
+    bool any = false;
+    for (;;) {
+      if (at == got) {
+        if (eof) break;
+        const int n = gzread(gz, buf.data(), (unsigned)buf.size());
+        if (n <= 0) {
+          int err = Z_OK;
+          const char* msg = gzerror(gz, &err);
+          if (n < 0 || err != Z_OK)
+            return pfail(DCB_ERR_INVALID, "%s: cannot read past line %lld: %s", path.c_str(), (long long)line_no,
+                         msg && *msg ? msg : "read error");
+          eof = true;
+          break;
+        }
+        at = 0; got = (size_t)n;
+      }
+      any = true;
+      const char* s = buf.data() + at;
+      const char* nl = static_cast<const char*>(memchr(s, '\n', got - at));
+      if (nl) { line->append(s, nl - s); at += (nl - s) + 1; break; }
+      line->append(s, got - at);
+      at = got;
+    }
+    if (!any) return 0;
+    ++line_no;
+    if (!line->empty() && line->back() == '\r') line->pop_back();
+    return 1;
+  }
+};
+
+namespace {
+
+std::string header_name(const std::string& line) {
+  size_t k = 1;
+  while (k < line.size() && !isspace((unsigned char)line[k])) ++k;
+  return line.substr(1, k - 1);
+}
+
+void append_bases(dcb_seq_reader* p, const char* s, size_t n) {
+  for (size_t i = 0; i < n; ++i) p->seq.push_back((uint8_t)toupper((unsigned char)s[i]));
+}
+
+// The next record of a text file into the batch: 1 = record, 0 = end of file, < 0 = error.
+int next_text_record(dcb_seq_reader* p) {
+  std::string line;
+  int rc;
+  if (p->fastq) {
+    do { if ((rc = p->getline(&line)) <= 0) return rc; } while (line.empty());
+    if (line[0] != '@') return pfail(DCB_ERR_INVALID, "%s:%lld: a FASTQ record must start with '@'", p->path.c_str(), (long long)p->line_no);
+    const std::string name = header_name(line);
+    std::string s, plus, q;
+    for (std::string* l : {&s, &plus, &q}) {
+      if ((rc = p->getline(l)) < 0) return rc;
+      if (rc == 0 || (l == &plus && (plus.empty() || plus[0] != '+')))
+        return pfail(DCB_ERR_INVALID, "%s: FASTQ record %s is truncated", p->path.c_str(), name.c_str());
+    }
+    if (q.size() != s.size())
+      return pfail(DCB_ERR_INVALID, "%s: FASTQ record %s has %zu bases and %zu qualities", p->path.c_str(), name.c_str(),
+                   s.size(), q.size());
+    append_bases(p, s.data(), s.size());
+    for (char c : q) {
+      if ((unsigned char)c < 33 || (unsigned char)c > 126)
+        return pfail(DCB_ERR_INVALID, "%s: FASTQ record %s has a quality character outside '!'..'~'", p->path.c_str(), name.c_str());
+      p->qual.push_back((uint8_t)(c - 33));
+    }
+    p->names.push_back(name);
+    p->has_qual.push_back(1);
+    return 1;
+  }
+  if (p->pending.empty()) {
+    do { if ((rc = p->getline(&line)) <= 0) return rc; } while (line.empty());
+    if (line[0] != '>') return pfail(DCB_ERR_INVALID, "%s:%lld: a FASTA record must start with '>'", p->path.c_str(), (long long)p->line_no);
+    p->pending = line;
+  }
+  p->names.push_back(header_name(p->pending));
+  p->pending.clear();
+  while ((rc = p->getline(&line)) > 0) {
+    if (!line.empty() && line[0] == '>') { p->pending = line; break; }
+    append_bases(p, line.data(), line.size());
+  }
+  if (rc < 0) return rc;
+  p->qual.resize(p->seq.size(), 0);
+  p->has_qual.push_back(0);
+  return 1;
+}
+
+// The next record of a BAM file into the batch: secondary and supplementary records are skipped.
+int next_bam_record(dcb_seq_reader* p) {
+  BamRecord r;
+  for (;;) {
+    const int rc = p->bam.next(&r);
+    if (rc < 0) return pfail(DCB_ERR_INVALID, "%s: %s", p->path.c_str(), g_prep_error.c_str());
+    if (rc == 0) return 0;
+    if (!(r.flag & (0x100 | 0x800))) break;
+  }
+  if (r.seq.empty()) return pfail(DCB_ERR_INVALID, "%s: read %s has no SEQ", p->path.c_str(), r.qname.c_str());
+  append_bases(p, r.seq.data(), r.seq.size());
+  const bool q = r.qual[0] != 0xff;
+  if (q) p->qual.insert(p->qual.end(), r.qual.begin(), r.qual.end());
+  else p->qual.resize(p->seq.size(), 0);
+  p->names.push_back(r.qname);
+  p->has_qual.push_back(q ? 1 : 0);
+  return 1;
+}
+
+}  // namespace
+
+extern "C" {
+
+int dcb_seq_open(const char* path, dcb_seq_reader** out) {
+  if (!path || !out) return pfail(DCB_ERR_INVALID, "dcb_seq_open: null argument");
+  *out = nullptr;
+  std::unique_ptr<dcb_seq_reader> p(new dcb_seq_reader());
+  p->path = path;
+  FILE* f = fopen(path, "rb");
+  if (!f) return pfail(DCB_ERR_INVALID, "cannot open %s", path);
+  uint8_t magic[4] = {0, 0, 0, 0};
+  const size_t n = fread(magic, 1, 4, f);
+  fclose(f);
+  if (n == 4 && magic[0] == 31 && magic[1] == 139 && (magic[3] & 4)) {   // BGZF: BAM or a bgzipped text file
+    gzFile g = gzopen(path, "rb");
+    char head[4] = {0, 0, 0, 0};
+    const bool is_bam = g && gzread(g, head, 4) == 4 && memcmp(head, "BAM\1", 4) == 0;
+    if (g) gzclose(g);
+    if (is_bam) {
+      p->bam_mode = true;
+      const int rc = p->bam.open(path);
+      if (rc) return rc;
+      *out = p.release();
+      return DCB_OK;
+    }
+  }
+  if (!(p->gz = gzopen(path, "rb"))) return pfail(DCB_ERR_INVALID, "cannot open %s", path);
+  p->buf.resize(1 << 20);
+  std::string line;
+  int rc;
+  while ((rc = p->getline(&line)) > 0 && line.empty()) {}
+  if (rc < 0) return rc;
+  if (line.empty()) { p->done = true; *out = p.release(); return DCB_OK; }   // an empty file holds no reads
+  if (line[0] == '@') {
+    p->fastq = true;
+    gzrewind(p->gz);
+    p->at = p->got = 0; p->eof = false; p->line_no = 0;
+  } else if (line[0] == '>') {
+    p->pending = line;
+  } else {
+    return pfail(DCB_ERR_INVALID, "%s is not a FASTA, FASTQ or BAM file", path);
+  }
+  *out = p.release();
+  return DCB_OK;
+}
+
+int dcb_seq_next_batch(dcb_seq_reader* p, int64_t max_bases, int64_t* sizes) {
+  if (!p || !sizes || max_bases < 1) return pfail(DCB_ERR_INVALID, "dcb_seq_next_batch: bad argument");
+  sizes[0] = sizes[1] = 0;
+  p->seq.clear(); p->qual.clear(); p->has_qual.clear(); p->names.clear();
+  p->off.assign(1, 0);
+  max_bases = std::min<int64_t>(max_bases, (int64_t)1 << 31);
+  while (!p->done && (int64_t)p->seq.size() < max_bases) {
+    const int rc = p->bam_mode ? next_bam_record(p) : next_text_record(p);
+    if (rc < 0) return rc;
+    if (rc == 0) { p->done = true; break; }
+    p->off.push_back((int64_t)p->seq.size());
+  }
+  sizes[0] = (int64_t)p->names.size();
+  sizes[1] = (int64_t)p->seq.size();
+  return sizes[0] ? 1 : 0;
+}
+
+int dcb_seq_get_batch(dcb_seq_reader* p, uint8_t* bases, uint8_t* qual, int64_t* offsets, uint8_t* has_qual) {
+  if (!p) return pfail(DCB_ERR_INVALID, "dcb_seq_get_batch: null handle");
+  if (bases && !p->seq.empty()) memcpy(bases, p->seq.data(), p->seq.size());
+  if (qual && !p->qual.empty()) memcpy(qual, p->qual.data(), p->qual.size());
+  if (offsets) memcpy(offsets, p->off.data(), p->off.size() * sizeof(int64_t));
+  if (has_qual && !p->has_qual.empty()) memcpy(has_qual, p->has_qual.data(), p->has_qual.size());
+  return DCB_OK;
+}
+
+const char* dcb_seq_read_name(dcb_seq_reader* p, int64_t i) {
+  if (!p || i < 0 || i >= (int64_t)p->names.size()) return "";
+  return p->names[(size_t)i].c_str();
+}
+
+void dcb_seq_close(dcb_seq_reader* p) { delete p; }
 
 }  // extern "C"

@@ -21,10 +21,11 @@ build_one() {   # $1 = output .so, $2 = extra flags
   $NVCC $flags -c eval_kernels.cu -o $tag.eval.o & pids+=($!)
   $NVCC $flags -c prep_kernels.cu -o $tag.prep.o & pids+=($!)
   $NVCC $flags -c calib_kernels.cu -o $tag.calib.o & pids+=($!)
+  $NVCC $flags -c kmer_kernels.cu -o $tag.kmer.o & pids+=($!)
   $NVCC $flags -Xcompiler -fvisibility=default -c bam_prep.cpp -o $tag.bam.o & pids+=($!)
   $NVCC $flags -Xcompiler -fvisibility=default -c engine.cu -o $tag.engine.o & pids+=($!)
   for p in "${pids[@]}"; do wait $p; done     # a failed compile fails the build (set -e)
-  $NVCC -gencode arch=compute_90a,code=sm_90a -shared -o $out $tag.kernels.o $tag.strict.o $tag.tf32x3.o $tag.post.o $tag.eval.o $tag.prep.o $tag.calib.o $tag.bam.o $tag.engine.o -lz -Xlinker -soname=$out
+  $NVCC -gencode arch=compute_90a,code=sm_90a -shared -o $out $tag.kernels.o $tag.strict.o $tag.tf32x3.o $tag.post.o $tag.eval.o $tag.prep.o $tag.calib.o $tag.kmer.o $tag.bam.o $tag.engine.o -lz -Xlinker -soname=$out
   echo "built $(pwd)/$out"
 }
 

@@ -222,6 +222,24 @@ struct dcb_engine {
     DevBuf<long long> counts;
     DevBuf<double> avg_q;
   } ri;
+  struct {   // dcb_kmer_*: the k-mer table and two pipeline slots of staged batches and per-read outputs
+    DevBuf<unsigned long long> keys, stats, hist_partial, hist;
+    DevBuf<unsigned int> counts;
+    unsigned long long capacity = 0;
+    int k = 0, partition = 0, n_partitions = 1;
+    struct Slot {
+      DevBuf<uint8_t> bases, qual, has_qual;
+      DevBuf<int64_t> offsets;
+      DevBuf<int32_t> seg_read, seg_first;
+      std::vector<int32_t> h_seg_read, h_seg_first;   // kept until the slot is reused: the copies read them
+      DevBuf<long long> counts, partial;
+      DevBuf<double> avg_q;
+      DevBuf<int32_t> border;
+      cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+      int n_reads = 0;
+      bool query = false, quality = false;
+    } slot[2];
+  } km;
   cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;   // around the kernel of dcb_evaluate / _distill_loss / _loss_grad
 
   // Safe on a partly built engine.  The caller has made cfg.device current; the DevBuf members free themselves after
@@ -229,7 +247,7 @@ struct dcb_engine {
   ~dcb_engine() {
     for (cudaStream_t s : {copy_stream, stream, out_stream})
       if (s) cudaStreamSynchronize(s);
-    std::vector<cudaEvent_t> events = {ev_eval0, ev_eval1};
+    std::vector<cudaEvent_t> events = {ev_eval0, ev_eval1, km.slot[0].ev0, km.slot[0].ev1, km.slot[1].ev0, km.slot[1].ev1};
     for (Slot& sl : slots) {
       events.insert(events.end(), {sl.rows_ready, sl.ev0, sl.ev1, sl.done});
       for (const ProfRegion& r : sl.prof) events.insert(events.end(), {r.start, r.end});
@@ -2214,6 +2232,185 @@ int dcb_read_identity(dcb_engine* e, const dcb_identity_input* in, int64_t* coun
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  return DCB_OK;
+}
+
+static_assert(kKmerHist == DCB_KMER_HIST && kKmerStatSlots + 1 == DCB_KMER_STATS, "the ABI's k-mer table sizes");
+
+int dcb_kmer_table_init(dcb_engine* e, int64_t table_bytes, int32_t k, int64_t* capacity) {
+  if (!e) return DCB_ERR_INVALID;
+  if (k < 1 || k > 31) return fail(e, DCB_ERR_INVALID, "dcb_kmer_table_init: k must be between 1 and 31, got %d", k);
+  auto& km = e->km;
+  CU(e, cudaSetDevice(e->cfg.device));
+  CU(e, cudaStreamSynchronize(e->stream));
+  km.keys.reset(); km.counts.reset(); km.capacity = 0;
+  if (table_bytes <= 0) {
+    size_t free_b = 0, total_b = 0;
+    CU(e, cudaMemGetInfo(&free_b, &total_b));
+    table_bytes = (int64_t)(free_b / 2);
+  }
+  constexpr int64_t kSlotBytes = sizeof(unsigned long long) + sizeof(unsigned int);
+  unsigned long long cap = 64;
+  while (cap < (1ull << 32) && (int64_t)(2 * cap) * kSlotBytes <= table_bytes) cap *= 2;
+  if ((int64_t)cap * kSlotBytes > table_bytes)
+    return fail(e, DCB_ERR_INVALID, "dcb_kmer_table_init: %lld bytes hold fewer than 64 slots", (long long)table_bytes);
+  for (auto& sl : km.slot)
+    for (cudaEvent_t* ev : {&sl.ev0, &sl.ev1})
+      if (!*ev) CU(e, cudaEventCreate(ev));
+  int rc;
+  if ((rc = ensure(e, km.keys, cap)) || (rc = ensure(e, km.counts, cap)) || (rc = ensure(e, km.stats, kKmerStatSlots)) ||
+      (rc = ensure(e, km.hist, kKmerHist + 1)) ||
+      (rc = ensure(e, km.hist_partial, (size_t)kmer_hist_grid(cap) * (kKmerHist + 1))))
+    return rc;
+  km.capacity = cap;
+  km.k = k;
+  if (capacity) *capacity = (int64_t)cap;
+  return dcb_kmer_table_clear(e, 0, 1);
+}
+
+int dcb_kmer_table_clear(dcb_engine* e, int32_t partition, int32_t n_partitions) {
+  if (!e) return DCB_ERR_INVALID;
+  auto& km = e->km;
+  if (!km.capacity) return fail(e, DCB_ERR_STATE, "dcb_kmer_table_clear: no table (dcb_kmer_table_init)");
+  if (n_partitions < 1 || partition < 0 || partition >= n_partitions)
+    return fail(e, DCB_ERR_INVALID, "dcb_kmer_table_clear: partition %d of %d", partition, n_partitions);
+  CU(e, cudaSetDevice(e->cfg.device));
+  CU(e, cudaMemsetAsync(km.keys.p, 0xff, km.capacity * sizeof(unsigned long long), e->stream));   // every key empty
+  CU(e, cudaMemsetAsync(km.counts.p, 0, km.capacity * sizeof(unsigned int), e->stream));
+  CU(e, cudaMemsetAsync(km.stats.p, 0, kKmerStatSlots * sizeof(unsigned long long), e->stream));
+  CU(e, cudaStreamSynchronize(e->stream));
+  km.partition = partition;
+  km.n_partitions = n_partitions;
+  return DCB_OK;
+}
+
+namespace {
+
+// Stages one batch into pipeline slot `slot`: the bases and offsets, and with `quality` the qualities and flags.
+int kmer_stage(dcb_engine* e, const char* who, const dcb_kmer_batch* b, int32_t slot, bool quality, KmerBatch* kb) {
+  auto& km = e->km;
+  if (!km.capacity) return fail(e, DCB_ERR_STATE, "%s: no table (dcb_kmer_table_init)", who);
+  if (!b || slot < 0 || slot > 1) return fail(e, DCB_ERR_INVALID, "%s: null batch or slot %d", who, slot);
+  if (b->n_reads < 0 || b->n_bases < 0) return fail(e, DCB_ERR_INVALID, "%s: bad sizes", who);
+  if (b->n_reads && (!b->offsets || (b->n_bases && !b->bases) || (quality && (!b->has_qual || (b->n_bases && !b->qual)))))
+    return fail(e, DCB_ERR_INVALID, "%s: null array", who);
+  if (b->n_reads) {
+    if (b->offsets[0] != 0 || b->offsets[b->n_reads] != b->n_bases)
+      return fail(e, DCB_ERR_INVALID, "%s: offsets must run from 0 to n_bases", who);
+    for (int32_t r = 0; r < b->n_reads; ++r)
+      if (b->offsets[r + 1] < b->offsets[r]) return fail(e, DCB_ERR_INVALID, "%s: offsets decrease at read %d", who, r);
+  }
+  auto& sl = km.slot[slot];
+  CU(e, cudaSetDevice(e->cfg.device));
+  const uint8_t *d_bases, *d_qual = nullptr, *d_has = nullptr;
+  const int64_t* d_off;
+  int rc;
+  if ((rc = stage_in(e, sl.bases, b->bases, (size_t)b->n_bases, false, &d_bases)) ||
+      (rc = stage_in(e, sl.offsets, b->offsets, (size_t)b->n_reads + 1, false, &d_off)) ||
+      (quality && ((rc = stage_in(e, sl.qual, b->qual, (size_t)b->n_bases, false, &d_qual)) ||
+                   (rc = stage_in(e, sl.has_qual, b->has_qual, (size_t)b->n_reads, false, &d_has)))))
+    return rc;
+  *kb = KmerBatch{d_bases, d_qual, d_off, d_has, b->n_reads, b->n_bases};
+  sl.n_reads = b->n_reads;
+  return DCB_OK;
+}
+
+KmerTable kmer_table(dcb_engine* e) {
+  auto& km = e->km;
+  return KmerTable{km.keys.p, km.counts.p, km.stats.p, km.capacity, km.k, km.partition, km.n_partitions};
+}
+
+}  // namespace
+
+int dcb_kmer_count(dcb_engine* e, const dcb_kmer_batch* b, int32_t slot) {
+  if (!e) return DCB_ERR_INVALID;
+  KmerBatch kb;
+  int rc = kmer_stage(e, "dcb_kmer_count", b, slot, false, &kb);
+  if (rc) return rc;
+  auto& sl = e->km.slot[slot];
+  sl.query = false;
+  CU(e, cudaEventRecord(sl.ev0, e->stream));
+  launch_kmer_count(kmer_table(e), kb, e->stream);
+  CU(e, cudaGetLastError());
+  CU(e, cudaEventRecord(sl.ev1, e->stream));
+  return DCB_OK;
+}
+
+int dcb_kmer_query(dcb_engine* e, const dcb_kmer_batch* b, int32_t min_count, int32_t with_quality, int32_t slot) {
+  if (!e) return DCB_ERR_INVALID;
+  if (min_count < 1) return fail(e, DCB_ERR_INVALID, "dcb_kmer_query: min_count must be at least 1, got %d", min_count);
+  KmerBatch kb;
+  int rc = kmer_stage(e, "dcb_kmer_query", b, slot, with_quality != 0, &kb);
+  if (rc) return rc;
+  auto& sl = e->km.slot[slot];
+  const size_t n = (size_t)std::max(b->n_reads, 1);
+  // one CTA per kKmerSegment k-mer end positions of a read, at least one per read
+  sl.h_seg_first.assign(1, 0);
+  sl.h_seg_read.clear();
+  for (int32_t r = 0; r < b->n_reads; ++r) {
+    const int64_t segs = std::max<int64_t>(1, (b->offsets[r + 1] - b->offsets[r] + kKmerSegment - 1) / kKmerSegment);
+    if ((int64_t)sl.h_seg_read.size() + segs > INT32_MAX)
+      return fail(e, DCB_ERR_INVALID, "dcb_kmer_query: the batch needs more than 2^31 segments");
+    sl.h_seg_read.insert(sl.h_seg_read.end(), (size_t)segs, r);
+    sl.h_seg_first.push_back((int32_t)sl.h_seg_read.size());
+  }
+  const size_t n_seg = sl.h_seg_read.size();
+  const int32_t *d_seg_read, *d_seg_first;
+  if ((rc = ensure(e, sl.counts, 2 * n)) || (rc = ensure(e, sl.avg_q, n)) || (rc = ensure(e, sl.border, n)) ||
+      (rc = ensure(e, sl.partial, 2 * std::max<size_t>(n_seg, 1))) ||
+      (rc = stage_in(e, sl.seg_read, sl.h_seg_read.data(), n_seg, false, &d_seg_read)) ||
+      (rc = stage_in(e, sl.seg_first, sl.h_seg_first.data(), sl.h_seg_first.size(), false, &d_seg_first)))
+    return rc;
+  sl.query = true;
+  sl.quality = with_quality != 0;
+  CU(e, cudaEventRecord(sl.ev0, e->stream));
+  launch_kmer_query(kmer_table(e), kb, KmerSegments{d_seg_read, d_seg_first, (int)n_seg}, (unsigned int)min_count,
+                    with_quality ? e->d_p10.p : nullptr, sl.partial.p, sl.counts.p, sl.avg_q.p, sl.border.p, e->stream);
+  CU(e, cudaGetLastError());
+  CU(e, cudaEventRecord(sl.ev1, e->stream));
+  return DCB_OK;
+}
+
+int dcb_kmer_wait(dcb_engine* e, int32_t slot, int64_t* counts, double* avg_q, int32_t* borderline, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  if (ms_out) *ms_out = 0.f;
+  if (slot < 0 || slot > 1 || !e->km.slot[slot].ev1) return fail(e, DCB_ERR_INVALID, "dcb_kmer_wait: bad slot %d", slot);
+  auto& sl = e->km.slot[slot];
+  CU(e, cudaSetDevice(e->cfg.device));
+  // The copies run on the output stream behind this slot's kernel only, so the other slot's kernel keeps running.
+  cudaStream_t os = e->out_stream;
+  CU(e, cudaStreamWaitEvent(os, sl.ev1, 0));
+  const size_t n = (size_t)sl.n_reads;
+  if (sl.query && n) {
+    if (counts) CU(e, cudaMemcpyAsync(counts, sl.counts.p, 2 * n * sizeof(long long), cudaMemcpyDeviceToHost, os));
+    if (sl.quality && avg_q) CU(e, cudaMemcpyAsync(avg_q, sl.avg_q.p, n * sizeof(double), cudaMemcpyDeviceToHost, os));
+    if (sl.quality && borderline)
+      CU(e, cudaMemcpyAsync(borderline, sl.border.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, os));
+  }
+  CU(e, cudaStreamSynchronize(os));
+  CU(e, cudaGetLastError());
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, sl.ev0, sl.ev1));
+  return DCB_OK;
+}
+
+int dcb_kmer_table_stats(dcb_engine* e, int64_t* stats, int64_t* histogram) {
+  if (!e) return DCB_ERR_INVALID;
+  auto& km = e->km;
+  if (!km.capacity) return fail(e, DCB_ERR_STATE, "dcb_kmer_table_stats: no table (dcb_kmer_table_init)");
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  unsigned long long s[kKmerStatSlots], h[kKmerHist + 1];
+  if (histogram) launch_kmer_histogram(kmer_table(e), km.hist_partial.p, kmer_hist_grid(km.capacity), km.hist.p, st);
+  CU(e, cudaGetLastError());
+  CU(e, cudaMemcpyAsync(s, km.stats.p, sizeof s, cudaMemcpyDeviceToHost, st));
+  if (histogram) CU(e, cudaMemcpyAsync(h, km.hist.p, sizeof h, cudaMemcpyDeviceToHost, st));
+  CU(e, cudaStreamSynchronize(st));
+  if (stats) {
+    stats[0] = (int64_t)km.capacity;
+    for (int i = 0; i < kKmerStatSlots; ++i) stats[i + 1] = (int64_t)s[i];
+  }
+  if (histogram)
+    for (int c = 0; c <= kKmerHist; ++c) histogram[c] = (int64_t)h[c];
   return DCB_OK;
 }
 

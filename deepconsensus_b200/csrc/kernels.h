@@ -177,6 +177,46 @@ struct IdentityBatch {
   const double* p10;          // 10^(-q/10), q = 0..255
 };
 void launch_read_identity(const IdentityBatch& c, long long* counts, double* avg_q, int32_t* status, cudaStream_t st);
+// ---- k-mer table (kmer_kernels.cu, dcb_kmer_*).  keys: capacity uint64 (kKmerEmpty = free), counts: capacity uint32,
+// capacity a power of two.  stats: uint64 [kKmerStatSlots] = claimed keys, overflow flag, k-mers counted, their probe
+// steps, k-mers queried, their probe steps.  Device pointers.
+constexpr unsigned long long kKmerEmpty = ~0ull;
+constexpr int kKmerStatSlots = 6;
+constexpr int kKmerHist = 256;   // DCB_KMER_HIST
+struct KmerTable {
+  unsigned long long* keys;
+  unsigned int* counts;
+  unsigned long long* stats;
+  unsigned long long capacity;
+  int k, partition, n_partitions;
+};
+struct KmerBatch {
+  const uint8_t* bases;
+  const uint8_t* qual;
+  const int64_t* offsets;      // [n_reads + 1]
+  const uint8_t* has_qual;
+  int n_reads;
+  int64_t n_bases;
+};
+void launch_kmer_count(const KmerTable& t, const KmerBatch& b, cudaStream_t st);
+// The query's CTAs: read r is segments first[r] .. first[r + 1] - 1 (at least one), each of kKmerSegment k-mer end
+// positions but the last; read[s] is segment s's read.
+constexpr int kKmerSegment = 16384;
+struct KmerSegments {
+  const int32_t* read;    // [n_segments]
+  const int32_t* first;   // [n_reads + 1]
+  int n_segments;
+};
+// per read: counts [2r] = k-mer positions of the partition, [2r + 1] = those with a count below min_count; with p10
+// (not null), avg_q [r] and borderline [r] as dcb_read_identity's avg_phred.  partial: 2 x n_segments entries.
+void launch_kmer_query(const KmerTable& t, const KmerBatch& b, const KmerSegments& sg, unsigned int min_count,
+                       const double* p10, long long* partial, long long* counts, double* avg_q, int32_t* borderline,
+                       cudaStream_t st);
+// hist [kKmerHist + 1]: [c] = keys with count c (c = 1..255), [kKmerHist] = keys with count >= 256; partial holds
+// grid x (kKmerHist + 1) entries, grid from kmer_hist_grid
+int kmer_hist_grid(unsigned long long capacity);
+void launch_kmer_histogram(const KmerTable& t, unsigned long long* partial, int grid, unsigned long long* hist,
+                           cudaStream_t st);
 // the CCS ids / qualities of windows list[0..n_list) at full width, window j at off[j] of ccs_ids / ccs_bq
 void launch_features_ccs(const PrepBatch& b, const int4* window, const int32_t* list, int n_list, const int64_t* off,
                          uint8_t* ccs_ids, int16_t* ccs_bq, cudaStream_t st);

@@ -49,6 +49,9 @@ DCB_CALIB_PAST_CONTIG, DCB_CALIB_BAD_QUALITY, DCB_CALIB_BAD_INPUT = 1, 2, 3
 IDENTITY_COUNTS = 5
 (DCB_IDENTITY_OK, DCB_IDENTITY_PAST_CONTIG, DCB_IDENTITY_SKIP_OP, DCB_IDENTITY_BORDERLINE,
  DCB_IDENTITY_BAD_INPUT) = range(5)
+# dcb_kmer_table_stats: its stats entries and the count histogram's last bin (counts >= DCB_KMER_HIST)
+KMER_STAT_KEYS = ("capacity", "claimed", "overflow", "count_kmers", "count_probes", "query_kmers", "query_probes")
+KMER_HIST = 256
 DCB_LOGIT_LOSS_MSE, DCB_LOGIT_LOSS_KL = 0, 1
 # Keras loss identifiers (tf.keras.losses.get) of the two logit losses DistillationLoss is used with
 LOGIT_LOSS_IDS = {"mean_squared_error": DCB_LOGIT_LOSS_MSE, "mse": DCB_LOGIT_LOSS_MSE, "MSE": DCB_LOGIT_LOSS_MSE,
@@ -131,6 +134,13 @@ class DcbIdentityInput(ctypes.Structure):
               ("ref_start", ctypes.c_int64), ("ref_count", ctypes.c_int64), ("contig_length", ctypes.c_int64)]
 
 
+class DcbKmerBatch(ctypes.Structure):
+  """dcb_kmer_batch: one batch of concatenated sequences (include/dcb200.h "k-mer QV")."""
+  _fields_ = [("n_reads", ctypes.c_int32), ("reserved", ctypes.c_int32), ("n_bases", ctypes.c_int64),
+              ("bases", ctypes.c_void_p), ("qual", ctypes.c_void_p), ("offsets", ctypes.c_void_p),
+              ("has_qual", ctypes.c_void_p)]
+
+
 # Every symbol include/dcb200.h declares; tests check the built library exports all of them.
 ABI_SYMBOLS = (
     "dcb_create", "dcb_load_weights", "dcb_forward", "dcb_submit", "dcb_wait", "dcb_stitch", "dcb_last_forward_ms",
@@ -144,6 +154,9 @@ ABI_SYMBOLS = (
     "dcb_prep_get_label", "dcb_features_labels", "dcb_features_eval",
     "dcb_calib_open", "dcb_calib_contigs", "dcb_calib_fetch_reference", "dcb_calib_query", "dcb_calib_next_batch",
     "dcb_calib_get_batch", "dcb_calib_read_name", "dcb_calib_close", "dcb_calib_count", "dcb_read_identity",
+    "dcb_seq_open", "dcb_seq_next_batch", "dcb_seq_get_batch", "dcb_seq_read_name", "dcb_seq_close",
+    "dcb_kmer_table_init", "dcb_kmer_table_clear", "dcb_kmer_count", "dcb_kmer_query", "dcb_kmer_wait",
+    "dcb_kmer_table_stats",
     "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
     "dcb_last_forward_launches", "dcb_set_profile", "dcb_get_profile", "dcb_get_profile_kernels", "dcb_alloc_host",
     "dcb_free_host", "dcb_alloc_device", "dcb_free_device", "dcb_memcpy_h2d", "dcb_memcpy_d2h",
@@ -222,6 +235,12 @@ def _load(path: str) -> ctypes.CDLL:
                                     ctypes.POINTER(ctypes.c_float)]
   lib.dcb_calib_count.argtypes = [vp, ctypes.POINTER(DcbCalibInput), vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_read_identity.argtypes = [vp, ctypes.POINTER(DcbIdentityInput), vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_kmer_table_init.argtypes = [vp, ctypes.c_int64, i32, ctypes.POINTER(ctypes.c_int64)]
+  lib.dcb_kmer_table_clear.argtypes = [vp, i32, i32]
+  lib.dcb_kmer_count.argtypes = [vp, ctypes.POINTER(DcbKmerBatch), i32]
+  lib.dcb_kmer_query.argtypes = [vp, ctypes.POINTER(DcbKmerBatch), i32, i32, i32]
+  lib.dcb_kmer_wait.argtypes = [vp, i32, vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_kmer_table_stats.argtypes = [vp, vp, vp]
   lib.dcb_last_forward_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_launches.argtypes = [vp, ctypes.POINTER(i32)]
   lib.dcb_set_debug.argtypes = [vp, i32]
@@ -831,6 +850,61 @@ class B200Model:
     self._check(self._lib.dcb_read_identity(self._handle, ctypes.byref(arg), _ptr(counts), _ptr(avg_q), _ptr(status),
                                             ctypes.byref(ms)))
     return dict(counts=counts, avg_q=avg_q, status=status, ms=float(ms.value))
+
+  # -- k-mer QV (include/dcb200.h "k-mer QV") ---------------------------------------------------------------------
+  def kmer_table_init(self, table_bytes: int, k: int) -> int:
+    """dcb_kmer_table_init: an empty k-mer table in at most table_bytes of device memory (<= 0: half the free
+    memory); returns its capacity in slots."""
+    cap = ctypes.c_int64(0)
+    self._check(self._lib.dcb_kmer_table_init(self._handle, int(table_bytes), int(k), ctypes.byref(cap)))
+    return int(cap.value)
+
+  def kmer_table_clear(self, partition: int, n_partitions: int) -> None:
+    self._check(self._lib.dcb_kmer_table_clear(self._handle, int(partition), int(n_partitions)))
+
+  def kmer_submit(self, batch: Dict[str, np.ndarray], slot: int, min_count: int = 0, with_quality: bool = False
+                  ) -> Tuple[int, int, DcbKmerBatch, Tuple[np.ndarray, ...]]:
+    """dcb_kmer_count (min_count 0) or dcb_kmer_query of one batch (dict of bases uint8, offsets int64 [n + 1],
+    qual uint8 and has_qual uint8 [n]) on pipeline slot 0 / 1.  Returns the handle kmer_wait takes."""
+    arrays = tuple(np.ascontiguousarray(batch[k], dt) for k, dt in (("bases", np.uint8), ("offsets", np.int64),
+                                                                    ("qual", np.uint8), ("has_qual", np.uint8)))
+    bases, offsets, qual, has_qual = arrays
+    arg = DcbKmerBatch(n_reads=len(offsets) - 1, n_bases=bases.size, bases=_ptr(bases), qual=_ptr(qual),
+                       offsets=_ptr(offsets), has_qual=_ptr(has_qual))
+    if min_count:
+      self._check(self._lib.dcb_kmer_query(self._handle, ctypes.byref(arg), int(min_count), int(with_quality), int(slot)))
+    else:
+      self._check(self._lib.dcb_kmer_count(self._handle, ctypes.byref(arg), int(slot)))
+    return int(slot), int(min_count), arg, arrays
+
+  def kmer_wait(self, handle) -> Dict[str, Any]:
+    """dcb_kmer_wait for a kmer_submit: dict(ms) and, for a query, counts int64 [n, 2] (k-mers of the partition,
+    unsupported), avg_q float64 [n] and borderline bool [n]."""
+    slot, query, arg, _ = handle
+    n = arg.n_reads
+    counts, avg_q, border = np.zeros((n, 2), np.int64), np.zeros(n, np.float64), np.zeros(n, np.int32)
+    ms = ctypes.c_float(0)
+    self._check(self._lib.dcb_kmer_wait(self._handle, slot, _ptr(counts), _ptr(avg_q), _ptr(border), ctypes.byref(ms)))
+    out: Dict[str, Any] = dict(ms=float(ms.value))
+    if query:
+      out.update(counts=counts, avg_q=avg_q, borderline=border.astype(bool))
+    return out
+
+  def kmer_retire(self, handle) -> None:
+    try:
+      self.kmer_wait(handle)
+    except DcbError:
+      pass
+
+  def kmer_table_stats(self, histogram: bool = True) -> Dict[str, Any]:
+    """dcb_kmer_table_stats: dict of KMER_STAT_KEYS and, with `histogram`, histogram int64 [KMER_HIST + 1] ([c] = keys
+    with count c, [KMER_HIST] = keys with count >= KMER_HIST)."""
+    stats, hist = np.zeros(len(KMER_STAT_KEYS), np.int64), np.zeros(KMER_HIST + 1, np.int64)
+    self._check(self._lib.dcb_kmer_table_stats(self._handle, _ptr(stats), _ptr(hist) if histogram else None))
+    out: Dict[str, Any] = {k: int(v) for k, v in zip(KMER_STAT_KEYS, stats)}
+    if histogram:
+      out["histogram"] = hist
+    return out
 
   def stitch_raw(self, bases_ptr: int, quals_ptr: int, n_windows: int, zmw_start: np.ndarray, flags: int,
                  seq_ptr: int, qual_ptr: int, len_ptr: int, length: Optional[int] = None) -> None:

@@ -611,6 +611,62 @@ typedef struct dcb_identity_input {
 int dcb_read_identity(dcb_engine* e, const dcb_identity_input* in, int64_t* counts, double* avg_q, int32_t* status,
                       float* ms_out);
 
+/* ---- k-mer QV (kmer_qv.py) -----------------------------------------------------------------------------------------
+ * A sequential reader of FASTA, FASTQ or BAM files (the format comes from the content; text may be plain or gzip):
+ * dcb_seq_next_batch reads whole records until the batch holds at least max_bases bases (at least one record), sets
+ * sizes[0] = reads and sizes[1] = bases, and returns 1, or 0 at the end of the file (< 0: error, dcb_prep_last_error;
+ * a gzip stream that is corrupt or ends early is an error, naming the file).
+ * dcb_seq_get_batch copies out the concatenated upper-cased bases [n_bases], the Phred qualities [n_bases] (0 where a
+ * read has none), the offsets [n_reads + 1] and has_qual [n_reads] (0 for FASTA records and BAM QUAL 0xFF).  A BAM is
+ * read in file order without an index; its secondary (0x100) and supplementary (0x800) records are skipped, and a
+ * record without SEQ is refused.  FASTA records may span lines. */
+typedef struct dcb_seq_reader dcb_seq_reader;
+int dcb_seq_open(const char* path, dcb_seq_reader** out);
+int dcb_seq_next_batch(dcb_seq_reader* r, int64_t max_bases, int64_t* sizes);
+int dcb_seq_get_batch(dcb_seq_reader* r, uint8_t* bases, uint8_t* qual, int64_t* offsets, uint8_t* has_qual);
+const char* dcb_seq_read_name(dcb_seq_reader* r, int64_t i);
+void dcb_seq_close(dcb_seq_reader* r);
+
+/* The engine's k-mer table: an open-addressing table of canonical k-mer codes (2 bits per base, A=0 C=1 G=2 T=3, first
+ * base most significant; canonical = the smaller of the k-mer's and its reverse complement's code) with a uint32 count
+ * per key.  A key's slot is the low bits of splitmix64's finalizer of the key, probed linearly; the key belongs to
+ * partition (mix >> 32) % n_partitions.  Any byte other than A, C, G or T breaks the k-mers that contain it.
+ *   dcb_kmer_table_init   allocates capacity slots, the largest power of two that fits table_bytes (12 bytes a slot;
+ *                         table_bytes <= 0: half the device's free memory), for 1 <= k <= 31.
+ *   dcb_kmer_table_clear  empties it for the keys of one partition.
+ *   dcb_kmer_count        counts every k-mer of the batch's reads that belongs to the partition (both strands to one
+ *                         key; counts saturate near 2^32).  When the number of distinct keys exceeds 0.8 x capacity the
+ *                         table stops accepting keys and reports overflow in dcb_kmer_table_stats: the caller repeats
+ *                         the work with more partitions.
+ *   dcb_kmer_query        per read of the batch: the k-mer positions of the partition (counts[2r]) and how many of
+ *                         them have a count below min_count (counts[2r + 1]).  With with_quality, also avg_phred of the
+ *                         read's qualities (the engine's 10^(-q/10) table, as dcb_read_identity) in avg_q[r] and
+ *                         borderline[r] = 1 where it lies within 1e-7 of q - 5e-6 for an integer q; reads without
+ *                         qualities get avg_q 0.
+ * dcb_kmer_count and dcb_kmer_query enqueue their work on pipeline slot 0 or 1 and return; dcb_kmer_wait waits for
+ * the slot's work, writes its query outputs (host arrays of the batch's n_reads; NULL for a count) and its device time.
+ * Two slots may be in flight at once, so the host reads the next batch while the device works on the last.
+ * dcb_kmer_table_stats (after a wait): stats[DCB_KMER_STATS] = capacity, distinct keys claimed, overflow, k-mers
+ * counted, their probe steps, k-mers queried, their probe steps; histogram[DCB_KMER_HIST + 1]: [c] = keys with count
+ * c for c = 1..255, [256] = keys with count >= 256.  Every output is an integer, so none depends on the batch split,
+ * the insertion order or the number of partitions. */
+#define DCB_KMER_STATS 7
+#define DCB_KMER_HIST 256
+typedef struct dcb_kmer_batch {
+  int32_t n_reads, reserved;
+  int64_t n_bases;
+  const uint8_t* bases;            /* [n_bases] */
+  const uint8_t* qual;             /* [n_bases] Phred; dcb_kmer_query with with_quality only */
+  const int64_t* offsets;          /* [n_reads + 1], offsets[0] = 0 */
+  const uint8_t* has_qual;         /* [n_reads]; dcb_kmer_query with with_quality only */
+} dcb_kmer_batch;
+int dcb_kmer_table_init(dcb_engine* e, int64_t table_bytes, int32_t k, int64_t* capacity);
+int dcb_kmer_table_clear(dcb_engine* e, int32_t partition, int32_t n_partitions);
+int dcb_kmer_count(dcb_engine* e, const dcb_kmer_batch* b, int32_t slot);
+int dcb_kmer_query(dcb_engine* e, const dcb_kmer_batch* b, int32_t min_count, int32_t with_quality, int32_t slot);
+int dcb_kmer_wait(dcb_engine* e, int32_t slot, int64_t* counts, double* avg_q, int32_t* borderline, float* ms_out);
+int dcb_kmer_table_stats(dcb_engine* e, int64_t* stats, int64_t* histogram);
+
 /* Device time of the last dcb_forward (milliseconds, CUDA events on the engine's stream). */
 int dcb_last_forward_ms(dcb_engine* e, float* ms);
 /* Number of engine kernels launched by the last dcb_forward. */
