@@ -31,6 +31,17 @@
 //                         histogram of the qualities gives avg_phred by read_outcome_kernel's arithmetic
 //                         (quality.cuh).  A fixed-order block reduction writes the read's five int64 counts; the read's
 //                         status says whether they count (see include/dcb200.h).  No global atomics.
+//
+// Read errors (dcb_read_errors) bin each read's errors by the truth homopolymer they touch:
+//   run_edges_kernel, run_carry_kernel, run_bounds_kernel
+//                         every position of the batch's truth slice gets its maximal ACGT run by segmented scans: per
+//                         4 096-base chunk its last run start and first run end, one CTA scanning those across chunks,
+//                         then each chunk's prefix-max / suffix-min scans seeded with the carries.  No thread walks a
+//                         run, and a run longer than a chunk comes out whole.
+//   read_errors_tally_kernel  one CTA per read.  The same block scan places each operation; threads over the query
+//                         bases bin each mismatch and mark the insertions that are not one ACGT base; the thread that
+//                         owns an I or D operation bins it; threads over the read's truth span count the runs inside
+//                         it.  Shared histograms, then a fixed-order write of the read's int64 row.  No global atomics.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -112,12 +123,50 @@ __device__ __forceinline__ unsigned long long calib_scan(unsigned long long v, u
   return v;
 }
 
+// One 256-operation chunk of a read's cigar, placed: each operation's query bases [qbeg, qend) and its first reference
+// base rbeg, relative to the chunk's start.
+struct OpChunk {
+  int qbeg[kCalibThreads], qend[kCalibThreads], rbeg[kCalibThreads];
+  uint8_t op[kCalibThreads];
+};
+
+// Places operations [base, base + 256) of a cigar of n_ops: thread t takes operation base + t (op 15 past the end) and
+// receives its op, length and exclusive packed offsets (reference << 32 | query); a block scan fills `s` for the
+// threads over the chunk's bases.  Returns the chunk's packed total.  Ends with a barrier after `s` is written.
+__device__ __forceinline__ unsigned long long place_ops(const uint32_t* cig, int n_ops, int base, OpChunk& s,
+                                                        unsigned long long* warp, int* op, unsigned long long* len,
+                                                        unsigned long long* excl) {
+  const int tid = threadIdx.x, k = base + tid;
+  const uint32_t v = k < n_ops ? cig[k] : 0u;
+  *op = k < n_ops ? (int)(v & 15) : 15;
+  *len = v >> 4;
+  const unsigned long long x = (calib_ref(*op) ? *len << 32 : 0ull) | (calib_query(*op) ? *len : 0ull);
+  unsigned long long total;
+  const unsigned long long incl = calib_scan(x, warp, &total);
+  *excl = incl - x;
+  s.qbeg[tid] = (int)(uint32_t)*excl;
+  s.qend[tid] = (int)(uint32_t)incl;
+  s.rbeg[tid] = (int)(*excl >> 32);
+  s.op[tid] = (uint8_t)*op;
+  __syncthreads();
+  return total;
+}
+
+// The operation of the chunk (0..last) that holds the chunk's query base j: the first whose inclusive query end exceeds j.
+__device__ __forceinline__ int op_of_base(const OpChunk& s, int last, int j) {
+  int lo = 0, hi = last;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (s.qend[mid] > j) hi = mid; else lo = mid + 1;
+  }
+  return lo;
+}
+
 __global__ void __launch_bounds__(kCalibThreads) calib_count_kernel(CalibBatch c, long long* partial, long long* partial_fail) {
   __shared__ unsigned hist[2 * kCalibBins];
   __shared__ unsigned long long acc[2 * kCalibBins];
   __shared__ unsigned long long warp_sums[kCalibWarps];
-  __shared__ int s_qbeg[kCalibThreads], s_qend[kCalibThreads], s_rbeg[kCalibThreads];
-  __shared__ uint8_t s_op[kCalibThreads];
+  __shared__ OpChunk s;
   __shared__ unsigned long long s_fail;
   const int tid = threadIdx.x;
   for (int k = tid; k < 2 * kCalibBins; k += kCalibThreads) { hist[k] = 0; acc[k] = 0; }
@@ -134,31 +183,17 @@ __global__ void __launch_bounds__(kCalibThreads) calib_count_kernel(CalibBatch c
     if (tid == 0) s_fail = ~0ull;
     int64_t q0 = 0, r0 = pos;
     for (int base = 0; base < n_ops; base += kCalibThreads) {
-      const int k = base + tid;
-      const uint32_t v = k < n_ops ? cig[k] : 0u;
-      const int op = k < n_ops ? (int)(v & 15) : 15;
-      const unsigned long long len = v >> 4;
-      const unsigned long long x = (calib_ref(op) ? len << 32 : 0ull) | (calib_query(op) ? len : 0ull);
-      unsigned long long total;
-      const unsigned long long incl = calib_scan(x, warp_sums, &total);
-      const unsigned long long excl = incl - x;
-      s_qbeg[tid] = (int)(uint32_t)excl;
-      s_qend[tid] = (int)(uint32_t)incl;
-      s_rbeg[tid] = (int)(excl >> 32);
-      s_op[tid] = (uint8_t)op;
-      __syncthreads();
+      int op;
+      unsigned long long len, excl;
+      const unsigned long long total = place_ops(cig, n_ops, base, s, warp_sums, &op, &len, &excl);
       const int chunk_q = (int)(uint32_t)total;
       const int last = min(kCalibThreads, n_ops - base) - 1;
       for (int j = tid; j < chunk_q; j += kCalibThreads) {
-        int lo = 0, hi = last;   // the first operation whose inclusive query end exceeds j
-        while (lo < hi) {
-          const int mid = (lo + hi) >> 1;
-          if (s_qend[mid] > j) hi = mid; else lo = mid + 1;
-        }
-        const int o = s_op[lo];
+        const int lo = op_of_base(s, last, j);
+        const int o = s.op[lo];
         const bool aligned = calib_aligned(o);
         const int64_t i = q0 + j;
-        const int64_t r = r0 + s_rbeg[lo] + (aligned ? j - s_qbeg[lo] : 0);
+        const int64_t r = r0 + s.rbeg[lo] + (aligned ? j - s.qbeg[lo] : 0);
         const int mult = calib_multiplicity(r, pos, endpos, c);
         if (mult == 0) continue;
         int mismatch = 1;
@@ -218,8 +253,7 @@ __global__ void __launch_bounds__(kCalibThreads) read_identity_kernel(IdentityBa
   static_assert(kCalibThreads == 256, "one histogram bin per thread");
   __shared__ int hist[256];
   __shared__ unsigned long long warp_sums[kCalibWarps];
-  __shared__ int s_qbeg[kCalibThreads], s_qend[kCalibThreads], s_rbeg[kCalibThreads];
-  __shared__ uint8_t s_op[kCalibThreads];
+  __shared__ OpChunk s;
   __shared__ long long s_red[kIdentityCounts][kCalibWarps];
   const int tid = threadIdx.x, rd = blockIdx.x;
   const int32_t* m = c.read_meta + (size_t)rd * kCalibMeta;
@@ -234,33 +268,19 @@ __global__ void __launch_bounds__(kCalibThreads) read_identity_kernel(IdentityBa
   int skip = 0, bad = 0;
   int64_t q0 = 0, r0 = m[0];
   for (int base = 0; base < n_ops; base += kCalibThreads) {
-    const int k = base + tid;
-    const uint32_t x = k < n_ops ? cig[k] : 0u;
-    const int op = k < n_ops ? (int)(x & 15) : 15;
-    const unsigned long long len = x >> 4;
+    int op;
+    unsigned long long len, excl;
+    const unsigned long long total = place_ops(cig, n_ops, base, s, warp_sums, &op, &len, &excl);
     if (op == 1) v[2] += (long long)len;
     else if (op == 2) v[3] += (long long)len;
     else if (op == 4) v[4] += (long long)len;
     skip |= op == 3;
-    const unsigned long long e = (calib_ref(op) ? len << 32 : 0ull) | (calib_query(op) ? len : 0ull);
-    unsigned long long total;
-    const unsigned long long incl = calib_scan(e, warp_sums, &total);
-    const unsigned long long excl = incl - e;
-    s_qbeg[tid] = (int)(uint32_t)excl;
-    s_qend[tid] = (int)(uint32_t)incl;
-    s_rbeg[tid] = (int)(excl >> 32);
-    s_op[tid] = (uint8_t)op;
-    __syncthreads();
     const int chunk_q = (int)(uint32_t)total;
     const int last = min(kCalibThreads, n_ops - base) - 1;
     for (int j = tid; j < chunk_q; j += kCalibThreads) {
-      int lo = 0, hi = last;   // the first operation whose inclusive query end exceeds j
-      while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (s_qend[mid] > j) hi = mid; else lo = mid + 1;
-      }
-      if (!calib_aligned(s_op[lo])) continue;
-      const int64_t r = r0 + s_rbeg[lo] + (j - s_qbeg[lo]);
+      const int lo = op_of_base(s, last, j);
+      if (!calib_aligned(s.op[lo])) continue;
+      const int64_t r = r0 + s.rbeg[lo] + (j - s.qbeg[lo]);
       if (r >= c.contig_length) continue;   // the read runs past the contig and does not count
       const int64_t at = r - c.ref_start;
       if (at < 0 || at >= c.ref_count) { bad = 1; continue; }
@@ -300,7 +320,275 @@ __global__ void __launch_bounds__(kCalibThreads) read_identity_kernel(IdentityBa
   }
 }
 
+// ---- read errors: run bounds of the truth slice, then one CTA per read
+constexpr int kRunPer = 16;                          // slice positions per thread
+constexpr int kRunChunk = kCalibThreads * kRunPer;   // per CTA
+constexpr int kNoEnd = 0x7fffffff;
+
+// 0..3 for A, C, G, T in either case, 4 for any other byte
+__device__ __forceinline__ int truth_class(uint8_t b) {
+  const int u = b >= 'a' && b <= 'z' ? b - 32 : b;
+  return u == 'A' ? 0 : u == 'C' ? 1 : u == 'G' ? 2 : u == 'T' ? 3 : 4;
+}
+// 0..3 for the 4-bit SEQ codes of A, C, G, T, 4 for any other code
+__device__ __forceinline__ int read_class(uint8_t code) {
+  return code == 1 ? 0 : code == 2 ? 1 : code == 4 ? 2 : code == 8 ? 3 : 4;
+}
+
+// Exclusive prefix maximum (lower threads first) and exclusive suffix minimum (higher threads first) over the CTA;
+// *total receives the maximum / minimum over every thread.  `warp` may be reused after the next barrier.
+__device__ __forceinline__ int block_prefix_max(int v, int* warp, int* total) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int incl = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, incl, d);
+    if (lane >= d) incl = max(incl, y);
+  }
+  int excl = __shfl_up_sync(0xffffffffu, incl, 1);
+  if (lane == 0) excl = -1;
+  if (lane == 31) warp[w] = incl;
+  __syncthreads();
+  int t = -1;
+#pragma unroll
+  for (int k = 0; k < kCalibWarps; ++k) {
+    if (k < w) excl = max(excl, warp[k]);
+    t = max(t, warp[k]);
+  }
+  *total = t;
+  return excl;
+}
+__device__ __forceinline__ int block_suffix_min(int v, int* warp, int* total) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int incl = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int y = __shfl_down_sync(0xffffffffu, incl, d);
+    if (lane + d < 32) incl = min(incl, y);
+  }
+  int excl = __shfl_down_sync(0xffffffffu, incl, 1);
+  if (lane == 31) excl = kNoEnd;
+  if (lane == 0) warp[w] = incl;
+  __syncthreads();
+  int t = kNoEnd;
+#pragma unroll
+  for (int k = 0; k < kCalibWarps; ++k) {
+    if (k > w) excl = min(excl, warp[k]);
+    t = min(t, warp[k]);
+  }
+  *total = t;
+  return excl;
+}
+
+// The truth classes of the CTA's chunk [c0, c0 + kRunChunk) and one position either side (4 outside the slice), in
+// cls[0 .. kRunChunk + 2) for positions c0 - 1 ...
+__device__ __forceinline__ void load_classes(const uint8_t* ref, int n, int c0, uint8_t* cls) {
+  for (int k = threadIdx.x; k < kRunChunk + 2; k += kCalibThreads) {
+    const int p = c0 - 1 + k;
+    cls[k] = p >= 0 && p < n ? (uint8_t)truth_class(ref[p]) : (uint8_t)4;
+  }
+  __syncthreads();
+}
+
+// Slice position p (class cls[p - c0 + 1]) starts a run -- the run's first base, or a non-ACGT byte, which is a run of
+// its own -- when run_key_start(p) = p; it ends one when run_key_end(p) = p + 1.  Otherwise -1 / kNoEnd: the scans'
+// identities.  The slice's edges cut runs (the caller widens the slice to whole runs).
+__device__ __forceinline__ int run_key_start(const uint8_t* cls, int c0, int p) {
+  const int a = cls[p - c0], b = cls[p - c0 + 1];
+  return b == 4 || a != b ? p : -1;
+}
+__device__ __forceinline__ int run_key_end(const uint8_t* cls, int c0, int p) {
+  const int b = cls[p - c0 + 1], a = cls[p - c0 + 2];
+  return b == 4 || a != b ? p + 1 : kNoEnd;
+}
+
+// run bounds, pass 1: per chunk the last run start and the first run end in it
+__global__ void __launch_bounds__(kCalibThreads) run_edges_kernel(const uint8_t* ref, int n, int* chunk_start,
+                                                                  int* chunk_end) {
+  __shared__ uint8_t cls[kRunChunk + 2];
+  __shared__ int warp[kCalibWarps];
+  const int c0 = blockIdx.x * kRunChunk, p0 = c0 + threadIdx.x * kRunPer;
+  load_classes(ref, n, c0, cls);
+  int a = -1, b = kNoEnd;
+  for (int k = 0; k < kRunPer && p0 + k < n; ++k) {
+    a = max(a, run_key_start(cls, c0, p0 + k));
+    b = min(b, run_key_end(cls, c0, p0 + k));
+  }
+  int ta, tb;
+  block_prefix_max(a, warp, &ta);
+  __syncthreads();
+  block_suffix_min(b, warp, &tb);
+  if (threadIdx.x == 0) { chunk_start[blockIdx.x] = ta; chunk_end[blockIdx.x] = tb; }
+}
+
+// run bounds, pass 2 (one CTA): per chunk the last run start before it and the first run end after it
+__global__ void __launch_bounds__(kCalibThreads) run_carry_kernel(const int* chunk_start, const int* chunk_end,
+                                                                  int n_chunks, int* carry_start, int* carry_end) {
+  __shared__ int warp[kCalibWarps];
+  int carry = -1;
+  for (int c = 0; c < n_chunks; c += kCalibThreads) {
+    const int i = c + threadIdx.x;
+    int t;
+    const int x = block_prefix_max(i < n_chunks ? chunk_start[i] : -1, warp, &t);
+    if (i < n_chunks) carry_start[i] = max(carry, x);
+    carry = max(carry, t);
+    __syncthreads();
+  }
+  carry = kNoEnd;
+  for (int c = (n_chunks - 1) / kCalibThreads * kCalibThreads; c >= 0; c -= kCalibThreads) {
+    const int i = c + threadIdx.x;
+    int t;
+    const int x = block_suffix_min(i < n_chunks ? chunk_end[i] : kNoEnd, warp, &t);
+    if (i < n_chunks) carry_end[i] = min(carry, x);
+    carry = min(carry, t);
+    __syncthreads();
+  }
+}
+
+// run bounds, pass 3: each position's run [run_start, run_end), slice-relative; a non-ACGT byte gets [p, p)
+__global__ void __launch_bounds__(kCalibThreads) run_bounds_kernel(const uint8_t* ref, int n, const int* carry_start,
+                                                                   const int* carry_end, int* run_start, int* run_end) {
+  __shared__ uint8_t cls[kRunChunk + 2];
+  __shared__ int warp[kCalibWarps];
+  __shared__ int out[kRunChunk];
+  const int tid = threadIdx.x, c0 = blockIdx.x * kRunChunk, p0 = c0 + tid * kRunPer;
+  load_classes(ref, n, c0, cls);
+  const int m = min(kRunPer, n - p0);   // this thread's positions (may be <= 0)
+  int a = -1, b = kNoEnd, t;
+  for (int k = 0; k < m; ++k) {
+    a = max(a, run_key_start(cls, c0, p0 + k));
+    b = min(b, run_key_end(cls, c0, p0 + k));
+  }
+  int run = max(carry_start[blockIdx.x], block_prefix_max(a, warp, &t));
+  for (int k = 0; k < m; ++k) {
+    run = max(run, run_key_start(cls, c0, p0 + k));
+    out[tid * kRunPer + k] = run;
+  }
+  __syncthreads();
+  for (int k = tid; k < kRunChunk && c0 + k < n; k += kCalibThreads) run_start[c0 + k] = out[k];
+  __syncthreads();
+  run = min(carry_end[blockIdx.x], block_suffix_min(b, warp, &t));
+  for (int k = m - 1; k >= 0; --k) {
+    const int p = p0 + k;
+    run = min(run, run_key_end(cls, c0, p));
+    out[tid * kRunPer + k] = cls[p - c0 + 1] == 4 ? p : run;
+  }
+  __syncthreads();
+  for (int k = tid; k < kRunChunk && c0 + k < n; k += kCalibThreads) run_end[c0 + k] = out[k];
+}
+
+// The homopolymer bin of slice position at: min(run length, 20), 0 for a non-ACGT byte.
+__device__ __forceinline__ int hp_bin(const int* run_start, const int* run_end, int64_t at) {
+  return min(run_end[at] - run_start[at], kErrorBins - 1);
+}
+
+__global__ void __launch_bounds__(kCalibThreads) read_errors_tally_kernel(IdentityBatch c, const int* run_start,
+                                                                          const int* run_end, long long* errors) {
+  __shared__ unsigned hist[kErrorCols];
+  __shared__ unsigned long long warp_sums[kCalibWarps];
+  __shared__ OpChunk s;
+  __shared__ uint8_t s_mixed[kCalibThreads];   // per I operation of the chunk: its bases are not one ACGT base
+  const int tid = threadIdx.x, rd = blockIdx.x;
+  const int32_t* m = c.read_meta + (size_t)rd * kCalibMeta;
+  const uint32_t* cig = c.cigar + m[2];
+  const int n_ops = m[3];
+  const uint8_t* seq = c.seq + m[4];
+  for (int k = tid; k < kErrorCols; k += kCalibThreads) hist[k] = 0;
+  int skip = 0, bad = 0;
+  int64_t q0 = 0, r0 = m[0];
+  // the slice position of truth position r, or -1 (and the read is bad) when the slice lacks it
+  auto slice_at = [&](int64_t r) -> int64_t {
+    const int64_t at = r - c.ref_start;
+    if (at < 0 || at >= c.ref_count) { bad = 1; return -1; }
+    return at;
+  };
+  for (int base = 0; base < n_ops; base += kCalibThreads) {
+    s_mixed[tid] = 0;   // published by place_ops' barrier
+    int op;
+    unsigned long long len, excl;
+    const unsigned long long total = place_ops(cig, n_ops, base, s, warp_sums, &op, &len, &excl);
+    skip |= op == 3;
+    const int chunk_q = (int)(uint32_t)total;
+    const int last = min(kCalibThreads, n_ops - base) - 1;
+    // threads over the query bases: substitutions, and whether each insertion is one ACGT base
+    for (int j = tid; j < chunk_q; j += kCalibThreads) {
+      const int lo = op_of_base(s, last, j);
+      const int o = s.op[lo];
+      const uint8_t q = seq[q0 + j];
+      if (o == 1) {
+        if (read_class(q) == 4 || q != seq[q0 + s.qbeg[lo]]) s_mixed[lo] = 1;
+        continue;
+      }
+      if (!calib_aligned(o)) continue;
+      const int64_t r = r0 + s.rbeg[lo] + (j - s.qbeg[lo]);
+      if (r >= c.contig_length) continue;   // the read runs past the contig: its row is zero
+      const int64_t at = slice_at(r);
+      if (at < 0) continue;
+      const int tc = truth_class(c.ref[at]), qc = read_class(q);
+      if (tc != 4 && tc == qc) continue;   // a match
+      atomicAdd(&hist[kErrorSub + hp_bin(run_start, run_end, at)], 1u);
+      atomicAdd(&hist[kErrorMatrix + 5 * tc + qc], 1u);
+    }
+    __syncthreads();
+    // the thread that owns an I or D operation classifies it
+    const int64_t r = r0 + (int64_t)(excl >> 32);
+    if (op == 1) {
+      const int b = len == 0 || s_mixed[tid] ? 4 : read_class(seq[q0 + (uint32_t)excl]);
+      int h = 0;
+      if (b != 4) {
+        int64_t at;
+        if (r >= 1 && (at = slice_at(r - 1)) >= 0 && truth_class(c.ref[at]) == b) {
+          h = hp_bin(run_start, run_end, at);
+        } else if (r < c.contig_length && (at = slice_at(r)) >= 0 && truth_class(c.ref[at]) == b) {
+          h = hp_bin(run_start, run_end, at);
+        }
+      }
+      atomicAdd(&hist[kErrorInsEvents + h], 1u);
+      atomicAdd(&hist[kErrorInsBases + h], (unsigned)len);
+    } else if (op == 2 && r + (int64_t)len <= c.contig_length) {
+      int h = 0;
+      int64_t at;
+      if (len > 0 && (at = slice_at(r)) >= 0 && run_end[at] - at >= (int64_t)len) h = hp_bin(run_start, run_end, at);
+      atomicAdd(&hist[kErrorDelEvents + h], 1u);
+      atomicAdd(&hist[kErrorDelBases + h], (unsigned)len);
+    }
+    q0 += chunk_q;
+    r0 += (int64_t)(total >> 32);
+    __syncthreads();
+  }
+  // r0 is now the read's end on the truth: the runs that lie inside [pos, r0)
+  skip = __syncthreads_or(skip);
+  const bool counted = !skip && r0 <= c.contig_length;
+  if (counted) {
+    for (int64_t p = m[0] + tid; p < r0; p += kCalibThreads) {
+      const int64_t at = slice_at(p);
+      if (at < 0 || run_start[at] != at || run_end[at] == at || run_end[at] > r0 - c.ref_start) continue;
+      atomicAdd(&hist[kErrorRuns + hp_bin(run_start, run_end, at)], 1u);
+    }
+  }
+  bad = __syncthreads_or(bad);
+  const bool ok = counted && !bad;
+  long long* out = errors + (size_t)rd * kErrorCols;
+  for (int k = tid; k < kErrorCols; k += kCalibThreads) out[k] = ok ? (long long)hist[k] : 0;
+}
+
 }  // namespace
+
+void launch_run_bounds(const uint8_t* ref, int n, int* chunk_start, int* chunk_end, int* carry_start, int* carry_end,
+                       int* run_start, int* run_end, cudaStream_t st) {
+  const int n_chunks = (n + kRunChunk - 1) / kRunChunk;
+  if (n_chunks == 0) return;
+  run_edges_kernel<<<n_chunks, kCalibThreads, 0, st>>>(ref, n, chunk_start, chunk_end);
+  run_carry_kernel<<<1, kCalibThreads, 0, st>>>(chunk_start, chunk_end, n_chunks, carry_start, carry_end);
+  run_bounds_kernel<<<n_chunks, kCalibThreads, 0, st>>>(ref, n, carry_start, carry_end, run_start, run_end);
+}
+
+int run_bounds_chunks(int n) { return (n + kRunChunk - 1) / kRunChunk; }
+
+void launch_read_errors(const IdentityBatch& c, const int* run_start, const int* run_end, long long* errors,
+                        cudaStream_t st) {
+  if (c.n_reads > 0) read_errors_tally_kernel<<<c.n_reads, kCalibThreads, 0, st>>>(c, run_start, run_end, errors);
+}
 
 void launch_calib_count(const CalibBatch& c, int grid, long long* partial, long long* partial_fail, long long* out,
                         cudaStream_t st) {

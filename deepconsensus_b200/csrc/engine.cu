@@ -222,6 +222,12 @@ struct dcb_engine {
     DevBuf<long long> counts;
     DevBuf<double> avg_q;
   } ri;
+  struct {   // dcb_read_errors: the batch, its truth slice and the slice's run bounds
+    DevBuf<int32_t> meta, chunk_start, chunk_end, carry_start, carry_end, run_start, run_end;
+    DevBuf<uint32_t> cigar;
+    DevBuf<uint8_t> seq, qual, ref;
+    DevBuf<long long> errors;
+  } re;
   struct {   // dcb_kmer_*: the k-mer table and two pipeline slots of staged batches and per-read outputs
     DevBuf<unsigned long long> keys, stats, hist_partial, hist;
     DevBuf<unsigned int> counts;
@@ -2191,20 +2197,28 @@ static_assert(kIdentityCounts == DCB_IDENTITY_COUNTS && kIdentityOk == DCB_IDENT
               kIdentityBorderline == DCB_IDENTITY_BORDERLINE && kIdentityBadInput == DCB_IDENTITY_BAD_INPUT,
               "the kernel writes the ABI's status codes");
 
+// A dcb_identity_input as the identity and errors kernels may trust it: sizes, arrays, and every read as
+// check_aligned_read has it.
+static int check_identity_input(dcb_engine* e, const char* who, const dcb_identity_input* in) {
+  if (in->n_reads < 0 || in->n_cigar < 0 || in->n_bases < 0 || in->ref_count < 0 || in->contig_length < 0 ||
+      in->n_bases > INT32_MAX || in->n_cigar > INT32_MAX)
+    return fail(e, DCB_ERR_INVALID, "%s: bad sizes", who);
+  if ((in->n_reads && (!in->read_meta || (in->n_cigar && !in->cigar) || (in->n_bases && (!in->seq || !in->qual)))) ||
+      (in->ref_count && !in->ref_bases))
+    return fail(e, DCB_ERR_INVALID, "%s: null array", who);
+  int rc;
+  for (int32_t r = 0; r < in->n_reads; ++r)
+    if ((rc = check_aligned_read(e, who, r, in->read_meta, in->cigar, in->n_cigar, in->n_bases))) return rc;
+  return DCB_OK;
+}
+
 int dcb_read_identity(dcb_engine* e, const dcb_identity_input* in, int64_t* counts, double* avg_q, int32_t* status,
                       float* ms_out) {
   if (!e) return DCB_ERR_INVALID;
   if (ms_out) *ms_out = 0.f;
   if (!in || !counts || !avg_q || !status) return fail(e, DCB_ERR_INVALID, "dcb_read_identity: null argument");
-  if (in->n_reads < 0 || in->n_cigar < 0 || in->n_bases < 0 || in->ref_count < 0 || in->contig_length < 0 ||
-      in->n_bases > INT32_MAX || in->n_cigar > INT32_MAX)
-    return fail(e, DCB_ERR_INVALID, "dcb_read_identity: bad sizes");
-  if ((in->n_reads && (!in->read_meta || (in->n_cigar && !in->cigar) || (in->n_bases && (!in->seq || !in->qual)))) ||
-      (in->ref_count && !in->ref_bases))
-    return fail(e, DCB_ERR_INVALID, "dcb_read_identity: null array");
   int rc;
-  for (int32_t r = 0; r < in->n_reads; ++r)
-    if ((rc = check_aligned_read(e, "dcb_read_identity", r, in->read_meta, in->cigar, in->n_cigar, in->n_bases))) return rc;
+  if ((rc = check_identity_input(e, "dcb_read_identity", in))) return rc;
   auto& ri = e->ri;
   CU(e, cudaSetDevice(e->cfg.device));
   cudaStream_t st = e->stream;
@@ -2229,6 +2243,61 @@ int dcb_read_identity(dcb_engine* e, const dcb_identity_input* in, int64_t* coun
   launch_read_identity(c, o_counts.d, o_avg.d, o_status.d, st);
   CU(e, cudaEventRecord(e->ev_eval1, st));
   if ((rc = copy_out(e, o_counts)) || (rc = copy_out(e, o_avg)) || (rc = copy_out(e, o_status))) return rc;
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  return DCB_OK;
+}
+
+static_assert(kErrorBins == DCB_ERRORS_BINS && kErrorSub == DCB_ERRORS_SUB && kErrorInsEvents == DCB_ERRORS_INS_EVENTS &&
+              kErrorInsBases == DCB_ERRORS_INS_BASES && kErrorDelEvents == DCB_ERRORS_DEL_EVENTS &&
+              kErrorDelBases == DCB_ERRORS_DEL_BASES && kErrorRuns == DCB_ERRORS_RUNS &&
+              kErrorMatrix == DCB_ERRORS_MATRIX && kErrorCols == DCB_ERRORS_COLS && kErrorMatrix + 25 == kErrorCols,
+              "the kernel writes the ABI's error columns");
+
+int dcb_read_errors(dcb_engine* e, const dcb_identity_input* in, int64_t* errors, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  if (ms_out) *ms_out = 0.f;
+  if (!in || !errors) return fail(e, DCB_ERR_INVALID, "dcb_read_errors: null argument");
+  int rc;
+  if ((rc = check_identity_input(e, "dcb_read_errors", in))) return rc;
+  if (in->ref_start < 0 || in->ref_count > INT32_MAX || in->ref_start + in->ref_count > in->contig_length)
+    return fail(e, DCB_ERR_INVALID, "dcb_read_errors: the slice [%lld, +%lld) is not inside the contig (length %lld)",
+                (long long)in->ref_start, (long long)in->ref_count, (long long)in->contig_length);
+  for (int32_t r = 0; r < in->n_reads; ++r) {   // the truth positions the kernel may read, whole runs aside
+    const int32_t* m = in->read_meta + (size_t)r * DCB_CALIB_META;
+    const int64_t lo = std::max<int64_t>(m[0] - 1, 0), hi = std::min<int64_t>((int64_t)m[1] + 1, in->contig_length);
+    if (lo < hi && (lo < in->ref_start || hi > in->ref_start + in->ref_count))
+      return fail(e, DCB_ERR_INVALID, "dcb_read_errors: read %d: the slice [%lld, +%lld) does not hold [%lld, %lld)", r,
+                  (long long)in->ref_start, (long long)in->ref_count, (long long)lo, (long long)hi);
+  }
+  auto& re = e->re;
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  const int32_t* d_meta;
+  const uint32_t* d_cigar;
+  const uint8_t *d_seq, *d_qual, *d_ref;
+  Output<long long> o_errors;
+  const size_t n = (size_t)in->n_reads, n_ref = (size_t)in->ref_count;
+  const size_t n_chunks = (size_t)std::max(run_bounds_chunks((int)in->ref_count), 1);
+  if ((rc = stage_in(e, re.meta, in->read_meta, n * DCB_CALIB_META, false, &d_meta)) ||
+      (rc = stage_in(e, re.cigar, in->cigar, (size_t)in->n_cigar, false, &d_cigar)) ||
+      (rc = stage_in(e, re.seq, in->seq, (size_t)in->n_bases, false, &d_seq)) ||
+      (rc = stage_in(e, re.qual, in->qual, (size_t)in->n_bases, false, &d_qual)) ||
+      (rc = stage_in(e, re.ref, in->ref_bases, n_ref, false, &d_ref)) ||
+      (rc = ensure(e, re.run_start, std::max<size_t>(n_ref, 1))) || (rc = ensure(e, re.run_end, std::max<size_t>(n_ref, 1))) ||
+      (rc = ensure(e, re.chunk_start, n_chunks)) || (rc = ensure(e, re.chunk_end, n_chunks)) ||
+      (rc = ensure(e, re.carry_start, n_chunks)) || (rc = ensure(e, re.carry_end, n_chunks)) ||
+      (rc = stage_out(e, re.errors, reinterpret_cast<long long*>(errors), n * kErrorCols, false, &o_errors)))
+    return rc;
+  IdentityBatch c{d_meta, d_cigar, d_seq, d_qual, in->n_reads, d_ref, in->ref_start, in->ref_count, in->contig_length,
+                  e->d_p10.p};
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  launch_run_bounds(d_ref, (int)in->ref_count, re.chunk_start.p, re.chunk_end.p, re.carry_start.p, re.carry_end.p,
+                    re.run_start.p, re.run_end.p, st);
+  launch_read_errors(c, re.run_start.p, re.run_end.p, o_errors.d, st);
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  if ((rc = copy_out(e, o_errors))) return rc;
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));

@@ -177,6 +177,19 @@ struct IdentityBatch {
   const double* p10;          // 10^(-q/10), q = 0..255
 };
 void launch_read_identity(const IdentityBatch& c, long long* counts, double* avg_q, int32_t* status, cudaStream_t st);
+// ---- read errors (calib_kernels.cu, dcb_read_errors).  launch_run_bounds: every position p of the truth slice ref [n]
+// gets its maximal ACGT run [run_start[p], run_end[p]) (slice-relative, the slice's edges cutting runs; [p, p) for a
+// non-ACGT byte), by segmented scans in three launches; chunk_* and carry_* hold run_bounds_chunks(n) entries each.
+// launch_read_errors: one CTA per read of a batch validated as for read identity, whose slice c.ref the run bounds
+// describe; errors: int64 [n_reads][kErrorCols], the DCB_ERRORS_* layout.
+constexpr int kErrorBins = 21;   // DCB_ERRORS_*
+constexpr int kErrorSub = 0, kErrorInsEvents = 21, kErrorInsBases = 42, kErrorDelEvents = 63, kErrorDelBases = 84,
+              kErrorRuns = 105, kErrorMatrix = 126, kErrorCols = 151;
+int run_bounds_chunks(int n);
+void launch_run_bounds(const uint8_t* ref, int n, int* chunk_start, int* chunk_end, int* carry_start, int* carry_end,
+                       int* run_start, int* run_end, cudaStream_t st);
+void launch_read_errors(const IdentityBatch& c, const int* run_start, const int* run_end, long long* errors,
+                        cudaStream_t st);
 // ---- k-mer table (kmer_kernels.cu, dcb_kmer_*).  keys: capacity uint64 (kKmerEmpty = free), counts: capacity uint32,
 // capacity a power of two.  stats: uint64 [kKmerStatSlots] = claimed keys, overflow flag, k-mers counted, their probe
 // steps, k-mers queried, their probe steps.  Device pointers.

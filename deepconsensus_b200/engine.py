@@ -49,6 +49,11 @@ DCB_CALIB_PAST_CONTIG, DCB_CALIB_BAD_QUALITY, DCB_CALIB_BAD_INPUT = 1, 2, 3
 IDENTITY_COUNTS = 5
 (DCB_IDENTITY_OK, DCB_IDENTITY_PAST_CONTIG, DCB_IDENTITY_SKIP_OP, DCB_IDENTITY_BORDERLINE,
  DCB_IDENTITY_BAD_INPUT) = range(5)
+# dcb_read_errors: per-read rows of six ERRORS_BINS-bin tables at these column offsets, then the 5 x 5 substitution matrix
+ERRORS_BINS = 21
+(ERRORS_SUB, ERRORS_INS_EVENTS, ERRORS_INS_BASES, ERRORS_DEL_EVENTS, ERRORS_DEL_BASES, ERRORS_RUNS,
+ ERRORS_MATRIX) = range(0, 7 * ERRORS_BINS, ERRORS_BINS)
+ERRORS_COLS = ERRORS_MATRIX + 25
 # dcb_kmer_table_stats: its stats entries and the count histogram's last bin (counts >= DCB_KMER_HIST)
 KMER_STAT_KEYS = ("capacity", "claimed", "overflow", "count_kmers", "count_probes", "query_kmers", "query_probes")
 KMER_HIST = 256
@@ -154,6 +159,7 @@ ABI_SYMBOLS = (
     "dcb_prep_get_label", "dcb_features_labels", "dcb_features_eval",
     "dcb_calib_open", "dcb_calib_contigs", "dcb_calib_fetch_reference", "dcb_calib_query", "dcb_calib_next_batch",
     "dcb_calib_get_batch", "dcb_calib_read_name", "dcb_calib_close", "dcb_calib_count", "dcb_read_identity",
+    "dcb_read_errors",
     "dcb_seq_open", "dcb_seq_next_batch", "dcb_seq_get_batch", "dcb_seq_read_name", "dcb_seq_close",
     "dcb_kmer_table_init", "dcb_kmer_table_clear", "dcb_kmer_count", "dcb_kmer_query", "dcb_kmer_wait",
     "dcb_kmer_table_stats",
@@ -235,6 +241,7 @@ def _load(path: str) -> ctypes.CDLL:
                                     ctypes.POINTER(ctypes.c_float)]
   lib.dcb_calib_count.argtypes = [vp, ctypes.POINTER(DcbCalibInput), vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_read_identity.argtypes = [vp, ctypes.POINTER(DcbIdentityInput), vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_read_errors.argtypes = [vp, ctypes.POINTER(DcbIdentityInput), vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_kmer_table_init.argtypes = [vp, ctypes.c_int64, i32, ctypes.POINTER(ctypes.c_int64)]
   lib.dcb_kmer_table_clear.argtypes = [vp, i32, i32]
   lib.dcb_kmer_count.argtypes = [vp, ctypes.POINTER(DcbKmerBatch), i32]
@@ -850,6 +857,24 @@ class B200Model:
     self._check(self._lib.dcb_read_identity(self._handle, ctypes.byref(arg), _ptr(counts), _ptr(avg_q), _ptr(status),
                                             ctypes.byref(ms)))
     return dict(counts=counts, avg_q=avg_q, status=status, ms=float(ms.value))
+
+  def read_errors(self, batch: Dict[str, np.ndarray], ref: np.ndarray, ref_start: int,
+                  contig_length: int) -> Dict[str, Any]:
+    """dcb_read_errors: per read of one batch (as read_identity takes it) its errors by type and homopolymer length
+    against `ref`, the contig's bases [ref_start, ref_start + len(ref)), which must hold every read's [pos - 1,
+    endpos + 1) within the contig and the whole runs at both of its ends.  Returns dict(errors int64 [n, ERRORS_COLS],
+    ms)."""
+    meta = np.ascontiguousarray(batch["read_meta"], np.int32).reshape(-1, CALIB_META)
+    cig, seq, qual = (np.ascontiguousarray(batch[k], dt) for k, dt in (("cigar", np.uint32), ("seq", np.uint8),
+                                                                       ("qual", np.uint8)))
+    ref = np.ascontiguousarray(ref, np.uint8)
+    n = len(meta)
+    arg = DcbIdentityInput(n_reads=n, n_cigar=cig.size, n_bases=seq.size, read_meta=_ptr(meta), cigar=_ptr(cig),
+                           seq=_ptr(seq), qual=_ptr(qual), ref_bases=_ptr(ref), ref_start=int(ref_start),
+                           ref_count=ref.size, contig_length=int(contig_length))
+    errors, ms = np.zeros((n, ERRORS_COLS), np.int64), ctypes.c_float(0)
+    self._check(self._lib.dcb_read_errors(self._handle, ctypes.byref(arg), _ptr(errors), ctypes.byref(ms)))
+    return dict(errors=errors, ms=float(ms.value))
 
   # -- k-mer QV (include/dcb200.h "k-mer QV") ---------------------------------------------------------------------
   def kmer_table_init(self, table_bytes: int, k: int) -> int:

@@ -611,6 +611,37 @@ typedef struct dcb_identity_input {
 int dcb_read_identity(dcb_engine* e, const dcb_identity_input* in, int64_t* counts, double* avg_q, int32_t* status,
                       float* ms_out);
 
+/* ---- read errors (read_yield.py --error_profile) ---------------------------------------------------------------------
+ * dcb_read_errors walks the same batch as dcb_read_identity and returns per read, in errors int64
+ * [n_reads][DCB_ERRORS_COLS], its errors by type and homopolymer length: six tables of DCB_ERRORS_BINS bins h = 0..20
+ * at the DCB_ERRORS_* column offsets, then the 5 x 5 substitution matrix (rows the truth class, columns the read
+ * class, in the order A, C, G, T, other).
+ *   hp(r)         the length of the maximal run of one base of A, C, G, T (upper-cased first) that holds truth
+ *                 position r, measured over the whole contig; 0 for any other byte, which breaks runs.  h = min(hp, 20).
+ *   substitutions an M, = or X base that dcb_read_identity counts as a mismatch at r: 1 in SUB[hp(r)] and in
+ *                 MATRIX[truth class][read class of the 4-bit SEQ code].
+ *   deletions     a D of n bases at [r, r + n): 1 in DEL_EVENTS[h], n in DEL_BASES[h], h = hp(r) when the n truth
+ *                 bases are one base of A, C, G, T, else 0.
+ *   insertions    an I of n bases where the walk has reached r: 1 in INS_EVENTS[h], n in INS_BASES[h].  When the n
+ *                 bases are one base b of A, C, G, T: h = hp(r - 1) if r >= 1 and truth[r - 1] is b, else hp(r) if
+ *                 r < contig_length and truth[r] is b; otherwise h = 0.
+ *   runs          RUNS[h]: the maximal runs that lie inside the read's truth span [pos, endpos); RUNS[0] is 0.
+ * Adjacent I (or D) operations are separate events; S, H and P count nothing.  A read that dcb_read_identity gives
+ * PAST_CONTIG, SKIP_OP or BAD_INPUT has a zero row.  ref_bases must hold, for every read, [max(pos - 1, 0),
+ * min(endpos + 1, contig_length)) and the whole runs at both ends of the slice (the kernel takes the slice's edges
+ * as run ends); a batch whose slice does not reach that far is refused.  ms_out (nullable): device time of the
+ * kernels.  The results do not depend on how the reads are split into batches; there are no global atomics. */
+#define DCB_ERRORS_BINS 21
+#define DCB_ERRORS_SUB 0
+#define DCB_ERRORS_INS_EVENTS 21
+#define DCB_ERRORS_INS_BASES 42
+#define DCB_ERRORS_DEL_EVENTS 63
+#define DCB_ERRORS_DEL_BASES 84
+#define DCB_ERRORS_RUNS 105
+#define DCB_ERRORS_MATRIX 126
+#define DCB_ERRORS_COLS 151
+int dcb_read_errors(dcb_engine* e, const dcb_identity_input* in, int64_t* errors, float* ms_out);
+
 /* ---- k-mer QV (kmer_qv.py) -----------------------------------------------------------------------------------------
  * A sequential reader of FASTA, FASTQ or BAM files (the format comes from the content; text may be plain or gzip):
  * dcb_seq_next_batch reads whole records until the batch holds at least max_bases bases (at least one record), sets
