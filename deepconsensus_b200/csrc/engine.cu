@@ -234,7 +234,7 @@ struct dcb_engine {
     unsigned long long capacity = 0;
     int k = 0, partition = 0, n_partitions = 1;
     struct Slot {
-      DevBuf<uint8_t> bases, qual, has_qual;
+      DevBuf<uint8_t> bases, qual, has_qual, keep;
       DevBuf<int64_t> offsets;
       DevBuf<int32_t> seg_read, seg_first;
       std::vector<int32_t> h_seg_read, h_seg_first;   // kept until the slot is reused: the copies read them
@@ -243,8 +243,15 @@ struct dcb_engine {
       DevBuf<int32_t> border;
       cudaEvent_t ev0 = nullptr, ev1 = nullptr;
       int n_reads = 0;
+      int64_t n_bases = -1;   // of the batch staged last (dcb_kmer_set_count reuses it); -1: none
       bool query = false, quality = false;
     } slot[2];
+    struct {   // dcb_kmer_set_* and dcb_kmer_spectrum: the evaluated reads' own k-mers, and the spectrum's bins
+      DevBuf<unsigned long long> keys, stats, matrix;
+      DevBuf<unsigned int> counts;
+      unsigned long long capacity = 0;
+      int partition = 0, n_partitions = 1;
+    } set;
   } km;
   cudaEvent_t ev_eval0 = nullptr, ev_eval1 = nullptr;   // around the kernel of dcb_evaluate / _distill_loss / _loss_grad
 
@@ -2305,14 +2312,13 @@ int dcb_read_errors(dcb_engine* e, const dcb_identity_input* in, int64_t* errors
 }
 
 static_assert(kKmerHist == DCB_KMER_HIST && kKmerStatSlots + 1 == DCB_KMER_STATS, "the ABI's k-mer table sizes");
+static_assert(kSpecBins == DCB_KMER_SPECTRUM_BINS && DCB_KMER_SPECTRUM_STATS == 5, "the ABI's spectrum sizes");
 
-int dcb_kmer_table_init(dcb_engine* e, int64_t table_bytes, int32_t k, int64_t* capacity) {
-  if (!e) return DCB_ERR_INVALID;
-  if (k < 1 || k > 31) return fail(e, DCB_ERR_INVALID, "dcb_kmer_table_init: k must be between 1 and 31, got %d", k);
-  auto& km = e->km;
-  CU(e, cudaSetDevice(e->cfg.device));
-  CU(e, cudaStreamSynchronize(e->stream));
-  km.keys.reset(); km.counts.reset(); km.capacity = 0;
+namespace {
+
+// The slots of a k-mer table in table_bytes (<= 0: half the device's free memory): the largest power of two, at
+// least 64 and at most 2^32, of 12-byte slots that fits.
+int kmer_capacity(dcb_engine* e, const char* who, int64_t table_bytes, unsigned long long* out) {
   if (table_bytes <= 0) {
     size_t free_b = 0, total_b = 0;
     CU(e, cudaMemGetInfo(&free_b, &total_b));
@@ -2322,11 +2328,26 @@ int dcb_kmer_table_init(dcb_engine* e, int64_t table_bytes, int32_t k, int64_t* 
   unsigned long long cap = 64;
   while (cap < (1ull << 32) && (int64_t)(2 * cap) * kSlotBytes <= table_bytes) cap *= 2;
   if ((int64_t)cap * kSlotBytes > table_bytes)
-    return fail(e, DCB_ERR_INVALID, "dcb_kmer_table_init: %lld bytes hold fewer than 64 slots", (long long)table_bytes);
+    return fail(e, DCB_ERR_INVALID, "%s: %lld bytes hold fewer than 64 slots", who, (long long)table_bytes);
+  *out = cap;
+  return DCB_OK;
+}
+
+}  // namespace
+
+int dcb_kmer_table_init(dcb_engine* e, int64_t table_bytes, int32_t k, int64_t* capacity) {
+  if (!e) return DCB_ERR_INVALID;
+  if (k < 1 || k > 31) return fail(e, DCB_ERR_INVALID, "dcb_kmer_table_init: k must be between 1 and 31, got %d", k);
+  auto& km = e->km;
+  CU(e, cudaSetDevice(e->cfg.device));
+  CU(e, cudaStreamSynchronize(e->stream));
+  km.keys.reset(); km.counts.reset(); km.capacity = 0;
+  unsigned long long cap;
+  int rc = kmer_capacity(e, "dcb_kmer_table_init", table_bytes, &cap);
+  if (rc) return rc;
   for (auto& sl : km.slot)
     for (cudaEvent_t* ev : {&sl.ev0, &sl.ev1})
       if (!*ev) CU(e, cudaEventCreate(ev));
-  int rc;
   if ((rc = ensure(e, km.keys, cap)) || (rc = ensure(e, km.counts, cap)) || (rc = ensure(e, km.stats, kKmerStatSlots)) ||
       (rc = ensure(e, km.hist, kKmerHist + 1)) ||
       (rc = ensure(e, km.hist_partial, (size_t)kmer_hist_grid(cap) * (kKmerHist + 1))))
@@ -2381,12 +2402,18 @@ int kmer_stage(dcb_engine* e, const char* who, const dcb_kmer_batch* b, int32_t 
     return rc;
   *kb = KmerBatch{d_bases, d_qual, d_off, d_has, b->n_reads, b->n_bases};
   sl.n_reads = b->n_reads;
+  sl.n_bases = b->n_bases;
   return DCB_OK;
 }
 
 KmerTable kmer_table(dcb_engine* e) {
   auto& km = e->km;
   return KmerTable{km.keys.p, km.counts.p, km.stats.p, km.capacity, km.k, km.partition, km.n_partitions};
+}
+
+KmerTable kmer_set_table(dcb_engine* e) {
+  auto& s = e->km.set;
+  return KmerTable{s.keys.p, s.counts.p, s.stats.p, s.capacity, e->km.k, s.partition, s.n_partitions};
 }
 
 }  // namespace
@@ -2480,6 +2507,97 @@ int dcb_kmer_table_stats(dcb_engine* e, int64_t* stats, int64_t* histogram) {
   }
   if (histogram)
     for (int c = 0; c <= kKmerHist; ++c) histogram[c] = (int64_t)h[c];
+  return DCB_OK;
+}
+
+int dcb_kmer_set_init(dcb_engine* e, int64_t table_bytes, int64_t* capacity) {
+  if (!e) return DCB_ERR_INVALID;
+  auto& km = e->km;
+  auto& s = km.set;
+  if (!km.capacity) return fail(e, DCB_ERR_STATE, "dcb_kmer_set_init: no table (dcb_kmer_table_init)");
+  CU(e, cudaSetDevice(e->cfg.device));
+  CU(e, cudaStreamSynchronize(e->stream));
+  s.keys.reset(); s.counts.reset(); s.capacity = 0;
+  unsigned long long cap;
+  int rc = kmer_capacity(e, "dcb_kmer_set_init", table_bytes, &cap);
+  if (rc) return rc;
+  if ((rc = ensure(e, s.keys, cap)) || (rc = ensure(e, s.counts, cap)) || (rc = ensure(e, s.stats, kKmerStatSlots)) ||
+      (rc = ensure(e, s.matrix, (size_t)kSpecBins * kSpecBins)))
+    return rc;
+  s.capacity = cap;
+  if (capacity) *capacity = (int64_t)cap;
+  return dcb_kmer_set_clear(e, 0, 1);
+}
+
+int dcb_kmer_set_clear(dcb_engine* e, int32_t partition, int32_t n_partitions) {
+  if (!e) return DCB_ERR_INVALID;
+  auto& s = e->km.set;
+  if (!s.capacity) return fail(e, DCB_ERR_STATE, "dcb_kmer_set_clear: no set table (dcb_kmer_set_init)");
+  if (n_partitions < 1 || partition < 0 || partition >= n_partitions)
+    return fail(e, DCB_ERR_INVALID, "dcb_kmer_set_clear: partition %d of %d", partition, n_partitions);
+  CU(e, cudaSetDevice(e->cfg.device));
+  CU(e, cudaMemsetAsync(s.keys.p, 0xff, s.capacity * sizeof(unsigned long long), e->stream));   // every key empty
+  CU(e, cudaMemsetAsync(s.counts.p, 0, s.capacity * sizeof(unsigned int), e->stream));
+  CU(e, cudaMemsetAsync(s.stats.p, 0, kKmerStatSlots * sizeof(unsigned long long), e->stream));
+  CU(e, cudaStreamSynchronize(e->stream));
+  s.partition = partition;
+  s.n_partitions = n_partitions;
+  return DCB_OK;
+}
+
+int dcb_kmer_set_count(dcb_engine* e, const dcb_kmer_batch* b, const uint8_t* keep, int32_t slot) {
+  if (!e) return DCB_ERR_INVALID;
+  auto& km = e->km;
+  if (!km.set.capacity) return fail(e, DCB_ERR_STATE, "dcb_kmer_set_count: no set table (dcb_kmer_set_init)");
+  if (!b || slot < 0 || slot > 1) return fail(e, DCB_ERR_INVALID, "dcb_kmer_set_count: null batch or slot %d", slot);
+  if (b->n_reads < 0 || b->n_bases < 0) return fail(e, DCB_ERR_INVALID, "dcb_kmer_set_count: bad sizes");
+  if (b->n_reads && !keep) return fail(e, DCB_ERR_INVALID, "dcb_kmer_set_count: null array");
+  auto& sl = km.slot[slot];
+  // the batch the last dcb_kmer_query or dcb_kmer_count staged on this slot: its bases and offsets are on the device
+  if (sl.n_bases < 0 || sl.n_reads != b->n_reads || sl.n_bases != b->n_bases)
+    return fail(e, DCB_ERR_INVALID,
+                "dcb_kmer_set_count: slot %d holds %d reads and %lld bases, not this batch's %d and %lld (stage it "
+                "with dcb_kmer_query first)", slot, sl.n_reads, (long long)sl.n_bases, b->n_reads, (long long)b->n_bases);
+  CU(e, cudaSetDevice(e->cfg.device));
+  const uint8_t* d_keep;
+  int rc = stage_in(e, sl.keep, keep, (size_t)b->n_reads, false, &d_keep);
+  if (rc) return rc;
+  const KmerBatch kb{sl.bases.p, nullptr, sl.offsets.p, nullptr, b->n_reads, b->n_bases};
+  sl.query = false;
+  CU(e, cudaEventRecord(sl.ev0, e->stream));
+  launch_kmer_set_count(kmer_set_table(e), kb, d_keep, e->stream);
+  CU(e, cudaGetLastError());
+  CU(e, cudaEventRecord(sl.ev1, e->stream));
+  return DCB_OK;
+}
+
+int dcb_kmer_spectrum(dcb_engine* e, int64_t* matrix, int64_t* stats) {
+  if (!e) return DCB_ERR_INVALID;
+  auto& km = e->km;
+  auto& s = km.set;
+  if (!km.capacity) return fail(e, DCB_ERR_STATE, "dcb_kmer_spectrum: no table (dcb_kmer_table_init)");
+  if (!s.capacity) return fail(e, DCB_ERR_STATE, "dcb_kmer_spectrum: no set table (dcb_kmer_set_init)");
+  if (!matrix) return fail(e, DCB_ERR_INVALID, "dcb_kmer_spectrum: null array");
+  if (s.partition != km.partition || s.n_partitions != km.n_partitions)
+    return fail(e, DCB_ERR_STATE, "dcb_kmer_spectrum: the set table holds partition %d of %d, the table %d of %d",
+                s.partition, s.n_partitions, km.partition, km.n_partitions);
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  constexpr size_t kCells = (size_t)kSpecBins * kSpecBins;
+  CU(e, cudaMemsetAsync(s.matrix.p, 0, kCells * sizeof(unsigned long long), st));
+  launch_kmer_spectrum(kmer_table(e), kmer_set_table(e), s.matrix.p, st);
+  CU(e, cudaGetLastError());
+  std::vector<unsigned long long> m(kCells);
+  unsigned long long v[kKmerStatSlots];
+  CU(e, cudaMemcpyAsync(m.data(), s.matrix.p, kCells * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  CU(e, cudaMemcpyAsync(v, s.stats.p, sizeof v, cudaMemcpyDeviceToHost, st));
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  for (size_t i = 0; i < kCells; ++i) matrix[i] = (int64_t)m[i];
+  if (stats) {
+    stats[0] = (int64_t)s.capacity;
+    for (int i = 0; i < DCB_KMER_SPECTRUM_STATS - 1; ++i) stats[i + 1] = (int64_t)v[i];
+  }
   return DCB_OK;
 }
 

@@ -230,6 +230,13 @@ void launch_kmer_query(const KmerTable& t, const KmerBatch& b, const KmerSegment
 int kmer_hist_grid(unsigned long long capacity);
 void launch_kmer_histogram(const KmerTable& t, unsigned long long* partial, int grid, unsigned long long* hist,
                            cudaStream_t st);
+// The set table (`kmer_qv --spectrum`): the same layout, slot and partition rule, and stats slots 0..3.
+// launch_kmer_set_count counts the k-mers of the reads with keep[r] != 0 (device [n_reads]) into it.
+void launch_kmer_set_count(const KmerTable& set, const KmerBatch& b, const uint8_t* keep, cudaStream_t st);
+// matrix [kSpecBins][kSpecBins] (zeroed by the caller) += distinct keys of the partition by (short count, set count),
+// each capped at kKmerHist.  Both tables hold the same partition.
+constexpr int kSpecBins = kKmerHist + 1;   // DCB_KMER_SPECTRUM_BINS
+void launch_kmer_spectrum(const KmerTable& shrt, const KmerTable& set, unsigned long long* matrix, cudaStream_t st);
 // the CCS ids / qualities of windows list[0..n_list) at full width, window j at off[j] of ccs_ids / ccs_bq
 void launch_features_ccs(const PrepBatch& b, const int4* window, const int32_t* list, int n_list, const int64_t* off,
                          uint8_t* ccs_ids, int16_t* ccs_bq, cudaStream_t st);

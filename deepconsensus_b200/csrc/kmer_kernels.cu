@@ -14,6 +14,11 @@
 //                          dcb_read_identity's arithmetic (quality.cuh).
 //   kmer_combine_kernel    one thread per read sums its segments' counts in segment order.
 //   kmer_histogram_kernel  per-CTA shared histograms of the counts over the table, then a fixed-order reduction.
+//   kmer_set_count_kernel  the count kernel over the reads a per-read keep mask selects, into the set table (the
+//                          evaluated reads' own k-mers, `kmer_qv --spectrum`).
+//   kmer_spectrum_kernel   the copy-number spectrum of the two tables in two grid-stride passes: every set key looked
+//                          up in the short table (bin [c][m]), then every short key missing from the set table (bin
+//                          [c][0]).
 //
 // The slot is the low bits of splitmix64's finalizer of the key and the partition is (mix >> 32) % n_partitions.  The
 // capacity is at most 2^32, so the slot never uses the bits that pick the partition.  Every output is an integer.
@@ -33,6 +38,8 @@ constexpr int kKmerWarps = kKmerThreads / 32;
 constexpr int kKmerRun = 64;                           // k-mer end positions per thread of the count and query kernels
 static_assert(kKmerSegment == kKmerThreads * kKmerRun, "a query segment is one run per thread");
 constexpr unsigned int kKmerSaturate = 0xFFFFFF00u;    // counts stop growing here instead of wrapping
+constexpr int kSpecLowC = 128, kSpecLowM = 64;         // the spectrum's bins kept in shared memory: 32 KB a CTA
+static_assert(kSpecBins == kKmerHist + 1, "the spectrum's axes are the histogram's counts 0..256");
 
 // splitmix64's finalizer (Steele, Lea and Flood, "Fast splittable pseudorandom number generators", 2014)
 __device__ __forceinline__ unsigned long long kmer_mix(unsigned long long z) {
@@ -73,7 +80,10 @@ __device__ __forceinline__ unsigned long long warp_sum(unsigned long long v) {
   return v;
 }
 
-__global__ void __launch_bounds__(kKmerThreads) kmer_count_kernel(KmerTable t, KmerBatch b) {
+// The count kernels' body: this thread's run of kKmerRun end positions, inserted into t.  kMasked: only the reads with
+// keep[r] != 0 (the set count); otherwise every read (the short-read count).
+template <bool kMasked>
+__device__ __forceinline__ void count_run(const KmerTable& t, const KmerBatch& b, const uint8_t* keep) {
   const int64_t g = (int64_t)blockIdx.x * kKmerThreads + threadIdx.x;
   int64_t lo = g * kKmerRun;
   const int64_t hi = min(lo + kKmerRun, b.n_bases);
@@ -89,6 +99,7 @@ __global__ void __launch_bounds__(kKmerThreads) kmer_count_kernel(KmerTable t, K
     for (int r = a; lo < hi && r < b.n_reads; ++r) {
       const int64_t end = min(hi, b.offsets[r + 1]);
       if (end <= lo) continue;
+      if (kMasked && !keep[r]) { lo = end; continue; }
       const int64_t warm = max(b.offsets[r], lo - (t.k - 1));
       for_each_kmer(b.bases, warm, lo, end, t.k, [&](unsigned long long key) {
         const unsigned long long h = kmer_mix(key);
@@ -123,6 +134,72 @@ __global__ void __launch_bounds__(kKmerThreads) kmer_count_kernel(KmerTable t, K
     atomicAdd(&t.stats[2], kmers);
     atomicAdd(&t.stats[3], probes);
   }
+}
+
+__global__ void __launch_bounds__(kKmerThreads) kmer_count_kernel(KmerTable t, KmerBatch b) {
+  count_run<false>(t, b, nullptr);
+}
+
+__global__ void __launch_bounds__(kKmerThreads) kmer_set_count_kernel(KmerTable t, KmerBatch b, const uint8_t* keep) {
+  count_run<true>(t, b, keep);
+}
+
+// The count of `key` (whose mix is h) in t; 0 when the key is absent: its slot run ends at an empty slot.
+__device__ __forceinline__ unsigned int kmer_lookup(const KmerTable& t, unsigned long long key, unsigned long long h) {
+  const unsigned long long mask = t.capacity - 1;
+  unsigned long long slot = h & mask;
+  for (unsigned long long i = 0; i < t.capacity; ++i, slot = (slot + 1) & mask) {
+    const unsigned long long cur = t.keys[slot];
+    if (cur == key) return t.counts[slot];
+    if (cur == kKmerEmpty) return 0;
+  }
+  return 0;
+}
+
+// One pass of the spectrum scan: every key of `scan` with count x is looked up in `probe` (count y).  kSetPass (scan =
+// the set table, probe = the short table): bin [y][x].  Otherwise (scan = the short table, probe = the set table): bin
+// [x][0] for the keys the set lacks.  Both tables hold the same partition, and a present key's count is at least 1.
+//
+// The 257 x 257 bins do not fit in shared memory, but the mass of a spectrum lies at low copy numbers: each CTA keeps
+// the corner c < kSpecLowC, m < kSpecLowM in shared uint32 bins and adds the nonzero ones to the int64 matrix at the
+// end; any other bin goes straight to global memory, one atomicAdd per group of lanes of a warp that share the bin.
+// Every addition is an integer, so the sums are exact and the same for every thread order.  With kmer_hist_grid's
+// grid a CTA scans at most 2^22 slots, so its shared bins cannot wrap.
+template <bool kSetPass>
+__global__ void __launch_bounds__(kKmerThreads) kmer_spectrum_kernel(KmerTable scan, KmerTable probe,
+                                                                      unsigned long long* matrix) {
+  __shared__ unsigned int low[kSpecLowC * kSpecLowM];
+  for (int i = threadIdx.x; i < kSpecLowC * kSpecLowM; i += kKmerThreads) low[i] = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const unsigned long long stride = (unsigned long long)gridDim.x * kKmerThreads;
+  // Warps step in whole groups of 32 slots, and the capacity is a power of two >= 64, so a warp's lanes leave the
+  // loop together and the warp-wide votes below see every lane.
+#pragma unroll 1
+  for (unsigned long long s0 = (unsigned long long)blockIdx.x * kKmerThreads + (threadIdx.x & ~31); s0 < scan.capacity;
+       s0 += stride) {
+    const unsigned long long s = s0 + lane;
+    const unsigned long long key = scan.keys[s];
+    int bin = -1;   // global bin of a key outside the shared corner; -1: none
+    if (key != kKmerEmpty) {
+      const unsigned int x = scan.counts[s];
+      const unsigned int y = kmer_lookup(probe, key, kmer_mix(key));
+      if (kSetPass || y == 0) {
+        const unsigned int c = min(kSetPass ? y : x, (unsigned int)kKmerHist);
+        const unsigned int m = kSetPass ? min(x, (unsigned int)kKmerHist) : 0u;
+        if (c < kSpecLowC && m < kSpecLowM) atomicAdd(&low[c * kSpecLowM + m], 1u);
+        else bin = (int)(c * kSpecBins + m);
+      }
+    }
+    const unsigned int high = __ballot_sync(0xffffffffu, bin >= 0);
+    if (bin >= 0) {
+      const unsigned int peers = __match_any_sync(high, bin);
+      if (lane == __ffs(peers) - 1) atomicAdd(&matrix[bin], (unsigned long long)__popc(peers));
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < kSpecLowC * kSpecLowM; i += kKmerThreads)
+    if (low[i]) atomicAdd(&matrix[(i / kSpecLowM) * kSpecBins + i % kSpecLowM], (unsigned long long)low[i]);
 }
 
 __global__ void __launch_bounds__(kKmerThreads) kmer_query_kernel(KmerTable t, KmerBatch b, KmerSegments sg,
@@ -256,6 +333,17 @@ void launch_kmer_histogram(const KmerTable& t, unsigned long long* partial, int 
                            cudaStream_t st) {
   kmer_histogram_kernel<<<grid, kKmerThreads, 0, st>>>(t.keys, t.counts, t.capacity, partial);
   kmer_histogram_reduce_kernel<<<1, kKmerThreads, 0, st>>>(partial, grid, hist);
+}
+
+void launch_kmer_set_count(const KmerTable& set, const KmerBatch& b, const uint8_t* keep, cudaStream_t st) {
+  if (b.n_reads <= 0 || b.n_bases <= 0) return;
+  const int64_t threads = (b.n_bases + kKmerRun - 1) / kKmerRun;
+  kmer_set_count_kernel<<<(unsigned)((threads + kKmerThreads - 1) / kKmerThreads), kKmerThreads, 0, st>>>(set, b, keep);
+}
+
+void launch_kmer_spectrum(const KmerTable& shrt, const KmerTable& set, unsigned long long* matrix, cudaStream_t st) {
+  kmer_spectrum_kernel<true><<<kmer_hist_grid(set.capacity), kKmerThreads, 0, st>>>(set, shrt, matrix);
+  kmer_spectrum_kernel<false><<<kmer_hist_grid(shrt.capacity), kKmerThreads, 0, st>>>(shrt, set, matrix);
 }
 
 }  // namespace dcb

@@ -57,6 +57,9 @@ ERRORS_COLS = ERRORS_MATRIX + 25
 # dcb_kmer_table_stats: its stats entries and the count histogram's last bin (counts >= DCB_KMER_HIST)
 KMER_STAT_KEYS = ("capacity", "claimed", "overflow", "count_kmers", "count_probes", "query_kmers", "query_probes")
 KMER_HIST = 256
+# dcb_kmer_spectrum: its stats entries and the bins of each axis (counts 0..256, 256 meaning >= 256)
+KMER_SET_STAT_KEYS = ("capacity", "claimed", "overflow", "count_kmers", "count_probes")
+KMER_SPECTRUM_BINS = 257
 DCB_LOGIT_LOSS_MSE, DCB_LOGIT_LOSS_KL = 0, 1
 # Keras loss identifiers (tf.keras.losses.get) of the two logit losses DistillationLoss is used with
 LOGIT_LOSS_IDS = {"mean_squared_error": DCB_LOGIT_LOSS_MSE, "mse": DCB_LOGIT_LOSS_MSE, "MSE": DCB_LOGIT_LOSS_MSE,
@@ -162,7 +165,7 @@ ABI_SYMBOLS = (
     "dcb_read_errors",
     "dcb_seq_open", "dcb_seq_next_batch", "dcb_seq_get_batch", "dcb_seq_read_name", "dcb_seq_close",
     "dcb_kmer_table_init", "dcb_kmer_table_clear", "dcb_kmer_count", "dcb_kmer_query", "dcb_kmer_wait",
-    "dcb_kmer_table_stats",
+    "dcb_kmer_table_stats", "dcb_kmer_set_init", "dcb_kmer_set_clear", "dcb_kmer_set_count", "dcb_kmer_spectrum",
     "dcb_bamw_open", "dcb_bamw_write", "dcb_bamw_close",
     "dcb_last_forward_launches", "dcb_set_profile", "dcb_get_profile", "dcb_get_profile_kernels", "dcb_alloc_host",
     "dcb_free_host", "dcb_alloc_device", "dcb_free_device", "dcb_memcpy_h2d", "dcb_memcpy_d2h",
@@ -248,6 +251,10 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_kmer_query.argtypes = [vp, ctypes.POINTER(DcbKmerBatch), i32, i32, i32]
   lib.dcb_kmer_wait.argtypes = [vp, i32, vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_kmer_table_stats.argtypes = [vp, vp, vp]
+  lib.dcb_kmer_set_init.argtypes = [vp, ctypes.c_int64, ctypes.POINTER(ctypes.c_int64)]
+  lib.dcb_kmer_set_clear.argtypes = [vp, i32, i32]
+  lib.dcb_kmer_set_count.argtypes = [vp, ctypes.POINTER(DcbKmerBatch), vp, i32]
+  lib.dcb_kmer_spectrum.argtypes = [vp, vp, vp]
   lib.dcb_last_forward_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_last_forward_launches.argtypes = [vp, ctypes.POINTER(i32)]
   lib.dcb_set_debug.argtypes = [vp, i32]
@@ -930,6 +937,35 @@ class B200Model:
     if histogram:
       out["histogram"] = hist
     return out
+
+  def kmer_set_init(self, table_bytes: int) -> int:
+    """dcb_kmer_set_init: an empty set table (the evaluated reads' k-mers) in at most table_bytes of device memory
+    (<= 0: half the free memory), after kmer_table_init; returns its capacity in slots."""
+    cap = ctypes.c_int64(0)
+    self._check(self._lib.dcb_kmer_set_init(self._handle, int(table_bytes), ctypes.byref(cap)))
+    return int(cap.value)
+
+  def kmer_set_clear(self, partition: int, n_partitions: int) -> None:
+    self._check(self._lib.dcb_kmer_set_clear(self._handle, int(partition), int(n_partitions)))
+
+  def kmer_set_submit(self, handle, keep: np.ndarray) -> Tuple[int, int, DcbKmerBatch, Tuple[np.ndarray, ...]]:
+    """dcb_kmer_set_count of the batch a kmer_submit `handle` (already waited for) staged, on the same slot, for the
+    reads with keep[r] (bool or uint8 [n]).  Returns the handle kmer_wait takes."""
+    slot, _, arg, arrays = handle
+    keep = np.ascontiguousarray(keep, np.uint8)
+    if keep.shape != (arg.n_reads,):
+      raise ValueError("keep must have one entry per read of the batch, got shape %s" % (keep.shape,))
+    self._check(self._lib.dcb_kmer_set_count(self._handle, ctypes.byref(arg), _ptr(keep), int(slot)))
+    return int(slot), 0, arg, arrays + (keep,)
+
+  def kmer_spectrum(self) -> Dict[str, Any]:
+    """dcb_kmer_spectrum of the partition both tables hold: dict(matrix int64 [KMER_SPECTRUM_BINS,
+    KMER_SPECTRUM_BINS] ([c][m] = distinct k-mers with table count c and set count m, 256 meaning >= 256), stats dict
+    of KMER_SET_STAT_KEYS)."""
+    b = KMER_SPECTRUM_BINS
+    matrix, stats = np.zeros((b, b), np.int64), np.zeros(len(KMER_SET_STAT_KEYS), np.int64)
+    self._check(self._lib.dcb_kmer_spectrum(self._handle, _ptr(matrix), _ptr(stats)))
+    return dict(matrix=matrix, stats={k: int(v) for k, v in zip(KMER_SET_STAT_KEYS, stats)})
 
   def stitch_raw(self, bases_ptr: int, quals_ptr: int, n_windows: int, zmw_start: np.ndarray, flags: int,
                  seq_ptr: int, qual_ptr: int, len_ptr: int, length: Optional[int] = None) -> None:

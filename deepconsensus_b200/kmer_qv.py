@@ -8,6 +8,10 @@ below the predicted quality `--min_quality` (round(avg_phred(QUAL), 5), as `run`
 a baseline (the CCS reads of the same run) the JSON also holds the baseline's object and the relative yield gain per
 threshold.  The contract is stated in the README ("k-mer QV").
 
+With `--spectrum`, a second device table (the set table) counts the k-mers of each read set's counted reads, and a
+scan of both tables gives the copy-number spectrum (distinct k-mers by short-read count and count in the set) and
+k-mer completeness (the share of the short reads' solid k-mers the set holds), as Merqury and KAT report them.
+
 When the short reads' distinct k-mers do not fit the table, the k-mers are split into partitions by their hash and
 each partition is counted and queried in a pass of its own, re-reading the files.  The files are read by host C++
 (csrc/bam_prep.cpp, dcb_seq_*); counting and lookup are CUDA kernels (csrc/kmer_kernels.cu, dcb_kmer_*).  The device
@@ -33,6 +37,7 @@ YIELD_THRESHOLDS = (20, 30, 40)
 CURVE_MAX_Q = 60
 MAX_K = 31
 BATCH_BASES = 1 << 26
+SLOT_BYTES = 12   # a table slot: uint64 key and uint32 count
 
 
 class KmerQvError(RuntimeError):
@@ -117,10 +122,16 @@ class KmerTable:
   """The short reads' k-mer counts on the device, one partition at a time (count_kmers builds it)."""
 
   def __init__(self, model: engine_lib.B200Model, own: bool, files: Sequence[str], k: int, min_count: int,
-               partitions: int, capacity: int, batch_bases: int):
+               partitions: int, capacity: int, batch_bases: int, set_capacity: int = 0):
     self.model, self._own, self.files, self.k, self.min_count = model, own, list(files), k, min_count
     self.partitions, self.capacity, self.batch_bases = partitions, capacity, batch_bases
+    self.set_capacity = set_capacity   # slots of the set table (count_kmers(..., spectrum=True)); 0: none
     self.partition = -1   # the partition the device holds; -1: none
+
+  def split(self) -> None:
+    """Twice the partitions (the set table overflowed): the next load recounts from the short reads."""
+    self.partitions *= 2
+    self.partition = -1
 
   def load(self, p: int, timing: Optional[Dict[str, float]] = None) -> Dict[str, Any]:
     """Counts partition p of the short reads into the table (a no-op when it is there); returns the table's stats
@@ -150,11 +161,12 @@ class KmerTable:
 
 def count_kmers(files: Sequence[str], k: int = MAX_K, min_count: int = 2, partitions: int = 1,
                 table_bytes: int = 0, model: Optional[engine_lib.B200Model] = None, batch_bases: int = BATCH_BASES,
-                timing: Optional[Dict[str, float]] = None) -> Tuple[KmerTable, Dict[str, Any]]:
+                timing: Optional[Dict[str, float]] = None, spectrum: bool = False) -> Tuple[KmerTable, Dict[str, Any]]:
   """Counts the canonical k-mers of the short reads in `files`.  The table takes table_bytes of device memory (<= 0:
-  half the free memory).  Starting from `partitions`, the partition count doubles until no partition's distinct
-  k-mers exceed 0.8 x the table's capacity.  Returns the table (holding its last partition) and the JSON object
-  `short_reads`."""
+  half the free memory).  With `spectrum`, that budget is split evenly between the table and the set table that
+  read_kmers(..., spectrum=True) counts the evaluated reads into, so each gets half the slots the table alone would.
+  Starting from `partitions`, the partition count doubles until no partition's distinct k-mers exceed 0.8 x the
+  table's capacity.  Returns the table (holding its last partition) and the JSON object `short_reads`."""
   if not 1 <= k <= MAX_K:
     raise ValueError("k must be between 1 and %d, got %d" % (MAX_K, k))
   if not 1 <= min_count <= engine_lib.KMER_HIST:
@@ -167,10 +179,16 @@ def count_kmers(files: Sequence[str], k: int = MAX_K, min_count: int = 2, partit
   if own:
     model = cbc._default_model()
   try:
-    capacity = model.kmer_table_init(table_bytes, k)
+    set_capacity = 0
+    if spectrum:
+      budget = table_bytes if table_bytes > 0 else SLOT_BYTES * model.kmer_table_init(0, k)   # the default's slots
+      capacity = model.kmer_table_init(budget // 2, k)
+      set_capacity = model.kmer_set_init(budget // 2)
+    else:
+      capacity = model.kmer_table_init(table_bytes, k)
     P = partitions
     while True:
-      table = KmerTable(model, own, files, k, min_count, P, capacity, batch_bases)
+      table = KmerTable(model, own, files, k, min_count, P, capacity, batch_bases, set_capacity)
       hist = np.zeros(engine_lib.KMER_HIST + 1, np.int64)
       kmers = 0
       t: Dict[str, float] = {}
@@ -198,11 +216,36 @@ def count_kmers(files: Sequence[str], k: int = MAX_K, min_count: int = 2, partit
 
 
 def read_kmers(files: Sequence[str], table: KmerTable, batch_bases: int = BATCH_BASES,
-               timing: Optional[Dict[str, float]] = None) -> Dict[str, Any]:
+               timing: Optional[Dict[str, float]] = None, spectrum: bool = False,
+               min_quality: int = 20) -> Dict[str, Any]:
   """The per-read arrays of the reads in `files`, in input order: names (list), length, kmers (T), unsupported (U)
   (int64), avg_q (float64: avg_phred of the qualities, NaN for a read without them; NumPy's own value where the
   quality filter could turn on its last bits) and has_quality (bool).  Each partition of the table is one pass over
-  the files; T and U are summed over the passes."""
+  the files; T and U are summed over the passes.
+
+  With `spectrum` (the table from count_kmers(..., spectrum=True)), each pass also counts the k-mers of the reads that
+  qv_summary(..., min_quality) counts (reads without qualities always) into the set table, and scans both tables.
+  The result then also holds `spectrum`: dict(matrix int64 [257, 257], [c][m] = distinct k-mers with short count c
+  and count m in the counted reads, 256 meaning >= 256, summed over the partitions; stats: the set table's capacity,
+  and its claimed keys, k-mers counted and probe steps summed).  When the set table overflows, the table's
+  partitions double and the reads are read again from the start."""
+  if spectrum and not table.set_capacity:
+    raise ValueError("read_kmers(..., spectrum=True) needs the table of count_kmers(..., spectrum=True)")
+  while True:
+    out = _read_pass(files, table, batch_bases, timing, spectrum, min_quality)
+    if out is not None:
+      return out
+    table.split()
+
+
+def _passes_quality(avg_q: np.ndarray, has_q: np.ndarray, min_quality: int) -> np.ndarray:
+  """qv_summary's quality rule per read: no qualities, or round(avg_q, 5) >= min_quality (uint8)."""
+  return np.array([not h or round(float(a), 5) >= min_quality for a, h in zip(avg_q, has_q)], np.uint8)
+
+
+def _read_pass(files: Sequence[str], table: KmerTable, batch_bases: int, timing: Optional[Dict[str, float]],
+               spectrum: bool, min_quality: int) -> Optional[Dict[str, Any]]:
+  """read_kmers over the table's partitions as they stand; None when the set table overflowed."""
   model = table.model
   order = ([table.partition] if table.partition >= 0 else []) + [p for p in range(table.partitions)
                                                                   if p != table.partition]
@@ -213,6 +256,11 @@ def read_kmers(files: Sequence[str], table: KmerTable, batch_bases: int = BATCH_
   has_q: List[np.ndarray] = []
   first: List[np.ndarray] = []
   counts = np.zeros((0, 2), np.int64)
+  keeps: List[np.ndarray] = []   # per batch: the reads the set table counts (from the first pass's avg_q)
+  matrix = np.zeros((engine_lib.KMER_SPECTRUM_BINS,) * 2, np.int64)
+  set_stats = dict(capacity=table.set_capacity, claimed=0, overflow=0, count_kmers=0, count_probes=0)
+  if spectrum:
+    t["set_device_ms"] = 0.0
   for i, p in enumerate(order):
     tc: Dict[str, float] = {}
     if table.load(p, tc).get("overflow"):
@@ -220,10 +268,20 @@ def read_kmers(files: Sequence[str], table: KmerTable, batch_bases: int = BATCH_
     t["count_host_s"] += tc.get("host_s", 0.0)
     t["count_device_ms"] += tc.get("device_ms", 0.0)
     items = ((j % 2, b) for j, b in enumerate(read_batches(files, batch_bases, t, names=i == 0)))
-    submit = lambda it: model.kmer_submit(it[1], it[0], table.min_count, with_quality=i == 0)
+    pending: List[Any] = [None, None]   # per slot: its set count, not yet waited for
+
+    def submit(it):
+      if pending[it[0]] is not None:   # the slot's set count is done (and timed) before the slot takes a new batch
+        t["set_device_ms"] += model.kmer_wait(pending[it[0]])["ms"]
+        pending[it[0]] = None
+      return model.kmer_submit(it[1], it[0], table.min_count, with_quality=i == 0)
+
+    wait = lambda h: dict(model.kmer_wait(h), handle=h)
+    if spectrum:
+      model.kmer_set_clear(p, table.partitions)
     at = 0
-    with contextlib.closing(engine_lib.pipelined(items, submit, model.kmer_wait, model.kmer_retire)) as done:
-      for (_, b), res in done:
+    with contextlib.closing(engine_lib.pipelined(items, submit, wait, model.kmer_retire)) as done:
+      for bi, ((slot, b), res) in enumerate(done):
         t["device_ms"] += res["ms"]
         n = len(b["offsets"]) - 1
         if i == 0:
@@ -242,17 +300,34 @@ def read_kmers(files: Sequence[str], table: KmerTable, batch_bases: int = BATCH_
           avg_q.append(q)
           has_q.append(hq)
           first.append(res["counts"])
+          if spectrum:
+            keeps.append(_passes_quality(q, hq, min_quality))
           t["host_s"] += time.perf_counter() - t0
         else:
           counts[at:at + n] += res["counts"]
+        if spectrum:   # the reads the QV counts, into the set table, from the batch the query staged on this slot
+          pending[slot] = model.kmer_set_submit(res["handle"], keeps[bi])
         at += n
+    for h in pending:
+      if h is not None:
+        t["set_device_ms"] += model.kmer_wait(h)["ms"]
     if i == 0:
       counts = np.concatenate(first) if first else np.zeros((0, 2), np.int64)
+    if spectrum:
+      sp = model.kmer_spectrum()
+      if sp["stats"]["overflow"]:
+        return None
+      matrix += sp["matrix"]
+      for key in ("claimed", "count_kmers", "count_probes"):
+        set_stats[key] += sp["stats"][key]
   if timing is not None:
     timing.update(t)
   cat = lambda parts, dt: np.concatenate(parts).astype(dt) if parts else np.zeros(0, dt)
-  return dict(names=names, length=cat(length, np.int64), kmers=counts[:, 0].copy(), unsupported=counts[:, 1].copy(),
-              avg_q=cat(avg_q, np.float64), has_quality=cat(has_q, bool))
+  out = dict(names=names, length=cat(length, np.int64), kmers=counts[:, 0].copy(), unsupported=counts[:, 1].copy(),
+             avg_q=cat(avg_q, np.float64), has_quality=cat(has_q, bool))
+  if spectrum:
+    out["spectrum"] = dict(matrix=matrix, stats=set_stats)
+  return out
 
 
 def error_rate(kmers: np.ndarray, unsupported: np.ndarray, k: int) -> np.ndarray:
@@ -301,6 +376,18 @@ def qv_summary(per_read: Dict[str, Any], k: int, min_quality: int) -> Dict[str, 
   return out
 
 
+def spectrum_summary(spectrum: Dict[str, Any], min_count: int, k: int) -> Dict[str, Any]:
+  """The JSON object `spectrum` of one read set from read_kmers(..., spectrum=True)'s `spectrum`: k; solid_kmers
+  (distinct k-mers with short count >= min_count), solid_found (those the set holds), completeness (their ratio, None
+  without solid k-mers), set_distinct_kmers (distinct k-mers of the set), set_only_kmers (those with short count 0)
+  and matrix, the nonzero cells as [c, m, n] sorted by c, then m."""
+  M = np.asarray(spectrum["matrix"], np.int64)
+  solid, found = int(M[min_count:].sum()), int(M[min_count:, 1:].sum())
+  return dict(k=int(k), solid_kmers=solid, solid_found=found, completeness=found / solid if solid else None,
+              set_distinct_kmers=int(M[:, 1:].sum()), set_only_kmers=int(M[0, 1:].sum()),
+              matrix=[[int(c), int(m), int(M[c, m])] for c, m in zip(*np.nonzero(M))])
+
+
 def yield_over_baseline(summary: Dict[str, Any], baseline: Dict[str, Any]) -> Dict[str, Optional[float]]:
   """(dc - ccs) / ccs of the yield per threshold; None where the baseline's yield is 0."""
   return {key: (summary["yield"][key] - v) / v if v else None for key, v in baseline["yield"].items()}
@@ -328,19 +415,31 @@ def main(argv: Optional[List[str]] = None) -> int:
   ap.add_argument("--k", type=int, default=MAX_K)
   ap.add_argument("--min_count", type=int, default=2, help="short-read count at which a k-mer is supported")
   ap.add_argument("--min_quality", type=int, default=20, help="reads with round(avg_phred, 5) below it are not counted")
-  ap.add_argument("--table_gb", type=float, default=0.0, help="device memory of the k-mer table; default half the free")
+  ap.add_argument("--table_gb", type=float, default=0.0,
+                  help="device memory of the k-mer table(s); default half the free; --spectrum splits it evenly")
   ap.add_argument("--partitions", type=int, default=1, help="k-mer partitions to start from (doubled on overflow)")
+  ap.add_argument("--spectrum", action="store_true",
+                  help="add k-mer completeness and the copy-number spectrum to each read set's object")
   ap.add_argument("--output_tsv", default=None, help="per-read name, length, kmers, unsupported, avg_q, qv")
   ap.add_argument("--output_json", required=True)
   a = ap.parse_args(argv)
   model = cbc._default_model()
   try:
-    table, short = count_kmers(a.short_reads, a.k, a.min_count, a.partitions, int(a.table_gb * 2**30), model)
-    dc = read_kmers(a.reads, table)
-    out = qv_summary(dc, a.k, a.min_quality)
+    table, short = count_kmers(a.short_reads, a.k, a.min_count, a.partitions, int(a.table_gb * 2**30), model,
+                               spectrum=a.spectrum)
+
+    def measure(files):
+      pr = read_kmers(files, table, spectrum=a.spectrum, min_quality=a.min_quality)
+      s = qv_summary(pr, a.k, a.min_quality)
+      if a.spectrum:
+        s["spectrum"] = spectrum_summary(pr["spectrum"], a.min_count, a.k)
+      return pr, s
+
+    dc, out = measure(a.reads)
     if a.baseline:
-      out["baseline"] = qv_summary(read_kmers(a.baseline, table), a.k, a.min_quality)
+      out["baseline"] = measure(a.baseline)[1]
       out["yield_over_baseline"] = yield_over_baseline(out, out["baseline"])
+    short["partitions"] = table.partitions   # a set table's overflow doubles them
     out["short_reads"] = short
   except ValueError as e:   # k, min_count or partitions out of range
     ap.error(str(e))

@@ -698,6 +698,29 @@ int dcb_kmer_query(dcb_engine* e, const dcb_kmer_batch* b, int32_t min_count, in
 int dcb_kmer_wait(dcb_engine* e, int32_t slot, int64_t* counts, double* avg_q, int32_t* borderline, float* ms_out);
 int dcb_kmer_table_stats(dcb_engine* e, int64_t* stats, int64_t* histogram);
 
+/* The copy-number spectrum (`kmer_qv --spectrum`): a second table, the set table, counts the evaluated reads' own
+ * k-mers with the table's layout, slot and partition rule and k, and a scan bins every distinct key of one partition
+ * by its count in both tables.
+ *   dcb_kmer_set_init   allocates the set table as dcb_kmer_table_init sizes the table (after dcb_kmer_table_init).
+ *   dcb_kmer_set_clear  empties it for the keys of one partition.
+ *   dcb_kmer_set_count  counts the k-mers of the partition of the reads r with keep[r] != 0 (host [n_reads]) into the
+ *                       set table, as dcb_kmer_count counts.  It reuses the bases and offsets that the last
+ *                       dcb_kmer_query (or dcb_kmer_count) on the same slot staged; b must be that batch, and only its
+ *                       sizes are checked.  It overflows as the table does.  Waited on with dcb_kmer_wait, which writes
+ *                       nothing but the device time.
+ *   dcb_kmer_spectrum   (both tables holding the same partition) matrix[c * DCB_KMER_SPECTRUM_BINS + m] = distinct
+ *                       keys of the partition with table count min(c, 256) and set count min(m, 256): the set's keys
+ *                       for m >= 1, the table's keys the set lacks in column 0; [0][0] is 0.  stats
+ *                       [DCB_KMER_SPECTRUM_STATS] = the set table's capacity, distinct keys claimed, overflow, k-mers
+ *                       counted, their probe steps.  Exact integers, whatever the thread order: the host sums the
+ *                       partitions. */
+#define DCB_KMER_SPECTRUM_BINS 257
+#define DCB_KMER_SPECTRUM_STATS 5
+int dcb_kmer_set_init(dcb_engine* e, int64_t table_bytes, int64_t* capacity);
+int dcb_kmer_set_clear(dcb_engine* e, int32_t partition, int32_t n_partitions);
+int dcb_kmer_set_count(dcb_engine* e, const dcb_kmer_batch* b, const uint8_t* keep, int32_t slot);
+int dcb_kmer_spectrum(dcb_engine* e, int64_t* matrix, int64_t* stats);
+
 /* Device time of the last dcb_forward (milliseconds, CUDA events on the engine's stream). */
 int dcb_last_forward_ms(dcb_engine* e, float* ms);
 /* Number of engine kernels launched by the last dcb_forward. */
