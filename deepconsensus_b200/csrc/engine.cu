@@ -166,6 +166,8 @@ struct dcb_engine {
   struct Strict {
     DevBuf<float> emb, x, y, q, k, v, att, hid;
     int chunk_windows = 0;   // 0 until the workspace is allocated
+    DevBuf<float> dbg;       // debug capture of the float32 forward (f32_images), allocated while debug is on
+    int dbg_tokens = -1;     // tokens of the last captured chunk; -1: no float32 forward since capture was turned on
   } strict;
   // Host-or-device staging of the entry points besides the forward, one buffer per array, grown on demand (ensure,
   // stage_in, stage_out).  Every such call ends with a stream synchronisation, so the next one may reuse them.
@@ -680,8 +682,43 @@ struct StrictGemm {
 const StrictGemm kStrictGemm{launch_strict_gemm, false};
 const StrictGemm kTf32x3Gemm{launch_tf32x3_gemm, true};
 
+// One float32 image the debug capture of the float32 forward keeps: the stage and DCB_DEBUG_F32_* id it is read back
+// by, the workspace buffer it is copied from, and its width.
+struct F32Image { int stage, which; DevBuf<float> dcb_engine::Strict::*src; int width; };
+
+// Every image the float32 capture keeps, in the order Strict::dbg stores them, each [strict chunk tokens][width]
+// (include/dcb200_debug.h documents the list).
+std::vector<F32Image> f32_images(const dcb_engine* e) {
+  using S = dcb_engine::Strict;
+  const int layers = e->cfg.num_hidden_layers, ff = e->cfg.filter_size;
+  const bool ln = !e->cfg.rezero;
+  std::vector<F32Image> v = {{0, DCB_DEBUG_F32_EMB, &S::emb, e->E}, {0, DCB_DEBUG_F32_X, &S::x, kD}};
+  for (int n = 0; n < layers; ++n) {
+    const int sa = 1 + 2 * n, sf = 2 + 2 * n;
+    if (ln) v.push_back({sa, DCB_DEBUG_F32_Y, &S::y, kD});
+    v.insert(v.end(), {{sa, DCB_DEBUG_F32_Q, &S::q, kD}, {sa, DCB_DEBUG_F32_K, &S::k, kD},
+                       {sa, DCB_DEBUG_F32_V, &S::v, kD}, {sa, DCB_DEBUG_F32_ATT, &S::att, kD},
+                       {sa, DCB_DEBUG_F32_X, &S::x, kD}});
+    if (ln) v.push_back({sf, DCB_DEBUG_F32_Y, &S::y, kD});
+    v.insert(v.end(), {{sf, DCB_DEBUG_F32_HID, &S::hid, ff}, {sf, DCB_DEBUG_F32_X, &S::x, kD}});
+  }
+  return v;
+}
+
+// Where Strict::dbg keeps image `which` of `stage`: its first column (per token of a full strict chunk) and its width.
+// False for a pair that is not captured.
+bool f32_image_slot(const dcb_engine* e, int stage, int which, size_t* cols, int* width) {
+  *cols = 0;
+  for (const F32Image& im : f32_images(e)) {
+    if (im.stage == stage && im.which == which) { *width = im.width; return true; }
+    *cols += im.width;
+  }
+  return false;
+}
+
 // One chunk of the strict-fp32 or tf32x3 forward (strict_kernels.cu, with the GEMM of `gemm`): rows [bw, R, L] ->
-// outputs via hp.  Its launches are counted, not profiled.
+// outputs via hp.  Its launches are counted, not profiled.  With debug capture on, the images of f32_images are
+// copied aside as the launches write them (stream-ordered copies, no launches).
 void strict_forward_chunk(dcb_engine* e, LaunchRecorder& rec, const float* rows_chunk, int bw, HeadParams hp,
                           int* d_status, const StrictGemm& gemm) {
   const dcb_config& c = e->cfg;
@@ -689,17 +726,31 @@ void strict_forward_chunk(dcb_engine* e, LaunchRecorder& rec, const float* rows_
   const Weights& W = e->w;
   const int L = e->L, M = bw * L, ff = c.filter_size;
   const cudaStream_t st = rec.st;
+  // copies the images of `stage` whose id is in `whiches` (the ones the launches since the previous call wrote)
+  auto snap = [&](int stage, std::initializer_list<int> whiches) {
+    if (!e->debug || !S.dbg) return;
+    const size_t Mc = (size_t)S.chunk_windows * L;
+    size_t cols = 0;
+    for (const F32Image& im : f32_images(e)) {
+      if (im.stage == stage && std::find(whiches.begin(), whiches.end(), im.which) != whiches.end())
+        cudaMemcpyAsync(S.dbg + cols * Mc, (S.*im.src).p, (size_t)M * im.width * sizeof(float), cudaMemcpyDeviceToDevice,
+                        st);
+      cols += im.width;
+    }
+  };
   rec.run(kProfNone, 2, [&] {
     launch_strict_embed(rows_chunk, e->R, L, e->E, bw, W.strict.embed, W.strict.tables, S.emb, d_status, st);
     StrictEpi ep;
     if (c.add_pos_encoding) { ep.pe = W.strict.pe; ep.pe_L = L; }
     gemm.launch(S.emb, gemm.tf32x3 ? W.tf32x3_wc.p : W.strict.wc.p, S.x, M, kD, e->E, ep, st);   // networks.py:509-516, :319-323
+    snap(0, {DCB_DEBUG_F32_EMB, DCB_DEBUG_F32_X});
   });
   const float qscale = 1.0f / sqrtf((float)kDH);                                       // attention_layer.py:196-197
   for (int n_ = 0; n_ < c.num_hidden_layers; ++n_) {
     const LayerDev& ld = W.layers[n_];
     const StrictMats& wm = gemm.tf32x3 ? ld.tf32x3 : static_cast<const StrictMats&>(ld.strict);
     const float* yin = c.rezero ? S.x.p : S.y.p;   // each sub-layer's input: x, or LayerNorm(x) in y
+    const int sa = 1 + 2 * n_, sf = 2 + 2 * n_;
     rec.run(kProfNone, c.rezero ? 7 : 9, [&] {
       if (!c.rezero) launch_strict_layernorm(S.x, S.y, M, ld.ln_g[0], ld.ln_b[0], st);
       StrictEpi eq; eq.scale = qscale;
@@ -709,15 +760,18 @@ void strict_forward_chunk(dcb_engine* e, LaunchRecorder& rec, const float* rows_
       launch_strict_attention(S.q, S.k, S.v, S.att, bw, L, c.attn_win_size, st);
       StrictEpi eo; eo.residual = S.x; eo.scale = c.rezero ? ld.strict.alpha[0] : 1.f;     // encoder_stack.py:88-92
       gemm.launch(S.att, wm.wo, S.x, M, kD, kD, eo, st);
+      snap(sa, {DCB_DEBUG_F32_Y, DCB_DEBUG_F32_Q, DCB_DEBUG_F32_K, DCB_DEBUG_F32_V, DCB_DEBUG_F32_ATT, DCB_DEBUG_F32_X});
       if (!c.rezero) launch_strict_layernorm(S.x, S.y, M, ld.ln_g[1], ld.ln_b[1], st);
       StrictEpi e1; e1.bias = ld.b1; e1.relu = 1;                                      // ffn_layer.py:83-86
       gemm.launch(yin, wm.w1, S.hid, M, ff, kD, e1, st);
       StrictEpi e2; e2.bias = ld.strict.b2; e2.residual = S.x; e2.scale = c.rezero ? ld.strict.alpha[1] : 1.f;
       gemm.launch(S.hid, wm.w2, S.x, M, kD, ff, e2, st);
+      snap(sf, {DCB_DEBUG_F32_Y, DCB_DEBUG_F32_HID, DCB_DEBUG_F32_X});
     });
   }
   hp.x = S.x; hp.M = M; hp.L = L; hp.Lw = L;
   rec.run(kProfNone, 1, [&] { launch_strict_head(S.x, M, hp, st); });
+  if (e->debug && S.dbg) S.dbg_tokens = M;
 }
 
 // The row epilogue of the bf16 forward's residual GEMMs: x = [x_old +] product [+ bias] [+ positional encoding], and
@@ -1030,6 +1084,11 @@ int dcb_load_weights(dcb_engine* e, const dcb_tensor* tensors, int32_t n) {
 int dcb_set_debug(dcb_engine* e, int32_t enabled) {
   if (!e) return DCB_ERR_INVALID;
   e->debug = enabled != 0;
+  if (!e->debug && e->strict.dbg) {   // the float32 capture exists only while debug is on (it can be large)
+    CU(e, cudaSetDevice(e->cfg.device));
+    e->strict.dbg.reset();
+    e->strict.dbg_tokens = -1;
+  }
   if (e->debug && !e->d_dbg) {
     CU(e, cudaSetDevice(e->cfg.device));
     const size_t stages = 1 + 2 * (size_t)e->cfg.num_hidden_layers;
@@ -1085,6 +1144,13 @@ static int submit_impl(dcb_engine* e, const float* rows, const uint8_t* packed, 
     if (!rc) rc = alloc(e, S.hid, Mc * c.filter_size);
     if (rc) return rc;
     S.chunk_windows = cw;
+  }
+  if (f32 && e->debug && !e->strict.dbg) {
+    // the float32 capture, on the first float32 forward with debug on: every image of f32_images for a full chunk
+    size_t cols = 0;
+    for (const F32Image& im : f32_images(e)) cols += im.width;
+    int rc = alloc(e, e->strict.dbg, cols * e->strict.chunk_windows * L);
+    if (rc) return rc;
   }
   cudaStream_t st = e->stream;
   if (packed && !rows_dev && !sl.d_packed) {
@@ -1298,6 +1364,23 @@ int dcb_debug_operand(dcb_engine* e, int32_t stage, int32_t which, uint16_t* out
     return fail(e, DCB_ERR_INVALID, "operand %d is not captured at stage %d", which, stage);
   const __nv_bfloat16* img = e->d_dbg_op + cols * e->chunk_tiles * kTileM;
   return read_capture<8>(e, reinterpret_cast<const uint16_t*>(img), w, w, out, out_elems);
+}
+
+int dcb_debug_f32(dcb_engine* e, int32_t stage, int32_t which, float* out, int64_t out_elems) {
+  if (!e || !out) return DCB_ERR_INVALID;
+  const dcb_engine::Strict& S = e->strict;
+  if (!e->debug) return fail(e, DCB_ERR_STATE, "debug capture not enabled");
+  if (!S.dbg || S.dbg_tokens < 0) return fail(e, DCB_ERR_STATE, "no float32 forward since debug capture was enabled");
+  size_t cols = 0;
+  int w = 0;
+  if (!f32_image_slot(e, stage, which, &cols, &w))
+    return fail(e, DCB_ERR_INVALID, "float32 image %d is not captured at stage %d", which, stage);
+  const size_t n = (size_t)S.dbg_tokens * w;
+  if (out_elems < (int64_t)n) return fail(e, DCB_ERR_INVALID, "output too small: need %lld", (long long)n);
+  CU(e, cudaSetDevice(e->cfg.device));
+  CU(e, cudaStreamSynchronize(e->stream));
+  CU(e, cudaMemcpy(out, S.dbg + cols * S.chunk_windows * e->L, n * sizeof(float), cudaMemcpyDeviceToHost));
+  return DCB_OK;
 }
 
 // read z is the windows [zmw_start[z], zmw_start[z + 1]) of n_windows

@@ -172,9 +172,11 @@ ABI_SYMBOLS = (
     "dcb_synchronize", "dcb_last_error", "dcb_version", "dcb_destroy",
 )
 # include/dcb200_debug.h: developer / test hooks, not part of the drop-in boundary
-DEBUG_SYMBOLS = ("dcb_set_debug", "dcb_debug_residual", "dcb_debug_operand", "dcb_debug_head_epilogue")
+DEBUG_SYMBOLS = ("dcb_set_debug", "dcb_debug_residual", "dcb_debug_operand", "dcb_debug_f32", "dcb_debug_head_epilogue")
 # dcb_debug_operand's image ids (DCB_DEBUG_*)
 DEBUG_OPERANDS = {"embed": 0, "xb": 1, "qkv": 2, "att": 3, "hid": 4}
+# dcb_debug_f32's image ids (DCB_DEBUG_F32_*)
+DEBUG_F32 = {"emb": 0, "x": 1, "y": 2, "q": 3, "k": 4, "v": 5, "att": 6, "hid": 7}
 
 
 def library_path() -> str:
@@ -264,6 +266,7 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_get_profile_kernels.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(i32)]
   lib.dcb_debug_residual.argtypes = [vp, i32, vp, ctypes.c_int64]
   lib.dcb_debug_operand.argtypes = [vp, i32, i32, vp, ctypes.c_int64]
+  lib.dcb_debug_f32.argtypes = [vp, i32, i32, vp, ctypes.c_int64]
   lib.dcb_debug_head_epilogue.argtypes = [vp, vp, ctypes.c_int64, vp, vp, vp]
   lib.dcb_alloc_host.argtypes = [ctypes.c_size_t, ctypes.POINTER(vp)]
   lib.dcb_free_host.argtypes = [vp]
@@ -1195,6 +1198,26 @@ class B200Model:
                 qkv=[self.debug_operand(1 + 2 * n, "qkv", tokens) for n in range(nl)],
                 att=[self.debug_operand(1 + 2 * n, "att", tokens) for n in range(nl)],
                 hid=[self.debug_operand(2 + 2 * n, "hid", tokens) for n in range(nl)])
+
+  def debug_f32(self, stage: int, which: str, tokens: int) -> np.ndarray:
+    """dcb_debug_f32: float32 image `which` (a DEBUG_F32 key) of the last float32 forward's last chunk, captured at
+    `stage`, as float32 [tokens, width]."""
+    width = {"emb": params_lib.embedded_width(self.params), "hid": int(self.params.filter_size)}.get(which, 280)
+    out = np.empty((tokens, width), np.float32)
+    self._check(self._lib.dcb_debug_f32(self._handle, stage, DEBUG_F32[which], _ptr(out), out.size))
+    return out
+
+  def debug_capture_f32(self, tokens: int) -> Dict[str, object]:
+    """Everything the float32 capture kept of the last chunk's `tokens` tokens, shaped like debug_capture's: emb; x,
+    the residual of every stage; y, the LayerNorm output by stage (pre-LN models; empty for ReZero); and per layer q,
+    k, v, att and hid."""
+    nl = int(self.params.num_hidden_layers)
+    att_stages, ffn_stages = [1 + 2 * n for n in range(nl)], [2 + 2 * n for n in range(nl)]
+    return dict(emb=self.debug_f32(0, "emb", tokens),
+                x=[self.debug_f32(s, "x", tokens) for s in range(1 + 2 * nl)],
+                y={} if self.params.rezero else {s: self.debug_f32(s, "y", tokens) for s in att_stages + ffn_stages},
+                **{k: [self.debug_f32(s, k, tokens) for s in att_stages] for k in ("q", "k", "v", "att")},
+                hid=[self.debug_f32(s, "hid", tokens) for s in ffn_stages])
 
   def debug_head_epilogue(self, logits: np.ndarray) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
     """dcb_debug_head_epilogue: the head's per-token epilogue (softmax .. ASCII, with this engine's calibration and
