@@ -8,6 +8,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <functional>
 #include <map>
@@ -182,6 +183,7 @@ struct dcb_engine {
     DevBuf<uint8_t> ids, bases, quals; DevBuf<int16_t> bq; DevBuf<int32_t> dst; DevBuf<int64_t> src_off, dst_off; DevBuf<int> status;
   } fs;
   struct { DevBuf<float> probs, loss; DevBuf<uint8_t> labels, ccs, exact; DevBuf<int32_t> pred, ccs_counts; DevBuf<int> bad; } ev;   // dcb_evaluate
+  struct { DevBuf<uint8_t> bq; DevBuf<unsigned long long> counts; DevBuf<int> bad_window; } evc;   // dcb_evaluate_calibration
   struct { DevBuf<float> teacher, student, loss, grad; } ds;   // dcb_distill_loss, dcb_distill_loss_grad
   struct { DevBuf<float> probs, loss, grad, matches, dp; DevBuf<uint8_t> labels; } lg;   // dcb_alignment_loss_grad
   struct { DevBuf<float> bias, logits, probs; DevBuf<uint8_t> bases, quals; } he;   // dcb_debug_head_epilogue
@@ -1722,6 +1724,66 @@ int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const
   CU(e, cudaStreamSynchronize(st));
   CU(e, cudaGetLastError());
   if (bad) return fail(e, DCB_ERR_INVALID, "dcb_evaluate: a device label id lies outside 0..4");
+  if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
+  return DCB_OK;
+}
+
+int dcb_evaluate_calibration(dcb_engine* e, const float* probs, const uint8_t* labels, const uint8_t* ccs_ids,
+                             const uint8_t* ccs_bq, int32_t batch, int32_t L, uint32_t flags, int64_t* counts_out,
+                             int64_t* deletions_out, int32_t* pred_counts, int32_t* ccs_counts, float* ms_out) {
+  if (!e) return DCB_ERR_INVALID;
+  int rc = check_alignment_args(e, "dcb_evaluate_calibration", batch, L, 0.0, DCB_BAND_WIDTH_NONE);
+  if (rc) return rc;
+  if (ms_out) *ms_out = 0.f;
+  if (!counts_out || !deletions_out) return fail(e, DCB_ERR_INVALID, "dcb_evaluate_calibration: null pointer");
+  std::fill(counts_out, counts_out + 2 * DCB_CALIB_BINS * 2, (int64_t)0);
+  deletions_out[0] = deletions_out[1] = 0;
+  if (batch == 0) return DCB_OK;
+  if (!probs || !labels || !ccs_ids || !ccs_bq || !pred_counts || !ccs_counts)
+    return fail(e, DCB_ERR_INVALID, "dcb_evaluate_calibration: null pointer");
+  const size_t ntok = (size_t)batch * L;
+  const bool lab_dev = flags & DCB_LABELS_ON_DEVICE;
+  if (!lab_dev && (rc = check_labels(e, "dcb_evaluate_calibration", labels, batch, L, false))) return rc;
+  CU(e, cudaSetDevice(e->cfg.device));
+  cudaStream_t st = e->stream;
+  const float* d_probs;
+  const uint8_t *d_labels, *d_ccs, *d_bq;
+  Output<int32_t> pred, ccs;
+  constexpr size_t kCounts = 2 * DCB_CALIB_BINS * 2;   // then the two deletion totals
+  if ((rc = stage_in(e, e->ev.probs, probs, ntok * kVocab, flags & DCB_ROWS_ON_DEVICE, &d_probs)) ||
+      (rc = stage_in(e, e->ev.labels, labels, ntok, lab_dev, &d_labels)) || (rc = stage_in(e, e->ev.ccs, ccs_ids, ntok, lab_dev, &d_ccs)) ||
+      (rc = stage_in(e, e->evc.bq, ccs_bq, ntok, lab_dev, &d_bq)) ||
+      (lab_dev && ((rc = ensure(e, e->ev.labels, ntok)) || (rc = ensure(e, e->ev.bad, 1)))) ||
+      (rc = ensure(e, e->ev.exact, (size_t)batch)) || (rc = ensure(e, e->evc.counts, kCounts + 2)) ||
+      (rc = ensure(e, e->evc.bad_window, 1)) ||
+      (rc = stage_out(e, e->ev.pred, pred_counts, (size_t)batch * 5, false, &pred)) ||
+      (rc = stage_out(e, e->ev.ccs_counts, ccs_counts, (size_t)batch * 5, false, &ccs)))
+    return rc;
+  int bad = 0, bad_window = INT_MAX;
+  if (lab_dev) {   // as dcb_evaluate: device labels are checked on the device
+    CU(e, cudaMemsetAsync(e->ev.bad.p, 0, sizeof(int), st));
+    launch_copy_label_ids(labels, e->ev.labels.p, ntok, e->ev.bad.p, st);
+    d_labels = e->ev.labels.p;
+  }
+  CU(e, cudaMemsetAsync(e->evc.counts.p, 0, (kCounts + 2) * sizeof(unsigned long long), st));
+  CU(e, cudaMemcpyAsync(e->evc.bad_window.p, &bad_window, sizeof(int), cudaMemcpyHostToDevice, st));
+  static_assert(DCB_CALIB_BINS == kCalibBins, "one bin per quality 0..99");
+  const EvalCalibOut calib{d_bq, e->evc.counts.p, e->evc.counts.p + kCounts, e->evc.bad_window.p};
+  CU(e, cudaEventRecord(e->ev_eval0, st));
+  CU(e, launch_evaluate_calibration(d_probs, d_labels, d_ccs, batch, L, e->ev.exact.p, pred.d, ccs.d, calib, st));
+  CU(e, cudaEventRecord(e->ev_eval1, st));
+  if ((rc = copy_out(e, pred)) || (rc = copy_out(e, ccs))) return rc;
+  static_assert(sizeof(unsigned long long) == sizeof(int64_t), "int64 counts");
+  CU(e, cudaMemcpyAsync(counts_out, e->evc.counts.p, kCounts * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  CU(e, cudaMemcpyAsync(deletions_out, e->evc.counts.p + kCounts, 2 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  CU(e, cudaMemcpyAsync(&bad_window, e->evc.bad_window.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  if (lab_dev) CU(e, cudaMemcpyAsync(&bad, e->ev.bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(e, cudaStreamSynchronize(st));
+  CU(e, cudaGetLastError());
+  if (bad) return fail(e, DCB_ERR_INVALID, "dcb_evaluate_calibration: a device label id lies outside 0..4");
+  if (bad_window != INT_MAX)
+    return fail(e, DCB_ERR_INVALID, "dcb_evaluate_calibration: window %d of the batch has a CCS base quality outside "
+                "0..%d", bad_window, DCB_CALIB_BINS - 1);
   if (ms_out) CU(e, cudaEventElapsedTime(ms_out, e->ev_eval0, e->ev_eval1));
   return DCB_OK;
 }

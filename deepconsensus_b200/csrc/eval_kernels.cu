@@ -18,12 +18,15 @@
 //                           the reference's first-max tie-breaking in the order [match, ins, del]; the three argmax
 //                           directions of every cell are kept as one byte in shared memory ((L+1)^2 bytes, 66 KB at
 //                           L = 256) and one thread walks the traceback, counting the trans_enc edges 1-5.  The y = 0
-//                           CTA also writes PerExampleAccuracy's exact-match flag (:43-65).
+//                           CTA also writes PerExampleAccuracy's exact-match flag (:43-65).  A compile-time variant
+//                           also bins each aligned base's quality as a match or a mismatch (base-quality calibration
+//                           counts of the prediction and of the CCS row).
 //   distill_loss_kernel     DistillationLoss.call (:1170-1213) on teacher and student logits, one warp per window: the
 //                           temperature-scaled softmax of both, the Keras logit loss (mean squared error or KL
 //                           divergence) per position, the mean over the window.  A compile-time variant also writes
 //                           the gradient with respect to the student's logits (same loss bits).
-// Results are deterministic: every reduction is a fixed-order loop, no atomics.
+// Results are deterministic: every reduction is a fixed-order loop, and the only atomics add or take the minimum of
+// integers.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -31,6 +34,7 @@
 #include <algorithm>
 
 #include "kernels.h"
+#include "quality.cuh"
 
 namespace dcb {
 
@@ -112,6 +116,30 @@ __device__ __forceinline__ void neg_log_probs(const float* p, float* lp) {
   float tot = q[0];
   for (int t = 1; t < kVocab; ++t) tot = __fadd_rn(tot, q[t]);
   for (int t = 0; t < kVocab; ++t) lp[t] = -logf(fminf(fmaxf(q[t] / tot, kEps), kOneMinusEps));
+}
+
+// The model head's per-token quality of a probability row, uncalibrated (head_finish.cuh with calibration off):
+// -10 log10(1 - p_max), capped at kCalibMaxQ and rounded half to even, then clamped at 0.
+__device__ __forceinline__ int pred_quality(const float* p) {
+  float pmax = -1.f;
+  for (int t = 0; t < kVocab; ++t)
+    if (p[t] > pmax) pmax = p[t];
+  HeadParams hp{};
+  hp.max_q = (float)kCalibMaxQ;
+  const int qi = head_quality(hp, -10.f * (float)log10((double)(1.f - pmax)));
+  return qi < 0 ? 0 : qi;
+}
+
+// One base of the traceback into the shared histogram (column 0 match, 1 mismatch): the base at j_opt - 1 of the
+// left-shifted sequence.
+__device__ __forceinline__ void calib_bin(int32_t* hist, const uint8_t* q, int j_opt, int col, int b, int* bad_window) {
+  if (j_opt < 1) return;
+  const int v = q[j_opt - 1];
+  if (v >= kCalibBins) {
+    atomicMin(bad_window, b);
+    return;
+  }
+  hist[v * 2 + col] += 1;
 }
 
 }  // namespace
@@ -289,10 +317,20 @@ align_loss_grad_kernel(const float* __restrict__ probs, const uint8_t* __restric
 
 // Directions byte of a cell: bits 0-1 match-state argmax (0..2), bit 2 insert-state argmax (0..1), bits 3-4 delete-state
 // argmax (0..2).
+//
+// kCalib also bins the quality of every base of the aligned sequence by how the traceback classifies it (the
+// calculate_baseq_calibration rules): an edge-1 base whose label base is equal is a match; an edge-1 base that differs
+// and every inserted base (edges 2, 3) are mismatches; label bases on edges 4, 5 are deletions and carry no quality.
+// The prediction's quality is the head's uncalibrated epilogue of the probability row it was decoded from, the CCS
+// row's its raw ccs_bq; each quality moves with its base through the left shift.  Thread 0 walks the traceback and
+// bins into shared memory, then adds the non-zero bins to the int64 totals with integer atomics, so the sums are exact
+// and do not depend on the batch split or on the order the CTAs finish.  A quality above kCalibBins - 1 is not binned:
+// the lowest such window index goes to *calib.bad_window.
+template <bool kCalib>
 __global__ void __launch_bounds__(kEvalThreads)
 align_identity_kernel(const float* __restrict__ probs, const uint8_t* __restrict__ labels,
                       const uint8_t* __restrict__ ccs_ids, int L, int32_t* __restrict__ pred_counts,
-                      int32_t* __restrict__ ccs_counts, uint8_t* __restrict__ exact_out) {
+                      int32_t* __restrict__ ccs_counts, uint8_t* __restrict__ exact_out, EvalCalibOut calib) {
   extern __shared__ __align__(16) uint8_t smem[];
   const int b = blockIdx.x, which = blockIdx.y, tid = threadIdx.x;
   const int m = L, n = L, W = L + 1;
@@ -302,19 +340,33 @@ align_identity_kernel(const float* __restrict__ probs, const uint8_t* __restrict
   uint8_t* s_y = s_x_in + L;
   uint8_t* s_x = s_y + L;
   uint8_t* s_dir = s_x + L;                                          // [L + 1][L + 1]
+  uint8_t* s_q_in = s_dir + W * W;                                   // kCalib: quality per position, then shifted
+  uint8_t* s_q = s_q_in + L;
+  int32_t* s_hist = reinterpret_cast<int32_t*>(smem + eval_calib_hist_offset(L));   // kCalib: [kCalibBins][2]
   __shared__ int s_tl, s_pl;
   for (int j = tid; j < L; j += blockDim.x) {
     s_y_in[j] = labels[(size_t)b * L + j];
     if (which == 0) {
       s_x_in[j] = (uint8_t)argmax5(probs + ((size_t)b * L + j) * kVocab);
+      if constexpr (kCalib) s_q_in[j] = (uint8_t)pred_quality(probs + ((size_t)b * L + j) * kVocab);
     } else {
       const uint8_t c = ccs_ids[(size_t)b * L + j];
       s_x_in[j] = c < kVocab ? c : 0;          // one_hot of an id outside the vocabulary is all zeros: argmax 0
+      if constexpr (kCalib) s_q_in[j] = calib.ccs_bq[(size_t)b * L + j];
     }
   }
+  if constexpr (kCalib)
+    for (int t = tid; t < 2 * kCalibBins; t += blockDim.x) s_hist[t] = 0;
   __syncthreads();
   if (tid == 0) s_tl = left_shift_serial(s_y_in, s_y, L);
-  if (tid == 32) s_pl = left_shift_serial(s_x_in, s_x, L);
+  if (tid == 32) {
+    s_pl = left_shift_serial(s_x_in, s_x, L);
+    if constexpr (kCalib) {
+      int k = 0;
+      for (int i = 0; i < L; ++i)
+        if (s_x_in[i] != 0) s_q[k++] = s_q_in[i];
+    }
+  }
   __syncthreads();
   if (which == 0) {   // PerExampleAccuracy: all L left-shifted positions equal
     int eq = 1;
@@ -397,9 +449,12 @@ align_identity_kernel(const float* __restrict__ probs, const uint8_t* __restrict
     const int edge = trans_enc[ss][s_n > 0 ? s_n : 0];
     if (edge == 1) {
       ++nm;
-      if (i_opt >= 1 && j_opt >= 1 && s_y[i_opt - 1] == s_x[j_opt - 1]) ++nc;
+      const bool correct = i_opt >= 1 && j_opt >= 1 && s_y[i_opt - 1] == s_x[j_opt - 1];
+      if (correct) ++nc;
+      if constexpr (kCalib) calib_bin(s_hist, s_q, j_opt, correct ? 0 : 1, b, calib.bad_window);
     } else if (edge <= 3) {
       ++ni;
+      if constexpr (kCalib) calib_bin(s_hist, s_q, j_opt, 1, b, calib.bad_window);
     } else {
       ++nd;
     }
@@ -409,6 +464,12 @@ align_identity_kernel(const float* __restrict__ probs, const uint8_t* __restrict
   }
   int32_t* out = (which == 0 ? pred_counts : ccs_counts) + (size_t)b * 5;
   out[0] = nm; out[1] = ni; out[2] = nd; out[3] = nc; out[4] = nm + ni + nd;
+  if constexpr (kCalib) {
+    unsigned long long* tot = calib.counts + (size_t)which * kCalibBins * 2;
+    for (int t = 0; t < 2 * kCalibBins; ++t)
+      if (s_hist[t]) atomicAdd(tot + t, (unsigned long long)s_hist[t]);
+    if (nd) atomicAdd(calib.deletions + which, (unsigned long long)nd);
+  }
 }
 
 // DistillationLoss.call (losses_and_metrics.py:1170-1213), one warp per window, lanes over positions.  Per position
@@ -528,9 +589,24 @@ cudaError_t launch_evaluate(const float* probs, const uint8_t* labels, const uin
   if (B <= 0) return cudaSuccess;
   align_loss_kernel<<<B, kEvalThreads, 0, st>>>(probs, labels, L, del_cost, loss_reg, hard_min, loss);
   const size_t smem = eval_identity_smem_bytes(L);
-  cudaError_t err = cudaFuncSetAttribute(align_identity_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaError_t err = cudaFuncSetAttribute(align_identity_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem);
   if (err != cudaSuccess) return err;
-  align_identity_kernel<<<dim3(B, 2), kEvalThreads, smem, st>>>(probs, labels, ccs_ids, L, pred_counts, ccs_counts, exact);
+  align_identity_kernel<false><<<dim3(B, 2), kEvalThreads, smem, st>>>(probs, labels, ccs_ids, L, pred_counts,
+                                                                       ccs_counts, exact, EvalCalibOut{});
+  return cudaGetLastError();
+}
+
+cudaError_t launch_evaluate_calibration(const float* probs, const uint8_t* labels, const uint8_t* ccs_ids, int B,
+                                        int L, uint8_t* exact, int32_t* pred_counts, int32_t* ccs_counts,
+                                        const EvalCalibOut& calib, cudaStream_t st) {
+  if (B <= 0) return cudaSuccess;
+  const size_t smem = eval_calib_hist_offset(L) + (size_t)2 * kCalibBins * sizeof(int32_t);
+  cudaError_t err = cudaFuncSetAttribute(align_identity_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem);
+  if (err != cudaSuccess) return err;
+  align_identity_kernel<true><<<dim3(B, 2), kEvalThreads, smem, st>>>(probs, labels, ccs_ids, L, pred_counts,
+                                                                      ccs_counts, exact, calib);
   return cudaGetLastError();
 }
 

@@ -246,6 +246,23 @@ void launch_features_ccs(const PrepBatch& b, const int4* window, const int32_t* 
 cudaError_t launch_evaluate(const float* probs, const uint8_t* labels, const uint8_t* ccs_ids, int B, int L,
                             float del_cost, float loss_reg, int hard_min, float* loss, uint8_t* exact,
                             int32_t* pred_counts, int32_t* ccs_counts, cudaStream_t st);
+// Base-quality calibration counts of align_identity_kernel<true>: qualities 0..kCalibBins-1 (the bins of
+// dcb_calib_count), column 0 match, 1 mismatch.
+constexpr int kCalibMaxQ = 93;   // the head's cap (max_base_quality) on the prediction's quality
+struct EvalCalibOut {
+  const uint8_t* ccs_bq;         // [B, L] raw CCS base quality of every position
+  unsigned long long* counts;    // int64 [2][kCalibBins][2] (prediction, CCS), zeroed by the caller; added to
+  unsigned long long* deletions; // int64 [2], zeroed by the caller; added to
+  int* bad_window;               // INT_MAX from the caller; the lowest window with a quality above kCalibBins - 1
+};
+// Byte offset of the shared histogram in align_identity_kernel<true>'s dynamic shared memory.
+__host__ __device__ constexpr size_t eval_calib_hist_offset(int L) {
+  return ((size_t)9 * (L + 1) * sizeof(float) + 6 * (size_t)L + (size_t)(L + 1) * (L + 1) + 3) / 4 * 4;
+}
+// launch_evaluate's identity kernel with the calibration counts (no loss).  Device pointers.
+cudaError_t launch_evaluate_calibration(const float* probs, const uint8_t* labels, const uint8_t* ccs_ids, int B,
+                                        int L, uint8_t* exact, int32_t* pred_counts, int32_t* ccs_counts,
+                                        const EvalCalibOut& calib, cudaStream_t st);
 // labels u8 [n] (device) copied to out with every id above 4 replaced by 0; *bad (zeroed by the caller) is set to 1 when
 // there was one, so that the evaluation kernels index only inside their tables and the call can refuse the labels
 void launch_copy_label_ids(const uint8_t* labels, uint8_t* out, size_t n, int* bad, cudaStream_t st);

@@ -154,7 +154,7 @@ ABI_SYMBOLS = (
     "dcb_create", "dcb_load_weights", "dcb_forward", "dcb_submit", "dcb_wait", "dcb_stitch", "dcb_last_forward_ms",
     "dcb_packed_window_bytes", "dcb_pack_rows", "dcb_forward_packed", "dcb_submit_packed",
     "dcb_stitch_fastq", "dcb_skip_mask", "dcb_fill_skipped", "dcb_stitch_ragged", "dcb_stitch_fastq_ragged",
-    "dcb_fill_skipped_ragged", "dcb_evaluate", "dcb_distill_loss",
+    "dcb_fill_skipped_ragged", "dcb_evaluate", "dcb_evaluate_calibration", "dcb_distill_loss",
     "dcb_alignment_loss_grad", "dcb_distill_loss_grad", "dcb_prep_open", "dcb_prep_set_threads", "dcb_prep_next_zmw", "dcb_prep_get_windows", "dcb_prep_ccs_header", "dcb_prep_close",
     "dcb_prep_last_error", "dcb_prep_export_records", "dcb_prep_get_records", "dcb_prep_use_ccs_smart_windows",
     "dcb_prep_get_window_widths", "dcb_prep_get_overflow_ccs", "dcb_features_layout", "dcb_features_pack",
@@ -231,6 +231,7 @@ def _load(path: str) -> ctypes.CDLL:
   lib.dcb_fill_skipped_ragged.argtypes = [vp, vp, vp, vp, vp, i32, vp, i32, i32, f64, f64, f64, u32, vp, vp]
   lib.dcb_evaluate.argtypes = [vp, vp, vp, vp, i32, i32, f64, f64, i32, u32, vp, vp, vp, vp,
                                ctypes.POINTER(ctypes.c_float)]
+  lib.dcb_evaluate_calibration.argtypes = [vp, vp, vp, vp, vp, i32, i32, u32, vp, vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_distill_loss.argtypes = [vp, vp, vp, i32, i32, f64, i32, u32, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_distill_loss_grad.argtypes = [vp, vp, vp, i32, i32, f64, i32, u32, vp, vp, ctypes.POINTER(ctypes.c_float)]
   lib.dcb_alignment_loss_grad.argtypes = [vp, vp, vp, i32, i32, f64, f64, i32, u32, vp, vp, vp,
@@ -344,6 +345,13 @@ def _arg(x: Any, dtype: Any, on_device: bool = False) -> Tuple[Optional[ctypes.c
     return _ptr(x), None
   a = np.ascontiguousarray(x, dtype=dtype)
   return _ptr(a), a
+
+
+def ccs_bq_bytes(ccs_bq: Any) -> np.ndarray:
+  """CCS base qualities (int16 from a tf.Example or the feature layout) as the uint8 rows dcb_evaluate_calibration reads:
+  a value outside 0..255, such as a gap's -1, becomes 255, which the call refuses wherever a base carries it."""
+  q = np.asarray(ccs_bq)
+  return np.ascontiguousarray(np.where((q < 0) | (q > 255), 255, q), dtype=np.uint8)
 
 
 def _outputs(out: Optional[Dict[str, int]], shapes: Dict[str, Optional[Tuple[int, ...]]]):
@@ -1018,6 +1026,40 @@ class B200Model:
     self._check(self._lib.dcb_evaluate(self._handle, p_ptr, _ptr(labels), _ptr(ccs_ids), B, L, dc, reg, bw,
                                        flags, _ptr(out["loss"]), _ptr(out["exact"]),
                                        _ptr(out["pred_counts"]), _ptr(out["ccs_counts"]), ctypes.byref(ms)))
+    out["ms"] = float(ms.value)
+    return out
+
+  def evaluate_calibration(self, probs, labels, ccs_ids, ccs_bq, on_device: bool = False,
+                           batch: Optional[int] = None, labels_on_device: bool = False) -> Dict[str, Any]:
+    """dcb_evaluate_calibration: base-quality calibration counts of the prediction and of the CCS row, from the
+    traceback of evaluate_windows()'s AlignmentMetric counts.  probs / labels / ccs_ids as in evaluate_windows();
+    ccs_bq uint8 [B, L] (ccs_bq_bytes) beside ccs_ids, host or, with labels_on_device, device.  Returns counts int64
+    [2, CALIB_BINS, 2] ([prediction, CCS][quality][match, mismatch]), deletions int64 [2], pred_counts / ccs_counts
+    int32 [B, 5] (bitwise evaluate_windows()'s) and ms, the kernel's device time."""
+    if labels_on_device:
+      if batch is None:
+        raise ValueError("evaluate_calibration(labels_on_device=True) needs batch")
+      B, L = int(batch), self.max_length
+    else:
+      labels = np.ascontiguousarray(labels, dtype=np.uint8)
+      ccs_ids = np.ascontiguousarray(ccs_ids, dtype=np.uint8)
+      ccs_bq = np.ascontiguousarray(ccs_bq, dtype=np.uint8)
+      if labels.ndim != 2 or ccs_ids.shape != labels.shape or ccs_bq.shape != labels.shape:
+        raise ValueError("labels, ccs_ids and ccs_bq must all be uint8 [B, L]")
+      B, L = labels.shape
+    if on_device and (batch is None or int(batch) != B):
+      raise ValueError("evaluate_calibration(on_device=True) needs batch == labels.shape[0]")
+    p_ptr, probs = _arg(probs, np.float32, on_device)
+    if not on_device and probs.shape != (B, L, 5):
+      raise ValueError("probs must be float32 [%d, %d, 5], got %s" % (B, L, probs.shape))
+    out = dict(counts=np.zeros((2, CALIB_BINS, 2), np.int64), deletions=np.zeros(2, np.int64),
+               pred_counts=np.zeros((B, 5), np.int32), ccs_counts=np.zeros((B, 5), np.int32))
+    ms = ctypes.c_float()
+    flags = (DCB_ROWS_ON_DEVICE if on_device else 0) | (DCB_LABELS_ON_DEVICE if labels_on_device else 0)
+    self._check(self._lib.dcb_evaluate_calibration(self._handle, p_ptr, _ptr(labels), _ptr(ccs_ids), _ptr(ccs_bq), B, L,
+                                                   flags, _ptr(out["counts"]), _ptr(out["deletions"]),
+                                                   _ptr(out["pred_counts"]), _ptr(out["ccs_counts"]),
+                                                   ctypes.byref(ms)))
     out["ms"] = float(ms.value)
     return out
 

@@ -42,6 +42,14 @@ per batch their sum / batch_size (tf.nn.compute_average_loss), `loss` (eval/loss
 create_input_fn batches with drop_remainder=True and get_step_counts counts n // batch_size steps.  distill_alpha,
 student_alpha, temperature and logit_loss_identifier come from the student's params.json (defaults: the
 transformer_learn_values_distill config).  `inference.csv` and the other entries stay the student-only numbers.
+
+`--calibration` also measures the base-quality calibration of the windows scored (every dataset, summed) and writes
+`dc_calibration.csv` and `ccs_calibration.csv` (calculate_baseq_calibration's format) and `calibration.json` to
+--out_dir.  dcb_evaluate_calibration walks the same AlignmentMetric traceback as the identity: each base of the argmax
+prediction is a match or a mismatch (insertions count as mismatches) in the bin of its uncalibrated head quality, each
+base of the CCS row in the bin of its raw CCS base quality, and label bases deleted are only counted.  From the counts
+calibration.fit_calibration fits the `threshold,w,b` strings `run --dc_calibration` and `--ccs_calibration` take
+(`--calibration_threshold`, `--calibration_min_bases`).  Without the flag every output is unchanged.
 """
 from __future__ import annotations
 
@@ -50,11 +58,14 @@ import collections
 import contextlib
 import json
 import os
+import re
 import time
 from typing import Any, Dict, Iterable, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 
+from deepconsensus_b200 import calculate_baseq_calibration
+from deepconsensus_b200 import calibration as calibration_lib
 from deepconsensus_b200 import engine as engine_lib
 from deepconsensus_b200 import inference
 from deepconsensus_b200 import params as params_lib
@@ -137,6 +148,36 @@ def aggregate_distillation(student_loss: np.ndarray, distill_loss: np.ndarray, e
   return out
 
 
+def calibration_summary(counts: np.ndarray, deletions: np.ndarray, windows: int, threshold: float, min_bases: int,
+                        params_dc_calibration: Optional[str]) -> Dict[str, Any]:
+  """calibration.json: per sequence (dc: the prediction, ccs: the CCS row) its counts [q, match, mismatch], deletions,
+  binned bases, the empirical quality [q, E] of the bins the fit uses, and the fitted "threshold,w,b" string, or null
+  with the reason in fit_error."""
+  out: Dict[str, Any] = dict(windows=int(windows), threshold=float(threshold), min_bases=int(min_bases))
+  for which, key in enumerate(("dc", "ccs")):
+    c = np.asarray(counts[which], np.int64)
+    q, e, _ = calibration_lib.empirical_quality(c, threshold, min_bases)
+    entry: Dict[str, Any] = dict(counts=[[i, int(m), int(x)] for i, (m, x) in enumerate(c)],
+                                 deletions=int(deletions[which]), bases=int(c.sum()),
+                                 empirical=[[int(a), float(b)] for a, b in zip(q, e)])
+    try:
+      entry["fit"] = calibration_lib.fit_calibration(c, threshold, min_bases)[1]
+    except ValueError as err:
+      entry["fit"], entry["fit_error"] = None, str(err)
+    out[key] = entry
+  out["params_dc_calibration"] = params_dc_calibration
+  return out
+
+
+def write_calibration(out_dir: str, counts: np.ndarray, summary: Dict[str, Any]) -> None:
+  """dc_calibration.csv, ccs_calibration.csv (calculate_baseq_calibration's CSV) and calibration.json."""
+  for which, key in enumerate(("dc", "ccs")):
+    with open(os.path.join(out_dir, "%s_calibration.csv" % key), "w") as f:
+      f.write(calculate_baseq_calibration.csv_text(counts[which]))
+  with open(os.path.join(out_dir, "calibration.json"), "w") as f:
+    json.dump(summary, f, indent=1)
+
+
 def write_inference_csv(path: str, rows: Sequence[Tuple[str, float, float]]) -> None:
   """inference.csv in model_utils.run_inference_and_write_results' layout: header, one line per dataset, blank line."""
   lines = ["dataset,loss,eval/per_example_accuracy\n"] + ["%s,%s,%s\n" % (p, l, a) for p, l, a in rows]
@@ -147,11 +188,13 @@ def write_inference_csv(path: str, rows: Sequence[Tuple[str, float, float]]) -> 
 
 class HostRowsChunk:
   """One chunk of host float32 rows (the tf.Example path): staged into the pipeline slot's pinned rows and submitted
-  with dcb_submit; dcb_evaluate gets its label and CCS rows as host arrays."""
+  with dcb_submit; dcb_evaluate gets its label and CCS rows (and dcb_evaluate_calibration the CCS qualities, uint8
+  [n, L] or None) as host arrays."""
   packed, rows_flag, labels_on_device = False, 0, False
 
-  def __init__(self, model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndarray, ccs: np.ndarray):
-    self.model, self.rows, self.labels, self.ccs_ids = model, rows, labels, ccs
+  def __init__(self, model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndarray, ccs: np.ndarray,
+               ccs_bq: Optional[np.ndarray] = None):
+    self.model, self.rows, self.labels, self.ccs_ids, self.ccs_bq = model, rows, labels, ccs, ccs_bq
     self.n = int(rows.shape[0])
 
   def stage(self, slot: int) -> int:
@@ -160,18 +203,20 @@ class HostRowsChunk:
     return staging.ctypes.data
 
 
-def host_row_chunks(model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndarray,
-                    chunk: int) -> Iterator[HostRowsChunk]:
-  """The chunk source of float32 rows [N, R, L] and uint8 labels [N, L] in host memory."""
+def host_row_chunks(model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndarray, chunk: int,
+                    ccs_bq: Optional[np.ndarray] = None) -> Iterator[HostRowsChunk]:
+  """The chunk source of float32 rows [N, R, L] and uint8 labels [N, L] in host memory; ccs_bq (the tf.Examples'
+  ccs_base_quality_scores [N, L]) is needed for the calibration counts only."""
   ccs = model.ccs_ids(rows)
+  bq = None if ccs_bq is None else engine_lib.ccs_bq_bytes(ccs_bq)
   for b0 in range(0, rows.shape[0], chunk):
     b1 = min(rows.shape[0], b0 + chunk)
-    yield HostRowsChunk(model, rows[b0:b1], labels[b0:b1], ccs[b0:b1])
+    yield HostRowsChunk(model, rows[b0:b1], labels[b0:b1], ccs[b0:b1], None if bq is None else bq[b0:b1])
 
 
 def evaluate_chunks(model: engine_lib.B200Model, chunks: Iterable[Any], chunk: int, strict: Optional[bool] = None,
                     teacher: Optional[engine_lib.B200Model] = None, temperature: float = 1.0,
-                    logit_loss: Any = "kl_divergence") -> Dict[str, Any]:
+                    logit_loss: Any = "kl_divergence", calibration: bool = False) -> Dict[str, Any]:
   """Per-window evaluation of a chunk source: per chunk of at most `chunk` windows the forward runs through the submit
   path (device outputs, two chunks in flight) and dcb_evaluate reads its probabilities on the device.  A chunk has `n`
   windows and `stage(slot)`, which returns the address of its rows: pinned host float32 rows (packed False), or
@@ -181,7 +226,12 @@ def evaluate_chunks(model: engine_lib.B200Model, chunks: Iterable[Any], chunk: i
 
   With the `teacher` of a distilled student, the teacher's forward runs from the same rows, and once both are done
   dcb_distill_loss_grad compares the two engines' logits on the device.  This adds distill_loss float32 [N] and the
-  teacher's forward and the distillation kernel's device times (teacher_forward_ms, distill_ms)."""
+  teacher's forward and the distillation kernel's device times (teacher_forward_ms, distill_ms).
+
+  With `calibration`, every chunk also has `ccs_bq` beside its CCS rows, and dcb_evaluate_calibration reads the same
+  probabilities: this adds calibration_counts int64 [2, CALIB_BINS, 2] and calibration_deletions int64 [2], summed over
+  the chunks, and calibration_ms.  Its per-window counts must equal dcb_evaluate's and its binned totals their sums; a
+  CCS quality outside 0..99 raises ValueError naming the window (its index among the windows of `chunks`)."""
   L = model.max_length
   flag = engine_lib.DCB_OUT_ON_DEVICE | model._precision_flag(strict)
   engines = [model] if teacher is None else [model, teacher]
@@ -192,6 +242,7 @@ def evaluate_chunks(model: engine_lib.B200Model, chunks: Iterable[Any], chunk: i
     times = dict(forward_ms=0.0, eval_ms=0.0)
   else:
     times = dict(forward_ms=0.0, teacher_forward_ms=0.0, eval_ms=0.0, distill_ms=0.0)
+  cal = dict(counts=np.zeros((2, engine_lib.CALIB_BINS, 2), np.int64), deletions=np.zeros(2, np.int64), ms=0.0, w0=0)
 
   def alloc(m, nbytes):
     owned.append((m, m.alloc_device(nbytes)))
@@ -244,6 +295,8 @@ def evaluate_chunks(model: engine_lib.B200Model, chunks: Iterable[Any], chunk: i
         r = model.evaluate_windows(bufs[slot][0]["probs"], c.labels, c.ccs_ids, on_device=True, batch=c.n,
                                    labels_on_device=c.labels_on_device)
         times["eval_ms"] += r.pop("ms")
+        if calibration:
+          add_calibration(model, cal, bufs[slot][0]["probs"], c, r)
         if teacher is not None:
           d = model.distill_loss(bufs[slot][1]["logits"], bufs[slot][0]["logits"], temperature, logit_loss,
                                  on_device=True, batch=c.n, length=L)
@@ -255,24 +308,54 @@ def evaluate_chunks(model: engine_lib.B200Model, chunks: Iterable[Any], chunk: i
       m.free_device(addr)
   out = engine_lib._concat_eval(parts, () if teacher is None else ("distill_loss",))
   out.update(times)
+  if calibration:
+    out.update(calibration_counts=cal["counts"], calibration_deletions=cal["deletions"], calibration_ms=cal["ms"])
   return out
+
+
+def add_calibration(model: engine_lib.B200Model, cal: Dict[str, Any], probs: int, c: Any, r: Dict[str, Any]) -> None:
+  """dcb_evaluate_calibration of one chunk whose probabilities are at device address `probs`, added to `cal`; `r` is
+  dcb_evaluate's result for the same chunk, which the calibration's per-window counts and totals must agree with."""
+  try:
+    k = model.evaluate_calibration(probs, c.labels, c.ccs_ids, c.ccs_bq, on_device=True, batch=c.n,
+                                   labels_on_device=c.labels_on_device)
+  except engine_lib.DcbError as err:
+    m = re.search(r"window (\d+) of the batch", str(err))
+    if m is None:
+      raise
+    raise ValueError("window %d: %s" % (cal["w0"] + int(m.group(1)), err)) from err
+  for which, key in enumerate(("pred_counts", "ccs_counts")):
+    if not np.array_equal(k[key], r[key]):
+      raise RuntimeError("dcb_evaluate_calibration's %s differ from dcb_evaluate's" % key)
+    nm, ni, nd, nc = (int(v) for v in r[key][:, :4].sum(0))
+    got = k["counts"][which].sum(0)
+    if (int(got[0]), int(got[1]), int(k["deletions"][which])) != (nc, nm - nc + ni, nd):
+      raise RuntimeError("calibration totals (%d, %d, %d) do not match the alignment counts (%d, %d, %d)" %
+                         (int(got[0]), int(got[1]), int(k["deletions"][which]), nc, nm - nc + ni, nd))
+  cal["counts"] += k["counts"]
+  cal["deletions"] += k["deletions"]
+  cal["ms"] += k["ms"]
+  cal["w0"] += c.n
 
 
 def evaluate_rows(model: engine_lib.B200Model, rows: np.ndarray, labels: np.ndarray, chunk: int,
                   strict: Optional[bool] = None, teacher: Optional[engine_lib.B200Model] = None,
-                  temperature: float = 1.0, logit_loss: Any = "kl_divergence") -> Dict[str, Any]:
+                  temperature: float = 1.0, logit_loss: Any = "kl_divergence",
+                  ccs_bq: Optional[np.ndarray] = None) -> Dict[str, Any]:
   """evaluate_chunks() of float32 rows [N, R, L] and uint8 labels [N, L] in host memory: per chunk the rows go
-  through the pipeline slot's pinned staging and dcb_submit."""
-  return evaluate_chunks(model, host_row_chunks(model, rows, labels, chunk), chunk, strict, teacher, temperature,
-                         logit_loss)
+  through the pipeline slot's pinned staging and dcb_submit.  With ccs_bq (int16 [N, L], the tf.Examples'
+  ccs_base_quality_scores) the calibration counts are added."""
+  return evaluate_chunks(model, host_row_chunks(model, rows, labels, chunk, ccs_bq), chunk, strict, teacher,
+                         temperature, logit_loss, calibration=ccs_bq is not None)
 
 
 class DevicePackedChunk:
-  """One chunk of the BAM path: packed rows, label rows and CCS rows that dcb_features_eval left in device memory."""
+  """One chunk of the BAM path: packed rows, label rows and CCS rows that dcb_features_eval left in device memory, and
+  with the calibration counts the CCS qualities beside them (ccs_bq, a device address, else 0)."""
   packed, rows_flag, labels_on_device = True, engine_lib.DCB_ROWS_ON_DEVICE, True
 
-  def __init__(self, packed: int, labels: int, ccs: int, n: int):
-    self.packed_ptr, self.labels, self.ccs_ids, self.n = packed, labels, ccs, int(n)
+  def __init__(self, packed: int, labels: int, ccs: int, n: int, ccs_bq: int = 0):
+    self.packed_ptr, self.labels, self.ccs_ids, self.n, self.ccs_bq = packed, labels, ccs, int(n), ccs_bq
 
   def stage(self, slot: int) -> int:
     return self.packed_ptr
@@ -288,14 +371,17 @@ class BamWindows:
   buffer sets.  Chunks of at most `chunk` windows are slices of that set, so nothing goes through the host.  The sets
   alternate between ZMW batches that keep a window: when a batch is laid out, every chunk of the batch before the
   previous one has been waited for, on both engines.  `counter` receives preprocess's counters of every ZMW read;
-  `limit_windows` > 0 stops after that many windows."""
+  `limit_windows` > 0 stops after that many windows.  With `calibration`, the CCS qualities of the kept windows (the
+  layout's ccs_bq, compacted in dcb_features_eval's window order) are copied beside their CCS rows, L bytes each."""
 
   def __init__(self, model: engine_lib.B200Model, subreads_to_ccs: str, ccs_bam: str, truth_to_ccs: str,
                bed: Dict[str, Dict[str, Any]], contig_split: Dict[str, str], split: str, chunk: int,
-               ins_trim: int = 5, cpus: int = 0, batch_zmws: int = 64, limit_windows: int = 0):
+               ins_trim: int = 5, cpus: int = 0, batch_zmws: int = 64, limit_windows: int = 0,
+               calibration: bool = False):
     self.model, self.split, self.chunk, self.ins_trim = model, split, int(chunk), int(ins_trim)
     self.bed, self.contig_split = bed, contig_split
     self.batch_zmws, self.limit_windows = max(int(batch_zmws), 1), int(limit_windows)
+    self.calibration = bool(calibration)
     self.paths = (subreads_to_ccs, ccs_bam, truth_to_ccs)
     self.cpus = max(int(cpus), 0)
     self.counter: collections.Counter = collections.Counter()
@@ -312,13 +398,16 @@ class BamWindows:
     m, L, cap = self.model, self.model.max_length, max(n, self.chunk)
     self._sets[which] = dict(cap=cap, packed=m.alloc_device(cap * m.packed_window_bytes), labels=m.alloc_device(cap * L),
                              ccs=m.alloc_device(cap * L))
+    if self.calibration:
+      self._sets[which]["bq"] = m.alloc_device(cap * L)
     return self._sets[which]
 
   def _free(self, which: int) -> None:
     cur, self._sets[which] = self._sets[which], None
     if cur is not None:
-      for k in ("packed", "labels", "ccs"):
-        self.model.free_device(cur[k])
+      for k in ("packed", "labels", "ccs", "bq"):
+        if k in cur:
+          self.model.free_device(cur[k])
 
   def close(self) -> None:
     for which in (0, 1):
@@ -344,9 +433,12 @@ class BamWindows:
     if self.limit_windows:
       k = min(k, self.limit_windows - self.n_windows)
     self.n_windows += k
+    if self.calibration and k:
+      m.memcpy_h2d(buf["bq"], engine_lib.ccs_bq_bytes(lay["ccs_bq"][r["windows"][:k]]))
     stride = m.packed_window_bytes
     return [DevicePackedChunk(buf["packed"] + j0 * stride, buf["labels"] + j0 * L, buf["ccs"] + j0 * L,
-                              min(k, j0 + self.chunk) - j0) for j0 in range(0, k, self.chunk)]
+                              min(k, j0 + self.chunk) - j0, buf["bq"] + j0 * L if self.calibration else 0)
+            for j0 in range(0, k, self.chunk)]
 
   def __iter__(self) -> Iterator[DevicePackedChunk]:
     stream = preprocess.BamFeatureStream(self.paths[0], self.paths[1], self.model.params.max_passes,
@@ -428,7 +520,8 @@ def run(checkpoint: str, eval_path: Optional[Sequence[str]] = None, out_dir: str
         teacher_random_weights: Optional[int] = None, subreads_to_ccs: Optional[str] = None,
         ccs_bam: Optional[str] = None, truth_to_ccs: Optional[str] = None, truth_bed: Optional[str] = None,
         truth_split: Optional[str] = None, split: Optional[Sequence[str]] = None, ins_trim: int = 5, cpus: int = 0,
-        batch_zmws: int = 64, use_ccs_smart_windows: bool = False) -> Dict[str, Any]:
+        batch_zmws: int = 64, use_ccs_smart_windows: bool = False, calibration: bool = False,
+        calibration_threshold: float = 0.0, calibration_min_bases: int = 1000) -> Dict[str, Any]:
   truth = check_bam_source(eval_path, subreads_to_ccs, ccs_bam, truth_to_ccs, truth_bed, truth_split, split,
                            use_ccs_smart_windows)
   if truth is not None and cpus == 1:
@@ -464,6 +557,7 @@ def run(checkpoint: str, eval_path: Optional[Sequence[str]] = None, out_dir: str
       raise
   os.makedirs(out_dir, exist_ok=True)
   csv_rows, metrics = [], {}
+  cal_counts, cal_deletions, cal_windows = np.zeros((2, engine_lib.CALIB_BINS, 2), np.int64), np.zeros(2, np.int64), 0
   kw = {} if teacher is None else dict(teacher=teacher, temperature=float(distill["temperature"]),
                                        logit_loss=distill["logit_loss_identifier"])
   try:
@@ -476,14 +570,15 @@ def run(checkpoint: str, eval_path: Optional[Sequence[str]] = None, out_dir: str
           raise ValueError("%s: windows of shape %s, the checkpoint's params expect [%d, %d]" %
                            (path, rows.shape[1:], model.total_rows, model.max_length))
         t1 = time.time()
-        per = evaluate_rows(model, rows, labels, chunk, **kw)
+        per = evaluate_rows(model, rows, labels, chunk, ccs_bq=d["ccs_base_quality_scores"] if calibration else None,
+                            **kw)
         timing = dict(seconds_read=t1 - t0, seconds_model_and_eval=time.time() - t1)
       else:
         source = BamWindows(model, subreads_to_ccs, ccs_bam, truth_to_ccs, truth["bed"], truth["contig_split"], path,
                             chunk, ins_trim=ins_trim, cpus=cpus, batch_zmws=batch_zmws,
-                            limit_windows=0 if limit < 0 else limit * bs)
+                            limit_windows=0 if limit < 0 else limit * bs, calibration=calibration)
         try:
-          per = evaluate_chunks(model, source, chunk, **kw)
+          per = evaluate_chunks(model, source, chunk, calibration=calibration, **kw)
         finally:
           source.close()
         timing = dict(features_ms=source.features_ms, seconds=time.time() - t0)
@@ -501,6 +596,10 @@ def run(checkpoint: str, eval_path: Optional[Sequence[str]] = None, out_dir: str
         agg["distillation"] = dist
       csv_rows.append((path, agg["loss"], agg["per_example_accuracy"]))
       metrics[path] = agg
+      if calibration:
+        cal_counts += per["calibration_counts"]
+        cal_deletions += per["calibration_deletions"]
+        cal_windows += int(per["loss"].shape[0])
   finally:
     model.close()
     if teacher is not None:
@@ -508,6 +607,10 @@ def run(checkpoint: str, eval_path: Optional[Sequence[str]] = None, out_dir: str
   write_inference_csv(os.path.join(out_dir, "inference.csv"), csv_rows)
   with open(os.path.join(out_dir, "eval_metrics.json"), "w") as f:
     json.dump(metrics, f, indent=1)
+  if calibration:
+    write_calibration(out_dir, cal_counts, calibration_summary(cal_counts, cal_deletions, cal_windows,
+                                                               calibration_threshold, calibration_min_bases,
+                                                               params.get("dc_calibration")))
   return metrics
 
 
@@ -536,6 +639,11 @@ def main(argv: Optional[List[str]] = None) -> None:
   ap.add_argument("--teacher_model_dir", default=None,
                   help="checkpoint of the teacher of a distilled student: adds the distillation losses")
   ap.add_argument("--teacher_random_weights", type=int, default=None)
+  ap.add_argument("--calibration", action="store_true",
+                  help="also write dc_calibration.csv, ccs_calibration.csv and calibration.json (fitted threshold,w,b)")
+  ap.add_argument("--calibration_threshold", type=float, default=0.0,
+                  help="fit only bins above this quality, the threshold of the fitted string (0: every bin)")
+  ap.add_argument("--calibration_min_bases", type=int, default=1000, help="fit only bins with at least this many bases")
   a = ap.parse_args(argv)
   try:
     check_bam_source(a.eval_path, a.subreads_to_ccs, a.ccs_bam, a.truth_to_ccs, a.truth_bed, a.truth_split, a.split,

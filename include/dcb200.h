@@ -270,6 +270,29 @@ int dcb_evaluate(dcb_engine* e, const float* probs, const uint8_t* labels, const
                  int32_t L, double del_cost, double loss_reg, int32_t band_width, uint32_t flags, float* loss_out,
                  uint8_t* exact_out, int32_t* pred_counts, int32_t* ccs_counts, float* ms_out);
 
+/* Base-quality calibration counts of labelled windows: the traceback of dcb_evaluate's AlignmentMetric counts
+ * classifies every base of the left-shifted argmax prediction and of the left-shifted CCS row, and each base's quality
+ * is binned by that class, as calculate_baseq_calibration bins a read's M / I / D operations:
+ *   an edge-1 base equal to its label base        match
+ *   an edge-1 base that differs, an edge-2/3 base  mismatch (an inserted base is unaligned)
+ *   a label base on edge 4/5                       a deletion: no quality, only counted
+ * The prediction's quality is the head's epilogue without calibration, -10 log10(1 - p_max) of the probability row
+ * the base was decoded from, capped at 93 and rounded half to even (the quality byte minus 33 of a forward with
+ * calibration skipped); the CCS row's is ccs_bq u8 [B, L], its raw base quality.  A quality stays with its base through
+ * the left shift.  Per window, sum match = num_correct_matches, sum mismatch = num_matches - num_correct_matches +
+ * num_insertions, deletions = num_deletions.
+ *   counts_out int64 [2][DCB_CALIB_BINS][2]   [prediction, CCS][quality][match, mismatch] of the batch
+ *   deletions_out int64 [2]                   label bases deleted against the prediction and against the CCS row
+ *   pred_counts, ccs_counts int32 [B][5]      bitwise dcb_evaluate's
+ * probs, labels, ccs_ids, flags and the argument checks are dcb_evaluate's (no loss is computed, so there is no
+ * del_cost, loss_reg or band_width); with DCB_LABELS_ON_DEVICE ccs_bq is a device array too.  A binned CCS quality
+ * above DCB_CALIB_BINS - 1 is DCB_ERR_INVALID naming the window.  Outputs are host arrays; ms_out (nullable) receives
+ * the kernel's device time.  The counts are integer sums: they do not depend on how windows are split into calls. */
+#define DCB_CALIB_BINS 100
+int dcb_evaluate_calibration(dcb_engine* e, const float* probs, const uint8_t* labels, const uint8_t* ccs_ids,
+                             const uint8_t* ccs_bq, int32_t batch, int32_t L, uint32_t flags, int64_t* counts_out,
+                             int64_t* deletions_out, int32_t* pred_counts, int32_t* ccs_counts, float* ms_out);
+
 /* The gradient of the alignment loss, for training: AlignmentLoss.eval(return_matches=True)
  * (losses_and_metrics.py:549-595, width=None) and the gradient the training loop's tape takes of the per-window loss
  * with respect to y_pred (model_train_custom_loop.py, model_distillation.py).  For B windows of length L <= 256, probs
